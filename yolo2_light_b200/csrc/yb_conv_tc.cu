@@ -10,9 +10,12 @@
 //     Tiles are rectangles of TW x TH = 128 output pixels over (x, merged batch*row) so that the 19*2^k-wide
 //     YOLO grids tile exactly.  Stride-2 convolutions use a 5-D view that splits x and y into (half, parity).
 //   * W ([filters][K] bf16, K ordered (ky, kx, c)) is the K-major B operand, loaded by TMA as well.
-//   * Two consumer warpgroups issue wgmma.mma_async (bf16 x bf16 -> f32, M=64 each, N=BN<=128, K=16) straight from
+//   * Two consumer warpgroups issue wgmma.mma_async (bf16 x bf16 -> f32, M=64 each, N=BN, K=16) straight from
 //     the shared-memory ring; each releases a ring stage through an mbarrier once the wgmmas reading it have retired.
-//   * At the end of a tile the register accumulators go to a padded [128][BN+4] shared-memory tile, and the same 8
+//   * bf16-output stride-1 layers (most of the FLOPs) run k_conv_tc_reg: BN <= 256, the epilogue works on the register
+//     fragments and stores bf16 slabs by TMA (see there).
+//   * Everything else runs k_conv_tc (BN <= 128): at the end of a tile the register accumulators go to a padded
+//     [128][BN+4] shared-memory tile, and the same 8
 //     warps run the epilogue from it with one pixel row per thread: add bias (folded batch-norm), apply leaky-ReLU,
 //     add the shortcut residual when fused (reference :443-449), and store bf16 NHWC through a swizzled staging tile
 //     (whole 128-byte lines) or TMA, or f32 for detection heads -- optionally with the following [yolo] layer applied
@@ -21,7 +24,7 @@
 //     yolov2_forward_network_quantized.c:474-490), wide XNOR layers as +-1 bytes on the s8 wgmma, and the float heads
 //     of the exact networks on tf32 wgmma.  KS = true: K-split of the tail wave (opt-in).
 //
-// Warp roles (288 threads): warps 0-7 = two consumer warpgroups (wgmma + epilogue), warp 8 = TMA producer.
+// Warp roles of k_conv_tc (288 threads): warps 0-7 = two consumer warpgroups (wgmma + epilogue), warp 8 = TMA producer.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -73,14 +76,11 @@ struct TcParams {
     int bstat;                                // 1: the whole filter matrix (nt == 1, <= 72 KB) is loaded once per CTA and stays in
                                               //    shared memory; the ring then streams activations only
     uint32_t bstat_bytes;
-    // TMA epilogue (bf16 output, stride 1): each group of four epilogue warps writes its 128 x 32-column slab as bf16 into a
-    // swizzled shared-memory tile and one thread stores it with cp.async.bulk.tensor; the shortcut residual comes in the same
-    // way (TMA load + mbarrier).  No shuffles, no staging transposes, no LSU global traffic.
+    // TMA epilogue: slab width in columns (0: off).  Each epilogue group writes its slab into a swizzled shared-memory tile and
+    // one thread stores it with cp.async.bulk.tensor; the shortcut residual comes in the same way (TMA load + mbarrier).
+    // Non-zero for every k_conv_tc_reg plan (bf16 slabs) and for the integer kinds (f32 slabs of k_conv_tc).
     int tma_epi;
     int l2_hint;              // 1: shortcut tiles are loaded with the L2 evict-first policy
-    // epi_bufs (TMA epilogue): OUT tiles per warp group.  With one tile a slab cannot be written before the bulk store of the previous
-    // slab has finished READING the tile; with two the group only waits for the store before the last one.
-    int epi_bufs;
     uint32_t stg_bytes;       // epilogue staging / TMA-epilogue tiles
     int acc_pitch;            // words per row of the shared-memory accumulator tile (BN + 4: conflict-free row reads)
     // Fused 2x2 / stride-2 max-pool + input conversion of the NEXT integer layer (integer kinds, tiles of 8 x 16 pixels):
@@ -238,6 +238,16 @@ template <> struct Wg<0, 128> {
             : "l"(a), "l"(b), "r"(scale_d) : "memory");
     }
 };
+template <> struct Wg<0, 256> {
+    static __device__ __forceinline__ void mma(float (&d)[128], uint64_t a, uint64_t b, uint32_t scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+            : "l"(a), "l"(b), "r"(scale_d) : "memory");
+    }
+};
 template <> struct Wg<1, 32> {
     static __device__ __forceinline__ void mma(uint32_t (&d)[16], uint64_t a, uint64_t b, uint32_t scale_d) {
         asm volatile(
@@ -381,12 +391,122 @@ __device__ __forceinline__ void st_release_u32(unsigned *p, unsigned v) {
     asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 
+// Shared-memory barriers of both kernels: full[stages], empty[stages], then the resident-filter barrier.
+__device__ __forceinline__ uint32_t full_bar(uint32_t bars, int s) { return bars + 8u * (uint32_t)s; }
+__device__ __forceinline__ uint32_t empty_bar(uint32_t bars, int stages, int s) { return bars + 8u * (uint32_t)(stages + s); }
+
+// TMA producer (one elected thread): walks the consumers' schedule and keeps the ring full.  smemB: resident filter matrix
+// (p.bstat), smem0: the ring.
+template <bool KS, bool ST>
+__device__ __forceinline__ void tc_produce(const CUtensorMap *tmA, const CUtensorMap *tmB, const TcParams &p, uint32_t smemB,
+                                           uint32_t smem0, uint32_t bars, int w_first, int w_step) {
+    int stage = 0; uint32_t phase = 0;
+    long long w_empty = 0, w_tma = 0; const long long t_begin = ST ? clock64() : 0;
+    // loop-invariant parameters in registers; the (tap, channel-block) walk is incremental (no integer divisions per
+    // K-block in this single thread)
+    const int sps = p.sps, kblocks = p.kblocks, cblocks = p.cblocks, BK = p.BK, fsize = p.size, stages = p.stages;
+    const int xoff = p.xoff, yoff = p.yoff, stride2 = p.stride2, nt = p.nt, xt = p.xt;
+    const uint32_t a_bytes = p.a_bytes, b_bytes = p.b_bytes, stage_bytes = p.stage_bytes;
+    const uint32_t b_off = (uint32_t)sps * a_bytes;
+    const uint32_t bstat_bar = bars + 16u * (uint32_t)stages;
+    const int bstat = p.bstat;
+    if (bstat) {   // resident filter matrix: kblocks boxes of [BN filters][BK], once
+        mbar_arrive_expect_tx(bstat_bar, p.bstat_bytes);
+        for (int kb = 0; kb < kblocks; ++kb) tma_load_2d(smemB + (uint32_t)kb * b_bytes, tmB, bstat_bar, kb * BK, 0);
+    }
+    TcSched sch = sched_init<KS>(p, w_first, w_step);
+    int w, seg0, seg1;
+    while (sched_next<KS>(sch, w, seg0, seg1)) {
+        const int n_idx = w % nt;
+        const int m = w / nt;
+        const int x0 = (m % xt) * p.TW;
+        const int J0 = (m / xt) * p.TH + p.jshift;
+        const int n0 = n_idx * p.BN;
+        const int kb_begin = seg0 * sps, kb_end = min(kblocks, seg1 * sps);
+        // channel block, tap x/y, K column of the weight matrix at the first K-block of the segment
+        const int tap0 = kb_begin / cblocks;
+        int cb = kb_begin - tap0 * cblocks, ky = tap0 / fsize, kx = tap0 - (tap0 / fsize) * fsize, kcol = kb_begin * BK;
+        for (int kb0 = kb_begin; kb0 < kb_end; kb0 += sps) {
+            const int nsub = min(sps, kb_end - kb0);
+            if constexpr (ST) { const long long c0 = clock64(); mbar_wait(empty_bar(bars, stages, stage), phase ^ 1u); w_empty += clock64() - c0; }
+            else mbar_wait(empty_bar(bars, stages, stage), phase ^ 1u);
+            const uint32_t fb = full_bar(bars, stage);
+            const uint32_t a_dst = smem0 + (uint32_t)stage * stage_bytes;
+            const uint32_t b_dst = a_dst + b_off;
+            if (p.dbg & 1) {
+                mbar_arrive(fb);
+                if (++stage == stages) { stage = 0; phase ^= 1u; }
+                continue;
+            }
+            mbar_arrive_expect_tx(fb, (uint32_t)nsub * (a_bytes + (bstat ? 0u : b_bytes)));
+            const long long ct0 = ST ? clock64() : 0;
+            for (int j = 0; j < nsub; ++j) {
+                const uint32_t ad = a_dst + (uint32_t)j * a_bytes, bd = b_dst + (uint32_t)j * b_bytes;
+                const int c0 = cb * BK;
+                if (stride2) tma_load_5d(ad, tmA, fb, c0, kx & 1, x0 + (kx >> 1), ky & 1, J0 + (ky >> 1));
+                else tma_load_3d(ad, tmA, fb, c0, x0 + kx + xoff, J0 + ky + yoff);
+                if (!bstat) tma_load_2d(bd, tmB, fb, kcol, n0);
+                kcol += BK;
+                if (++cb == cblocks) { cb = 0; if (++kx == fsize) { kx = 0; ++ky; } }
+            }
+            if constexpr (ST) w_tma += clock64() - ct0;
+            if (++stage == stages) { stage = 0; phase ^= 1u; }
+        }
+    }
+    if (ST && p.stats) { p.stats[blockIdx.x * 16 + 0] = (unsigned long long)w_empty; p.stats[blockIdx.x * 16 + 1] = (unsigned long long)(clock64() - t_begin); p.stats[blockIdx.x * 16 + 7] = (unsigned long long)w_tma; }
+}
+
+// The K-blocks of stages [seg0, seg1) of the current work item into warpgroup wg's accumulator fragment d (rows 64 wg .. + 63
+// of the tile; KK wgmmas of K = 32 bytes per K-block).  A ring stage is released once the wgmmas that read it have retired,
+// one stage behind the issue (wgmma.wait_group 1) so that the tensor pipe never drains.  Nothing but wgmmas touches the
+// accumulators while wgmmas are in flight, and every batch is the same KK wgmmas: ptxas then inserts no fences of its own
+// and serializes nothing (the -Xptxas -v log has no C75xx notes).
+template <int KIND, int BN, int KK, bool ST, typename T>
+__device__ __forceinline__ void tc_mma_loop(T (&d)[BN / 2], const TcParams &p, uint32_t smemB, uint32_t smem0, uint32_t bars,
+                                            int wg, int lane, int &stage, uint32_t &phase, long long &w_full, int seg0, int seg1) {
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) d[i] = T(0);
+    wg_fence_operand(d);
+    const int sps = p.sps, stages = p.stages;
+    const uint32_t a_bytes = p.a_bytes, b_bytes = p.b_bytes, stage_bytes = p.stage_bytes, hi = p.desc_hi;
+    const uint32_t b_off = (uint32_t)sps * a_bytes, a_wg = (uint32_t)wg * (a_bytes >> 1);
+    const int kb_begin = seg0 * sps, kb_end = min(p.kblocks, seg1 * sps);
+    auto release = [&](int s) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar(bars, stages, s)); };
+    // one commit group per K-block; a stage (sps K-blocks, fewer at the end of the segment) is released once the group of
+    // its last K-block has retired, which wgmma.wait_group 1 shows one K-block later
+    int pend = -1, jj = 0;
+    for (int kb = kb_begin; kb < kb_end; ++kb) {
+        if (jj == 0) {
+            if constexpr (ST) { const long long c0 = clock64(); mbar_wait(full_bar(bars, stage), phase); w_full += clock64() - c0; }
+            else mbar_wait(full_bar(bars, stage), phase);
+        }
+        const uint32_t st_base = smem0 + (uint32_t)stage * stage_bytes;
+        const uint32_t a_kb = st_base + a_wg + (uint32_t)jj * a_bytes;
+        const uint32_t b_kb = p.bstat ? smemB + (uint32_t)kb * b_bytes : st_base + b_off + (uint32_t)jj * b_bytes;
+        wg_fence();
+#pragma unroll
+        for (int k = 0; k < KK; ++k)
+            Wg<KIND, BN>::mma(d, wg_desc(a_kb + 32u * (uint32_t)k, hi), wg_desc(b_kb + 32u * (uint32_t)k, hi),
+                              (kb > kb_begin || k > 0) ? 1u : 0u);
+        wg_commit();
+        wg_wait<1>();
+        if (pend >= 0) { release(pend); pend = -1; }
+        if (++jj == sps || kb + 1 == kb_end) {
+            pend = stage; jj = 0;
+            if (++stage == stages) { stage = 0; phase ^= 1u; }
+        }
+    }
+    wg_wait<0>();
+    wg_fence_operand(d);
+    if (pend >= 0) release(pend);
+}
+
 // One CTA per 128-pixel x BN-filter tile, persistent over the tiles (grid <= #SMs, one CTA per SM).
 // KS: compiled with the K-split tail schedule (TcParams::sk_T); the KS = false instantiations carry none of its code.
 // ST: compiled with the per-role cycle counters of YB_TC_STATS=1 (diagnostic); the production instantiations (ST = false)
 // contain no clock64() reads.
-// EPI: which epilogue family is compiled in -- 0: LSU stores, float kinds (bf16 / f32 heads / fused [yolo]); 1: TMA epilogue
-// (bf16 tiles stored with cp.async.bulk.tensor); 2: the integer kinds (s8 requantising and XNOR-as-+-1 epilogues).
+// EPI: which epilogue family is compiled in -- 0: LSU stores, float kinds (bf16 / f32 heads / fused [yolo]); 2: the integer
+// kinds (s8 requantising and XNOR-as-+-1 epilogues).  The bf16 stride-1 layers run k_conv_tc_reg.
 template <bool KS, bool ST, int EPI>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
@@ -395,10 +515,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
     const uint32_t smemB = (smem_u32(smem_raw) + 1023u) & ~1023u;   // 128B swizzle atoms are 1024B aligned
     const uint32_t smem0 = smemB + p.bstat_bytes;                   // [resident filter matrix][pipeline ring]
     const uint32_t bars = smem0 + (uint32_t)p.stages * p.stage_bytes;
-    auto full_bar = [&](int s) { return bars + 8u * (uint32_t)s; };
-    auto empty_bar = [&](int s) { return bars + 8u * (uint32_t)(p.stages + s); };
     const uint32_t bstat_bar = bars + 8u * (uint32_t)(2 * p.stages);
-    auto resfull_bar = [&](int g) { return bstat_bar + 8u + 8u * (uint32_t)g; };   // TMA epilogue: residual landed
     const uint32_t misc = (bstat_bar + 24u + 15u) & ~15u;
 
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
@@ -409,13 +526,9 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
         // full: one arrival (the producer's expect_tx); empty: one arrival per consumer warp
-        for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), TC_EPI_WARPS); }
+        for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar(bars, s), 1); mbar_init(empty_bar(bars, p.stages, s), TC_EPI_WARPS); }
         mbar_init(bstat_bar, 1);
-        mbar_init(resfull_bar(0), 1); mbar_init(resfull_bar(1), 1);
-        if (p.tma_epi) {
-            asm volatile("prefetch.tensormap [%0];" ::"l"(&tmO) : "memory");
-            if (p.res && EPI == 1) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmR) : "memory");
-        }
+        if (p.tma_epi) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmO) : "memory");
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     // bias (folded batch-norm) for all filter tiles -> shared memory, once per CTA
@@ -442,61 +555,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
 
     if (warp == TC_PRODUCER_WARP) {
         // ======================= TMA producer =======================
-        if (elect_one()) {
-            int stage = 0; uint32_t phase = 0;
-            long long w_empty = 0, w_tma = 0; const long long t_begin = ST ? clock64() : 0;
-            // loop-invariant parameters in registers; the (tap, channel-block) walk is incremental (no integer divisions per
-            // K-block in this single thread)
-            const int sps = p.sps, kblocks = p.kblocks, cblocks = p.cblocks, BK = p.BK, fsize = p.size, stages = p.stages;
-            const int xoff = p.xoff, yoff = p.yoff, stride2 = p.stride2, nt = p.nt, xt = p.xt;
-            const uint32_t a_bytes = p.a_bytes, b_bytes = p.b_bytes, stage_bytes = p.stage_bytes;
-            const uint32_t b_off = (uint32_t)sps * a_bytes;
-            const int bstat = p.bstat;
-            if (bstat) {   // resident filter matrix: kblocks boxes of [BN filters][BK], once
-                mbar_arrive_expect_tx(bstat_bar, p.bstat_bytes);
-                for (int kb = 0; kb < kblocks; ++kb) tma_load_2d(smemB + (uint32_t)kb * b_bytes, &tmB, bstat_bar, kb * BK, 0);
-            }
-            TcSched sch = sched_init<KS>(p, w_first, w_step);
-            int w, seg0, seg1;
-            while (sched_next<KS>(sch, w, seg0, seg1)) {
-                const int n_idx = w % nt;
-                const int m = w / nt;
-                const int x0 = (m % xt) * p.TW;
-                const int J0 = (m / xt) * p.TH + p.jshift;
-                const int n0 = n_idx * p.BN;
-                const int kb_begin = seg0 * sps, kb_end = min(kblocks, seg1 * sps);
-                // channel block, tap x/y, K column of the weight matrix at the first K-block of the segment
-                const int tap0 = kb_begin / cblocks;
-                int cb = kb_begin - tap0 * cblocks, ky = tap0 / fsize, kx = tap0 - (tap0 / fsize) * fsize, kcol = kb_begin * BK;
-                for (int kb0 = kb_begin; kb0 < kb_end; kb0 += sps) {
-                    const int nsub = min(sps, kb_end - kb0);
-                    if constexpr (ST) { const long long c0 = clock64(); mbar_wait(empty_bar(stage), phase ^ 1u); w_empty += clock64() - c0; }
-                    else mbar_wait(empty_bar(stage), phase ^ 1u);
-                    const uint32_t fb = full_bar(stage);
-                    const uint32_t a_dst = smem0 + (uint32_t)stage * stage_bytes;
-                    const uint32_t b_dst = a_dst + b_off;
-                    if (p.dbg & 1) {
-                        mbar_arrive(fb);
-                        if (++stage == stages) { stage = 0; phase ^= 1u; }
-                        continue;
-                    }
-                    mbar_arrive_expect_tx(fb, (uint32_t)nsub * (a_bytes + (bstat ? 0u : b_bytes)));
-                    const long long ct0 = ST ? clock64() : 0;
-                    for (int j = 0; j < nsub; ++j) {
-                        const uint32_t ad = a_dst + (uint32_t)j * a_bytes, bd = b_dst + (uint32_t)j * b_bytes;
-                        const int c0 = cb * BK;
-                        if (stride2) tma_load_5d(ad, &tmA, fb, c0, kx & 1, x0 + (kx >> 1), ky & 1, J0 + (ky >> 1));
-                        else tma_load_3d(ad, &tmA, fb, c0, x0 + kx + xoff, J0 + ky + yoff);
-                        if (!bstat) tma_load_2d(bd, &tmB, fb, kcol, n0);
-                        kcol += BK;
-                        if (++cb == cblocks) { cb = 0; if (++kx == fsize) { kx = 0; ++ky; } }
-                    }
-                    if constexpr (ST) w_tma += clock64() - ct0;
-                    if (++stage == stages) { stage = 0; phase ^= 1u; }
-                }
-            }
-            if (ST && p.stats) { p.stats[blockIdx.x * 16 + 0] = (unsigned long long)w_empty; p.stats[blockIdx.x * 16 + 1] = (unsigned long long)(clock64() - t_begin); p.stats[blockIdx.x * 16 + 7] = (unsigned long long)w_tma; }
-        }
+        if (elect_one()) tc_produce<KS, ST>(&tmA, &tmB, p, smemB, smem0, bars, w_first, w_step);
     } else {
         // ======================= consumers (warps 0..7): wgmma main loop, then the epilogue of the same tile =======================
         const int ew = warp;                      // consumer warp; warpgroup ew >> 2 computes accumulator rows 64 * (ew >> 2) .. + 63
@@ -504,52 +563,15 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
         int stage = 0; uint32_t phase = 0;
         long long w_full = 0;
         if (p.bstat) mbar_wait(bstat_bar, 0);
-        // The K-blocks of stages [seg0, seg1) of the current work item into this warpgroup's registers (KK wgmmas of K = 32 bytes
-        // per K-block), then both warpgroups' accumulators into the shared-memory tile.  A ring stage is released once the wgmmas
-        // that read it have retired, one stage behind the issue (wgmma.wait_group 1) so that the tensor pipe never drains.
+        // The K-blocks of stages [seg0, seg1) of the current work item into this warpgroup's registers, then both warpgroups'
+        // accumulators into the shared-memory tile.
         auto mainloop = [&](auto kind_c, auto bn_c, auto kk_c, int seg0, int seg1) {
             constexpr int KIND = decltype(kind_c)::value;
             constexpr int BN = decltype(bn_c)::value;
             constexpr int KK = decltype(kk_c)::value;   // wgmmas per K-block
             using T = typename std::conditional<KIND == 1 || KIND == 2, uint32_t, float>::type;
-            // Nothing but wgmmas touches the accumulators while wgmmas are in flight, and every batch is the same KK wgmmas:
-            // ptxas then inserts no fences of its own and serializes nothing (the -Xptxas -v log has no C75xx notes).
             T d[BN / 2];
-#pragma unroll
-            for (int i = 0; i < BN / 2; ++i) d[i] = T(0);
-            wg_fence_operand(d);
-            const int sps = p.sps, stages = p.stages;
-            const uint32_t a_bytes = p.a_bytes, b_bytes = p.b_bytes, stage_bytes = p.stage_bytes, hi = p.desc_hi;
-            const uint32_t b_off = (uint32_t)sps * a_bytes, a_wg = (uint32_t)wg * (a_bytes >> 1);
-            const int kb_begin = seg0 * sps, kb_end = min(p.kblocks, seg1 * sps);
-            auto release = [&](int s) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar(s)); };
-            // one commit group per K-block; a stage (sps K-blocks, fewer at the end of the segment) is released once the group of
-            // its last K-block has retired, which wgmma.wait_group 1 shows one K-block later
-            int pend = -1, jj = 0;
-            for (int kb = kb_begin; kb < kb_end; ++kb) {
-                if (jj == 0) {
-                    if constexpr (ST) { const long long c0 = clock64(); mbar_wait(full_bar(stage), phase); w_full += clock64() - c0; }
-                    else mbar_wait(full_bar(stage), phase);
-                }
-                const uint32_t st_base = smem0 + (uint32_t)stage * stage_bytes;
-                const uint32_t a_kb = st_base + a_wg + (uint32_t)jj * a_bytes;
-                const uint32_t b_kb = p.bstat ? smemB + (uint32_t)kb * b_bytes : st_base + b_off + (uint32_t)jj * b_bytes;
-                wg_fence();
-#pragma unroll
-                for (int k = 0; k < KK; ++k)
-                    Wg<KIND, BN>::mma(d, wg_desc(a_kb + 32u * (uint32_t)k, hi), wg_desc(b_kb + 32u * (uint32_t)k, hi),
-                                      (kb > kb_begin || k > 0) ? 1u : 0u);
-                wg_commit();
-                wg_wait<1>();
-                if (pend >= 0) { release(pend); pend = -1; }
-                if (++jj == sps || kb + 1 == kb_end) {
-                    pend = stage; jj = 0;
-                    if (++stage == stages) { stage = 0; phase ^= 1u; }
-                }
-            }
-            wg_wait<0>();
-            wg_fence_operand(d);
-            if (pend >= 0) release(pend);
+            tc_mma_loop<KIND, BN, KK, ST>(d, p, smemB, smem0, bars, wg, lane, stage, phase, w_full, seg0, seg1);
             named_bar_sync(TC_ACC_BAR, 32 * TC_EPI_WARPS);   // every warp is done with the previous tile's accumulators
             acc_store_frag(acc_base, p.acc_pitch, wg * 64, d);
             named_bar_sync(TC_ACC_BAR, 32 * TC_EPI_WARPS);   // the whole 128 x BN tile is in place
@@ -566,7 +588,6 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                 else by_kk(kind_c, std::integral_constant<int, 32>{});
             };
             if constexpr (EPI == 2) by_bn(std::integral_constant<int, 1>{});
-            else if constexpr (EPI == 1) by_bn(std::integral_constant<int, 0>{});
             else if (p.kind == 0) by_bn(std::integral_constant<int, 0>{});
             else by_bn(std::integral_constant<int, 3>{});
         };
@@ -580,9 +601,6 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
         const int tx = r & (p.TW - 1), ty = r >> p.TWlog2;
         const bool leaky = p.act == ACT_LEAKY, leaky2 = p.act2 == ACT_LEAKY;
         const uint32_t taddr = acc_base + 4u * (uint32_t)(r * p.acc_pitch);
-        uint32_t epi_res_phase = 0;               // TMA epilogue: parity of this group's residual barrier
-        bool res_requested = false;               // TMA epilogue: the residual tile of the slab about to be processed is on its way
-        int out_buf = 0;                          // TMA epilogue: which of the group's epi_bufs OUT tiles the next slab uses
         long long w_res = 0; const long long t_begin = ST ? clock64() : 0;
         TcSched sch = sched_init<KS>(p, w_first, w_step);
         int w, seg0, seg1;
@@ -838,11 +856,10 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
             // the 128B swizzle, written by one thread per row and stored by one cp.async.bulk.tensor
             auto tma_store_f32_slab = [&](const float (&y)[32], int f0) {
                 const int g = half;
-                const uint32_t out_tile = stg_base + (uint32_t)(g * p.epi_bufs + out_buf) * 16384u;
+                const uint32_t out_tile = stg_base + (uint32_t)g * 16384u;
                 const bool boss = (q == 0) && (lane == 0);
                 const uint32_t rsw = (uint32_t)(r & 7), row_off = (uint32_t)r * 128u;
-                if (boss) { if (p.epi_bufs == 2) tma_store_wait_read1(); else tma_store_wait_read0(); }   // the store that last used this tile has finished reading it
-                if (p.epi_bufs == 2) out_buf ^= 1;
+                if (boss) tma_store_wait_read0();   // the store that last used this tile has finished reading it
                 named_bar_sync(1 + g, 128);
 #pragma unroll
                 for (int c = 0; c < 8; ++c) {
@@ -860,95 +877,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                 }
             };
 
-            if constexpr (EPI == 1) {
-                // ---- TMA epilogue.  Group g = the four warps that own column half `half` (128 threads, named barrier 1 + half);
-                // per slab of SW = 64 (or 32) columns: [OUT tile][RES tile], both [128 pixel rows][SW * 2 bytes] with the swizzle of
-                // the tensor maps -- 16-byte chunk c of row r at r*128 + ((c ^ (r & 7)) << 4) for 128-byte rows, at r*64 +
-                // ((c ^ ((r >> 1) & 3)) << 4) for 64-byte rows: conflict-free for one thread per row.
-                auto slabs = [&](auto nv_c) {
-                    constexpr int NV = decltype(nv_c)::value;          // 32-column accumulator reads per slab: 2 (SW = 64) or 1 (SW = 32)
-                    constexpr int SW = 32 * NV;
-                    constexpr uint32_t tile_bytes = 128u * SW * 2u, rowb = SW * 2u;
-                    const int g = half;
-                    const uint32_t grp_base = stg_base + (uint32_t)g * ((uint32_t)(p.epi_bufs + 1) * tile_bytes);   // [OUT x epi_bufs][RES]
-                    const uint32_t res_tile = grp_base + (uint32_t)p.epi_bufs * tile_bytes;
-                    const bool boss = (q == 0) && (lane == 0);           // issues this group's TMA traffic
-                    const int x0 = (m % p.xt) * p.TW, J0 = (m / p.xt) * p.TH + p.jshift;
-                    const uint32_t rsw = (NV == 2) ? (uint32_t)(r & 7) : (uint32_t)((r >> 1) & 3);
-                    const uint32_t row_off = (uint32_t)r * rowb;
-                    const bool has_res = p.res != nullptr;
-                    // residual tiles are requested one slab AHEAD, across tile boundaries (the next work item of this group is
-                    // known: w + step): the TMA latency hides behind the store phase of this slab and the accumulator wait of the next
-                                        auto request_res = [&](int w_, int f_) {
-                        const int m_ = w_ / p.nt;
-                        mbar_arrive_expect_tx(resfull_bar(g), tile_bytes);
-                        if (p.l2_hint) tma_load_3d_hint(res_tile, &tmR, resfull_bar(g), (w_ % p.nt) * p.BN + f_, (m_ % p.xt) * p.TW + 1, (m_ / p.xt) * p.TH + p.jshift, l2_policy_evict_first());
-                        else tma_load_3d(res_tile, &tmR, resfull_bar(g), (w_ % p.nt) * p.BN + f_, (m_ % p.xt) * p.TW + 1, (m_ / p.xt) * p.TH + p.jshift);
-                    };
-                    if (has_res && boss && !res_requested && cbeg < cend) request_res(w, cbeg);   // very first slab of this group
-                    res_requested = true;
-                    for (int f0 = cbeg; f0 < cend; f0 += SW) {
-                        uint32_t v[NV][32];
-#pragma unroll
-                        for (int h2 = 0; h2 < NV; ++h2) acc_ld32(taddr + 4u * (uint32_t)(f0 + 32 * h2), v[h2]);
-#pragma unroll
-                        for (int h2 = 0; h2 < NV; ++h2)
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) {
-                                const float a0 = __uint_as_float(v[h2][j]) + bs[f0 + 32 * h2 + j];
-                                v[h2][j] = __float_as_uint(leaky ? fmaxf(a0, 0.1f * a0) : a0);
-                            }
-                        if (has_res) {
-                            if constexpr (ST) { const long long c0 = clock64(); mbar_wait(resfull_bar(g), epi_res_phase); w_res += clock64() - c0; }
-                            else mbar_wait(resfull_bar(g), epi_res_phase);
-                            epi_res_phase ^= 1u;
-#pragma unroll
-                            for (int c = 0; c < 4 * NV; ++c) {             // own row of the residual tile, 16 bytes at a time
-                                uint32_t w0, w1, w2, w3;
-                                asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(w0), "=r"(w1), "=r"(w2), "=r"(w3)
-                                             : "r"(res_tile + row_off + (((uint32_t)c ^ rsw) << 4)) : "memory");
-                                const uint32_t wv[4] = {w0, w1, w2, w3};
-#pragma unroll
-                                for (int h = 0; h < 4; ++h) {
-                                    uint32_t &lo_ = v[c / 4][(c % 4) * 8 + 2 * h], &hi_ = v[c / 4][(c % 4) * 8 + 2 * h + 1];
-                                    float a = __uint_as_float(lo_) + __uint_as_float(wv[h] << 16);
-                                    float b = __uint_as_float(hi_) + __uint_as_float(wv[h] & 0xffff0000u);
-                                    if (leaky2) { a = fmaxf(a, 0.1f * a); b = fmaxf(b, 0.1f * b); }
-                                    lo_ = __float_as_uint(a); hi_ = __float_as_uint(b);
-                                }
-                            }
-                        }
-                        // the TMA store that last used this OUT tile must have finished READING it before it is overwritten
-                        const uint32_t out_tile = grp_base + (uint32_t)out_buf * tile_bytes;
-                        if (boss) { if (p.epi_bufs == 2) tma_store_wait_read1(); else tma_store_wait_read0(); }
-                        if (p.epi_bufs == 2) out_buf ^= 1;
-                        named_bar_sync(1 + g, 128);
-                        if (has_res && boss) {                             // everybody is done with the RES tile: request the next one
-                            if (f0 + SW < cend) request_res(w, f0 + SW);
-                            else if (w + w_step < p.num_work) request_res(w + w_step, cbeg);
-                        }
-#pragma unroll
-                        for (int c = 0; c < 4 * NV; ++c) {                 // own row -> OUT tile (border / padding rows: zeros)
-                            const uint32_t *src = &v[c / 4][(c % 4) * 8];
-                            uint32_t o0 = pack_bf16x2(__uint_as_float(src[0]), __uint_as_float(src[1]));
-                            uint32_t o1 = pack_bf16x2(__uint_as_float(src[2]), __uint_as_float(src[3]));
-                            uint32_t o2 = pack_bf16x2(__uint_as_float(src[4]), __uint_as_float(src[5]));
-                            uint32_t o3 = pack_bf16x2(__uint_as_float(src[6]), __uint_as_float(src[7]));
-                            if (!valid) { o0 = o1 = o2 = o3 = 0u; }
-                            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(out_tile + row_off + (((uint32_t)c ^ rsw) << 4)),
-                                         "r"(o0), "r"(o1), "r"(o2), "r"(o3) : "memory");
-                        }
-                        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the TMA engine
-                        named_bar_sync(1 + g, 128);
-                        if (boss) {
-                            tma_store_3d(&tmO, out_tile, n0 + f0, x0 + 1, J0);
-                            tma_store_commit();
-                        }
-                    }
-                };
-                if (p.tma_epi == 64) slabs(std::integral_constant<int, 2>{});
-                else slabs(std::integral_constant<int, 1>{});
-            } else if constexpr (EPI == 2) {
+            if constexpr (EPI == 2) {
             if (p.kind == 2) {
                 // ---- XNOR as +-1 int8: acc == 2*count - K (exact); out = act((float)acc * mean + bias) in the reference's
                 // float op order (additionally.c:1531, yolov2_forward_network.c:243-261)
@@ -1189,10 +1118,185 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
             }
             }
         }
-        if ((EPI == 1 || (EPI == 2 && p.tma_epi)) && q == 0 && lane == 0) tma_store_wait_all();   // this group's bulk stores have completed
+        if (EPI == 2 && p.tma_epi && q == 0 && lane == 0) tma_store_wait_all();   // this group's bulk stores have completed
         if (ST && p.stats && ew == 0 && lane == 0) { p.stats[blockIdx.x * 16 + 2] = (unsigned long long)w_full; p.stats[blockIdx.x * 16 + 6] = (unsigned long long)(clock64() - t_begin);
                                                      p.stats[blockIdx.x * 16 + 8] = (unsigned long long)w_res; }
     }
+}
+
+// Register-accumulator kernel of the bf16-output, stride-1 layers (384 threads).  Warpgroup 2 is the TMA producer (one elected
+// thread; the warpgroup gives its registers away with setmaxnreg), warpgroups 0 and 1 are consumers with up to 216 registers
+// each: a consumer warpgroup keeps the f32 accumulators of its 64 rows x BN (<= 256) filters of the tile in registers and runs
+// the epilogue straight on its wgmma fragment -- bias, leaky, the fused shortcut residual and the second leaky in fp32, then
+// round to bf16 -- writing SW-column slabs (SW = 64, or 32 when BN == 32) into a swizzled shared-memory tile that one thread
+// stores with cp.async.bulk.tensor.  The residual slab comes in the same way, one slab ahead (across work items), with the L2
+// evict-first hint.  No shared-memory accumulator tile and no barrier between the two consumer warpgroups: the shared memory
+// goes to the ring, and each warpgroup stores its half tile (64 pixels) on its own.
+constexpr int TCR_THREADS = 384;
+constexpr int TCR_PRODUCER_REGS = 40, TCR_CONSUMER_REGS = 216;   // 128 * 40 + 256 * 216 <= 64 K registers
+
+template <bool ST>
+__global__ void __launch_bounds__(TCR_THREADS, 1)
+k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
+              const __grid_constant__ CUtensorMap tmR, const TcParams p) {
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t smemB = (smem_u32(smem_raw) + 1023u) & ~1023u;   // [resident filter matrix][pipeline ring][barriers][bias][epilogue tiles]
+    const uint32_t smem0 = smemB + p.bstat_bytes;
+    const uint32_t bars = smem0 + (uint32_t)p.stages * p.stage_bytes;
+    const uint32_t bstat_bar = bars + 8u * (uint32_t)(2 * p.stages);
+    auto resfull_bar = [&](int g) { return bstat_bar + 8u + 8u * (uint32_t)g; };   // residual slab of warpgroup g landed
+    const uint32_t misc = (bstat_bar + 24u + 15u) & ~15u;
+    float *bias_s = reinterpret_cast<float *>(smem_raw + (misc - smem_u32(smem_raw)));
+    // per consumer warpgroup: [OUT 0][OUT 1][RES], each 64 pixel rows x SW bf16 with the tensor maps' swizzle (1024-byte aligned)
+    const uint32_t epi_base = (misc + 4u * (uint32_t)(p.nt * p.BN) + (uint32_t)(p.nt * p.BN / 8) + 1023u) & ~1023u;
+
+    const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+    const int lane = threadIdx.x & 31;
+    const int wg = warp >> 2;
+    const int w_first = (int)blockIdx.x, w_step = (int)gridDim.x;
+
+    if (warp == 8 && elect_one()) {
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmO) : "memory");
+        if (p.res) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmR) : "memory");
+        for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar(bars, s), 1); mbar_init(empty_bar(bars, p.stages, s), TC_EPI_WARPS); }
+        mbar_init(bstat_bar, 1);
+        mbar_init(resfull_bar(0), 1); mbar_init(resfull_bar(1), 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    for (int i = threadIdx.x; i < p.nt * p.BN; i += TCR_THREADS) bias_s[i] = (i < p.n) ? __ldg(p.bias + i) : 0.f;
+    __syncthreads();
+    // Programmatic dependent launch: everything above overlapped the tail of the previous kernel
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+
+    if (wg == 2) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(TCR_PRODUCER_REGS));
+        if (warp == 8 && elect_one()) tc_produce<false, ST>(&tmA, &tmB, p, smemB, smem0, bars, w_first, w_step);
+        return;
+    }
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(TCR_CONSUMER_REGS));
+
+    // ======================= consumers: warpgroup wg owns rows 64 wg .. + 63 of every tile =======================
+    // wgmma fragment: this thread holds rows rl and rl + 8 (of the warpgroup's 64), columns 8 j + cq, 8 j + cq + 1
+    const int rl = 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);
+    const bool boss = (warp & 3) == 0 && lane == 0;    // issues this warpgroup's epilogue TMA traffic
+    const bool leaky = p.act == ACT_LEAKY, leaky2 = p.act2 == ACT_LEAKY;
+    const bool epi_mem = !(p.dbg & 4);
+    const bool has_res = p.res != nullptr && epi_mem;
+    // the half tile as a TMA box: 64 of the TW x TH pixels (TW == 128: one half row; else TH / 2 whole rows)
+    const int hx = (p.TW == 128) ? 64 * wg : 0, hy = (p.TW == 128) ? 0 : wg * (p.TH >> 1);
+    int stage = 0; uint32_t phase = 0;
+    uint32_t res_phase = 0;
+    int out_buf = 0;
+    long long w_full = 0, w_res = 0; const long long t_begin = ST ? clock64() : 0;
+    if (p.bstat) mbar_wait(bstat_bar, 0);
+
+    auto run = [&](auto bn_c, auto kk_c) {
+        constexpr int BN = decltype(bn_c)::value;
+        constexpr int KK = decltype(kk_c)::value;
+        constexpr int SW = BN >= 64 ? 64 : 32;             // slab width (columns); rows of 128 B (128B swizzle) or 64 B (64B swizzle)
+        constexpr uint32_t ROWB = SW * 2, TILE = 64u * ROWB;
+        const uint32_t grp = epi_base + (uint32_t)wg * 3u * TILE, res_tile = grp + 2u * TILE;
+        // byte offset of (row, 16-byte chunk c) in a slab tile + this thread's column pair: conflict-free for the fragment layout
+        auto slab_off = [&](int row, int c) -> uint32_t {
+            const int sw = (SW == 64) ? (row & 7) : ((row >> 1) & 3);
+            return (uint32_t)row * ROWB + ((uint32_t)(c ^ sw) << 4) + 2u * (uint32_t)cq;
+        };
+        auto request_res = [&](int w_, int f_) {
+            const int m_ = w_ / p.nt;
+            const int c0 = (w_ % p.nt) * BN + f_, x = (m_ % p.xt) * p.TW + 1 + hx, y = (m_ / p.xt) * p.TH + p.jshift + hy;
+            mbar_arrive_expect_tx(resfull_bar(wg), TILE);
+            if (p.l2_hint) tma_load_3d_hint(res_tile, &tmR, resfull_bar(wg), c0, x, y, l2_policy_evict_first());
+            else tma_load_3d(res_tile, &tmR, resfull_bar(wg), c0, x, y);
+        };
+        if (has_res && boss && w_first < p.num_work) request_res(w_first, 0);
+        for (int w = w_first; w < p.num_work; w += w_step) {
+            float d[BN / 2];
+            tc_mma_loop<0, BN, KK, ST>(d, p, smemB, smem0, bars, wg, lane, stage, phase, w_full, 0, p.kbs);
+            if (!epi_mem) continue;
+            const int n0 = (w % p.nt) * BN, m = w / p.nt;
+            const int x0 = (m % p.xt) * p.TW, J0 = (m / p.xt) * p.TH + p.jshift;
+            bool valid[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {                  // border / padding rows of the merged-row tiling are stored as zeros
+                const int r = 64 * wg + rl + 8 * h;
+                const int ox = x0 + (r & (p.TW - 1)), J = J0 + (r >> p.TWlog2);
+                const int img = J / p.PR, oy = J - img * p.PR - p.row_off;
+                valid[h] = img < p.N && oy >= 0 && oy < p.OH && ox < p.OW;
+            }
+            const int nslab = (min(BN, p.n - n0) + SW - 1) / SW;   // slabs holding filters < n
+#pragma unroll
+            for (int s = 0; s < BN / SW; ++s) {
+                if (s >= nslab) break;
+#pragma unroll
+                for (int jj = 0; jj < SW / 8; ++jj) {
+                    const int j = s * (SW / 8) + jj;
+                    const float2 b = *reinterpret_cast<const float2 *>(bias_s + n0 + 8 * j + cq);
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        const float a = d[4 * j + e] + ((e & 1) ? b.y : b.x);
+                        d[4 * j + e] = leaky ? fmaxf(a, 0.1f * a) : a;   // == a > 0 ? a : 0.1a
+                    }
+                }
+                if (has_res) {
+                    if constexpr (ST) { const long long c0 = clock64(); mbar_wait(resfull_bar(wg), res_phase); w_res += clock64() - c0; }
+                    else mbar_wait(resfull_bar(wg), res_phase);
+                    res_phase ^= 1u;
+#pragma unroll
+                    for (int jj = 0; jj < SW / 8; ++jj) {
+                        const int j = s * (SW / 8) + jj;
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            uint32_t u;
+                            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(u) : "r"(res_tile + slab_off(rl + 8 * h, jj)) : "memory");
+                            float a = d[4 * j + 2 * h] + __uint_as_float(u << 16);
+                            float c = d[4 * j + 2 * h + 1] + __uint_as_float(u & 0xffff0000u);
+                            if (leaky2) { a = fmaxf(a, 0.1f * a); c = fmaxf(c, 0.1f * c); }
+                            d[4 * j + 2 * h] = a; d[4 * j + 2 * h + 1] = c;
+                        }
+                    }
+                }
+                // the bulk store that last read this OUT tile (two slabs ago) must be done reading it
+                const uint32_t out_tile = grp + (uint32_t)out_buf * TILE;
+                if (boss) tma_store_wait_read1();
+                named_bar_sync(1 + wg, 128);
+                if (has_res && boss) {                         // everybody is done with the RES tile: request the next slab
+                    if (s + 1 < nslab) request_res(w, (s + 1) * SW);
+                    else if (w + w_step < p.num_work) request_res(w + w_step, 0);
+                }
+#pragma unroll
+                for (int jj = 0; jj < SW / 8; ++jj) {
+                    const int j = s * (SW / 8) + jj;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const uint32_t o = valid[h] ? pack_bf16x2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]) : 0u;
+                        asm volatile("st.shared.b32 [%0], %1;" ::"r"(out_tile + slab_off(rl + 8 * h, jj)), "r"(o) : "memory");
+                    }
+                }
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the TMA engine
+                named_bar_sync(1 + wg, 128);
+                if (boss) {
+                    tma_store_3d(&tmO, out_tile, n0 + s * SW, x0 + 1 + hx, J0 + hy);
+                    tma_store_commit();
+                }
+                out_buf ^= 1;
+            }
+        }
+    };
+    auto by_kk = [&](auto bn_c) {
+        if (p.kk == 4) run(bn_c, std::integral_constant<int, 4>{});
+        else if (p.kk == 2) run(bn_c, std::integral_constant<int, 2>{});
+        else run(bn_c, std::integral_constant<int, 1>{});
+    };
+    if (p.BN == 256) by_kk(std::integral_constant<int, 256>{});
+    else if (p.BN == 128) by_kk(std::integral_constant<int, 128>{});
+    else if (p.BN == 64) by_kk(std::integral_constant<int, 64>{});
+    else by_kk(std::integral_constant<int, 32>{});
+    if (boss) tma_store_wait_all();   // this warpgroup's bulk stores have completed (shared memory stays valid until then)
+    if (ST && p.stats && warp == 0 && lane == 0) { p.stats[blockIdx.x * 16 + 2] = (unsigned long long)w_full; p.stats[blockIdx.x * 16 + 6] = (unsigned long long)(clock64() - t_begin);
+                                                    p.stats[blockIdx.x * 16 + 8] = (unsigned long long)w_res; }
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -1396,6 +1500,7 @@ struct TcPlan {
     CUtensorMap tmA, tmB, tmO, tmR;   // activation, filters; TMA epilogue: output, residual
     TcParams p;
     int grid;
+    int threads;                      // TC_THREADS (k_conv_tc) or TCR_THREADS (k_conv_tc_reg)
     size_t smem;
     int pdl;
     char desc[96];
@@ -1404,8 +1509,30 @@ struct TcPlan {
 int pick_bk(int C) { return (C % 64 == 0) ? 64 : (C % 32 == 0) ? 32 : (C % 16 == 0) ? 16 : 0; }
 int pick_bk_i8(int cpad) { return (cpad % 128 == 0) ? 128 : (cpad % 64 == 0) ? 64 : (cpad % 32 == 0) ? 32 : 0; }
 int pick_bk_f32(int C) { return (C % 32 == 0) ? 32 : (C % 16 == 0) ? 16 : (C % 8 == 0) ? 8 : 0; }
-// at most 128 filters per tile: the [128][BN + 4] f32 accumulator tile shares the 227 KB of shared memory with the ring
+// k_conv_tc: at most 128 filters per tile -- the [128][BN + 4] f32 accumulator tile shares the 227 KB of shared memory with the ring
 int pick_bn(int n) { return n <= 32 ? 32 : n <= 64 ? 64 : 128; }
+// k_conv_tc_reg: BN in {32, 64, 128, 256} (no wider than the filters need) with the least wave-quantised cost
+//     ceil(work items / SMs) * (K-blocks * (BN + 64) + 2 * BN).
+// A K-block of a 128 x BN tile feeds 128 activation rows and BN filter rows for BN columns of MMA work: the + 64 charges the
+// activation tile's share of the feed, 2 * BN the register epilogue.  E.g. 1x1 512 -> 256 at 38x38, batch 16: 380 work items
+// at BN = 128 (3 waves) against 190 at BN = 256 (2 waves of double-length tiles), and BN = 128 is cheaper.
+// YB_TC_BN=32/64/128/256 takes that width instead (capped at the filters' width; A/B experiments).
+int pick_bn_reg(int n, long m_tiles, int kblocks, int sms) {
+    int cap = 32;
+    while (cap < n && cap < 256) cap *= 2;
+    if (const char *e = getenv("YB_TC_BN")) {
+        int bn = 32;
+        while (bn * 2 <= std::min(atoi(e), cap)) bn *= 2;
+        return bn;
+    }
+    int best = 32; double best_cost = 1e300;
+    for (int bn = 32; bn <= cap; bn *= 2) {
+        const long items = m_tiles * ((n + bn - 1) / bn);
+        const double cost = (double)((items + sms - 1) / sms) * ((double)kblocks * (bn + 64) + 2.0 * bn);
+        if (cost < best_cost) { best_cost = cost; best = bn; }
+    }
+    return best;
+}
 
 }  // namespace
 
@@ -1432,13 +1559,19 @@ static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &
     const bool i8 = kind == 1 || kind == 2;
     const int esz = kind == 3 ? 4 : i8 ? 1 : 2;              // operand element size
     const int cin = i8 ? in.ldc : l.c;                       // s8: channels padded with zeros in both operands
-    const int BK = kind == 3 ? pick_bk_f32(l.c) : i8 ? pick_bk_i8(cin) : pick_bk(l.c), BN = pick_bn(l.n);
+    const int BK = kind == 3 ? pick_bk_f32(l.c) : i8 ? pick_bk_i8(cin) : pick_bk(l.c);
+    // bf16 NHWC output of a stride-1 layer: the register-accumulator kernel with its TMA epilogue
+    // (stride-2 layers keep the LSU epilogue: their tiles walk the input's merged half-rows, OH + 1 per image, while the output has
+    // OH + 2 rows per image -- a per-image (c, x, y, image) store would need a negative start row for the second image of a
+    // straddling tile, and bulk tensor STORES fault on negative coordinates)
+    const bool reg = kind == 0 && out_bf16 && l.stride == 1 && !no_tma_epi && !getenv("YB_TC_NO_TMA_EPI") &&
+                     !getenv("YB_TC_NO_COALESCE") && (!res.base || res_bf16);
     p.kind = kind; p.alpha1 = alpha1; p.acc_out = acc_out;
     p.kk = BK * esz / 32;
     const bool s2 = l.stride == 2;
     p.N = in.N;
     p.OH = l.out_h; p.OW = l.out_w; p.OHp = out.Hp; p.OWp = out.Wp;
-    p.size = l.size; p.BK = BK; p.BN = BN;
+    p.size = l.size; p.BK = BK;
     p.cblocks = cin / BK; p.kblocks = l.size * l.size * p.cblocks;
     p.stride2 = s2 ? 1 : 0;
     p.xoff = 1 - l.pad; p.yoff = -l.pad;
@@ -1471,9 +1604,11 @@ static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &
     int sms = 132;
     { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); }
     const uint32_t row_bytes = (uint32_t)(BK * esz);
-    p.nt = (l.n + BN - 1) / BN;
     p.xt = (p.OW + p.TW - 1) / p.TW;
     p.jt = (int)((rows - p.jshift + p.TH - 1) / p.TH);
+    const int BN = reg ? pick_bn_reg(l.n, (long)p.xt * p.jt, p.kblocks, sms) : pick_bn(l.n);
+    p.BN = BN;
+    p.nt = (l.n + BN - 1) / BN;
     p.num_tiles = p.xt * p.jt * p.nt;
     p.num_work = p.num_tiles;
     p.a_bytes = (uint32_t)(TC_BM * BK * esz);
@@ -1481,26 +1616,16 @@ static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &
     // small filter matrices stay resident in shared memory for the whole kernel (one TMA pass per CTA)
     p.bstat = (p.nt == 1 && (size_t)p.kblocks * p.b_bytes <= 48 * 1024 && !getenv("YB_TC_NO_BSTAT")) ? 1 : 0;
     p.bstat_bytes = p.bstat ? (uint32_t)p.kblocks * p.b_bytes : 0u;
-    // TMA epilogue: bf16 NHWC output of a stride-1 layer, 32-column slabs (8 KB tiles: no more shared memory than the LSU
-    // staging, so the ring stays deep beside the accumulator tile)
+    // TMA epilogue: slab width in columns.  k_conv_tc_reg: bf16 slabs of 64 columns (32 when BN == 32), per consumer warpgroup
+    // [OUT 0][OUT 1][RES] tiles of 64 pixels; integer kinds: f32 slabs of 32 columns (128-byte rows), one 128-pixel tile per warp
+    // group -- the raw-accumulator dump (tests) keeps the LSU path
     p.tma_epi = 0;
     const bool i8kind = kind == 1 || kind == 2;
-    // (stride-2 layers keep the LSU epilogue: their tiles walk the input's merged half-rows, OH + 1 per image, while the output has
-    // OH + 2 rows per image -- a per-image (c, x, y, image) store would need a negative start row for the second image of a
-    // straddling tile, and bulk tensor STORES fault on negative coordinates)
-    if (kind == 0 && out_bf16 && !s2 && BN >= 32 && !no_tma_epi && !getenv("YB_TC_NO_TMA_EPI") &&
-        !getenv("YB_TC_NO_COALESCE") && (!res.base || res_bf16)) {
-        p.tma_epi = 32;
-        if (getenv("YB_TC_TMA_EPI_SW")) p.tma_epi = (atoi(getenv("YB_TC_TMA_EPI_SW")) == 64 && BN >= 128) ? 64 : 32;
-    }
-    // integer kinds: f32 slabs of 32 columns (128-byte rows) stored by TMA; the raw-accumulator dump (tests) keeps the LSU path
+    if (reg) p.tma_epi = BN >= 64 ? 64 : 32;
     if (i8kind && !s2 && !acc_out && !getenv("YB_TC_NO_TMA_EPI") && !getenv("YB_TC_NO_COALESCE")) p.tma_epi = 32;
-    p.epi_bufs = (getenv("YB_TC_EPI_BUFS") && p.tma_epi && atoi(getenv("YB_TC_EPI_BUFS")) == 2) ? 2 : 1;
-    const size_t epi_tile = i8kind ? 16384 : (size_t)128 * p.tma_epi * 2;
-    const size_t epi_tiles_bytes = !p.tma_epi ? 0 : i8kind ? 2 * p.epi_bufs * epi_tile : 2 * (p.epi_bufs + 1) * epi_tile;
-    p.stg_bytes = (uint32_t)(p.tma_epi ? std::max<size_t>(epi_tiles_bytes, 4 * (size_t)(128 * p.tma_epi * 2)) : 4096 * TC_EPI_WARPS);
+    p.stg_bytes = reg ? 2u * 3u * 64u * (uint32_t)p.tma_epi * 2u : p.tma_epi ? 2u * 16384u : 4096u * TC_EPI_WARPS;
     p.acc_pitch = BN + 4;
-    const size_t acc_bytes = (size_t)TC_BM * p.acc_pitch * 4;
+    const size_t acc_bytes = reg ? 0 : (size_t)TC_BM * p.acc_pitch * 4;   // k_conv_tc_reg keeps the accumulators in registers
     // what is left of 227 KB beside the epilogue tiles and the accumulator tile (5 KB: barriers, alignment slack)
     const size_t ring_budget = (size_t)(227 - 5) * 1024 - p.stg_bytes - acc_bytes;
     // several K-blocks per stage when they are small: fewer barrier round trips per K
@@ -1536,7 +1661,7 @@ static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &
     p.dbg = getenv("YB_TC_DBG") ? atoi(getenv("YB_TC_DBG")) : 0;
     p.l2_hint = (kind == 0 && !getenv("YB_TC_NO_L2_HINT")) ? 1 : 0;
     p.no_coalesce = getenv("YB_TC_NO_COALESCE") ? 1 : 0;
-    snprintf(plan->desc, sizeof(plan->desc), "%dx%dx%d -> n%d k%d s%d%s", l.c, l.h, l.w, l.n, l.size, l.stride, p.tma_epi ? " tepi" : "");
+    snprintf(plan->desc, sizeof(plan->desc), "%dx%dx%d -> n%d k%d s%d%s", l.c, l.h, l.w, l.n, l.size, l.stride, reg ? " reg" : "");
 
     const CUtensorMapSwizzle swz = row_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
                                  : row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
@@ -1581,7 +1706,9 @@ static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &
             // slab of a pixel tile
             cuuint64_t dims[3] = {(cuuint64_t)l.n, (cuuint64_t)t.Wp, (cuuint64_t)t.N * t.Hp};
             cuuint64_t strides[2] = {(cuuint64_t)t.ldc * oesz, (cuuint64_t)t.Wp * t.ldc * oesz};
-            cuuint32_t box[3] = {(cuuint32_t)p.tma_epi, (cuuint32_t)p.TW, (cuuint32_t)p.TH};
+            // (k_conv_tc_reg: half a tile, the 64 pixels of one consumer warpgroup)
+            cuuint32_t box[3] = {(cuuint32_t)p.tma_epi, (cuuint32_t)std::min(p.TW, reg ? 64 : 128),
+                                 (cuuint32_t)(reg ? std::max(p.TH / 2, 1) : p.TH)};
             cuuint32_t es[3] = {1, 1, 1};
             CUresult rr = enc(tm, out_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, t.base, dims, strides, box, es,
                               CU_TENSOR_MAP_INTERLEAVE_NONE, p.tma_epi * oesz == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
@@ -1593,19 +1720,20 @@ static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &
     }
     plan->pdl = (getenv("YB_NO_PDL") == nullptr) ? 1 : 0;
     plan->grid = std::min(p.num_tiles, sms);
+    plan->threads = reg ? TCR_THREADS : TC_THREADS;
     if (getenv("YB_TC_STATS")) {
         cudaMalloc(&p.stats, sizeof(unsigned long long) * 16 * plan->grid);
         cudaMemset(p.stats, 0, sizeof(unsigned long long) * 16 * plan->grid);
     }
     plan->smem = 1024 /*alignment slack*/ + p.bstat_bytes + (size_t)p.stages * p.stage_bytes + 8 * (2 * p.stages + 3) + 16 +
                  sizeof(float) * (size_t)p.nt * BN /*bias*/ + (size_t)p.nt * BN / 8 /*yolo mask*/ +
-                 (p.tma_epi ? 1024 : 128) + p.stg_bytes /*epilogue staging or TMA-epilogue tiles: [OUT x bufs | RES] per warp group*/ +
+                 (p.tma_epi ? 1024 : 128) + p.stg_bytes /*epilogue staging or TMA-epilogue tiles*/ +
                  acc_bytes /*accumulator tile*/;
     if (plan->smem > 227 * 1024) { delete plan; fatal_throw("tc plan: shared memory budget exceeded"); }
     {
-        const void *fns[] = {(const void *)k_conv_tc<false, false, 0>, (const void *)k_conv_tc<false, false, 1>,
+        const void *fns[] = {(const void *)k_conv_tc<false, false, 0>, (const void *)k_conv_tc_reg<false>,
                              (const void *)k_conv_tc<false, false, 2>, (const void *)k_conv_tc<true, false, 0>,
-                             (const void *)k_conv_tc<false, true, 0>, (const void *)k_conv_tc<false, true, 1>,
+                             (const void *)k_conv_tc<false, true, 0>, (const void *)k_conv_tc_reg<true>,
                              (const void *)k_conv_tc<false, true, 2>};
         for (const void *f : fns)
             if (cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
@@ -1765,7 +1893,7 @@ void tc_stem_free_plan(void *vp) { delete reinterpret_cast<StemPlan *>(vp); }
 void tc_launch(void *vp, cudaStream_t s) {
     TcPlan *plan = reinterpret_cast<TcPlan *>(vp);
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)plan->grid); cfg.blockDim = dim3(TC_THREADS);
+    cfg.gridDim = dim3((unsigned)plan->grid); cfg.blockDim = dim3((unsigned)plan->threads);
     cfg.dynamicSmemBytes = plan->smem; cfg.stream = s;
     cudaLaunchAttribute attr[2];
     int na = 0;
@@ -1775,14 +1903,17 @@ void tc_launch(void *vp, cudaStream_t s) {
         ++na;
     }
     cfg.attrs = attr; cfg.numAttrs = na;
-    const int epi = (plan->p.kind == 1 || plan->p.kind == 2) ? 2 : plan->p.tma_epi ? 1 : 0;
+    const int epi = (plan->p.kind == 1 || plan->p.kind == 2) ? 2 : plan->p.tma_epi ? 1 : 0;   // 1: k_conv_tc_reg
     static const bool ks_always = getenv("YB_TC_KS_ALWAYS") != nullptr;   // experiment: one kernel variant for every LSU-epilogue layer
     const bool ks = plan->p.sk_T > 0 || (ks_always && epi == 0);
     const bool st = plan->p.stats != nullptr && !ks;   // role counters: a separate instantiation (YB_TC_STATS=1)
     const TcPlan &P = *plan;
 #define YB_TC_LAUNCH(KS_, ST_, EPI_) cudaLaunchKernelEx(&cfg, k_conv_tc<KS_, ST_, EPI_>, P.tmA, P.tmB, P.tmO, P.tmR, P.p)
     if (ks) YB_TC_LAUNCH(true, false, 0);
-    else if (epi == 1) { if (st) YB_TC_LAUNCH(false, true, 1); else YB_TC_LAUNCH(false, false, 1); }
+    else if (epi == 1) {
+        if (st) cudaLaunchKernelEx(&cfg, k_conv_tc_reg<true>, P.tmA, P.tmB, P.tmO, P.tmR, P.p);
+        else cudaLaunchKernelEx(&cfg, k_conv_tc_reg<false>, P.tmA, P.tmB, P.tmO, P.tmR, P.p);
+    }
     else if (epi == 2) { if (st) YB_TC_LAUNCH(false, true, 2); else YB_TC_LAUNCH(false, false, 2); }
     else { if (st) YB_TC_LAUNCH(false, true, 0); else YB_TC_LAUNCH(false, false, 0); }
 #undef YB_TC_LAUNCH
