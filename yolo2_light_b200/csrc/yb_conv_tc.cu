@@ -178,7 +178,6 @@ __device__ __forceinline__ void tma_store_3d(const CUtensorMap *tm, uint32_t src
 }
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
@@ -1124,36 +1123,114 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
     }
 }
 
-// Register-accumulator kernel of the bf16-output, stride-1 layers (384 threads).  Warpgroup 2 is the TMA producer (one elected
-// thread; the warpgroup gives its registers away with setmaxnreg), warpgroups 0 and 1 are consumers with up to 216 registers
-// each: a consumer warpgroup keeps the f32 accumulators of its 64 rows x BN (<= 256) filters of the tile in registers and runs
-// the epilogue straight on its wgmma fragment -- bias, leaky, the fused shortcut residual and the second leaky in fp32, then
-// round to bf16 -- writing SW-column slabs (SW = 64, or 32 when BN == 32) into a swizzled shared-memory tile that one thread
-// stores with cp.async.bulk.tensor.  The residual slab comes in the same way, one slab ahead (across work items), with the L2
-// evict-first hint.  No shared-memory accumulator tile and no barrier between the two consumer warpgroups: the shared memory
-// goes to the ring, and each warpgroup stores its half tile (64 pixels) on its own.
+// Register-accumulator kernel of the bf16-output, stride-1 layers (384 threads).  Warpgroups 0 and 1 are consumers with up to 216
+// registers each: a consumer warpgroup keeps the f32 accumulators of its 64 rows x BN (<= 256) filters of the tile in registers
+// and runs the epilogue straight on its wgmma fragment -- bias, leaky, the fused shortcut residual and the second leaky in fp32,
+// then round to bf16.  Warpgroup 2 gives its registers away with setmaxnreg: warp 8 is the TMA producer, warps 9 and 10 are the
+// store warps of consumer warpgroups 0 and 1 (one elected thread each).
+//
+// Each consumer warpgroup has one staging buffer: its half tile, 64 pixel rows x BN bf16, laid out as BN / SW slabs of SW columns
+// (SW = 64, or 32 when BN == 32) with the tensor maps' swizzle.  The epilogue reads each residual word from it and writes the
+// output word to the same address (the same thread owns both).  The store thread stores each slab with cp.async.bulk.tensor as
+// soon as the consumers have written it, and once that store has read the slab it loads the next work item's residual slab into
+// it (L2 evict-first).  So the epilogue's memory traffic runs while the consumers finish the epilogue, when the operand ring is
+// full and the TMA engine would otherwise idle (issued under the next main loop instead, it held up the operand loads), and the
+// residual has a whole main loop to land.  The mbarriers per consumer warpgroup g:
+//   stg_full[g][s] -- 4 arrivals, one per consumer warp after fence.proxy.async: slab s is written;
+//   stg_ready[g]   -- the store thread's arrival (expect_tx = the residual bytes): the buffer is free and holds the residual.
+// A consumer goes from its epilogue straight into the next main loop: no named barrier and no TMA call in the consumers, and the
+// two warpgroups never wait for each other.
 constexpr int TCR_THREADS = 384;
 constexpr int TCR_PRODUCER_REGS = 40, TCR_CONSUMER_REGS = 216;   // 128 * 40 + 256 * 216 <= 64 K registers
+constexpr int TCR_STORE_WARP = 9;                                // store warps 9 (consumer warpgroup 0) and 10 (warpgroup 1)
+constexpr int TCR_MAX_SLABS = 4;                                 // BN / SW <= 256 / 64
+
+// Store thread of consumer warpgroup g: walks the consumers' work items (see k_conv_tc_reg).  buf: the warpgroup's staging buffer,
+// stg_full: its first per-slab barrier.  ST: cycles spent waiting on stg_full and in cp.async.bulk.wait_group.read go to stats
+// slots 4 and 5 (warpgroup 0's thread).
+template <bool ST>
+__device__ __forceinline__ void tcr_store(const CUtensorMap *tmO, const CUtensorMap *tmR, const TcParams &p, uint32_t buf,
+                                          uint32_t stg_full, uint32_t stg_ready, int g, int w_first, int w_step) {
+    const int SW = p.tma_epi, BN = p.BN;
+    const uint32_t tile = 64u * 2u * (uint32_t)SW;                  // one slab: 64 pixel rows x SW bf16
+    // the half tile as a TMA box: 64 of the TW x TH pixels (TW == 128: one half row; else TH / 2 whole rows)
+    const int hx = (p.TW == 128) ? 64 * g : 0, hy = (p.TW == 128) ? 0 : g * (p.TH >> 1);
+    long long w_full = 0, w_read = 0;
+    // box origin of work item w's half tile (first filter, padded x, merged padded row); returns its slabs holding filters < n
+    auto item = [&](int w, int &n0, int &x, int &y) {
+        const int m = w / p.nt;
+        n0 = (w % p.nt) * BN; x = (m % p.xt) * p.TW + 1 + hx; y = (m / p.xt) * p.TH + p.jshift + hy;
+        return (min(BN, p.n - n0) + SW - 1) / SW;
+    };
+    auto wait_read = [&]() {   // the bulk stores issued so far have read shared memory
+        if constexpr (ST) { const long long c0 = clock64(); tma_store_wait_read0(); w_read += clock64() - c0; }
+        else tma_store_wait_read0();
+    };
+    auto load_res = [&](int s, int n0, int x, int y) {
+        if (p.l2_hint) tma_load_3d_hint(buf + (uint32_t)s * tile, tmR, stg_ready, n0 + s * SW, x, y, l2_policy_evict_first());
+        else tma_load_3d(buf + (uint32_t)s * tile, tmR, stg_ready, n0 + s * SW, x, y);
+    };
+    if (w_first < p.num_work) {   // the first item's residual overlaps the first main loop
+        if (p.res) {
+            int n0, x, y;
+            const int ns = item(w_first, n0, x, y);
+            mbar_arrive_expect_tx(stg_ready, (uint32_t)ns * tile);
+            for (int s = 0; s < ns; ++s) load_res(s, n0, x, y);
+        } else mbar_arrive(stg_ready);
+    }
+    // Per item: store each slab as soon as the consumers have written it, and once that store has read the slab, load the
+    // next item's residual slab into it -- all of it while the consumers are still in the epilogue, when the operand ring is
+    // full and the TMA engine would otherwise idle.
+    uint32_t phases = 0;   // bit s: phase parity of slab s's stg_full (masked filter tiles skip the slabs >= their ns)
+    for (int w = w_first; w < p.num_work; w += w_step) {
+        int n0, x, y, n0n = 0, xn = 0, yn = 0;
+        const int ns = item(w, n0, x, y);
+        const bool next = w + w_step < p.num_work, res_next = next && p.res;
+        const int nsn = next ? item(w + w_step, n0n, xn, yn) : 0;
+        for (int s = 0; s < ns; ++s) {
+            const uint32_t fb = stg_full + 8u * (uint32_t)s;
+            if constexpr (ST) { const long long c0 = clock64(); mbar_wait(fb, (phases >> s) & 1u); w_full += clock64() - c0; }
+            else mbar_wait(fb, (phases >> s) & 1u);
+            phases ^= 1u << s;
+            // the consumers are past this item's stg_ready: its phase is complete and the next item's may begin
+            if (s == 0 && res_next) mbar_arrive_expect_tx(stg_ready, (uint32_t)nsn * tile);
+            tma_store_3d(tmO, buf + (uint32_t)s * tile, n0 + s * SW, x, y);
+            tma_store_commit();
+            if (res_next && s < nsn) { wait_read(); load_res(s, n0n, xn, yn); }
+        }
+        if (res_next) {
+            for (int s = ns; s < nsn; ++s) { wait_read(); load_res(s, n0n, xn, yn); }
+        } else if (next) {
+            wait_read();
+            mbar_arrive(stg_ready);
+        }
+    }
+    tma_store_wait_all();   // bulk groups are per thread: these are this warpgroup's stores only
+    if (ST && p.stats && g == 0) { p.stats[blockIdx.x * 16 + 4] = (unsigned long long)w_full; p.stats[blockIdx.x * 16 + 5] = (unsigned long long)w_read; }
+}
 
 template <bool ST>
 __global__ void __launch_bounds__(TCR_THREADS, 1)
 k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
               const __grid_constant__ CUtensorMap tmR, const TcParams p) {
     extern __shared__ uint8_t smem_raw[];
-    const uint32_t smemB = (smem_u32(smem_raw) + 1023u) & ~1023u;   // [resident filter matrix][pipeline ring][barriers][bias][epilogue tiles]
+    const uint32_t smemB = (smem_u32(smem_raw) + 1023u) & ~1023u;   // [resident filter matrix][pipeline ring][barriers][bias][staging]
     const uint32_t smem0 = smemB + p.bstat_bytes;
     const uint32_t bars = smem0 + (uint32_t)p.stages * p.stage_bytes;
     const uint32_t bstat_bar = bars + 8u * (uint32_t)(2 * p.stages);
-    auto resfull_bar = [&](int g) { return bstat_bar + 8u + 8u * (uint32_t)g; };   // residual slab of warpgroup g landed
-    const uint32_t misc = (bstat_bar + 24u + 15u) & ~15u;
+    // per consumer warpgroup g: stg_full for each of up to TCR_MAX_SLABS slabs, then stg_ready
+    auto stg_full = [&](int g, int s) { return bstat_bar + 8u + 8u * (uint32_t)(g * TCR_MAX_SLABS + s); };
+    auto stg_ready = [&](int g) { return bstat_bar + 8u + 8u * (uint32_t)(2 * TCR_MAX_SLABS + g); };
+    const uint32_t misc = (bstat_bar + 8u * (uint32_t)(2 * TCR_MAX_SLABS + 3) + 15u) & ~15u;
     float *bias_s = reinterpret_cast<float *>(smem_raw + (misc - smem_u32(smem_raw)));
-    // per consumer warpgroup: [OUT 0][OUT 1][RES], each 64 pixel rows x SW bf16 with the tensor maps' swizzle (1024-byte aligned)
-    const uint32_t epi_base = (misc + 4u * (uint32_t)(p.nt * p.BN) + (uint32_t)(p.nt * p.BN / 8) + 1023u) & ~1023u;
+    // staging buffers of warpgroups 0 and 1, 64 * BN bf16 each (1024-byte aligned for the swizzle)
+    const uint32_t stg_base = (misc + 4u * (uint32_t)(p.nt * p.BN) + (uint32_t)(p.nt * p.BN / 8) + 1023u) & ~1023u;
 
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
     const int lane = threadIdx.x & 31;
     const int wg = warp >> 2;
     const int w_first = (int)blockIdx.x, w_step = (int)gridDim.x;
+    const bool epi_mem = !(p.dbg & 4);
 
     if (warp == 8 && elect_one()) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
@@ -1162,7 +1239,10 @@ k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
         if (p.res) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmR) : "memory");
         for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar(bars, s), 1); mbar_init(empty_bar(bars, p.stages, s), TC_EPI_WARPS); }
         mbar_init(bstat_bar, 1);
-        mbar_init(resfull_bar(0), 1); mbar_init(resfull_bar(1), 1);
+        for (int g = 0; g < 2; ++g) {
+            for (int s = 0; s < TCR_MAX_SLABS; ++s) mbar_init(stg_full(g, s), 4);
+            mbar_init(stg_ready(g), 1);
+        }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     for (int i = threadIdx.x; i < p.nt * p.BN; i += TCR_THREADS) bias_s[i] = (i < p.n) ? __ldg(p.bias + i) : 0.f;
@@ -1173,7 +1253,12 @@ k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
 
     if (wg == 2) {
         asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(TCR_PRODUCER_REGS));
-        if (warp == 8 && elect_one()) tc_produce<false, ST>(&tmA, &tmB, p, smemB, smem0, bars, w_first, w_step);
+        if (warp == 8) {
+            if (elect_one()) tc_produce<false, ST>(&tmA, &tmB, p, smemB, smem0, bars, w_first, w_step);
+        } else if (warp < TCR_STORE_WARP + 2 && epi_mem) {
+            const int g = warp - TCR_STORE_WARP;
+            if (elect_one()) tcr_store<ST>(&tmO, &tmR, p, stg_base + (uint32_t)g * 128u * (uint32_t)p.BN, stg_full(g, 0), stg_ready(g), g, w_first, w_step);
+        }
         return;
     }
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(TCR_CONSUMER_REGS));
@@ -1181,16 +1266,13 @@ k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     // ======================= consumers: warpgroup wg owns rows 64 wg .. + 63 of every tile =======================
     // wgmma fragment: this thread holds rows rl and rl + 8 (of the warpgroup's 64), columns 8 j + cq, 8 j + cq + 1
     const int rl = 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);
-    const bool boss = (warp & 3) == 0 && lane == 0;    // issues this warpgroup's epilogue TMA traffic
     const bool leaky = p.act == ACT_LEAKY, leaky2 = p.act2 == ACT_LEAKY;
-    const bool epi_mem = !(p.dbg & 4);
-    const bool has_res = p.res != nullptr && epi_mem;
-    // the half tile as a TMA box: 64 of the TW x TH pixels (TW == 128: one half row; else TH / 2 whole rows)
-    const int hx = (p.TW == 128) ? 64 * wg : 0, hy = (p.TW == 128) ? 0 : wg * (p.TH >> 1);
+    const bool has_res = p.res != nullptr;
     int stage = 0; uint32_t phase = 0;
-    uint32_t res_phase = 0;
-    int out_buf = 0;
-    long long w_full = 0, w_res = 0; const long long t_begin = ST ? clock64() : 0;
+    uint32_t stg_phase = 0;
+    // w_ready: waits on stg_ready after the first work item (the first item's, whose residual fetch overlaps only one main loop,
+    // goes to stats slot 3 right away)
+    long long w_full = 0, w_ready = 0; const long long t_begin = ST ? clock64() : 0;
     if (p.bstat) mbar_wait(bstat_bar, 0);
 
     auto run = [&](auto bn_c, auto kk_c) {
@@ -1198,20 +1280,12 @@ k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
         constexpr int KK = decltype(kk_c)::value;
         constexpr int SW = BN >= 64 ? 64 : 32;             // slab width (columns); rows of 128 B (128B swizzle) or 64 B (64B swizzle)
         constexpr uint32_t ROWB = SW * 2, TILE = 64u * ROWB;
-        const uint32_t grp = epi_base + (uint32_t)wg * 3u * TILE, res_tile = grp + 2u * TILE;
-        // byte offset of (row, 16-byte chunk c) in a slab tile + this thread's column pair: conflict-free for the fragment layout
+        const uint32_t buf = stg_base + (uint32_t)wg * (uint32_t)(BN / SW) * TILE;
+        // byte offset of (row, 16-byte chunk c) in a slab + this thread's column pair: conflict-free for the fragment layout
         auto slab_off = [&](int row, int c) -> uint32_t {
             const int sw = (SW == 64) ? (row & 7) : ((row >> 1) & 3);
             return (uint32_t)row * ROWB + ((uint32_t)(c ^ sw) << 4) + 2u * (uint32_t)cq;
         };
-        auto request_res = [&](int w_, int f_) {
-            const int m_ = w_ / p.nt;
-            const int c0 = (w_ % p.nt) * BN + f_, x = (m_ % p.xt) * p.TW + 1 + hx, y = (m_ / p.xt) * p.TH + p.jshift + hy;
-            mbar_arrive_expect_tx(resfull_bar(wg), TILE);
-            if (p.l2_hint) tma_load_3d_hint(res_tile, &tmR, resfull_bar(wg), c0, x, y, l2_policy_evict_first());
-            else tma_load_3d(res_tile, &tmR, resfull_bar(wg), c0, x, y);
-        };
-        if (has_res && boss && w_first < p.num_work) request_res(w_first, 0);
         for (int w = w_first; w < p.num_work; w += w_step) {
             float d[BN / 2];
             tc_mma_loop<0, BN, KK, ST>(d, p, smemB, smem0, bars, wg, lane, stage, phase, w_full, 0, p.kbs);
@@ -1227,9 +1301,20 @@ k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
                 valid[h] = img < p.N && oy >= 0 && oy < p.OH && ox < p.OW;
             }
             const int nslab = (min(BN, p.n - n0) + SW - 1) / SW;   // slabs holding filters < n
+            // the buffer is back from the store thread: the previous item's bulk stores have read it, this item's residual is in it
+            if constexpr (ST) {
+                const long long c0 = clock64();
+                mbar_wait(stg_ready(wg), stg_phase);
+                const long long dt = clock64() - c0;
+                if (w != w_first) w_ready += dt;
+                else if (p.stats && warp == 0 && lane == 0) p.stats[blockIdx.x * 16 + 3] = (unsigned long long)dt;
+            }
+            else mbar_wait(stg_ready(wg), stg_phase);
+            stg_phase ^= 1u;
 #pragma unroll
             for (int s = 0; s < BN / SW; ++s) {
                 if (s >= nslab) break;
+                const uint32_t slab = buf + (uint32_t)s * TILE;
 #pragma unroll
                 for (int jj = 0; jj < SW / 8; ++jj) {
                     const int j = s * (SW / 8) + jj;
@@ -1240,31 +1325,26 @@ k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
                         d[4 * j + e] = leaky ? fmaxf(a, 0.1f * a) : a;   // == a > 0 ? a : 0.1a
                     }
                 }
+                // (no "memory" clobbers on the slab accesses: only this thread touches these words between the barriers, and the
+                // bias loads may then be scheduled freely around them)
                 if (has_res) {
-                    if constexpr (ST) { const long long c0 = clock64(); mbar_wait(resfull_bar(wg), res_phase); w_res += clock64() - c0; }
-                    else mbar_wait(resfull_bar(wg), res_phase);
-                    res_phase ^= 1u;
+                    uint32_t u[SW / 8][2];
+#pragma unroll
+                    for (int jj = 0; jj < SW / 8; ++jj)
+#pragma unroll
+                        for (int h = 0; h < 2; ++h)
+                            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(u[jj][h]) : "r"(slab + slab_off(rl + 8 * h, jj)));
 #pragma unroll
                     for (int jj = 0; jj < SW / 8; ++jj) {
                         const int j = s * (SW / 8) + jj;
 #pragma unroll
                         for (int h = 0; h < 2; ++h) {
-                            uint32_t u;
-                            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(u) : "r"(res_tile + slab_off(rl + 8 * h, jj)) : "memory");
-                            float a = d[4 * j + 2 * h] + __uint_as_float(u << 16);
-                            float c = d[4 * j + 2 * h + 1] + __uint_as_float(u & 0xffff0000u);
+                            float a = d[4 * j + 2 * h] + __uint_as_float(u[jj][h] << 16);
+                            float c = d[4 * j + 2 * h + 1] + __uint_as_float(u[jj][h] & 0xffff0000u);
                             if (leaky2) { a = fmaxf(a, 0.1f * a); c = fmaxf(c, 0.1f * c); }
                             d[4 * j + 2 * h] = a; d[4 * j + 2 * h + 1] = c;
                         }
                     }
-                }
-                // the bulk store that last read this OUT tile (two slabs ago) must be done reading it
-                const uint32_t out_tile = grp + (uint32_t)out_buf * TILE;
-                if (boss) tma_store_wait_read1();
-                named_bar_sync(1 + wg, 128);
-                if (has_res && boss) {                         // everybody is done with the RES tile: request the next slab
-                    if (s + 1 < nslab) request_res(w, (s + 1) * SW);
-                    else if (w + w_step < p.num_work) request_res(w + w_step, 0);
                 }
 #pragma unroll
                 for (int jj = 0; jj < SW / 8; ++jj) {
@@ -1272,16 +1352,12 @@ k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
                         const uint32_t o = valid[h] ? pack_bf16x2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]) : 0u;
-                        asm volatile("st.shared.b32 [%0], %1;" ::"r"(out_tile + slab_off(rl + 8 * h, jj)), "r"(o) : "memory");
+                        asm volatile("st.shared.b32 [%0], %1;" ::"r"(slab + slab_off(rl + 8 * h, jj)), "r"(o));
                     }
                 }
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the TMA engine
-                named_bar_sync(1 + wg, 128);
-                if (boss) {
-                    tma_store_3d(&tmO, out_tile, n0 + s * SW, x0 + 1 + hx, J0 + hy);
-                    tma_store_commit();
-                }
-                out_buf ^= 1;
+                __syncwarp();
+                if (lane == 0) mbar_arrive(stg_full(wg, s));
             }
         }
     };
@@ -1294,9 +1370,8 @@ k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     else if (p.BN == 128) by_kk(std::integral_constant<int, 128>{});
     else if (p.BN == 64) by_kk(std::integral_constant<int, 64>{});
     else by_kk(std::integral_constant<int, 32>{});
-    if (boss) tma_store_wait_all();   // this warpgroup's bulk stores have completed (shared memory stays valid until then)
     if (ST && p.stats && warp == 0 && lane == 0) { p.stats[blockIdx.x * 16 + 2] = (unsigned long long)w_full; p.stats[blockIdx.x * 16 + 6] = (unsigned long long)(clock64() - t_begin);
-                                                    p.stats[blockIdx.x * 16 + 8] = (unsigned long long)w_res; }
+                                                    p.stats[blockIdx.x * 16 + 8] = (unsigned long long)w_ready; }
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -1534,6 +1609,13 @@ int pick_bn_reg(int n, long m_tiles, int kblocks, int sms) {
     return best;
 }
 
+// Persistent grid size of the tensor-core plans: one CTA per SM, or fewer under YB_TC_GRID=n (tests: several work items per CTA
+// reuse the epilogue buffers and flip the barrier phases many times on small layers).
+int grid_cap(int sms) {
+    const char *e = getenv("YB_TC_GRID");
+    return (e && atoi(e) > 0) ? std::min(sms, atoi(e)) : sms;
+}
+
 }  // namespace
 
 int tc_conv_supported(const Layer &l, const TV &in, const TV &out, bool out_bf16) {
@@ -1617,13 +1699,13 @@ static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &
     p.bstat = (p.nt == 1 && (size_t)p.kblocks * p.b_bytes <= 48 * 1024 && !getenv("YB_TC_NO_BSTAT")) ? 1 : 0;
     p.bstat_bytes = p.bstat ? (uint32_t)p.kblocks * p.b_bytes : 0u;
     // TMA epilogue: slab width in columns.  k_conv_tc_reg: bf16 slabs of 64 columns (32 when BN == 32), per consumer warpgroup
-    // [OUT 0][OUT 1][RES] tiles of 64 pixels; integer kinds: f32 slabs of 32 columns (128-byte rows), one 128-pixel tile per warp
-    // group -- the raw-accumulator dump (tests) keeps the LSU path
+    // one staging buffer of 64 pixels x BN (64 / 32 / 16 / 8 KB per CTA at BN = 256 / 128 / 64 / 32); integer kinds: f32 slabs of
+    // 32 columns (128-byte rows), one 128-pixel tile per warp group -- the raw-accumulator dump (tests) keeps the LSU path
     p.tma_epi = 0;
     const bool i8kind = kind == 1 || kind == 2;
     if (reg) p.tma_epi = BN >= 64 ? 64 : 32;
     if (i8kind && !s2 && !acc_out && !getenv("YB_TC_NO_TMA_EPI") && !getenv("YB_TC_NO_COALESCE")) p.tma_epi = 32;
-    p.stg_bytes = reg ? 2u * 3u * 64u * (uint32_t)p.tma_epi * 2u : p.tma_epi ? 2u * 16384u : 4096u * TC_EPI_WARPS;
+    p.stg_bytes = reg ? 2u * 64u * (uint32_t)BN * 2u : p.tma_epi ? 2u * 16384u : 4096u * TC_EPI_WARPS;
     p.acc_pitch = BN + 4;
     const size_t acc_bytes = reg ? 0 : (size_t)TC_BM * p.acc_pitch * 4;   // k_conv_tc_reg keeps the accumulators in registers
     // what is left of 227 KB beside the epilogue tiles and the accumulator tile (5 KB: barriers, alignment slack)
@@ -1719,13 +1801,14 @@ static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &
         if (res.base && out_bf16) encode_px(&plan->tmR, res, "residual");
     }
     plan->pdl = (getenv("YB_NO_PDL") == nullptr) ? 1 : 0;
-    plan->grid = std::min(p.num_tiles, sms);
+    plan->grid = std::min(p.num_tiles, grid_cap(sms));
     plan->threads = reg ? TCR_THREADS : TC_THREADS;
     if (getenv("YB_TC_STATS")) {
         cudaMalloc(&p.stats, sizeof(unsigned long long) * 16 * plan->grid);
         cudaMemset(p.stats, 0, sizeof(unsigned long long) * 16 * plan->grid);
     }
-    plan->smem = 1024 /*alignment slack*/ + p.bstat_bytes + (size_t)p.stages * p.stage_bytes + 8 * (2 * p.stages + 3) + 16 +
+    // barriers: full / empty per stage, the resident-filter barrier, k_conv_tc_reg's stg_full / stg_ready per consumer warpgroup
+    plan->smem = 1024 /*alignment slack*/ + p.bstat_bytes + (size_t)p.stages * p.stage_bytes + 8 * (2 * p.stages + 11) + 16 +
                  sizeof(float) * (size_t)p.nt * BN /*bias*/ + (size_t)p.nt * BN / 8 /*yolo mask*/ +
                  (p.tma_epi ? 1024 : 128) + p.stg_bytes /*epilogue staging or TMA-epilogue tiles*/ +
                  acc_bytes /*accumulator tile*/;
@@ -1830,7 +1913,7 @@ int tc_plan_enable_ksplit(void *vp, float *ws, unsigned *flags) {
     int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const int G = sms;
+    const int G = grid_cap(sms);
     const int R = p.num_work / G, T = p.num_work % G;
     if (T == 0) return 0;
     // Only deep-K layers: with few stages per work item the epilogue, not the tensor pipe, bounds the tile, and the
@@ -1927,10 +2010,13 @@ void tc_free_plan(void *vp) {
         cudaMemcpy(h.data(), plan->p.stats, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
         double m[16] = {0};
         for (int b = 0; b < plan->grid; ++b) for (int k = 0; k < 16; ++k) m[k] += (double)h[16 * b + k] / plan->grid;
-        fprintf(stderr, "TCSTATS %-28s tiles/cta %.1f kb %d sps %d BN %d ksplit T%d L%d/%d | producer: wait_empty %.0f tma_issue %.0f total %.0f | "
-                        "consumers: wait_full %.0f wait_res %.0f total %.0f\n", plan->desc,
-                (double)plan->p.num_tiles / plan->grid * 1.0, plan->p.kblocks, plan->p.sps, plan->p.BN, plan->p.sk_T, plan->p.sk_L, plan->p.kbs,
-                m[0], m[7], m[1], m[2], m[8], m[6]);
+        fprintf(stderr, "TCSTATS %-28s tiles/cta %.1f kb %d sps %d BN %d ksplit T%d L%d/%d | producer: wait_empty %.0f tma_issue %.0f total %.0f | ",
+                plan->desc, (double)plan->p.num_tiles / plan->grid * 1.0, plan->p.kblocks, plan->p.sps, plan->p.BN, plan->p.sk_T, plan->p.sk_L,
+                plan->p.kbs, m[0], m[7], m[1]);
+        if (plan->threads == TCR_THREADS)   // k_conv_tc_reg: the consumers' wait on stg_ready (first work item apart) and the store warps
+            fprintf(stderr, "consumers: wait_full %.0f wait_ready %.0f (first item %.0f) total %.0f | store: wait_full %.0f wait_read %.0f\n",
+                    m[2], m[8], m[3], m[6], m[4], m[5]);
+        else fprintf(stderr, "consumers: wait_full %.0f wait_res %.0f total %.0f\n", m[2], m[8], m[6]);
         cudaFree(plan->p.stats);
     }
     delete plan;
