@@ -212,12 +212,10 @@ int yb_network_weight_arena(yb_network *net, int quantized, int upload, void **d
 int  yb_network_last_launches(const yb_network *net);
 
 /* Diagnostic switches (tests): "fuse" (1: conv+shortcut fusion and route aliasing, default), "keep_counts"
- * (1: keep the raw XNOR popcounts / INT8 s32 accumulators of every integer conv), "q_index_offset", "ksplit"
- * (1: split the tail wave of the deep-K tensor-core convolutions along K: ~1 % faster on yolov3-608 b16, but the f32
- * summation order then depends on the batch size; default 0 keeps image k of any batch bit-identical to a batch of 1). */
+ * (1: keep the raw XNOR popcounts / INT8 s32 accumulators of every integer conv), "q_index_offset".  Returns -1 for an
+ * unknown name. */
 int  yb_network_set_option(yb_network *net, const char *name, int value);
-/* Engine facts (builds the engine if needed): "launches", "tc_layers" (convolutions on the tensor cores), "ksplit_layers"
- * (of those, how many run with a K-split tail wave).  -1: unknown key. */
+/* Engine facts (builds the engine if needed): "launches", "tc_layers" (convolutions on the tensor cores).  -1: unknown key. */
 long yb_network_get_info(yb_network *net, int quantized, const char *key);
 /* Raw integer results of conv layer i (NCHW, batch-major) when "keep_counts" is on; returns the element count. */
 int  yb_network_fetch_counts(yb_network *net, int i, int quantized, int32_t *dst, size_t count);

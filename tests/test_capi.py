@@ -55,6 +55,17 @@ def test_predict_without_gpu_fails_loudly(workdir):
         net.predict(util.images("tiny64", 1))
 
 
+def test_set_option_rejects_unknown_names(workdir):
+    """An unknown option name, such as the removed "ksplit", fails loudly; the known options still work."""
+    import yolo2_light_b200 as yb
+    cfg, wts = util.model_files("tiny64", workdir)
+    net = yb.load_network(cfg, wts, batch=1)
+    with pytest.raises(yb.YbError, match="unknown option ksplit"):
+        net.set_option("ksplit", 1)
+    for name, value in (("fuse", 0), ("keep_counts", 1), ("q_index_offset", 0), ("fuse", 1)):
+        net.set_option(name, value)
+
+
 def test_from_layers_roundtrip(workdir):
     """The drop-in path: descriptors exported from one network rebuild an identical one (yb_network_from_layers)."""
     import yolo2_light_b200 as yb

@@ -43,7 +43,6 @@ static Engine *get_engine(yb_network *n, int quantized, bool upload = true) {
         const char *nf = getenv("YB_NO_FUSE");
         opt.fuse = !(nf && nf[0] == '1') && net.fuse;
         opt.keep_counts = net.keep_counts;
-        opt.ksplit = net.ksplit;
         opt.q_index_offset = net.q_index_offset;
         net.engine[slot] = build_engine(&net, opt);
     }
@@ -223,7 +222,6 @@ int yb_network_set_option(yb_network *n, const char *name, int value) {
     if (!strcmp(name, "fuse")) net.fuse = value != 0;
     else if (!strcmp(name, "keep_counts")) net.keep_counts = value != 0;
     else if (!strcmp(name, "q_index_offset")) net.q_index_offset = value;
-    else if (!strcmp(name, "ksplit")) net.ksplit = value != 0;
     else { report(std::string("unknown option ") + name); return -1; }
     drop_engines(&net);
     return 0;
@@ -405,7 +403,7 @@ static std::vector<Engine *> get_replicas(yb_network *n, int quantized, int ngpu
         opt.precision = n->net.precision; opt.qrule = quantized != 0; opt.upload = false;   // weights arrive by the broadcast
         const char *nf = getenv("YB_NO_FUSE");
         opt.fuse = !(nf && nf[0] == '1') && n->net.fuse;
-        opt.keep_counts = n->net.keep_counts; opt.ksplit = n->net.ksplit; opt.q_index_offset = n->net.q_index_offset;
+        opt.keep_counts = n->net.keep_counts; opt.q_index_offset = n->net.q_index_offset;
         reps.push_back(build_engine(&n->net, opt));
         built = true;
     }

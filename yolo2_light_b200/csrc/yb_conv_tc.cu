@@ -18,11 +18,11 @@
 //     [128][BN+4] shared-memory tile, and the same 8
 //     warps run the epilogue from it with one pixel row per thread: add bias (folded batch-norm), apply leaky-ReLU,
 //     add the shortcut residual when fused (reference :443-449), and store bf16 NHWC through a swizzled staging tile
-//     (whole 128-byte lines) or TMA, or f32 for detection heads -- optionally with the following [yolo] layer applied
-//     (:453-472).  The producer warp keeps loading the next tile's stages meanwhile.
+//     (whole 128-byte lines; the stride-2 layers), or f32 for detection heads -- optionally with the following [yolo]
+//     layer applied (:453-472).  The producer warp keeps loading the next tile's stages meanwhile.
 //   * The same kernel runs the INT8 variant (s8 x s8 -> s32 wgmma, exact requantising epilogue,
 //     yolov2_forward_network_quantized.c:474-490), wide XNOR layers as +-1 bytes on the s8 wgmma, and the float heads
-//     of the exact networks on tf32 wgmma.  KS = true: K-split of the tail wave (opt-in).
+//     of the exact networks on tf32 wgmma.
 //
 // Warp roles of k_conv_tc (288 threads): warps 0-7 = two consumer warpgroups (wgmma + epilogue), warp 8 = TMA producer.
 #include <cuda.h>
@@ -53,8 +53,7 @@ struct TcParams {
     int N;                    // images
     int TW, TWlog2, TH;       // tile = TW x TH output pixels (TW*TH == 128)
     int xt, jt, nt;           // #tiles along x, merged rows, filters
-    int num_tiles;
-    int num_work;             // work items of the persistent loop (== num_tiles)
+    int num_work;             // tiles = work items of the persistent loop (xt * jt * nt)
     int kind;                 // 0: bf16 x bf16 -> f32;  1: s8 x s8 -> s32, exact requantising epilogue;
                               // 2: XNOR layer as +-1 s8 on the s8 wgmma (dot = 2*count - K exactly), reference float epilogue;
                               // 3: f32 operands read as tf32 (K = 8 per MMA) -> f32: float heads of the exact nets
@@ -78,7 +77,8 @@ struct TcParams {
     uint32_t bstat_bytes;
     // TMA epilogue: slab width in columns (0: off).  Each epilogue group writes its slab into a swizzled shared-memory tile and
     // one thread stores it with cp.async.bulk.tensor; the shortcut residual comes in the same way (TMA load + mbarrier).
-    // Non-zero for every k_conv_tc_reg plan (bf16 slabs) and for the integer kinds (f32 slabs of k_conv_tc).
+    // Non-zero for every k_conv_tc_reg plan (bf16 slabs) and for the stride-1 integer kinds without the raw-accumulator dump
+    // (f32 slabs of k_conv_tc); the other k_conv_tc plans store through the per-warp LSU staging tiles.
     int tma_epi;
     int l2_hint;              // 1: shortcut tiles are loaded with the L2 evict-first policy
     uint32_t stg_bytes;       // epilogue staging / TMA-epilogue tiles
@@ -93,18 +93,11 @@ struct TcParams {
     signed char *pool_out; long pool_ldc; int pool_Hp, pool_Wp;   // next layer's s8 input: padded NHWC, bytes
     int sps;                                  // K-blocks per pipeline stage (amortises the per-stage barrier round trip)
     int kbs;                                  // pipeline stages per work item = ceil(kblocks / sps)
-    // K-split tail (wave quantisation): the last num_work % G work items ("tail") are cut along K into slices of sk_L
-    // stages, one slice per CTA (pair); a slice that does not end its work item dumps the raw f32 accumulator to
-    // sk_ws, the slice that does (the owner) adds those partials in its epilogue.  sk_T == 0: off.
-    int sk_T, sk_L;
-    float *sk_ws;                             // [grid][BN/4][128] float4
-    unsigned *sk_flags;                       // [grid][8 epilogue warps]: 1 = partial published (reset by its reader)
     uint32_t desc_hi;         // high word of the wgmma shared-memory descriptors (SBO, swizzle mode)
     char *out; long out_ldc; int out_bf16; int n, n_store;
-    const char *res; long res_ldc; int res_bf16;
+    const char *res; long res_ldc; int res_bf16;   // fused shortcut operand (bf16, bf16 outputs only), or null
     const float *bias; int act, act2;
     unsigned long long *stats; // YB_TC_STATS=1: per-CTA cycle counters [grid][16] (diagnostic)
-    int no_coalesce;          // YB_TC_NO_COALESCE=1: per-thread row stores (the pre-staging epilogue), for A/B comparison
     int dbg;                  // YB_TC_DBG bit mask for bottleneck experiments: 1 no TMA, 2 no MMA, 4 no epilogue memory ops
 };
 
@@ -321,12 +314,6 @@ __device__ __forceinline__ void acc_ld32(uint32_t addr, uint32_t (&v)[32]) {
         asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v[4 * c]), "=r"(v[4 * c + 1]), "=r"(v[4 * c + 2]), "=r"(v[4 * c + 3])
                      : "r"(addr + 16u * (uint32_t)c) : "memory");
 }
-__device__ __forceinline__ void acc_st32(uint32_t addr, const uint32_t (&v)[32]) {
-#pragma unroll
-    for (int c = 0; c < 8; ++c)
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr + 16u * (uint32_t)c), "r"(v[4 * c]), "r"(v[4 * c + 1]),
-                     "r"(v[4 * c + 2]), "r"(v[4 * c + 3]) : "memory");
-}
 // wgmma accumulator fragment of one warpgroup (rows row0 .. row0 + 63) -> accumulator tile.  Thread (warp w, lane l) holds rows
 // row0 + 16 w + l / 4 (+ 8) and columns 8 j + 2 (l % 4) (+ 1).
 template <typename T, int NR>
@@ -343,60 +330,13 @@ __device__ __forceinline__ void acc_store_frag(uint32_t acc, int pitch, int row0
     }
 }
 
-// Work schedule of one CTA, identical in every warp role: first this unit's slice of the
-// K-split tail (units of pipeline stages over the first sk_T work items), then whole work items round-robin.
-struct TcSched { int u, u_end, w_dp, w_step, num_work, kbs, lead0, lead1; };
-template <bool KS>
-__device__ __forceinline__ TcSched sched_init(const TcParams &p, int unit, int nunits) {
-    TcSched s;
-    s.kbs = p.kbs; s.num_work = p.num_work; s.w_step = nunits;
-    if constexpr (!KS) { s.u = s.u_end = s.lead0 = s.lead1 = 0; s.w_dp = unit; return s; }
-    const int U = p.sk_T * p.kbs;
-    s.u = min(unit * p.sk_L, U); s.u_end = min(s.u + p.sk_L, U);
-    s.w_dp = p.sk_T + unit;
-    // A slice whose last segment stops short of its work item's end only PUBLISHES a partial sum; it goes first, so
-    // that no partial ever waits behind a segment that itself waits for partials (which would chain the CTAs up).
-    s.lead0 = s.lead1 = 0;
-    if (s.u < s.u_end) {
-        const int wl = (s.u_end - 1) / s.kbs;
-        if (s.u_end < (wl + 1) * s.kbs) { s.lead0 = max(s.u, wl * s.kbs); s.lead1 = s.u_end; s.u_end = s.lead0; }
-    }
-    return s;
-}
-// next segment: work item w, stages [s0, s1) of its kbs stages
-template <bool KS>
-__device__ __forceinline__ bool sched_next(TcSched &s, int &w, int &s0, int &s1) {
-    if constexpr (!KS) {
-        if (s.w_dp >= s.num_work) return false;
-        w = s.w_dp; s.w_dp += s.w_step; s0 = 0; s1 = s.kbs;
-        return true;
-    }
-    if (s.lead0 < s.lead1) {
-        w = s.lead0 / s.kbs; s0 = s.lead0 - w * s.kbs; s1 = s.lead1 - w * s.kbs; s.lead1 = s.lead0;
-        return true;
-    }
-    if (s.u < s.u_end) {
-        w = s.u / s.kbs; s0 = s.u - w * s.kbs; s1 = min(s.kbs, s0 + (s.u_end - s.u)); s.u += s1 - s0;
-        return true;
-    }
-    if (s.w_dp >= s.num_work) return false;
-    w = s.w_dp; s.w_dp += s.w_step; s0 = 0; s1 = s.kbs;
-    return true;
-}
-__device__ __forceinline__ unsigned ld_acquire_u32(const unsigned *p) {
-    unsigned v; asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v;
-}
-__device__ __forceinline__ void st_release_u32(unsigned *p, unsigned v) {
-    asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-
 // Shared-memory barriers of both kernels: full[stages], empty[stages], then the resident-filter barrier.
 __device__ __forceinline__ uint32_t full_bar(uint32_t bars, int s) { return bars + 8u * (uint32_t)s; }
 __device__ __forceinline__ uint32_t empty_bar(uint32_t bars, int stages, int s) { return bars + 8u * (uint32_t)(stages + s); }
 
-// TMA producer (one elected thread): walks the consumers' schedule and keeps the ring full.  smemB: resident filter matrix
+// TMA producer (one elected thread): walks the consumers' work items and keeps the ring full.  smemB: resident filter matrix
 // (p.bstat), smem0: the ring.
-template <bool KS, bool ST>
+template <bool ST>
 __device__ __forceinline__ void tc_produce(const CUtensorMap *tmA, const CUtensorMap *tmB, const TcParams &p, uint32_t smemB,
                                            uint32_t smem0, uint32_t bars, int w_first, int w_step) {
     int stage = 0; uint32_t phase = 0;
@@ -413,20 +353,16 @@ __device__ __forceinline__ void tc_produce(const CUtensorMap *tmA, const CUtenso
         mbar_arrive_expect_tx(bstat_bar, p.bstat_bytes);
         for (int kb = 0; kb < kblocks; ++kb) tma_load_2d(smemB + (uint32_t)kb * b_bytes, tmB, bstat_bar, kb * BK, 0);
     }
-    TcSched sch = sched_init<KS>(p, w_first, w_step);
-    int w, seg0, seg1;
-    while (sched_next<KS>(sch, w, seg0, seg1)) {
+    for (int w = w_first; w < p.num_work; w += w_step) {
         const int n_idx = w % nt;
         const int m = w / nt;
         const int x0 = (m % xt) * p.TW;
         const int J0 = (m / xt) * p.TH + p.jshift;
         const int n0 = n_idx * p.BN;
-        const int kb_begin = seg0 * sps, kb_end = min(kblocks, seg1 * sps);
-        // channel block, tap x/y, K column of the weight matrix at the first K-block of the segment
-        const int tap0 = kb_begin / cblocks;
-        int cb = kb_begin - tap0 * cblocks, ky = tap0 / fsize, kx = tap0 - (tap0 / fsize) * fsize, kcol = kb_begin * BK;
-        for (int kb0 = kb_begin; kb0 < kb_end; kb0 += sps) {
-            const int nsub = min(sps, kb_end - kb0);
+        // channel block, tap x/y, K column of the weight matrix
+        int cb = 0, ky = 0, kx = 0, kcol = 0;
+        for (int kb0 = 0; kb0 < kblocks; kb0 += sps) {
+            const int nsub = min(sps, kblocks - kb0);
             if constexpr (ST) { const long long c0 = clock64(); mbar_wait(empty_bar(bars, stages, stage), phase ^ 1u); w_empty += clock64() - c0; }
             else mbar_wait(empty_bar(bars, stages, stage), phase ^ 1u);
             const uint32_t fb = full_bar(bars, stage);
@@ -455,26 +391,25 @@ __device__ __forceinline__ void tc_produce(const CUtensorMap *tmA, const CUtenso
     if (ST && p.stats) { p.stats[blockIdx.x * 16 + 0] = (unsigned long long)w_empty; p.stats[blockIdx.x * 16 + 1] = (unsigned long long)(clock64() - t_begin); p.stats[blockIdx.x * 16 + 7] = (unsigned long long)w_tma; }
 }
 
-// The K-blocks of stages [seg0, seg1) of the current work item into warpgroup wg's accumulator fragment d (rows 64 wg .. + 63
+// The K-blocks of the current work item into warpgroup wg's accumulator fragment d (rows 64 wg .. + 63
 // of the tile; KK wgmmas of K = 32 bytes per K-block).  A ring stage is released once the wgmmas that read it have retired,
 // one stage behind the issue (wgmma.wait_group 1) so that the tensor pipe never drains.  Nothing but wgmmas touches the
 // accumulators while wgmmas are in flight, and every batch is the same KK wgmmas: ptxas then inserts no fences of its own
 // and serializes nothing (the -Xptxas -v log has no C75xx notes).
 template <int KIND, int BN, int KK, bool ST, typename T>
 __device__ __forceinline__ void tc_mma_loop(T (&d)[BN / 2], const TcParams &p, uint32_t smemB, uint32_t smem0, uint32_t bars,
-                                            int wg, int lane, int &stage, uint32_t &phase, long long &w_full, int seg0, int seg1) {
+                                            int wg, int lane, int &stage, uint32_t &phase, long long &w_full) {
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) d[i] = T(0);
     wg_fence_operand(d);
-    const int sps = p.sps, stages = p.stages;
+    const int sps = p.sps, stages = p.stages, kblocks = p.kblocks;
     const uint32_t a_bytes = p.a_bytes, b_bytes = p.b_bytes, stage_bytes = p.stage_bytes, hi = p.desc_hi;
     const uint32_t b_off = (uint32_t)sps * a_bytes, a_wg = (uint32_t)wg * (a_bytes >> 1);
-    const int kb_begin = seg0 * sps, kb_end = min(p.kblocks, seg1 * sps);
     auto release = [&](int s) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar(bars, stages, s)); };
-    // one commit group per K-block; a stage (sps K-blocks, fewer at the end of the segment) is released once the group of
+    // one commit group per K-block; a stage (sps K-blocks, fewer at the end of the work item) is released once the group of
     // its last K-block has retired, which wgmma.wait_group 1 shows one K-block later
     int pend = -1, jj = 0;
-    for (int kb = kb_begin; kb < kb_end; ++kb) {
+    for (int kb = 0; kb < kblocks; ++kb) {
         if (jj == 0) {
             if constexpr (ST) { const long long c0 = clock64(); mbar_wait(full_bar(bars, stage), phase); w_full += clock64() - c0; }
             else mbar_wait(full_bar(bars, stage), phase);
@@ -486,11 +421,11 @@ __device__ __forceinline__ void tc_mma_loop(T (&d)[BN / 2], const TcParams &p, u
 #pragma unroll
         for (int k = 0; k < KK; ++k)
             Wg<KIND, BN>::mma(d, wg_desc(a_kb + 32u * (uint32_t)k, hi), wg_desc(b_kb + 32u * (uint32_t)k, hi),
-                              (kb > kb_begin || k > 0) ? 1u : 0u);
+                              (kb > 0 || k > 0) ? 1u : 0u);
         wg_commit();
         wg_wait<1>();
         if (pend >= 0) { release(pend); pend = -1; }
-        if (++jj == sps || kb + 1 == kb_end) {
+        if (++jj == sps || kb + 1 == kblocks) {
             pend = stage; jj = 0;
             if (++stage == stages) { stage = 0; phase ^= 1u; }
         }
@@ -500,13 +435,29 @@ __device__ __forceinline__ void tc_mma_loop(T (&d)[BN / 2], const TcParams &p, u
     if (pend >= 0) release(pend);
 }
 
+// The reference's float epilogue of the integer kinds, with its operations in its order (bit-exact results):
+//   kind 1, INT8 (yolov2_forward_network_quantized.c:474-490, :598-627): q16 = clamp(+-32767, acc / 32) [C truncating
+//     division]; y = (float)q16 * ALPHA1; y += bias; leaky: y / 10.
+//   kind 2, XNOR as +-1 s8 (acc == 2*count - K exactly): y = act((float)acc * mean + bias) (additionally.c:1531,
+//     yolov2_forward_network.c:243-261).
+// f: filter index (kind 2 reads its mean |w|).
+__device__ __forceinline__ float int_epilogue(const TcParams &p, int kind, int acc, int f, float bias) {
+    if (kind == 1) {
+        int q16 = acc / 32;
+        q16 = q16 > 32767 ? 32767 : (q16 < -32767 ? -32767 : q16);
+        const float t = __fadd_rn(__fmul_rn((float)q16, p.alpha1), bias);
+        return (p.act == ACT_LEAKY) ? ((t > 0.f) ? t : __fdiv_rn(t, 10.f)) : t;
+    }
+    const float t = __fadd_rn(__fmul_rn((float)acc, (f < p.n) ? __ldg(p.mean + f) : 0.f), bias);
+    return act_exact(t, p.act);
+}
+
 // One CTA per 128-pixel x BN-filter tile, persistent over the tiles (grid <= #SMs, one CTA per SM).
-// KS: compiled with the K-split tail schedule (TcParams::sk_T); the KS = false instantiations carry none of its code.
 // ST: compiled with the per-role cycle counters of YB_TC_STATS=1 (diagnostic); the production instantiations (ST = false)
 // contain no clock64() reads.
 // EPI: which epilogue family is compiled in -- 0: LSU stores, float kinds (bf16 / f32 heads / fused [yolo]); 2: the integer
 // kinds (s8 requantising and XNOR-as-+-1 epilogues).  The bf16 stride-1 layers run k_conv_tc_reg.
-template <bool KS, bool ST, int EPI>
+template <bool ST, int EPI>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
           const __grid_constant__ CUtensorMap tmR, const TcParams p) {
@@ -554,7 +505,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
 
     if (warp == TC_PRODUCER_WARP) {
         // ======================= TMA producer =======================
-        if (elect_one()) tc_produce<KS, ST>(&tmA, &tmB, p, smemB, smem0, bars, w_first, w_step);
+        if (elect_one()) tc_produce<ST>(&tmA, &tmB, p, smemB, smem0, bars, w_first, w_step);
     } else {
         // ======================= consumers (warps 0..7): wgmma main loop, then the epilogue of the same tile =======================
         const int ew = warp;                      // consumer warp; warpgroup ew >> 2 computes accumulator rows 64 * (ew >> 2) .. + 63
@@ -562,24 +513,24 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
         int stage = 0; uint32_t phase = 0;
         long long w_full = 0;
         if (p.bstat) mbar_wait(bstat_bar, 0);
-        // The K-blocks of stages [seg0, seg1) of the current work item into this warpgroup's registers, then both warpgroups'
-        // accumulators into the shared-memory tile.
-        auto mainloop = [&](auto kind_c, auto bn_c, auto kk_c, int seg0, int seg1) {
+        // The K-blocks of the current work item into this warpgroup's registers, then both warpgroups' accumulators into the
+        // shared-memory tile.
+        auto mainloop = [&](auto kind_c, auto bn_c, auto kk_c) {
             constexpr int KIND = decltype(kind_c)::value;
             constexpr int BN = decltype(bn_c)::value;
             constexpr int KK = decltype(kk_c)::value;   // wgmmas per K-block
             using T = typename std::conditional<KIND == 1 || KIND == 2, uint32_t, float>::type;
             T d[BN / 2];
-            tc_mma_loop<KIND, BN, KK, ST>(d, p, smemB, smem0, bars, wg, lane, stage, phase, w_full, seg0, seg1);
+            tc_mma_loop<KIND, BN, KK, ST>(d, p, smemB, smem0, bars, wg, lane, stage, phase, w_full);
             named_bar_sync(TC_ACC_BAR, 32 * TC_EPI_WARPS);   // every warp is done with the previous tile's accumulators
             acc_store_frag(acc_base, p.acc_pitch, wg * 64, d);
             named_bar_sync(TC_ACC_BAR, 32 * TC_EPI_WARPS);   // the whole 128 x BN tile is in place
         };
-        auto run_mainloop = [&](int seg0, int seg1) {
+        auto run_mainloop = [&]() {
             auto by_kk = [&](auto kind_c, auto bn_c) {
-                if (p.kk == 4) mainloop(kind_c, bn_c, std::integral_constant<int, 4>{}, seg0, seg1);
-                else if (p.kk == 2) mainloop(kind_c, bn_c, std::integral_constant<int, 2>{}, seg0, seg1);
-                else mainloop(kind_c, bn_c, std::integral_constant<int, 1>{}, seg0, seg1);
+                if (p.kk == 4) mainloop(kind_c, bn_c, std::integral_constant<int, 4>{});
+                else if (p.kk == 2) mainloop(kind_c, bn_c, std::integral_constant<int, 2>{});
+                else mainloop(kind_c, bn_c, std::integral_constant<int, 1>{});
             };
             auto by_bn = [&](auto kind_c) {
                 if (p.BN == 128) by_kk(kind_c, std::integral_constant<int, 128>{});
@@ -591,7 +542,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
             else by_bn(std::integral_constant<int, 3>{});
         };
 
-        // Epilogue.  Per 64-column slab: read the accumulator row(s) and the residual first, then the math and the stores.
+        // Epilogue.  Per slab: read the accumulator row(s) and the residual first, then the math and the stores.
         const int q = ew & 3;                     // 32-row quarter of the accumulator tile this warp reads
         const int half = ew >> 2;                 // which half of the columns this warp owns
         const int cbeg = (p.BN >= 64) ? half * (p.BN >> 1) : 0;
@@ -601,14 +552,8 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
         const bool leaky = p.act == ACT_LEAKY, leaky2 = p.act2 == ACT_LEAKY;
         const uint32_t taddr = acc_base + 4u * (uint32_t)(r * p.acc_pitch);
         long long w_res = 0; const long long t_begin = ST ? clock64() : 0;
-        TcSched sch = sched_init<KS>(p, w_first, w_step);
-        int w, seg0, seg1;
-        while (sched_next<KS>(sch, w, seg0, seg1)) {
-            run_mainloop(seg0, seg1);
-            // K-split tail: a segment that stops short of the work item's last stage only publishes its raw accumulator;
-            // the segment that ends the work item adds the npart partials of the CTAs gA .. unit-1 before it
-            const bool seg_partial = KS && seg1 < p.kbs;
-            const int npart = (KS && seg0 > 0 && !seg_partial) ? w_first - (w * p.kbs) / p.sk_L : 0;
+        for (int w = w_first; w < p.num_work; w += w_step) {
+            run_mainloop();
             const int n_idx = w % p.nt;
             const int m = w / p.nt;
             const int ox = (m % p.xt) * p.TW + tx;
@@ -622,98 +567,8 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
             const char *rrow = (p.res && valid) ? p.res + pix * p.res_ldc * 2 : nullptr;
             const float *bs = bias_s + n0;
 
-            uint4 rv[2][4];
-            auto load_res = [&](int f0, uint4 (&dst)[4]) {
-#pragma unroll
-                for (int g = 0; g < 4; ++g) {
-                    dst[g] = make_uint4(0u, 0u, 0u, 0u);
-                    if (rrow && (n0 + f0 + g * 8) < p.n_store)
-                        dst[g] = __ldg(reinterpret_cast<const uint4 *>(rrow + (size_t)(n0 + f0) * 2) + g);
-                }
-            };
-            // the staged bf16 store paths fetch their own residual, the integer / tf32 kinds never have one: rv[] is only
-            // prefetched for the per-thread store path (f32 heads, YB_TC_NO_COALESCE)
-            const bool own_res = EPI != 0 || (p.out_bf16 && ((cend - cbeg) >= 64 || (cend - cbeg) == 32) && !p.no_coalesce) || !p.res;
-            if (!own_res) {
-                if (cbeg < cend) load_res(cbeg, rv[0]);
-                if (cend - cbeg > 32) load_res(cbeg + 32, rv[1]);
-            }
-
-            const bool path64 = EPI == 0 && !seg_partial && p.out_bf16 && (cend - cbeg) >= 64 && !p.no_coalesce;
-
-            if constexpr (KS) {
-                auto flag_of = [&](int unit) { return p.sk_flags + ((size_t)unit * TC_EPI_WARPS + ew); };
-                auto ws_of = [&](int unit) { return reinterpret_cast<float4 *>(p.sk_ws) + (size_t)unit * (size_t)(TC_BM * 64); };
-                if (seg_partial) {
-                    // publish the raw f32 accumulator ([column/4][row] float4: a warp store is 512 contiguous bytes)
-                    float4 *dst = ws_of(w_first);
-                    for (int f0 = cbeg; f0 < cend; f0 += 32) {
-                        uint32_t v0[32];
-                        acc_ld32(taddr + 4u * (uint32_t)f0, v0);
-#pragma unroll
-                        for (int g4 = 0; g4 < 8; ++g4)
-                            __stcg(dst + (size_t)((f0 >> 2) + g4) * TC_BM + r,
-                                   make_float4(__uint_as_float(v0[g4 * 4]), __uint_as_float(v0[g4 * 4 + 1]),
-                                               __uint_as_float(v0[g4 * 4 + 2]), __uint_as_float(v0[g4 * 4 + 3])));
-                    }
-                    __threadfence();
-                    __syncwarp();
-                    if (lane == 0) st_release_u32(flag_of(w_first), 1u);
-                } else if (npart) {
-                    // owner: fold the partial sums of CTAs gA .. unit-1 into the accumulator tile, then run the
-                    // ordinary epilogue below on it
-                    const int gA = w_first - npart;
-                    for (int pc = 0; pc < npart; ++pc) {
-                        const unsigned *fl = flag_of(gA + pc);
-                        if (ld_acquire_u32(fl) == 0u) {
-                            const long long t0 = clock64();
-                            while (ld_acquire_u32(fl) == 0u) {
-                                if (clock64() - t0 > 4000000000LL) __trap();   // K-split partial never published
-                            }
-                        }
-                    }
-                    // 16 float4 loads in flight per thread: the fold is a latency-bound L2 read
-                    auto add4 = [](uint32_t (&v)[32], int g4, const float4 &t) {
-                        v[g4 * 4 + 0] = __float_as_uint(__uint_as_float(v[g4 * 4 + 0]) + t.x);
-                        v[g4 * 4 + 1] = __float_as_uint(__uint_as_float(v[g4 * 4 + 1]) + t.y);
-                        v[g4 * 4 + 2] = __float_as_uint(__uint_as_float(v[g4 * 4 + 2]) + t.z);
-                        v[g4 * 4 + 3] = __float_as_uint(__uint_as_float(v[g4 * 4 + 3]) + t.w);
-                    };
-                    for (int f0 = cbeg; f0 < cend; f0 += 64) {
-                        if (cend - f0 >= 64) {
-                            uint32_t v0[32], v1[32];
-                            acc_ld32(taddr + 4u * (uint32_t)f0, v0);
-                            acc_ld32(taddr + 4u * (uint32_t)f0 + 128u, v1);
-                            for (int pc = 0; pc < npart; ++pc) {
-                                const float4 *src = ws_of(gA + pc) + (size_t)(f0 >> 2) * TC_BM + r;
-                                float4 t[16];
-#pragma unroll
-                                for (int g4 = 0; g4 < 16; ++g4) t[g4] = __ldcg(src + (size_t)g4 * TC_BM);
-#pragma unroll
-                                for (int g4 = 0; g4 < 8; ++g4) { add4(v0, g4, t[g4]); add4(v1, g4, t[8 + g4]); }
-                            }
-                            acc_st32(taddr + 4u * (uint32_t)f0, v0);
-                            acc_st32(taddr + 4u * (uint32_t)f0 + 128u, v1);
-                        } else {
-                            uint32_t v[32];
-                            acc_ld32(taddr + 4u * (uint32_t)f0, v);
-                            for (int pc = 0; pc < npart; ++pc) {
-                                const float4 *src = ws_of(gA + pc) + (size_t)(f0 >> 2) * TC_BM + r;
-                                float4 t[8];
-#pragma unroll
-                                for (int g4 = 0; g4 < 8; ++g4) t[g4] = __ldcg(src + (size_t)g4 * TC_BM);
-#pragma unroll
-                                for (int g4 = 0; g4 < 8; ++g4) add4(v, g4, t[g4]);
-                            }
-                            acc_st32(taddr + 4u * (uint32_t)f0, v);
-                        }
-                    }
-                    __syncwarp();
-                    if (lane == 0) for (int pc = 0; pc < npart; ++pc) *flag_of(gA + pc) = 0u;   // re-arm for the next launch
-                }
-            }
-
-            auto finish = [&](const uint32_t (&v)[32], const uint4 (&rr)[4], int f0) {
+            // ---- f32 output (detection heads) of one 32-column slab, one row per thread
+            auto finish_f32 = [&](const uint32_t (&v)[32], int f0) {
                 if (!valid || (n0 + f0) >= p.n_store) return;
                 float x[32];
 #pragma unroll
@@ -721,34 +576,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                     float a = __uint_as_float(v[j]) + bs[f0 + j];
                     x[j] = leaky ? fmaxf(a, 0.1f * a) : a;   // == a > 0 ? a : 0.1a
                 }
-                if (p.res) {
-#pragma unroll
-                    for (int g = 0; g < 4; ++g) {
-                        const uint32_t wv[4] = {rr[g].x, rr[g].y, rr[g].z, rr[g].w};
-#pragma unroll
-                        for (int h = 0; h < 4; ++h) {
-                            x[g * 8 + 2 * h] += __uint_as_float(wv[h] << 16);
-                            x[g * 8 + 2 * h + 1] += __uint_as_float(wv[h] & 0xffff0000u);
-                        }
-                    }
-                    if (leaky2) {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) x[j] = fmaxf(x[j], 0.1f * x[j]);
-                    }
-                }
-                if (p.out_bf16) {
-                    uint4 *op = reinterpret_cast<uint4 *>(orow + (size_t)(n0 + f0) * 2);
-#pragma unroll
-                    for (int g = 0; g < 4; ++g) {
-                        if (n0 + f0 + g * 8 >= p.n_store) break;
-                        uint4 o;
-                        o.x = pack_bf16x2(x[g * 8 + 0], x[g * 8 + 1]);
-                        o.y = pack_bf16x2(x[g * 8 + 2], x[g * 8 + 3]);
-                        o.z = pack_bf16x2(x[g * 8 + 4], x[g * 8 + 5]);
-                        o.w = pack_bf16x2(x[g * 8 + 6], x[g * 8 + 7]);
-                        op[g] = o;
-                    }
-                } else if (p.yolo_out) {
+                if (p.yolo_out) {
                     // detection head with the [yolo] layer fused: logistic on x, y, objectness and class entries (w, h stay
                     // raw), written straight into the NCHW tensor the reference decoder reads -- the f32 NHWC copy of the
                     // head and the separate yolo kernel disappear
@@ -773,10 +601,10 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                 }
             };
 
-            // ---- coalesced f32 store of one 32-column slab (the integer kinds and the f32 heads): a row is 128 B; the warp's 32
-            // rows go through its private XOR-swizzled 4 KB staging tile so that every global store instruction writes 4 rows x
-            // 128 contiguous bytes instead of 32 rows x 16 B (32 different lines per instruction: what kept the early INT8
-            // layers at 0.8 TB/s in round 1)
+            // ---- coalesced f32 store of one 32-column slab (integer kinds at stride 2 or with the raw-accumulator dump): a row
+            // is 128 B; the warp's 32 rows go through its private XOR-swizzled 4 KB staging tile so that every global store
+            // instruction writes 4 rows x 128 contiguous bytes instead of 32 rows x 16 B (32 different lines per instruction:
+            // what kept the early INT8 layers at 0.8 TB/s in round 1)
             auto store_f32_slab = [&](const float (&y)[32], int f0) {
                 const uint32_t stg = stg_base + (uint32_t)ew * 4096u;
                 const int srow = lane >> 3, schunk = lane & 7;
@@ -830,16 +658,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
                     const int f = n0 + cbase + j;
-                    float t;
-                    if (p.kind == 1) {
-                        int q16 = h8[j] / 32;
-                        q16 = q16 > 32767 ? 32767 : (q16 < -32767 ? -32767 : q16);
-                        t = __fadd_rn(__fmul_rn((float)q16, p.alpha1), bs[cbase + j]);
-                        t = (p.act == ACT_LEAKY) ? ((t > 0.f) ? t : __fdiv_rn(t, 10.f)) : t;
-                    } else {
-                        t = __fadd_rn(__fmul_rn((float)h8[j], (f < p.n) ? __ldg(p.mean + f) : 0.f), bs[cbase + j]);
-                        t = act_exact(t, p.act);
-                    }
+                    const float t = int_epilogue(p, p.kind, h8[j], f, bs[cbase + j]);
                     int b8 = (p.pool_mode == 1) ? quant_i8(t, p.pool_mult) : (t > 0.f ? 1 : -1);
                     if (f >= p.n) b8 = 0;
                     if (j < 4) w0 |= (uint32_t)(b8 & 0xff) << (8 * j); else w1 |= (uint32_t)(b8 & 0xff) << (8 * (j - 4));
@@ -876,101 +695,27 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                 }
             };
 
-            if constexpr (EPI == 2) {
-            if (p.kind == 2) {
-                // ---- XNOR as +-1 int8: acc == 2*count - K (exact); out = act((float)acc * mean + bias) in the reference's
-                // float op order (additionally.c:1531, yolov2_forward_network.c:243-261)
-                for (int f0 = cbeg; f0 < cend; f0 += 32) {
-                    uint32_t v0[32];
-                    acc_ld32(taddr + 4u * (uint32_t)f0, v0);
-                    if (p.pool_mode) { pool_store_raw(v0, f0); continue; }
-                    float y[32];
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        const int f = n0 + f0 + j;
-                        float t = __fmul_rn((float)(int)v0[j], (f < p.n) ? __ldg(p.mean + f) : 0.f);
-                        t = __fadd_rn(t, bs[f0 + j]);
-                        y[j] = act_exact(t, p.act);
-                    }
-                    if (p.no_coalesce) {
-                        if (valid) {
-                            float *orow_f = reinterpret_cast<float *>(orow);
-#pragma unroll
-                            for (int g = 0; g < 8; ++g) {
-                                if (n0 + f0 + g * 4 >= p.n_store) break;
-                                *reinterpret_cast<float4 *>(orow_f + n0 + f0 + g * 4) = make_float4(y[g * 4], y[g * 4 + 1], y[g * 4 + 2], y[g * 4 + 3]);
-                            }
-                        }
-                    } else if (p.tma_epi) tma_store_f32_slab(y, f0);
-                    else store_f32_slab(y, f0);
-                    if (!valid) continue;
-                    if (p.acc_out) {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            const int f = n0 + f0 + j;
-                            if (f < p.n) p.acc_out[(((size_t)img * p.n + f) * p.OH + oy) * p.OW + ox] = ((int)v0[j] + p.xK) / 2;
-                        }
-                    }
-                }
-            } else
-            if (p.kind == 1) {
-                // ---- INT8: exact requantisation of the reference (yolov2_forward_network_quantized.c:474-490, :598-627):
-                // q16 = clamp(+-32767, acc / 32) [C truncating division]; y = (float)q16 * ALPHA1; y += bias; leaky: y / 10.
-                for (int f0 = cbeg; f0 < cend; f0 += 32) {
-                    uint32_t v0[32];
-                    acc_ld32(taddr + 4u * (uint32_t)f0, v0);
-                    if (p.pool_mode) { pool_store_raw(v0, f0); continue; }
-                    float y[32];
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        const int a = (int)v0[j];
-                        int q16 = a / 32;
-                        q16 = q16 > 32767 ? 32767 : (q16 < -32767 ? -32767 : q16);
-                        float t = __fmul_rn((float)q16, p.alpha1);
-                        t = __fadd_rn(t, bs[f0 + j]);
-                        y[j] = (p.act == ACT_LEAKY) ? ((t > 0.f) ? t : __fdiv_rn(t, 10.f)) : t;
-                    }
-                    if (p.no_coalesce) {
-                        if (valid) {
-                            float *orow_f = reinterpret_cast<float *>(orow);
-#pragma unroll
-                            for (int g = 0; g < 8; ++g) {
-                                if (n0 + f0 + g * 4 >= p.n_store) break;
-                                *reinterpret_cast<float4 *>(orow_f + n0 + f0 + g * 4) = make_float4(y[g * 4], y[g * 4 + 1], y[g * 4 + 2], y[g * 4 + 3]);
-                            }
-                        }
-                    } else if (p.tma_epi) tma_store_f32_slab(y, f0);
-                    else store_f32_slab(y, f0);
-                    if (!valid) continue;
-                    if (p.acc_out) {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            const int f = n0 + f0 + j;
-                            if (f < p.n) p.acc_out[(((size_t)img * p.n + f) * p.OH + oy) * p.OW + ox] = (int)v0[j];
-                        }
-                    }
-                }
-            }
-            } else {
-            if (seg_partial) {
-                // accumulator already published above
-            } else
-            if (path64) {
-                // ---- coalesced path: every global access of this warp is a run of whole 128-byte lines.
-                // Each warp owns 32 accumulator rows; per 64-column slab a row is 128 B of bf16.  Rows are
-                // transposed through the warp's private swizzled staging tile so that one warp instruction moves
-                // 4 rows x 128 B instead of 32 rows x 16 B (the latter costs 32 LSU cycles per instruction and made
-                // the epilogue the bottleneck of every layer).
+            // ---- bf16 output (the stride-2 layers) in slabs of SW = 64 or 32 columns: every global access of this warp is a
+            // run of whole 2 * SW-byte rows.  Each warp owns 32 accumulator rows; they are transposed through the warp's private
+            // staging tile (16-byte chunk c of row r at r * 2 SW + ((c ^ swizzle(r)) << 4)) so that one warp instruction moves
+            // 4 rows x 128 B (SW = 64) or 8 rows x 64 B (SW = 32) instead of 32 rows x 16 B (the latter costs 32 LSU cycles per
+            // instruction and made the epilogue the bottleneck of every layer).  The shortcut residual comes in the same way.
+            auto bf16_slabs = [&](auto sw_c) {
+                constexpr int SW = decltype(sw_c)::value;
+                constexpr int CH = SW / 8, RPI = 32 / CH;   // 16-byte chunks per row, rows per warp instruction
                 const uint32_t stg = stg_base + (uint32_t)ew * 4096u;
-                const int srow = lane >> 3, schunk = lane & 7;
+                const int srow = lane / CH, schunk = lane % CH;
                 const unsigned long long obase = (unsigned long long)(uintptr_t)orow;
                 const unsigned long long rbase = (unsigned long long)(uintptr_t)rrow;
                 const int vflag = valid ? 1 : 0;
-                auto stage_addr = [&](int row, int chunk) { return stg + (uint32_t)row * 128u + (uint32_t)((chunk ^ (row & 7)) << 4); };
+                auto stage_addr = [&](int row, int chunk) {
+                    const int sw = (SW == 64) ? (row & 7) : ((row >> 1) & 3);
+                    return stg + (uint32_t)row * (2u * SW) + (uint32_t)((chunk ^ sw) << 4);
+                };
                 auto res_to_stage = [&](int f0) {     // coalesced global -> staging
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        const int row = i * 4 + srow;
+                    for (int i = 0; i < CH; ++i) {
+                        const int row = i * RPI + srow;
                         const unsigned long long rp = __shfl_sync(0xffffffffu, rbase, row);
                         uint4 v = make_uint4(0u, 0u, 0u, 0u);
                         if (rp && (n0 + f0 + schunk * 8) < p.n_store)
@@ -979,21 +724,23 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                     }
                 };
                 if (p.res) res_to_stage(cbeg);
-                for (int f0 = cbeg; f0 < cend; f0 += 64) {
-                    uint32_t v0[32], v1[32];
-                    acc_ld32(taddr + 4u * (uint32_t)f0, v0);
-                    acc_ld32(taddr + 4u * (uint32_t)f0 + 128u, v1);
-                    float x[64];
+                for (int f0 = cbeg; f0 < cend; f0 += SW) {
+                    uint32_t v[SW / 32][32];
+#pragma unroll
+                    for (int h = 0; h < SW / 32; ++h) acc_ld32(taddr + 4u * (uint32_t)(f0 + 32 * h), v[h]);
+                    float x[SW];
 #pragma unroll
                     for (int j = 0; j < 32; ++j) {
-                        const float a0 = __uint_as_float(v0[j]) + bs[f0 + j], a1 = __uint_as_float(v1[j]) + bs[f0 + 32 + j];
-                        x[j] = leaky ? fmaxf(a0, 0.1f * a0) : a0;
-                        x[32 + j] = leaky ? fmaxf(a1, 0.1f * a1) : a1;
+#pragma unroll
+                        for (int h = 0; h < SW / 32; ++h) {
+                            const float a = __uint_as_float(v[h][j]) + bs[f0 + 32 * h + j];
+                            x[32 * h + j] = leaky ? fmaxf(a, 0.1f * a) : a;
+                        }
                     }
                     if (p.res) {
                         __syncwarp();
 #pragma unroll
-                        for (int c = 0; c < 8; ++c) {          // own row back from staging
+                        for (int c = 0; c < CH; ++c) {          // own row back from staging
                             uint32_t w0, w1, w2, w3;
                             asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(w0), "=r"(w1), "=r"(w2), "=r"(w3) : "r"(stage_addr(lane, c)) : "memory");
                             const uint32_t wv[4] = {w0, w1, w2, w3};
@@ -1005,19 +752,19 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                         }
                         if (leaky2) {
 #pragma unroll
-                            for (int j = 0; j < 64; ++j) x[j] = fmaxf(x[j], 0.1f * x[j]);
+                            for (int j = 0; j < SW; ++j) x[j] = fmaxf(x[j], 0.1f * x[j]);
                         }
                         __syncwarp();
                     }
 #pragma unroll
-                    for (int c = 0; c < 8; ++c)                 // own row -> staging
+                    for (int c = 0; c < CH; ++c)                // own row -> staging
                         asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(stage_addr(lane, c)),
                                      "r"(pack_bf16x2(x[c * 8 + 0], x[c * 8 + 1])), "r"(pack_bf16x2(x[c * 8 + 2], x[c * 8 + 3])),
                                      "r"(pack_bf16x2(x[c * 8 + 4], x[c * 8 + 5])), "r"(pack_bf16x2(x[c * 8 + 6], x[c * 8 + 7])) : "memory");
                     __syncwarp();
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) {               // staging -> coalesced global
-                        const int row = i * 4 + srow;
+                    for (int i = 0; i < CH; ++i) {              // staging -> coalesced global
+                        const int row = i * RPI + srow;
                         const unsigned long long op = __shfl_sync(0xffffffffu, obase, row);
                         const int ok = __shfl_sync(0xffffffffu, vflag, row);
                         uint32_t w0, w1, w2, w3;
@@ -1026,95 +773,51 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                             *(reinterpret_cast<uint4 *>(op + (size_t)(n0 + f0) * 2) + schunk) = make_uint4(w0, w1, w2, w3);
                     }
                     __syncwarp();
-                    if (p.res && f0 + 64 < cend) res_to_stage(f0 + 64);   // next slab's residual in flight
+                    if (p.res && f0 + SW < cend) res_to_stage(f0 + SW);   // next slab's residual in flight
                 }
-            } else if (p.out_bf16 && (cend - cbeg) == 32 && !p.no_coalesce) {
-                // ---- coalesced path for 32-column slabs (BN = 32 / 64): a row is 64 B of bf16; the warp's staging
-                // tile is 32 rows x 64 B (16-byte chunk j of row r at r*64 + ((j ^ ((r >> 1) & 3)) << 4)); one
-                // instruction moves 8 rows x 64 B.
-                const uint32_t stg = stg_base + (uint32_t)ew * 4096u;
-                const int srow = lane >> 2, schunk = lane & 3;
-                const unsigned long long obase = (unsigned long long)(uintptr_t)orow;
-                const unsigned long long rbase = (unsigned long long)(uintptr_t)rrow;
-                const int vflag = valid ? 1 : 0;
-                auto stage_addr = [&](int row, int chunk) { return stg + (uint32_t)row * 64u + (uint32_t)((chunk ^ ((row >> 1) & 3)) << 4); };
-                const int f0 = cbeg;
-                if (p.res) {
+            };
+
+            if constexpr (EPI == 2) {
+                // ---- integer kinds: the exact float epilogue per 32-column slab (or the fused max-pool), f32 stores
+                auto int_slabs = [&](auto kind_c) {
+                    constexpr int KIND = decltype(kind_c)::value;
+                    for (int f0 = cbeg; f0 < cend; f0 += 32) {
+                        uint32_t v0[32];
+                        acc_ld32(taddr + 4u * (uint32_t)f0, v0);
+                        if (p.pool_mode) { pool_store_raw(v0, f0); continue; }
+                        float y[32];
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        const int row = i * 8 + srow;
-                        const unsigned long long rp = __shfl_sync(0xffffffffu, rbase, row);
-                        uint4 v = make_uint4(0u, 0u, 0u, 0u);
-                        if (rp && (n0 + f0 + schunk * 8) < p.n_store)
-                            v = __ldg(reinterpret_cast<const uint4 *>(rp + (size_t)(n0 + f0) * 2) + schunk);
-                        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(stage_addr(row, schunk)), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-                    }
-                }
-                uint32_t v0[32];
-                acc_ld32(taddr + 4u * (uint32_t)f0, v0);
-                float x[32];
+                        for (int j = 0; j < 32; ++j) y[j] = int_epilogue(p, KIND, (int)v0[j], n0 + f0 + j, bs[f0 + j]);
+                        if (p.tma_epi) tma_store_f32_slab(y, f0);
+                        else store_f32_slab(y, f0);
+                        if (!valid || !p.acc_out) continue;
 #pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const float a0 = __uint_as_float(v0[j]) + bs[f0 + j];
-                    x[j] = leaky ? fmaxf(a0, 0.1f * a0) : a0;
-                }
-                if (p.res) {
-                    __syncwarp();
-#pragma unroll
-                    for (int c = 0; c < 4; ++c) {
-                        uint32_t w0, w1, w2, w3;
-                        asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(w0), "=r"(w1), "=r"(w2), "=r"(w3) : "r"(stage_addr(lane, c)) : "memory");
-                        const uint32_t wv[4] = {w0, w1, w2, w3};
-#pragma unroll
-                        for (int h = 0; h < 4; ++h) {
-                            x[c * 8 + 2 * h] += __uint_as_float(wv[h] << 16);
-                            x[c * 8 + 2 * h + 1] += __uint_as_float(wv[h] & 0xffff0000u);
+                        for (int j = 0; j < 32; ++j) {
+                            const int f = n0 + f0 + j;
+                            // raw results: the INT8 accumulator; XNOR: the reference's popcount, (dot + K) / 2
+                            if (f < p.n) p.acc_out[(((size_t)img * p.n + f) * p.OH + oy) * p.OW + ox] = KIND == 2 ? ((int)v0[j] + p.xK) / 2 : (int)v0[j];
                         }
                     }
-                    if (leaky2) {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) x[j] = fmaxf(x[j], 0.1f * x[j]);
+                };
+                if (p.kind == 2) int_slabs(std::integral_constant<int, 2>{});
+                else int_slabs(std::integral_constant<int, 1>{});
+            } else if (p.out_bf16) {
+                if (cend - cbeg >= 64) bf16_slabs(std::integral_constant<int, 64>{});
+                else if (cend > cbeg) bf16_slabs(std::integral_constant<int, 32>{});
+            } else {
+                for (int f0 = cbeg; f0 < cend; f0 += 64) {
+                    if (cend - f0 >= 64) {
+                        uint32_t v0[32], v1[32];
+                        acc_ld32(taddr + 4u * (uint32_t)f0, v0);
+                        acc_ld32(taddr + 4u * (uint32_t)f0 + 128u, v1);
+                        finish_f32(v0, f0);
+                        finish_f32(v1, f0 + 32);
+                    } else {
+                        uint32_t v0[32];
+                        acc_ld32(taddr + 4u * (uint32_t)f0, v0);
+                        finish_f32(v0, f0);
                     }
-                    __syncwarp();
                 }
-#pragma unroll
-                for (int c = 0; c < 4; ++c)
-                    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(stage_addr(lane, c)),
-                                 "r"(pack_bf16x2(x[c * 8 + 0], x[c * 8 + 1])), "r"(pack_bf16x2(x[c * 8 + 2], x[c * 8 + 3])),
-                                 "r"(pack_bf16x2(x[c * 8 + 4], x[c * 8 + 5])), "r"(pack_bf16x2(x[c * 8 + 6], x[c * 8 + 7])) : "memory");
-                __syncwarp();
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const int row = i * 8 + srow;
-                    const unsigned long long op = __shfl_sync(0xffffffffu, obase, row);
-                    const int ok = __shfl_sync(0xffffffffu, vflag, row);
-                    uint32_t w0, w1, w2, w3;
-                    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(w0), "=r"(w1), "=r"(w2), "=r"(w3) : "r"(stage_addr(row, schunk)) : "memory");
-                    if (ok && (n0 + f0 + schunk * 8) < p.n_store)
-                        *(reinterpret_cast<uint4 *>(op + (size_t)(n0 + f0) * 2) + schunk) = make_uint4(w0, w1, w2, w3);
-                }
-                __syncwarp();
-            } else
-            for (int f0 = cbeg; f0 < cend; f0 += 64) {
-                if (cend - f0 >= 64) {
-                    uint32_t v0[32], v1[32];
-                    acc_ld32(taddr + 4u * (uint32_t)f0, v0);
-                    acc_ld32(taddr + 4u * (uint32_t)f0 + 128u, v1);
-                    uint4 r0[4], r1[4];
-#pragma unroll
-                    for (int g = 0; g < 4; ++g) { r0[g] = rv[0][g]; r1[g] = rv[1][g]; }
-                    if (f0 + 64 < cend) {                                   // next slab's residual in flight
-                        load_res(f0 + 64, rv[0]);
-                        if (cend - (f0 + 64) > 32) load_res(f0 + 96, rv[1]);
-                    }
-                    finish(v0, r0, f0);
-                    finish(v1, r1, f0 + 32);
-                } else {
-                    uint32_t v0[32];
-                    acc_ld32(taddr + 4u * (uint32_t)f0, v0);
-                    finish(v0, rv[0], f0);
-                }
-            }
             }
         }
         if (EPI == 2 && p.tma_epi && q == 0 && lane == 0) tma_store_wait_all();   // this group's bulk stores have completed
@@ -1254,7 +957,7 @@ k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     if (wg == 2) {
         asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(TCR_PRODUCER_REGS));
         if (warp == 8) {
-            if (elect_one()) tc_produce<false, ST>(&tmA, &tmB, p, smemB, smem0, bars, w_first, w_step);
+            if (elect_one()) tc_produce<ST>(&tmA, &tmB, p, smemB, smem0, bars, w_first, w_step);
         } else if (warp < TCR_STORE_WARP + 2 && epi_mem) {
             const int g = warp - TCR_STORE_WARP;
             if (elect_one()) tcr_store<ST>(&tmO, &tmR, p, stg_base + (uint32_t)g * 128u * (uint32_t)p.BN, stg_full(g, 0), stg_ready(g), g, w_first, w_step);
@@ -1288,7 +991,7 @@ k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
         };
         for (int w = w_first; w < p.num_work; w += w_step) {
             float d[BN / 2];
-            tc_mma_loop<0, BN, KK, ST>(d, p, smemB, smem0, bars, wg, lane, stage, phase, w_full, 0, p.kbs);
+            tc_mma_loop<0, BN, KK, ST>(d, p, smemB, smem0, bars, wg, lane, stage, phase, w_full);
             if (!epi_mem) continue;
             const int n0 = (w % p.nt) * BN, m = w / p.nt;
             const int x0 = (m % p.xt) * p.TW, J0 = (m / p.xt) * p.TH + p.jshift;
@@ -1634,7 +1337,7 @@ int tc_conv_supported(const Layer &l, const TV &in, const TV &out, bool out_bf16
 
 static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &out, bool out_bf16, const TV &res,
                               bool res_bf16, int act2, const void *d_weights_bf16, int ldn, const float *d_bias,
-                              float alpha1, int *acc_out, int wide_rows = 0, int no_tma_epi = 0, int want_pool_tile = 0) {
+                              float alpha1, int *acc_out, int wide_rows = 0, int want_pool_tile = 0) {
     TcPlan *plan = new TcPlan();
     memset(plan, 0, sizeof(*plan));
     TcParams &p = plan->p;
@@ -1646,8 +1349,7 @@ static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &
     // (stride-2 layers keep the LSU epilogue: their tiles walk the input's merged half-rows, OH + 1 per image, while the output has
     // OH + 2 rows per image -- a per-image (c, x, y, image) store would need a negative start row for the second image of a
     // straddling tile, and bulk tensor STORES fault on negative coordinates)
-    const bool reg = kind == 0 && out_bf16 && l.stride == 1 && !no_tma_epi && !getenv("YB_TC_NO_TMA_EPI") &&
-                     !getenv("YB_TC_NO_COALESCE") && (!res.base || res_bf16);
+    const bool reg = kind == 0 && out_bf16 && l.stride == 1;
     p.kind = kind; p.alpha1 = alpha1; p.acc_out = acc_out;
     p.kk = BK * esz / 32;
     const bool s2 = l.stride == 2;
@@ -1691,8 +1393,7 @@ static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &
     const int BN = reg ? pick_bn_reg(l.n, (long)p.xt * p.jt, p.kblocks, sms) : pick_bn(l.n);
     p.BN = BN;
     p.nt = (l.n + BN - 1) / BN;
-    p.num_tiles = p.xt * p.jt * p.nt;
-    p.num_work = p.num_tiles;
+    p.num_work = p.xt * p.jt * p.nt;
     p.a_bytes = (uint32_t)(TC_BM * BK * esz);
     p.b_bytes = (uint32_t)(BN * BK * esz);
     // small filter matrices stay resident in shared memory for the whole kernel (one TMA pass per CTA)
@@ -1702,9 +1403,8 @@ static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &
     // one staging buffer of 64 pixels x BN (64 / 32 / 16 / 8 KB per CTA at BN = 256 / 128 / 64 / 32); integer kinds: f32 slabs of
     // 32 columns (128-byte rows), one 128-pixel tile per warp group -- the raw-accumulator dump (tests) keeps the LSU path
     p.tma_epi = 0;
-    const bool i8kind = kind == 1 || kind == 2;
     if (reg) p.tma_epi = BN >= 64 ? 64 : 32;
-    if (i8kind && !s2 && !acc_out && !getenv("YB_TC_NO_TMA_EPI") && !getenv("YB_TC_NO_COALESCE")) p.tma_epi = 32;
+    if (i8 && !s2 && !acc_out) p.tma_epi = 32;
     p.stg_bytes = reg ? 2u * 64u * (uint32_t)BN * 2u : p.tma_epi ? 2u * 16384u : 4096u * TC_EPI_WARPS;
     p.acc_pitch = BN + 4;
     const size_t acc_bytes = reg ? 0 : (size_t)TC_BM * p.acc_pitch * 4;   // k_conv_tc_reg keeps the accumulators in registers
@@ -1724,7 +1424,6 @@ static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &
     }
     p.stage_bytes = (uint32_t)p.sps * ring_blk;
     p.kbs = (p.kblocks + p.sps - 1) / p.sps;
-    p.sk_T = 0; p.sk_L = 1;
     const size_t max_stages = getenv("YB_TC_MAX_STAGES") ? (size_t)atoi(getenv("YB_TC_MAX_STAGES")) : 8;
     p.stages = (int)std::min<size_t>(max_stages, (ring_budget - p.bstat_bytes - fixed_smem) / p.stage_bytes);
     if (p.stages < 2) fatal_throw("tc plan: tile does not fit shared memory");
@@ -1738,11 +1437,11 @@ static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &
     p.res = res.base; p.res_ldc = res.ldc; p.res_bf16 = res_bf16 ? 1 : 0;
     if (res.base && (res.H != l.out_h || res.W != l.out_w || res.C != l.n)) fatal_throw("tc plan: residual shape mismatch");
     if (res.base && !res_bf16) fatal_throw("tc plan: residual must be bf16");
+    if (res.base && !out_bf16) fatal_throw("tc plan: a fused residual needs a bf16 output");
     if (res.base && res_bf16 && (res.ldc % 8 != 0 || (reinterpret_cast<uintptr_t>(res.base) & 15))) fatal_throw("tc plan: residual alignment");
     p.bias = d_bias; p.act = l.activation; p.act2 = act2;
     p.dbg = getenv("YB_TC_DBG") ? atoi(getenv("YB_TC_DBG")) : 0;
     p.l2_hint = (kind == 0 && !getenv("YB_TC_NO_L2_HINT")) ? 1 : 0;
-    p.no_coalesce = getenv("YB_TC_NO_COALESCE") ? 1 : 0;
     snprintf(plan->desc, sizeof(plan->desc), "%dx%dx%d -> n%d k%d s%d%s", l.c, l.h, l.w, l.n, l.size, l.stride, reg ? " reg" : "");
 
     const CUtensorMapSwizzle swz = row_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
@@ -1801,7 +1500,7 @@ static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &
         if (res.base && out_bf16) encode_px(&plan->tmR, res, "residual");
     }
     plan->pdl = (getenv("YB_NO_PDL") == nullptr) ? 1 : 0;
-    plan->grid = std::min(p.num_tiles, grid_cap(sms));
+    plan->grid = std::min(p.num_work, grid_cap(sms));
     plan->threads = reg ? TCR_THREADS : TC_THREADS;
     if (getenv("YB_TC_STATS")) {
         cudaMalloc(&p.stats, sizeof(unsigned long long) * 16 * plan->grid);
@@ -1814,10 +1513,8 @@ static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &
                  acc_bytes /*accumulator tile*/;
     if (plan->smem > 227 * 1024) { delete plan; fatal_throw("tc plan: shared memory budget exceeded"); }
     {
-        const void *fns[] = {(const void *)k_conv_tc<false, false, 0>, (const void *)k_conv_tc_reg<false>,
-                             (const void *)k_conv_tc<false, false, 2>, (const void *)k_conv_tc<true, false, 0>,
-                             (const void *)k_conv_tc<false, true, 0>, (const void *)k_conv_tc_reg<true>,
-                             (const void *)k_conv_tc<false, true, 2>};
+        const void *fns[] = {(const void *)k_conv_tc<false, 0>, (const void *)k_conv_tc_reg<false>, (const void *)k_conv_tc<false, 2>,
+                             (const void *)k_conv_tc<true, 0>, (const void *)k_conv_tc_reg<true>, (const void *)k_conv_tc<true, 2>};
         for (const void *f : fns)
             if (cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
                 fatal_throw("cudaFuncSetAttribute(k_conv_tc) failed");
@@ -1826,8 +1523,8 @@ static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &
 }
 
 void *tc_make_plan(const Layer &l, const TV &in, const TV &out, bool out_bf16, const TV &res, bool res_bf16,
-                   int act2, const void *d_weights_bf16, int ldn, const float *d_bias, int wide_rows, int want_ksplit) {
-    return make_plan_common(0, l, in, out, out_bf16, res, res_bf16, act2, d_weights_bf16, ldn, d_bias, 0.f, nullptr, wide_rows, want_ksplit);
+                   int act2, const void *d_weights_bf16, int ldn, const float *d_bias, int wide_rows) {
+    return make_plan_common(0, l, in, out, out_bf16, res, res_bf16, act2, d_weights_bf16, ldn, d_bias, 0.f, nullptr, wide_rows);
 }
 
 // FP32 convolution of the exact (INT8 / XNOR) networks on the tf32 wgmma: f32 NHWC activations and f32 [ldn][K] weights go
@@ -1884,7 +1581,7 @@ int tc_plan_fuse_pool(void *vp, int mode, float mult, const TV &qnext) {
 void *tc_make_plan_i8(const Layer &l, const TV &q, const TV &out, const void *d_weights_s8, int ldn, const float *d_bias,
                       float alpha1, int *acc_out, int want_pool_tile) {
     TV none{};
-    return make_plan_common(1, l, q, out, false, none, false, ACT_LINEAR, d_weights_s8, ldn, d_bias, alpha1, acc_out, 0, 0, want_pool_tile);
+    return make_plan_common(1, l, q, out, false, none, false, ACT_LINEAR, d_weights_s8, ldn, d_bias, alpha1, acc_out, 0, want_pool_tile);
 }
 
 // XNOR layer mapped onto the s8 wgmma: activations and weights as +-1 bytes, so the s32 accumulator is 2*count - K.
@@ -1892,48 +1589,10 @@ void *tc_make_plan_xnor(const Layer &l, const TV &q, const TV &out, const void *
                         const float *d_mean, int *counts_out, int want_pool_tile) {
     TV none{};
     TcPlan *plan = reinterpret_cast<TcPlan *>(
-        make_plan_common(2, l, q, out, false, none, false, ACT_LINEAR, d_weights_pm1, ldn, d_bias, 0.f, counts_out, 0, 0, want_pool_tile));
+        make_plan_common(2, l, q, out, false, none, false, ACT_LINEAR, d_weights_pm1, ldn, d_bias, 0.f, counts_out, 0, want_pool_tile));
     plan->p.mean = d_mean;
     plan->p.xK = l.size * l.size * l.c;
     return plan;
-}
-
-// K-split of the tail wave (see TcParams::sk_T).  With G CTAs and num_work = R*G + T work items, the plain
-// schedule costs R+1 waves; cutting the T tail items along K into G equal slices costs R + L/kbs waves plus the
-// partial-sum round trip through L2 (hidden behind the next work item's main loop when R > 0).
-// `ws`: sms * 128 KB, `flags`: sms * 8 words, zero-initialised, owned by the caller (one per stream of execution).
-size_t tc_ksplit_ws_bytes(int sms) { return (size_t)sms * TC_BM * 256 * sizeof(float); }
-size_t tc_ksplit_flag_bytes(int sms) { return (size_t)sms * TC_EPI_WARPS * sizeof(unsigned); }
-int tc_plan_enable_ksplit(void *vp, float *ws, unsigned *flags) {
-    TcPlan *plan = reinterpret_cast<TcPlan *>(vp);
-    TcParams &p = plan->p;
-    const char *ev = getenv("YB_TC_KSPLIT");                 // 0: never (even when the option asks for it)
-    if (ev && ev[0] == '0') return 0;
-    if (p.kind != 0 || !ws || !flags || p.tma_epi) return 0;   // (the K-split kernel has the LSU epilogue only)
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const int G = grid_cap(sms);
-    const int R = p.num_work / G, T = p.num_work % G;
-    if (T == 0) return 0;
-    // Only deep-K layers: with few stages per work item the epilogue, not the tensor pipe, bounds the tile, and the
-    // partial-sum round trip (one more accumulator read + ~2 us of L2 latency per partial) costs more than the wave saves.
-    const int mink = getenv("YB_TC_KSPLIT_MINK") ? atoi(getenv("YB_TC_KSPLIT_MINK")) : 16;
-    if (p.kbs < mink) return 0;
-    const int pmax = getenv("YB_TC_KSPLIT_PIECES") ? std::max(1, atoi(getenv("YB_TC_KSPLIT_PIECES"))) : 3;
-    const int lmin = std::max(2, (p.kbs + pmax - 1) / pmax);           // at most ~pmax slices per work item
-    int L = std::max(lmin, (T * p.kbs + G - 1) / G);
-    if (L >= p.kbs) return 0;
-    // stage-times: exposed cost of the partial round trip (hidden behind the next item unless this is the only wave)
-    // Predicted gain in stage-times.  The partial round trip costs ~6 stages, and the idle tail of the plain schedule is
-    // not all waste: the next kernel's prologue runs in it (programmatic dependent launch); hence the 12 % minimum.
-    const double ovh = (R == 0) ? 10.0 : 6.0;
-    const double before = (double)(R + 1) * p.kbs, after = (double)R * p.kbs + L + ovh;
-    const double mingain = getenv("YB_TC_KSPLIT_MINGAIN") ? atof(getenv("YB_TC_KSPLIT_MINGAIN")) : 0.12;
-    if (before - after < mingain * before) return 0;
-    p.sk_T = T; p.sk_L = L; p.sk_ws = ws; p.sk_flags = flags;
-    plan->grid = G;
-    return 1;
 }
 
 struct StemPlan { StemTcP p; int grid; };
@@ -1986,19 +1645,12 @@ void tc_launch(void *vp, cudaStream_t s) {
         ++na;
     }
     cfg.attrs = attr; cfg.numAttrs = na;
-    const int epi = (plan->p.kind == 1 || plan->p.kind == 2) ? 2 : plan->p.tma_epi ? 1 : 0;   // 1: k_conv_tc_reg
-    static const bool ks_always = getenv("YB_TC_KS_ALWAYS") != nullptr;   // experiment: one kernel variant for every LSU-epilogue layer
-    const bool ks = plan->p.sk_T > 0 || (ks_always && epi == 0);
-    const bool st = plan->p.stats != nullptr && !ks;   // role counters: a separate instantiation (YB_TC_STATS=1)
+    const bool st = plan->p.stats != nullptr;   // role counters: a separate instantiation (YB_TC_STATS=1)
     const TcPlan &P = *plan;
-#define YB_TC_LAUNCH(KS_, ST_, EPI_) cudaLaunchKernelEx(&cfg, k_conv_tc<KS_, ST_, EPI_>, P.tmA, P.tmB, P.tmO, P.tmR, P.p)
-    if (ks) YB_TC_LAUNCH(true, false, 0);
-    else if (epi == 1) {
-        if (st) cudaLaunchKernelEx(&cfg, k_conv_tc_reg<true>, P.tmA, P.tmB, P.tmO, P.tmR, P.p);
-        else cudaLaunchKernelEx(&cfg, k_conv_tc_reg<false>, P.tmA, P.tmB, P.tmO, P.tmR, P.p);
-    }
-    else if (epi == 2) { if (st) YB_TC_LAUNCH(false, true, 2); else YB_TC_LAUNCH(false, false, 2); }
-    else { if (st) YB_TC_LAUNCH(false, true, 0); else YB_TC_LAUNCH(false, false, 0); }
+#define YB_TC_LAUNCH(KERNEL) cudaLaunchKernelEx(&cfg, KERNEL, P.tmA, P.tmB, P.tmO, P.tmR, P.p)
+    if (plan->threads == TCR_THREADS) { if (st) YB_TC_LAUNCH(k_conv_tc_reg<true>); else YB_TC_LAUNCH(k_conv_tc_reg<false>); }
+    else if (P.p.kind == 1 || P.p.kind == 2) { if (st) YB_TC_LAUNCH((k_conv_tc<true, 2>)); else YB_TC_LAUNCH((k_conv_tc<false, 2>)); }
+    else { if (st) YB_TC_LAUNCH((k_conv_tc<true, 0>)); else YB_TC_LAUNCH((k_conv_tc<false, 0>)); }
 #undef YB_TC_LAUNCH
 }
 
@@ -2010,9 +1662,8 @@ void tc_free_plan(void *vp) {
         cudaMemcpy(h.data(), plan->p.stats, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
         double m[16] = {0};
         for (int b = 0; b < plan->grid; ++b) for (int k = 0; k < 16; ++k) m[k] += (double)h[16 * b + k] / plan->grid;
-        fprintf(stderr, "TCSTATS %-28s tiles/cta %.1f kb %d sps %d BN %d ksplit T%d L%d/%d | producer: wait_empty %.0f tma_issue %.0f total %.0f | ",
-                plan->desc, (double)plan->p.num_tiles / plan->grid * 1.0, plan->p.kblocks, plan->p.sps, plan->p.BN, plan->p.sk_T, plan->p.sk_L,
-                plan->p.kbs, m[0], m[7], m[1]);
+        fprintf(stderr, "TCSTATS %-28s tiles/cta %.1f kb %d sps %d BN %d | producer: wait_empty %.0f tma_issue %.0f total %.0f | ",
+                plan->desc, (double)plan->p.num_work / plan->grid, plan->p.kblocks, plan->p.sps, plan->p.BN, m[0], m[7], m[1]);
         if (plan->threads == TCR_THREADS)   // k_conv_tc_reg: the consumers' wait on stg_ready (first work item apart) and the store warps
             fprintf(stderr, "consumers: wait_full %.0f wait_ready %.0f (first item %.0f) total %.0f | store: wait_full %.0f wait_read %.0f\n",
                     m[2], m[8], m[3], m[6], m[4], m[5]);

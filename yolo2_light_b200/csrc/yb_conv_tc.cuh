@@ -12,9 +12,9 @@ namespace yb {
 int tc_conv_supported(const Layer &l, const TV &in, const TV &out, bool out_bf16);
 // builds the per-layer launch state (TMA tensor maps, tile schedule); throws yb::Error on failure.
 // wide_rows: prefer wide pixel tiles (the plan will get tc_plan_fuse_yolo: NCHW plane stores in the epilogue)
-// want_ksplit: the plan may get tc_plan_enable_ksplit (keeps the LSU epilogue: the K-split kernel has no TMA epilogue)
+// res: fused shortcut operand (bf16; needs a bf16 output)
 void *tc_make_plan(const Layer &l, const TV &in, const TV &out, bool out_bf16, const TV &res, bool res_bf16,
-                   int act2, const void *d_weights_bf16, int ldn, const float *d_bias, int wide_rows = 0, int want_ksplit = 0);
+                   int act2, const void *d_weights_bf16, int ldn, const float *d_bias, int wide_rows = 0);
 // tf32 variant for the FP32 detection heads of the exact (INT8 / XNOR) networks: f32 in, f32 [ldn][K] weights, f32 out
 int tc_tf32_supported(const Layer &l, const TV &in, const TV &out);
 void *tc_make_plan_tf32(const Layer &l, const TV &in, const TV &out, const void *d_weights_f32, int ldn, const float *d_bias,
@@ -30,12 +30,6 @@ void *tc_make_plan_xnor(const Layer &l, const TV &q, const TV &out, const void *
 int tc_plan_fuse_pool(void *plan, int mode, float mult, const TV &qnext);
 // fuse the following [yolo] layer into the (f32-output) plan: logistic + NCHW store in the epilogue
 void tc_plan_fuse_yolo(void *plan, float *d_yolo_nchw, int classes);
-// K-split of the tail wave of a bf16 plan (wave quantisation): `ws` (tc_ksplit_ws_bytes) and `flags`
-// (tc_ksplit_flag_bytes, zeroed) belong to the caller and may be shared by all plans that run on one stream.
-// Returns 1 if the plan's schedule was changed.
-size_t tc_ksplit_ws_bytes(int sms);
-size_t tc_ksplit_flag_bytes(int sms);
-int tc_plan_enable_ksplit(void *plan, float *ws, unsigned *flags);
 // tensor-core stem (3-channel 3x3 from the caller's NCHW f32 image, bf16 NHWC out)
 int tc_stem_supported(const Layer &l, const TV &out);
 void *tc_stem_make_plan(const Layer &l, const TV &out, const void *d_w_32x32_bf16, const float *d_bias);

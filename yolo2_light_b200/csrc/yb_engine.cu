@@ -77,8 +77,7 @@ struct Engine {
     bool graph_failed = false;
     std::vector<void *> tc_plans;      // opaque per-layer state of the tensor-core path (tensor maps)
     // device-side decode + NMS workspace (engine_detect), sized for det_cap rows per image
-    int n_tc = 0, n_ksplit = 0;
-    float *ksplit_ws = nullptr; unsigned *ksplit_flags = nullptr;   // partial sums / flags of the K-split tail (yb_conv_tc.cu)
+    int n_tc = 0;
     std::function<void(const float *, cudaStream_t)> first_op;   // consumes the caller's NCHW images (pointer varies per call)
     std::function<void(const unsigned char *, cudaStream_t)> first_op_u8;   // same from 8-bit HWC frames of the network size (if set)
     int first_kind = OP_INPUT, first_layer = -1;
@@ -119,8 +118,6 @@ Engine::~Engine() {
     if (det.mask) cudaFree(det.mask);
     if (det.blkcnt) cudaFree(det.blkcnt);
     if (det.counts) cudaFree(det.counts);
-    if (ksplit_ws) cudaFree(ksplit_ws);
-    if (ksplit_flags) cudaFree(ksplit_flags);
     if (d_u8) cudaFree(d_u8);
     for (Slot &sl : slots) {
         if (sl.d_u8) cudaFree(sl.d_u8);
@@ -692,23 +689,11 @@ std::shared_ptr<Engine> build_engine(Network *net, const EngineOptions &opt) {
                     const bool fuse_yolo = opt.fuse && fused_into[i] < 0 && odt == DT_F32 && i + 1 < nl &&
                                            net->layers[i + 1].type == YB_YOLO && cons[i].size() == 1 && cons[i][0] == i + 1 &&
                                            e->d_final[i + 1] && !getenv("YB_NO_YOLO_FUSE");
-                    const char *ks_env = getenv("YB_TC_KSPLIT");   // 1: on without the option (A/B runs)
-                    const bool want_ksplit = opt.ksplit || (ks_env && ks_env[0] == '1');
                     void *plan = tc_make_plan(l, tin, tout, odt == DT_BF16, res, rdt == DT_BF16, act2,
                                               e->w_arena + cw[i].w_bf16, cw[i].ldn,
-                                              reinterpret_cast<const float *>(e->w_arena + cw[i].bias), fuse_yolo ? 1 : 0,
-                                              want_ksplit ? 1 : 0);
+                                              reinterpret_cast<const float *>(e->w_arena + cw[i].bias), fuse_yolo ? 1 : 0);
                     e->tc_plans.push_back(plan);
-                    if (!e->ksplit_ws) {
-                        int sms = 132;
-                        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, opt.device);
-                        CUDA_OK(cudaMalloc(&e->ksplit_ws, tc_ksplit_ws_bytes(sms)));
-                        CUDA_OK(cudaMalloc(&e->ksplit_flags, tc_ksplit_flag_bytes(sms)));
-                        CUDA_OK(cudaMemset(e->ksplit_flags, 0, tc_ksplit_flag_bytes(sms)));
-                    }
                     ++e->n_tc;
-                    if (want_ksplit)
-                        e->n_ksplit += tc_plan_enable_ksplit(plan, e->ksplit_ws, e->ksplit_flags);
                     if (fuse_yolo) {
                         tc_plan_fuse_yolo(plan, e->d_final[i + 1], net->layers[i + 1].classes);
                         yolo_fused[i + 1] = 1;
@@ -1512,7 +1497,6 @@ int engine_num_launches(Engine *e) { return (int)e->ops.size(); }
 long engine_info(Engine *e, const char *key) {
     if (!strcmp(key, "launches")) return (long)e->ops.size();
     if (!strcmp(key, "tc_layers")) return e->n_tc;
-    if (!strcmp(key, "ksplit_layers")) return e->n_ksplit;
     return -1;
 }
 

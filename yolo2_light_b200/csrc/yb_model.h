@@ -50,8 +50,6 @@ struct Network {
     int last_launches = 0;
     bool fuse = true;          // conv+shortcut fusion / route aliasing (diagnostic switch)
     bool keep_counts = false;  // keep raw XNOR popcounts / INT8 accumulators (tests)
-    bool ksplit = false;       // K-split tail wave of the tensor-core convolutions (yb_conv_tc.cu); off by default: it makes
-                               // the f32 summation order -- hence the last bits -- depend on the batch size
     int q_index_offset = 0;    // see EngineOptions
 };
 
