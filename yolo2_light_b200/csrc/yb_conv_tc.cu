@@ -12,14 +12,13 @@
 //   * W ([filters][K] bf16, K ordered (ky, kx, c)) is the K-major B operand, loaded by TMA as well.
 //   * Two consumer warpgroups issue wgmma.mma_async (bf16 x bf16 -> f32, M=64 each, N=BN, K=16) straight from
 //     the shared-memory ring; each releases a ring stage through an mbarrier once the wgmmas reading it have retired.
-//   * bf16-output stride-1 layers (most of the FLOPs) run k_conv_tc_reg: BN <= 256, the epilogue works on the register
-//     fragments and stores bf16 slabs by TMA (see there).
+//   * bf16-output layers, stride 1 and 2 (all but the detection heads), run k_conv_tc_reg: BN <= 256, the epilogue works
+//     on the register fragments, adds the shortcut residual when fused (reference :443-449), and stores bf16 slabs by
+//     TMA (see there).
 //   * Everything else runs k_conv_tc (BN <= 128): at the end of a tile the register accumulators go to a padded
-//     [128][BN+4] shared-memory tile, and the same 8
-//     warps run the epilogue from it with one pixel row per thread: add bias (folded batch-norm), apply leaky-ReLU,
-//     add the shortcut residual when fused (reference :443-449), and store bf16 NHWC through a swizzled staging tile
-//     (whole 128-byte lines; the stride-2 layers), or f32 for detection heads -- optionally with the following [yolo]
-//     layer applied (:453-472).  The producer warp keeps loading the next tile's stages meanwhile.
+//     [128][BN+4] shared-memory tile, and the same 8 warps run the epilogue from it with one pixel row per thread: add
+//     bias (folded batch-norm), apply leaky-ReLU and store f32 for detection heads -- optionally with the following
+//     [yolo] layer applied (:453-472).  The producer warp keeps loading the next tile's stages meanwhile.
 //   * The same kernel runs the INT8 variant (s8 x s8 -> s32 wgmma, exact requantising epilogue,
 //     yolov2_forward_network_quantized.c:474-490), wide XNOR layers as +-1 bytes on the s8 wgmma, and the float heads
 //     of the exact networks on tf32 wgmma.
@@ -94,8 +93,8 @@ struct TcParams {
     int sps;                                  // K-blocks per pipeline stage (amortises the per-stage barrier round trip)
     int kbs;                                  // pipeline stages per work item = ceil(kblocks / sps)
     uint32_t desc_hi;         // high word of the wgmma shared-memory descriptors (SBO, swizzle mode)
-    char *out; long out_ldc; int out_bf16; int n, n_store;
-    const char *res; long res_ldc; int res_bf16;   // fused shortcut operand (bf16, bf16 outputs only), or null
+    char *out; long out_ldc; int n, n_store;
+    const char *res;          // fused shortcut operand (bf16, k_conv_tc_reg at stride 1 only), or null
     const float *bias; int act, act2;
     unsigned long long *stats; // YB_TC_STATS=1: per-CTA cycle counters [grid][16] (diagnostic)
     int dbg;                  // YB_TC_DBG bit mask for bottleneck experiments: 1 no TMA, 2 no MMA, 4 no epilogue memory ops
@@ -455,8 +454,8 @@ __device__ __forceinline__ float int_epilogue(const TcParams &p, int kind, int a
 // One CTA per 128-pixel x BN-filter tile, persistent over the tiles (grid <= #SMs, one CTA per SM).
 // ST: compiled with the per-role cycle counters of YB_TC_STATS=1 (diagnostic); the production instantiations (ST = false)
 // contain no clock64() reads.
-// EPI: which epilogue family is compiled in -- 0: LSU stores, float kinds (bf16 / f32 heads / fused [yolo]); 2: the integer
-// kinds (s8 requantising and XNOR-as-+-1 epilogues).  The bf16 stride-1 layers run k_conv_tc_reg.
+// EPI: which epilogue family is compiled in -- 0: LSU stores, float kinds (f32 heads / fused [yolo]); 2: the integer
+// kinds (s8 requantising and XNOR-as-+-1 epilogues).  The bf16-output layers run k_conv_tc_reg.
 template <bool ST, int EPI>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
@@ -563,8 +562,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
             const int oy = J - img * p.PR - p.row_off;
             const bool valid = (img < p.N) && (oy >= 0) && (oy < p.OH) && (ox < p.OW) && !(p.dbg & 4);
             const long pix = ((long)(img * p.OHp + oy + 1) * p.OWp + ox + 1);
-            char *orow = p.out + pix * p.out_ldc * (p.out_bf16 ? 2 : 4);
-            const char *rrow = (p.res && valid) ? p.res + pix * p.res_ldc * 2 : nullptr;
+            char *orow = p.out + pix * p.out_ldc * 4;
             const float *bs = bias_s + n0;
 
             // ---- f32 output (detection heads) of one 32-column slab, one row per thread
@@ -695,88 +693,6 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                 }
             };
 
-            // ---- bf16 output (the stride-2 layers) in slabs of SW = 64 or 32 columns: every global access of this warp is a
-            // run of whole 2 * SW-byte rows.  Each warp owns 32 accumulator rows; they are transposed through the warp's private
-            // staging tile (16-byte chunk c of row r at r * 2 SW + ((c ^ swizzle(r)) << 4)) so that one warp instruction moves
-            // 4 rows x 128 B (SW = 64) or 8 rows x 64 B (SW = 32) instead of 32 rows x 16 B (the latter costs 32 LSU cycles per
-            // instruction and made the epilogue the bottleneck of every layer).  The shortcut residual comes in the same way.
-            auto bf16_slabs = [&](auto sw_c) {
-                constexpr int SW = decltype(sw_c)::value;
-                constexpr int CH = SW / 8, RPI = 32 / CH;   // 16-byte chunks per row, rows per warp instruction
-                const uint32_t stg = stg_base + (uint32_t)ew * 4096u;
-                const int srow = lane / CH, schunk = lane % CH;
-                const unsigned long long obase = (unsigned long long)(uintptr_t)orow;
-                const unsigned long long rbase = (unsigned long long)(uintptr_t)rrow;
-                const int vflag = valid ? 1 : 0;
-                auto stage_addr = [&](int row, int chunk) {
-                    const int sw = (SW == 64) ? (row & 7) : ((row >> 1) & 3);
-                    return stg + (uint32_t)row * (2u * SW) + (uint32_t)((chunk ^ sw) << 4);
-                };
-                auto res_to_stage = [&](int f0) {     // coalesced global -> staging
-#pragma unroll
-                    for (int i = 0; i < CH; ++i) {
-                        const int row = i * RPI + srow;
-                        const unsigned long long rp = __shfl_sync(0xffffffffu, rbase, row);
-                        uint4 v = make_uint4(0u, 0u, 0u, 0u);
-                        if (rp && (n0 + f0 + schunk * 8) < p.n_store)
-                            v = __ldg(reinterpret_cast<const uint4 *>(rp + (size_t)(n0 + f0) * 2) + schunk);
-                        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(stage_addr(row, schunk)), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-                    }
-                };
-                if (p.res) res_to_stage(cbeg);
-                for (int f0 = cbeg; f0 < cend; f0 += SW) {
-                    uint32_t v[SW / 32][32];
-#pragma unroll
-                    for (int h = 0; h < SW / 32; ++h) acc_ld32(taddr + 4u * (uint32_t)(f0 + 32 * h), v[h]);
-                    float x[SW];
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-#pragma unroll
-                        for (int h = 0; h < SW / 32; ++h) {
-                            const float a = __uint_as_float(v[h][j]) + bs[f0 + 32 * h + j];
-                            x[32 * h + j] = leaky ? fmaxf(a, 0.1f * a) : a;
-                        }
-                    }
-                    if (p.res) {
-                        __syncwarp();
-#pragma unroll
-                        for (int c = 0; c < CH; ++c) {          // own row back from staging
-                            uint32_t w0, w1, w2, w3;
-                            asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(w0), "=r"(w1), "=r"(w2), "=r"(w3) : "r"(stage_addr(lane, c)) : "memory");
-                            const uint32_t wv[4] = {w0, w1, w2, w3};
-#pragma unroll
-                            for (int h = 0; h < 4; ++h) {
-                                x[c * 8 + 2 * h] += __uint_as_float(wv[h] << 16);
-                                x[c * 8 + 2 * h + 1] += __uint_as_float(wv[h] & 0xffff0000u);
-                            }
-                        }
-                        if (leaky2) {
-#pragma unroll
-                            for (int j = 0; j < SW; ++j) x[j] = fmaxf(x[j], 0.1f * x[j]);
-                        }
-                        __syncwarp();
-                    }
-#pragma unroll
-                    for (int c = 0; c < CH; ++c)                // own row -> staging
-                        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(stage_addr(lane, c)),
-                                     "r"(pack_bf16x2(x[c * 8 + 0], x[c * 8 + 1])), "r"(pack_bf16x2(x[c * 8 + 2], x[c * 8 + 3])),
-                                     "r"(pack_bf16x2(x[c * 8 + 4], x[c * 8 + 5])), "r"(pack_bf16x2(x[c * 8 + 6], x[c * 8 + 7])) : "memory");
-                    __syncwarp();
-#pragma unroll
-                    for (int i = 0; i < CH; ++i) {              // staging -> coalesced global
-                        const int row = i * RPI + srow;
-                        const unsigned long long op = __shfl_sync(0xffffffffu, obase, row);
-                        const int ok = __shfl_sync(0xffffffffu, vflag, row);
-                        uint32_t w0, w1, w2, w3;
-                        asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(w0), "=r"(w1), "=r"(w2), "=r"(w3) : "r"(stage_addr(row, schunk)) : "memory");
-                        if (ok && (n0 + f0 + schunk * 8) < p.n_store)
-                            *(reinterpret_cast<uint4 *>(op + (size_t)(n0 + f0) * 2) + schunk) = make_uint4(w0, w1, w2, w3);
-                    }
-                    __syncwarp();
-                    if (p.res && f0 + SW < cend) res_to_stage(f0 + SW);   // next slab's residual in flight
-                }
-            };
-
             if constexpr (EPI == 2) {
                 // ---- integer kinds: the exact float epilogue per 32-column slab (or the fused max-pool), f32 stores
                 auto int_slabs = [&](auto kind_c) {
@@ -801,9 +717,6 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                 };
                 if (p.kind == 2) int_slabs(std::integral_constant<int, 2>{});
                 else int_slabs(std::integral_constant<int, 1>{});
-            } else if (p.out_bf16) {
-                if (cend - cbeg >= 64) bf16_slabs(std::integral_constant<int, 64>{});
-                else if (cend > cbeg) bf16_slabs(std::integral_constant<int, 32>{});
             } else {
                 for (int f0 = cbeg; f0 < cend; f0 += 64) {
                     if (cend - f0 >= 64) {
@@ -826,7 +739,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
     }
 }
 
-// Register-accumulator kernel of the bf16-output, stride-1 layers (384 threads).  Warpgroups 0 and 1 are consumers with up to 216
+// Register-accumulator kernel of the bf16-output layers, stride 1 and 2 (384 threads).  Warpgroups 0 and 1 are consumers with up to 216
 // registers each: a consumer warpgroup keeps the f32 accumulators of its 64 rows x BN (<= 256) filters of the tile in registers
 // and runs the epilogue straight on its wgmma fragment -- bias, leaky, the fused shortcut residual and the second leaky in fp32,
 // then round to bf16.  Warpgroup 2 gives its registers away with setmaxnreg: warp 8 is the TMA producer, warps 9 and 10 are the
@@ -843,6 +756,17 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
 //   stg_ready[g]   -- the store thread's arrival (expect_tx = the residual bytes): the buffer is free and holds the residual.
 // A consumer goes from its epilogue straight into the next main loop: no named barrier and no TMA call in the consumers, and the
 // two warpgroups never wait for each other.
+//
+// Stride 2: tile row J (a merged half row of the input, J = image * (OH + 1) + oy) goes to output merged padded row J + image + 1,
+// which is affine only within one image.  A half tile inside one image is stored as one box; its rows with oy == OH (not an output
+// row) land on that image's bottom border, and the epilogue writes them as zeros.  A half tile that straddles two images goes out
+// one tile row at a time through tmO1 (box: SW channels x TW pixels x 1 row), skipping the rows with oy == OH and those past the
+// batch: no store touches an image's top border or needs a negative row (bulk tensor stores fault on negative coordinates).
+// Tile row t of a slab starts at byte t * TW * 2 SW.  Bulk tensor copies need 128-byte aligned shared memory (make_plan_common
+// keeps TW * SW >= 64), and the TMA engine takes the swizzle phase from the shared-memory address (16-byte chunk c of the
+// 128-byte row at address a is chunk c ^ ((a >> 7) & 7) at 128B, c ^ ((a >> 7) & 3) at 64B), the rule slab_off follows from
+// the 1024-byte aligned buffer: a row box that starts off the swizzle's 1024 / 512-byte repeat reads its rows as written.
+// Stride-2 plans have no fused residual.
 constexpr int TCR_THREADS = 384;
 constexpr int TCR_PRODUCER_REGS = 40, TCR_CONSUMER_REGS = 216;   // 128 * 40 + 256 * 216 <= 64 K registers
 constexpr int TCR_STORE_WARP = 9;                                // store warps 9 (consumer warpgroup 0) and 10 (warpgroup 1)
@@ -852,18 +776,35 @@ constexpr int TCR_MAX_SLABS = 4;                                 // BN / SW <= 2
 // stg_full: its first per-slab barrier.  ST: cycles spent waiting on stg_full and in cp.async.bulk.wait_group.read go to stats
 // slots 4 and 5 (warpgroup 0's thread).
 template <bool ST>
-__device__ __forceinline__ void tcr_store(const CUtensorMap *tmO, const CUtensorMap *tmR, const TcParams &p, uint32_t buf,
-                                          uint32_t stg_full, uint32_t stg_ready, int g, int w_first, int w_step) {
+__device__ __forceinline__ void tcr_store(const CUtensorMap *tmO, const CUtensorMap *tmO1, const CUtensorMap *tmR, const TcParams &p,
+                                          uint32_t buf, uint32_t stg_full, uint32_t stg_ready, int g, int w_first, int w_step) {
     const int SW = p.tma_epi, BN = p.BN;
     const uint32_t tile = 64u * 2u * (uint32_t)SW;                  // one slab: 64 pixel rows x SW bf16
     // the half tile as a TMA box: 64 of the TW x TH pixels (TW == 128: one half row; else TH / 2 whole rows)
     const int hx = (p.TW == 128) ? 64 * g : 0, hy = (p.TW == 128) ? 0 : g * (p.TH >> 1);
     long long w_full = 0, w_read = 0;
-    // box origin of work item w's half tile (first filter, padded x, merged padded row); returns its slabs holding filters < n
+    // box origin of work item w's half tile (first filter, padded x, merged padded output row); returns its slabs holding
+    // filters < n.  Stride 1: tile rows are the output's padded rows.  Stride 2: y = J0 + image + 1 for a half tile inside one
+    // image (rows past the batch fall outside the tensor), y = -1 - J0 for one that straddles two images (stored row by row;
+    // J0: merged row of its first tile row).
     auto item = [&](int w, int &n0, int &x, int &y) {
         const int m = w / p.nt;
         n0 = (w % p.nt) * BN; x = (m % p.xt) * p.TW + 1 + hx; y = (m / p.xt) * p.TH + p.jshift + hy;
+        if (p.stride2) {
+            const int i0 = y / p.PR, i1 = min((y + max(p.TH >> 1, 1) - 1) / p.PR, p.N - 1);
+            y = i0 == i1 ? y + i0 + 1 : -1 - y;
+        }
         return (min(BN, p.n - n0) + SW - 1) / SW;
+    };
+    auto store_slab = [&](uint32_t src, int c, int x, int y) {
+        if (y >= 0) { tma_store_3d(tmO, src, c, x, y); return; }
+        const int J0 = -1 - y;
+        int img = J0 / p.PR, oy = J0 - img * p.PR;
+        for (int t = 0; t < (p.TH >> 1); ++t) {   // TW <= 32 here: the half tile is TH / 2 rows of TW pixels
+            if (img < p.N && oy < p.OH) tma_store_3d(tmO1, src, c, x, J0 + t + img + 1);
+            if (++oy == p.PR) { oy = 0; ++img; }
+            src += (uint32_t)(p.TW * 2 * SW);
+        }
     };
     auto wait_read = [&]() {   // the bulk stores issued so far have read shared memory
         if constexpr (ST) { const long long c0 = clock64(); tma_store_wait_read0(); w_read += clock64() - c0; }
@@ -897,7 +838,7 @@ __device__ __forceinline__ void tcr_store(const CUtensorMap *tmO, const CUtensor
             phases ^= 1u << s;
             // the consumers are past this item's stg_ready: its phase is complete and the next item's may begin
             if (s == 0 && res_next) mbar_arrive_expect_tx(stg_ready, (uint32_t)nsn * tile);
-            tma_store_3d(tmO, buf + (uint32_t)s * tile, n0 + s * SW, x, y);
+            store_slab(buf + (uint32_t)s * tile, n0 + s * SW, x, y);
             tma_store_commit();
             if (res_next && s < nsn) { wait_read(); load_res(s, n0n, xn, yn); }
         }
@@ -915,7 +856,7 @@ __device__ __forceinline__ void tcr_store(const CUtensorMap *tmO, const CUtensor
 template <bool ST>
 __global__ void __launch_bounds__(TCR_THREADS, 1)
 k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
-              const __grid_constant__ CUtensorMap tmR, const TcParams p) {
+              const __grid_constant__ CUtensorMap tmO1, const __grid_constant__ CUtensorMap tmR, const TcParams p) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smemB = (smem_u32(smem_raw) + 1023u) & ~1023u;   // [resident filter matrix][pipeline ring][barriers][bias][staging]
     const uint32_t smem0 = smemB + p.bstat_bytes;
@@ -939,6 +880,7 @@ k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmO) : "memory");
+        if (p.stride2) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmO1) : "memory");
         if (p.res) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmR) : "memory");
         for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar(bars, s), 1); mbar_init(empty_bar(bars, p.stages, s), TC_EPI_WARPS); }
         mbar_init(bstat_bar, 1);
@@ -960,7 +902,7 @@ k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
             if (elect_one()) tc_produce<ST>(&tmA, &tmB, p, smemB, smem0, bars, w_first, w_step);
         } else if (warp < TCR_STORE_WARP + 2 && epi_mem) {
             const int g = warp - TCR_STORE_WARP;
-            if (elect_one()) tcr_store<ST>(&tmO, &tmR, p, stg_base + (uint32_t)g * 128u * (uint32_t)p.BN, stg_full(g, 0), stg_ready(g), g, w_first, w_step);
+            if (elect_one()) tcr_store<ST>(&tmO, &tmO1, &tmR, p, stg_base + (uint32_t)g * 128u * (uint32_t)p.BN, stg_full(g, 0), stg_ready(g), g, w_first, w_step);
         }
         return;
     }
@@ -1275,7 +1217,7 @@ EncodeTiledFn encode_fn() {
 }
 
 struct TcPlan {
-    CUtensorMap tmA, tmB, tmO, tmR;   // activation, filters; TMA epilogue: output, residual
+    CUtensorMap tmA, tmB, tmO, tmO1, tmR;   // activation, filters; TMA epilogue: output, its one-row view (stride 2), residual
     TcParams p;
     int grid;
     int threads;                      // TC_THREADS (k_conv_tc) or TCR_THREADS (k_conv_tc_reg)
@@ -1345,11 +1287,8 @@ static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &
     const int esz = kind == 3 ? 4 : i8 ? 1 : 2;              // operand element size
     const int cin = i8 ? in.ldc : l.c;                       // s8: channels padded with zeros in both operands
     const int BK = kind == 3 ? pick_bk_f32(l.c) : i8 ? pick_bk_i8(cin) : pick_bk(l.c);
-    // bf16 NHWC output of a stride-1 layer: the register-accumulator kernel with its TMA epilogue
-    // (stride-2 layers keep the LSU epilogue: their tiles walk the input's merged half-rows, OH + 1 per image, while the output has
-    // OH + 2 rows per image -- a per-image (c, x, y, image) store would need a negative start row for the second image of a
-    // straddling tile, and bulk tensor STORES fault on negative coordinates)
-    const bool reg = kind == 0 && out_bf16 && l.stride == 1;
+    // bf16 NHWC output: the register-accumulator kernel with its TMA epilogue
+    const bool reg = kind == 0 && out_bf16;
     p.kind = kind; p.alpha1 = alpha1; p.acc_out = acc_out;
     p.kk = BK * esz / 32;
     const bool s2 = l.stride == 2;
@@ -1391,6 +1330,13 @@ static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &
     p.xt = (p.OW + p.TW - 1) / p.TW;
     p.jt = (int)((rows - p.jshift + p.TH - 1) / p.TH);
     const int BN = reg ? pick_bn_reg(l.n, (long)p.xt * p.jt, p.kblocks, sms) : pick_bn(l.n);
+    if (reg && s2 && BN == 32 && p.TW == 1) {
+        // k_conv_tc_reg stores straddling stride-2 half tiles one tile row at a time, from byte t * TW * 2 SW of a slab: with
+        // 64-byte slab rows (SW = 32) and TW = 1 that is not 128-byte aligned, as bulk tensor copies need
+        p.TW = 2; p.TH = 64; p.TWlog2 = 1;
+        p.xt = (p.OW + p.TW - 1) / p.TW;
+        p.jt = (int)((rows - p.jshift + p.TH - 1) / p.TH);
+    }
     p.BN = BN;
     p.nt = (l.n + BN - 1) / BN;
     p.num_work = p.xt * p.jt * p.nt;
@@ -1430,14 +1376,16 @@ static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &
     // wgmma descriptor high word: SBO (8 rows * row bytes) >> 4 at bits 32..45, swizzle mode at 62..63 (1: 128B, 2: 64B, 3: 32B)
     const uint32_t layout_type = row_bytes == 128 ? 1u : row_bytes == 64 ? 2u : 3u;
     p.desc_hi = ((8u * row_bytes) >> 4) | (layout_type << 30);
-    p.out = out.base; p.out_ldc = out.ldc; p.out_bf16 = out_bf16 ? 1 : 0;
+    p.out = out.base; p.out_ldc = out.ldc;
     p.n = l.n;
     p.n_store = out_bf16 ? l.n : std::min<int>((l.n + 3) / 4 * 4, out.ldc);
     if (!out_bf16 && (out.ldc % 4 != 0)) fatal_throw("tc plan: f32 output rows must be 16-byte aligned");
-    p.res = res.base; p.res_ldc = res.ldc; p.res_bf16 = res_bf16 ? 1 : 0;
+    p.res = res.base;
     if (res.base && (res.H != l.out_h || res.W != l.out_w || res.C != l.n)) fatal_throw("tc plan: residual shape mismatch");
     if (res.base && !res_bf16) fatal_throw("tc plan: residual must be bf16");
     if (res.base && !out_bf16) fatal_throw("tc plan: a fused residual needs a bf16 output");
+    if (res.base && s2) fatal_throw("tc plan: a fused residual needs a stride-1 layer");
+    if (reg && s2 && out.P != 1) fatal_throw("tc plan: a stride-2 output needs a border of 1");
     if (res.base && res_bf16 && (res.ldc % 8 != 0 || (reinterpret_cast<uintptr_t>(res.base) & 15))) fatal_throw("tc plan: residual alignment");
     p.bias = d_bias; p.act = l.activation; p.act2 = act2;
     p.dbg = getenv("YB_TC_DBG") ? atoi(getenv("YB_TC_DBG")) : 0;
@@ -1479,25 +1427,25 @@ static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &
                 CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) { delete plan; fatal_throw("cuTensorMapEncodeTiled(B) failed: " + std::to_string((int)r)); }
     }
-    plan->tmO = plan->tmA; plan->tmR = plan->tmA;   // valid placeholders when the TMA epilogue is off
+    plan->tmO = plan->tmA; plan->tmO1 = plan->tmA; plan->tmR = plan->tmA;   // valid placeholders when unused
     if (p.tma_epi) {
         const int oesz = out_bf16 ? 2 : 4;
-        auto encode_px = [&](CUtensorMap *tm, const TV &t, const char *what) {
+        auto encode_px = [&](CUtensorMap *tm, const TV &t, const char *what, int box_rows) {
             // (channels, padded x, merged padded rows) of a padded-NHWC tensor (bf16, or f32 for the integer kinds); box = one
-            // slab of a pixel tile
+            // slab of a pixel tile (k_conv_tc_reg: half a tile, the 64 pixels of one consumer warpgroup), box_rows rows of it
             cuuint64_t dims[3] = {(cuuint64_t)l.n, (cuuint64_t)t.Wp, (cuuint64_t)t.N * t.Hp};
             cuuint64_t strides[2] = {(cuuint64_t)t.ldc * oesz, (cuuint64_t)t.Wp * t.ldc * oesz};
-            // (k_conv_tc_reg: half a tile, the 64 pixels of one consumer warpgroup)
-            cuuint32_t box[3] = {(cuuint32_t)p.tma_epi, (cuuint32_t)std::min(p.TW, reg ? 64 : 128),
-                                 (cuuint32_t)(reg ? std::max(p.TH / 2, 1) : p.TH)};
+            cuuint32_t box[3] = {(cuuint32_t)p.tma_epi, (cuuint32_t)std::min(p.TW, reg ? 64 : 128), (cuuint32_t)box_rows};
             cuuint32_t es[3] = {1, 1, 1};
             CUresult rr = enc(tm, out_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, t.base, dims, strides, box, es,
                               CU_TENSOR_MAP_INTERLEAVE_NONE, p.tma_epi * oesz == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
                               CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
             if (rr != CUDA_SUCCESS) { delete plan; fatal_throw(std::string("cuTensorMapEncodeTiled(") + what + ") failed: " + std::to_string((int)rr)); }
         };
-        encode_px(&plan->tmO, out, "output");
-        if (res.base && out_bf16) encode_px(&plan->tmR, res, "residual");
+        const int box_rows = reg ? std::max(p.TH / 2, 1) : p.TH;
+        encode_px(&plan->tmO, out, "output", box_rows);
+        if (reg && s2) encode_px(&plan->tmO1, out, "output row", 1);   // straddling half tiles, one tile row per store
+        if (res.base && out_bf16) encode_px(&plan->tmR, res, "residual", box_rows);
     }
     plan->pdl = (getenv("YB_NO_PDL") == nullptr) ? 1 : 0;
     plan->grid = std::min(p.num_work, grid_cap(sms));
@@ -1648,7 +1596,10 @@ void tc_launch(void *vp, cudaStream_t s) {
     const bool st = plan->p.stats != nullptr;   // role counters: a separate instantiation (YB_TC_STATS=1)
     const TcPlan &P = *plan;
 #define YB_TC_LAUNCH(KERNEL) cudaLaunchKernelEx(&cfg, KERNEL, P.tmA, P.tmB, P.tmO, P.tmR, P.p)
-    if (plan->threads == TCR_THREADS) { if (st) YB_TC_LAUNCH(k_conv_tc_reg<true>); else YB_TC_LAUNCH(k_conv_tc_reg<false>); }
+    if (plan->threads == TCR_THREADS) {
+        if (st) cudaLaunchKernelEx(&cfg, k_conv_tc_reg<true>, P.tmA, P.tmB, P.tmO, P.tmO1, P.tmR, P.p);
+        else cudaLaunchKernelEx(&cfg, k_conv_tc_reg<false>, P.tmA, P.tmB, P.tmO, P.tmO1, P.tmR, P.p);
+    }
     else if (P.p.kind == 1 || P.p.kind == 2) { if (st) YB_TC_LAUNCH((k_conv_tc<true, 2>)); else YB_TC_LAUNCH((k_conv_tc<false, 2>)); }
     else { if (st) YB_TC_LAUNCH((k_conv_tc<true, 0>)); else YB_TC_LAUNCH((k_conv_tc<false, 0>)); }
 #undef YB_TC_LAUNCH

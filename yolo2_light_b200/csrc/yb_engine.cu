@@ -267,6 +267,7 @@ std::shared_ptr<Engine> build_engine(Network *net, const EngineOptions &opt) {
             const Layer &l = net->layers[i], &s = net->layers[i + 1];
             if (l.type != YB_CONVOLUTIONAL || s.type != YB_SHORTCUT) continue;
             if (conv_variant(i) != 0) continue;
+            if (l.stride != 1) continue;   // the tensor-core stride-2 path stores straddling tiles row by row, without a residual
             if (cons[i].size() != 1 || cons[i][0] != i + 1) continue;
             if (s.index == i) continue;
             if (!(s.w == s.out_w && s.h == s.out_h && s.c == s.out_c)) continue;
