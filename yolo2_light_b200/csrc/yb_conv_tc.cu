@@ -1029,13 +1029,17 @@ k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
 // ------------------------------------------------------------------------------------------------------
 struct StemTcP {
     const float *in;          // NCHW f32, set per call
-    const unsigned char *in8; // or: HWC 8-bit frames of exactly the network size (k_stem_tc<true>), set per call
-    char *out; int out_ldc;   // bf16 padded NHWC
+    const unsigned char *in8; // or: HWC 8-bit frames of exactly the network size (U8 instantiations), set per call
+    char *out; int out_ldc;   // bf16 padded NHWC (k_stem_s2_tc: layer 1's output)
     const __nv_bfloat16 *w;   // [32 rows (filters, zero padded)][32 k] bf16, k = (ky,kx,c), k >= 27 zero
     const float *bias;
     int N, H, W, OHp, OWp, nf, act;
     long npix;
     int ntiles;
+    // k_stem_s2_tc only: layer 1 (3x3 / stride 2 / pad 1, 32 -> 64 filters) and its tiling
+    const __nv_bfloat16 *w1;  // [64 filters][9 * 32] bf16, K ordered (ky, kx, c)
+    const float *bias1;
+    int act1, OH, OW, xt, yt;
 };
 
 // U8: the input is the caller's 8-bit HWC frame (already of the network size): value = (float)((double)v / 255.0) exactly as
@@ -1194,6 +1198,244 @@ __global__ void __launch_bounds__(128) k_stem_tc(StemTcP p) {
             }
         }
         __syncthreads();   // accumulator row drained and A tile consumed before the next tile overwrites them
+    }
+}
+
+// ------------------------------------------------------------------------------------------------------
+// The tensor-core stem fused with the 3x3 / stride-2 / pad-1 convolution that reads it (32 -> 64 filters): the stem output
+// (378 MB in bf16 for yolov3 at 608^2, batch 16) stays in shared memory, HBM sees the image and layer 1's output only.
+// Work item: a 16 x 8 tile of layer-1 output pixels of one image, all 64 filters.  Per tile:
+//   1. The tile's image patch (3 x 19 x 35 values, f32 or 8-bit through the same table as k_stem_tc, zeros outside the image)
+//      is loaded into registers while the previous tile's layer 1 runs and stored to shared memory; from it, the im2col rows of the 17 x 33 stem pixels the tile
+//      reads (2 * 8 + 1 rows, 2 * 16 + 1 columns, pad 1 included), k_stem_tc's A operand with no bounds logic.  561 rows padded
+//      to 640 = 10 M=64 chunks.
+//   2. stem wgmmas: warpgroup g takes chunks 5 g .. 5 g + 4, two m64n32k16 each, as k_stem_tc does; then bias, leaky and
+//      bf16, k_stem_tc's arithmetic: the stem values are bit-identical.  Stem pixels outside the image are layer 1's zero pad
+//      and are written as zeros.
+//   3. Layer 1 reads those values from "sets": 16 rows of 64 bytes (1 KB), row ox = stem pixel (sy, 2 ox + kx), one set per
+//      stem row sy and column phase kx (odd region columns sit in two sets).  Per kx: the 9 even rows' sets, then the 8 odd
+//      ones, so that tap (ky, kx) of the 128 tile pixels (oy, ox) -> stem (2 oy + ky, 2 ox + kx) is one canonical 128-row
+//      K-major matrix (64B swizzle) starting at set ky / 2 of parity ky & 1; warpgroup g's 64 rows start 4 sets further.  Every
+//      operand base is 1 KB aligned: plain descriptors, no gather, no bank conflicts.  Layer 1 then runs k_conv_tc_reg's
+//      instruction sequence at BN = 64 (filter matrix resident in shared memory, taps in (ky, kx) order, two m64n64k16 per
+//      tap) and its epilogue (bias, leaky, bf16): bit-identical to the unfused layer.
+//   4. The accumulators go through a swizzled staging tile (8 KB per warpgroup) to 16-byte coalesced stores into layer 1's
+//      padded NHWC output; pixels past OW / OH are not stored, the zero border is never written.
+// Shared memory: the im2col rows, the sets and the staging tiles share one region (their lifetimes are separated by the
+// block barriers), ~104 KB per CTA in all: two CTAs per SM, so that one CTA's patch loads and stores overlap the other's
+// wgmmas.  Persistent grid of 2 CTAs per SM (YB_TC_GRID caps it).
+// ------------------------------------------------------------------------------------------------------
+constexpr int S2_TW = 16, S2_TH = 8;                           // layer-1 output pixels per tile
+constexpr int S2_RW = 2 * S2_TW + 1, S2_RH = 2 * S2_TH + 1;    // stem region of a tile: 33 x 17
+constexpr int S2_ROWS = 640;                                   // 561 stem pixels padded to 10 chunks of 64
+constexpr uint32_t S2_B1 = 0;                                  // layer-1 filters: 9 taps x [64 filters][64 B]
+constexpr uint32_t S2_BS = 9u * 4096u;                         // stem filters: [32][64 B]
+constexpr uint32_t S2_U = S2_BS + 2048u;                       // im2col rows | sets | staging
+constexpr uint32_t S2_SETS_KX = 17u * 1024u;                   // per kx: 9 even-row sets, then 8 odd-row sets
+constexpr uint32_t S2_STG = (uint32_t)S2_ROWS * 64u;           // staging tiles (in U), past the im2col rows
+constexpr uint32_t S2_MISC = S2_U + S2_STG + 2u * 8192u;       // biases (32 + 64 floats), u8 table (256 floats), image patch
+constexpr int S2_PH = S2_RH + 2, S2_PW = S2_RW + 2, S2_PP = 36; // image patch of a tile: 3 x 19 x 35 f32, rows of 36
+constexpr size_t S2_SMEM = 1024 + S2_MISC + 4 * (32 + 64 + 256) + 4 * 3 * S2_PH * S2_PP;
+static_assert(S2_STG + 2u * 8192u >= 3u * S2_SETS_KX, "sets must fit the shared region");
+
+template <bool U8>
+__global__ void __launch_bounds__(256, 2) k_stem_s2_tc(StemTcP p) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t *sm = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // 64B swizzle atoms: 512-byte aligned
+    const uint32_t base = smem_u32(sm), U = base + S2_U;
+    float *bias0_s = reinterpret_cast<float *>(sm + S2_MISC), *bias1_s = bias0_s + 32, *lut = bias1_s + 64, *patch = lut + 256;
+    const int t = threadIdx.x, lane = t & 31;
+    const int warp = __shfl_sync(0xffffffffu, t >> 5, 0), wg = warp >> 2;
+    if constexpr (U8) lut[t] = (float)((double)(float)t / 255.0);
+    if (t < 32) bias0_s[t] = p.bias[t];
+    if (t < 64) bias1_s[t] = p.bias1[t];
+    if (t < 128) {   // stem filters, swizzled as in k_stem_tc
+        const int f = t >> 2, j = t & 3;
+        *reinterpret_cast<uint4 *>(sm + S2_BS + f * 64 + ((j ^ ((f >> 1) & 3)) << 4)) = *reinterpret_cast<const uint4 *>(p.w + f * 32 + j * 8);
+    }
+    for (int i = t; i < 9 * 64 * 4; i += 256) {   // layer-1 filters: tap r, filter f, 16-byte chunk j (the TMA box layout of k_conv_tc_reg)
+        const int r = i >> 8, f = (i >> 2) & 63, j = i & 3;
+        *reinterpret_cast<uint4 *>(sm + S2_B1 + r * 4096 + f * 64 + ((j ^ ((f >> 1) & 3)) << 4)) =
+            *reinterpret_cast<const uint4 *>(p.w1 + f * 288 + r * 32 + j * 8);
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+
+    const uint32_t hi = ((8u * 64u) >> 4) | (2u << 30);   // K-major, 64-byte rows, 64B swizzle, SBO = 8 rows * 64 B
+    const bool leaky0 = p.act == ACT_LEAKY, leaky1 = p.act1 == ACT_LEAKY;
+    const int rl = 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);   // wgmma fragment: rows rl, rl + 8; columns 8 j + cq, + 1
+    // The image patch of a tile (zeros outside the image): each thread loads PER values into registers, all issued back to
+    // back, and stores them into `patch` later -- the next tile's loads are in flight while this tile's layer 1 runs.
+    constexpr int PER = (3 * S2_PH * S2_PW + 255) / 256;
+    auto patch_index = [&](int e, int &c, int &r, int &col) {
+        if constexpr (U8) { r = e / (3 * S2_PW); const int b = e - r * 3 * S2_PW; col = b / 3; c = b - col * 3; }
+        else { c = e / (S2_PH * S2_PW); const int b = e - c * S2_PH * S2_PW; r = b / S2_PW; col = b - r * S2_PW; }
+    };
+    auto load_patch = [&](int tile, float (&v)[PER]) {
+        const int tx = tile % p.xt, rest = tile / p.xt, ty = rest % p.yt, n = rest / p.yt;
+        const int py0 = 2 * ty * S2_TH - 2, px0 = 2 * tx * S2_TW - 2;   // image pixel of patch (0, 0)
+        const size_t img = (size_t)n * 3 * p.H * p.W;   // first value of image n (both layouts); offsets in it fit 32 bits
+#pragma unroll
+        for (int k = 0; k < PER; ++k) {
+            const int e = t + 256 * k;
+            int c, r, col;
+            patch_index(e, c, r, col);
+            const int y = py0 + r, x = px0 + col;
+            const bool in_img = e < 3 * S2_PH * S2_PW && y >= 0 && y < p.H && x >= 0 && x < p.W;
+            if constexpr (U8) v[k] = in_img ? lut[__ldg(p.in8 + img + (unsigned)((y * p.W + x) * 3 + c))] : 0.f;
+            else v[k] = in_img ? __ldg(p.in + img + (unsigned)((c * p.H + y) * p.W + x)) : 0.f;
+        }
+    };
+    float pv[PER];
+    if ((int)blockIdx.x < p.ntiles) load_patch(blockIdx.x, pv);
+    for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
+        const int tx = tile % p.xt, rest = tile / p.xt, ty = rest % p.yt, n = rest / p.yt;
+        const int ox0 = tx * S2_TW, oy0 = ty * S2_TH;
+        const int gy0 = 2 * oy0 - 1, gx0 = 2 * ox0 - 1;   // stem pixel of region (0, 0)
+
+        // ---- 1. the image patch -> shared memory (the previous tile's im2col, which read it, is behind two block barriers)
+#pragma unroll
+        for (int k = 0; k < PER; ++k) {
+            const int e = t + 256 * k;
+            if (e >= 3 * S2_PH * S2_PW) break;
+            int c, r, col;
+            patch_index(e, c, r, col);
+            patch[(c * S2_PH + r) * S2_PP + col] = pv[k];
+        }
+        __syncthreads();
+
+        // ---- stem im2col rows, i = sy * 33 + sx: k_stem_tc's window (k = (ky*3 + kx)*3 + c, padded to 32) as bf16 pairs
+        for (int i = t; i < S2_ROWS; i += 256) {
+            const int sy = i / S2_RW, sx = i - sy * S2_RW;
+            const float *w0 = patch + sy * S2_PP + sx;
+            const bool ok = i < S2_RW * S2_RH;
+            uint32_t packed[16];
+            {
+                float v[32];
+#pragma unroll
+                for (int ky = 0; ky < 3; ++ky)
+#pragma unroll
+                    for (int kx = 0; kx < 3; ++kx)
+#pragma unroll
+                        for (int c = 0; c < 3; ++c) v[(ky * 3 + kx) * 3 + c] = ok ? w0[(c * S2_PH + ky) * S2_PP + kx] : 0.f;
+#pragma unroll
+                for (int k = 27; k < 32; ++k) v[k] = 0.f;
+#pragma unroll
+                for (int k = 0; k < 16; ++k) packed[k] = pack_bf16x2(v[2 * k], v[2 * k + 1]);
+            }
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+                *reinterpret_cast<uint4 *>(sm + S2_U + i * 64 + ((j ^ ((i >> 1) & 3)) << 4)) =
+                    make_uint4(packed[4 * j], packed[4 * j + 1], packed[4 * j + 2], packed[4 * j + 3]);
+        }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the tensor core
+        __syncthreads();
+
+        // ---- 2. stem wgmmas
+        float ds[5][16];
+#pragma unroll
+        for (int c = 0; c < 5; ++c)
+#pragma unroll
+            for (int i = 0; i < 16; ++i) ds[c][i] = 0.f;
+#pragma unroll
+        for (int c = 0; c < 5; ++c) wg_fence_operand(ds[c]);
+        wg_fence();
+#pragma unroll
+        for (int c = 0; c < 5; ++c)
+#pragma unroll
+            for (int k = 0; k < 2; ++k)
+                Wg<0, 32>::mma(ds[c], wg_desc(U + (uint32_t)(5 * wg + c) * 4096u + 32u * k, hi), wg_desc(base + S2_BS + 32u * k, hi), (uint32_t)k);
+        wg_commit();
+        wg_wait<0>();
+#pragma unroll
+        for (int c = 0; c < 5; ++c) wg_fence_operand(ds[c]);
+        __syncthreads();   // every stem wgmma has read its rows: the sets may overwrite them
+
+        // ---- stem epilogue into the sets.  Region column sx goes to set kx = 1 (sx odd), or to kx = 0 and / or kx = 2 (sx even).
+        // (no "memory" clobbers on these stores: the bias loads may be scheduled freely around them; the barrier below orders them)
+        {
+#pragma unroll
+            for (int c = 0; c < 5; ++c)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int i = 64 * (5 * wg + c) + rl + 8 * h;
+                    if (i >= S2_RW * S2_RH) continue;
+                    const int sy = i / S2_RW, sx = i - sy * S2_RW, y = gy0 + sy, x = gx0 + sx;
+                    const bool in_img = y >= 0 && y < p.H && x >= 0 && x < p.W;
+                    uint32_t v[4];
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        float a = ds[c][4 * j + 2 * h] + bias0_s[8 * j + cq], b = ds[c][4 * j + 2 * h + 1] + bias0_s[8 * j + cq + 1];
+                        if (leaky0) { a = fmaxf(a, 0.1f * a); b = fmaxf(b, 0.1f * b); }
+                        v[j] = in_img ? pack_bf16x2(a, b) : 0u;
+                    }
+                    const uint32_t set = U + ((sy & 1) ? 9u * 1024u : 0u) + (uint32_t)(sy >> 1) * 1024u + 2u * (uint32_t)cq;
+                    auto put = [&](int kx, int ox) {
+                        const uint32_t row = set + (uint32_t)kx * S2_SETS_KX + (uint32_t)ox * 64u;
+#pragma unroll
+                        for (int j = 0; j < 4; ++j)
+                            asm volatile("st.shared.b32 [%0], %1;" ::"r"(row + ((uint32_t)(j ^ ((ox >> 1) & 3)) << 4)), "r"(v[j]));
+                    };
+                    const bool odd = sx & 1, last = sx == 2 * S2_TW;
+                    put(odd ? 1 : last ? 2 : 0, last ? (sx >> 1) - 1 : sx >> 1);
+                    if (!odd && !last && sx >= 2) put(2, (sx >> 1) - 1);
+                }
+        }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        __syncthreads();
+
+        if (tile + (int)gridDim.x < p.ntiles) load_patch(tile + gridDim.x, pv);
+
+        // ---- 3. layer 1: 9 taps x two m64n64k16 into warpgroup wg's 64 rows (tile rows oy = 4 wg .. 4 wg + 3)
+        float d[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) d[i] = 0.f;
+        wg_fence_operand(d);
+        wg_fence();
+#pragma unroll
+        for (int r = 0; r < 9; ++r) {
+            const int ky = r / 3, kx = r % 3;
+            const uint32_t a = U + (uint32_t)kx * S2_SETS_KX + ((ky & 1) ? 9u * 1024u : 0u) + (uint32_t)(ky >> 1) * 1024u + (uint32_t)wg * 4096u;
+            const uint32_t b = base + S2_B1 + (uint32_t)r * 4096u;
+#pragma unroll
+            for (int k = 0; k < 2; ++k)
+                Wg<0, 64>::mma(d, wg_desc(a + 32u * k, hi), wg_desc(b + 32u * k, hi), (r > 0 || k > 0) ? 1u : 0u);
+        }
+        wg_commit();
+        wg_wait<0>();
+        wg_fence_operand(d);
+        __syncthreads();   // both warpgroups are done with the sets: the staging tiles may overwrite them
+
+        // ---- 4. epilogue: staging tile [64 pixels][128 B], 16-byte chunk j of row q at j ^ (q & 7)
+        const uint32_t stg = U + S2_STG + (uint32_t)wg * 8192u;
+        float b1[16];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) { b1[2 * j] = bias1_s[8 * j + cq]; b1[2 * j + 1] = bias1_s[8 * j + cq + 1]; }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int q = rl + 8 * h;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                float a = d[4 * j + 2 * h] + b1[2 * j], b = d[4 * j + 2 * h + 1] + b1[2 * j + 1];
+                if (leaky1) { a = fmaxf(a, 0.1f * a); b = fmaxf(b, 0.1f * b); }   // == a > 0 ? a : 0.1a
+                asm volatile("st.shared.b32 [%0], %1;" ::"r"(stg + (uint32_t)q * 128u + ((uint32_t)(j ^ (q & 7)) << 4) + 2u * (uint32_t)cq),
+                             "r"(pack_bf16x2(a, b)) : "memory");
+            }
+        }
+        if (wg == 0) named_bar_sync(1, 128);   // constant barrier ids: ptxas reserves 2 barriers, not all 16
+        else named_bar_sync(2, 128);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const int idx = (t & 127) + 128 * k, q = idx >> 3, ch = idx & 7;
+            const int oy = oy0 + 4 * wg + (q >> 4), ox = ox0 + (q & 15);
+            if (oy < p.OH && ox < p.OW) {
+                uint4 o;
+                asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(o.x), "=r"(o.y), "=r"(o.z), "=r"(o.w)
+                             : "r"(stg + (uint32_t)q * 128u + ((uint32_t)(ch ^ (q & 7)) << 4)) : "memory");
+                *reinterpret_cast<uint4 *>(p.out + ((size_t)(n * p.OHp + oy + 1) * p.OWp + ox + 1) * (size_t)p.out_ldc * 2 + ch * 16) = o;
+            }
+        }
+        // the next tile writes this staging tile only after two block barriers, which every thread reaches after its stores
     }
 }
 
@@ -1543,7 +1785,7 @@ void *tc_make_plan_xnor(const Layer &l, const TV &q, const TV &out, const void *
     return plan;
 }
 
-struct StemPlan { StemTcP p; int grid; };
+struct StemPlan { StemTcP p; int grid; bool s2; };   // s2: k_stem_s2_tc (stem + layer 1)
 int tc_stem_supported(const Layer &l, const TV &out) {
     return l.c == 3 && l.size == 3 && l.stride == 1 && l.pad == 1 && (l.n == 16 || l.n == 32) &&
            (l.activation == YB_LEAKY || l.activation == YB_LINEAR) && out.base && out.ldc % 8 == 0 &&
@@ -1565,18 +1807,51 @@ void *tc_stem_make_plan(const Layer &l, const TV &out, const void *d_w, const fl
     sp->grid = std::min(p.ntiles, sms * 8);
     return sp;
 }
+int tc_stem_s2_supported(const Layer &l0, const Layer &l1, const TV &out1) {
+    return l0.n == 32 && l1.c == 32 && l1.n == 64 && l1.size == 3 && l1.stride == 2 && l1.pad == 1 && l1.h == l0.h && l1.w == l0.w &&
+           l0.h % 2 == 0 && l0.w % 2 == 0 && (l1.activation == YB_LEAKY || l1.activation == YB_LINEAR) && out1.base && out1.P == 1 &&
+           out1.H == l0.h / 2 && out1.W == l0.w / 2 && out1.ldc % 8 == 0 && (reinterpret_cast<uintptr_t>(out1.base) & 15) == 0;
+}
+// d_w1: layer 1's bf16 [64][9 * 32] filter matrix (K ordered (ky, kx, c)), d_bias1: its f32 bias
+void *tc_stem_s2_make_plan(const Layer &l0, const Layer &l1, const TV &out1, const void *d_w, const float *d_bias, const void *d_w1,
+                           const float *d_bias1) {
+    StemPlan *sp = new StemPlan();
+    memset(sp, 0, sizeof(*sp));
+    sp->s2 = true;
+    StemTcP &p = sp->p;
+    p.out = out1.base; p.out_ldc = out1.ldc; p.w = reinterpret_cast<const __nv_bfloat16 *>(d_w); p.bias = d_bias;
+    p.N = out1.N; p.H = l0.h; p.W = l0.w; p.OHp = out1.Hp; p.OWp = out1.Wp; p.nf = l0.n; p.act = l0.activation;
+    p.w1 = reinterpret_cast<const __nv_bfloat16 *>(d_w1); p.bias1 = d_bias1; p.act1 = l1.activation;
+    p.OH = out1.H; p.OW = out1.W;
+    p.xt = (p.OW + S2_TW - 1) / S2_TW; p.yt = (p.OH + S2_TH - 1) / S2_TH;
+    const long ntiles = (long)p.N * p.xt * p.yt;
+    if (ntiles >= INT_MAX) fatal_throw("stem plan: too many tiles");
+    p.ntiles = (int)ntiles;
+    int dev = 0, sms = 132;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    sp->grid = std::min(p.ntiles, grid_cap(2 * sms));
+    for (const void *f : {(const void *)k_stem_s2_tc<false>, (const void *)k_stem_s2_tc<true>}) {
+        if (cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S2_SMEM) != cudaSuccess ||
+            cudaFuncSetAttribute(f, cudaFuncAttributePreferredSharedMemoryCarveout, 100) != cudaSuccess)
+            fatal_throw("cudaFuncSetAttribute(k_stem_s2_tc) failed");
+    }
+    return sp;
+}
 void tc_stem_launch(void *vp, const float *d_in_nchw, cudaStream_t s) {
     StemPlan *sp = reinterpret_cast<StemPlan *>(vp);
     StemTcP p = sp->p;
     p.in = d_in_nchw;
-    k_stem_tc<false><<<sp->grid, 128, 0, s>>>(p);
+    if (sp->s2) k_stem_s2_tc<false><<<sp->grid, 256, S2_SMEM, s>>>(p);
+    else k_stem_tc<false><<<sp->grid, 128, 0, s>>>(p);
 }
 // 8-bit HWC frames of exactly the network size (3 channels): no planar-float staging
 void tc_stem_launch_u8(void *vp, const unsigned char *d_in_hwc, cudaStream_t s) {
     StemPlan *sp = reinterpret_cast<StemPlan *>(vp);
     StemTcP p = sp->p;
     p.in8 = d_in_hwc;
-    k_stem_tc<true><<<sp->grid, 128, 0, s>>>(p);
+    if (sp->s2) k_stem_s2_tc<true><<<sp->grid, 256, S2_SMEM, s>>>(p);
+    else k_stem_tc<true><<<sp->grid, 128, 0, s>>>(p);
 }
 void tc_stem_free_plan(void *vp) { delete reinterpret_cast<StemPlan *>(vp); }
 

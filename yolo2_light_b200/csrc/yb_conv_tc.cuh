@@ -33,6 +33,11 @@ void tc_plan_fuse_yolo(void *plan, float *d_yolo_nchw, int classes);
 // tensor-core stem (3-channel 3x3 from the caller's NCHW f32 image, bf16 NHWC out)
 int tc_stem_supported(const Layer &l, const TV &out);
 void *tc_stem_make_plan(const Layer &l, const TV &out, const void *d_w_32x32_bf16, const float *d_bias);
+// the tensor-core stem fused with layer 1, a 3x3 / stride-2 convolution 32 -> 64 filters (bf16 out1): the stem output never
+// reaches HBM.  The plan takes the same launch / free calls as the stem's.
+int tc_stem_s2_supported(const Layer &l0, const Layer &l1, const TV &out1);
+void *tc_stem_s2_make_plan(const Layer &l0, const Layer &l1, const TV &out1, const void *d_w_32x32_bf16, const float *d_bias,
+                           const void *d_w1_bf16, const float *d_bias1);
 void tc_stem_launch(void *plan, const float *d_in_nchw, cudaStream_t s);
 void tc_stem_launch_u8(void *plan, const unsigned char *d_in_hwc, cudaStream_t s);   // frames already of the network size
 void tc_stem_free_plan(void *plan);

@@ -555,7 +555,7 @@ std::shared_ptr<Engine> build_engine(Network *net, const EngineOptions &opt) {
 
     // ---- op list -----------------------------------------------------------------------------------
     Engine *E = e.get();
-    bool stem_fused = false, stem_pool_fused = false;
+    bool stem_fused = false, stem_pool_fused = false, stem_s2_fused = false;
     {
         // ops[0] consumes the caller's NCHW f32 images.  Usually that is the stem convolution itself (3 input
         // channels, 3x3/1/1), reading NCHW directly; otherwise a plain NCHW -> padded-NHWC conversion.
@@ -603,12 +603,24 @@ std::shared_ptr<Engine> build_engine(Network *net, const EngineOptions &opt) {
             };
         } else if (stem_ok && stem_w_off != (size_t)-1 && e->out_dt[0] == DT_BF16 && tc_stem_supported(l0, e->out_tv[0]) &&
             !getenv("YB_NO_STEM_TC")) {
-            // tensor-core stem: gathers the 3x3x3 window from NCHW, K padded 27 -> 32
+            // tensor-core stem: gathers the 3x3x3 window from NCHW, K padded 27 -> 32.  When layer 1 is a bf16 tensor-core
+            // 3x3 / stride-2 convolution 32 -> 64 and the stem's only reader, both run as one kernel (k_stem_s2_tc) and the
+            // stem output is never written (its buffer stays allocated but unused).
             stem_fused = true;
-            void *sp = tc_stem_make_plan(l0, e->out_tv[0], e->w_arena + stem_w_off,
-                                         reinterpret_cast<const float *>(e->w_arena + cw[0].bias));
+            const float *bias0 = reinterpret_cast<const float *>(e->w_arena + cw[0].bias);
+            stem_s2_fused = opt.fuse && !getenv("YB_NO_STEM_S2_FUSE") && nl > 1 && cons[0].size() == 1 && cons[0][0] == 1 &&
+                            net->layers[1].type == YB_CONVOLUTIONAL && conv_variant(1) == 0 && use_tc[1] == 1 &&
+                            fused_into[1] < 0 && e->out_dt[1] == DT_BF16 && tc_stem_s2_supported(l0, net->layers[1], e->out_tv[1]);
+            void *sp = stem_s2_fused ? tc_stem_s2_make_plan(l0, net->layers[1], e->out_tv[1], e->w_arena + stem_w_off, bias0,
+                                                            e->w_arena + cw[1].w_bf16, reinterpret_cast<const float *>(e->w_arena + cw[1].bias))
+                                     : tc_stem_make_plan(l0, e->out_tv[0], e->w_arena + stem_w_off, bias0);
             e->stem_plan = sp;
             e->first_kind = OP_CONV_TC; e->first_layer = 0;
+            if (stem_s2_fused) {
+                e->not_materialised[0] = 1;
+                e->first_layer = 1;
+                ++e->n_tc;
+            }
             e->first_op = [sp](const float *din, cudaStream_t s) { tc_stem_launch(sp, din, s); };
             if (!getenv("YB_NO_STEM_U8")) e->first_op_u8 = [sp](const unsigned char *d8, cudaStream_t s) { tc_stem_launch_u8(sp, d8, s); };
         } else if (stem_ok) {
@@ -654,7 +666,7 @@ std::shared_ptr<Engine> build_engine(Network *net, const EngineOptions &opt) {
             if (!prev_ok) fatal_throw("engine: layer " + std::to_string(i) + " has no image input");
         };
         if (i == 0 && stem_fused) continue;
-        if (i == 1 && stem_pool_fused) continue;
+        if (i == 1 && (stem_pool_fused || stem_s2_fused)) continue;
         switch (l.type) {
         case YB_CONVOLUTIONAL: {
             need_prev();
