@@ -215,7 +215,8 @@ int  yb_network_last_launches(const yb_network *net);
  * (1: keep the raw XNOR popcounts / INT8 s32 accumulators of every integer conv), "q_index_offset".  Returns -1 for an
  * unknown name. */
 int  yb_network_set_option(yb_network *net, const char *name, int value);
-/* Engine facts (builds the engine if needed): "launches", "tc_layers" (convolutions on the tensor cores).  -1: unknown key. */
+/* Engine facts (builds the engine if needed): "launches", "tc_layers" (convolutions on the tensor cores),
+   "act_bytes" (device memory of the activation buffers).  -1: unknown key. */
 long yb_network_get_info(yb_network *net, int quantized, const char *key);
 /* Raw integer results of conv layer i (NCHW, batch-major) when "keep_counts" is on; returns the element count. */
 int  yb_network_fetch_counts(yb_network *net, int i, int quantized, int32_t *dst, size_t count);

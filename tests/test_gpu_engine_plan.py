@@ -1,0 +1,70 @@
+"""The engine's op sequence, pinned per model, precision and fusion setting (tests/golden/engine_plans.json, recorded with
+tests/golden/make_engine_plans.py): the same ops in the same order on the same layers, the same launch and tensor-core counts.
+Activation memory holds only outputs some op writes: every layer whose fetch_layer raises has no buffer, the NHWC input copy
+exists only when the first op makes it, and a detection head whose [yolo] layer runs in its epilogue raises too."""
+import json
+import os
+import sys
+
+import pytest
+
+import ybtest_util as util
+
+sys.path.insert(0, util.GOLDEN)
+import make_engine_plans as plans  # noqa: E402
+
+pytestmark = pytest.mark.gpu
+
+with open(os.path.join(util.GOLDEN, "engine_plans.json")) as _f:
+    PINNED = json.load(_f)
+MODELS = sorted({c["model"] for c in PINNED["cases"]})
+
+DT_BYTES = {"f32": 4, "bf16": 2}
+
+
+def _align(v, a=1024):
+    return (v + a - 1) // a * a
+
+
+def _freed_bytes(net, prec, case, raises):
+    """Bytes of the buffers that a recorded case allocated and the current engine does not: the outputs of layers that now
+    raise (other than convolutions fused into the shortcut behind them, which never had one) and the NHWC input copy when a
+    stem reads the caller's images."""
+    layers = net.layers
+    B = PINNED["batch"]
+    exact = prec in ("fp32", "int8") or any(l["type_name"] == "CONVOLUTIONAL" and l["xnor"] for l in layers)
+    act = "f32" if exact else "bf16"
+    freed = 0
+    if case["ops"][0][1] != "input":
+        freed += _align(B * (net.h + 2) * (net.w + 2) * net.c * DT_BYTES[act])
+    for i in raises:
+        l = layers[i]
+        nxt = layers[i + 1]["type_name"] if i + 1 < len(layers) else None
+        if case["fuse"] and l["type_name"] == "CONVOLUTIONAL" and nxt == "SHORTCUT":
+            continue
+        head = l["type_name"] == "CONVOLUTIONAL" and nxt in ("YOLO", "REGION")
+        dt = "f32" if head else act
+        freed += _align(B * (l["out_h"] + 2) * (l["out_w"] + 2) * _align(l["out_c"], 8) * DT_BYTES[dt])
+    return freed
+
+
+@pytest.mark.parametrize("model", MODELS)
+def test_engine_plan_matches_pinned(model, workdir):
+    cases = [c for c in PINNED["cases"] if c["model"] == model]
+    assert len(cases) == len([k for k in plans.cases() if k[0] == model])
+    nets = {}
+    for case in cases:
+        prec, fuse, no_s2 = case["prec"], case["fuse"], case["no_s2"]
+        q = prec == "int8"
+        if q not in nets:
+            nets[q] = plans.load(model, prec, workdir)
+        net = nets[q]
+        got = plans.record(net, prec, fuse, no_s2)
+        what = (model, prec, fuse, no_s2)
+        assert got["ops"] == case["ops"], what
+        assert got["launches"] == case["launches"] and got["tc_layers"] == case["tc_layers"], what
+        # the [yolo] layers with no op of their own are written by their head's epilogue: the head now raises
+        ops_layers = {li for li, _ in case["ops"]}
+        fused_heads = {i - 1 for i, l in enumerate(net.layers) if l["type_name"] == "YOLO" and i not in ops_layers}
+        assert set(got["raises"]) == set(case["raises"]) | fused_heads, what
+        assert got["act_bytes"] == case["act_bytes"] - _freed_bytes(net, prec, case, got["raises"]), what

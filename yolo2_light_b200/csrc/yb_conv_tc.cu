@@ -1620,7 +1620,8 @@ static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &
     p.desc_hi = ((8u * row_bytes) >> 4) | (layout_type << 30);
     p.out = out.base; p.out_ldc = out.ldc;
     p.n = l.n;
-    p.n_store = out_bf16 ? l.n : std::min<int>((l.n + 3) / 4 * 4, out.ldc);
+    // f32: whole float4 groups, within the output's pixel stride (a fused [yolo] head has no NHWC output)
+    p.n_store = out_bf16 ? l.n : out.base ? std::min<int>((l.n + 3) / 4 * 4, out.ldc) : (l.n + 3) / 4 * 4;
     if (!out_bf16 && (out.ldc % 4 != 0)) fatal_throw("tc plan: f32 output rows must be 16-byte aligned");
     p.res = res.base;
     if (res.base && (res.H != l.out_h || res.W != l.out_w || res.C != l.n)) fatal_throw("tc plan: residual shape mismatch");
@@ -1670,7 +1671,7 @@ static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &
         if (r != CUDA_SUCCESS) { delete plan; fatal_throw("cuTensorMapEncodeTiled(B) failed: " + std::to_string((int)r)); }
     }
     plan->tmO = plan->tmA; plan->tmO1 = plan->tmA; plan->tmR = plan->tmA;   // valid placeholders when unused
-    if (p.tma_epi) {
+    if (p.tma_epi && out.base) {   // a plan with a fused max-pool has no output to map
         const int oesz = out_bf16 ? 2 : 4;
         auto encode_px = [&](CUtensorMap *tm, const TV &t, const char *what, int box_rows) {
             // (channels, padded x, merged padded rows) of a padded-NHWC tensor (bf16, or f32 for the integer kinds); box = one
@@ -1755,17 +1756,25 @@ void tc_plan_fuse_yolo(void *vp, float *d_yolo_nchw, int classes) {
     plan->p.yolo_per = 4 + classes + 1;
 }
 
+// Whether an integer-kind plan of `l` made with want_pool_tile can take the following 2x2 / stride-2 max-pool (tc_plan_fuse_pool):
+// its 8 x 16 tiles (stride-1 3x3 layers only) start one merged row down, so 2x2 windows never straddle tiles when the padded
+// height and the output size are even.
+int tc_pool_fuse_supported(const Layer &l, const TV &qnext) {
+    return l.size == 3 && l.stride == 1 && l.h % 2 == 0 && l.out_h % 2 == 0 && l.out_w % 2 == 0 && l.n % 32 == 0 &&
+           qnext.H == l.out_h / 2 && qnext.W == l.out_w / 2 && qnext.ldc % 16 == 0 && (reinterpret_cast<uintptr_t>(qnext.base) & 15) == 0;
+}
+
 // Fuse the following 2x2 / stride-2 max-pool and the next integer layer's input conversion into an integer-kind plan with 8 x 16 tiles:
 // mode 1 = s8 quantised with `mult` (INT8 layer next), 2 = +-1 bytes (XNOR layer on the tensor cores next).  `qnext` is that layer's
-// s8 input (padded NHWC).  Returns 0 (and changes nothing) when the plan's tiling cannot do it.
-int tc_plan_fuse_pool(void *vp, int mode, float mult, const TV &qnext) {
+// s8 input (padded NHWC).  The caller has checked tc_pool_fuse_supported.
+void tc_plan_fuse_pool(void *vp, int mode, float mult, const TV &qnext) {
     TcPlan *plan = reinterpret_cast<TcPlan *>(vp);
     TcParams &p = plan->p;
-    if (!(p.kind == 1 || p.kind == 2) || p.TW != 8 || p.jshift != 1 || (p.PR & 1) || (p.OW & 1) || (p.OH & 1) || p.acc_out) return 0;
-    if (qnext.H != p.OH / 2 || qnext.W != p.OW / 2 || qnext.ldc % 16 != 0 || (reinterpret_cast<uintptr_t>(qnext.base) & 15) || p.n % 32 != 0) return 0;
+    if (!(p.kind == 1 || p.kind == 2) || p.TW != 8 || p.jshift != 1 || (p.PR & 1) || (p.OW & 1) || (p.OH & 1) || p.acc_out ||
+        qnext.H != p.OH / 2 || qnext.W != p.OW / 2 || qnext.ldc % 16 != 0 || (reinterpret_cast<uintptr_t>(qnext.base) & 15) || p.n % 32 != 0)
+        fatal_throw("tc plan: the max-pool does not fit the plan's tiling");
     p.pool_mode = mode; p.pool_mult = mult;
     p.pool_out = reinterpret_cast<signed char *>(qnext.base); p.pool_ldc = qnext.ldc; p.pool_Hp = qnext.Hp; p.pool_Wp = qnext.Wp;
-    return 1;
 }
 
 void *tc_make_plan_i8(const Layer &l, const TV &q, const TV &out, const void *d_weights_s8, int ldn, const float *d_bias,

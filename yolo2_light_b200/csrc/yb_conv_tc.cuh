@@ -26,9 +26,13 @@ void *tc_make_plan_i8(const Layer &l, const TV &q, const TV &out, const void *d_
 // XNOR layer as +-1 s8 on the s8 wgmma (q: s8 activation with -1 borders)
 void *tc_make_plan_xnor(const Layer &l, const TV &q, const TV &out, const void *d_weights_pm1, int ldn, const float *d_bias,
                         const float *d_mean, int *counts_out, int want_pool_tile = 0);
-// fuse the following 2x2/2 max-pool + the next integer layer's input conversion (1: s8 quantised, 2: +-1 bytes) into an integer plan
-int tc_plan_fuse_pool(void *plan, int mode, float mult, const TV &qnext);
-// fuse the following [yolo] layer into the (f32-output) plan: logistic + NCHW store in the epilogue
+// non-zero if an integer plan of `l` made with want_pool_tile takes tc_plan_fuse_pool (qnext: the next integer layer's input)
+int tc_pool_fuse_supported(const Layer &l, const TV &qnext);
+// fuse the following 2x2/2 max-pool + the next integer layer's input conversion (1: s8 quantised, 2: +-1 bytes) into an integer
+// plan; the plan then writes no output of its own (`out` may have no base)
+void tc_plan_fuse_pool(void *plan, int mode, float mult, const TV &qnext);
+// fuse the following [yolo] layer into the (f32-output) plan: logistic + NCHW store in the epilogue; the plan then writes no
+// NHWC output (`out` may have no base)
 void tc_plan_fuse_yolo(void *plan, float *d_yolo_nchw, int classes);
 // tensor-core stem (3-channel 3x3 from the caller's NCHW f32 image, bf16 NHWC out)
 int tc_stem_supported(const Layer &l, const TV &out);

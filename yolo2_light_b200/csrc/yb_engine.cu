@@ -54,15 +54,32 @@ struct ConvWeights {   // offsets into the weight arena
     int cpad = 0;     // padded channels of the s8 / bits / bf16 layouts
 };
 
+// The diagnostic YB_* switches of the engine (DESIGN, appendix), read once when an engine is built.
+struct Switches {
+    bool no_graph, no_nccl, no_tc, no_tf32, no_stem, no_stem_tc, no_stem_u8, no_stem_pool_fuse, no_stem_s2_fuse,
+         no_conv_pool_fuse, no_pool_fuse, no_yolo_fuse;
+    bool xnor_tc;       // YB_XNOR_TC=0 puts every XNOR layer on the popcount kernels
+    int xnor_tc_minc;   // narrowest XNOR layer on the tensor cores
+    static Switches read() {
+        auto set = [](const char *name) { return getenv(name) != nullptr; };
+        const char *xtc = getenv("YB_XNOR_TC"), *minc = getenv("YB_XNOR_TC_MINC");
+        return Switches{set("YB_NO_GRAPH"), set("YB_NO_NCCL"), set("YB_NO_TC"), set("YB_NO_TF32"), set("YB_NO_STEM"),
+                        set("YB_NO_STEM_TC"), set("YB_NO_STEM_U8"), set("YB_NO_STEM_POOL_FUSE"), set("YB_NO_STEM_S2_FUSE"),
+                        set("YB_NO_CONV_POOL_FUSE"), set("YB_NO_POOL_FUSE"), set("YB_NO_YOLO_FUSE"),
+                        !(xtc && xtc[0] == '0'), minc ? atoi(minc) : 16};
+    }
+};
+
 struct Engine {
     EngineOptions opt;
+    Switches sw{};
     int batch = 0;
     int act_dt = DT_F32;
     cudaStream_t stream = nullptr;
     char *act_arena = nullptr; size_t act_bytes = 0;
     char *w_arena = nullptr;   size_t w_bytes = 0;
     float *d_input = nullptr;  size_t input_count = 0;
-    std::vector<TV> out_tv;            // per layer (base == nullptr: no NHWC output)
+    std::vector<TV> out_tv;            // per layer (base == nullptr: no NHWC output, or one that exists only in a fused form)
     std::vector<int> out_dt;
     std::vector<float *> d_final;      // yolo / region device outputs
     std::vector<float *> h_final;      // pinned host mirrors
@@ -70,8 +87,7 @@ struct Engine {
     std::vector<int32_t *> d_counts;   // optional raw integer results per conv layer
     std::vector<size_t> counts_count;
     std::vector<Op> ops;
-    std::vector<char> not_materialised;   // layer outputs that exist only in a consumer's fused form
-    TV in0{};
+    TV in0{};                          // NHWC copy of the caller's images (base == nullptr: the stem reads them directly)
     int in0_dt = DT_F32;
     cudaGraphExec_t graph_exec = nullptr;
     bool graph_failed = false;
@@ -183,6 +199,876 @@ static void dispatch_dt(int dt, F &&f) {
     else f((__nv_bfloat16 *)nullptr);
 }
 
+// ---- engine build --------------------------------------------------------------------------------------------------------
+// Four passes, in this order: plan_layers decides every kernel path and fusion, each layer output's dtype and home, and which
+// outputs are materialised; place allocates the activation buffers that some op writes; pack_weights fills the weight arena;
+// the emit_* functions turn the plan into the op list in layer order, reading the plan only.
+
+enum FirstOp { FIRST_NHWC, FIRST_STEM_SIMT, FIRST_STEM_TC, FIRST_STEM_S2, FIRST_STEM_POOL };
+enum ConvPath { CP_NONE, CP_TC, CP_TF32, CP_SIMT, CP_XNOR_FALLBACK, CP_XNOR_TC, CP_XNOR_SMALLK, CP_XNOR_GENERAL, CP_I8_TC, CP_I8_SIMT };
+enum SideFmt { SIDE_NONE, SIDE_PM1_F32, SIDE_S8, SIDE_BITS };   // a convolution's converted input
+
+struct LayerPlan {
+    int variant = 0;            // convolutions: 0 fp32, 1 xnor, 2 int8
+    int path = CP_NONE;
+    int fused_into = -1;        // conv + shortcut: this convolution writes the shortcut's output
+    bool fused_sc = false;      // shortcut computed in the epilogue of the convolution in front of it
+    bool yolo_fused = false;    // conv: writes the [yolo] layer behind it from its epilogue; [yolo]: written that way
+    bool pool_tile = false;     // integer tensor-core conv: 8 x 16 pixel tiles, as a fused 2x2 max-pool needs
+    int pool_mode = 0;          // conv: runs the max-pool behind it and layer i+2's input conversion (1 s8, 2 +-1 bytes, 3 sign bits)
+    bool pool_in_conv = false;  // max-pool: runs in the epilogue of the convolution in front of it
+    bool pool_to_side = false;  // max-pool: writes the next convolution's converted input instead of its own output
+    bool prefilled = false;     // conv: its converted input is written by the op in front of it
+    bool in_first_op = false;   // computed by the op that reads the caller's images
+    int out_dt = DT_F32;
+    int side = SIDE_NONE, side_ld = 0;   // converted input of a convolution and its pixel stride
+    bool has_out = false;       // has an NHWC output: own buffer, channel slice of a route's buffer, or alias
+    bool materialised = false;  // ... and some op writes it
+    int owner = -1, coff = 0;   // channel slice at `coff` of route `owner`'s buffer (owner -1: own buffer or alias)
+    int ldc = 0;                // pixel stride of an own buffer
+};
+
+// Stands in for the activation arena while the plan is made.  Every buffer starts 1024-byte aligned in the arena, so the
+// predicates that check a view's alignment answer the same for views rooted here as for the placed ones.
+static char *const kLayoutBase = reinterpret_cast<char *>(uintptr_t(1) << 40);
+
+static bool vec4_view(const TV &t) { return t.ldc % 4 == 0 && (reinterpret_cast<uintptr_t>(t.base) & 15) == 0; }
+
+// calls put(filter, channel, tap, index into l.weights) for every weight of convolution l
+template <typename F>
+static void for_each_weight(const Layer &l, F &&put) {
+    const int taps = l.size * l.size;
+    for (int f = 0; f < l.n; ++f)
+        for (int c = 0; c < l.c; ++c)
+            for (int t = 0; t < taps; ++t) put(f, c, t, ((size_t)f * l.c + c) * taps + t);
+}
+
+// stem weights as by-value kernel constants: [27 = (ky,kx,c)][NF] + bias
+template <int NF>
+static StemW<NF> stem_weights(const Layer &l0) {
+    StemW<NF> w{};
+    for_each_weight(l0, [&](int f, int c, int t, size_t k) { w.w[(t * 3 + c) * NF + f] = l0.weights[k]; });
+    for (int f = 0; f < l0.n; ++f) w.b[f] = l0.biases[f];
+    return w;
+}
+
+namespace {
+constexpr int P = 1;   // border of every activation buffer
+
+struct Builder {
+    Network &net;
+    const EngineOptions &opt;
+    Engine &e;
+    const Switches &sw;
+    const int B, nl;
+    int ADT = DT_F32;
+    std::vector<std::vector<int>> cons;
+    std::vector<LayerPlan> L;
+    int first = FIRST_NHWC;
+    std::vector<size_t> buf_off, side_off;
+    std::vector<ConvWeights> cw;
+    size_t stem_w_off = (size_t)-1;
+
+    Builder(Network &n, const EngineOptions &o, Engine &en)
+        : net(n), opt(o), e(en), sw(en.sw), B(n.batch), nl((int)n.layers.size()), cons(consumers_of(n)), L(nl),
+          buf_off(nl, (size_t)-1), side_off(nl, (size_t)-1), cw(nl) {}
+
+    const Layer &layer(int i) const { return net.layers[i]; }
+    bool is_conv(int i) const { return layer(i).type == YB_CONVOLUTIONAL; }
+    bool sole_reader(int i, int r) const { return cons[i].size() == 1 && cons[i][0] == r; }
+    bool is_alias(int i) const { return layer(i).type == YB_ROUTE && layer(i).n == 1 && opt.fuse; }
+
+    int conv_variant(int i) const {   // 0 fp32, 1 xnor, 2 int8
+        const Layer &l = layer(i);
+        if (opt.qrule && (i + opt.q_index_offset) >= 1 && l.activation != YB_LINEAR) return 2;
+        return l.xnor ? 1 : 0;
+    }
+    // XNOR layers with enough channels run on the tensor cores as +-1 int8 (dot == 2*count - K, exact); the small ones stay on
+    // the popcount kernels.  Channels are padded to a multiple of 32 with zero WEIGHT bytes (whatever the activation pad bytes
+    // hold contributes 0), so even the 16- and 32-channel layers run there: the popcount kernels are bound by the 16 POPC/clk/SM
+    // of the integer pipe, while the same layers as +-1 bytes on the s8 tensor cores are not.
+    bool xnor_on_tc(const Layer &l) const {
+        return sw.xnor_tc && l.xnor && l.c % 16 == 0 && l.c >= sw.xnor_tc_minc && l.size == 3 && l.stride == 1 && l.pad == 1 && l.n >= 8;
+    }
+    // XNOR layers with stride != 1 or pad != 1 never reach the bit GEMM in the reference: forward_convolutional_layer_cpu
+    // binarises the input to +-1 floats (binarize_cpu, additionally.c:128-134), swaps in the +-mean weights (binarize_weights,
+    // :113-126) and runs the ordinary im2col + gemm_nn (yolov2_forward_network.c:40-50, :204) -- out-of-image taps count 0 there,
+    // not -1.  Same here: k_binarize_pm1 + the exact-order float convolution.
+    static bool xnor_fallback(const Layer &l) { return l.xnor && !(l.stride == 1 && l.pad == 1); }
+
+    // integer conv i -> 2x2/2 max-pool i+1 -> integer conv i+2, nothing else reading i or i+1: the pool and the next layer's
+    // input conversion may run in conv i's epilogue.  Returns the mode (1 s8 quantised, 2 +-1 bytes, 3 sign bits) or 0.
+    int conv_pool_mode(int i) const {
+        if (!opt.fuse || opt.keep_counts || sw.no_conv_pool_fuse || i + 2 >= nl) return 0;
+        const Layer &mp = layer(i + 1), &c2 = layer(i + 2);
+        if (mp.type != YB_MAXPOOL || mp.size != 2 || mp.stride != 2 || mp.pad != 1 || c2.type != YB_CONVOLUTIONAL) return 0;
+        if (!sole_reader(i, i + 1) || !sole_reader(i + 1, i + 2)) return 0;
+        const int v2 = L[i + 2].variant;
+        if (v2 == 2) return 1;
+        if (v2 == 1 && xnor_on_tc(c2) && !xnor_fallback(c2)) return 2;
+        if (v2 == 1 && !xnor_fallback(c2)) return 3;     // next XNOR layer reads sign bits (popcount kernels)
+        return 0;
+    }
+
+    // layer i's NHWC output view; buf(j) is the start of layer j's own buffer
+    template <typename F>
+    TV out_view(int i, F &&buf) const {
+        const Layer &l = layer(i);
+        if (is_alias(i)) return out_view(l.input_layers[0], buf);
+        if (L[i].owner >= 0)
+            return make_tv(buf(L[i].owner), B, l.out_h, l.out_w, l.out_c, L[L[i].owner].ldc, P, ADT, L[i].coff);
+        return make_tv(buf(i), B, l.out_h, l.out_w, l.out_c, L[i].ldc, P, L[i].out_dt, 0);
+    }
+    TV layout_view(int i) const { return L[i].has_out ? out_view(i, [](int) { return kLayoutBase; }) : TV{}; }
+    TV in0_view(char *base) const { return make_tv(base, B, net.h, net.w, net.c, net.c, P, ADT, 0); }
+    TV layout_in(int i) const { return i == 0 ? in0_view(kLayoutBase) : layout_view(i - 1); }
+    int in_dt(int i) const { return i == 0 ? ADT : L[i - 1].out_dt; }
+    TV side_view(int i, char *base) const {
+        const Layer &l = layer(i);
+        const int ld = L[i].side_ld;
+        if (L[i].side == SIDE_PM1_F32) return make_tv(base, B, l.h, l.w, l.c, ld, P, DT_F32, 0);
+        if (L[i].side == SIDE_S8) return make_tv(base, B, l.h, l.w, l.c, ld, P, DT_S8, 0);
+        return make_tv(base, B, l.h, l.w, ld, ld, P, DT_BITS, 0);
+    }
+    TV side_placed(int i) const { return side_view(i, e.act_arena + side_off[i]); }
+
+    // ---- pass 1: the layer plan ------------------------------------------------------------------------------------------
+    void plan_layers() {
+        bool any_xnor = false;
+        for (const Layer &l : net.layers) {
+            if (l.type != YB_CONVOLUTIONAL) continue;
+            if (l.batch_normalize) fatal_throw("engine: batch-norm not folded -- call yb_fuse_conv_batchnorm first");
+            if (l.xnor) {
+                any_xnor = true;
+                if (!l.has_mean_arr) fatal_throw("engine: xnor layer without mean_arr -- call yb_calculate_binary_weights first");
+            }
+            if (opt.qrule && !l.has_int8)
+                fatal_throw("engine: -quantized rule without int8 weights -- call yb_quantinization_and_get_multipliers first");
+        }
+        // f32 activations whenever an integer path must see exactly the reference's inputs
+        ADT = (opt.qrule || any_xnor || opt.precision == YB_PREC_FP32) ? DT_F32 : DT_BF16;
+        for (int i = 0; i < nl; ++i)
+            if (is_conv(i)) L[i].variant = conv_variant(i);
+
+        // conv i + same-shape shortcut i+1 whose only reader is that shortcut
+        if (opt.fuse) {
+            for (int i = 0; i + 1 < nl; ++i) {
+                const Layer &l = layer(i), &s = layer(i + 1);
+                if (l.type != YB_CONVOLUTIONAL || s.type != YB_SHORTCUT) continue;
+                if (L[i].variant != 0) continue;
+                if (l.stride != 1) continue;   // the tensor-core stride-2 path stores straddling tiles row by row, without a residual
+                if (!sole_reader(i, i + 1)) continue;
+                if (s.index == i) continue;
+                if (!(s.w == s.out_w && s.h == s.out_h && s.c == s.out_c)) continue;
+                L[i].fused_into = i + 1;
+                L[i + 1].fused_sc = true;
+            }
+        }
+
+        // output dtypes and homes (own buffer, or a channel slice of a concat buffer)
+        for (int i = 0; i < nl; ++i) {
+            const Layer &l = layer(i);
+            L[i].has_out = !(l.type == YB_YOLO || l.type == YB_REGION || l.type == YB_BLANK) && L[i].fused_into < 0 &&
+                           l.out_h > 0 && l.out_w > 0 && l.out_c > 0;
+            L[i].materialised = L[i].has_out;   // until a fusion below takes the output away
+            L[i].out_dt = ADT;
+            if (l.type == YB_CONVOLUTIONAL && !cons[i].empty()) {
+                bool all_final = true;
+                for (int c : cons[i]) if (layer(c).type != YB_YOLO && layer(c).type != YB_REGION) all_final = false;
+                if (all_final) L[i].out_dt = DT_F32;   // detection heads stay f32 (bf16 would cost ~1e-3 rel by itself)
+            }
+            if (l.type == YB_CONVOLUTIONAL && cons[i].empty()) L[i].out_dt = DT_F32;
+            // pixel stride rounded up to 8 channels: 16-byte aligned rows for TMA / vector stores (e.g. 255 -> 256)
+            L[i].ldc = (int)align_up(l.out_c, 8);
+        }
+        if (opt.fuse) {
+            for (int r = 0; r < nl; ++r) {
+                const Layer &l = layer(r);
+                if (l.type != YB_ROUTE || l.n < 2 || l.out_c <= 0) continue;
+                int off = 0;
+                for (int k = 0; k < l.n; ++k) {
+                    const int j = l.input_layers[k];
+                    if (L[j].has_out && L[j].owner < 0 && layer(j).type != YB_ROUTE && L[j].out_dt == ADT) {
+                        L[j].owner = r;
+                        L[j].coff = off;
+                    }
+                    off += layer(j).out_c;
+                }
+            }
+        }
+        for (int i = 0; i < nl; ++i)
+            if (L[i].has_out && is_alias(i)) L[i].out_dt = L[layer(i).input_layers[0]].out_dt;
+
+        // converted inputs of the integer paths
+        for (int i = 0; i < nl; ++i) {
+            if (!is_conv(i)) continue;
+            const Layer &l = layer(i);
+            LayerPlan &p = L[i];
+            if (p.variant == 1 && xnor_fallback(l)) { p.side = SIDE_PM1_F32; p.side_ld = l.c; }
+            else if (p.variant == 1 && xnor_on_tc(l)) { p.side = SIDE_S8; p.side_ld = (int)align_up(l.c, 32); }   // pad channels meet zero weights
+            else if (p.variant == 1) { p.side = SIDE_BITS; p.side_ld = (l.c + 31) / 32; }
+            else if (p.variant == 2) { p.side = SIDE_S8; p.side_ld = (int)align_up(l.c, 32); }   // every INT8 layer fits the s8 wgmma tile
+        }
+
+        for (int i = 0; i < nl; ++i)
+            if (is_conv(i)) L[i].path = conv_path(i);
+        plan_first_op();
+        plan_fusions();
+        for (int i = 0; i < nl; ++i)
+            if (is_alias(i)) L[i].materialised = L[i].has_out && L[layer(i).input_layers[0]].materialised;
+    }
+
+    int conv_path(int i) const {
+        const Layer &l = layer(i);
+        const LayerPlan &p = L[i];
+        const int tgt = p.fused_into >= 0 ? p.fused_into : i;
+        const TV tin = layout_in(i), tout = layout_view(tgt);
+        const int idt = in_dt(i), odt = L[tgt].out_dt;
+        if (p.variant == 0) {
+            int tc = (ADT == DT_BF16 && idt == DT_BF16) ? tc_conv_supported(l, tin, tout, odt == DT_BF16) : 0;
+            // float detection heads of the INT8 / XNOR networks (default precision): tf32 wgmma.  Only layers whose every
+            // reader is a yolo / region layer -- nothing they compute can reach an integer layer.
+            if (ADT == DT_F32 && opt.precision == YB_PREC_BF16_TC && idt == DT_F32 && odt == DT_F32 && p.fused_into < 0 &&
+                !cons[i].empty() && !sw.no_tf32) {
+                bool heads_only = true;
+                for (int r : cons[i]) heads_only &= layer(r).type == YB_YOLO || layer(r).type == YB_REGION;
+                if (heads_only && tc_tf32_supported(l, tin, tout)) tc = 2;
+            }
+            if (sw.no_tc) tc = 0;
+            return tc == 2 ? CP_TF32 : tc ? CP_TC : CP_SIMT;
+        }
+        if (idt != DT_F32 || odt != DT_F32)
+            fatal_throw(p.variant == 1 ? "engine: xnor path needs f32 activations" : "engine: int8 path needs f32 activations");
+        if (p.variant == 2) return (!sw.no_tc && tc_i8_supported(l, side_view(i, kLayoutBase), tout)) ? CP_I8_TC : CP_I8_SIMT;
+        if (xnor_fallback(l)) return CP_XNOR_FALLBACK;
+        if (xnor_on_tc(l) && vec4_view(tin)) {
+            if (!tc_i8_supported(l, side_view(i, kLayoutBase), tout)) fatal_throw("engine: xnor tensor-core layer not supported by the i8 tile");
+            return CP_XNOR_TC;
+        }
+        // small K: one thread per pixel, all filters (weights broadcast from shared memory)
+        const int CW = p.side_ld;
+        if (CW <= 2 && l.size == 3 && (size_t)l.n * 9 * CW * 4 <= 40 * 1024 && tout.ldc % 4 == 0) return CP_XNOR_SMALLK;
+        return CP_XNOR_GENERAL;
+    }
+
+    // ops[0] consumes the caller's NCHW f32 images.  Usually that is the stem convolution itself (3 input channels, 3x3/1/1),
+    // reading NCHW directly; otherwise a plain NCHW -> padded-NHWC conversion.
+    void plan_first_op() {
+        const Layer &l0 = layer(0);
+        const TV out0 = layout_view(0);
+        const bool stem_ok = l0.type == YB_CONVOLUTIONAL && L[0].variant == 0 && L[0].path == CP_SIMT && l0.c == 3 &&
+                             l0.size == 3 && l0.stride == 1 && l0.pad == 1 && (l0.n == 16 || l0.n == 32) && L[0].fused_into < 0 &&
+                             L[0].has_out && !sw.no_stem && (L[0].out_dt == DT_F32 || out0.ldc % 8 == 0);
+        // exact nets: stem + 2x2/2 max-pool + the integer layer's input conversion in one kernel (k_stem_pool): layers 0 and 1
+        // are then never written to HBM
+        bool pool_ok = stem_ok && opt.fuse && L[0].out_dt == DT_F32 && l0.n == 16 && nl > 2 && !sw.no_stem_pool_fuse &&
+                       (l0.activation == YB_LEAKY || l0.activation == YB_LINEAR);
+        if (pool_ok) {
+            const Layer &mp = layer(1), &c2 = layer(2);
+            pool_ok = mp.type == YB_MAXPOOL && mp.size == 2 && mp.stride == 2 && mp.pad == 1 && sole_reader(0, 1) &&
+                      sole_reader(1, 2) && c2.type == YB_CONVOLUTIONAL && L[2].variant != 0 && L[2].side != SIDE_NONE &&
+                      !xnor_fallback(c2) && (L[2].side == SIDE_BITS || L[2].side_ld % 16 == 0);
+        }
+        if (pool_ok) {
+            first = FIRST_STEM_POOL;
+        } else if (stem_ok && L[0].out_dt == DT_BF16 && tc_stem_supported(l0, out0) && !sw.no_stem_tc) {
+            // tensor-core stem: gathers the 3x3x3 window from NCHW, K padded 27 -> 32.  When layer 1 is a bf16 tensor-core
+            // 3x3 / stride-2 convolution 32 -> 64 and the stem's only reader, both run as one kernel (k_stem_s2_tc) and the
+            // stem output is never written.
+            const bool s2 = opt.fuse && !sw.no_stem_s2_fuse && nl > 1 && sole_reader(0, 1) && is_conv(1) && L[1].variant == 0 &&
+                            L[1].path == CP_TC && L[1].fused_into < 0 && L[1].out_dt == DT_BF16 &&
+                            tc_stem_s2_supported(l0, layer(1), layout_view(1));
+            first = s2 ? FIRST_STEM_S2 : FIRST_STEM_TC;
+        } else if (stem_ok) {
+            first = FIRST_STEM_SIMT;
+        }
+        if (first != FIRST_NHWC) L[0].in_first_op = true;
+        if (first == FIRST_STEM_S2 || first == FIRST_STEM_POOL) {
+            L[0].materialised = false;
+            L[1].in_first_op = true;
+        }
+        if (first == FIRST_STEM_POOL) {
+            L[1].materialised = false;
+            L[2].prefilled = true;
+        }
+    }
+
+    // the fusions in the op list behind the first op
+    void plan_fusions() {
+        for (int i = 0; i < nl; ++i) {
+            LayerPlan &p = L[i];
+            if (!is_conv(i) || p.in_first_op) continue;
+            // max-pool i+1 and layer i+2's input conversion in the epilogue
+            const int pm = conv_pool_mode(i);
+            bool pool = false;
+            if (p.path == CP_XNOR_TC || p.path == CP_I8_TC) {
+                p.pool_tile = pm != 0;
+                pool = pm != 0 && tc_pool_fuse_supported(layer(i), side_view(i + 2, kLayoutBase));
+            } else if (p.path == CP_XNOR_SMALLK) {
+                pool = pm == 2 || pm == 3;
+            }
+            if (pool) {
+                p.pool_mode = pm;
+                L[i + 1].pool_in_conv = L[i + 2].prefilled = true;
+                p.materialised = L[i + 1].materialised = false;
+            }
+            // detection-head conv i + [yolo] i+1: logistic and NCHW store in the epilogue
+            if ((p.path == CP_TF32 || p.path == CP_TC) && opt.fuse && p.fused_into < 0 && p.out_dt == DT_F32 && i + 1 < nl &&
+                layer(i + 1).type == YB_YOLO && sole_reader(i, i + 1) && !sw.no_yolo_fuse) {
+                p.yolo_fused = L[i + 1].yolo_fused = true;
+                p.materialised = false;
+            }
+        }
+        // max-pool -> integer convolution: the pool writes the convolution's s8 / sign input directly (same values in the same
+        // order as max-pool + quantise / binarise; the pooled f32 tensor never goes to HBM)
+        for (int i = 0; i + 1 < nl; ++i) {
+            if (layer(i).type != YB_MAXPOOL || L[i].in_first_op || L[i].pool_in_conv) continue;
+            const Layer &c = layer(i + 1);
+            if (opt.fuse && in_dt(i) == DT_F32 && sole_reader(i, i + 1) && c.type == YB_CONVOLUTIONAL && L[i + 1].variant != 0 &&
+                L[i + 1].side != SIDE_NONE && !xnor_fallback(c) && !sw.no_pool_fuse) {
+                L[i].pool_to_side = L[i + 1].prefilled = true;
+                L[i].materialised = false;
+            }
+        }
+    }
+
+    // ---- pass 2: placement -----------------------------------------------------------------------------------------------
+    void place() {
+        size_t total = 0;
+        auto take = [&](size_t bytes) { const size_t off = total; total += align_up(bytes, 1024); return off; };
+        const size_t in0_off = first == FIRST_NHWC ? take(tv_bytes(B, net.h, net.w, net.c, P, ADT)) : 0;
+        for (int i = 0; i < nl; ++i) {
+            const Layer &l = layer(i);
+            if (L[i].materialised && !is_alias(i) && L[i].owner < 0)
+                buf_off[i] = take(tv_bytes(B, l.out_h, l.out_w, L[i].ldc, P, L[i].out_dt));
+        }
+        for (int i = 0; i < nl; ++i) {
+            const Layer &l = layer(i);
+            const int sdt = L[i].side == SIDE_PM1_F32 ? DT_F32 : L[i].side == SIDE_S8 ? DT_S8 : DT_BITS;
+            if (L[i].side != SIDE_NONE) side_off[i] = take(tv_bytes(B, l.h, l.w, L[i].side_ld, P, sdt));
+        }
+        e.act_bytes = total;
+        CUDA_OK(cudaMalloc(&e.act_arena, total));
+        CUDA_OK(cudaMemsetAsync(e.act_arena, 0, total, e.stream));   // zero borders, once
+        for (int i = 0; i < nl; ++i)   // +-1 activation buffers: borders are -1 (out-of-image taps count as -1, SURVEY F9)
+            if (L[i].variant == 1 && L[i].side == SIDE_S8)
+                CUDA_OK(cudaMemsetAsync(e.act_arena + side_off[i], 0xFF, tv_bytes(B, layer(i).h, layer(i).w, L[i].side_ld, P, DT_S8), e.stream));
+        e.in0 = first == FIRST_NHWC ? in0_view(e.act_arena + in0_off) : TV{};
+        e.in0_dt = ADT;
+        e.act_dt = ADT;
+        e.out_tv.assign(nl, TV{});
+        e.out_dt.assign(nl, ADT);
+        for (int i = 0; i < nl; ++i) {
+            e.out_dt[i] = L[i].out_dt;
+            if (L[i].materialised) e.out_tv[i] = out_view(i, [&](int j) { return e.act_arena + buf_off[j]; });
+        }
+    }
+
+    // detection-layer outputs, and the last layer's output whatever its type (the reference returns it)
+    void place_finals() {
+        e.d_final.assign(nl, nullptr);
+        e.h_final.assign(nl, nullptr);
+        e.final_count.assign(nl, 0);
+        e.d_counts.assign(nl, nullptr);
+        e.counts_count.assign(nl, 0);
+        for (int i = 0; i < nl; ++i) {
+            const Layer &l = layer(i);
+            if (!(l.type == YB_YOLO || l.type == YB_REGION || (i == nl - 1 && l.outputs > 0))) continue;
+            e.final_count[i] = (size_t)l.outputs * B;
+            CUDA_OK(cudaMalloc(&e.d_final[i], e.final_count[i] * sizeof(float)));
+            CUDA_OK(cudaHostAlloc(&e.h_final[i], e.final_count[i] * sizeof(float), cudaHostAllocDefault));
+        }
+    }
+
+    // ---- pass 3: weights -------------------------------------------------------------------------------------------------
+    void pack_weights() {
+        std::vector<char> hostw;
+        auto reserve = [&](size_t bytes) { size_t off = align_up(hostw.size(), 1024); hostw.resize(off + bytes, 0); return off; };
+        for (int i = 0; i < nl; ++i) {
+            if (!is_conv(i)) continue;
+            const Layer &l = layer(i);
+            const LayerPlan &p = L[i];
+            const int taps = l.size * l.size, K = taps * l.c;
+            ConvWeights &w = cw[i];
+            w.bias = reserve(sizeof(float) * align_up(l.n, 64));
+            memcpy(&hostw[w.bias], l.biases.data(), sizeof(float) * l.n);
+            w.ldn = (int)align_up(l.n, 64);
+            if (p.path == CP_TF32) {
+                // f32 [ldn][K], K ordered (ky, kx, c)
+                w.w_f32km = reserve(sizeof(float) * (size_t)w.ldn * K);
+                float *dst = reinterpret_cast<float *>(&hostw[w.w_f32km]);
+                for_each_weight(l, [&](int f, int c, int t, size_t k) { dst[(size_t)f * K + (size_t)t * l.c + c] = l.weights[k]; });
+            } else if (p.path == CP_TC) {
+                // bf16 [ldn][K], K ordered (ky, kx, c): the K-major B operand of the implicit GEMM
+                w.w_bf16 = reserve(sizeof(__nv_bfloat16) * (size_t)w.ldn * K);
+                __nv_bfloat16 *dst = reinterpret_cast<__nv_bfloat16 *>(&hostw[w.w_bf16]);
+                for_each_weight(l, [&](int f, int c, int t, size_t k) {
+                    dst[(size_t)f * K + (size_t)t * l.c + c] = __float2bfloat16_rn(l.weights[k]); });
+            } else if (p.variant == 0) {
+                // f32 [K][ldw]; K ordered (ky, kx, c), or -- f32 activations: the exact order of the reference's gemm_nn
+                // (k_conv_simt<EXACT>) -- (c, ky, kx)
+                w.ldw = w.ldn;
+                w.w_f32 = reserve(sizeof(float) * (size_t)K * w.ldw);
+                float *dst = reinterpret_cast<float *>(&hostw[w.w_f32]);
+                for_each_weight(l, [&](int f, int c, int t, size_t k) {
+                    dst[(ADT == DT_F32 ? (size_t)c * taps + t : (size_t)t * l.c + c) * w.ldw + f] = l.weights[k]; });
+            } else if (p.side == SIDE_PM1_F32) {
+                // f32 [K][ldw], K in the reference's (c, ky, kx) order: +mean where w > 0, -mean otherwise (binarize_weights)
+                w.ldw = w.ldn;
+                w.w_f32 = reserve(sizeof(float) * (size_t)K * w.ldw);
+                float *dst = reinterpret_cast<float *>(&hostw[w.w_f32]);
+                for_each_weight(l, [&](int f, int c, int t, size_t k) {
+                    dst[((size_t)c * taps + t) * w.ldw + f] = l.weights[k] > 0 ? l.mean_arr[f] : -l.mean_arr[f]; });
+            } else if (p.side == SIDE_BITS) {
+                // sign bits [ldn][taps][CW]; bit = (w > 0) (binarize_weights additionally.c:113 + float_to_bit :1536)
+                const int CW = p.side_ld;
+                w.cpad = CW * 32;
+                w.w_bits = reserve(sizeof(uint32_t) * (size_t)w.ldn * taps * CW);
+                uint32_t *dst = reinterpret_cast<uint32_t *>(&hostw[w.w_bits]);
+                for_each_weight(l, [&](int f, int c, int t, size_t k) {
+                    if (l.weights[k] > 0) dst[((size_t)f * taps + t) * CW + c / 32] |= 1u << (c & 31); });
+            } else {
+                // s8 [ldn][taps][cpad], zero channel padding and zero padded filter rows: INT8 weights, or XNOR weights as
+                // +1 where w > 0 and -1 otherwise
+                w.cpad = p.side_ld;
+                w.w_s8 = reserve((size_t)w.ldn * taps * w.cpad);
+                int8_t *dst = reinterpret_cast<int8_t *>(&hostw[w.w_s8]);
+                for_each_weight(l, [&](int f, int c, int t, size_t k) {
+                    dst[((size_t)f * taps + t) * w.cpad + c] = p.variant == 2 ? l.weights_int8[k] : l.weights[k] > 0 ? 1 : -1; });
+            }
+            if (p.variant == 1 && p.side != SIDE_PM1_F32) {
+                w.mean = reserve(sizeof(float) * align_up(l.n, 64));
+                memcpy(&hostw[w.mean], l.mean_arr.data(), sizeof(float) * l.n);
+            }
+        }
+        if (first == FIRST_STEM_TC || first == FIRST_STEM_S2) {
+            // bf16 [32 filters][32], K = (ky, kx, c) padded 27 -> 32
+            stem_w_off = reserve(sizeof(__nv_bfloat16) * 32 * 32);
+            __nv_bfloat16 *dst = reinterpret_cast<__nv_bfloat16 *>(&hostw[stem_w_off]);
+            for (int k = 0; k < 32 * 32; ++k) dst[k] = __float2bfloat16_rn(0.f);
+            const Layer &l0 = layer(0);
+            for_each_weight(l0, [&](int f, int c, int t, size_t k) { dst[f * 32 + t * 3 + c] = __float2bfloat16_rn(l0.weights[k]); });
+        }
+        e.w_bytes = align_up(std::max<size_t>(hostw.size(), 1024), 1024);
+        CUDA_OK(cudaMalloc(&e.w_arena, e.w_bytes));
+        if (opt.upload) CUDA_OK(cudaMemcpyAsync(e.w_arena, hostw.data(), hostw.size(), cudaMemcpyHostToDevice, e.stream));
+        CUDA_OK(cudaStreamSynchronize(e.stream));   // hostw goes out of scope below
+    }
+
+    // ---- pass 4: op emission ---------------------------------------------------------------------------------------------
+    const float *bias(int i) const { return reinterpret_cast<const float *>(e.w_arena + cw[i].bias); }
+    void push(int kind, int i, std::function<void(cudaStream_t)> f) { e.ops.push_back(Op{kind, i, std::move(f)}); }
+
+    // a tensor-core plan of layer i, with the [yolo] layer or the max-pool the plan decided to fuse
+    void push_tc_plan(int kind, int i, void *plan) {
+        e.tc_plans.push_back(plan);
+        if (kind == OP_CONV_TC || kind == OP_CONV_TC_TF32) ++e.n_tc;
+        if (L[i].yolo_fused) tc_plan_fuse_yolo(plan, e.d_final[i + 1], layer(i + 1).classes);
+        if (const int pm = L[i].pool_mode) tc_plan_fuse_pool(plan, pm, pm == 1 ? layer(i + 2).input_quant_multipler : 0.f, side_placed(i + 2));
+        push(kind, i, [plan](cudaStream_t s) { tc_launch(plan, s); });
+    }
+
+    int32_t *counts_buffer(int i) {   // raw XNOR popcounts / INT8 accumulators (keep_counts)
+        if (!opt.keep_counts) return nullptr;
+        const Layer &l = layer(i);
+        e.counts_count[i] = (size_t)B * l.n * l.out_h * l.out_w;
+        CUDA_OK(cudaMalloc(&e.d_counts[i], e.counts_count[i] * sizeof(int32_t)));
+        return e.d_counts[i];
+    }
+
+    void emit_first() {
+        const Layer &l0 = layer(0);
+        const int act = l0.activation, H = l0.h, W = l0.w;
+        e.first_kind = OP_CONV_SIMT;
+        e.first_layer = 0;
+        if (first == FIRST_STEM_POOL) {
+            const Layer &c2 = layer(2);
+            const int v2 = L[2].variant;
+            const bool pm1 = v2 == 1 && L[2].side == SIDE_S8;   // next layer reads +-1 bytes
+            const TV q = side_placed(2);
+            const StemW<16> w16 = stem_weights<16>(l0);
+            const float mult = (v2 == 2) ? c2.input_quant_multipler : 0.f;
+            const int grid = (int)(((long)B * c2.h * c2.w + 127) / 128);
+            e.first_op = [=](const float *din, cudaStream_t s) {
+                if (v2 == 2 && act == ACT_LEAKY) k_stem_pool<0, ACT_LEAKY><<<grid, 128, 0, s>>>(din, q, w16, act, H, W, mult);
+                else if (v2 == 2) k_stem_pool<0, ACT_LINEAR><<<grid, 128, 0, s>>>(din, q, w16, act, H, W, mult);
+                else if (pm1 && act == ACT_LEAKY) k_stem_pool<1, ACT_LEAKY><<<grid, 128, 0, s>>>(din, q, w16, act, H, W, mult);
+                else if (pm1) k_stem_pool<1, ACT_LINEAR><<<grid, 128, 0, s>>>(din, q, w16, act, H, W, mult);
+                else if (act == ACT_LEAKY) k_stem_pool<2, ACT_LEAKY><<<grid, 128, 0, s>>>(din, q, w16, act, H, W, mult);
+                else k_stem_pool<2, ACT_LINEAR><<<grid, 128, 0, s>>>(din, q, w16, act, H, W, mult);
+            };
+        } else if (first == FIRST_STEM_TC || first == FIRST_STEM_S2) {
+            void *sp = first == FIRST_STEM_S2
+                ? tc_stem_s2_make_plan(l0, layer(1), e.out_tv[1], e.w_arena + stem_w_off, bias(0), e.w_arena + cw[1].w_bf16, bias(1))
+                : tc_stem_make_plan(l0, e.out_tv[0], e.w_arena + stem_w_off, bias(0));
+            e.stem_plan = sp;
+            e.first_kind = OP_CONV_TC;
+            if (first == FIRST_STEM_S2) {
+                e.first_layer = 1;
+                ++e.n_tc;
+            }
+            e.first_op = [sp](const float *din, cudaStream_t s) { tc_stem_launch(sp, din, s); };
+            if (!sw.no_stem_u8) e.first_op_u8 = [sp](const unsigned char *d8, cudaStream_t s) { tc_stem_launch_u8(sp, d8, s); };
+        } else if (first == FIRST_STEM_SIMT) {
+            const TV tout = e.out_tv[0];
+            const int nf = l0.n, odt = L[0].out_dt;
+            const StemW<32> w32 = nf == 32 ? stem_weights<32>(l0) : StemW<32>{};
+            const StemW<16> w16 = nf == 16 ? stem_weights<16>(l0) : StemW<16>{};
+            const int grid = (int)(((long)B * H * W + 127) / 128);
+            e.first_op = [=](const float *din, cudaStream_t s) {
+                if (nf == 32 && odt == DT_BF16) k_conv_stem<32, __nv_bfloat16><<<grid, 128, 0, s>>>(din, tout, w32, act, H, W);
+                else if (nf == 32) k_conv_stem<32, float, true><<<grid, 128, 0, s>>>(din, tout, w32, act, H, W);
+                else if (odt == DT_BF16) k_conv_stem<16, __nv_bfloat16><<<grid, 128, 0, s>>>(din, tout, w16, act, H, W);
+                else k_conv_stem<16, float, true><<<grid, 128, 0, s>>>(din, tout, w16, act, H, W);
+            };
+        } else {
+            const TV in0 = e.in0;
+            const int dt = ADT;
+            const int g = grid_for((long)in0.N * in0.H * in0.W);
+            e.first_kind = OP_INPUT;
+            e.first_layer = -1;
+            e.first_op = [=](const float *din, cudaStream_t s) {
+                if (dt == DT_F32) k_input_nchw_to_nhwc<float><<<g, 256, 0, s>>>(din, in0);
+                else k_input_nchw_to_nhwc<__nv_bfloat16><<<g, 256, 0, s>>>(din, in0);
+            };
+        }
+        push(e.first_kind, e.first_layer, nullptr);   // launched specially: pointer varies per call
+    }
+
+    void need_input(int i) const {
+        if (i > 0 && !L[i - 1].has_out) fatal_throw("engine: layer " + std::to_string(i) + " has no image input");
+    }
+
+    void emit_conv(int i) {
+        const Layer &l = layer(i);
+        need_input(i);
+        const int tgt = L[i].fused_into >= 0 ? L[i].fused_into : i;
+        if (!L[tgt].has_out) fatal_throw("engine: conv output not placed");
+        const int in_c = i == 0 ? net.c : layer(i - 1).out_c, in_h = i == 0 ? net.h : layer(i - 1).out_h,
+                  in_w = i == 0 ? net.w : layer(i - 1).out_w;
+        if (in_c != l.c || in_h != l.h || in_w != l.w) fatal_throw("engine: conv input shape mismatch");
+        const TV tin = i == 0 ? e.in0 : e.out_tv[i - 1];   // no base where the input is fused away
+        if (L[i].variant == 0) emit_conv_fp32(i, tin);
+        else if (L[i].variant == 1) emit_conv_xnor(i, tin);
+        else emit_conv_int8(i, tin);
+    }
+
+    void emit_conv_fp32(int i, const TV &tin) {
+        const Layer &l = layer(i);
+        const LayerPlan &p = L[i];
+        const int tgt = p.fused_into >= 0 ? p.fused_into : i;
+        const TV tout = e.out_tv[tgt];   // no base where the [yolo] layer is fused
+        const int odt = L[tgt].out_dt;
+        TV res{}; int rdt = DT_F32; int act2 = ACT_LINEAR;
+        if (p.fused_into >= 0) {
+            const Layer &s = layer(tgt);
+            res = e.out_tv[s.index];
+            rdt = L[s.index].out_dt;
+            act2 = s.activation;
+            if (!res.base) fatal_throw("engine: shortcut source not placed");
+        }
+        if (p.path == CP_TF32) {
+            push_tc_plan(OP_CONV_TC_TF32, i, tc_make_plan_tf32(l, tin, tout, e.w_arena + cw[i].w_f32km, cw[i].ldn, bias(i), p.yolo_fused));
+            return;
+        }
+        if (p.path == CP_TC) {
+            push_tc_plan(OP_CONV_TC, i, tc_make_plan(l, tin, tout, odt == DT_BF16, res, rdt == DT_BF16, act2, e.w_arena + cw[i].w_bf16,
+                                                     cw[i].ldn, bias(i), p.yolo_fused));
+            return;
+        }
+        const long M = (long)B * l.out_h * l.out_w;
+        ConvP cp{};
+        cp.in = tin; cp.out = tout; cp.res = res;
+        cp.w = e.w_arena + cw[i].w_f32;
+        cp.bias = bias(i);
+        cp.n = l.n; cp.ldw = cw[i].ldw; cp.size = l.size; cp.stride = l.stride; cp.pad = l.pad;
+        cp.act = l.activation; cp.act2 = act2; cp.K = l.size * l.size * l.c; cp.M = M;
+        dim3 grid((unsigned)((M + 63) / 64), (unsigned)((l.n + 63) / 64));
+        const int key = in_dt(i) * 4 + odt * 2 + rdt;
+        push(OP_CONV_SIMT, i, [cp, grid, key](cudaStream_t s) {
+            switch (key) {
+            case 0: k_conv_simt<float, float, float, true><<<grid, 256, 0, s>>>(cp); break;   // reference order, bit-exact
+            case 1: k_conv_simt<float, float, __nv_bfloat16><<<grid, 256, 0, s>>>(cp); break;
+            case 2: k_conv_simt<float, __nv_bfloat16, float><<<grid, 256, 0, s>>>(cp); break;
+            case 3: k_conv_simt<float, __nv_bfloat16, __nv_bfloat16><<<grid, 256, 0, s>>>(cp); break;
+            case 4: k_conv_simt<__nv_bfloat16, float, float><<<grid, 256, 0, s>>>(cp); break;
+            case 5: k_conv_simt<__nv_bfloat16, float, __nv_bfloat16><<<grid, 256, 0, s>>>(cp); break;
+            case 6: k_conv_simt<__nv_bfloat16, __nv_bfloat16, float><<<grid, 256, 0, s>>>(cp); break;
+            default: k_conv_simt<__nv_bfloat16, __nv_bfloat16, __nv_bfloat16><<<grid, 256, 0, s>>>(cp); break;
+            }
+        });
+    }
+
+    void emit_conv_xnor(int i, const TV &tin) {
+        const Layer &l = layer(i);
+        const LayerPlan &p = L[i];
+        const TV tout = e.out_tv[i];   // no base where the max-pool behind it is fused
+        const long M = (long)B * l.out_h * l.out_w;
+        if (p.path == CP_XNOR_FALLBACK) {
+            const TV pm1 = side_placed(i);
+            const int gb = grid_for((long)B * l.h * l.w * l.c);
+            push(OP_BINARIZE, i, [tin, pm1, gb](cudaStream_t s) { k_binarize_pm1<<<gb, 256, 0, s>>>(tin, pm1); });
+            ConvP cp{};
+            cp.in = pm1; cp.out = tout; cp.res = TV{};
+            cp.w = e.w_arena + cw[i].w_f32;
+            cp.bias = bias(i);
+            cp.n = l.n; cp.ldw = cw[i].ldw; cp.size = l.size; cp.stride = l.stride; cp.pad = l.pad;
+            cp.act = l.activation; cp.act2 = ACT_LINEAR; cp.K = l.size * l.size * l.c; cp.M = M;
+            dim3 grid((unsigned)((M + 63) / 64), (unsigned)((l.n + 63) / 64));
+            push(OP_CONV_SIMT, i, [cp, grid](cudaStream_t s) { k_conv_simt<float, float, float, true><<<grid, 256, 0, s>>>(cp); });
+            return;
+        }
+        int32_t *cnt_dbg = counts_buffer(i);
+        if (p.path == CP_XNOR_TC) {
+            const TV q = side_placed(i);
+            const int g = grid_for((long)B * l.h * l.w * (l.c / 16));
+            if (!p.prefilled) push(OP_BINARIZE, i, [tin, q, g](cudaStream_t s) { k_binarize_s8<<<g, 256, 0, s>>>(tin, q); });
+            push_tc_plan(OP_CONV_TC_I8, i, tc_make_plan_xnor(l, q, tout, e.w_arena + cw[i].w_s8, cw[i].ldn, bias(i),
+                                                             reinterpret_cast<const float *>(e.w_arena + cw[i].mean), cnt_dbg, p.pool_tile));
+            return;
+        }
+        const int CW = p.side_ld;
+        const TV bits = make_tv(e.act_arena + side_off[i], B, l.h, l.w, CW, CW, P, DT_BITS, 0);
+        if (!p.prefilled) {
+            if (vec4_view(tin)) {
+                const int g = grid_for((long)B * l.h * l.w * CW);
+                push(OP_BINARIZE, i, [tin, bits, g](cudaStream_t s) { k_binarize_vec<float><<<g, 256, 0, s>>>(tin, bits); });
+            } else {
+                const int g = grid_for((long)B * l.h * l.w * CW * 32);
+                push(OP_BINARIZE, i, [tin, bits, g](cudaStream_t s) { k_binarize<float><<<g, 256, 0, s>>>(tin, bits); });
+            }
+        }
+        XnorP xp{};
+        xp.bits = bits; xp.out = tout;
+        xp.w = reinterpret_cast<const uint32_t *>(e.w_arena + cw[i].w_bits);
+        xp.mean = reinterpret_cast<const float *>(e.w_arena + cw[i].mean);
+        xp.bias = bias(i);
+        xp.n = l.n; xp.size = l.size; xp.pad = l.pad; xp.K = l.size * l.size * l.c;
+        xp.padbits = (CW * 32 - l.c) * l.size * l.size;
+        xp.act = l.activation; xp.M = M; xp.counts = cnt_dbg;
+        if (p.path == CP_XNOR_GENERAL) {
+            dim3 grid((unsigned)((M + 63) / 64), (unsigned)((l.n + 63) / 64));
+            push(OP_CONV_XNOR, i, [xp, grid](cudaStream_t s) { k_conv_xnor<<<grid, 256, 0, s>>>(xp); });
+            return;
+        }
+        const size_t smem = (size_t)l.n * 9 * CW * 4;
+        if (const int pm = p.pool_mode) {
+            // the 2x2 max-pool behind this layer and the next XNOR layer's sign extraction run in this kernel, which reads only
+            // the shape of the output it does not write
+            xp.out = make_tv(nullptr, B, l.out_h, l.out_w, l.n, L[i].ldc, P, DT_F32, 0);
+            const Layer &c2 = layer(i + 2);
+            const TV qn = side_placed(i + 2);
+            const unsigned gp = (unsigned)(((long)B * c2.h * c2.w + 127) / 128);
+            push(OP_CONV_XNOR, i, [xp, qn, gp, smem, CW, pm](cudaStream_t s) {
+                if (CW == 1 && pm == 2) k_conv_xnor_smallk_pool<1, 2><<<gp, 128, smem, s>>>(xp, qn);
+                else if (CW == 1) k_conv_xnor_smallk_pool<1, 3><<<gp, 128, smem, s>>>(xp, qn);
+                else if (pm == 2) k_conv_xnor_smallk_pool<2, 2><<<gp, 128, smem, s>>>(xp, qn);
+                else k_conv_xnor_smallk_pool<2, 3><<<gp, 128, smem, s>>>(xp, qn);
+            });
+            return;
+        }
+        const unsigned gsm = (unsigned)((M + 127) / 128);
+        push(OP_CONV_XNOR, i, [xp, gsm, smem, CW](cudaStream_t s) {
+            if (CW == 1) k_conv_xnor_smallk<1><<<gsm, 128, smem, s>>>(xp);
+            else k_conv_xnor_smallk<2><<<gsm, 128, smem, s>>>(xp);
+        });
+    }
+
+    void emit_conv_int8(int i, const TV &tin) {
+        const Layer &l = layer(i);
+        const LayerPlan &p = L[i];
+        const TV tout = e.out_tv[i];   // no base where the max-pool behind it is fused
+        const TV q = side_placed(i);
+        const float mult = l.input_quant_multipler;
+        const int g = grid_for((long)B * l.h * l.w * (p.side_ld / 4));
+        if (!p.prefilled) push(OP_QUANTIZE, i, [tin, q, mult, g](cudaStream_t s) { k_quantize<float><<<g, 256, 0, s>>>(tin, q, mult); });
+        int *acc_dbg = counts_buffer(i);
+        const float alpha1 = 32 / (l.input_quant_multipler * l.weights_quant_multipler);   // ALPHA1, ..._quantized.c:598
+        if (p.path == CP_I8_TC) {
+            // s8 x s8 -> s32 on the s8 wgmma; weights [ldn][taps][cpad] are already K-major
+            push_tc_plan(OP_CONV_TC_I8, i, tc_make_plan_i8(l, q, tout, e.w_arena + cw[i].w_s8, cw[i].ldn, bias(i), alpha1, acc_dbg, p.pool_tile));
+            return;
+        }
+        const long M = (long)B * l.out_h * l.out_w;
+        Int8P ip{};
+        ip.q = q; ip.out = tout;
+        ip.w = reinterpret_cast<const uint32_t *>(e.w_arena + cw[i].w_s8);
+        ip.bias = bias(i);
+        ip.alpha1 = alpha1;
+        ip.n = l.n; ip.size = l.size; ip.stride = l.stride; ip.pad = l.pad; ip.act = l.activation;
+        ip.CW = p.side_ld / 4; ip.M = M; ip.acc_out = acc_dbg;
+        dim3 grid((unsigned)((M + 63) / 64), (unsigned)((l.n + 63) / 64));
+        push(OP_CONV_INT8, i, [ip, grid](cudaStream_t s) { k_conv_int8_simt<<<grid, 256, 0, s>>>(ip); });
+    }
+
+    // max-pool, upsample, shortcut, route, reorg, yolo, region
+    void emit_small(int i) {
+        const Layer &l = layer(i);
+        const LayerPlan &p = L[i];
+        const TV tin = i == 0 ? e.in0 : e.out_tv[i - 1];
+        const int dt = in_dt(i);
+        const TV tout = e.out_tv[i];
+        const int g = grid_for((long)B * l.out_h * l.out_w * l.out_c);
+        switch (l.type) {
+        case YB_MAXPOOL: {
+            if (p.pool_in_conv) break;    // done in the epilogue of the integer convolution in front of it
+            need_input(i);
+            const int size = l.size, stride = l.stride, pad = l.pad;
+            if (p.pool_to_side) {
+                const Layer &c = layer(i + 1);
+                const TV q = side_placed(i + 1);
+                const float mult = c.input_quant_multipler;
+                if (L[i + 1].side == SIDE_BITS) {
+                    const int gb = grid_for((long)B * c.h * c.w * q.ldc);
+                    push(OP_MAXPOOL, i, [tin, q, size, stride, pad, gb](cudaStream_t s) {
+                        k_maxpool_fused<2><<<gb, 256, 0, s>>>(tin, q, size, stride, pad, 0.f); });
+                } else {
+                    const int gq = grid_for((long)B * c.h * c.w * (q.ldc / 4));
+                    if (L[i + 1].variant == 2)
+                        push(OP_MAXPOOL, i, [tin, q, size, stride, pad, mult, gq](cudaStream_t s) {
+                            k_maxpool_fused<0><<<gq, 256, 0, s>>>(tin, q, size, stride, pad, mult); });
+                    else
+                        push(OP_MAXPOOL, i, [tin, q, size, stride, pad, gq](cudaStream_t s) {
+                            k_maxpool_fused<1><<<gq, 256, 0, s>>>(tin, q, size, stride, pad, 0.f); });
+                }
+                break;
+            }
+            const int esz = (int)dt_size(dt);
+            const bool vec = (l.out_c * esz) % 16 == 0 && (tin.ldc * esz) % 16 == 0 && (tout.ldc * esz) % 16 == 0 &&
+                             (reinterpret_cast<uintptr_t>(tin.base) & 15) == 0 && (reinterpret_cast<uintptr_t>(tout.base) & 15) == 0;
+            const int gv = grid_for((long)B * l.out_h * l.out_w * ((l.out_c * esz) / 16 + 1));
+            push(OP_MAXPOOL, i, [tin, tout, size, stride, pad, g, dt, vec, gv](cudaStream_t s) {
+                if (vec && dt == DT_F32) k_maxpool_vec<float><<<gv, 256, 0, s>>>(tin, tout, size, stride, pad);
+                else if (vec) k_maxpool_vec<__nv_bfloat16><<<gv, 256, 0, s>>>(tin, tout, size, stride, pad);
+                else if (dt == DT_F32) k_maxpool<float><<<g, 256, 0, s>>>(tin, tout, size, stride, pad);
+                else k_maxpool<__nv_bfloat16><<<g, 256, 0, s>>>(tin, tout, size, stride, pad);
+            });
+            break;
+        }
+        case YB_UPSAMPLE: {
+            need_input(i);
+            if (l.reverse) fatal_throw("engine: reverse upsample (downsample) is not supported");
+            const int stride = l.stride; const float scale = l.scale;
+            const int esz = (int)dt_size(dt);
+            const bool vec = scale == 1.f && (l.out_c * esz) % 16 == 0 && (tin.ldc * esz) % 16 == 0 && (tout.ldc * esz) % 16 == 0 &&
+                             (reinterpret_cast<uintptr_t>(tin.base) & 15) == 0 && (reinterpret_cast<uintptr_t>(tout.base) & 15) == 0;
+            const int gv = grid_for((long)B * l.out_h * l.out_w * ((l.out_c * esz) / 16 + 1));
+            push(OP_UPSAMPLE, i, [tin, tout, stride, scale, g, dt, vec, gv, esz](cudaStream_t s) {
+                if (vec) k_upsample_vec16<<<gv, 256, 0, s>>>(tin, tout, stride, esz);
+                else if (dt == DT_F32) k_upsample<float><<<g, 256, 0, s>>>(tin, tout, stride, scale);
+                else k_upsample<__nv_bfloat16><<<g, 256, 0, s>>>(tin, tout, stride, scale);
+            });
+            break;
+        }
+        case YB_SHORTCUT: {
+            if (p.fused_sc) break;
+            need_input(i);
+            const TV from = e.out_tv[l.index];
+            if (!from.base) fatal_throw("engine: shortcut source not placed");
+            if (L[l.index].out_dt != dt) fatal_throw("engine: shortcut dtype mismatch");
+            // shortcut_cpu(batch, w1=l.w, h1=l.h, c1=l.c (from), add, w2=l.out_w, ...): yolov2_forward_network.c:410
+            const int stride = std::max(l.w / l.out_w, 1), sample = std::max(l.out_w / l.w, 1);
+            const int minw = std::min(l.w, l.out_w), minh = std::min(l.h, l.out_h), minc = std::min(l.c, l.out_c);
+            const int act = l.activation;
+            push(OP_SHORTCUT, i, [=](cudaStream_t s) {
+                if (dt == DT_F32) k_shortcut<float><<<g, 256, 0, s>>>(tin, from, tout, stride, sample, minw, minh, minc, act);
+                else k_shortcut<__nv_bfloat16><<<g, 256, 0, s>>>(tin, from, tout, stride, sample, minw, minh, minc, act);
+            });
+            break;
+        }
+        case YB_ROUTE: {
+            if (!p.has_out) fatal_throw("engine: route over layers of different spatial size is not supported");
+            if (is_alias(i)) break;
+            int off = 0;
+            for (int k = 0; k < l.n; ++k) {
+                const int j = l.input_layers[k];
+                const Layer &src = layer(j);
+                if (L[j].owner != i) {
+                    const TV tsrc = e.out_tv[j];
+                    if (!tsrc.base) fatal_throw("engine: route source not placed");
+                    if (L[j].out_dt != p.out_dt) fatal_throw("engine: route dtype mismatch");
+                    TV slice = tout;
+                    slice.base += (size_t)off * dt_size(p.out_dt);
+                    slice.C = src.out_c;
+                    const int gs = grid_for((long)B * src.out_h * src.out_w * src.out_c);
+                    const int odt = p.out_dt;
+                    push(OP_ROUTE_COPY, i, [tsrc, slice, gs, odt](cudaStream_t s) {
+                        if (odt == DT_F32) k_copy_channels<float><<<gs, 256, 0, s>>>(tsrc, slice);
+                        else k_copy_channels<__nv_bfloat16><<<gs, 256, 0, s>>>(tsrc, slice);
+                    });
+                }
+                off += src.out_c;
+            }
+            break;
+        }
+        case YB_REORG: {
+            need_input(i);
+            if (l.reverse) fatal_throw("engine: reverse reorg is not supported");
+            const int stride = l.stride;
+            push(OP_REORG, i, [tin, tout, stride, g, dt](cudaStream_t s) {
+                if (dt == DT_F32) k_reorg<float><<<g, 256, 0, s>>>(tin, tout, stride);
+                else k_reorg<__nv_bfloat16><<<g, 256, 0, s>>>(tin, tout, stride);
+            });
+            break;
+        }
+        case YB_YOLO: {
+            if (p.yolo_fused) break;   // written by the head convolution's epilogue
+            need_input(i);
+            float *dst = e.d_final[i];
+            const int classes = l.classes;
+            const int gy = grid_for((long)B * ((l.h * l.w + 31) / 32) * ((l.c + 31) / 32) * 256);
+            const int fast = (ADT == DT_BF16) ? 1 : 0;
+            push(OP_YOLO, i, [tin, dst, classes, gy, dt, fast](cudaStream_t s) {
+                if (dt == DT_F32) k_yolo<float><<<gy, 256, 0, s>>>(tin, dst, classes, fast);
+                else k_yolo<__nv_bfloat16><<<gy, 256, 0, s>>>(tin, dst, classes, fast);
+            });
+            break;
+        }
+        case YB_REGION: {
+            need_input(i);
+            float *dst = e.d_final[i];
+            const int n = l.n, classes = l.classes, coords = l.coords, softmax = l.softmax;
+            const int gr = grid_for((long)B * l.h * l.w * l.n);
+            push(OP_REGION, i, [tin, dst, n, classes, coords, softmax, gr, dt](cudaStream_t s) {
+                if (dt == DT_F32) k_region<float><<<gr, 256, 0, s>>>(tin, dst, n, classes, coords, softmax);
+                else k_region<__nv_bfloat16><<<gr, 256, 0, s>>>(tin, dst, n, classes, coords, softmax);
+            });
+            break;
+        }
+        default:
+            break;
+        }
+    }
+
+    // last layer that is not yolo / region: keep an NCHW f32 copy as "the network output"
+    void emit_last_copy() {
+        const int last = nl - 1;
+        const Layer &l = layer(last);
+        if (l.type == YB_YOLO || l.type == YB_REGION || !e.d_final[last]) return;
+        const int src = L[last].fused_into >= 0 ? L[last].fused_into : last;
+        const TV t = e.out_tv[src];
+        if (!t.base) return;
+        float *dst = e.d_final[last];
+        const int dt = L[src].out_dt;
+        const int g = grid_for((long)B * l.outputs);
+        push(OP_YOLO, last, [t, dst, g, dt](cudaStream_t s) {
+            if (dt == DT_F32) k_nhwc_to_nchw_f32<float><<<g, 256, 0, s>>>(t, dst);
+            else k_nhwc_to_nchw_f32<__nv_bfloat16><<<g, 256, 0, s>>>(t, dst);
+        });
+    }
+
+    void emit_ops() {
+        emit_first();
+        for (int i = 0; i < nl; ++i) {
+            if (L[i].in_first_op) continue;
+            if (is_conv(i)) emit_conv(i);
+            else emit_small(i);
+        }
+        emit_last_copy();
+    }
+};
+}  // namespace
+
 std::shared_ptr<Engine> build_engine(Network *net, const EngineOptions &opt) {
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
@@ -194,867 +1080,22 @@ std::shared_ptr<Engine> build_engine(Network *net, const EngineOptions &opt) {
         fatal_throw(std::string("yolo2_light_b200: device '") + prop.name + "' is compute capability " +
                     std::to_string(prop.major) + "." + std::to_string(prop.minor) +
                     "; this build contains sm_90a code only");
+    if (net->layers.empty()) fatal_throw("empty network");
 
     auto e = std::make_shared<Engine>();
     e->opt = opt;
     e->batch = net->batch;
-    const int B = net->batch;
-    const int nl = (int)net->layers.size();
-    if (nl == 0) fatal_throw("empty network");
+    e->sw = Switches::read();
     CUDA_OK(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
 
-    bool any_xnor = false;
-    for (const Layer &l : net->layers) {
-        if (l.type != YB_CONVOLUTIONAL) continue;
-        if (l.batch_normalize) fatal_throw("engine: batch-norm not folded -- call yb_fuse_conv_batchnorm first");
-        if (l.xnor) {
-            any_xnor = true;
-            if (!l.has_mean_arr) fatal_throw("engine: xnor layer without mean_arr -- call yb_calculate_binary_weights first");
-        }
-        if (opt.qrule && !l.has_int8)
-            fatal_throw("engine: -quantized rule without int8 weights -- call yb_quantinization_and_get_multipliers first");
-    }
-    // f32 activations whenever an integer path must see exactly the reference's inputs
-    const bool exact = opt.qrule || any_xnor || opt.precision == YB_PREC_FP32;
-    e->act_dt = exact ? DT_F32 : DT_BF16;
-    const int ADT = e->act_dt;
-
-    auto conv_variant = [&](int i) -> int {   // 0 fp32, 1 xnor, 2 int8
-        const Layer &l = net->layers[i];
-        if (opt.qrule && (i + opt.q_index_offset) >= 1 && l.activation != YB_LINEAR) return 2;
-        if (l.xnor) return 1;
-        return 0;
-    };
-
-    const auto cons = consumers_of(*net);
-    // XNOR layers with enough channels run on the tensor cores as +-1 int8 (dot == 2*count - K, exact); the small
-    // ones stay on the popcount kernels.  YB_XNOR_TC=0 forces popcount everywhere.
-    auto xnor_on_tc = [&](const Layer &l) {
-        const char *ev = getenv("YB_XNOR_TC");
-        if (ev && ev[0] == '0') return false;
-        // channels are padded to a multiple of 32 with zero WEIGHT bytes (whatever the activation pad bytes hold contributes 0), so
-        // even the 16- and 32-channel layers run here: the popcount kernels are bound by the 16 POPC/clk/SM of the integer pipe,
-        // while the same layers as +-1 bytes on the s8 tensor cores are not
-        const int minc = getenv("YB_XNOR_TC_MINC") ? atoi(getenv("YB_XNOR_TC_MINC")) : 16;
-        return l.xnor && l.c % 16 == 0 && l.c >= minc && l.size == 3 && l.stride == 1 && l.pad == 1 && l.n >= 8;
-    };
-
-    // XNOR layers with stride != 1 or pad != 1 never reach the bit GEMM in the reference: forward_convolutional_layer_cpu
-    // binarises the input to +-1 floats (binarize_cpu, additionally.c:128-134), swaps in the +-mean weights (binarize_weights,
-    // :113-126) and runs the ordinary im2col + gemm_nn (yolov2_forward_network.c:40-50, :204) -- out-of-image taps count 0 there,
-    // not -1.  Same here: k_binarize_pm1 + the exact-order float convolution.
-    auto xnor_fallback = [&](const Layer &l) { return l.xnor && !(l.stride == 1 && l.pad == 1); };
-
-    // integer conv i -> 2x2/2 max-pool i+1 -> integer conv i+2, nothing else reading i or i+1: the pool and the next layer's input
-    // conversion can run in conv i's epilogue (tc_plan_fuse_pool).  Returns the mode (1 s8 quantised, 2 +-1 bytes) or 0.
-    auto conv_pool_mode = [&](int i) -> int {
-        if (!opt.fuse || opt.keep_counts || getenv("YB_NO_CONV_POOL_FUSE") || i + 2 >= nl) return 0;
-        const Layer &mp = net->layers[i + 1], &c2 = net->layers[i + 2];
-        if (mp.type != YB_MAXPOOL || mp.size != 2 || mp.stride != 2 || mp.pad != 1 || c2.type != YB_CONVOLUTIONAL) return 0;
-        if (cons[i].size() != 1 || cons[i][0] != i + 1 || cons[i + 1].size() != 1 || cons[i + 1][0] != i + 2) return 0;
-        const int v2 = conv_variant(i + 2);
-        if (v2 == 2) return 1;
-        if (v2 == 1 && xnor_on_tc(c2) && !xnor_fallback(c2)) return 2;
-        if (v2 == 1 && !xnor_fallback(c2)) return 3;     // next XNOR layer reads sign bits (popcount kernels)
-        return 0;
-    };
-
-    // ---- fusion plan: conv i + same-shape shortcut i+1 whose only reader is that shortcut -------------
-    std::vector<int> fused_into(nl, -1);   // conv i writes layer fused_into[i]'s output
-    std::vector<char> is_fused_sc(nl, 0);
-    if (opt.fuse) {
-        for (int i = 0; i + 1 < nl; ++i) {
-            const Layer &l = net->layers[i], &s = net->layers[i + 1];
-            if (l.type != YB_CONVOLUTIONAL || s.type != YB_SHORTCUT) continue;
-            if (conv_variant(i) != 0) continue;
-            if (l.stride != 1) continue;   // the tensor-core stride-2 path stores straddling tiles row by row, without a residual
-            if (cons[i].size() != 1 || cons[i][0] != i + 1) continue;
-            if (s.index == i) continue;
-            if (!(s.w == s.out_w && s.h == s.out_h && s.c == s.out_c)) continue;
-            fused_into[i] = i + 1;
-            is_fused_sc[i + 1] = 1;
-        }
-    }
-
-    // ---- fusion plan: detection-head conv i + [yolo] i+1 (tensor-core path only; decided again when ops are emitted)
-    std::vector<char> yolo_fused(nl, 0);
-
-    // ---- output placement --------------------------------------------------------------------------
-    // pass 1: decide dtype + home of every layer output (own buffer, or a channel slice of a concat buffer)
-    struct Home { int owner = -1; int coff = 0; int ldc = 0; };   // owner: layer whose buffer holds it
-    std::vector<Home> home(nl);
-    e->out_dt.assign(nl, ADT);
-    auto has_nhwc_out = [&](int i) {
-        const Layer &l = net->layers[i];
-        if (l.type == YB_YOLO || l.type == YB_REGION || l.type == YB_BLANK) return false;
-        if (fused_into[i] >= 0) return false;
-        if (l.out_h <= 0 || l.out_w <= 0 || l.out_c <= 0) return false;
-        return true;
-    };
-    for (int i = 0; i < nl; ++i) {
-        const Layer &l = net->layers[i];
-        if (l.type == YB_CONVOLUTIONAL && !cons[i].empty()) {
-            bool all_final = true;
-            for (int c : cons[i]) if (net->layers[c].type != YB_YOLO && net->layers[c].type != YB_REGION) all_final = false;
-            if (all_final) e->out_dt[i] = DT_F32;   // detection heads stay f32 (bf16 would cost ~1e-3 rel by itself)
-        }
-        if (l.type == YB_CONVOLUTIONAL && cons[i].empty()) e->out_dt[i] = DT_F32;
-    }
-    if (opt.fuse) {
-        for (int r = 0; r < nl; ++r) {
-            const Layer &l = net->layers[r];
-            if (l.type != YB_ROUTE || l.n < 2 || l.out_c <= 0) continue;
-            int off = 0;
-            for (int k = 0; k < l.n; ++k) {
-                const int j = l.input_layers[k];
-                const Layer &src = net->layers[j];
-                const bool ok = has_nhwc_out(j) && home[j].owner < 0 && src.type != YB_ROUTE &&
-                                e->out_dt[j] == ADT;
-                if (ok) { home[j].owner = r; home[j].coff = off; home[j].ldc = l.out_c; }
-                off += src.out_c;
-            }
-        }
-    }
-    // pass 2: sizes + arena offsets
-    std::vector<size_t> buf_off(nl, (size_t)-1);
-    size_t act_total = 0;
-    const int P = 1;
-    auto own_buffer = [&](int i) {
-        const Layer &l = net->layers[i];
-        buf_off[i] = act_total;
-        act_total += align_up(tv_bytes(B, l.out_h, l.out_w, (int)align_up(l.out_c, 8), P, e->out_dt[i]), 1024);
-    };
-    const size_t in0_off = act_total;
-    e->in0_dt = ADT;
-    act_total += align_up(tv_bytes(B, net->h, net->w, net->c, P, ADT), 1024);
-    for (int i = 0; i < nl; ++i) {
-        const Layer &l = net->layers[i];
-        if (!has_nhwc_out(i)) continue;
-        if (l.type == YB_ROUTE && l.n == 1 && opt.fuse) continue;   // pure alias
-        if (home[i].owner >= 0) continue;                           // lives inside a concat buffer
-        own_buffer(i);
-    }
-    // side buffers of the integer paths
-    std::vector<size_t> side_off(nl, (size_t)-1);
-    std::vector<int> side_ld(nl, 0);
-    for (int i = 0; i < nl; ++i) {
-        const Layer &l = net->layers[i];
-        if (l.type != YB_CONVOLUTIONAL) continue;
-        const int v = conv_variant(i);
-        if (v == 1 && xnor_fallback(l)) {
-            side_ld[i] = l.c;   // +-1 floats
-            side_off[i] = act_total;
-            act_total += align_up(tv_bytes(B, l.h, l.w, side_ld[i], P, DT_F32), 1024);
-        } else if (v == 1 && xnor_on_tc(l)) {
-            side_ld[i] = (int)align_up(l.c, 32);   // +-1 bytes; pad channels meet zero weights
-            side_off[i] = act_total;
-            act_total += align_up(tv_bytes(B, l.h, l.w, side_ld[i], P, DT_S8), 1024);
-        } else if (v == 1) {
-            side_ld[i] = (l.c + 31) / 32;
-            side_off[i] = act_total;
-            act_total += align_up(tv_bytes(B, l.h, l.w, side_ld[i], P, DT_BITS), 1024);
-        } else if (v == 2) {
-            side_ld[i] = (int)align_up(l.c, 32);   // zero-padded channels: every INT8 layer fits the s8 wgmma tensor-core tile
-            side_off[i] = act_total;
-            act_total += align_up(tv_bytes(B, l.h, l.w, side_ld[i], P, DT_S8), 1024);
-        }
-    }
-    e->act_bytes = act_total;
-    CUDA_OK(cudaMalloc(&e->act_arena, act_total));
-    CUDA_OK(cudaMemsetAsync(e->act_arena, 0, act_total, e->stream));   // zero borders, once
-
-    for (int i = 0; i < nl; ++i) {   // +-1 activation buffers: borders are -1 (out-of-image taps count as -1, SURVEY F9)
-        const Layer &l = net->layers[i];
-        if (l.type == YB_CONVOLUTIONAL && conv_variant(i) == 1 && xnor_on_tc(l) && !xnor_fallback(l))
-            CUDA_OK(cudaMemsetAsync(e->act_arena + side_off[i], 0xFF, tv_bytes(B, l.h, l.w, side_ld[i], P, DT_S8), e->stream));
-    }
-    e->in0 = make_tv(e->act_arena + in0_off, B, net->h, net->w, net->c, net->c, P, ADT, 0);
-    e->out_tv.assign(nl, TV{});
-    for (int i = 0; i < nl; ++i) {
-        const Layer &l = net->layers[i];
-        if (!has_nhwc_out(i)) continue;
-        if (l.type == YB_ROUTE && l.n == 1 && opt.fuse) {
-            e->out_tv[i] = e->out_tv[l.input_layers[0]];
-            e->out_dt[i] = e->out_dt[l.input_layers[0]];
-            continue;
-        }
-        if (home[i].owner >= 0) continue;
-        // pixel stride rounded up to 8 channels: 16-byte aligned rows for TMA / vector stores (e.g. 255 -> 256)
-        e->out_tv[i] = make_tv(e->act_arena + buf_off[i], B, l.out_h, l.out_w, l.out_c, (int)align_up(l.out_c, 8), P, e->out_dt[i], 0);
-    }
-    // slices (owner buffers are allocated above since routes own their buffers)
-    for (int i = 0; i < nl; ++i) {
-        if (home[i].owner < 0) continue;
-        const Layer &l = net->layers[i];
-        const int r = home[i].owner;
-        e->out_tv[i] = make_tv(e->act_arena + buf_off[r], B, l.out_h, l.out_w, l.out_c, e->out_tv[r].ldc, P, ADT, home[i].coff);
-    }
-    // single-input route aliases may point at slices that were only resolved now
-    for (int i = 0; i < nl; ++i) {
-        const Layer &l = net->layers[i];
-        if (has_nhwc_out(i) && l.type == YB_ROUTE && l.n == 1 && opt.fuse) {
-            e->out_tv[i] = e->out_tv[l.input_layers[0]];
-            e->out_dt[i] = e->out_dt[l.input_layers[0]];
-        }
-    }
-
-    // ---- final (host-visible) outputs ----------------------------------------------------------------
-    e->d_final.assign(nl, nullptr);
-    e->h_final.assign(nl, nullptr);
-    e->final_count.assign(nl, 0);
-    e->d_counts.assign(nl, nullptr);
-    e->counts_count.assign(nl, 0);
-    for (int i = 0; i < nl; ++i) {
-        const Layer &l = net->layers[i];
-        if (l.type == YB_YOLO || l.type == YB_REGION) {
-            e->final_count[i] = (size_t)l.outputs * B;
-            CUDA_OK(cudaMalloc(&e->d_final[i], e->final_count[i] * sizeof(float)));
-            CUDA_OK(cudaHostAlloc(&e->h_final[i], e->final_count[i] * sizeof(float), cudaHostAllocDefault));
-        }
-    }
-    {   // the reference returns the LAST layer's output; keep a host copy for it whatever its type
-        const int last = nl - 1;
-        const Layer &l = net->layers[last];
-        if (!e->d_final[last] && l.outputs > 0) {
-            e->final_count[last] = (size_t)l.outputs * B;
-            CUDA_OK(cudaMalloc(&e->d_final[last], e->final_count[last] * sizeof(float)));
-            CUDA_OK(cudaHostAlloc(&e->h_final[last], e->final_count[last] * sizeof(float), cudaHostAllocDefault));
-        }
-    }
-
-    // ---- weight arena ------------------------------------------------------------------------------
-    std::vector<ConvWeights> cw(nl);
-    std::vector<char> hostw;
-    auto reserve = [&](size_t bytes) { size_t off = align_up(hostw.size(), 1024); hostw.resize(off + bytes, 0); return off; };
-    std::vector<int> use_tc(nl, 0);
-    e->not_materialised.assign(nl, 0);
-    std::vector<char> prefilled(nl, 0);   // the producing max-pool already wrote this conv's s8 / sign input (fused)
-    std::vector<char> pool_in_conv(nl, 0); // this max-pool runs inside the epilogue of the integer convolution in front of it
-    for (int i = 0; i < nl; ++i) {
-        const Layer &l = net->layers[i];
-        if (l.type != YB_CONVOLUTIONAL) continue;
-        const int v = conv_variant(i);
-        const int taps = l.size * l.size;
-        const int K = taps * l.c;
-        ConvWeights &w = cw[i];
-        w.bias = reserve(sizeof(float) * align_up(l.n, 64));
-        memcpy(&hostw[w.bias], l.biases.data(), sizeof(float) * l.n);
-        if (v == 0) {
-            const TV &tin = (i == 0) ? e->in0 : e->out_tv[i - 1];
-            const int in_dt = (i == 0) ? e->in0_dt : e->out_dt[i - 1];
-            const int odt = fused_into[i] >= 0 ? e->out_dt[fused_into[i]] : e->out_dt[i];
-            const TV &tout = e->out_tv[fused_into[i] >= 0 ? fused_into[i] : i];
-            use_tc[i] = (ADT == DT_BF16 && in_dt == DT_BF16) ? tc_conv_supported(l, tin, tout, odt == DT_BF16) : 0;
-            // float detection heads of the INT8 / XNOR networks (default precision): tf32 wgmma.  Only layers whose every
-            // reader is a yolo / region layer -- nothing they compute can reach an integer layer.
-            if (ADT == DT_F32 && opt.precision == YB_PREC_BF16_TC && in_dt == DT_F32 && odt == DT_F32 && fused_into[i] < 0 &&
-                !cons[i].empty() && !getenv("YB_NO_TF32")) {
-                bool heads_only = true;
-                for (int r : cons[i]) heads_only &= net->layers[r].type == YB_YOLO || net->layers[r].type == YB_REGION;
-                if (heads_only && tc_tf32_supported(l, tin, tout)) use_tc[i] = 2;
-            }
-            if (getenv("YB_NO_TC")) use_tc[i] = 0;
-            if (use_tc[i] == 2) {
-                w.ldn = (int)align_up(l.n, 64);
-                w.w_f32km = reserve(sizeof(float) * (size_t)w.ldn * K);
-                float *dst = reinterpret_cast<float *>(&hostw[w.w_f32km]);
-                for (int f = 0; f < l.n; ++f)
-                    for (int c = 0; c < l.c; ++c)
-                        for (int t = 0; t < taps; ++t)
-                            dst[(size_t)f * K + (size_t)t * l.c + c] = l.weights[((size_t)f * l.c + c) * taps + t];
-            } else if (use_tc[i]) {
-                // bf16 [ldn][K], K ordered (ky, kx, c): the K-major B operand of the implicit GEMM
-                w.ldn = (int)align_up(l.n, 64);
-                w.w_bf16 = reserve(sizeof(__nv_bfloat16) * (size_t)w.ldn * K);
-                __nv_bfloat16 *dst = reinterpret_cast<__nv_bfloat16 *>(&hostw[w.w_bf16]);
-                for (int f = 0; f < l.n; ++f)
-                    for (int c = 0; c < l.c; ++c)
-                        for (int t = 0; t < taps; ++t)
-                            dst[(size_t)f * K + (size_t)t * l.c + c] =
-                                __float2bfloat16_rn(l.weights[((size_t)f * l.c + c) * taps + t]);
-            } else {
-                // f32 [K][ldw]; K ordered (ky, kx, c), or -- f32 activations: the exact order of the reference's gemm_nn
-                // (k_conv_simt<EXACT>) -- (c, ky, kx)
-                w.ldw = (int)align_up(l.n, 64);
-                w.w_f32 = reserve(sizeof(float) * (size_t)K * w.ldw);
-                float *dst = reinterpret_cast<float *>(&hostw[w.w_f32]);
-                for (int f = 0; f < l.n; ++f)
-                    for (int c = 0; c < l.c; ++c)
-                        for (int t = 0; t < taps; ++t)
-                            dst[(ADT == DT_F32 ? (size_t)c * taps + t : (size_t)t * l.c + c) * w.ldw + f] =
-                                l.weights[((size_t)f * l.c + c) * taps + t];
-            }
-        } else if (v == 1 && xnor_fallback(l)) {
-            // f32 [K][ldw], K in the reference's (c, ky, kx) order: +mean where w > 0, -mean otherwise (binarize_weights)
-            w.ldw = (int)align_up(l.n, 64);
-            w.w_f32 = reserve(sizeof(float) * (size_t)K * w.ldw);
-            float *dst = reinterpret_cast<float *>(&hostw[w.w_f32]);
-            for (int f = 0; f < l.n; ++f)
-                for (int c = 0; c < l.c; ++c)
-                    for (int t = 0; t < taps; ++t)
-                        dst[((size_t)c * taps + t) * w.ldw + f] = l.weights[((size_t)f * l.c + c) * taps + t] > 0 ? l.mean_arr[f] : -l.mean_arr[f];
-        } else if (v == 1 && xnor_on_tc(l)) {
-            // +-1 bytes [ldn][taps][cpad]: +1 where w > 0, -1 otherwise; padded filter rows and padded channels stay 0
-            w.cpad = side_ld[i];
-            w.ldn = (int)align_up(l.n, 64);
-            w.w_s8 = reserve((size_t)w.ldn * taps * w.cpad);
-            int8_t *dst = reinterpret_cast<int8_t *>(&hostw[w.w_s8]);
-            for (int f = 0; f < l.n; ++f)
-                for (int c = 0; c < l.c; ++c)
-                    for (int t = 0; t < taps; ++t)
-                        dst[((size_t)f * taps + t) * w.cpad + c] = l.weights[((size_t)f * l.c + c) * taps + t] > 0 ? 1 : -1;
-            w.mean = reserve(sizeof(float) * align_up(l.n, 64));
-            memcpy(&hostw[w.mean], l.mean_arr.data(), sizeof(float) * l.n);
-        } else if (v == 1) {
-            // sign bits [ldn][taps][CW]; bit = (w > 0) (binarize_weights additionally.c:113 + float_to_bit :1536)
-            const int CW = (l.c + 31) / 32;
-            w.ldn = (int)align_up(l.n, 64);
-            w.cpad = CW * 32;
-            w.w_bits = reserve(sizeof(uint32_t) * (size_t)w.ldn * taps * CW);
-            uint32_t *dst = reinterpret_cast<uint32_t *>(&hostw[w.w_bits]);
-            for (int f = 0; f < l.n; ++f)
-                for (int c = 0; c < l.c; ++c)
-                    for (int t = 0; t < taps; ++t)
-                        if (l.weights[((size_t)f * l.c + c) * taps + t] > 0)
-                            dst[((size_t)f * taps + t) * CW + c / 32] |= 1u << (c & 31);
-            w.mean = reserve(sizeof(float) * align_up(l.n, 64));
-            memcpy(&hostw[w.mean], l.mean_arr.data(), sizeof(float) * l.n);
-        } else {
-            // s8 [ldn][taps][cpad], zero channel padding
-            w.cpad = side_ld[i];
-            w.ldn = (int)align_up(l.n, 64);
-            w.w_s8 = reserve((size_t)w.ldn * taps * w.cpad);
-            int8_t *dst = reinterpret_cast<int8_t *>(&hostw[w.w_s8]);
-            for (int f = 0; f < l.n; ++f)
-                for (int c = 0; c < l.c; ++c)
-                    for (int t = 0; t < taps; ++t)
-                        dst[((size_t)f * taps + t) * w.cpad + c] = l.weights_int8[((size_t)f * l.c + c) * taps + t];
-        }
-    }
-    size_t stem_w_off = (size_t)-1;
-    {
-        const Layer &l0 = net->layers[0];
-        if (ADT == DT_BF16 && l0.type == YB_CONVOLUTIONAL && conv_variant(0) == 0 && l0.c == 3 && l0.size == 3 && l0.n <= 32) {
-            stem_w_off = reserve(sizeof(__nv_bfloat16) * 32 * 32);
-            __nv_bfloat16 *dst = reinterpret_cast<__nv_bfloat16 *>(&hostw[stem_w_off]);
-            for (int i = 0; i < 32 * 32; ++i) dst[i] = __float2bfloat16_rn(0.f);
-            for (int f = 0; f < l0.n; ++f)
-                for (int c = 0; c < 3; ++c)
-                    for (int t = 0; t < 9; ++t)
-                        dst[f * 32 + t * 3 + c] = __float2bfloat16_rn(l0.weights[((size_t)f * 3 + c) * 9 + t]);
-        }
-    }
-    e->w_bytes = align_up(std::max<size_t>(hostw.size(), 1024), 1024);
-    CUDA_OK(cudaMalloc(&e->w_arena, e->w_bytes));
-    if (opt.upload) CUDA_OK(cudaMemcpyAsync(e->w_arena, hostw.data(), hostw.size(), cudaMemcpyHostToDevice, e->stream));
-    CUDA_OK(cudaStreamSynchronize(e->stream));   // hostw goes out of scope below
-
-    // ---- input staging -----------------------------------------------------------------------------
-    e->input_count = (size_t)B * net->c * net->h * net->w;
+    Builder b(*net, opt, *e);
+    b.plan_layers();
+    b.place();
+    b.place_finals();
+    b.pack_weights();
+    e->input_count = (size_t)net->batch * net->c * net->h * net->w;   // staging of the caller's images
     CUDA_OK(cudaMalloc(&e->d_input, e->input_count * sizeof(float)));
-
-    // ---- op list -----------------------------------------------------------------------------------
-    Engine *E = e.get();
-    bool stem_fused = false, stem_pool_fused = false, stem_s2_fused = false;
-    {
-        // ops[0] consumes the caller's NCHW f32 images.  Usually that is the stem convolution itself (3 input
-        // channels, 3x3/1/1), reading NCHW directly; otherwise a plain NCHW -> padded-NHWC conversion.
-        const Layer &l0 = net->layers[0];
-        const bool stem_ok = l0.type == YB_CONVOLUTIONAL && conv_variant(0) == 0 && !use_tc[0] && l0.c == 3 &&
-                             l0.size == 3 && l0.stride == 1 && l0.pad == 1 && (l0.n == 16 || l0.n == 32) &&
-                             fused_into[0] < 0 && e->out_tv[0].base && !getenv("YB_NO_STEM") &&
-                             (e->out_dt[0] == DT_F32 || (e->out_tv[0].ldc % 8 == 0));
-        // exact nets: stem + 2x2/2 max-pool + the integer layer's input conversion in one kernel (k_stem_pool): layers 0 and 1
-        // are then never written to HBM
-        bool pool_ok = stem_ok && opt.fuse && e->out_dt[0] == DT_F32 && l0.n == 16 && nl > 2 && !getenv("YB_NO_STEM_POOL_FUSE") &&
-                       (l0.activation == YB_LEAKY || l0.activation == YB_LINEAR);
-        if (pool_ok) {
-            const Layer &mp = net->layers[1], &c2 = net->layers[2];
-            pool_ok = mp.type == YB_MAXPOOL && mp.size == 2 && mp.stride == 2 && mp.pad == 1 && cons[0].size() == 1 && cons[0][0] == 1 &&
-                      cons[1].size() == 1 && cons[1][0] == 2 && c2.type == YB_CONVOLUTIONAL && conv_variant(2) != 0 &&
-                      side_off[2] != (size_t)-1 && !xnor_fallback(c2) && (conv_variant(2) == 1 && !xnor_on_tc(c2) ? true : side_ld[2] % 16 == 0);
-        }
-        if (pool_ok) {
-            stem_fused = true; stem_pool_fused = true;
-            const Layer &c2 = net->layers[2];
-            const int v2 = conv_variant(2);
-            const bool pm1 = v2 == 1 && xnor_on_tc(c2);      // next layer reads +-1 bytes
-            const TV q = (v2 == 2 || pm1) ? make_tv(e->act_arena + side_off[2], B, c2.h, c2.w, c2.c, side_ld[2], P, DT_S8, 0)
-                                          : make_tv(e->act_arena + side_off[2], B, c2.h, c2.w, side_ld[2], side_ld[2], P, DT_BITS, 0);
-            StemW<16> w16{};
-            for (int f = 0; f < 16; ++f) {
-                for (int c = 0; c < 3; ++c)
-                    for (int t = 0; t < 9; ++t) w16.w[(t * 3 + c) * 16 + f] = l0.weights[((size_t)f * 3 + c) * 9 + t];
-                w16.b[f] = l0.biases[f];
-            }
-            const int act = l0.activation, H = l0.h, W = l0.w;
-            const float mult = (v2 == 2) ? c2.input_quant_multipler : 0.f;
-            const int grid = (int)(((long)B * c2.h * c2.w + 127) / 128);
-            prefilled[2] = 1;
-            e->not_materialised[0] = e->not_materialised[1] = 1;
-            e->first_kind = OP_CONV_SIMT; e->first_layer = 0;
-            e->first_op = [=](const float *din, cudaStream_t s) {
-                if (v2 == 2 && act == ACT_LEAKY) k_stem_pool<0, ACT_LEAKY><<<grid, 128, 0, s>>>(din, q, w16, act, H, W, mult);
-                else if (v2 == 2) k_stem_pool<0, ACT_LINEAR><<<grid, 128, 0, s>>>(din, q, w16, act, H, W, mult);
-                else if (pm1 && act == ACT_LEAKY) k_stem_pool<1, ACT_LEAKY><<<grid, 128, 0, s>>>(din, q, w16, act, H, W, mult);
-                else if (pm1) k_stem_pool<1, ACT_LINEAR><<<grid, 128, 0, s>>>(din, q, w16, act, H, W, mult);
-                else if (act == ACT_LEAKY) k_stem_pool<2, ACT_LEAKY><<<grid, 128, 0, s>>>(din, q, w16, act, H, W, mult);
-                else k_stem_pool<2, ACT_LINEAR><<<grid, 128, 0, s>>>(din, q, w16, act, H, W, mult);
-            };
-        } else if (stem_ok && stem_w_off != (size_t)-1 && e->out_dt[0] == DT_BF16 && tc_stem_supported(l0, e->out_tv[0]) &&
-            !getenv("YB_NO_STEM_TC")) {
-            // tensor-core stem: gathers the 3x3x3 window from NCHW, K padded 27 -> 32.  When layer 1 is a bf16 tensor-core
-            // 3x3 / stride-2 convolution 32 -> 64 and the stem's only reader, both run as one kernel (k_stem_s2_tc) and the
-            // stem output is never written (its buffer stays allocated but unused).
-            stem_fused = true;
-            const float *bias0 = reinterpret_cast<const float *>(e->w_arena + cw[0].bias);
-            stem_s2_fused = opt.fuse && !getenv("YB_NO_STEM_S2_FUSE") && nl > 1 && cons[0].size() == 1 && cons[0][0] == 1 &&
-                            net->layers[1].type == YB_CONVOLUTIONAL && conv_variant(1) == 0 && use_tc[1] == 1 &&
-                            fused_into[1] < 0 && e->out_dt[1] == DT_BF16 && tc_stem_s2_supported(l0, net->layers[1], e->out_tv[1]);
-            void *sp = stem_s2_fused ? tc_stem_s2_make_plan(l0, net->layers[1], e->out_tv[1], e->w_arena + stem_w_off, bias0,
-                                                            e->w_arena + cw[1].w_bf16, reinterpret_cast<const float *>(e->w_arena + cw[1].bias))
-                                     : tc_stem_make_plan(l0, e->out_tv[0], e->w_arena + stem_w_off, bias0);
-            e->stem_plan = sp;
-            e->first_kind = OP_CONV_TC; e->first_layer = 0;
-            if (stem_s2_fused) {
-                e->not_materialised[0] = 1;
-                e->first_layer = 1;
-                ++e->n_tc;
-            }
-            e->first_op = [sp](const float *din, cudaStream_t s) { tc_stem_launch(sp, din, s); };
-            if (!getenv("YB_NO_STEM_U8")) e->first_op_u8 = [sp](const unsigned char *d8, cudaStream_t s) { tc_stem_launch_u8(sp, d8, s); };
-        } else if (stem_ok) {
-            stem_fused = true;
-            const TV tout = e->out_tv[0];
-            const int act = l0.activation, H = l0.h, W = l0.w, nf = l0.n, odt = e->out_dt[0];
-            // weights go to the kernel as by-value constants: [27 = (ky,kx,c)][n] + bias
-            StemW<32> w32{}; StemW<16> w16{};
-            for (int f = 0; f < nf; ++f) {
-                for (int c = 0; c < 3; ++c)
-                    for (int t = 0; t < 9; ++t) {
-                        const float v = l0.weights[((size_t)f * 3 + c) * 9 + t];
-                        if (nf == 32) w32.w[(t * 3 + c) * 32 + f] = v; else w16.w[(t * 3 + c) * 16 + f] = v;
-                    }
-                if (nf == 32) w32.b[f] = l0.biases[f]; else w16.b[f] = l0.biases[f];
-            }
-            const long total = (long)B * H * W;
-            const int grid = (int)((total + 127) / 128);
-            e->first_kind = OP_CONV_SIMT; e->first_layer = 0;
-            e->first_op = [=](const float *din, cudaStream_t s) {
-                if (nf == 32 && odt == DT_BF16) k_conv_stem<32, __nv_bfloat16><<<grid, 128, 0, s>>>(din, tout, w32, act, H, W);
-                else if (nf == 32) k_conv_stem<32, float, true><<<grid, 128, 0, s>>>(din, tout, w32, act, H, W);
-                else if (odt == DT_BF16) k_conv_stem<16, __nv_bfloat16><<<grid, 128, 0, s>>>(din, tout, w16, act, H, W);
-                else k_conv_stem<16, float, true><<<grid, 128, 0, s>>>(din, tout, w16, act, H, W);
-            };
-        } else {
-            const TV in0 = e->in0;
-            const int dt = e->in0_dt;
-            const int g = grid_for((long)in0.N * in0.H * in0.W);
-            e->first_op = [=](const float *din, cudaStream_t s) {
-                if (dt == DT_F32) k_input_nchw_to_nhwc<float><<<g, 256, 0, s>>>(din, in0);
-                else k_input_nchw_to_nhwc<__nv_bfloat16><<<g, 256, 0, s>>>(din, in0);
-            };
-        }
-        e->ops.push_back(Op{e->first_kind, e->first_layer, nullptr});   // launched specially: pointer varies per call
-    }
-    for (int i = 0; i < nl; ++i) {
-        const Layer &l = net->layers[i];
-        const TV tin = (i == 0) ? e->in0 : e->out_tv[i - 1];
-        const int in_dt = (i == 0) ? e->in0_dt : e->out_dt[i - 1];
-        const bool prev_ok = (i == 0) || e->out_tv[i - 1].base != nullptr;
-        auto need_prev = [&]() {
-            if (!prev_ok) fatal_throw("engine: layer " + std::to_string(i) + " has no image input");
-        };
-        if (i == 0 && stem_fused) continue;
-        if (i == 1 && (stem_pool_fused || stem_s2_fused)) continue;
-        switch (l.type) {
-        case YB_CONVOLUTIONAL: {
-            need_prev();
-            const int v = conv_variant(i);
-            const int tgt = fused_into[i] >= 0 ? fused_into[i] : i;
-            const TV tout = e->out_tv[tgt];
-            const int odt = e->out_dt[tgt];
-            if (!tout.base) fatal_throw("engine: conv output not placed");
-            if (tin.C != l.c || tin.H != l.h || tin.W != l.w) fatal_throw("engine: conv input shape mismatch");
-            const long M = (long)B * l.out_h * l.out_w;
-            if (v == 0) {
-                TV res{}; int rdt = DT_F32; int act2 = ACT_LINEAR;
-                if (fused_into[i] >= 0) {
-                    const Layer &s = net->layers[tgt];
-                    res = e->out_tv[s.index];
-                    rdt = e->out_dt[s.index];
-                    act2 = s.activation;
-                    if (!res.base) fatal_throw("engine: shortcut source not placed");
-                }
-                if (use_tc[i] == 2) {
-                    const bool fuse_yolo = opt.fuse && i + 1 < nl && net->layers[i + 1].type == YB_YOLO && cons[i].size() == 1 &&
-                                           cons[i][0] == i + 1 && e->d_final[i + 1] && !getenv("YB_NO_YOLO_FUSE");
-                    void *plan = tc_make_plan_tf32(l, tin, tout, e->w_arena + cw[i].w_f32km, cw[i].ldn,
-                                                   reinterpret_cast<const float *>(e->w_arena + cw[i].bias), fuse_yolo ? 1 : 0);
-                    e->tc_plans.push_back(plan);
-                    ++e->n_tc;
-                    if (fuse_yolo) {
-                        tc_plan_fuse_yolo(plan, e->d_final[i + 1], net->layers[i + 1].classes);
-                        yolo_fused[i + 1] = 1;
-                    }
-                    e->ops.push_back(Op{OP_CONV_TC_TF32, i, [plan](cudaStream_t s) { tc_launch(plan, s); }});
-                } else if (use_tc[i]) {
-                    const bool fuse_yolo = opt.fuse && fused_into[i] < 0 && odt == DT_F32 && i + 1 < nl &&
-                                           net->layers[i + 1].type == YB_YOLO && cons[i].size() == 1 && cons[i][0] == i + 1 &&
-                                           e->d_final[i + 1] && !getenv("YB_NO_YOLO_FUSE");
-                    void *plan = tc_make_plan(l, tin, tout, odt == DT_BF16, res, rdt == DT_BF16, act2,
-                                              e->w_arena + cw[i].w_bf16, cw[i].ldn,
-                                              reinterpret_cast<const float *>(e->w_arena + cw[i].bias), fuse_yolo ? 1 : 0);
-                    e->tc_plans.push_back(plan);
-                    ++e->n_tc;
-                    if (fuse_yolo) {
-                        tc_plan_fuse_yolo(plan, e->d_final[i + 1], net->layers[i + 1].classes);
-                        yolo_fused[i + 1] = 1;
-                    }
-                    e->ops.push_back(Op{OP_CONV_TC, i, [plan](cudaStream_t s) { tc_launch(plan, s); }});
-                } else {
-                    ConvP p{};
-                    p.in = tin; p.out = tout; p.res = res;
-                    p.w = e->w_arena + cw[i].w_f32;
-                    p.bias = reinterpret_cast<const float *>(e->w_arena + cw[i].bias);
-                    p.n = l.n; p.ldw = cw[i].ldw; p.size = l.size; p.stride = l.stride; p.pad = l.pad;
-                    p.act = l.activation; p.act2 = act2; p.K = l.size * l.size * l.c; p.M = M;
-                    dim3 grid((unsigned)((M + 63) / 64), (unsigned)((l.n + 63) / 64));
-                    const int key = in_dt * 4 + odt * 2 + rdt;
-                    e->ops.push_back(Op{OP_CONV_SIMT, i, [p, grid, key](cudaStream_t s) {
-                        switch (key) {
-                        case 0: k_conv_simt<float, float, float, true><<<grid, 256, 0, s>>>(p); break;   // reference order, bit-exact
-                        case 1: k_conv_simt<float, float, __nv_bfloat16><<<grid, 256, 0, s>>>(p); break;
-                        case 2: k_conv_simt<float, __nv_bfloat16, float><<<grid, 256, 0, s>>>(p); break;
-                        case 3: k_conv_simt<float, __nv_bfloat16, __nv_bfloat16><<<grid, 256, 0, s>>>(p); break;
-                        case 4: k_conv_simt<__nv_bfloat16, float, float><<<grid, 256, 0, s>>>(p); break;
-                        case 5: k_conv_simt<__nv_bfloat16, float, __nv_bfloat16><<<grid, 256, 0, s>>>(p); break;
-                        case 6: k_conv_simt<__nv_bfloat16, __nv_bfloat16, float><<<grid, 256, 0, s>>>(p); break;
-                        default: k_conv_simt<__nv_bfloat16, __nv_bfloat16, __nv_bfloat16><<<grid, 256, 0, s>>>(p); break;
-                        }
-                    }});
-                }
-            } else if (v == 1) {
-                if (in_dt != DT_F32 || odt != DT_F32) fatal_throw("engine: xnor path needs f32 activations");
-                if (xnor_fallback(l)) {
-                    TV pm1 = make_tv(e->act_arena + side_off[i], B, l.h, l.w, l.c, l.c, P, DT_F32, 0);
-                    const int gb = grid_for((long)B * l.h * l.w * l.c);
-                    e->ops.push_back(Op{OP_BINARIZE, i, [tin, pm1, gb](cudaStream_t s) { k_binarize_pm1<<<gb, 256, 0, s>>>(tin, pm1); }});
-                    ConvP p{};
-                    p.in = pm1; p.out = tout; p.res = TV{};
-                    p.w = e->w_arena + cw[i].w_f32;
-                    p.bias = reinterpret_cast<const float *>(e->w_arena + cw[i].bias);
-                    p.n = l.n; p.ldw = cw[i].ldw; p.size = l.size; p.stride = l.stride; p.pad = l.pad;
-                    p.act = l.activation; p.act2 = ACT_LINEAR; p.K = l.size * l.size * l.c; p.M = M;
-                    dim3 grid((unsigned)((M + 63) / 64), (unsigned)((l.n + 63) / 64));
-                    e->ops.push_back(Op{OP_CONV_SIMT, i, [p, grid](cudaStream_t s) { k_conv_simt<float, float, float, true><<<grid, 256, 0, s>>>(p); }});
-                    break;
-                }
-                int32_t *cnt_dbg = nullptr;
-                if (opt.keep_counts) {
-                    e->counts_count[i] = (size_t)B * l.n * l.out_h * l.out_w;
-                    CUDA_OK(cudaMalloc(&e->d_counts[i], e->counts_count[i] * sizeof(int32_t)));
-                    cnt_dbg = e->d_counts[i];
-                }
-                const bool in_vec = (tin.ldc % 4 == 0) && (reinterpret_cast<uintptr_t>(tin.base) & 15) == 0;
-                if (xnor_on_tc(l) && in_vec) {
-                    TV q = make_tv(e->act_arena + side_off[i], B, l.h, l.w, l.c, side_ld[i], P, DT_S8, 0);
-                    if (tc_i8_supported(l, q, tout)) {
-                        const int g = grid_for((long)B * l.h * l.w * (l.c / 16));
-                        if (!prefilled[i])
-                            e->ops.push_back(Op{OP_BINARIZE, i, [tin, q, g](cudaStream_t s) { k_binarize_s8<<<g, 256, 0, s>>>(tin, q); }});
-                        void *plan = tc_make_plan_xnor(l, q, tout, e->w_arena + cw[i].w_s8, cw[i].ldn,
-                                                       reinterpret_cast<const float *>(e->w_arena + cw[i].bias),
-                                                       reinterpret_cast<const float *>(e->w_arena + cw[i].mean), cnt_dbg,
-                                                       conv_pool_mode(i) != 0);
-                        e->tc_plans.push_back(plan);
-                        if (const int pm = conv_pool_mode(i)) {
-                            const Layer &c2 = net->layers[i + 2];
-                            TV qn = make_tv(e->act_arena + side_off[i + 2], B, c2.h, c2.w, c2.c, side_ld[i + 2], P, DT_S8, 0);
-                            if (tc_plan_fuse_pool(plan, pm, pm == 1 ? c2.input_quant_multipler : 0.f, qn)) {
-                                prefilled[i + 2] = 1; pool_in_conv[i + 1] = 1;
-                                e->not_materialised[i] = e->not_materialised[i + 1] = 1;
-                            }
-                        }
-                        e->ops.push_back(Op{OP_CONV_TC_I8, i, [plan](cudaStream_t s) { tc_launch(plan, s); }});
-                        break;
-                    }
-                    fatal_throw("engine: xnor tensor-core layer not supported by the i8 tile");
-                }
-                const int CW = side_ld[i];
-                TV bits = make_tv(e->act_arena + side_off[i], B, l.h, l.w, CW, CW, P, DT_BITS, 0);
-                {
-                    if (in_vec) {
-                        const int g = grid_for((long)B * l.h * l.w * CW);
-                        if (!prefilled[i])
-                            e->ops.push_back(Op{OP_BINARIZE, i, [tin, bits, g](cudaStream_t s) { k_binarize_vec<float><<<g, 256, 0, s>>>(tin, bits); }});
-                    } else {
-                        const long total = (long)B * l.h * l.w * CW * 32;
-                        const int g = grid_for(total);
-                        if (!prefilled[i])
-                            e->ops.push_back(Op{OP_BINARIZE, i, [tin, bits, g](cudaStream_t s) { k_binarize<float><<<g, 256, 0, s>>>(tin, bits); }});
-                    }
-                }
-                XnorP p{};
-                p.bits = bits; p.out = tout;
-                p.w = reinterpret_cast<const uint32_t *>(e->w_arena + cw[i].w_bits);
-                p.mean = reinterpret_cast<const float *>(e->w_arena + cw[i].mean);
-                p.bias = reinterpret_cast<const float *>(e->w_arena + cw[i].bias);
-                p.n = l.n; p.size = l.size; p.pad = l.pad; p.K = l.size * l.size * l.c;
-                p.padbits = (CW * 32 - l.c) * l.size * l.size;
-                p.act = l.activation; p.M = M; p.counts = cnt_dbg;
-                if (CW <= 2 && l.size == 3 && (size_t)l.n * 9 * CW * 4 <= 40 * 1024 && tout.ldc % 4 == 0) {
-                    // small K: one thread per pixel, all filters (weights broadcast from shared memory)
-                    const unsigned gsm = (unsigned)((M + 127) / 128);
-                    const size_t smem = (size_t)l.n * 9 * CW * 4;
-                    const int cw1 = CW;
-                    const int pm = (cnt_dbg == nullptr) ? conv_pool_mode(i) : 0;
-                    if (pm == 2 || pm == 3) {
-                        // the 2x2 max-pool behind this layer and the next XNOR layer's sign extraction run in this kernel
-                        const Layer &c2 = net->layers[i + 2];
-                        const TV qn = (pm == 2) ? make_tv(e->act_arena + side_off[i + 2], B, c2.h, c2.w, c2.c, side_ld[i + 2], P, DT_S8, 0)
-                                                : make_tv(e->act_arena + side_off[i + 2], B, c2.h, c2.w, side_ld[i + 2], side_ld[i + 2], P, DT_BITS, 0);
-                        const unsigned gp = (unsigned)(((long)B * c2.h * c2.w + 127) / 128);
-                        prefilled[i + 2] = 1; pool_in_conv[i + 1] = 1;
-                        e->not_materialised[i] = e->not_materialised[i + 1] = 1;
-                        e->ops.push_back(Op{OP_CONV_XNOR, i, [p, qn, gp, smem, cw1, pm](cudaStream_t s) {
-                            if (cw1 == 1 && pm == 2) k_conv_xnor_smallk_pool<1, 2><<<gp, 128, smem, s>>>(p, qn);
-                            else if (cw1 == 1) k_conv_xnor_smallk_pool<1, 3><<<gp, 128, smem, s>>>(p, qn);
-                            else if (pm == 2) k_conv_xnor_smallk_pool<2, 2><<<gp, 128, smem, s>>>(p, qn);
-                            else k_conv_xnor_smallk_pool<2, 3><<<gp, 128, smem, s>>>(p, qn);
-                        }});
-                        break;
-                    }
-                    e->ops.push_back(Op{OP_CONV_XNOR, i, [p, gsm, smem, cw1](cudaStream_t s) {
-                        if (cw1 == 1) k_conv_xnor_smallk<1><<<gsm, 128, smem, s>>>(p);
-                        else k_conv_xnor_smallk<2><<<gsm, 128, smem, s>>>(p);
-                    }});
-                    break;
-                }
-                dim3 grid((unsigned)((M + 63) / 64), (unsigned)((l.n + 63) / 64));
-                e->ops.push_back(Op{OP_CONV_XNOR, i, [p, grid](cudaStream_t s) { k_conv_xnor<<<grid, 256, 0, s>>>(p); }});
-            } else {
-                if (in_dt != DT_F32 || odt != DT_F32) fatal_throw("engine: int8 path needs f32 activations");
-                const int cpad = side_ld[i];
-                TV q = make_tv(e->act_arena + side_off[i], B, l.h, l.w, l.c, cpad, P, DT_S8, 0);
-                const float mult = l.input_quant_multipler;
-                {
-                    const long total = (long)B * l.h * l.w * (cpad / 4);
-                    const int g = grid_for(total);
-                    if (!prefilled[i])
-                        e->ops.push_back(Op{OP_QUANTIZE, i, [tin, q, mult, g](cudaStream_t s) { k_quantize<float><<<g, 256, 0, s>>>(tin, q, mult); }});
-                }
-                int *acc_dbg = nullptr;
-                if (opt.keep_counts) {
-                    e->counts_count[i] = (size_t)B * l.n * l.out_h * l.out_w;
-                    CUDA_OK(cudaMalloc(&e->d_counts[i], e->counts_count[i] * sizeof(int32_t)));
-                    acc_dbg = e->d_counts[i];
-                }
-                const float alpha1 = 32 / (l.input_quant_multipler * l.weights_quant_multipler);   // ALPHA1, ..._quantized.c:598
-                if (!getenv("YB_NO_TC") && tc_i8_supported(l, q, tout)) {
-                    // s8 x s8 -> s32 on the s8 wgmma; weights [ldn][taps][cpad] are already K-major
-                    void *plan = tc_make_plan_i8(l, q, tout, e->w_arena + cw[i].w_s8, cw[i].ldn,
-                                                 reinterpret_cast<const float *>(e->w_arena + cw[i].bias), alpha1, acc_dbg,
-                                                 conv_pool_mode(i) != 0);
-                    e->tc_plans.push_back(plan);
-                    if (const int pm = conv_pool_mode(i)) {
-                        const Layer &c2 = net->layers[i + 2];
-                        TV qn = make_tv(e->act_arena + side_off[i + 2], B, c2.h, c2.w, c2.c, side_ld[i + 2], P, DT_S8, 0);
-                        if (tc_plan_fuse_pool(plan, pm, pm == 1 ? c2.input_quant_multipler : 0.f, qn)) {
-                            prefilled[i + 2] = 1; pool_in_conv[i + 1] = 1;
-                            e->not_materialised[i] = e->not_materialised[i + 1] = 1;
-                        }
-                    }
-                    e->ops.push_back(Op{OP_CONV_TC_I8, i, [plan](cudaStream_t s) { tc_launch(plan, s); }});
-                    break;
-                }
-                Int8P p{};
-                p.q = q; p.out = tout;
-                p.w = reinterpret_cast<const uint32_t *>(e->w_arena + cw[i].w_s8);
-                p.bias = reinterpret_cast<const float *>(e->w_arena + cw[i].bias);
-                p.alpha1 = alpha1;
-                p.n = l.n; p.size = l.size; p.stride = l.stride; p.pad = l.pad; p.act = l.activation;
-                p.CW = cpad / 4; p.M = M; p.acc_out = acc_dbg;
-                dim3 grid((unsigned)((M + 63) / 64), (unsigned)((l.n + 63) / 64));
-                e->ops.push_back(Op{OP_CONV_INT8, i, [p, grid](cudaStream_t s) { k_conv_int8_simt<<<grid, 256, 0, s>>>(p); }});
-            }
-            break;
-        }
-        case YB_MAXPOOL: {
-            if (pool_in_conv[i]) break;    // done in the epilogue of the integer convolution in front of it
-            need_prev();
-            const TV tout = e->out_tv[i];
-            const int size = l.size, stride = l.stride, pad = l.pad;
-            // max-pool -> integer convolution: write the convolution's s8 / sign input directly (same values in the same
-            // order as max-pool + quantise / binarise; the pooled f32 tensor never goes to HBM)
-            if (opt.fuse && in_dt == DT_F32 && i + 1 < nl && cons[i].size() == 1 && cons[i][0] == i + 1 &&
-                net->layers[i + 1].type == YB_CONVOLUTIONAL && conv_variant(i + 1) != 0 && side_off[i + 1] != (size_t)-1 &&
-                !xnor_fallback(net->layers[i + 1]) && !getenv("YB_NO_POOL_FUSE")) {
-                const Layer &c = net->layers[i + 1];
-                const int v = conv_variant(i + 1);
-                if (v == 2) {
-                    TV q = make_tv(e->act_arena + side_off[i + 1], B, c.h, c.w, c.c, side_ld[i + 1], P, DT_S8, 0);
-                    const float mult = c.input_quant_multipler;
-                    const int g = grid_for((long)B * c.h * c.w * (q.ldc / 4));
-                    e->ops.push_back(Op{OP_MAXPOOL, i, [tin, q, size, stride, pad, mult, g](cudaStream_t s) {
-                        k_maxpool_fused<0><<<g, 256, 0, s>>>(tin, q, size, stride, pad, mult); }});
-                } else if (xnor_on_tc(c)) {
-                    TV q = make_tv(e->act_arena + side_off[i + 1], B, c.h, c.w, c.c, side_ld[i + 1], P, DT_S8, 0);
-                    const int g = grid_for((long)B * c.h * c.w * (q.ldc / 4));
-                    e->ops.push_back(Op{OP_MAXPOOL, i, [tin, q, size, stride, pad, g](cudaStream_t s) {
-                        k_maxpool_fused<1><<<g, 256, 0, s>>>(tin, q, size, stride, pad, 0.f); }});
-                } else {
-                    const int CW = side_ld[i + 1];
-                    TV bits = make_tv(e->act_arena + side_off[i + 1], B, c.h, c.w, CW, CW, P, DT_BITS, 0);
-                    const int g = grid_for((long)B * c.h * c.w * CW);
-                    e->ops.push_back(Op{OP_MAXPOOL, i, [tin, bits, size, stride, pad, g](cudaStream_t s) {
-                        k_maxpool_fused<2><<<g, 256, 0, s>>>(tin, bits, size, stride, pad, 0.f); }});
-                }
-                prefilled[i + 1] = 1;
-                e->not_materialised[i] = 1;      // fetch_layer reports it
-                break;
-            }
-            const int g = grid_for((long)B * l.out_h * l.out_w * l.out_c);
-            const int dt = in_dt;
-            const int esz = (int)dt_size(dt);
-            const bool vec = (l.out_c * esz) % 16 == 0 && (tin.ldc * esz) % 16 == 0 && (tout.ldc * esz) % 16 == 0 &&
-                             (reinterpret_cast<uintptr_t>(tin.base) & 15) == 0 && (reinterpret_cast<uintptr_t>(tout.base) & 15) == 0;
-            const int gv = grid_for((long)B * l.out_h * l.out_w * ((l.out_c * esz) / 16 + 1));
-            e->ops.push_back(Op{OP_MAXPOOL, i, [tin, tout, size, stride, pad, g, dt, vec, gv](cudaStream_t s) {
-                if (vec && dt == DT_F32) k_maxpool_vec<float><<<gv, 256, 0, s>>>(tin, tout, size, stride, pad);
-                else if (vec) k_maxpool_vec<__nv_bfloat16><<<gv, 256, 0, s>>>(tin, tout, size, stride, pad);
-                else if (dt == DT_F32) k_maxpool<float><<<g, 256, 0, s>>>(tin, tout, size, stride, pad);
-                else k_maxpool<__nv_bfloat16><<<g, 256, 0, s>>>(tin, tout, size, stride, pad);
-            }});
-            break;
-        }
-        case YB_UPSAMPLE: {
-            need_prev();
-            if (l.reverse) fatal_throw("engine: reverse upsample (downsample) is not supported");
-            const TV tout = e->out_tv[i];
-            const int stride = l.stride; const float scale = l.scale;
-            const int g = grid_for((long)B * l.out_h * l.out_w * l.out_c);
-            const int dt = in_dt;
-            const int esz = (int)dt_size(dt);
-            const bool vec = scale == 1.f && (l.out_c * esz) % 16 == 0 && (tin.ldc * esz) % 16 == 0 && (tout.ldc * esz) % 16 == 0 &&
-                             (reinterpret_cast<uintptr_t>(tin.base) & 15) == 0 && (reinterpret_cast<uintptr_t>(tout.base) & 15) == 0;
-            const int gv = grid_for((long)B * l.out_h * l.out_w * ((l.out_c * esz) / 16 + 1));
-            e->ops.push_back(Op{OP_UPSAMPLE, i, [tin, tout, stride, scale, g, dt, vec, gv, esz](cudaStream_t s) {
-                if (vec) k_upsample_vec16<<<gv, 256, 0, s>>>(tin, tout, stride, esz);
-                else if (dt == DT_F32) k_upsample<float><<<g, 256, 0, s>>>(tin, tout, stride, scale);
-                else k_upsample<__nv_bfloat16><<<g, 256, 0, s>>>(tin, tout, stride, scale);
-            }});
-            break;
-        }
-        case YB_SHORTCUT: {
-            if (is_fused_sc[i]) break;
-            need_prev();
-            const TV tout = e->out_tv[i];
-            const TV from = e->out_tv[l.index];
-            if (!from.base) fatal_throw("engine: shortcut source not placed");
-            if (e->out_dt[l.index] != in_dt) fatal_throw("engine: shortcut dtype mismatch");
-            // shortcut_cpu(batch, w1=l.w, h1=l.h, c1=l.c (from), add, w2=l.out_w, ...): yolov2_forward_network.c:410
-            int stride = l.w / l.out_w, sample = l.out_w / l.w;
-            if (stride < 1) stride = 1;
-            if (sample < 1) sample = 1;
-            const int minw = std::min(l.w, l.out_w), minh = std::min(l.h, l.out_h), minc = std::min(l.c, l.out_c);
-            const int act = l.activation;
-            const int g = grid_for((long)B * l.out_h * l.out_w * l.out_c);
-            const int dt = in_dt;
-            e->ops.push_back(Op{OP_SHORTCUT, i, [=](cudaStream_t s) {
-                if (dt == DT_F32) k_shortcut<float><<<g, 256, 0, s>>>(tin, from, tout, stride, sample, minw, minh, minc, act);
-                else k_shortcut<__nv_bfloat16><<<g, 256, 0, s>>>(tin, from, tout, stride, sample, minw, minh, minc, act);
-            }});
-            break;
-        }
-        case YB_ROUTE: {
-            if (!has_nhwc_out(i)) fatal_throw("engine: route over layers of different spatial size is not supported");
-            if (l.n == 1 && opt.fuse) break;   // alias
-            int off = 0;
-            for (int k = 0; k < l.n; ++k) {
-                const int j = l.input_layers[k];
-                const Layer &src = net->layers[j];
-                if (!(home[j].owner == i)) {
-                    const TV tsrc = e->out_tv[j];
-                    if (!tsrc.base) fatal_throw("engine: route source not placed");
-                    if (e->out_dt[j] != e->out_dt[i]) fatal_throw("engine: route dtype mismatch");
-                    TV slice = e->out_tv[i];
-                    slice.base += (size_t)off * dt_size(e->out_dt[i]);
-                    slice.C = src.out_c;
-                    const int g = grid_for((long)B * src.out_h * src.out_w * src.out_c);
-                    const int dt = e->out_dt[i];
-                    e->ops.push_back(Op{OP_ROUTE_COPY, i, [tsrc, slice, g, dt](cudaStream_t s) {
-                        if (dt == DT_F32) k_copy_channels<float><<<g, 256, 0, s>>>(tsrc, slice);
-                        else k_copy_channels<__nv_bfloat16><<<g, 256, 0, s>>>(tsrc, slice);
-                    }});
-                }
-                off += src.out_c;
-            }
-            break;
-        }
-        case YB_REORG: {
-            need_prev();
-            if (l.reverse) fatal_throw("engine: reverse reorg is not supported");
-            const TV tout = e->out_tv[i];
-            const int stride = l.stride;
-            const int g = grid_for((long)B * l.out_h * l.out_w * l.out_c);
-            const int dt = in_dt;
-            e->ops.push_back(Op{OP_REORG, i, [tin, tout, stride, g, dt](cudaStream_t s) {
-                if (dt == DT_F32) k_reorg<float><<<g, 256, 0, s>>>(tin, tout, stride);
-                else k_reorg<__nv_bfloat16><<<g, 256, 0, s>>>(tin, tout, stride);
-            }});
-            break;
-        }
-        case YB_YOLO: {
-            if (yolo_fused[i]) break;   // written by the head convolution's epilogue
-            need_prev();
-            float *dst = e->d_final[i];
-            const int classes = l.classes;
-            const int g = grid_for((long)B * ((l.h * l.w + 31) / 32) * ((l.c + 31) / 32) * 256);
-            const int dt = in_dt;
-            const int fast = (ADT == DT_BF16) ? 1 : 0;
-            e->ops.push_back(Op{OP_YOLO, i, [tin, dst, classes, g, dt, fast](cudaStream_t s) {
-                if (dt == DT_F32) k_yolo<float><<<g, 256, 0, s>>>(tin, dst, classes, fast);
-                else k_yolo<__nv_bfloat16><<<g, 256, 0, s>>>(tin, dst, classes, fast);
-            }});
-            break;
-        }
-        case YB_REGION: {
-            need_prev();
-            float *dst = e->d_final[i];
-            const int n = l.n, classes = l.classes, coords = l.coords, softmax = l.softmax;
-            const int g = grid_for((long)B * l.h * l.w * l.n);
-            const int dt = in_dt;
-            e->ops.push_back(Op{OP_REGION, i, [tin, dst, n, classes, coords, softmax, g, dt](cudaStream_t s) {
-                if (dt == DT_F32) k_region<float><<<g, 256, 0, s>>>(tin, dst, n, classes, coords, softmax);
-                else k_region<__nv_bfloat16><<<g, 256, 0, s>>>(tin, dst, n, classes, coords, softmax);
-            }});
-            break;
-        }
-        default:
-            break;
-        }
-    }
-    // last layer that is not yolo/region: keep an NCHW f32 copy as "the network output"
-    {
-        const int last = nl - 1;
-        const Layer &l = net->layers[last];
-        if (l.type != YB_YOLO && l.type != YB_REGION && e->d_final[last]) {
-            int src = last;
-            if (fused_into[last] >= 0) src = fused_into[last];
-            const TV t = e->out_tv[src];
-            if (t.base) {
-                float *dst = e->d_final[last];
-                const int dt = e->out_dt[src];
-                const int g = grid_for((long)B * l.outputs);
-                e->ops.push_back(Op{OP_YOLO, last, [t, dst, g, dt](cudaStream_t s) {
-                    if (dt == DT_F32) k_nhwc_to_nchw_f32<float><<<g, 256, 0, s>>>(t, dst);
-                    else k_nhwc_to_nchw_f32<__nv_bfloat16><<<g, 256, 0, s>>>(t, dst);
-                }});
-            }
-        }
-    }
-    (void)E;
+    b.emit_ops();
     CUDA_OK(cudaStreamSynchronize(e->stream));
     CUDA_OK(cudaGetLastError());
     return e;
@@ -1094,7 +1135,7 @@ static void engine_forward_impl(Engine *e, const void *d_input, const unsigned c
     const float *din = d_input ? reinterpret_cast<const float *>(d_input) : e->d_input;
     if (d_u8_frames) e->first_op_u8(d_u8_frames, s);   // stem straight from the 8-bit frames
     else launch_input(e, din, s);
-    if (!e->graph_exec && !e->graph_failed && getenv("YB_NO_GRAPH")) e->graph_failed = true;   // profiling aid
+    if (!e->graph_exec && !e->graph_failed && e->sw.no_graph) e->graph_failed = true;   // profiling aid
     if (!e->graph_exec && !e->graph_failed) {
         // capture everything after the input conversion once
         cudaGraph_t graph = nullptr;
@@ -1229,7 +1270,7 @@ const char *engine_broadcast_arena(const std::vector<Engine *> &reps) {
     typedef int (*BcastFn)(const void *, void *, size_t, int, int, void *, cudaStream_t);
     typedef int (*VoidFn)(void);
     typedef int (*DestroyFn)(void *);
-    void *lib = (distinct && !getenv("YB_NO_NCCL")) ? dlopen("libnccl.so.2", RTLD_NOW | RTLD_GLOBAL) : nullptr;
+    void *lib = (distinct && !reps[0]->sw.no_nccl) ? dlopen("libnccl.so.2", RTLD_NOW | RTLD_GLOBAL) : nullptr;
     if (lib) {
         InitAllFn init_all = (InitAllFn)dlsym(lib, "ncclCommInitAll");
         BcastFn bcast = (BcastFn)dlsym(lib, "ncclBroadcast");
@@ -1269,8 +1310,8 @@ void engine_fetch_layer(Engine *e, Network *net, int layer, float *dst) {
         CUDA_OK(cudaMemcpy(dst, e->d_final[layer], count * sizeof(float), cudaMemcpyDeviceToHost));
         return;
     }
- const TV t = e->out_tv[layer];
-    if (!t.base || e->not_materialised[layer]) fatal_throw("fetch_layer: layer " + std::to_string(layer) + " has no materialised output "
+    const TV t = e->out_tv[layer];
+    if (!t.base) fatal_throw("fetch_layer: layer " + std::to_string(layer) + " has no materialised output "
                              "(fused or aliased away; build the engine with fusion off)");
     float *tmp = nullptr;
     CUDA_OK(cudaMalloc(&tmp, count * sizeof(float)));
@@ -1311,7 +1352,7 @@ void engine_input_histogram(Engine *e, Network *net, int layer, int img, float b
         k_abs_hist_flat<<<grid_for(n), 256, 0, e->stream>>>(e->d_input + (size_t)img * n, n, bin_width, max_bin, d_hist);
     } else {
         const TV t = e->out_tv[layer - 1];
-        if (!t.base || e->not_materialised[layer - 1]) { cudaFree(d_hist); fatal_throw("calibrate: the input of layer " + std::to_string(layer) +
+        if (!t.base) { cudaFree(d_hist); fatal_throw("calibrate: the input of layer " + std::to_string(layer) +
                                                      " is not materialised (fused away; set option fuse=0)"); }
         const long n = (long)t.C * t.H * t.W;
         if (e->out_dt[layer - 1] == DT_F32) k_abs_hist<float><<<grid_for(n), 256, 0, e->stream>>>(t, img, bin_width, max_bin, d_hist);
@@ -1510,6 +1551,7 @@ int engine_num_launches(Engine *e) { return (int)e->ops.size(); }
 long engine_info(Engine *e, const char *key) {
     if (!strcmp(key, "launches")) return (long)e->ops.size();
     if (!strcmp(key, "tc_layers")) return e->n_tc;
+    if (!strcmp(key, "act_bytes")) return (long)e->act_bytes;
     return -1;
 }
 

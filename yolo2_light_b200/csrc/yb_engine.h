@@ -52,7 +52,7 @@ int engine_detect(Engine *e, Network *net, int w, int h, float thresh, float nms
                   float *rows, int max_rows, int *counts);   // device-side decode + NMS of the whole batch
 void engine_input_histogram(Engine *e, Network *net, int layer, int img, float bin_width, int max_bin, uint32_t *hist);
 int engine_num_launches(Engine *e);
-long engine_info(Engine *e, const char *key);   // "launches", "tc_layers"; -1 unknown
+long engine_info(Engine *e, const char *key);   // "launches", "tc_layers", "act_bytes"; -1 unknown
 int engine_profile(Engine *e, const void *d_input, int *layer_idx, int *op_kind, float *ms, int max);
 void *engine_stream(Engine *e);
 const char *op_kind_name(int k);
