@@ -140,9 +140,19 @@ float *yb_network_predict_quantized(yb_network *net, const float *input);
 /* Input pipeline on the device (SURVEY 8f row 2): replaces load_image_stb's u8 -> float/255 conversion
  * (src/additionally.c:3080-3103) + resize_image (src/additionally.c:3021-3064) + network_predict_*.
  * images_hwc: net.batch interleaved 8-bit images (HWC, net.c channels, as stbi_load returns them), all w x h.
- * The bilinear resize to the network size is bit-identical to the reference's (scalar build). */
+ * The bilinear resize to the network size is bit-identical to the reference's (scalar build).  The one-size case of
+ * yb_network_predict_frames_u8. */
 float *yb_network_predict_image_u8(yb_network *net, const unsigned char *images_hwc, int w, int h, int quantized);
-/* Diagnostic: the planar float input (batch*c*h*w) the device pipeline produced for the last call. */
+/* 1 <= nimg <= net.batch 8-bit HWC frames (net.c channels), frame b is w[b] x h[b]; each is converted and resized exactly as
+ * load_image_stb + resize_image do it (src/additionally.c:3021-3103), as the reference app does per image (src/main.c:188-229).
+ * Batch items nimg .. batch-1 are zero images.  Each frame is copied to the device on its own (frames that lie back to back
+ * in host memory in one copy); the copies overlap other work only when the frames are in pinned memory (yb_alloc_pinned),
+ * pageable frames work but each copy then serialises.  Rejected before any device work: nimg outside 1..net.batch, a null
+ * frames / w / h array or frame, w[b] < 1 or h[b] < 1, a frame of more than INT_MAX bytes. */
+float *yb_network_predict_frames_u8(yb_network *net, const unsigned char *const *frames, const int *w, const int *h,
+                                    int nimg, int quantized);
+/* Diagnostic: the planar float input (batch*c*h*w) the device pipeline produced for the last predict_image_u8 /
+ * predict_frames_u8 call. */
 int    yb_network_fetch_input(yb_network *net, int quantized, float *dst);
 
 /* Pipelined form of the two calls above for throughput serving: yb_network_submit enqueues one batch (H2D of
@@ -167,6 +177,15 @@ int yb_network_submit_u8(yb_network *net, const unsigned char *images_hwc, int w
                          float nms, int relative, int letter, int max_rows);
 int yb_network_collect_detections(yb_network *net, int ticket, int quantized, const float **rows, const int **counts,
                                   size_t *d2h_bytes);
+/* The same serving loop for frames of different sizes and partial batches: 1 <= nimg <= net.batch frames, frame b is
+ * w[b] x h[b], each resized as load_image + resize_image do it and its boxes corrected for its own size (correct_yolo_boxes
+ * src/additionally.c:4281-4315), per image as in src/main.c:188-229.  Same slots, streams and ticket rules as
+ * yb_network_submit_u8 (which is its one-size case); collected with yb_network_collect_detections, whose counts[b] is 0 for
+ * b >= nimg.  When all nimg frames have the network size the stem reads the 8-bit frames directly.  Frames as in
+ * yb_network_predict_frames_u8 (pinned memory for overlapped copies; untouched until the ticket is collected), same argument
+ * checks, and max_rows in 1..16384. */
+int yb_network_submit_frames_u8(yb_network *net, const unsigned char *const *frames, const int *w, const int *h, int nimg,
+                                int quantized, float thresh, float nms, int relative, int letter, int max_rows);
 
 /* Host output (NCHW for yolo, HWC-flattened for region, as the reference lays them out) of layer i after a
  * predict call; only YOLO/REGION layers (and the last layer) are kept on the host. */
@@ -253,6 +272,12 @@ int yb_get_network_boxes(const yb_network *net, int b, int w, int h, float thres
  * Returns the row length 5 + classes, or -1. */
 int yb_network_detect(yb_network *net, int quantized, int w, int h, float thresh, float nms, int relative, int letter,
                       float *rows, int max_rows, int *counts);
+/* yb_network_detect for the first nimg images of the batch, image b's boxes corrected for a w[b] x h[b] frame
+ * (correct_yolo_boxes src/additionally.c:4281-4315; with letter, each image's own letterbox size); counts[b] = 0 for
+ * b >= nimg.  yb_network_detect is its one-size case.  Rejected before any device work: nimg outside 1..net.batch, a null w
+ * / h array, w[b] < 1 or h[b] < 1, max_rows outside 1..16384. */
+int yb_network_detect_frames(yb_network *net, int quantized, const int *w, const int *h, int nimg, float thresh, float nms,
+                             int relative, int letter, float *rows, int max_rows, int *counts);
 
 /* ---- INT8 input calibration (SURVEY 8f row 3) ---------------------------------------------------------- */
 

@@ -4,7 +4,8 @@ decode + NMS on the GPU and the reference's bookkeeping (yb_map_evaluate) on the
 
   python tools/map.py obj.data net.cfg net.weights [--quantized] [--batch 16] [--iou 0.5] [--thresh 0.24]
 
-Images: 24-bit BMP / binary PPM; consecutive images of equal size share a batch (yb_network_predict_image_u8).
+Images: 24-bit BMP / binary PPM.  Every batch takes the next --batch images whatever their sizes, each resized and
+decoded on its own terms (yb_network_predict_frames_u8 + yb_network_detect_frames); the last batch may be partial.
 """
 import argparse, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -22,7 +23,7 @@ paths, names, truth = dataset.load_validation_set(a.data)
 net = yb.load_network(a.cfg, a.weights, batch=a.batch, quantized=int(a.quantized))
 classes = max(net.layer_desc(i).classes for i in range(net.n))
 mAP, aps, st = dataset.evaluate_map(net, paths, truth, classes, a.iou, a.thresh, a.max_rows, a.quantized,
-                                    progress=lambda i, n: print(f"\r{i}/{n}", end="", file=sys.stderr))
+                                    progress=lambda i, n: print(f"\r{i}/{n}", end="", file=sys.stderr), mixed_sizes=True)
 print(file=sys.stderr)
 for c in range(classes):
     print(f"class_id = {c}, name = {names[c] if c < len(names) else c}, \t ap = {aps[c] * 100:2.2f} % ")

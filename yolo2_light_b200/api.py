@@ -95,6 +95,9 @@ def lib():
         "yb_map_evaluate": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, C.c_int, C.c_float, C.c_float, vp, vp, vp]),
         "yb_network_detect": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_int, C.c_int, vp, C.c_int, vp]),
         "yb_network_submit_u8": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_int, C.c_int, C.c_int]),
+        "yb_network_predict_frames_u8": (fp, [vp, vp, vp, vp, C.c_int, C.c_int]),
+        "yb_network_detect_frames": (C.c_int, [vp, C.c_int, vp, vp, C.c_int, C.c_float, C.c_float, C.c_int, C.c_int, vp, C.c_int, vp]),
+        "yb_network_submit_frames_u8": (C.c_int, [vp, vp, vp, vp, C.c_int, C.c_int, C.c_float, C.c_float, C.c_int, C.c_int, C.c_int]),
         "yb_network_collect_detections": (C.c_int, [vp, C.c_int, C.c_int, C.POINTER(fp), C.POINTER(ip), C.POINTER(C.c_size_t)]),
         "yb_network_set_devices": (C.c_int, [vp, ip, C.c_int]),
         "yb_network_predict_batch": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int]),
@@ -143,7 +146,8 @@ EXPORTED_SYMBOLS = [
     "yb_network_fetch_counts", "yb_forward_convolutional_layer", "yb_network_weight_arena",
     "yb_network_last_launches", "yb_network_profile", "yb_op_kind_name", "yb_get_network_boxes", "yb_alloc_pinned",
     "yb_free_pinned", "yb_network_submit_u8", "yb_network_collect_detections", "yb_network_set_devices",
-    "yb_network_predict_batch", "yb_network_batch_output", "yb_network_replication",
+    "yb_network_predict_batch", "yb_network_batch_output", "yb_network_replication", "yb_network_predict_frames_u8",
+    "yb_network_detect_frames", "yb_network_submit_frames_u8",
 ]
 
 
@@ -260,6 +264,30 @@ class Network:
         _check(bool(p))
         return self.layer_output(self.n - 1)
 
+    def _frames(self, frames, fn: str):
+        """1..batch uint8 [h_i, w_i, c] arrays -> (keep-alive list, pointer array, w array, h array)."""
+        frames = list(frames)
+        if not 1 <= len(frames) <= self.batch:
+            raise YbError(f"{fn}: {len(frames)} frames, the network takes 1..{self.batch}")
+        keep = []
+        for k, f in enumerate(frames):
+            if not isinstance(f, np.ndarray) or f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != self.c:
+                raise YbError(f"{fn}: frame {k} must be a uint8 [h, w, c={self.c}] array, got "
+                              f"{getattr(f, 'dtype', type(f).__name__)} {getattr(f, 'shape', None)}")
+            keep.append(np.ascontiguousarray(f))
+        ptrs = (C.c_void_p * len(keep))(*[f.ctypes.data for f in keep])
+        ws = (C.c_int * len(keep))(*[f.shape[1] for f in keep])
+        hs = (C.c_int * len(keep))(*[f.shape[0] for f in keep])
+        return keep, ptrs, ws, hs
+
+    def predict_frames_u8(self, frames, quantized: bool = False) -> np.ndarray:
+        """1..batch uint8 [h_i, w_i, c] frames, each of its own size -> the reference's per-image load + resize on the device ->
+        forward (``yb_network_predict_frames_u8``).  Batch items past the frames are zero images."""
+        keep, ptrs, ws, hs = self._frames(frames, "predict_frames_u8")
+        p = lib().yb_network_predict_frames_u8(self._h, ptrs, ws, hs, len(keep), int(quantized))
+        _check(bool(p))
+        return self.layer_output(self.n - 1)
+
     def fetch_input(self, quantized: bool = False) -> np.ndarray:
         dst = np.empty((self.batch, self.c, self.h, self.w), np.float32)
         _check(lib().yb_network_fetch_input(self._h, int(quantized), dst.ctypes.data_as(C.c_void_p)) == 0)
@@ -293,20 +321,33 @@ class Network:
         t = lib().yb_network_submit_u8(self._h, x.ctypes.data_as(C.c_void_p), int(x.shape[2]), int(x.shape[1]), int(quantized),
                                        thresh, nms, relative, letter, max_rows)
         _check(t >= 0)
-        self._inflight[("u8", t)] = (x, max_rows)
+        self._inflight[("u8", t)] = (x, max_rows, self.batch)
+        return t
+
+    def submit_frames_u8(self, frames, thresh: float, nms: float = 0.45, relative: int = 1, letter: int = 0,
+                         max_rows: int = 2048, quantized: bool = False) -> int:
+        """Pipelined frames of any sizes -> detections (``yb_network_submit_frames_u8``): 1..batch uint8 [h_i, w_i, c]
+        arrays; each image's boxes are corrected for its own frame size.  Returns a ticket for collect_detections."""
+        keep, ptrs, ws, hs = self._frames(frames, "submit_frames_u8")
+        self._inflight = getattr(self, "_inflight", {})
+        t = lib().yb_network_submit_frames_u8(self._h, ptrs, ws, hs, len(keep), int(quantized), thresh, nms, relative, letter,
+                                              max_rows)
+        _check(t >= 0)
+        self._inflight[("u8", t)] = (keep, max_rows, len(keep))
         return t
 
     def collect_detections(self, ticket: int, quantized: bool = False, copy: bool = True):
-        """Returns (list of [n_b, 5 + classes] arrays, counts int32[batch], bytes moved device -> host)."""
+        """Returns (list of [n_b, 5 + classes] arrays, counts int32, bytes moved device -> host) for the ticket's images:
+        batch of them for submit_u8, nimg for submit_frames_u8."""
         rows, counts, moved = C.POINTER(C.c_float)(), C.POINTER(C.c_int)(), C.c_size_t()
         stride = lib().yb_network_collect_detections(self._h, ticket, int(quantized), C.byref(rows), C.byref(counts), C.byref(moved))
         _check(stride > 0)
-        _, max_rows = getattr(self, "_inflight", {}).pop(("u8", ticket), (None, None))
-        cnt = np.ctypeslib.as_array(counts, shape=(self.batch,)).copy()
+        _, max_rows, nimg = getattr(self, "_inflight", {}).pop(("u8", ticket), (None, None, None))
         if max_rows is None:
             raise YbError("collect_detections: unknown ticket")
+        cnt = np.ctypeslib.as_array(counts, shape=(self.batch,))[:nimg].copy()
         allrows = np.ctypeslib.as_array(rows, shape=(self.batch, max_rows, stride))
-        out = [allrows[b, :min(int(cnt[b]), max_rows)] for b in range(self.batch)]
+        out = [allrows[b, :min(int(cnt[b]), max_rows)] for b in range(nimg)]
         if copy:
             out = [o.copy() for o in out]
         return out, cnt, int(moved.value)
@@ -442,6 +483,23 @@ class Network:
                                     rows.ctypes.data_as(C.c_void_p), max_rows, counts.ctypes.data_as(C.c_void_p))
         _check(r == 5 + classes)
         return [rows[b, :min(int(counts[b]), max_rows)] for b in range(self.batch)], counts
+
+    def detect_frames(self, sizes, thresh: float, nms: float = 0.45, relative: int = 1, letter: int = 0,
+                      max_rows: int = 1024, quantized: bool = False):
+        """``yb_network_detect_frames``: decode + NMS of the first len(sizes) images on the device, image b's boxes corrected
+        for a frame of sizes[b] = (w, h).  Returns one [candidates, 5 + classes] array per image and counts int32[nimg]."""
+        sizes = [(int(w), int(h)) for w, h in sizes]
+        classes = max((self.layer_desc(i).classes for i in range(self.n) if self.layer_desc(i).type in (YB_YOLO, YB_REGION)),
+                      default=0)
+        nimg = len(sizes)
+        ws = (C.c_int * max(nimg, 1))(*[w for w, _ in sizes])
+        hs = (C.c_int * max(nimg, 1))(*[h for _, h in sizes])
+        rows = np.zeros((self.batch, max(max_rows, 1), 5 + classes), np.float32)
+        counts = np.zeros(self.batch, np.int32)
+        r = lib().yb_network_detect_frames(self._h, int(quantized), ws, hs, nimg, thresh, nms, relative, letter,
+                                           rows.ctypes.data_as(C.c_void_p), max_rows, counts.ctypes.data_as(C.c_void_p))
+        _check(r == 5 + classes)
+        return [rows[b, :min(int(counts[b]), max_rows)] for b in range(nimg)], counts[:nimg].copy()
 
 
 def map_evaluate(rows_per_image_list, truth: np.ndarray, classes: int, iou_thresh: float = 0.5,

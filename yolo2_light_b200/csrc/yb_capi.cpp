@@ -1,9 +1,11 @@
 // yb_capi.cpp -- the extern "C" surface declared in include/yolo2_light_b200.h
+#include <climits>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <memory>
 #include <string>
+#include <vector>
 
 #include "yb_engine.h"
 #include "yb_model.h"
@@ -265,12 +267,59 @@ int yb_network_collect(yb_network *n, int ticket, int quantized) {
     YB_CATCH(-1)
 }
 
+}  // extern "C"
+
+// Argument checks of the frame entry points, all before any device work.  frames_call false: the decode-only call, which
+// takes sizes alone.
+static void check_sizes(const Network &net, const char *fn, const int *w, const int *h, int nimg, bool frames_call,
+                        const unsigned char *const *frames) {
+    const std::string f(fn);
+    if (nimg < 1 || nimg > net.batch)
+        fatal_throw(f + ": nimg " + std::to_string(nimg) + " outside 1.." + std::to_string(net.batch) + " (net.batch)");
+    if (!w || !h) fatal_throw(f + ": null w / h array");
+    if (frames_call && !frames) fatal_throw(f + ": null frames array");
+    for (int b = 0; b < nimg; ++b) {
+        if (frames_call && !frames[b]) fatal_throw(f + ": frame " + std::to_string(b) + " is null");
+        if (w[b] < 1 || h[b] < 1)
+            fatal_throw(f + ": frame " + std::to_string(b) + " has size " + std::to_string(w[b]) + "x" + std::to_string(h[b]));
+        // the resize indexes within a frame in 32 bits
+        if (frames_call && (long long)w[b] * h[b] * net.c > INT_MAX)
+            fatal_throw(f + ": frame " + std::to_string(b) + " has more than INT_MAX bytes");
+    }
+}
+static void check_max_rows(const char *fn, int max_rows) {
+    if (max_rows <= 0 || max_rows > DET_MAX_ROWS)
+        fatal_throw(std::string(fn) + ": max_rows must be in 1.." + std::to_string(DET_MAX_ROWS));
+}
+
+// net.batch frames of one size, stacked: the uniform case of the frame entry points
+struct Uniform {
+    std::vector<const unsigned char *> frames;
+    std::vector<int> w, h;
+    Uniform(const Network &net, const unsigned char *images_hwc, int w_, int h_)
+        : frames(net.batch), w(net.batch, w_), h(net.batch, h_) {
+        for (int b = 0; b < net.batch; ++b) frames[b] = images_hwc + (size_t)b * w_ * h_ * net.c;
+    }
+};
+
+extern "C" {
+
 int yb_network_submit_u8(yb_network *n, const unsigned char *images_hwc, int w, int h, int quantized, float thresh, float nms,
                          int relative, int letter, int max_rows) {
     YB_TRY
     if (w <= 0 || h <= 0 || !images_hwc) fatal_throw("submit_u8: bad image");
+    const Uniform u(n->net, images_hwc, w, h);
+    return yb_network_submit_frames_u8(n, u.frames.data(), u.w.data(), u.h.data(), n->net.batch, quantized, thresh, nms,
+                                       relative, letter, max_rows);
+    YB_CATCH(-1)
+}
+int yb_network_submit_frames_u8(yb_network *n, const unsigned char *const *frames, const int *w, const int *h, int nimg,
+                                int quantized, float thresh, float nms, int relative, int letter, int max_rows) {
+    YB_TRY
+    check_sizes(n->net, "submit_frames_u8", w, h, nimg, true, frames);
+    check_max_rows("submit_frames_u8", max_rows);
     Engine *e = get_engine(n, quantized);
-    const int t = engine_submit_u8(e, &n->net, images_hwc, w, h, thresh, nms, relative, letter, max_rows);
+    const int t = engine_submit_frames(e, &n->net, frames, w, h, nimg, thresh, nms, relative, letter, max_rows);
     n->net.last_launches = engine_num_launches(e) + 5;   // + resize, count, emit, iou, nms
     return t;
     YB_CATCH(-1)
@@ -284,10 +333,18 @@ int yb_network_collect_detections(yb_network *n, int ticket, int quantized, cons
 
 float *yb_network_predict_image_u8(yb_network *n, const unsigned char *images_hwc, int w, int h, int quantized) {
     YB_TRY
-    Network &net = n->net;
     if (w <= 0 || h <= 0) fatal_throw("predict_image_u8: bad image size");
+    const Uniform u(n->net, images_hwc, w, h);
+    return yb_network_predict_frames_u8(n, u.frames.data(), u.w.data(), u.h.data(), n->net.batch, quantized);
+    YB_CATCH(nullptr)
+}
+float *yb_network_predict_frames_u8(yb_network *n, const unsigned char *const *frames, const int *w, const int *h, int nimg,
+                                    int quantized) {
+    YB_TRY
+    Network &net = n->net;
+    check_sizes(net, "predict_frames_u8", w, h, nimg, true, frames);
     Engine *e = get_engine(n, quantized);
-    engine_upload_u8(e, images_hwc, w, h, net.c, net.w, net.h, nullptr);
+    engine_upload_frames(e, &net, frames, w, h, nimg);
     engine_forward(e, nullptr, nullptr);
     engine_download_outputs(e, &net, nullptr);
     net.last_launches = engine_num_launches(e) + 1;
@@ -494,7 +551,17 @@ int yb_get_network_boxes(const yb_network *n, int b, int w, int h, float thresh,
 int yb_network_detect(yb_network *n, int quantized, int w, int h, float thresh, float nms, int relative, int letter,
                       float *rows, int max_rows, int *counts) {
     YB_TRY
-    return engine_detect(get_engine(n, quantized), &n->net, w, h, thresh, nms, relative, letter, rows, max_rows, counts);
+    const std::vector<int> ws(n->net.batch, w), hs(n->net.batch, h);
+    return yb_network_detect_frames(n, quantized, ws.data(), hs.data(), n->net.batch, thresh, nms, relative, letter, rows,
+                                    max_rows, counts);
+    YB_CATCH(-1)
+}
+int yb_network_detect_frames(yb_network *n, int quantized, const int *w, const int *h, int nimg, float thresh, float nms,
+                             int relative, int letter, float *rows, int max_rows, int *counts) {
+    YB_TRY
+    check_sizes(n->net, "detect_frames", w, h, nimg, false, nullptr);
+    check_max_rows("detect_frames", max_rows);
+    return engine_detect(get_engine(n, quantized), &n->net, w, h, nimg, thresh, nms, relative, letter, rows, max_rows, counts);
     YB_CATCH(-1)
 }
 

@@ -7,7 +7,7 @@
 //     correct_yolo_boxes         src/additionally.c:4281-4315
 //   do_nms_sort                  src/box.c:296-328  (box_iou :46-70)
 //
-// Pipeline per image (4 launches for the whole batch, grid.y = image):
+// Pipeline per image (4 launches for the first nimg images of the batch, grid.y = image):
 //   k_det_count  : candidates per 256-box block, boxes enumerated in the reference's order (layer, cell, anchor)
 //   k_det_emit   : stable compaction (block offsets + ballot scan), decode, row = {x, y, w, h, objectness, prob[classes]}
 //   k_det_iou    : bit matrix  M[i][j] = box_iou(i, j) > nms   (once per image, shared by all classes)
@@ -17,6 +17,8 @@
 // multiplies without FMA contraction) so that thresholds and IoU comparisons decide identically.
 #pragma once
 #include <cuda_runtime.h>
+
+#include "yb_kernels.cuh"   // ImageGeo
 
 namespace yb {
 
@@ -34,7 +36,8 @@ struct DetLayer {
 struct DetParams {
     DetLayer L[DET_MAX_LAYERS];
     int nl, total, classes;
-    int netw, neth, imw, imh, new_w, new_h, relative;
+    const ImageGeo *geo;     // per image: frame size and correct_yolo_boxes' embedded size
+    int netw, neth, relative;
     float thresh, nms;
     int max_rows, nblk;
 };
@@ -133,14 +136,15 @@ static __global__ void __launch_bounds__(256) k_det_emit(DetParams P, const int 
             o[5 + j] = (prob > P.thresh) ? prob : 0.f;
         }
     }
-    // correct_yolo_boxes, additionally.c:4281-4315 (mixed float / double exactly as written there)
-    x = (float)(((double)x - (double)(P.netw - P.new_w) / 2. / (double)P.netw) / (double)__fdiv_rn((float)P.new_w, (float)P.netw));
-    y = (float)(((double)y - (double)(P.neth - P.new_h) / 2. / (double)P.neth) / (double)__fdiv_rn((float)P.new_h, (float)P.neth));
-    w = __fmul_rn(w, __fdiv_rn((float)P.netw, (float)P.new_w));
-    h = __fmul_rn(h, __fdiv_rn((float)P.neth, (float)P.new_h));
+    // correct_yolo_boxes, additionally.c:4281-4315 (mixed float / double exactly as written there), for image b's frame
+    const ImageGeo &G = P.geo[b];
+    x = (float)(((double)x - (double)(P.netw - G.new_w) / 2. / (double)P.netw) / (double)__fdiv_rn((float)G.new_w, (float)P.netw));
+    y = (float)(((double)y - (double)(P.neth - G.new_h) / 2. / (double)P.neth) / (double)__fdiv_rn((float)G.new_h, (float)P.neth));
+    w = __fmul_rn(w, __fdiv_rn((float)P.netw, (float)G.new_w));
+    h = __fmul_rn(h, __fdiv_rn((float)P.neth, (float)G.new_h));
     if (!P.relative) {
-        x = __fmul_rn(x, (float)P.imw); w = __fmul_rn(w, (float)P.imw);
-        y = __fmul_rn(y, (float)P.imh); h = __fmul_rn(h, (float)P.imh);
+        x = __fmul_rn(x, (float)G.w); w = __fmul_rn(w, (float)G.w);
+        y = __fmul_rn(y, (float)G.h); h = __fmul_rn(h, (float)G.h);
     }
     o[0] = x; o[1] = y; o[2] = w; o[3] = h; o[4] = obj;
 }

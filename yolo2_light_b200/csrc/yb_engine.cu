@@ -98,7 +98,12 @@ struct Engine {
     std::function<void(const unsigned char *, cudaStream_t)> first_op_u8;   // same from 8-bit HWC frames of the network size (if set)
     int first_kind = OP_INPUT, first_layer = -1;
     void *stem_plan = nullptr;
-    unsigned char *d_u8 = nullptr; size_t u8_bytes = 0;   // staging of the caller's u8 images (device-side input pipeline)
+    struct FrameStage {                 // the caller's 8-bit frames of one batch on the device, packed back to back
+        unsigned char *buf = nullptr; size_t bytes = 0;
+        ImageGeo *d_geo = nullptr, *h_geo = nullptr;   // per-image table (batch entries) and its pinned host twin
+    };
+    FrameStage u8;                      // device-side input pipeline + decode geometry of the synchronous calls
+    float *d_unit = nullptr;            // byte value -> float /255. (k_resize_frames)
     // ---- pipelined end-to-end path: H2D(k+1) | compute(k) | D2H(k-1) on three streams -----------------
     struct DetWs {                      // decode + NMS workspace for `cap` candidate rows per image
         float *rows = nullptr; unsigned *mask = nullptr; int *blkcnt = nullptr, *counts = nullptr;
@@ -109,11 +114,12 @@ struct Engine {
         std::vector<float *> d_out, h_out;
         cudaEvent_t ev_in = nullptr, ev_comp = nullptr, ev_done = nullptr, ev_det = nullptr;
         bool busy = false;
-        // device-side input pipeline + decode of the pipelined detection path (engine_submit_u8)
-        unsigned char *d_u8 = nullptr; size_t u8_bytes = 0;
+        // device-side input pipeline + decode of the pipelined detection path (engine_submit_frames)
+        FrameStage u8;
         DetWs det;
         float *h_rows = nullptr; size_t h_rows_bytes = 0; int *h_counts = nullptr;
-        int mode = 0;                   // 0: raw tensors (engine_submit), 1: detections (engine_submit_u8)
+        int mode = 0;                   // 0: raw tensors (engine_submit), 1: detections (engine_submit_frames)
+        int nimg = 0;                   // images of the batch in this slot (mode 1)
     };
     std::vector<Slot> slots;
     cudaStream_t s_in = nullptr, s_out = nullptr, s_det = nullptr;
@@ -121,6 +127,12 @@ struct Engine {
     DetWs det;                          // workspace of the synchronous engine_detect
     ~Engine();
 };
+
+static void free_stage(Engine::FrameStage &st) {
+    if (st.buf) cudaFree(st.buf);
+    if (st.d_geo) cudaFree(st.d_geo);
+    if (st.h_geo) cudaFreeHost(st.h_geo);
+}
 
 Engine::~Engine() {
     cudaSetDevice(opt.device);
@@ -134,9 +146,10 @@ Engine::~Engine() {
     if (det.mask) cudaFree(det.mask);
     if (det.blkcnt) cudaFree(det.blkcnt);
     if (det.counts) cudaFree(det.counts);
-    if (d_u8) cudaFree(d_u8);
+    free_stage(u8);
+    if (d_unit) cudaFree(d_unit);
     for (Slot &sl : slots) {
-        if (sl.d_u8) cudaFree(sl.d_u8);
+        free_stage(sl.u8);
         if (sl.det.rows) cudaFree(sl.det.rows);
         if (sl.det.mask) cudaFree(sl.det.mask);
         if (sl.det.blkcnt) cudaFree(sl.det.blkcnt);
@@ -1111,19 +1124,80 @@ void engine_upload_input(Engine *e, const float *host_input, void *stream) {
     CUDA_OK(cudaMemcpyAsync(e->d_input, host_input, e->input_count * sizeof(float), cudaMemcpyHostToDevice, s));
 }
 
-// u8 HWC images (all `w` x `h` x `c`) -> resized planar float in the engine's input staging buffer
-void engine_upload_u8(Engine *e, const unsigned char *host_u8, int w, int h, int c, int net_w, int net_h, void *stream) {
-    cudaStream_t s = stream ? (cudaStream_t)stream : e->stream;
-    CUDA_OK(cudaSetDevice(e->opt.device));
-    const size_t bytes = (size_t)e->batch * w * h * c;
-    if (bytes > e->u8_bytes) {
-        if (e->d_u8) cudaFree(e->d_u8);
-        CUDA_OK(cudaMalloc(&e->d_u8, bytes));
-        e->u8_bytes = bytes;
+// The per-image table: frame sizes, the resize's scales, and the size correct_yolo_boxes (additionally.c:4287-4296) embeds each image at -- the
+// network size, or with `letter` the reference's integer letterbox size of that image.  Entries nimg .. batch-1 are zero.
+static void fill_geo(Engine *e, Engine::FrameStage &st, const Network *net, const int *w, const int *h, int nimg, int letter) {
+    const int B = e->batch;
+    if (!st.h_geo) {
+        CUDA_OK(cudaHostAlloc(&st.h_geo, (size_t)B * sizeof(ImageGeo), cudaHostAllocDefault));
+        CUDA_OK(cudaMalloc(&st.d_geo, (size_t)B * sizeof(ImageGeo)));
     }
-    CUDA_OK(cudaMemcpyAsync(e->d_u8, host_u8, bytes, cudaMemcpyHostToDevice, s));
-    const long total = (long)e->batch * c * net_h * net_w;
-    k_resize_u8_to_nchw<<<grid_for(total), 256, 0, s>>>(e->d_u8, e->batch, w, h, c, e->d_input, net_w, net_h);
+    for (int b = 0; b < B; ++b) {
+        ImageGeo &g = st.h_geo[b];
+        g = ImageGeo{};
+        if (b >= nimg) continue;
+        g.w = w[b]; g.h = h[b]; g.new_w = net->w; g.new_h = net->h;
+        g.w_scale = (float)(g.w - 1) / (float)(net->w - 1);   // resize_image, additionally.c:3027-3028
+        g.h_scale = (float)(g.h - 1) / (float)(net->h - 1);
+        if (letter) {
+            if (((float)net->w / g.w) < ((float)net->h / g.h)) { g.new_w = net->w; g.new_h = (g.h * net->w) / g.w; }
+            else { g.new_h = net->h; g.new_w = (g.w * net->h) / g.h; }
+        }
+    }
+}
+
+// Enqueues on `s` the copies of nimg host frames (frame b: w[b] x h[b] x c bytes) into st.buf, packed back to back, and of the
+// per-image table.  Frames that lie back to back in host memory go in one copy (a stacked batch is one copy); each copy
+// overlaps other work only from pinned memory.  Returns true when every frame has the network size.
+static bool stage_frames(Engine *e, Engine::FrameStage &st, const Network *net, const unsigned char *const *frames,
+                         const int *w, const int *h, int nimg, int letter, cudaStream_t s) {
+    const int B = e->batch, c = net->c;
+    fill_geo(e, st, net, w, h, nimg, letter);
+    size_t total = 0;
+    bool net_size = true;
+    for (int b = 0; b < nimg; ++b) {
+        st.h_geo[b].off = total;
+        total += (size_t)w[b] * h[b] * c;
+        net_size &= w[b] == net->w && h[b] == net->h;
+    }
+    // room for a zero tail of network-size frames (the 8-bit stem reads whole batches), and 16 bytes for the last vector load
+    // of k_resize_frames
+    const size_t need = std::max(total, net_size ? (size_t)B * net->w * net->h * c : 0) + 16;
+    if (need > st.bytes) {
+        if (st.buf) cudaFree(st.buf);
+        CUDA_OK(cudaMalloc(&st.buf, need));
+        st.bytes = need;
+    }
+    for (int b = 0; b < nimg;) {
+        size_t run = (size_t)w[b] * h[b] * c;
+        int nb = b + 1;
+        while (nb < nimg && frames[nb] == frames[b] + run) run += (size_t)w[nb] * h[nb] * c, ++nb;
+        CUDA_OK(cudaMemcpyAsync(st.buf + st.h_geo[b].off, frames[b], run, cudaMemcpyHostToDevice, s));
+        b = nb;
+    }
+    CUDA_OK(cudaMemcpyAsync(st.d_geo, st.h_geo, (size_t)B * sizeof(ImageGeo), cudaMemcpyHostToDevice, s));
+    return net_size;
+}
+
+// staged frames -> the network's planar f32 input; images nimg .. batch-1 are zero
+static void launch_resize(Engine *e, const Engine::FrameStage &st, const Network *net, int nimg, float *dst, cudaStream_t s) {
+    if (!e->d_unit) {   // load_image_stb's conversion, additionally.c:3093-3103
+        float unit[256];
+        for (int v = 0; v < 256; ++v) unit[v] = (float)((double)(float)v / 255.);
+        CUDA_OK(cudaMalloc(&e->d_unit, sizeof(unit)));
+        CUDA_OK(cudaMemcpy(e->d_unit, unit, sizeof(unit), cudaMemcpyHostToDevice));
+    }
+    const dim3 grid((unsigned)((net->h + RS_ROWS - 1) / RS_ROWS), (unsigned)nimg);
+    k_resize_frames<<<grid, RS_THREADS, 0, s>>>(st.buf, st.d_geo, e->d_unit, net->c, dst, net->w, net->h);
+    const size_t per = (size_t)net->c * net->h * net->w;
+    if (nimg < e->batch) CUDA_OK(cudaMemsetAsync(dst + nimg * per, 0, (e->batch - nimg) * per * sizeof(float), s));
+}
+
+// nimg u8 HWC frames of their own sizes -> resized planar float in the engine's input staging buffer
+void engine_upload_frames(Engine *e, Network *net, const unsigned char *const *frames, const int *w, const int *h, int nimg) {
+    CUDA_OK(cudaSetDevice(e->opt.device));
+    stage_frames(e, e->u8, net, frames, w, h, nimg, 0, e->stream);
+    launch_resize(e, e->u8, net, nimg, e->d_input, e->stream);
     CUDA_OK(cudaGetLastError());
 }
 
@@ -1364,10 +1438,9 @@ void engine_input_histogram(Engine *e, Network *net, int layer, int img, float b
 }
 
 // ---- batched decode + NMS on the device (yb_detect.cuh) ---------------------------------------------------------
-static constexpr int DET_MAX_ROWS = 16384;   // the per-(class, image) sort lives in shared memory: 8 B per (power-of-two) row
-
-static DetParams det_params(Engine *e, Network *net, const std::vector<float *> &finals, int w, int h, float thresh, float nms,
-                            int relative, int letter, int max_rows) {
+// geometry: P.geo, set by the caller
+static DetParams det_params(Engine *e, Network *net, const std::vector<float *> &finals, float thresh, float nms,
+                            int relative, int max_rows) {
     if (max_rows <= 0 || max_rows > DET_MAX_ROWS) fatal_throw("detect: max_rows must be in 1.." + std::to_string(DET_MAX_ROWS));
     DetParams P{};
     int total = 0;
@@ -1390,12 +1463,7 @@ static DetParams det_params(Engine *e, Network *net, const std::vector<float *> 
         P.classes = l.classes;
     }
     if (!P.nl) fatal_throw("detect: the network has no yolo / region layer");
-    P.total = total; P.netw = net->w; P.neth = net->h; P.imw = w; P.imh = h; P.relative = relative;
-    P.new_w = net->w; P.new_h = net->h;
-    if (letter) {   // correct_yolo_boxes, additionally.c:4287-4296
-        if (((float)net->w / w) < ((float)net->h / h)) { P.new_w = net->w; P.new_h = (h * net->w) / w; }
-        else { P.new_h = net->h; P.new_w = (w * net->h) / h; }
-    }
+    P.total = total; P.netw = net->w; P.neth = net->h; P.relative = relative;
     P.thresh = thresh; P.nms = nms; P.max_rows = max_rows; P.nblk = (total + 255) / 256;
     (void)e;
     return P;
@@ -1416,39 +1484,44 @@ static void det_ws_ensure(Engine::DetWs &ws, int B, const DetParams &P) {
     ws.cap = P.max_rows; ws.stride = stride; ws.nblk = P.nblk;
 }
 
-static void det_launch_count_emit(const DetParams &P, Engine::DetWs &ws, int B, cudaStream_t s) {
-    k_det_count<<<dim3((unsigned)P.nblk, (unsigned)B), 256, 0, s>>>(P, ws.blkcnt);
-    k_det_emit<<<dim3((unsigned)P.nblk, (unsigned)B), 256, 0, s>>>(P, ws.blkcnt, ws.rows, ws.counts);
+// decode of the first nimg images; counts[b] = 0 for the others
+static void det_launch_count_emit(const DetParams &P, Engine::DetWs &ws, int B, int nimg, cudaStream_t s) {
+    k_det_count<<<dim3((unsigned)P.nblk, (unsigned)nimg), 256, 0, s>>>(P, ws.blkcnt);
+    k_det_emit<<<dim3((unsigned)P.nblk, (unsigned)nimg), 256, 0, s>>>(P, ws.blkcnt, ws.rows, ws.counts);
+    if (nimg < B) CUDA_OK(cudaMemsetAsync(ws.counts + nimg, 0, (size_t)(B - nimg) * sizeof(int), s));
 }
 // nmax: upper bound of the candidates of any image (the kernels read the true counts on the device and idle beyond them)
-static void det_launch_nms(const DetParams &P, Engine::DetWs &ws, int B, int nmax, cudaStream_t s) {
+static void det_launch_nms(const DetParams &P, Engine::DetWs &ws, int nimg, int nmax, cudaStream_t s) {
     if (!(P.nms > 0.f) || nmax <= 0) return;
     const int capw = (ws.cap + 31) / 32;
-    k_det_iou<<<dim3((unsigned)((capw + 127) / 128), (unsigned)std::min(nmax, 256), (unsigned)B), 128, 0, s>>>(P, ws.rows, ws.counts, ws.mask);
+    k_det_iou<<<dim3((unsigned)((capw + 127) / 128), (unsigned)std::min(nmax, 256), (unsigned)nimg), 128, 0, s>>>(P, ws.rows, ws.counts, ws.mask);
     int P2 = 1; while (P2 < nmax) P2 <<= 1;
     const size_t smem = (size_t)P2 * 8 + (size_t)capw * 4;
     if (smem > 48 * 1024)
         CUDA_OK(cudaFuncSetAttribute(k_det_nms, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_det_nms<<<dim3((unsigned)P.classes, (unsigned)B), 256, smem, s>>>(P, ws.rows, ws.counts, ws.mask, P2);
+    k_det_nms<<<dim3((unsigned)P.classes, (unsigned)nimg), 256, smem, s>>>(P, ws.rows, ws.counts, ws.mask, P2);
 }
 
-// Synchronous form.  rows: [batch][max_rows][5 + classes]; counts[b] = candidates of image b before the max_rows cap.
-// Returns 5 + classes.
-int engine_detect(Engine *e, Network *net, int w, int h, float thresh, float nms, int relative, int letter,
-                  float *rows, int max_rows, int *counts) {
+// Synchronous form.  Image b's boxes are corrected for a w[b] x h[b] frame.  rows: [batch][max_rows][5 + classes];
+// counts[b] = candidates of image b before the max_rows cap, 0 for b >= nimg.  Returns 5 + classes.
+int engine_detect(Engine *e, Network *net, const int *w, const int *h, int nimg, float thresh, float nms, int relative,
+                  int letter, float *rows, int max_rows, int *counts) {
     CUDA_OK(cudaSetDevice(e->opt.device));
-    const DetParams P = det_params(e, net, e->d_final, w, h, thresh, nms, relative, letter, max_rows);
+    DetParams P = det_params(e, net, e->d_final, thresh, nms, relative, max_rows);
     const int B = e->batch, stride = 5 + P.classes;
     det_ws_ensure(e->det, B, P);
     cudaStream_t s = e->stream;
-    det_launch_count_emit(P, e->det, B, s);
+    fill_geo(e, e->u8, net, w, h, nimg, letter);
+    CUDA_OK(cudaMemcpyAsync(e->u8.d_geo, e->u8.h_geo, (size_t)B * sizeof(ImageGeo), cudaMemcpyHostToDevice, s));
+    P.geo = e->u8.d_geo;
+    det_launch_count_emit(P, e->det, B, nimg, s);
     std::vector<int> hc(B);
     CUDA_OK(cudaMemcpyAsync(hc.data(), e->det.counts, B * sizeof(int), cudaMemcpyDeviceToHost, s));
     CUDA_OK(cudaStreamSynchronize(s));
     int nmax = 0;
     for (int b = 0; b < B; ++b) { counts[b] = hc[b]; nmax = std::max(nmax, std::min(hc[b], max_rows)); }
-    det_launch_nms(P, e->det, B, nmax, s);
-    for (int b = 0; b < B; ++b) {
+    det_launch_nms(P, e->det, nimg, nmax, s);
+    for (int b = 0; b < nimg; ++b) {
         const int n = std::min(hc[b], max_rows);
         if (n > 0)
             CUDA_OK(cudaMemcpyAsync(rows + (size_t)b * max_rows * stride, e->det.rows + (size_t)b * max_rows * stride,
@@ -1460,18 +1533,19 @@ int engine_detect(Engine *e, Network *net, int w, int h, float thresh, float nms
 }
 
 // ---- pipelined detection path (SURVEY 8f rows 1 + 2 in the serving loop) -----------------------------------------
-// One call enqueues, for one batch of 8-bit frames: H2D of the frames + the reference's resize on the copy-in stream, the
-// forward on the compute stream, decode + NMS on a side stream (under the forward of the NEXT batch), and returns a ticket.
-// engine_collect_detections waits for that batch and copies back exactly the candidate rows.  Host traffic per batch: the
-// u8 frames in (a quarter of the float images), counts + rows out (a few hundred KB instead of the 124 MB of yolo tensors).
-int engine_submit_u8(Engine *e, Network *net, const unsigned char *host_u8, int w, int h, float thresh, float nms,
-                     int relative, int letter, int max_rows) {
+// One call enqueues, for one batch of nimg 8-bit frames of any sizes: H2D of the frames and of their geometry table + the
+// reference's resize on the copy-in stream, the forward on the compute stream, decode + NMS on a side stream (under the
+// forward of the NEXT batch), and returns a ticket.  engine_collect_detections waits for that batch and copies back exactly
+// the candidate rows.  Host traffic per batch: the u8 frames in (a quarter of the float images), counts + rows out (a few
+// hundred KB instead of the 124 MB of yolo tensors).
+int engine_submit_frames(Engine *e, Network *net, const unsigned char *const *frames, const int *w, const int *h, int nimg,
+                         float thresh, float nms, int relative, int letter, int max_rows) {
     CUDA_OK(cudaSetDevice(e->opt.device));
     ensure_slots(e);
     const int k = e->next_slot;
     Engine::Slot &sl = e->slots[k];
     if (sl.busy) fatal_throw("submit: pipeline full (3 batches in flight) -- collect the oldest ticket first");
-    const DetParams P0 = det_params(e, net, sl.d_out, w, h, thresh, nms, relative, letter, max_rows);
+    const DetParams P0 = det_params(e, net, sl.d_out, thresh, nms, relative, max_rows);
     const int B = e->batch, stride = 5 + P0.classes;
     det_ws_ensure(sl.det, B, P0);
     const size_t rows_bytes = (size_t)B * max_rows * stride * sizeof(float);
@@ -1481,24 +1555,23 @@ int engine_submit_u8(Engine *e, Network *net, const unsigned char *host_u8, int 
         sl.h_rows_bytes = rows_bytes;
     }
     if (!sl.h_counts) CUDA_OK(cudaHostAlloc(&sl.h_counts, (size_t)B * sizeof(int), cudaHostAllocDefault));
-    const size_t bytes = (size_t)B * w * h * net->c;
-    if (bytes > sl.u8_bytes) {
-        if (sl.d_u8) cudaFree(sl.d_u8);
-        CUDA_OK(cudaMalloc(&sl.d_u8, bytes));
-        sl.u8_bytes = bytes;
-    }
     e->next_slot = (k + 1) % (int)e->slots.size();
     // the previous forward that read d_in[k] must have finished before it is overwritten
     CUDA_OK(cudaStreamWaitEvent(e->s_in, sl.ev_comp, 0));
-    CUDA_OK(cudaMemcpyAsync(sl.d_u8, host_u8, bytes, cudaMemcpyHostToDevice, e->s_in));
-    const bool direct = e->first_op_u8 && w == net->w && h == net->h && net->c == 3;   // frames of the network size: no staging
-    if (!direct) {
-        const long total = (long)B * net->c * net->h * net->w;
-        k_resize_u8_to_nchw<<<grid_for(total), 256, 0, e->s_in>>>(sl.d_u8, B, w, h, net->c, sl.d_in, net->w, net->h);
+    // The slot's frames and geometry table go on s_in.  The decode below reads the table on the compute stream behind ev_in,
+    // and the next submit to this slot rewrites it only after waiting for ev_comp (above) -- and only once this ticket has
+    // been collected, which waits for ev_det, so the pinned host table is no longer being copied either.
+    const bool net_size = stage_frames(e, sl.u8, net, frames, w, h, nimg, letter, e->s_in);
+    const bool direct = e->first_op_u8 && net_size && net->c == 3;   // frames of the network size: no staging
+    if (direct) {
+        const size_t frame = (size_t)net->w * net->h * net->c;
+        if (nimg < B) CUDA_OK(cudaMemsetAsync(sl.u8.buf + nimg * frame, 0, (B - nimg) * frame, e->s_in));
+    } else {
+        launch_resize(e, sl.u8, net, nimg, sl.d_in, e->s_in);
     }
     CUDA_OK(cudaEventRecord(sl.ev_in, e->s_in));
     CUDA_OK(cudaStreamWaitEvent(e->stream, sl.ev_in, 0));
-    engine_forward_impl(e, sl.d_in, direct ? sl.d_u8 : nullptr, e->stream);
+    engine_forward_impl(e, sl.d_in, direct ? sl.u8.buf : nullptr, e->stream);
     // Candidate selection + box decode (k_det_count / k_det_emit: they read the objectness planes and, for the few candidates,
     // their class scores) run right behind the forward on the compute stream, straight on the engine's yolo tensors -- the next
     // forward overwrites those, so this is the only part that must not slip.  What follows (IoU matrix + per-class NMS) works on
@@ -1506,23 +1579,25 @@ int engine_submit_u8(Engine *e, Network *net, const unsigned char *host_u8, int 
     // 124 MB of yolo tensors into the slot first, as the raw-tensor path does, cost more than the decode itself.)
     CUDA_OK(cudaStreamWaitEvent(e->stream, sl.ev_det, 0));     // the slot's previous NMS / counts copy are done with its workspace
     DetParams P1 = P0;
+    P1.geo = sl.u8.d_geo;
     {
         int k2 = 0;
         for (size_t i = 0; i < net->layers.size(); ++i)
             if (net->layers[i].type == YB_YOLO || net->layers[i].type == YB_REGION) P1.L[k2++].p = e->d_final[i];
     }
-    det_launch_count_emit(P1, sl.det, B, e->stream);
+    det_launch_count_emit(P1, sl.det, B, nimg, e->stream);
     CUDA_OK(cudaEventRecord(sl.ev_comp, e->stream));
     CUDA_OK(cudaStreamWaitEvent(e->s_det, sl.ev_comp, 0));
     CUDA_OK(cudaMemcpyAsync(sl.h_counts, sl.det.counts, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, e->s_det));
-    det_launch_nms(P0, sl.det, B, max_rows, e->s_det);   // no host round trip: grids sized for the cap, kernels read the counts
+    det_launch_nms(P0, sl.det, nimg, max_rows, e->s_det);   // no host round trip: grids sized for the cap, kernels read the counts
     CUDA_OK(cudaEventRecord(sl.ev_det, e->s_det));
     CUDA_OK(cudaGetLastError());
-    sl.busy = true; sl.mode = 1;
+    sl.busy = true; sl.mode = 1; sl.nimg = nimg;
     return k;
 }
 
-// rows: pinned [batch][max_rows][5 + classes] (valid until the slot is reused), counts[batch]; returns 5 + classes.
+// rows: pinned [batch][max_rows][5 + classes] (valid until the slot is reused), counts[batch] (0 beyond the ticket's images);
+// returns 5 + classes.
 int engine_collect_detections(Engine *e, int ticket, const float **rows, const int **counts, size_t *d2h_bytes) {
     if (ticket < 0 || ticket >= (int)e->slots.size() || !e->slots[ticket].busy || e->slots[ticket].mode != 1)
         fatal_throw("collect_detections: bad ticket");
@@ -1531,7 +1606,7 @@ int engine_collect_detections(Engine *e, int ticket, const float **rows, const i
     CUDA_OK(cudaEventSynchronize(sl.ev_det));
     const int B = e->batch, cap = sl.det.cap, stride = sl.det.stride;
     size_t moved = (size_t)B * sizeof(int);
-    for (int b = 0; b < B; ++b) {
+    for (int b = 0; b < sl.nimg; ++b) {
         const int n = std::min(sl.h_counts[b], cap);
         if (n > 0) {
             CUDA_OK(cudaMemcpyAsync(sl.h_rows + (size_t)b * cap * stride, sl.det.rows + (size_t)b * cap * stride,

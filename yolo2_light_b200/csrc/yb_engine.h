@@ -32,7 +32,9 @@ struct Engine;
 std::shared_ptr<Engine> build_engine(Network *net, const EngineOptions &opt);
 // d_input == nullptr: use the engine's staging buffer (filled by engine_upload_input)
 void engine_upload_input(Engine *e, const float *host_input, void *stream);
-void engine_upload_u8(Engine *e, const unsigned char *host_u8, int w, int h, int c, int net_w, int net_h, void *stream);
+// nimg (1..batch) host u8 HWC frames, frame b w[b] x h[b] -> the reference's resize into the staging buffer (images
+// nimg .. batch-1 zero)
+void engine_upload_frames(Engine *e, Network *net, const unsigned char *const *frames, const int *w, const int *h, int nimg);
 void engine_forward(Engine *e, const void *d_input, void *stream);
 void engine_download_outputs(Engine *e, Network *net, void *stream);   // async D2H into pinned, then sync
 int engine_submit(Engine *e, const float *host_input);
@@ -41,15 +43,18 @@ void engine_collect_ptrs(Engine *e, int ticket, std::vector<const float *> &ptrs
 const char *engine_broadcast_arena(const std::vector<Engine *> &replicas);   // "nccl" | "peer-copy" | "single"
 int engine_device_count();
 // pipelined u8 frames -> detections (device-side resize, forward, decode + NMS; only candidate rows come back)
-int engine_submit_u8(Engine *e, Network *net, const unsigned char *host_u8, int w, int h, float thresh, float nms,
-                     int relative, int letter, int max_rows);
+int engine_submit_frames(Engine *e, Network *net, const unsigned char *const *frames, const int *w, const int *h, int nimg,
+                         float thresh, float nms, int relative, int letter, int max_rows);
 int engine_collect_detections(Engine *e, int ticket, const float **rows, const int **counts, size_t *d2h_bytes);
 void engine_fetch_layer(Engine *e, Network *net, int layer, float *dst);
 void engine_fetch_input(Engine *e, float *dst);
 int engine_fetch_counts(Engine *e, int layer, int32_t *dst, size_t count);
 void engine_weight_arena(Engine *e, void **ptr, size_t *bytes);
-int engine_detect(Engine *e, Network *net, int w, int h, float thresh, float nms, int relative, int letter,
-                  float *rows, int max_rows, int *counts);   // device-side decode + NMS of the whole batch
+// device-side decode + NMS of the first nimg images, image b's boxes corrected for a w[b] x h[b] frame
+int engine_detect(Engine *e, Network *net, const int *w, const int *h, int nimg, float thresh, float nms, int relative,
+                  int letter, float *rows, int max_rows, int *counts);
+// the per-(class, image) sort of the decode lives in shared memory: 8 B per (power-of-two) row
+constexpr int DET_MAX_ROWS = 16384;
 void engine_input_histogram(Engine *e, Network *net, int layer, int img, float bin_width, int max_bin, uint32_t *hist);
 int engine_num_launches(Engine *e);
 long engine_info(Engine *e, const char *key);   // "launches", "tc_layers", "act_bytes"; -1 unknown

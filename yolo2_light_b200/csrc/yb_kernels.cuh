@@ -75,48 +75,122 @@ __global__ void k_nhwc_to_nchw_f32(TV in, float *__restrict__ out) {
 }
 
 // ------------------------------------------------------------------------------------------------------
-// input pipeline of the reference app on the device (SURVEY 8f row 2): u8 HWC image (what stbi_load returns) ->
-// planar float /255. (load_image_stb, additionally.c:3080-3103) -> resize_image's two-pass bilinear to the network
-// size (additionally.c:3021-3064), fused: one thread per output element recomputes the two x-interpolated values it
-// needs.  Every product and sum is rounded to float exactly where the reference rounds (no FMA contraction), so the
-// result is bit-identical to the reference's scalar build.
+// input pipeline of the reference app on the device (SURVEY 8f row 2): a batch of u8 HWC frames (what stbi_load
+// returns), each of its own size -> planar float /255. (load_image_stb, additionally.c:3080-3103) -> resize_image's
+// two-pass bilinear to the network size (additionally.c:3021-3064).  Every product and sum is rounded to float exactly
+// where the reference rounds (no FMA contraction), so the result is bit-identical to the reference's scalar build.
+//
+// One block = RS_ROWS output rows of one image (grid.y = image).  Per output row it stages the byte span of the one or
+// two source rows that row reads into shared memory with 16-byte loads, then every thread makes one output pixel for all
+// c channels (the x-interpolation is computed once per pixel, not once per channel) and the planes are written with
+// coalesced stores.  The /255. conversion is a 256-entry table (`unit`, made on the host with load_image_stb's own double
+// divide) read into shared memory: no divide in the kernel.  A span wider than RS_SPAN bytes (frames several thousand pixels wide) is read from global memory
+// directly; both ways give the same values.
 // ------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ float u8_to_unit(unsigned char v) { return (float)((double)(float)v / 255.0); }
+struct ImageGeo {               // one image of a batch (device table, uploaded with the frames)
+    unsigned long long off;     // byte offset of its 8-bit frame in the packed frame buffer
+    int w, h;                   // frame size
+    int new_w, new_h;           // correct_yolo_boxes' embedded size (the network size unless letterboxed)
+    float w_scale, h_scale;     // resize_image's (w - 1) / (out_w - 1), (h - 1) / (out_h - 1): IEEE float divides, made
+                                // on the host so that the kernel has no divide
+};
 
-__device__ __forceinline__ float resize_part(const unsigned char *img, int w, int c, int k, int r, int cc, int out_w, float w_scale) {
-    // value of the reference's `part` image at (cc, r, k)
-    if (cc == out_w - 1 || w == 1) return u8_to_unit(img[k + c * (w - 1) + c * w * r]);
-    const float sx = __fmul_rn((float)cc, w_scale);
-    const int ix = (int)sx;
-    const float dx = __fsub_rn(sx, (float)ix);
-    const float a = u8_to_unit(img[k + c * ix + c * w * r]), b = u8_to_unit(img[k + c * (ix + 1) + c * w * r]);
-    return __fadd_rn(__fmul_rn(__fsub_rn(1.f, dx), a), __fmul_rn(dx, b));
+constexpr int RS_THREADS = 256, RS_ROWS = 4, RS_COLS = 1024, RS_SPAN = 12288;
+static_assert(RS_THREADS == 256, "one thread per entry of the /255. table");
+
+// frame bytes [start, start + len) -> smem; returns the smem offset of byte `start`.  The frame buffer is allocated with a
+// 16-byte tail, so the last aligned vector never leaves it.
+__device__ __forceinline__ int rs_stage(const unsigned char *__restrict__ src, size_t start, int len, uint4 *smem) {
+    const size_t a = start & ~(size_t)15;
+    const int nvec = (int)((start + len - a + 15) >> 4);
+    const uint4 *g = reinterpret_cast<const uint4 *>(src + a);
+    for (int i = threadIdx.x; i < nvec; i += RS_THREADS) smem[i] = __ldg(g + i);
+    return (int)(start - a);
 }
 
-static __global__ void k_resize_u8_to_nchw(const unsigned char *__restrict__ src, int n_img, int w, int h, int c,
-                                           float *__restrict__ dst, int out_w, int out_h) {
-    const long total = (long)n_img * c * out_h * out_w;
+static __global__ void __launch_bounds__(RS_THREADS) k_resize_frames(const unsigned char *__restrict__ src,
+                                                                      const ImageGeo *__restrict__ geo,
+                                                                      const float *__restrict__ unit_tab, int c,
+                                                                      float *__restrict__ dst, int out_w, int out_h) {
+    __shared__ uint4 stage[2][RS_SPAN / 16];
+    __shared__ float unit[256];
+    unit[threadIdx.x] = unit_tab[threadIdx.x];   // RS_THREADS == 256; published by the first barrier
+    const int n = blockIdx.y;
+    const ImageGeo g = geo[n];
+    const int w = g.w, h = g.h, rowb = w * c;          // w * h * c fits in an int (checked at the API)
+    const unsigned char *img = src + g.off;
+    float *out = dst + (size_t)n * c * out_h * out_w;
+    const size_t plane = (size_t)out_h * out_w;
     const bool same = (out_w == w && out_h == h);
-    const float w_scale = (float)(w - 1) / (float)(out_w - 1);
-    const float h_scale = (float)(h - 1) / (float)(out_h - 1);
-    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-        const int cc = (int)(i % out_w);
-        const int r = (int)((i / out_w) % out_h);
-        const int k = (int)((i / ((long)out_w * out_h)) % c);
-        const int n = (int)(i / ((long)out_w * out_h * c));
-        const unsigned char *img = src + (size_t)n * w * h * c;
-        float val;
-        if (same) {
-            val = u8_to_unit(img[k + c * cc + c * w * r]);
-        } else {
+    const float w_scale = g.w_scale, h_scale = g.h_scale;
+    const unsigned char *s0 = reinterpret_cast<const unsigned char *>(stage[0]);
+    const unsigned char *s1 = reinterpret_cast<const unsigned char *>(stage[1]);
+    const int r_end = min(out_h, (int)(blockIdx.x + 1) * RS_ROWS);
+    for (int r = blockIdx.x * RS_ROWS; r < r_end; ++r) {
+        int iy = r;
+        float dy = 0.f;
+        bool two = false;
+        if (!same) {
             const float sy = __fmul_rn((float)r, h_scale);
-            const int iy = (int)sy;
-            const float dy = __fsub_rn(sy, (float)iy);
-            val = __fmul_rn(__fsub_rn(1.f, dy), resize_part(img, w, c, k, iy, cc, out_w, w_scale));
-            if (!(r == out_h - 1 || h == 1))
-                val = __fadd_rn(val, __fmul_rn(dy, resize_part(img, w, c, k, iy + 1, cc, out_w, w_scale)));
+            iy = (int)sy;
+            dy = __fsub_rn(sy, (float)iy);
+            two = !(r == out_h - 1 || h == 1);
         }
-        dst[i] = val;
+        for (int cc0 = 0; cc0 < out_w; cc0 += RS_COLS) {
+            const int cc1 = min(out_w, cc0 + RS_COLS) - 1;      // last column of this chunk
+            // source columns the chunk reads: ix(cc0) .. ix(cc1) + 1, or the last column
+            int lo, hi;
+            if (same) { lo = cc0; hi = cc1; }
+            else if (w == 1) { lo = hi = 0; }
+            else {
+                lo = cc0 == out_w - 1 ? w - 1 : (int)__fmul_rn((float)cc0, w_scale);
+                hi = cc1 == out_w - 1 ? w - 1 : (int)__fmul_rn((float)cc1, w_scale) + 1;
+            }
+            const int len = (hi - lo + 1) * c;
+            const size_t start0 = g.off + (size_t)iy * rowb + (size_t)lo * c;
+            const bool staged = (int)(start0 & 15) + len <= RS_SPAN &&
+                                (!two || (int)((start0 + rowb) & 15) + len <= RS_SPAN);
+            const unsigned char *p0, *p1;       // byte of column `lo`, channel 0, of rows iy / iy + 1
+            __syncthreads();                    // the previous chunk is done with the staging buffers
+            if (staged) {
+                p0 = s0 + rs_stage(src, start0, len, stage[0]);
+                p1 = two ? s1 + rs_stage(src, start0 + rowb, len, stage[1]) : p0;
+                __syncthreads();
+            } else {
+                p0 = img + (size_t)iy * rowb + (size_t)lo * c;
+                p1 = p0 + rowb;
+            }
+            for (int cc = cc0 + threadIdx.x; cc <= cc1; cc += RS_THREADS) {
+                float *o = out + (size_t)r * out_w + cc;
+                if (same) {
+                    for (int k = 0; k < c; ++k) o[k * plane] = unit[p0[(cc - lo) * c + k]];
+                    continue;
+                }
+                // the reference's `part` image at (cc, row): the last column (or a 1-pixel-wide frame) copies the edge
+                const bool edge = cc == out_w - 1 || w == 1;
+                int xa = w - 1 - lo;
+                float dx = 0.f;
+                if (!edge) {
+                    const float sx = __fmul_rn((float)cc, w_scale);
+                    const int ix = (int)sx;
+                    dx = __fsub_rn(sx, (float)ix);
+                    xa = ix - lo;
+                }
+                const float ndx = __fsub_rn(1.f, dx), ndy = __fsub_rn(1.f, dy);
+                for (int k = 0; k < c; ++k) {
+                    const int ia = xa * c + k;
+                    float part0 = unit[p0[ia]];
+                    if (!edge) part0 = __fadd_rn(__fmul_rn(ndx, part0), __fmul_rn(dx, unit[p0[ia + c]]));
+                    float val = __fmul_rn(ndy, part0);
+                    if (two) {
+                        float part1 = unit[p1[ia]];
+                        if (!edge) part1 = __fadd_rn(__fmul_rn(ndx, part1), __fmul_rn(dx, unit[p1[ia + c]]));
+                        val = __fadd_rn(val, __fmul_rn(dy, part1));
+                    }
+                    o[k * plane] = val;
+                }
+            }
+        }
     }
 }
 

@@ -95,10 +95,14 @@ def load_validation_set(datacfg: str):
 
 
 def evaluate_map(net, paths, truth: np.ndarray, classes: int, iou_thresh: float = 0.5, thresh_calc_avg_iou: float = 0.24,
-                 max_rows: int = 8192, quantized: bool = False, progress=None):
+                 max_rows: int = 8192, quantized: bool = False, progress=None, mixed_sizes: bool = False):
     """The loop of ``validate_detector_map`` (additionally.c:4614-4780) around any object with ``batch``,
     ``predict_image_u8(images_u8[batch, h, w, 3], quantized=)`` and ``detect(w, h, thresh, nms, relative=, letter=,
-    max_rows=, quantized=)`` -- ``yolo2_light_b200.Network`` -- then ``yb_map_evaluate``.  Returns (mAP, ap[classes], stats)."""
+    max_rows=, quantized=)`` -- ``yolo2_light_b200.Network`` -- then ``yb_map_evaluate``.  Returns (mAP, ap[classes], stats).
+
+    mixed_sizes=True uses ``predict_frames_u8(list of [h_i, w_i, 3] frames, quantized=)`` and ``detect_frames(sizes, ...)``
+    instead: every batch takes the next ``batch`` images whatever their sizes, and the last one is a partial batch, so a
+    dataset whose images rarely share a size runs ``batch`` images per forward rather than about one."""
     from . import api
     rows = []
     B = net.batch
@@ -119,6 +123,22 @@ def evaluate_map(net, paths, truth: np.ndarray, classes: int, iou_thresh: float 
         if progress:
             progress(done, len(paths))
 
+    def flush_mixed(chunk):
+        nonlocal done
+        net.predict_frames_u8(chunk, quantized=quantized)
+        dets, counts = net.detect_frames([(1, 1)] * len(chunk), 0.005, 0.45, relative=0, letter=0, max_rows=max_rows,
+                                         quantized=quantized)
+        if max(counts) > max_rows:
+            raise ValueError(f"{max(counts)} candidates in one image, only {max_rows} kept: raise max_rows")
+        rows.extend(dets)
+        done += len(chunk)
+        if progress:
+            progress(done, len(paths))
+
+    if mixed_sizes:
+        for first in range(0, len(paths), B):
+            flush_mixed([read_image_u8(p) for p in paths[first:first + B]])
+        return api.map_evaluate(rows, truth, classes, iou_thresh, thresh_calc_avg_iou)
     chunk = []
     for p in paths:                                                # images of one size share a batch, order is kept
         img = read_image_u8(p)
