@@ -460,7 +460,7 @@ def test_fused_stem_pool_is_bit_identical_to_the_three_kernels(builder, w, h, q,
     for i, o in a.detection_outputs().items():
         assert util.rel_l2(o, b.layer_output(i)) <= 1e-5, (builder.__name__, i)
     # production configuration (no raw-accumulator dump): the max-pools behind the integer convolutions run in their epilogues
-    # (tc_plan_fuse_pool) -- every integer layer that is still materialised is bit-identical to the unfused plan
+    # (TcConv::pool_mode) -- every integer layer that is still materialised is bit-identical to the unfused plan
     c = yb.load_network(cfg, wts, batch=B, quantized=q)
     c.predict(x, quantized=bool(q))
     assert c.last_launches() < b.last_launches()

@@ -32,6 +32,7 @@
 #include <climits>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <type_traits>
 #include <vector>
@@ -79,7 +80,6 @@ struct TcParams {
     // Non-zero for every k_conv_tc_reg plan (bf16 slabs) and for the stride-1 integer kinds without the raw-accumulator dump
     // (f32 slabs of k_conv_tc); the other k_conv_tc plans store through the per-warp LSU staging tiles.
     int tma_epi;
-    int l2_hint;              // 1: shortcut tiles are loaded with the L2 evict-first policy
     uint32_t stg_bytes;       // epilogue staging / TMA-epilogue tiles
     int acc_pitch;            // words per row of the shared-memory accumulator tile (BN + 4: conflict-free row reads)
     // Fused 2x2 / stride-2 max-pool + input conversion of the NEXT integer layer (integer kinds, tiles of 8 x 16 pixels):
@@ -91,13 +91,12 @@ struct TcParams {
     float pool_mult;
     signed char *pool_out; long pool_ldc; int pool_Hp, pool_Wp;   // next layer's s8 input: padded NHWC, bytes
     int sps;                                  // K-blocks per pipeline stage (amortises the per-stage barrier round trip)
-    int kbs;                                  // pipeline stages per work item = ceil(kblocks / sps)
     uint32_t desc_hi;         // high word of the wgmma shared-memory descriptors (SBO, swizzle mode)
     char *out; long out_ldc; int n, n_store;
     const char *res;          // fused shortcut operand (bf16, k_conv_tc_reg at stride 1 only), or null
     const float *bias; int act, act2;
     unsigned long long *stats; // YB_TC_STATS=1: per-CTA cycle counters [grid][16] (diagnostic)
-    int dbg;                  // YB_TC_DBG bit mask for bottleneck experiments: 1 no TMA, 2 no MMA, 4 no epilogue memory ops
+    int dbg;                  // YB_TC_DBG bit mask for bottleneck experiments: 1 no TMA, 4 no epilogue memory ops
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -459,7 +458,7 @@ __device__ __forceinline__ float int_epilogue(const TcParams &p, int kind, int a
 template <bool ST, int EPI>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
-          const __grid_constant__ CUtensorMap tmR, const TcParams p) {
+          const TcParams p) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smemB = (smem_u32(smem_raw) + 1023u) & ~1023u;   // 128B swizzle atoms are 1024B aligned
     const uint32_t smem0 = smemB + p.bstat_bytes;                   // [resident filter matrix][pipeline ring]
@@ -548,9 +547,9 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
         const int cend = (p.BN >= 64) ? cbeg + (p.BN >> 1) : (half == 0 ? p.BN : 0);
         const int r = q * 32 + lane;              // accumulator row == pixel within the tile
         const int tx = r & (p.TW - 1), ty = r >> p.TWlog2;
-        const bool leaky = p.act == ACT_LEAKY, leaky2 = p.act2 == ACT_LEAKY;
+        const bool leaky = p.act == ACT_LEAKY;
         const uint32_t taddr = acc_base + 4u * (uint32_t)(r * p.acc_pitch);
-        long long w_res = 0; const long long t_begin = ST ? clock64() : 0;
+        const long long t_begin = ST ? clock64() : 0;
         for (int w = w_first; w < p.num_work; w += w_step) {
             run_mainloop();
             const int n_idx = w % p.nt;
@@ -734,8 +733,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
             }
         }
         if (EPI == 2 && p.tma_epi && q == 0 && lane == 0) tma_store_wait_all();   // this group's bulk stores have completed
-        if (ST && p.stats && ew == 0 && lane == 0) { p.stats[blockIdx.x * 16 + 2] = (unsigned long long)w_full; p.stats[blockIdx.x * 16 + 6] = (unsigned long long)(clock64() - t_begin);
-                                                     p.stats[blockIdx.x * 16 + 8] = (unsigned long long)w_res; }
+        if (ST && p.stats && ew == 0 && lane == 0) { p.stats[blockIdx.x * 16 + 2] = (unsigned long long)w_full; p.stats[blockIdx.x * 16 + 6] = (unsigned long long)(clock64() - t_begin); }
     }
 }
 
@@ -762,7 +760,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
 // row) land on that image's bottom border, and the epilogue writes them as zeros.  A half tile that straddles two images goes out
 // one tile row at a time through tmO1 (box: SW channels x TW pixels x 1 row), skipping the rows with oy == OH and those past the
 // batch: no store touches an image's top border or needs a negative row (bulk tensor stores fault on negative coordinates).
-// Tile row t of a slab starts at byte t * TW * 2 SW.  Bulk tensor copies need 128-byte aligned shared memory (make_plan_common
+// Tile row t of a slab starts at byte t * TW * 2 SW.  Bulk tensor copies need 128-byte aligned shared memory (plan_tiles
 // keeps TW * SW >= 64), and the TMA engine takes the swizzle phase from the shared-memory address (16-byte chunk c of the
 // 128-byte row at address a is chunk c ^ ((a >> 7) & 7) at 128B, c ^ ((a >> 7) & 3) at 64B), the rule slab_off follows from
 // the 1024-byte aligned buffer: a row box that starts off the swizzle's 1024 / 512-byte repeat reads its rows as written.
@@ -811,8 +809,7 @@ __device__ __forceinline__ void tcr_store(const CUtensorMap *tmO, const CUtensor
         else tma_store_wait_read0();
     };
     auto load_res = [&](int s, int n0, int x, int y) {
-        if (p.l2_hint) tma_load_3d_hint(buf + (uint32_t)s * tile, tmR, stg_ready, n0 + s * SW, x, y, l2_policy_evict_first());
-        else tma_load_3d(buf + (uint32_t)s * tile, tmR, stg_ready, n0 + s * SW, x, y);
+        tma_load_3d_hint(buf + (uint32_t)s * tile, tmR, stg_ready, n0 + s * SW, x, y, l2_policy_evict_first());
     };
     if (w_first < p.num_work) {   // the first item's residual overlaps the first main loop
         if (p.res) {
@@ -1464,13 +1461,36 @@ struct TcPlan {
     int grid;
     int threads;                      // TC_THREADS (k_conv_tc) or TCR_THREADS (k_conv_tc_reg)
     size_t smem;
-    int pdl;
     char desc[96];
 };
 
-int pick_bk(int C) { return (C % 64 == 0) ? 64 : (C % 32 == 0) ? 32 : (C % 16 == 0) ? 16 : 0; }
-int pick_bk_i8(int cpad) { return (cpad % 128 == 0) ? 128 : (cpad % 64 == 0) ? 64 : (cpad % 32 == 0) ? 32 : 0; }
-int pick_bk_f32(int C) { return (C % 32 == 0) ? 32 : (C % 16 == 0) ? 16 : (C % 8 == 0) ? 8 : 0; }
+int sm_count() {
+    int dev = 0, sms = 132;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    return sms;
+}
+
+bool is_integer(int kind) { return kind == TC_S8 || kind == TC_XNOR; }
+int elem_size(int kind) { return kind == TC_TF32 ? 4 : is_integer(kind) ? 1 : 2; }   // operand element size
+// operand channels per pixel: the integer kinds read the s8 input's zero-padded channels (their weights are padded alike)
+int operand_channels(const TcConv &c) { return is_integer(c.kind) ? c.in.ldc : c.l->c; }
+
+// The filter geometries of the implicit GEMM: 3x3 / pad 1 and 1x1 / pad 0 at stride 1; 3x3 / pad 1 at stride 2 on even sizes
+// (the 5-D view splits x and y into (half, parity))
+bool geometry_ok(const Layer &l) {
+    if (l.stride == 1) return (l.size == 3 && l.pad == 1) || (l.size == 1 && l.pad == 0);
+    return l.stride == 2 && l.size == 3 && l.pad == 1 && l.h % 2 == 0 && l.w % 2 == 0;
+}
+
+// Channels per K-block: the widest 128 / 64 / 32-byte row (a TMA / wgmma swizzle width) that divides `channels` elements of
+// esz bytes, or 0
+int channel_row(int channels, int esz) {
+    for (int bytes = 128; bytes >= 32; bytes /= 2)
+        if (channels * esz % bytes == 0) return bytes / esz;
+    return 0;
+}
+
 // k_conv_tc: at most 128 filters per tile -- the [128][BN + 4] f32 accumulator tile shares the 227 KB of shared memory with the ring
 int pick_bn(int n) { return n <= 32 ? 32 : n <= 64 ? 64 : 128; }
 // k_conv_tc_reg: BN in {32, 64, 128, 256} (no wider than the filters need) with the least wave-quantised cost
@@ -1503,295 +1523,226 @@ int grid_cap(int sms) {
     return (e && atoi(e) > 0) ? std::min(sms, atoi(e)) : sms;
 }
 
-}  // namespace
-
-int tc_conv_supported(const Layer &l, const TV &in, const TV &out, bool out_bf16) {
-    if (!out.base || (reinterpret_cast<uintptr_t>(out.base) & 15) != 0) return 0;
-    if (out_bf16 ? (out.ldc % 8 != 0) : (out.ldc % 4 != 0)) return 0;
-    if (l.activation != YB_LEAKY && l.activation != YB_LINEAR) return 0;
-    if (pick_bk(l.c) == 0) return 0;
-    if (in.ldc % 8 != 0 || (reinterpret_cast<uintptr_t>(in.base) & 15) != 0 || in.P != 1) return 0;
-    const bool s1 = l.stride == 1 && ((l.size == 3 && l.pad == 1) || (l.size == 1 && l.pad == 0));
-    const bool s2 = l.stride == 2 && l.size == 3 && l.pad == 1 && (l.h % 2 == 0) && (l.w % 2 == 0);
-    if (!s1 && !s2) return 0;
-    if (out_bf16 && l.n % 8 != 0) return 0;
-    if (l.n < 8) return 0;
-    return 1;
-}
-
-static void *make_plan_common(int kind, const Layer &l, const TV &in, const TV &out, bool out_bf16, const TV &res,
-                              bool res_bf16, int act2, const void *d_weights_bf16, int ldn, const float *d_bias,
-                              float alpha1, int *acc_out, int wide_rows = 0, int want_pool_tile = 0) {
-    TcPlan *plan = new TcPlan();
-    memset(plan, 0, sizeof(*plan));
-    TcParams &p = plan->p;
-    const bool i8 = kind == 1 || kind == 2;
-    const int esz = kind == 3 ? 4 : i8 ? 1 : 2;              // operand element size
-    const int cin = i8 ? in.ldc : l.c;                       // s8: channels padded with zeros in both operands
-    const int BK = kind == 3 ? pick_bk_f32(l.c) : i8 ? pick_bk_i8(cin) : pick_bk(l.c);
-    // bf16 NHWC output: the register-accumulator kernel with its TMA epilogue
-    const bool reg = kind == 0 && out_bf16;
-    p.kind = kind; p.alpha1 = alpha1; p.acc_out = acc_out;
-    p.kk = BK * esz / 32;
+// Geometry, K-blocks, tile shape, filter tile width and the resident filter matrix.  reg: k_conv_tc_reg runs the plan.
+void plan_tiles(TcParams &p, const TcConv &c, bool reg, int sms) {
+    const Layer &l = *c.l;
     const bool s2 = l.stride == 2;
-    p.N = in.N;
-    p.OH = l.out_h; p.OW = l.out_w; p.OHp = out.Hp; p.OWp = out.Wp;
-    p.size = l.size; p.BK = BK;
-    p.cblocks = cin / BK; p.kblocks = l.size * l.size * p.cblocks;
+    const int esz = elem_size(c.kind), cin = operand_channels(c);
+    p.kind = c.kind;
+    p.N = c.in.N;
+    p.OH = l.out_h; p.OW = l.out_w; p.OHp = c.out.Hp; p.OWp = c.out.Wp;
+    p.size = l.size; p.BK = channel_row(cin, esz);
+    p.kk = p.BK * esz / 32;
+    p.cblocks = cin / p.BK; p.kblocks = l.size * l.size * p.cblocks;
     p.stride2 = s2 ? 1 : 0;
     p.xoff = 1 - l.pad; p.yoff = -l.pad;
-    p.PR = s2 ? (in.Hp / 2) : in.Hp;
+    p.PR = s2 ? (c.in.Hp / 2) : c.in.Hp;
     p.row_off = s2 ? 0 : 1;
+    // wgmma descriptor high word: SBO (8 rows * row bytes) >> 4 at bits 32..45, swizzle mode at 62..63 (1: 128B, 2: 64B, 3: 32B)
+    const uint32_t row_bytes = 32u * (uint32_t)p.kk;
+    p.desc_hi = ((8u * row_bytes) >> 4) | ((row_bytes == 128 ? 1u : row_bytes == 64 ? 2u : 3u) << 30);
+
     // tile width: power of two minimising padded work
-    const long rows = (long)in.N * p.PR;
-    double best = 1e30; int bestTW = 1;
-    for (int tw = 1; tw <= 128; tw *= 2) {
+    const long rows = (long)p.N * p.PR;
+    auto padded = [&](int tw) {
         const int th = 128 / tw;
-        const double cost = (double)((p.OW + tw - 1) / tw) * tw * (double)((rows + th - 1) / th) * th;
-        if (cost < best - 0.5) { best = cost; bestTW = tw; }
+        return (double)((p.OW + tw - 1) / tw) * tw * (double)((rows + th - 1) / th) * th;
+    };
+    double best = 1e30; int tw = 1;
+    for (int t = 1; t <= 128; t *= 2)
+        if (padded(t) < best - 0.5) { best = padded(t); tw = t; }
+    if (c.yolo_out) {
+        // the epilogue scatters NCHW planes (fused [yolo]): a warp's 32 accumulator rows should be as few image-row runs as
+        // possible, so take the widest tile whose padded work stays within 30 % of the minimum
+        for (int t = 64; t > tw; t /= 2)
+            if (padded(t) <= 1.3 * best) { tw = t; break; }
     }
-    if (wide_rows) {
-        // the epilogue will scatter NCHW planes (fused [yolo]): a warp's 32 accumulator rows should be as few image-row
-        // runs as possible, so take the widest tile whose padded work stays within 30 % of the minimum
-        for (int tw = 64; tw > bestTW; tw /= 2) {
-            const int th = 128 / tw;
-            const double cost = (double)((p.OW + tw - 1) / tw) * tw * (double)((rows + th - 1) / th) * th;
-            if (cost <= 1.3 * best) { bestTW = tw; break; }
-        }
-    }
-    // want_pool_tile: a fused 2x2 max-pool (tc_plan_fuse_pool) needs 8 x 16 tiles that start one merged row down -- row 0 is a
-    // border row, and 2x2 windows then never straddle tiles
-    const bool pool_tile = want_pool_tile && !s2 && l.size == 3;
-    if (pool_tile) bestTW = 8;
-    p.TW = bestTW; p.TH = 128 / bestTW;
-    p.TWlog2 = 0; while ((1 << p.TWlog2) < p.TW) ++p.TWlog2;
-    p.jshift = pool_tile ? 1 : 0;
-    int sms = 132;
-    { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); }
-    const uint32_t row_bytes = (uint32_t)(BK * esz);
-    p.xt = (p.OW + p.TW - 1) / p.TW;
-    p.jt = (int)((rows - p.jshift + p.TH - 1) / p.TH);
-    const int BN = reg ? pick_bn_reg(l.n, (long)p.xt * p.jt, p.kblocks, sms) : pick_bn(l.n);
-    if (reg && s2 && BN == 32 && p.TW == 1) {
-        // k_conv_tc_reg stores straddling stride-2 half tiles one tile row at a time, from byte t * TW * 2 SW of a slab: with
-        // 64-byte slab rows (SW = 32) and TW = 1 that is not 128-byte aligned, as bulk tensor copies need
-        p.TW = 2; p.TH = 64; p.TWlog2 = 1;
+    // a fused 2x2 max-pool needs 8 x 16 tiles that start one merged row down -- row 0 is a border row, and 2x2 windows then
+    // never straddle tiles
+    if (c.pool_mode) tw = 8;
+    p.jshift = c.pool_mode ? 1 : 0;
+    auto set_tw = [&](int t) {
+        p.TW = t; p.TH = 128 / t;
+        p.TWlog2 = 0; while ((1 << p.TWlog2) < p.TW) ++p.TWlog2;
         p.xt = (p.OW + p.TW - 1) / p.TW;
         p.jt = (int)((rows - p.jshift + p.TH - 1) / p.TH);
-    }
-    p.BN = BN;
-    p.nt = (l.n + BN - 1) / BN;
+    };
+    set_tw(tw);
+    p.BN = reg ? pick_bn_reg(l.n, (long)p.xt * p.jt, p.kblocks, sms) : pick_bn(l.n);
+    // k_conv_tc_reg stores straddling stride-2 half tiles one tile row at a time, from byte t * TW * 2 SW of a slab: with
+    // 64-byte slab rows (SW = 32) and TW = 1 that is not 128-byte aligned, as bulk tensor copies need
+    if (reg && s2 && p.BN == 32 && p.TW == 1) set_tw(2);
+    p.nt = (l.n + p.BN - 1) / p.BN;
     p.num_work = p.xt * p.jt * p.nt;
-    p.a_bytes = (uint32_t)(TC_BM * BK * esz);
-    p.b_bytes = (uint32_t)(BN * BK * esz);
+    p.a_bytes = (uint32_t)(TC_BM * p.BK * esz);
+    p.b_bytes = (uint32_t)(p.BN * p.BK * esz);
     // small filter matrices stay resident in shared memory for the whole kernel (one TMA pass per CTA)
     p.bstat = (p.nt == 1 && (size_t)p.kblocks * p.b_bytes <= 48 * 1024 && !getenv("YB_TC_NO_BSTAT")) ? 1 : 0;
     p.bstat_bytes = p.bstat ? (uint32_t)p.kblocks * p.b_bytes : 0u;
-    // TMA epilogue: slab width in columns.  k_conv_tc_reg: bf16 slabs of 64 columns (32 when BN == 32), per consumer warpgroup
-    // one staging buffer of 64 pixels x BN (64 / 32 / 16 / 8 KB per CTA at BN = 256 / 128 / 64 / 32); integer kinds: f32 slabs of
-    // 32 columns (128-byte rows), one 128-pixel tile per warp group -- the raw-accumulator dump (tests) keeps the LSU path
-    p.tma_epi = 0;
-    if (reg) p.tma_epi = BN >= 64 ? 64 : 32;
-    if (i8 && !s2 && !acc_out) p.tma_epi = 32;
-    p.stg_bytes = reg ? 2u * 64u * (uint32_t)BN * 2u : p.tma_epi ? 2u * 16384u : 4096u * TC_EPI_WARPS;
-    p.acc_pitch = BN + 4;
-    const size_t acc_bytes = reg ? 0 : (size_t)TC_BM * p.acc_pitch * 4;   // k_conv_tc_reg keeps the accumulators in registers
-    // what is left of 227 KB beside the epilogue tiles and the accumulator tile (5 KB: barriers, alignment slack)
-    const size_t ring_budget = (size_t)(227 - 5) * 1024 - p.stg_bytes - acc_bytes;
-    // several K-blocks per stage when they are small: fewer barrier round trips per K
-    const uint32_t sps_target = getenv("YB_TC_SPS_TARGET") ? (uint32_t)atoi(getenv("YB_TC_SPS_TARGET")) : 32u * 1024u;
-    const uint32_t ring_blk = p.a_bytes + (p.bstat ? 0u : p.b_bytes);
-    p.sps = (int)std::max<uint32_t>(1, std::min<uint32_t>(4, sps_target / std::max(ring_blk, 1u)));
-    if (getenv("YB_TC_SPS")) p.sps = std::max(1, atoi(getenv("YB_TC_SPS")));
-    p.sps = std::min(p.sps, p.kblocks);
-    const size_t fixed_smem = sizeof(float) * (size_t)p.nt * BN + (size_t)p.nt * BN / 8;
-    if (ring_budget < p.bstat_bytes + fixed_smem + 2 * (size_t)ring_blk) fatal_throw("tc plan: tile does not fit shared memory");
-    {   // keep the ring at least 3 stages deep
-        const size_t avail = ring_budget - p.bstat_bytes - fixed_smem;
-        while (p.sps > 1 && avail / ((size_t)p.sps * ring_blk) < 3) --p.sps;
-    }
-    p.stage_bytes = (uint32_t)p.sps * ring_blk;
-    p.kbs = (p.kblocks + p.sps - 1) / p.sps;
-    const size_t max_stages = getenv("YB_TC_MAX_STAGES") ? (size_t)atoi(getenv("YB_TC_MAX_STAGES")) : 8;
-    p.stages = (int)std::min<size_t>(max_stages, (ring_budget - p.bstat_bytes - fixed_smem) / p.stage_bytes);
-    if (p.stages < 2) fatal_throw("tc plan: tile does not fit shared memory");
-    // wgmma descriptor high word: SBO (8 rows * row bytes) >> 4 at bits 32..45, swizzle mode at 62..63 (1: 128B, 2: 64B, 3: 32B)
-    const uint32_t layout_type = row_bytes == 128 ? 1u : row_bytes == 64 ? 2u : 3u;
-    p.desc_hi = ((8u * row_bytes) >> 4) | (layout_type << 30);
-    p.out = out.base; p.out_ldc = out.ldc;
+}
+
+// The epilogue: the output, the per-kind parameters, the fusions and the staging tiles.  k_conv_tc_reg (reg): bf16 slabs of 64
+// columns (32 when BN == 32) stored by TMA, per consumer warpgroup one staging buffer of 64 pixels x BN (64 / 32 / 16 / 8 KB per
+// CTA at BN = 256 / 128 / 64 / 32).  k_conv_tc: the stride-1 integer kinds store f32 slabs of 32 columns (128-byte rows) by TMA,
+// one 128-pixel tile per warp group; the raw-accumulator dump (tests) and the float kinds store through per-warp LSU staging tiles.
+void plan_epilogue(TcParams &p, const TcConv &c, bool reg) {
+    const Layer &l = *c.l;
+    p.tma_epi = reg ? (p.BN >= 64 ? 64 : 32) : (is_integer(c.kind) && !p.stride2 && !c.acc_out) ? 32 : 0;
+    p.stg_bytes = reg ? 2u * 64u * (uint32_t)p.BN * 2u : p.tma_epi ? 2u * 16384u : 4096u * TC_EPI_WARPS;
+    p.acc_pitch = p.BN + 4;
+    p.out = c.out.base; p.out_ldc = c.out.ldc;
     p.n = l.n;
     // f32: whole float4 groups, within the output's pixel stride (a fused [yolo] head has no NHWC output)
-    p.n_store = out_bf16 ? l.n : out.base ? std::min<int>((l.n + 3) / 4 * 4, out.ldc) : (l.n + 3) / 4 * 4;
-    if (!out_bf16 && (out.ldc % 4 != 0)) fatal_throw("tc plan: f32 output rows must be 16-byte aligned");
-    p.res = res.base;
-    if (res.base && (res.H != l.out_h || res.W != l.out_w || res.C != l.n)) fatal_throw("tc plan: residual shape mismatch");
-    if (res.base && !res_bf16) fatal_throw("tc plan: residual must be bf16");
-    if (res.base && !out_bf16) fatal_throw("tc plan: a fused residual needs a bf16 output");
-    if (res.base && s2) fatal_throw("tc plan: a fused residual needs a stride-1 layer");
-    if (reg && s2 && out.P != 1) fatal_throw("tc plan: a stride-2 output needs a border of 1");
-    if (res.base && res_bf16 && (res.ldc % 8 != 0 || (reinterpret_cast<uintptr_t>(res.base) & 15))) fatal_throw("tc plan: residual alignment");
-    p.bias = d_bias; p.act = l.activation; p.act2 = act2;
-    p.dbg = getenv("YB_TC_DBG") ? atoi(getenv("YB_TC_DBG")) : 0;
-    p.l2_hint = (kind == 0 && !getenv("YB_TC_NO_L2_HINT")) ? 1 : 0;
-    snprintf(plan->desc, sizeof(plan->desc), "%dx%dx%d -> n%d k%d s%d%s", l.c, l.h, l.w, l.n, l.size, l.stride, reg ? " reg" : "");
+    p.n_store = c.out_bf16 ? l.n : c.out.base ? std::min<int>((l.n + 3) / 4 * 4, c.out.ldc) : (l.n + 3) / 4 * 4;
+    p.res = c.res.base;
+    p.bias = c.bias; p.act = l.activation; p.act2 = c.act2;
+    p.alpha1 = c.alpha1;
+    p.mean = c.mean;
+    p.xK = l.size * l.size * l.c;
+    p.acc_out = c.acc_out;
+    p.yolo_out = c.yolo_out;
+    p.yolo_per = c.yolo_out ? 4 + c.yolo_classes + 1 : 0;
+    p.pool_mode = c.pool_mode; p.pool_mult = c.pool_mult;
+    p.pool_out = reinterpret_cast<signed char *>(c.pool_next.base); p.pool_ldc = c.pool_next.ldc;
+    p.pool_Hp = c.pool_next.Hp; p.pool_Wp = c.pool_next.Wp;
+}
 
-    const CUtensorMapSwizzle swz = row_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
-                                 : row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
+// The operand ring: K-blocks per stage and stages, in what is left of 227 KB beside the epilogue's tiles (acc_bytes: k_conv_tc's
+// accumulator tile)
+void plan_ring(TcParams &p, size_t acc_bytes) {
+    // 5 KB: barriers, alignment slack
+    const size_t ring_budget = (size_t)(227 - 5) * 1024 - p.stg_bytes - acc_bytes;
+    // several K-blocks per stage when they are small: fewer barrier round trips per K
+    const uint32_t ring_blk = p.a_bytes + (p.bstat ? 0u : p.b_bytes);
+    p.sps = (int)std::max<uint32_t>(1, std::min<uint32_t>(4, 32u * 1024u / std::max(ring_blk, 1u)));
+    p.sps = std::min(p.sps, p.kblocks);
+    const size_t fixed_smem = sizeof(float) * (size_t)p.nt * p.BN + (size_t)p.nt * p.BN / 8;
+    if (ring_budget < p.bstat_bytes + fixed_smem + 2 * (size_t)ring_blk) fatal_throw("tc plan: tile does not fit shared memory");
+    const size_t avail = ring_budget - p.bstat_bytes - fixed_smem;
+    while (p.sps > 1 && avail / ((size_t)p.sps * ring_blk) < 3) --p.sps;   // keep the ring at least 3 stages deep
+    p.stage_bytes = (uint32_t)p.sps * ring_blk;
+    p.stages = (int)std::min<size_t>(8, avail / p.stage_bytes);
+    if (p.stages < 2) fatal_throw("tc plan: tile does not fit shared memory");
+}
+
+// The tensor maps: activation boxes of a K-block, filter boxes and, for the TMA epilogue, the output and residual slabs
+void encode_maps(TcPlan &plan, const TcConv &c, bool reg) {
+    const TcParams &p = plan.p;
+    const TV &in = c.in;
+    const int esz = elem_size(c.kind), cin = operand_channels(c);
+    const CUtensorMapSwizzle swz = p.kk == 4 ? CU_TENSOR_MAP_SWIZZLE_128B : p.kk == 2 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
+    const CUtensorMapDataType dtype = c.kind == TC_TF32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                    : is_integer(c.kind) ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
     EncodeTiledFn enc = encode_fn();
-    const CUtensorMapDataType dtype = kind == 3 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
-                                    : i8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-    CUresult r;
-    if (!s2) {
+    auto check = [](CUresult r, const char *what) {
+        if (r != CUDA_SUCCESS) fatal_throw(std::string("cuTensorMapEncodeTiled(") + what + ") failed: " + std::to_string((int)r));
+    };
+    if (!p.stride2) {
         // activation view (c, x_padded, merged padded rows)
         cuuint64_t dims[3] = {(cuuint64_t)cin, (cuuint64_t)in.Wp, (cuuint64_t)in.N * in.Hp};
         cuuint64_t strides[2] = {(cuuint64_t)in.ldc * esz, (cuuint64_t)in.Wp * in.ldc * esz};
-        cuuint32_t box[3] = {(cuuint32_t)BK, (cuuint32_t)p.TW, (cuuint32_t)p.TH};
+        cuuint32_t box[3] = {(cuuint32_t)p.BK, (cuuint32_t)p.TW, (cuuint32_t)p.TH};
         cuuint32_t es[3] = {1, 1, 1};
-        r = enc(&plan->tmA, dtype, 3, in.base, dims, strides, box, es,
-                CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        check(enc(&plan.tmA, dtype, 3, in.base, dims, strides, box, es,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE), "A");
     } else {
         // stride 2: (c, x parity, x half, y parity, merged y half)
         cuuint64_t dims[5] = {(cuuint64_t)cin, 2, (cuuint64_t)in.Wp / 2, 2, (cuuint64_t)in.N * in.Hp / 2};
         cuuint64_t strides[4] = {(cuuint64_t)in.ldc * esz, (cuuint64_t)in.ldc * 2 * esz, (cuuint64_t)in.Wp * in.ldc * esz,
                                  (cuuint64_t)in.Wp * in.ldc * 2 * esz};
-        cuuint32_t box[5] = {(cuuint32_t)BK, 1, (cuuint32_t)p.TW, 1, (cuuint32_t)p.TH};
+        cuuint32_t box[5] = {(cuuint32_t)p.BK, 1, (cuuint32_t)p.TW, 1, (cuuint32_t)p.TH};
         cuuint32_t es[5] = {1, 1, 1, 1, 1};
-        r = enc(&plan->tmA, dtype, 5, in.base, dims, strides, box, es,
-                CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        check(enc(&plan.tmA, dtype, 5, in.base, dims, strides, box, es,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE), "A");
     }
-    if (r != CUDA_SUCCESS) { delete plan; fatal_throw("cuTensorMapEncodeTiled(A) failed: " + std::to_string((int)r)); }
     {
-        const cuuint64_t K = (cuuint64_t)l.size * l.size * cin;
-        cuuint64_t dims[2] = {K, (cuuint64_t)ldn};
+        const cuuint64_t K = (cuuint64_t)p.size * p.size * cin;
+        cuuint64_t dims[2] = {K, (cuuint64_t)c.ldn};
         cuuint64_t strides[1] = {K * esz};
-        cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)BN};
+        cuuint32_t box[2] = {(cuuint32_t)p.BK, (cuuint32_t)p.BN};
         cuuint32_t es[2] = {1, 1};
-        r = enc(&plan->tmB, dtype, 2, const_cast<void *>(d_weights_bf16), dims, strides, box, es,
-                CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { delete plan; fatal_throw("cuTensorMapEncodeTiled(B) failed: " + std::to_string((int)r)); }
+        check(enc(&plan.tmB, dtype, 2, const_cast<void *>(c.w), dims, strides, box, es,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE), "B");
     }
-    plan->tmO = plan->tmA; plan->tmO1 = plan->tmA; plan->tmR = plan->tmA;   // valid placeholders when unused
-    if (p.tma_epi && out.base) {   // a plan with a fused max-pool has no output to map
-        const int oesz = out_bf16 ? 2 : 4;
+    plan.tmO = plan.tmA; plan.tmO1 = plan.tmA; plan.tmR = plan.tmA;   // valid placeholders when unused
+    if (p.tma_epi && c.out.base) {   // a plan with a fused max-pool has no output to map
+        const int oesz = c.out_bf16 ? 2 : 4;
         auto encode_px = [&](CUtensorMap *tm, const TV &t, const char *what, int box_rows) {
             // (channels, padded x, merged padded rows) of a padded-NHWC tensor (bf16, or f32 for the integer kinds); box = one
             // slab of a pixel tile (k_conv_tc_reg: half a tile, the 64 pixels of one consumer warpgroup), box_rows rows of it
-            cuuint64_t dims[3] = {(cuuint64_t)l.n, (cuuint64_t)t.Wp, (cuuint64_t)t.N * t.Hp};
+            cuuint64_t dims[3] = {(cuuint64_t)p.n, (cuuint64_t)t.Wp, (cuuint64_t)t.N * t.Hp};
             cuuint64_t strides[2] = {(cuuint64_t)t.ldc * oesz, (cuuint64_t)t.Wp * t.ldc * oesz};
             cuuint32_t box[3] = {(cuuint32_t)p.tma_epi, (cuuint32_t)std::min(p.TW, reg ? 64 : 128), (cuuint32_t)box_rows};
             cuuint32_t es[3] = {1, 1, 1};
-            CUresult rr = enc(tm, out_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, t.base, dims, strides, box, es,
-                              CU_TENSOR_MAP_INTERLEAVE_NONE, p.tma_epi * oesz == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                              CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-            if (rr != CUDA_SUCCESS) { delete plan; fatal_throw(std::string("cuTensorMapEncodeTiled(") + what + ") failed: " + std::to_string((int)rr)); }
+            check(enc(tm, c.out_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, t.base, dims, strides, box, es,
+                      CU_TENSOR_MAP_INTERLEAVE_NONE, p.tma_epi * oesz == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                      CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE), what);
         };
         const int box_rows = reg ? std::max(p.TH / 2, 1) : p.TH;
-        encode_px(&plan->tmO, out, "output", box_rows);
-        if (reg && s2) encode_px(&plan->tmO1, out, "output row", 1);   // straddling half tiles, one tile row per store
-        if (res.base && out_bf16) encode_px(&plan->tmR, res, "residual", box_rows);
+        encode_px(&plan.tmO, c.out, "output", box_rows);
+        if (reg && p.stride2) encode_px(&plan.tmO1, c.out, "output row", 1);   // straddling half tiles, one tile row per store
+        if (c.res.base) encode_px(&plan.tmR, c.res, "residual", box_rows);
     }
-    plan->pdl = (getenv("YB_NO_PDL") == nullptr) ? 1 : 0;
+}
+
+}  // namespace
+
+int tc_conv_supported(const TcConv &c) {
+    const Layer &l = *c.l;
+    const bool integer = is_integer(c.kind);
+    // a view TMA can address: 16-byte aligned base and pixel rows
+    auto aligned = [](const TV &t, int esz) { return (reinterpret_cast<uintptr_t>(t.base) & 15) == 0 && t.ldc * esz % 16 == 0; };
+    if (!geometry_ok(l) || l.n < 8 || (l.activation != YB_LEAKY && l.activation != YB_LINEAR)) return 0;
+    if (channel_row(operand_channels(c), elem_size(c.kind)) == 0 || c.in.P != 1 || !aligned(c.in, elem_size(c.kind))) return 0;
+    // bf16 output: the bf16 kind only, whole 16-byte filter groups
+    if (c.out_bf16 && (c.kind != TC_BF16 || l.n % 8 != 0)) return 0;
+    if (c.out.base ? (c.out.P != 1 || !aligned(c.out, c.out_bf16 ? 2 : 4)) : !(c.yolo_out || c.pool_mode)) return 0;
+    // fused shortcut: k_conv_tc_reg at stride 1
+    if (c.res.base && !(c.kind == TC_BF16 && c.out_bf16 && l.stride == 1 && c.res.H == l.out_h && c.res.W == l.out_w &&
+                        c.res.C == l.n && aligned(c.res, 2)))
+        return 0;
+    // fused [yolo]: the f32 epilogue of k_conv_tc
+    if (c.yolo_out && (integer || c.out_bf16)) return 0;
+    // fused max-pool: the 8 x 16 tiles of the stride-1 3x3 integer layers start one merged row down, so 2x2 windows never
+    // straddle tiles when the padded height and the output size are even; the epilogue writes whole 32-filter groups of bytes
+    if (c.pool_mode && !(integer && (c.pool_mode == 1 || c.pool_mode == 2) && !c.acc_out && l.size == 3 && l.stride == 1 &&
+                         l.h % 2 == 0 && l.out_h % 2 == 0 && l.out_w % 2 == 0 && l.n % 32 == 0 &&
+                         c.pool_next.H == l.out_h / 2 && c.pool_next.W == l.out_w / 2 && aligned(c.pool_next, 1)))
+        return 0;
+    return 1;
+}
+
+void *tc_make_plan(const TcConv &c) {
+    const Layer &l = *c.l;
+    if (!tc_conv_supported(c)) fatal_throw("tc plan: convolution not supported by the tensor-core kernels");
+    std::unique_ptr<TcPlan> plan(new TcPlan());
+    TcParams &p = plan->p;
+    const bool reg = c.kind == TC_BF16 && c.out_bf16;   // bf16 NHWC output: the register-accumulator kernel with its TMA epilogue
+    const int sms = sm_count();
+    plan_tiles(p, c, reg, sms);
+    plan_epilogue(p, c, reg);
+    const size_t acc_bytes = reg ? 0 : (size_t)TC_BM * p.acc_pitch * 4;   // k_conv_tc_reg keeps the accumulators in registers
+    plan_ring(p, acc_bytes);
+    p.dbg = getenv("YB_TC_DBG") ? atoi(getenv("YB_TC_DBG")) : 0;
+    snprintf(plan->desc, sizeof(plan->desc), "%dx%dx%d -> n%d k%d s%d%s", l.c, l.h, l.w, l.n, l.size, l.stride, reg ? " reg" : "");
+    encode_maps(*plan, c, reg);
     plan->grid = std::min(p.num_work, grid_cap(sms));
     plan->threads = reg ? TCR_THREADS : TC_THREADS;
+    // barriers: full / empty per stage, the resident-filter barrier, k_conv_tc_reg's stg_full / stg_ready per consumer warpgroup
+    plan->smem = 1024 /*alignment slack*/ + p.bstat_bytes + (size_t)p.stages * p.stage_bytes + 8 * (2 * p.stages + 11) + 16 +
+                 sizeof(float) * (size_t)p.nt * p.BN /*bias*/ + (size_t)p.nt * p.BN / 8 /*yolo mask*/ +
+                 (p.tma_epi ? 1024 : 128) + p.stg_bytes /*epilogue staging or TMA-epilogue tiles*/ +
+                 acc_bytes /*accumulator tile*/;
+    if (plan->smem > 227 * 1024) fatal_throw("tc plan: shared memory budget exceeded");
+    for (const void *f : {(const void *)k_conv_tc<false, 0>, (const void *)k_conv_tc_reg<false>, (const void *)k_conv_tc<false, 2>,
+                          (const void *)k_conv_tc<true, 0>, (const void *)k_conv_tc_reg<true>, (const void *)k_conv_tc<true, 2>})
+        if (cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
+            fatal_throw("cudaFuncSetAttribute(k_conv_tc) failed");
     if (getenv("YB_TC_STATS")) {
         cudaMalloc(&p.stats, sizeof(unsigned long long) * 16 * plan->grid);
         cudaMemset(p.stats, 0, sizeof(unsigned long long) * 16 * plan->grid);
     }
-    // barriers: full / empty per stage, the resident-filter barrier, k_conv_tc_reg's stg_full / stg_ready per consumer warpgroup
-    plan->smem = 1024 /*alignment slack*/ + p.bstat_bytes + (size_t)p.stages * p.stage_bytes + 8 * (2 * p.stages + 11) + 16 +
-                 sizeof(float) * (size_t)p.nt * BN /*bias*/ + (size_t)p.nt * BN / 8 /*yolo mask*/ +
-                 (p.tma_epi ? 1024 : 128) + p.stg_bytes /*epilogue staging or TMA-epilogue tiles*/ +
-                 acc_bytes /*accumulator tile*/;
-    if (plan->smem > 227 * 1024) { delete plan; fatal_throw("tc plan: shared memory budget exceeded"); }
-    {
-        const void *fns[] = {(const void *)k_conv_tc<false, 0>, (const void *)k_conv_tc_reg<false>, (const void *)k_conv_tc<false, 2>,
-                             (const void *)k_conv_tc<true, 0>, (const void *)k_conv_tc_reg<true>, (const void *)k_conv_tc<true, 2>};
-        for (const void *f : fns)
-            if (cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
-                fatal_throw("cudaFuncSetAttribute(k_conv_tc) failed");
-    }
-    return plan;
-}
-
-void *tc_make_plan(const Layer &l, const TV &in, const TV &out, bool out_bf16, const TV &res, bool res_bf16,
-                   int act2, const void *d_weights_bf16, int ldn, const float *d_bias, int wide_rows) {
-    return make_plan_common(0, l, in, out, out_bf16, res, res_bf16, act2, d_weights_bf16, ldn, d_bias, 0.f, nullptr, wide_rows);
-}
-
-// FP32 convolution of the exact (INT8 / XNOR) networks on the tf32 wgmma: f32 NHWC activations and f32 [ldn][K] weights go
-// through TMA untouched, the tensor core uses the upper 19 bits of each word (10-bit mantissa, ~3e-4 relative on the
-// sums).  Used for detection heads only (their error cannot reach an integer layer), f32 output.
-int tc_tf32_supported(const Layer &l, const TV &in, const TV &out) {
-    if (pick_bk_f32(l.c) == 0) return 0;
-    if ((reinterpret_cast<uintptr_t>(in.base) & 15) != 0 || in.P != 1 || in.ldc % 4 != 0) return 0;
-    const bool s1 = l.stride == 1 && ((l.size == 3 && l.pad == 1) || (l.size == 1 && l.pad == 0));
-    const bool s2 = l.stride == 2 && l.size == 3 && l.pad == 1 && (l.h % 2 == 0) && (l.w % 2 == 0);
-    if (!s1 && !s2) return 0;
-    if (!out.base || (reinterpret_cast<uintptr_t>(out.base) & 15) != 0 || out.ldc % 4 != 0 || l.n < 8) return 0;
-    if (l.activation != YB_LEAKY && l.activation != YB_LINEAR) return 0;
-    return 1;
-}
-void *tc_make_plan_tf32(const Layer &l, const TV &in, const TV &out, const void *d_weights_f32, int ldn, const float *d_bias,
-                        int wide_rows) {
-    TV none{};
-    return make_plan_common(3, l, in, out, false, none, false, ACT_LINEAR, d_weights_f32, ldn, d_bias, 0.f, nullptr, wide_rows);
-}
-
-// INT8 variant (reference forward_convolutional_layer_q, yolov2_forward_network_quantized.c:527-631) on
-// the s8 wgmma: `q` is the quantised s8 activation (padded NHWC, channels zero-padded to q.ldc), weights are
-// s8 [ldn][taps][q.ldc]; output f32.
-int tc_i8_supported(const Layer &l, const TV &q, const TV &out) {
-    if (pick_bk_i8(q.ldc) == 0) return 0;
-    if ((reinterpret_cast<uintptr_t>(q.base) & 15) != 0 || q.P != 1 || q.ldc % 16 != 0) return 0;
-    const bool s1 = l.stride == 1 && ((l.size == 3 && l.pad == 1) || (l.size == 1 && l.pad == 0));
-    const bool s2 = l.stride == 2 && l.size == 3 && l.pad == 1 && (l.h % 2 == 0) && (l.w % 2 == 0);
-    if (!s1 && !s2) return 0;
-    if (!out.base || (reinterpret_cast<uintptr_t>(out.base) & 15) != 0 || out.ldc % 4 != 0 || l.n < 8) return 0;
-    if (l.activation != YB_LEAKY && l.activation != YB_LINEAR) return 0;
-    return 1;
-}
-void tc_plan_fuse_yolo(void *vp, float *d_yolo_nchw, int classes) {
-    TcPlan *plan = reinterpret_cast<TcPlan *>(vp);
-    plan->p.yolo_out = d_yolo_nchw;
-    plan->p.yolo_per = 4 + classes + 1;
-}
-
-// Whether an integer-kind plan of `l` made with want_pool_tile can take the following 2x2 / stride-2 max-pool (tc_plan_fuse_pool):
-// its 8 x 16 tiles (stride-1 3x3 layers only) start one merged row down, so 2x2 windows never straddle tiles when the padded
-// height and the output size are even.
-int tc_pool_fuse_supported(const Layer &l, const TV &qnext) {
-    return l.size == 3 && l.stride == 1 && l.h % 2 == 0 && l.out_h % 2 == 0 && l.out_w % 2 == 0 && l.n % 32 == 0 &&
-           qnext.H == l.out_h / 2 && qnext.W == l.out_w / 2 && qnext.ldc % 16 == 0 && (reinterpret_cast<uintptr_t>(qnext.base) & 15) == 0;
-}
-
-// Fuse the following 2x2 / stride-2 max-pool and the next integer layer's input conversion into an integer-kind plan with 8 x 16 tiles:
-// mode 1 = s8 quantised with `mult` (INT8 layer next), 2 = +-1 bytes (XNOR layer on the tensor cores next).  `qnext` is that layer's
-// s8 input (padded NHWC).  The caller has checked tc_pool_fuse_supported.
-void tc_plan_fuse_pool(void *vp, int mode, float mult, const TV &qnext) {
-    TcPlan *plan = reinterpret_cast<TcPlan *>(vp);
-    TcParams &p = plan->p;
-    if (!(p.kind == 1 || p.kind == 2) || p.TW != 8 || p.jshift != 1 || (p.PR & 1) || (p.OW & 1) || (p.OH & 1) || p.acc_out ||
-        qnext.H != p.OH / 2 || qnext.W != p.OW / 2 || qnext.ldc % 16 != 0 || (reinterpret_cast<uintptr_t>(qnext.base) & 15) || p.n % 32 != 0)
-        fatal_throw("tc plan: the max-pool does not fit the plan's tiling");
-    p.pool_mode = mode; p.pool_mult = mult;
-    p.pool_out = reinterpret_cast<signed char *>(qnext.base); p.pool_ldc = qnext.ldc; p.pool_Hp = qnext.Hp; p.pool_Wp = qnext.Wp;
-}
-
-void *tc_make_plan_i8(const Layer &l, const TV &q, const TV &out, const void *d_weights_s8, int ldn, const float *d_bias,
-                      float alpha1, int *acc_out, int want_pool_tile) {
-    TV none{};
-    return make_plan_common(1, l, q, out, false, none, false, ACT_LINEAR, d_weights_s8, ldn, d_bias, alpha1, acc_out, 0, want_pool_tile);
-}
-
-// XNOR layer mapped onto the s8 wgmma: activations and weights as +-1 bytes, so the s32 accumulator is 2*count - K.
-void *tc_make_plan_xnor(const Layer &l, const TV &q, const TV &out, const void *d_weights_pm1, int ldn, const float *d_bias,
-                        const float *d_mean, int *counts_out, int want_pool_tile) {
-    TV none{};
-    TcPlan *plan = reinterpret_cast<TcPlan *>(
-        make_plan_common(2, l, q, out, false, none, false, ACT_LINEAR, d_weights_pm1, ldn, d_bias, 0.f, counts_out, 0, want_pool_tile));
-    plan->p.mean = d_mean;
-    plan->p.xK = l.size * l.size * l.c;
-    return plan;
+    return plan.release();
 }
 
 struct StemPlan { StemTcP p; int grid; bool s2; };   // s2: k_stem_s2_tc (stem + layer 1)
@@ -1810,10 +1761,7 @@ void *tc_stem_make_plan(const Layer &l, const TV &out, const void *d_w, const fl
     p.npix = (long)out.N * l.h * l.w;
     if (p.npix >= (1L << 31) - 256) fatal_throw("stem plan: more than 2^31 pixels per batch");
     p.ntiles = (int)((p.npix + 127) / 128);
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    sp->grid = std::min(p.ntiles, sms * 8);
+    sp->grid = std::min(p.ntiles, sm_count() * 8);
     return sp;
 }
 int tc_stem_s2_supported(const Layer &l0, const Layer &l1, const TV &out1) {
@@ -1836,10 +1784,7 @@ void *tc_stem_s2_make_plan(const Layer &l0, const Layer &l1, const TV &out1, con
     const long ntiles = (long)p.N * p.xt * p.yt;
     if (ntiles >= INT_MAX) fatal_throw("stem plan: too many tiles");
     p.ntiles = (int)ntiles;
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    sp->grid = std::min(p.ntiles, grid_cap(2 * sms));
+    sp->grid = std::min(p.ntiles, grid_cap(2 * sm_count()));
     for (const void *f : {(const void *)k_stem_s2_tc<false>, (const void *)k_stem_s2_tc<true>}) {
         if (cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S2_SMEM) != cudaSuccess ||
             cudaFuncSetAttribute(f, cudaFuncAttributePreferredSharedMemoryCarveout, 100) != cudaSuccess)
@@ -1869,17 +1814,13 @@ void tc_launch(void *vp, cudaStream_t s) {
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3((unsigned)plan->grid); cfg.blockDim = dim3((unsigned)plan->threads);
     cfg.dynamicSmemBytes = plan->smem; cfg.stream = s;
-    cudaLaunchAttribute attr[2];
-    int na = 0;
-    if (plan->pdl) {   // let this kernel's prologue start while the previous kernel drains
-        attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[na].val.programmaticStreamSerializationAllowed = 1;
-        ++na;
-    }
-    cfg.attrs = attr; cfg.numAttrs = na;
+    cudaLaunchAttribute attr[1];   // programmatic dependent launch: this kernel's prologue runs while the previous kernel drains
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr; cfg.numAttrs = 1;
     const bool st = plan->p.stats != nullptr;   // role counters: a separate instantiation (YB_TC_STATS=1)
     const TcPlan &P = *plan;
-#define YB_TC_LAUNCH(KERNEL) cudaLaunchKernelEx(&cfg, KERNEL, P.tmA, P.tmB, P.tmO, P.tmR, P.p)
+#define YB_TC_LAUNCH(KERNEL) cudaLaunchKernelEx(&cfg, KERNEL, P.tmA, P.tmB, P.tmO, P.p)
     if (plan->threads == TCR_THREADS) {
         if (st) cudaLaunchKernelEx(&cfg, k_conv_tc_reg<true>, P.tmA, P.tmB, P.tmO, P.tmO1, P.tmR, P.p);
         else cudaLaunchKernelEx(&cfg, k_conv_tc_reg<false>, P.tmA, P.tmB, P.tmO, P.tmO1, P.tmR, P.p);
@@ -1902,7 +1843,7 @@ void tc_free_plan(void *vp) {
         if (plan->threads == TCR_THREADS)   // k_conv_tc_reg: the consumers' wait on stg_ready (first work item apart) and the store warps
             fprintf(stderr, "consumers: wait_full %.0f wait_ready %.0f (first item %.0f) total %.0f | store: wait_full %.0f wait_read %.0f\n",
                     m[2], m[8], m[3], m[6], m[4], m[5]);
-        else fprintf(stderr, "consumers: wait_full %.0f wait_res %.0f total %.0f\n", m[2], m[8], m[6]);
+        else fprintf(stderr, "consumers: wait_full %.0f total %.0f\n", m[2], m[6]);
         cudaFree(plan->p.stats);
     }
     delete plan;

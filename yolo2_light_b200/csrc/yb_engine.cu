@@ -227,7 +227,6 @@ struct LayerPlan {
     int fused_into = -1;        // conv + shortcut: this convolution writes the shortcut's output
     bool fused_sc = false;      // shortcut computed in the epilogue of the convolution in front of it
     bool yolo_fused = false;    // conv: writes the [yolo] layer behind it from its epilogue; [yolo]: written that way
-    bool pool_tile = false;     // integer tensor-core conv: 8 x 16 pixel tiles, as a fused 2x2 max-pool needs
     int pool_mode = 0;          // conv: runs the max-pool behind it and layer i+2's input conversion (1 s8, 2 +-1 bytes, 3 sign bits)
     bool pool_in_conv = false;  // max-pool: runs in the epilogue of the convolution in front of it
     bool pool_to_side = false;  // max-pool: writes the next convolution's converted input instead of its own output
@@ -344,6 +343,47 @@ struct Builder {
         return make_tv(base, B, l.h, l.w, ld, ld, P, DT_BITS, 0);
     }
     TV side_placed(int i) const { return side_view(i, e.act_arena + side_off[i]); }
+    static float alpha1(const Layer &l) { return 32 / (l.input_quant_multipler * l.weights_quant_multipler); }   // ALPHA1, ..._quantized.c:598
+
+    // Convolution i as a tensor-core convolution (the kind follows the variant and the activation type), with the shortcut and
+    // [yolo] fusions of its plan and the max-pool fusion `pool_mode`.  placed == false: views rooted at kLayoutBase and no
+    // device pointers, for the queries of the layer plan; true: the placed buffers, the packed weights and the raw-count
+    // buffer (keep_counts) that counts_buffer made.
+    TcConv tc_conv(int i, bool placed, int pool_mode) const {
+        const Layer &l = layer(i);
+        const LayerPlan &p = L[i];
+        const int tgt = p.fused_into >= 0 ? p.fused_into : i;
+        auto out = [&](int j) { return placed ? e.out_tv[j] : layout_view(j); };
+        auto side = [&](int j) { return placed ? side_placed(j) : side_view(j, kLayoutBase); };
+        TcConv c;
+        c.kind = p.variant == 2 ? TC_S8 : p.variant == 1 ? TC_XNOR : ADT == DT_BF16 ? TC_BF16 : TC_TF32;
+        c.l = &l;
+        c.in = p.variant != 0 ? side(i) : !placed ? layout_in(i) : i == 0 ? e.in0 : e.out_tv[i - 1];
+        c.out = out(tgt);
+        c.out_bf16 = L[tgt].out_dt == DT_BF16;
+        if (p.fused_into >= 0) {
+            c.res = out(layer(tgt).index);
+            c.act2 = layer(tgt).activation;
+        }
+        c.pool_mode = pool_mode;
+        if (pool_mode) {
+            c.pool_mult = pool_mode == 1 ? layer(i + 2).input_quant_multipler : 0.f;
+            c.pool_next = side(i + 2);
+        }
+        if (!placed) return c;
+        // filters: [ldn][K] bf16, f32 (K-major copy) or s8 / +-1 bytes ([taps][cpad] per filter)
+        c.w = e.w_arena + (c.kind == TC_BF16 ? cw[i].w_bf16 : c.kind == TC_TF32 ? cw[i].w_f32km : cw[i].w_s8);
+        c.ldn = cw[i].ldn;
+        c.bias = bias(i);
+        if (c.kind == TC_S8) c.alpha1 = alpha1(l);
+        if (c.kind == TC_XNOR) c.mean = reinterpret_cast<const float *>(e.w_arena + cw[i].mean);
+        c.acc_out = e.d_counts[i];
+        if (p.yolo_fused) {
+            c.yolo_out = e.d_final[i + 1];
+            c.yolo_classes = layer(i + 1).classes;
+        }
+        return c;
+    }
 
     // ---- pass 1: the layer plan ------------------------------------------------------------------------------------------
     void plan_layers() {
@@ -437,25 +477,26 @@ struct Builder {
         const int tgt = p.fused_into >= 0 ? p.fused_into : i;
         const TV tin = layout_in(i), tout = layout_view(tgt);
         const int idt = in_dt(i), odt = L[tgt].out_dt;
+        const TcConv tc_query = tc_conv(i, false, 0);
         if (p.variant == 0) {
-            int tc = (ADT == DT_BF16 && idt == DT_BF16) ? tc_conv_supported(l, tin, tout, odt == DT_BF16) : 0;
+            int tc = (ADT == DT_BF16 && idt == DT_BF16) ? tc_conv_supported(tc_query) : 0;
             // float detection heads of the INT8 / XNOR networks (default precision): tf32 wgmma.  Only layers whose every
             // reader is a yolo / region layer -- nothing they compute can reach an integer layer.
             if (ADT == DT_F32 && opt.precision == YB_PREC_BF16_TC && idt == DT_F32 && odt == DT_F32 && p.fused_into < 0 &&
                 !cons[i].empty() && !sw.no_tf32) {
                 bool heads_only = true;
                 for (int r : cons[i]) heads_only &= layer(r).type == YB_YOLO || layer(r).type == YB_REGION;
-                if (heads_only && tc_tf32_supported(l, tin, tout)) tc = 2;
+                if (heads_only && tc_conv_supported(tc_query)) tc = 2;
             }
             if (sw.no_tc) tc = 0;
             return tc == 2 ? CP_TF32 : tc ? CP_TC : CP_SIMT;
         }
         if (idt != DT_F32 || odt != DT_F32)
             fatal_throw(p.variant == 1 ? "engine: xnor path needs f32 activations" : "engine: int8 path needs f32 activations");
-        if (p.variant == 2) return (!sw.no_tc && tc_i8_supported(l, side_view(i, kLayoutBase), tout)) ? CP_I8_TC : CP_I8_SIMT;
+        if (p.variant == 2) return (!sw.no_tc && tc_conv_supported(tc_query)) ? CP_I8_TC : CP_I8_SIMT;
         if (xnor_fallback(l)) return CP_XNOR_FALLBACK;
         if (xnor_on_tc(l) && vec4_view(tin)) {
-            if (!tc_i8_supported(l, side_view(i, kLayoutBase), tout)) fatal_throw("engine: xnor tensor-core layer not supported by the i8 tile");
+            if (!tc_conv_supported(tc_query)) fatal_throw("engine: xnor tensor-core layer not supported by the i8 tile");
             return CP_XNOR_TC;
         }
         // small K: one thread per pixel, all filters (weights broadcast from shared memory)
@@ -515,8 +556,7 @@ struct Builder {
             const int pm = conv_pool_mode(i);
             bool pool = false;
             if (p.path == CP_XNOR_TC || p.path == CP_I8_TC) {
-                p.pool_tile = pm != 0;
-                pool = pm != 0 && tc_pool_fuse_supported(layer(i), side_view(i + 2, kLayoutBase));
+                pool = pm != 0 && tc_conv_supported(tc_conv(i, false, pm));
             } else if (p.path == CP_XNOR_SMALLK) {
                 pool = pm == 2 || pm == 3;
             }
@@ -672,12 +712,11 @@ struct Builder {
     const float *bias(int i) const { return reinterpret_cast<const float *>(e.w_arena + cw[i].bias); }
     void push(int kind, int i, std::function<void(cudaStream_t)> f) { e.ops.push_back(Op{kind, i, std::move(f)}); }
 
-    // a tensor-core plan of layer i, with the [yolo] layer or the max-pool the plan decided to fuse
-    void push_tc_plan(int kind, int i, void *plan) {
+    // the tensor-core plan of layer i, with the [yolo] layer or the max-pool the layer plan fuses
+    void push_tc_plan(int kind, int i) {
+        void *plan = tc_make_plan(tc_conv(i, true, L[i].pool_mode));
         e.tc_plans.push_back(plan);
         if (kind == OP_CONV_TC || kind == OP_CONV_TC_TF32) ++e.n_tc;
-        if (L[i].yolo_fused) tc_plan_fuse_yolo(plan, e.d_final[i + 1], layer(i + 1).classes);
-        if (const int pm = L[i].pool_mode) tc_plan_fuse_pool(plan, pm, pm == 1 ? layer(i + 2).input_quant_multipler : 0.f, side_placed(i + 2));
         push(kind, i, [plan](cudaStream_t s) { tc_launch(plan, s); });
     }
 
@@ -780,13 +819,8 @@ struct Builder {
             act2 = s.activation;
             if (!res.base) fatal_throw("engine: shortcut source not placed");
         }
-        if (p.path == CP_TF32) {
-            push_tc_plan(OP_CONV_TC_TF32, i, tc_make_plan_tf32(l, tin, tout, e.w_arena + cw[i].w_f32km, cw[i].ldn, bias(i), p.yolo_fused));
-            return;
-        }
-        if (p.path == CP_TC) {
-            push_tc_plan(OP_CONV_TC, i, tc_make_plan(l, tin, tout, odt == DT_BF16, res, rdt == DT_BF16, act2, e.w_arena + cw[i].w_bf16,
-                                                     cw[i].ldn, bias(i), p.yolo_fused));
+        if (p.path == CP_TC || p.path == CP_TF32) {
+            push_tc_plan(p.path == CP_TC ? OP_CONV_TC : OP_CONV_TC_TF32, i);
             return;
         }
         const long M = (long)B * l.out_h * l.out_w;
@@ -836,8 +870,7 @@ struct Builder {
             const TV q = side_placed(i);
             const int g = grid_for((long)B * l.h * l.w * (l.c / 16));
             if (!p.prefilled) push(OP_BINARIZE, i, [tin, q, g](cudaStream_t s) { k_binarize_s8<<<g, 256, 0, s>>>(tin, q); });
-            push_tc_plan(OP_CONV_TC_I8, i, tc_make_plan_xnor(l, q, tout, e.w_arena + cw[i].w_s8, cw[i].ldn, bias(i),
-                                                             reinterpret_cast<const float *>(e.w_arena + cw[i].mean), cnt_dbg, p.pool_tile));
+            push_tc_plan(OP_CONV_TC_I8, i);
             return;
         }
         const int CW = p.side_ld;
@@ -896,10 +929,8 @@ struct Builder {
         const int g = grid_for((long)B * l.h * l.w * (p.side_ld / 4));
         if (!p.prefilled) push(OP_QUANTIZE, i, [tin, q, mult, g](cudaStream_t s) { k_quantize<float><<<g, 256, 0, s>>>(tin, q, mult); });
         int *acc_dbg = counts_buffer(i);
-        const float alpha1 = 32 / (l.input_quant_multipler * l.weights_quant_multipler);   // ALPHA1, ..._quantized.c:598
         if (p.path == CP_I8_TC) {
-            // s8 x s8 -> s32 on the s8 wgmma; weights [ldn][taps][cpad] are already K-major
-            push_tc_plan(OP_CONV_TC_I8, i, tc_make_plan_i8(l, q, tout, e.w_arena + cw[i].w_s8, cw[i].ldn, bias(i), alpha1, acc_dbg, p.pool_tile));
+            push_tc_plan(OP_CONV_TC_I8, i);
             return;
         }
         const long M = (long)B * l.out_h * l.out_w;
@@ -907,7 +938,7 @@ struct Builder {
         ip.q = q; ip.out = tout;
         ip.w = reinterpret_cast<const uint32_t *>(e.w_arena + cw[i].w_s8);
         ip.bias = bias(i);
-        ip.alpha1 = alpha1;
+        ip.alpha1 = alpha1(l);
         ip.n = l.n; ip.size = l.size; ip.stride = l.stride; ip.pad = l.pad; ip.act = l.activation;
         ip.CW = p.side_ld / 4; ip.M = M; ip.acc_out = acc_dbg;
         dim3 grid((unsigned)((M + 63) / 64), (unsigned)((l.n + 63) / 64));
