@@ -152,7 +152,7 @@ float *yb_network_predict_image_u8(yb_network *net, const unsigned char *images_
 float *yb_network_predict_frames_u8(yb_network *net, const unsigned char *const *frames, const int *w, const int *h,
                                     int nimg, int quantized);
 /* Diagnostic: the planar float input (batch*c*h*w) the device pipeline produced for the last predict_image_u8 /
- * predict_frames_u8 call. */
+ * predict_frames_u8 / predict_device_frames call. */
 int    yb_network_fetch_input(yb_network *net, int quantized, float *dst);
 
 /* Pipelined form of the two calls above for throughput serving: yb_network_submit enqueues one batch (H2D of
@@ -186,6 +186,54 @@ int yb_network_collect_detections(yb_network *net, int ticket, int quantized, co
  * checks, and max_rows in 1..16384. */
 int yb_network_submit_frames_u8(yb_network *net, const unsigned char *const *frames, const int *w, const int *h, int nimg,
                                 int quantized, float thresh, float nms, int relative, int letter, int max_rows);
+
+/* Frames already in device memory: what a hardware video decoder (NV12) or a GPU JPEG decoder (planar RGB) produces, or
+ * pitched RGB / BGR surfaces.  No host copy is made: the resize kernel reads each frame where it lies.  Frame b gives
+ * bit-for-bit what the host calls above give for its equivalent host frame (resized input, detection tensors, rows and
+ * counts), with boxes corrected for frame b's own w x h and `letter` as there:
+ *   YB_FRAME_RGB         the same bytes without the row padding;
+ *   YB_FRAME_BGR         each pixel's bytes reversed (the demo path's ipl_to_image + rgbgr_image, additionally.c:2915,3112);
+ *   YB_FRAME_RGB_PLANAR  the HWC transpose of the three planes;
+ *   YB_FRAME_NV12        the RGB frame of BT.601 limited-range fixed-point conversion (OpenCV's cvtColor
+ *                        COLOR_YUV2RGB_NV12): with Y, U, V the bytes of pixel (x, y), U and V at bytes 2 * (x / 2) and
+ *                        2 * (x / 2) + 1 of chroma row y / 2, yy = max(0, Y - 16) * 1220542, u = U - 128, v = V - 128,
+ *                        half = 1 << 19:  R = clamp((yy + half + 1673527 v) >> 20),
+ *                        G = clamp((yy + half - 852492 v - 409993 u) >> 20), B = clamp((yy + half + 2116026 u) >> 20),
+ *                        clamped to 0..255.
+ * Device frames are always resized by the kernel, also at the network size.  One format per call, 3-channel networks only. */
+enum { YB_FRAME_RGB = 0, YB_FRAME_BGR = 1, YB_FRAME_RGB_PLANAR = 2, YB_FRAME_NV12 = 3 };
+
+typedef struct yb_device_frame {
+    const unsigned char *data;    /* RGB/BGR: first pixel, 3 bytes per pixel (HWC); RGB_PLANAR: the R plane; NV12: the Y plane */
+    const unsigned char *chroma;  /* NV12: the interleaved U,V plane (h/2 rows, same pitch as Y); NULL for the other formats  */
+    int w, h;
+    int pitch;                    /* bytes from one row to the next: >= 3w (RGB/BGR), >= w (RGB_PLANAR, NV12)               */
+    long long plane_stride;       /* RGB_PLANAR: bytes from the R plane to G and from G to B (>= pitch * h); ignored otherwise  */
+} yb_device_frame;
+
+/* nimg (1..net.batch) device frames of one format -> resize, forward; fills the host yolo/region outputs like
+ * yb_network_predict_frames_u8 (synchronous).  Batch items nimg .. batch-1 are zero images.  yb_network_fetch_input returns
+ * the resized input it made. */
+float *yb_network_predict_device_frames(yb_network *net, const yb_device_frame *frames, int nimg, int format,
+                                        int quantized, void *stream);
+/* Pipelined form, like yb_network_submit_frames_u8: same 3 slots and ticket rules, collected with
+ * yb_network_collect_detections (counts[b] = 0 for b >= nimg).
+ *
+ * Ordering with the caller's stream (both calls): `stream` is the cudaStream_t on which the caller produced the frames
+ * (NULL = the legacy default stream).  The call records an event on `stream` and makes the engine's input stream wait on
+ * it, so the frames are read only after the work the caller enqueued before the call.  After the last kernel that reads
+ * the frames it records an event on the engine's input stream and makes `stream` wait on that, so work the caller enqueues
+ * on `stream` after the call -- such as the decoder's next write into the same surfaces -- runs only once the engine is done
+ * reading.  Neither call waits for the device before it returns (the predict call then waits for its own results).  Frames
+ * written from another stream must be ordered before `stream` by the caller.
+ *
+ * Rejected before any device work: nimg outside 1..net.batch, a null frames array, a null data (or, for NV12, chroma)
+ * pointer, w < 1 or h < 1, an odd w or h for NV12, a pitch or plane_stride below its minimum, an unknown format, a
+ * network whose input does not have 3 channels, a frame whose addressed span exceeds INT_MAX bytes, max_rows outside
+ * 1..16384.  Then a frame that is not device or managed memory of the network's device (host, pinned host, or another
+ * GPU's memory; cudaPointerGetAttributes) is rejected. */
+int yb_network_submit_device_frames(yb_network *net, const yb_device_frame *frames, int nimg, int format, int quantized,
+                                    float thresh, float nms, int relative, int letter, int max_rows, void *stream);
 
 /* Host output (NCHW for yolo, HWC-flattened for region, as the reference lays them out) of layer i after a
  * predict call; only YOLO/REGION layers (and the last layer) are kept on the host. */

@@ -55,6 +55,15 @@ class LayerDesc(C.Structure):
     ]
 
 
+class DeviceFrame(C.Structure):
+    """``yb_device_frame`` (include/yolo2_light_b200.h)."""
+    _fields_ = [("data", C.c_void_p), ("chroma", C.c_void_p), ("w", C.c_int), ("h", C.c_int), ("pitch", C.c_int),
+                ("plane_stride", C.c_longlong)]
+
+
+# ``YB_FRAME_*``: the layouts of device frames
+FRAME_FORMATS = {"rgb": 0, "bgr": 1, "planar": 2, "nv12": 3}
+
 _lib = None
 
 
@@ -99,6 +108,9 @@ def lib():
         "yb_network_detect_frames": (C.c_int, [vp, C.c_int, vp, vp, C.c_int, C.c_float, C.c_float, C.c_int, C.c_int, vp, C.c_int, vp]),
         "yb_network_submit_frames_u8": (C.c_int, [vp, vp, vp, vp, C.c_int, C.c_int, C.c_float, C.c_float, C.c_int, C.c_int, C.c_int]),
         "yb_network_collect_detections": (C.c_int, [vp, C.c_int, C.c_int, C.POINTER(fp), C.POINTER(ip), C.POINTER(C.c_size_t)]),
+        "yb_network_predict_device_frames": (fp, [vp, vp, C.c_int, C.c_int, C.c_int, vp]),
+        "yb_network_submit_device_frames": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_int,
+                                                      C.c_int, C.c_int, vp]),
         "yb_network_set_devices": (C.c_int, [vp, ip, C.c_int]),
         "yb_network_predict_batch": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int]),
         "yb_network_batch_output": (fp, [vp, C.c_int, ip]),
@@ -147,7 +159,8 @@ EXPORTED_SYMBOLS = [
     "yb_network_last_launches", "yb_network_profile", "yb_op_kind_name", "yb_get_network_boxes", "yb_alloc_pinned",
     "yb_free_pinned", "yb_network_submit_u8", "yb_network_collect_detections", "yb_network_set_devices",
     "yb_network_predict_batch", "yb_network_batch_output", "yb_network_replication", "yb_network_predict_frames_u8",
-    "yb_network_detect_frames", "yb_network_submit_frames_u8",
+    "yb_network_detect_frames", "yb_network_submit_frames_u8", "yb_network_predict_device_frames",
+    "yb_network_submit_device_frames",
 ]
 
 
@@ -336,9 +349,98 @@ class Network:
         self._inflight[("u8", t)] = (keep, max_rows, len(keep))
         return t
 
+    def _device_frames(self, frames, fmt: str, fn: str):
+        """1..batch device frames of format `fmt` -> (keep-alive list, yb_device_frame array, YB_FRAME_* value).
+
+        Each frame is an object with a ``__cuda_array_interface__`` of typestr ``|u1`` (a torch CUDA tensor, a CuPy array,
+        ...): rgb / bgr ``(h, w, 3)`` with strides ``(pitch, 3, 1)``; planar ``(3, h, w)`` with strides
+        ``(plane, pitch, 1)``; nv12 one ``(3h/2, w)`` array with strides ``(pitch, 1)`` (the chroma plane starts at row h),
+        or a ``(Y (h, w), UV (h/2, w))`` pair with the same pitch."""
+        if fmt not in FRAME_FORMATS:
+            raise YbError(f"{fn}: unknown format {fmt!r}, expected one of {', '.join(FRAME_FORMATS)}")
+        frames = list(frames)
+        if not 1 <= len(frames) <= self.batch:
+            raise YbError(f"{fn}: {len(frames)} frames, the network takes 1..{self.batch}")
+
+        def view(obj, k, what, ndim, inner):
+            """(pointer, shape, strides) of a uint8 array of rank ndim whose trailing strides are `inner`."""
+            cai = getattr(obj, "__cuda_array_interface__", None)
+            if not isinstance(cai, dict):
+                raise YbError(f"{fn}: frame {k} must expose __cuda_array_interface__ (a device array), got "
+                              f"{type(obj).__name__}")
+            shape = tuple(int(s) for s in cai.get("shape", ()))
+            if cai.get("typestr") != "|u1" or len(shape) != ndim:
+                raise YbError(f"{fn}: frame {k} must be a uint8 {what} array, got typestr {cai.get('typestr')!r} "
+                              f"shape {shape}")
+            strides = cai.get("strides")
+            if strides is None:   # C-contiguous
+                strides, acc = [], 1
+                for s in reversed(shape):
+                    strides.insert(0, acc)
+                    acc *= s
+            strides = tuple(int(s) for s in strides)
+            if strides[ndim - len(inner):] != inner or not 0 < strides[0] < 2 ** 31 or (ndim == 3 and not 0 < strides[1] < 2 ** 31):
+                raise YbError(f"{fn}: frame {k} must be a uint8 {what} array, got shape {shape} strides {strides}")
+            return int(cai["data"][0]), shape, strides
+
+        F = FRAME_FORMATS[fmt]
+        arr = (DeviceFrame * len(frames))()
+        for k, f in enumerate(frames):
+            d = arr[k]
+            if fmt in ("rgb", "bgr"):
+                p, (h, w, c), (pitch, _, _) = view(f, k, "[h, w, 3] (strides (pitch, 3, 1))", 3, (3, 1))
+                if c != 3:
+                    raise YbError(f"{fn}: frame {k} must be a uint8 [h, w, 3] (strides (pitch, 3, 1)) array, got shape {(h, w, c)}")
+                d.data, d.w, d.h, d.pitch = p, w, h, pitch
+            elif fmt == "planar":
+                p, (c, h, w), (plane, pitch, _) = view(f, k, "[3, h, w] (strides (plane, pitch, 1))", 3, (1,))
+                if c != 3:
+                    raise YbError(f"{fn}: frame {k} must be a uint8 [3, h, w] (strides (plane, pitch, 1)) array, got shape "
+                                  f"{(c, h, w)}")
+                d.data, d.w, d.h, d.pitch, d.plane_stride = p, w, h, pitch, plane
+            elif isinstance(f, (tuple, list)):
+                if len(f) != 2:
+                    raise YbError(f"{fn}: frame {k}: an nv12 pair is (Y [h, w], UV [h/2, w]), got {len(f)} arrays")
+                py, (h, w), (pitch, _) = view(f[0], k, "Y [h, w] (strides (pitch, 1))", 2, (1,))
+                pc, (hc, wc), (pitch_c, _) = view(f[1], k, "UV [h/2, w] (strides (pitch, 1))", 2, (1,))
+                if 2 * hc != h or wc != w or (hc > 1 and pitch_c != pitch):   # one UV row: its pitch is never used
+                    raise YbError(f"{fn}: frame {k}: UV plane {(hc, wc)} with pitch {pitch_c} does not match Y plane {(h, w)} "
+                                  f"with pitch {pitch} (UV must be [h/2, w] with the same pitch)")
+                d.data, d.chroma, d.w, d.h, d.pitch = py, pc, w, h, pitch
+            else:
+                p, (rows, w), (pitch, _) = view(f, k, "[3h/2, w] (strides (pitch, 1))", 2, (1,))
+                if rows % 3:
+                    raise YbError(f"{fn}: frame {k}: an nv12 array has 3h/2 rows, got {rows}")
+                h = rows // 3 * 2
+                d.data, d.chroma, d.w, d.h, d.pitch = p, p + h * pitch, w, h, pitch
+        return frames, arr, F
+
+    def predict_device_frames(self, frames, fmt: str = "rgb", quantized: bool = False, stream: Optional[int] = None):
+        """1..batch frames in device memory of one format (see ``_device_frames``) -> the reference's per-image resize on the
+        device -> forward (``yb_network_predict_device_frames``).  `stream`: the integer cudaStream_t the frames were written
+        on (``torch.cuda.current_stream().cuda_stream``), None for the legacy default stream."""
+        keep, arr, F = self._device_frames(frames, fmt, "predict_device_frames")
+        p = lib().yb_network_predict_device_frames(self._h, arr, len(keep), F, int(quantized), C.c_void_p(stream or 0))
+        _check(bool(p))
+        return self.layer_output(self.n - 1)
+
+    def submit_device_frames(self, frames, thresh: float, fmt: str = "rgb", nms: float = 0.45, relative: int = 1,
+                             letter: int = 0, max_rows: int = 2048, quantized: bool = False,
+                             stream: Optional[int] = None) -> int:
+        """Pipelined device frames -> detections (``yb_network_submit_device_frames``); frames and `stream` as in
+        predict_device_frames.  The frame objects are kept referenced until the ticket is collected with
+        collect_detections; the stream ordering rules of the C call say when their memory may be rewritten."""
+        keep, arr, F = self._device_frames(frames, fmt, "submit_device_frames")
+        self._inflight = getattr(self, "_inflight", {})
+        t = lib().yb_network_submit_device_frames(self._h, arr, len(keep), F, int(quantized), thresh, nms, relative, letter,
+                                                  max_rows, C.c_void_p(stream or 0))
+        _check(t >= 0)
+        self._inflight[("u8", t)] = (keep, max_rows, len(keep))
+        return t
+
     def collect_detections(self, ticket: int, quantized: bool = False, copy: bool = True):
         """Returns (list of [n_b, 5 + classes] arrays, counts int32, bytes moved device -> host) for the ticket's images:
-        batch of them for submit_u8, nimg for submit_frames_u8."""
+        batch of them for submit_u8, nimg for submit_frames_u8 and submit_device_frames."""
         rows, counts, moved = C.POINTER(C.c_float)(), C.POINTER(C.c_int)(), C.c_size_t()
         stride = lib().yb_network_collect_detections(self._h, ticket, int(quantized), C.byref(rows), C.byref(counts), C.byref(moved))
         _check(stride > 0)

@@ -291,6 +291,37 @@ static void check_max_rows(const char *fn, int max_rows) {
     if (max_rows <= 0 || max_rows > DET_MAX_ROWS)
         fatal_throw(std::string(fn) + ": max_rows must be in 1.." + std::to_string(DET_MAX_ROWS));
 }
+// The device-frame calls: everything but the memory kind (check_frame_memory), without touching the device.
+static void check_device_frames(const Network &net, const char *fn, const yb_device_frame *frames, int nimg, int format) {
+    const std::string f(fn);
+    if (nimg < 1 || nimg > net.batch)
+        fatal_throw(f + ": nimg " + std::to_string(nimg) + " outside 1.." + std::to_string(net.batch) + " (net.batch)");
+    if (!frames) fatal_throw(f + ": null frames array");
+    if (format < YB_FRAME_RGB || format > YB_FRAME_NV12) fatal_throw(f + ": unknown frame format " + std::to_string(format));
+    if (net.c != 3)
+        fatal_throw(f + ": device frames have 3 channels, the network's input has " + std::to_string(net.c));
+    const bool nv12 = format == YB_FRAME_NV12;
+    for (int b = 0; b < nimg; ++b) {
+        const yb_device_frame &d = frames[b];
+        const std::string fb = f + ": frame " + std::to_string(b);
+        if (!d.data) fatal_throw(fb + " is null");
+        if (nv12 && !d.chroma) fatal_throw(fb + " has a null chroma plane");
+        if (d.w < 1 || d.h < 1) fatal_throw(fb + " has size " + std::to_string(d.w) + "x" + std::to_string(d.h));
+        if (nv12 && (d.w % 2 || d.h % 2))
+            fatal_throw(fb + " has size " + std::to_string(d.w) + "x" + std::to_string(d.h) + ", NV12 needs an even width and height");
+        const long long row = format == YB_FRAME_RGB || format == YB_FRAME_BGR ? 3LL * d.w : d.w;
+        if (d.pitch < row)
+            fatal_throw(fb + " has pitch " + std::to_string(d.pitch) + " below its row of " + std::to_string(row) + " bytes");
+        long long span = (long long)(d.h - 1) * d.pitch + row;   // the resize indexes within a frame in 32 bits
+        if (format == YB_FRAME_RGB_PLANAR) {
+            if (d.plane_stride < (long long)d.pitch * d.h)
+                fatal_throw(fb + " has plane_stride " + std::to_string(d.plane_stride) + " below pitch * h = " +
+                            std::to_string((long long)d.pitch * d.h));
+            span += 2 * d.plane_stride;
+        }
+        if (span > INT_MAX) fatal_throw(fb + " addresses more than INT_MAX bytes");
+    }
+}
 
 // net.batch frames of one size, stacked: the uniform case of the frame entry points
 struct Uniform {
@@ -350,6 +381,32 @@ float *yb_network_predict_frames_u8(yb_network *n, const unsigned char *const *f
     net.last_launches = engine_num_launches(e) + 1;
     return net.layers.back().output;
     YB_CATCH(nullptr)
+}
+float *yb_network_predict_device_frames(yb_network *n, const yb_device_frame *frames, int nimg, int format, int quantized,
+                                        void *stream) {
+    YB_TRY
+    Network &net = n->net;
+    check_device_frames(net, "predict_device_frames", frames, nimg, format);
+    check_frame_memory(net.device, "predict_device_frames", frames, nimg, format);
+    Engine *e = get_engine(n, quantized);
+    engine_upload_device_frames(e, &net, frames, nimg, format, stream);
+    engine_forward(e, nullptr, nullptr);
+    engine_download_outputs(e, &net, nullptr);
+    net.last_launches = engine_num_launches(e) + 1;
+    return net.layers.back().output;
+    YB_CATCH(nullptr)
+}
+int yb_network_submit_device_frames(yb_network *n, const yb_device_frame *frames, int nimg, int format, int quantized,
+                                    float thresh, float nms, int relative, int letter, int max_rows, void *stream) {
+    YB_TRY
+    check_device_frames(n->net, "submit_device_frames", frames, nimg, format);
+    check_max_rows("submit_device_frames", max_rows);
+    check_frame_memory(n->net.device, "submit_device_frames", frames, nimg, format);
+    Engine *e = get_engine(n, quantized);
+    const int t = engine_submit_device_frames(e, &n->net, frames, nimg, format, thresh, nms, relative, letter, max_rows, stream);
+    n->net.last_launches = engine_num_launches(e) + 5;   // + resize, count, emit, iou, nms
+    return t;
+    YB_CATCH(-1)
 }
 /* diagnostic: the resized planar float images the device pipeline produced for the last predict_image_u8 */
 int yb_network_fetch_input(yb_network *n, int quantized, float *dst) {

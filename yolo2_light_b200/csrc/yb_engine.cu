@@ -104,6 +104,8 @@ struct Engine {
     };
     FrameStage u8;                      // device-side input pipeline + decode geometry of the synchronous calls
     float *d_unit = nullptr;            // byte value -> float /255. (k_resize_frames)
+    // hand-off of the caller's device frames: produced on the caller's stream (ev_frames_ready) / read (ev_frames_read)
+    cudaEvent_t ev_frames_ready = nullptr, ev_frames_read = nullptr;
     // ---- pipelined end-to-end path: H2D(k+1) | compute(k) | D2H(k-1) on three streams -----------------
     struct DetWs {                      // decode + NMS workspace for `cap` candidate rows per image
         float *rows = nullptr; unsigned *mask = nullptr; int *blkcnt = nullptr, *counts = nullptr;
@@ -148,6 +150,8 @@ Engine::~Engine() {
     if (det.counts) cudaFree(det.counts);
     free_stage(u8);
     if (d_unit) cudaFree(d_unit);
+    if (ev_frames_ready) cudaEventDestroy(ev_frames_ready);
+    if (ev_frames_read) cudaEventDestroy(ev_frames_read);
     for (Slot &sl : slots) {
         free_stage(sl.u8);
         if (sl.det.rows) cudaFree(sl.det.rows);
@@ -1184,34 +1188,49 @@ static bool stage_frames(Engine *e, Engine::FrameStage &st, const Network *net, 
                          const int *w, const int *h, int nimg, int letter, cudaStream_t s) {
     const int B = e->batch, c = net->c;
     fill_geo(e, st, net, w, h, nimg, letter);
+    std::vector<size_t> off(nimg);
     size_t total = 0;
     bool net_size = true;
     for (int b = 0; b < nimg; ++b) {
-        st.h_geo[b].off = total;
+        off[b] = total;
         total += (size_t)w[b] * h[b] * c;
         net_size &= w[b] == net->w && h[b] == net->h;
     }
-    // room for a zero tail of network-size frames (the 8-bit stem reads whole batches), and 16 bytes for the last vector load
-    // of k_resize_frames
-    const size_t need = std::max(total, net_size ? (size_t)B * net->w * net->h * c : 0) + 16;
+    // room for a zero tail of network-size frames (the 8-bit stem reads whole batches)
+    const size_t need = std::max(total, net_size ? (size_t)B * net->w * net->h * c : 0);
     if (need > st.bytes) {
         if (st.buf) cudaFree(st.buf);
         CUDA_OK(cudaMalloc(&st.buf, need));
         st.bytes = need;
     }
+    for (int b = 0; b < nimg; ++b) { st.h_geo[b].src = st.buf + off[b]; st.h_geo[b].pitch = w[b] * c; }
     for (int b = 0; b < nimg;) {
         size_t run = (size_t)w[b] * h[b] * c;
         int nb = b + 1;
         while (nb < nimg && frames[nb] == frames[b] + run) run += (size_t)w[nb] * h[nb] * c, ++nb;
-        CUDA_OK(cudaMemcpyAsync(st.buf + st.h_geo[b].off, frames[b], run, cudaMemcpyHostToDevice, s));
+        CUDA_OK(cudaMemcpyAsync(st.buf + off[b], frames[b], run, cudaMemcpyHostToDevice, s));
         b = nb;
     }
     CUDA_OK(cudaMemcpyAsync(st.d_geo, st.h_geo, (size_t)B * sizeof(ImageGeo), cudaMemcpyHostToDevice, s));
     return net_size;
 }
 
-// staged frames -> the network's planar f32 input; images nimg .. batch-1 are zero
-static void launch_resize(Engine *e, const Engine::FrameStage &st, const Network *net, int nimg, float *dst, cudaStream_t s) {
+// The table of nimg caller's device frames (each entry points at the frame where it lies), enqueued on `s`.
+static void stage_device_frames(Engine *e, Engine::FrameStage &st, const Network *net, const yb_device_frame *frames,
+                                int nimg, int letter, cudaStream_t s) {
+    std::vector<int> w(nimg), h(nimg);
+    for (int b = 0; b < nimg; ++b) { w[b] = frames[b].w; h[b] = frames[b].h; }
+    fill_geo(e, st, net, w.data(), h.data(), nimg, letter);
+    for (int b = 0; b < nimg; ++b) {
+        ImageGeo &g = st.h_geo[b];
+        g.src = frames[b].data; g.chroma = frames[b].chroma; g.pitch = frames[b].pitch; g.plane = frames[b].plane_stride;
+    }
+    CUDA_OK(cudaMemcpyAsync(st.d_geo, st.h_geo, (size_t)e->batch * sizeof(ImageGeo), cudaMemcpyHostToDevice, s));
+}
+
+// frames described by st.d_geo, of format fmt -> the network's planar f32 input; images nimg .. batch-1 are zero
+static void launch_resize(Engine *e, const Engine::FrameStage &st, const Network *net, int nimg, int fmt, float *dst,
+                          cudaStream_t s) {
     if (!e->d_unit) {   // load_image_stb's conversion, additionally.c:3093-3103
         float unit[256];
         for (int v = 0; v < 256; ++v) unit[v] = (float)((double)(float)v / 255.);
@@ -1219,17 +1238,62 @@ static void launch_resize(Engine *e, const Engine::FrameStage &st, const Network
         CUDA_OK(cudaMemcpy(e->d_unit, unit, sizeof(unit), cudaMemcpyHostToDevice));
     }
     const dim3 grid((unsigned)((net->h + RS_ROWS - 1) / RS_ROWS), (unsigned)nimg);
-    k_resize_frames<<<grid, RS_THREADS, 0, s>>>(st.buf, st.d_geo, e->d_unit, net->c, dst, net->w, net->h);
+    auto *k = fmt == YB_FRAME_BGR ? k_resize_frames<YB_FRAME_BGR> : fmt == YB_FRAME_RGB_PLANAR ? k_resize_frames<YB_FRAME_RGB_PLANAR>
+            : fmt == YB_FRAME_NV12 ? k_resize_frames<YB_FRAME_NV12> : k_resize_frames<YB_FRAME_RGB>;
+    k<<<grid, RS_THREADS, 0, s>>>(st.d_geo, e->d_unit, net->c, dst, net->w, net->h);
     const size_t per = (size_t)net->c * net->h * net->w;
     if (nimg < e->batch) CUDA_OK(cudaMemsetAsync(dst + nimg * per, 0, (e->batch - nimg) * per * sizeof(float), s));
+}
+
+// The caller's device frames -> dst, on the engine stream `s`: the table goes up, `s` waits for the work enqueued on the
+// caller's stream `user` before the call (the frames' producer), the resize reads the frames, and `user` waits for that
+// resize, so that the caller's later writes into the frames come after it.  The engine's events are recorded and waited on
+// at once, so each call may reuse them.
+static void resize_device_frames(Engine *e, Engine::FrameStage &st, const Network *net, const yb_device_frame *frames,
+                                 int nimg, int fmt, int letter, float *dst, cudaStream_t s, cudaStream_t user) {
+    if (!e->ev_frames_ready) {
+        CUDA_OK(cudaEventCreateWithFlags(&e->ev_frames_ready, cudaEventDisableTiming));
+        CUDA_OK(cudaEventCreateWithFlags(&e->ev_frames_read, cudaEventDisableTiming));
+    }
+    stage_device_frames(e, st, net, frames, nimg, letter, s);
+    CUDA_OK(cudaEventRecord(e->ev_frames_ready, user));
+    CUDA_OK(cudaStreamWaitEvent(s, e->ev_frames_ready, 0));
+    launch_resize(e, st, net, nimg, fmt, dst, s);
+    CUDA_OK(cudaEventRecord(e->ev_frames_read, s));
+    CUDA_OK(cudaStreamWaitEvent(user, e->ev_frames_read, 0));
 }
 
 // nimg u8 HWC frames of their own sizes -> resized planar float in the engine's input staging buffer
 void engine_upload_frames(Engine *e, Network *net, const unsigned char *const *frames, const int *w, const int *h, int nimg) {
     CUDA_OK(cudaSetDevice(e->opt.device));
     stage_frames(e, e->u8, net, frames, w, h, nimg, 0, e->stream);
-    launch_resize(e, e->u8, net, nimg, e->d_input, e->stream);
+    launch_resize(e, e->u8, net, nimg, YB_FRAME_RGB, e->d_input, e->stream);
     CUDA_OK(cudaGetLastError());
+}
+
+void engine_upload_device_frames(Engine *e, Network *net, const yb_device_frame *frames, int nimg, int fmt, void *stream) {
+    CUDA_OK(cudaSetDevice(e->opt.device));
+    resize_device_frames(e, e->u8, net, frames, nimg, fmt, 0, e->d_input, e->stream, (cudaStream_t)stream);
+    CUDA_OK(cudaGetLastError());
+}
+
+// Throws unless every frame's memory (data, and chroma for NV12) is device or managed memory of `device`.
+void check_frame_memory(int device, const char *fn, const yb_device_frame *frames, int nimg, int fmt) {
+    for (int b = 0; b < nimg; ++b) {
+        for (int p = 0; p < (fmt == YB_FRAME_NV12 ? 2 : 1); ++p) {
+            cudaPointerAttributes a{};
+            const cudaError_t r = cudaPointerGetAttributes(&a, p ? frames[b].chroma : frames[b].data);
+            if (r != cudaSuccess) cudaGetLastError();
+            const char *kind = r != cudaSuccess ? "unknown" : a.type == cudaMemoryTypeHost ? "pinned host memory"
+                             : a.type == cudaMemoryTypeDevice ? "device memory" : a.type == cudaMemoryTypeManaged ? "managed memory"
+                             : "host memory";
+            if (r != cudaSuccess || (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) || a.device != device)
+                fatal_throw(std::string(fn) + ": frame " + std::to_string(b) + (p ? " chroma" : "") + " is " + kind +
+                            (r == cudaSuccess && a.type != cudaMemoryTypeHost && a.type != cudaMemoryTypeUnregistered
+                                 ? " of device " + std::to_string(a.device) : std::string()) +
+                            ", not device memory of device " + std::to_string(device));
+        }
+    }
 }
 
 void *engine_stream(Engine *e) { return e->stream; }
@@ -1569,8 +1633,11 @@ int engine_detect(Engine *e, Network *net, const int *w, const int *h, int nimg,
 // forward of the NEXT batch), and returns a ticket.  engine_collect_detections waits for that batch and copies back exactly
 // the candidate rows.  Host traffic per batch: the u8 frames in (a quarter of the float images), counts + rows out (a few
 // hundred KB instead of the 124 MB of yolo tensors).
-int engine_submit_frames(Engine *e, Network *net, const unsigned char *const *frames, const int *w, const int *h, int nimg,
-                         float thresh, float nms, int relative, int letter, int max_rows) {
+//
+// `stage` enqueues on the copy-in stream what makes the slot's input, host or device frames: it fills the slot's geometry
+// table and either resizes into sl.d_in (returns nullptr) or returns 8-bit frames of the network size for the stem to read.
+static int submit_detections(Engine *e, Network *net, int nimg, float thresh, float nms, int relative, int max_rows,
+                             const std::function<const unsigned char *(Engine::Slot &)> &stage) {
     CUDA_OK(cudaSetDevice(e->opt.device));
     ensure_slots(e);
     const int k = e->next_slot;
@@ -1592,17 +1659,10 @@ int engine_submit_frames(Engine *e, Network *net, const unsigned char *const *fr
     // The slot's frames and geometry table go on s_in.  The decode below reads the table on the compute stream behind ev_in,
     // and the next submit to this slot rewrites it only after waiting for ev_comp (above) -- and only once this ticket has
     // been collected, which waits for ev_det, so the pinned host table is no longer being copied either.
-    const bool net_size = stage_frames(e, sl.u8, net, frames, w, h, nimg, letter, e->s_in);
-    const bool direct = e->first_op_u8 && net_size && net->c == 3;   // frames of the network size: no staging
-    if (direct) {
-        const size_t frame = (size_t)net->w * net->h * net->c;
-        if (nimg < B) CUDA_OK(cudaMemsetAsync(sl.u8.buf + nimg * frame, 0, (B - nimg) * frame, e->s_in));
-    } else {
-        launch_resize(e, sl.u8, net, nimg, sl.d_in, e->s_in);
-    }
+    const unsigned char *direct = stage(sl);
     CUDA_OK(cudaEventRecord(sl.ev_in, e->s_in));
     CUDA_OK(cudaStreamWaitEvent(e->stream, sl.ev_in, 0));
-    engine_forward_impl(e, sl.d_in, direct ? sl.u8.buf : nullptr, e->stream);
+    engine_forward_impl(e, sl.d_in, direct, e->stream);
     // Candidate selection + box decode (k_det_count / k_det_emit: they read the objectness planes and, for the few candidates,
     // their class scores) run right behind the forward on the compute stream, straight on the engine's yolo tensors -- the next
     // forward overwrites those, so this is the only part that must not slip.  What follows (IoU matrix + per-class NMS) works on
@@ -1625,6 +1685,28 @@ int engine_submit_frames(Engine *e, Network *net, const unsigned char *const *fr
     CUDA_OK(cudaGetLastError());
     sl.busy = true; sl.mode = 1; sl.nimg = nimg;
     return k;
+}
+
+int engine_submit_frames(Engine *e, Network *net, const unsigned char *const *frames, const int *w, const int *h, int nimg,
+                         float thresh, float nms, int relative, int letter, int max_rows) {
+    return submit_detections(e, net, nimg, thresh, nms, relative, max_rows, [&](Engine::Slot &sl) -> const unsigned char * {
+        const bool net_size = stage_frames(e, sl.u8, net, frames, w, h, nimg, letter, e->s_in);
+        if (e->first_op_u8 && net_size && net->c == 3) {   // frames of the network size: no staging
+            const size_t frame = (size_t)net->w * net->h * net->c;
+            if (nimg < e->batch) CUDA_OK(cudaMemsetAsync(sl.u8.buf + nimg * frame, 0, (e->batch - nimg) * frame, e->s_in));
+            return sl.u8.buf;
+        }
+        launch_resize(e, sl.u8, net, nimg, YB_FRAME_RGB, sl.d_in, e->s_in);
+        return nullptr;
+    });
+}
+
+int engine_submit_device_frames(Engine *e, Network *net, const yb_device_frame *frames, int nimg, int fmt, float thresh,
+                                float nms, int relative, int letter, int max_rows, void *stream) {
+    return submit_detections(e, net, nimg, thresh, nms, relative, max_rows, [&](Engine::Slot &sl) -> const unsigned char * {
+        resize_device_frames(e, sl.u8, net, frames, nimg, fmt, letter, sl.d_in, e->s_in, (cudaStream_t)stream);
+        return nullptr;
+    });
 }
 
 // rows: pinned [batch][max_rows][5 + classes] (valid until the slot is reused), counts[batch] (0 beyond the ticket's images);

@@ -46,6 +46,13 @@ int engine_device_count();
 int engine_submit_frames(Engine *e, Network *net, const unsigned char *const *frames, const int *w, const int *h, int nimg,
                          float thresh, float nms, int relative, int letter, int max_rows);
 int engine_collect_detections(Engine *e, int ticket, const float **rows, const int **counts, size_t *d2h_bytes);
+// the caller's device frames (one YB_FRAME_* format, 3-channel networks), read in order with the caller's `stream`:
+// resize into the staging buffer (synchronous calls), or the pipelined path of engine_submit_frames
+void engine_upload_device_frames(Engine *e, Network *net, const yb_device_frame *frames, int nimg, int fmt, void *stream);
+int engine_submit_device_frames(Engine *e, Network *net, const yb_device_frame *frames, int nimg, int fmt, float thresh,
+                                float nms, int relative, int letter, int max_rows, void *stream);
+// throws unless the frames' memory is device or managed memory of `device`
+void check_frame_memory(int device, const char *fn, const yb_device_frame *frames, int nimg, int fmt);
 void engine_fetch_layer(Engine *e, Network *net, int layer, float *dst);
 void engine_fetch_input(Engine *e, float *dst);
 int engine_fetch_counts(Engine *e, int layer, int32_t *dst, size_t count);

@@ -12,6 +12,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../../include/yolo2_light_b200.h"   // YB_FRAME_*
+
 namespace yb {
 
 struct TV {            // tensor view (POD, passed by value to kernels)
@@ -86,45 +88,91 @@ __global__ void k_nhwc_to_nchw_f32(TV in, float *__restrict__ out) {
 // coalesced stores.  The /255. conversion is a 256-entry table (`unit`, made on the host with load_image_stb's own double
 // divide) read into shared memory: no divide in the kernel.  A span wider than RS_SPAN bytes (frames several thousand pixels wide) is read from global memory
 // directly; both ways give the same values.
+//
+// The source format F is a template parameter (YB_FRAME_*, include/yolo2_light_b200.h); every image carries its own
+// pointer(s) and row pitch.  Host frames are staged as packed RGB (c = net.c bytes per pixel).  For the caller's device
+// frames (c = 3): BGR swaps R and B when a byte is read; planar stages the three plane spans; NV12 stages the Y span and
+// the chroma span of each source row and converts them to RGB bytes in shared memory, once per source pixel, with
+// BT.601 limited-range fixed-point arithmetic (OpenCV's COLOR_YUV2RGB_NV12 constants).  The interpolation that follows
+// is the same for every format, so a device frame gives bit-for-bit what its RGB equivalent gives through the host path.
 // ------------------------------------------------------------------------------------------------------
 struct ImageGeo {               // one image of a batch (device table, uploaded with the frames)
-    unsigned long long off;     // byte offset of its 8-bit frame in the packed frame buffer
+    const unsigned char *src;   // RGB / BGR: first pixel; planar: the R plane; NV12: the Y plane
+    const unsigned char *chroma;   // NV12: the interleaved U, V plane (h / 2 rows, same pitch as Y)
+    long long plane;            // planar: bytes from one plane to the next
+    int pitch;                  // bytes from one row to the next
     int w, h;                   // frame size
     int new_w, new_h;           // correct_yolo_boxes' embedded size (the network size unless letterboxed)
     float w_scale, h_scale;     // resize_image's (w - 1) / (out_w - 1), (h - 1) / (out_h - 1): IEEE float divides, made
                                 // on the host so that the kernel has no divide
 };
 
-constexpr int RS_THREADS = 256, RS_ROWS = 4, RS_COLS = 1024, RS_SPAN = 12288;
+constexpr int RS_THREADS = 256, RS_ROWS = 4, RS_COLS = 1024, RS_SPAN = 12288, RS_PLANE = RS_SPAN / 3;
 static_assert(RS_THREADS == 256, "one thread per entry of the /255. table");
 
-// frame bytes [start, start + len) -> smem; returns the smem offset of byte `start`.  The frame buffer is allocated with a
-// 16-byte tail, so the last aligned vector never leaves it.
-__device__ __forceinline__ int rs_stage(const unsigned char *__restrict__ src, size_t start, int len, uint4 *smem) {
-    const size_t a = start & ~(size_t)15;
-    const int nvec = (int)((start + len - a + 15) >> 4);
-    const uint4 *g = reinterpret_cast<const uint4 *>(src + a);
-    for (int i = threadIdx.x; i < nvec; i += RS_THREADS) smem[i] = __ldg(g + i);
-    return (int)(start - a);
+// frame bytes [p, p + len) -> smem; returns the smem offset of byte p.  The 16-byte vectors are aligned in memory: the ones
+// wholly inside the span are read with one 16-byte load, the (at most two) that straddle its ends byte by byte, and only
+// the span's own bytes of them.  So no byte outside [p, p + len) is read, and a frame may start at any address and end on
+// the last byte of its allocation.  The smem bytes of a straddling vector that lie outside the span stay unwritten; nothing
+// reads them.
+__device__ __forceinline__ int rs_stage(const unsigned char *__restrict__ p, int len, uint4 *smem) {
+    const uintptr_t s = reinterpret_cast<uintptr_t>(p), e = s + (uintptr_t)len, a = s & ~(uintptr_t)15;
+    const int nvec = (int)((e - a + 15) >> 4);
+    for (int i = threadIdx.x; i < nvec; i += RS_THREADS) {
+        const uintptr_t v = a + 16 * (uintptr_t)i;
+        if (v >= s && v + 16 <= e) {
+            smem[i] = __ldg(reinterpret_cast<const uint4 *>(v));
+        } else {
+            unsigned char *d = reinterpret_cast<unsigned char *>(smem + i);
+            for (int j = 0; j < 16; ++j)
+                if (v + j >= s && v + j < e) d[j] = __ldg(reinterpret_cast<const unsigned char *>(v + j));
+        }
+    }
+    return (int)(s - a);
 }
 
-static __global__ void __launch_bounds__(RS_THREADS) k_resize_frames(const unsigned char *__restrict__ src,
-                                                                      const ImageGeo *__restrict__ geo,
-                                                                      const float *__restrict__ unit_tab, int c,
+// BT.601 limited range -> 8-bit RGB, OpenCV's fixed-point form (cvtColor COLOR_YUV2RGB_NV12).  Every intermediate fits in
+// an int: |yy| + |1673527 * v| + 2^19 < 2^30.
+__device__ __forceinline__ int nv12_clamp(int x) { return min(255, max(0, x)); }
+__device__ __forceinline__ int nv12_ch(int Y, int U, int V, int k) {
+    const int yy = max(0, Y - 16) * 1220542 + (1 << 19), u = U - 128, v = V - 128;
+    return nv12_clamp((k == 0 ? yy + 1673527 * v : k == 1 ? yy - 852492 * v - 409993 * u : yy + 2116026 * u) >> 20);
+}
+
+struct RsSrc {                  // one source row of a chunk; index 0 is column `lo`
+    const unsigned char *q[3];  // RGB / BGR / NV12 staged (converted): q[0]; planar: the three planes; NV12 read
+                                // directly: the Y row (q[0]) and the chroma row from column lo & ~1 (q[1])
+    int odd;                    // NV12 read directly: lo & 1
+};
+
+// byte of channel k of pixel lo + x
+template <int F>
+__device__ __forceinline__ int rs_px(const RsSrc &s, bool staged, int c, int x, int k) {
+    if (F == YB_FRAME_RGB) return s.q[0][x * c + k];
+    if (F == YB_FRAME_BGR) return s.q[0][x * 3 + 2 - k];
+    if (F == YB_FRAME_RGB_PLANAR) return s.q[k][x];
+    if (staged) return s.q[0][x * 3 + k];
+    const int uv = (x + s.odd) & ~1;
+    return nv12_ch(__ldg(s.q[0] + x), __ldg(s.q[1] + uv), __ldg(s.q[1] + uv + 1), k);
+}
+
+template <int F>
+static __global__ void __launch_bounds__(RS_THREADS) k_resize_frames(const ImageGeo *__restrict__ geo,
+                                                                      const float *__restrict__ unit_tab, int c_,
                                                                       float *__restrict__ dst, int out_w, int out_h) {
+    constexpr bool NV12 = F == YB_FRAME_NV12;
     __shared__ uint4 stage[2][RS_SPAN / 16];
+    __shared__ uint4 raw[NV12 ? 2 : 1][2][NV12 ? (RS_PLANE + 32) / 16 : 1];   // NV12: the Y and chroma spans of each row
     __shared__ float unit[256];
     unit[threadIdx.x] = unit_tab[threadIdx.x];   // RS_THREADS == 256; published by the first barrier
+    const int c = F == YB_FRAME_RGB ? c_ : 3;
     const int n = blockIdx.y;
     const ImageGeo g = geo[n];
-    const int w = g.w, h = g.h, rowb = w * c;          // w * h * c fits in an int (checked at the API)
-    const unsigned char *img = src + g.off;
+    const int w = g.w, h = g.h;
     float *out = dst + (size_t)n * c * out_h * out_w;
     const size_t plane = (size_t)out_h * out_w;
     const bool same = (out_w == w && out_h == h);
     const float w_scale = g.w_scale, h_scale = g.h_scale;
-    const unsigned char *s0 = reinterpret_cast<const unsigned char *>(stage[0]);
-    const unsigned char *s1 = reinterpret_cast<const unsigned char *>(stage[1]);
     const int r_end = min(out_h, (int)(blockIdx.x + 1) * RS_ROWS);
     for (int r = blockIdx.x * RS_ROWS; r < r_end; ++r) {
         int iy = r;
@@ -146,24 +194,62 @@ static __global__ void __launch_bounds__(RS_THREADS) k_resize_frames(const unsig
                 lo = cc0 == out_w - 1 ? w - 1 : (int)__fmul_rn((float)cc0, w_scale);
                 hi = cc1 == out_w - 1 ? w - 1 : (int)__fmul_rn((float)cc1, w_scale) + 1;
             }
-            const int len = (hi - lo + 1) * c;
-            const size_t start0 = g.off + (size_t)iy * rowb + (size_t)lo * c;
-            const bool staged = (int)(start0 & 15) + len <= RS_SPAN &&
-                                (!two || (int)((start0 + rowb) & 15) + len <= RS_SPAN);
-            const unsigned char *p0, *p1;       // byte of column `lo`, channel 0, of rows iy / iy + 1
+            const int npix = hi - lo + 1, len = npix * c;
+            const unsigned char *row[2] = {g.src + (size_t)iy * g.pitch, g.src + (size_t)(iy + two) * g.pitch};
+            bool staged;
+            if (F == YB_FRAME_RGB || F == YB_FRAME_BGR)
+                staged = (int)(reinterpret_cast<uintptr_t>(row[0] + lo * c) & 15) + len <= RS_SPAN &&
+                         (!two || (int)(reinterpret_cast<uintptr_t>(row[1] + lo * c) & 15) + len <= RS_SPAN);
+            else   // per plane (planar) or per staged span (NV12: Y, and chroma of at most npix + 2 bytes in RS_PLANE + 32)
+                staged = npix + 15 <= RS_PLANE;
+            RsSrc src[2];                       // rows iy / iy + 1 (the same row when !two)
+            int oy[2] = {0, 0}, ouv[2] = {0, 0};   // NV12 staged: smem offsets of the Y and chroma spans in raw[t]
             __syncthreads();                    // the previous chunk is done with the staging buffers
-            if (staged) {
-                p0 = s0 + rs_stage(src, start0, len, stage[0]);
-                p1 = two ? s1 + rs_stage(src, start0 + rowb, len, stage[1]) : p0;
-                __syncthreads();
-            } else {
-                p0 = img + (size_t)iy * rowb + (size_t)lo * c;
-                p1 = p0 + rowb;
+#pragma unroll
+            for (int t = 0; t < 2; ++t) {
+                if (t && !two) break;
+                unsigned char *s = reinterpret_cast<unsigned char *>(stage[t]);
+                if (F == YB_FRAME_RGB || F == YB_FRAME_BGR) {
+                    src[t].q[0] = staged ? s + rs_stage(row[t] + lo * c, len, stage[t]) : row[t] + lo * c;
+                } else if (F == YB_FRAME_RGB_PLANAR) {
+#pragma unroll
+                    for (int k = 0; k < 3; ++k) {
+                        const unsigned char *p = row[t] + k * g.plane + lo;
+                        src[t].q[k] = staged ? s + k * RS_PLANE + rs_stage(p, npix, stage[t] + k * (RS_PLANE / 16)) : p;
+                    }
+                } else {
+                    const unsigned char *yr = row[t] + lo, *cr = g.chroma + (size_t)((iy + t) >> 1) * g.pitch + (lo & ~1);
+                    if (staged) {
+                        src[t].q[0] = s;
+                        oy[t] = rs_stage(yr, npix, raw[t][0]);
+                        ouv[t] = rs_stage(cr, ((hi | 1) - (lo & ~1)) + 1, raw[t][1]);
+                    } else {
+                        src[t].q[0] = yr; src[t].q[1] = cr;
+                    }
+                    src[t].odd = lo & 1;
+                }
             }
+            if (!two) src[1] = src[0];
+            if (staged) __syncthreads();
+            if (NV12 && staged) {               // staged Y / chroma -> RGB bytes, once per source pixel
+#pragma unroll
+                for (int t = 0; t < 2; ++t) {
+                    if (t && !two) break;
+                    unsigned char *d = reinterpret_cast<unsigned char *>(stage[t]);
+                    const unsigned char *ys = reinterpret_cast<const unsigned char *>(raw[t][0]) + oy[t];
+                    const unsigned char *uvs = reinterpret_cast<const unsigned char *>(raw[t][1]) + ouv[t];
+                    for (int x = threadIdx.x; x < npix; x += RS_THREADS) {
+                        const int Y = ys[x], uv = (x + (lo & 1)) & ~1, U = uvs[uv], V = uvs[uv + 1];
+                        for (int k = 0; k < 3; ++k) d[x * 3 + k] = (unsigned char)nv12_ch(Y, U, V, k);
+                    }
+                }
+                __syncthreads();
+            }
+            const RsSrc &p0 = src[0], &p1 = src[1];
             for (int cc = cc0 + threadIdx.x; cc <= cc1; cc += RS_THREADS) {
                 float *o = out + (size_t)r * out_w + cc;
                 if (same) {
-                    for (int k = 0; k < c; ++k) o[k * plane] = unit[p0[(cc - lo) * c + k]];
+                    for (int k = 0; k < c; ++k) o[k * plane] = unit[rs_px<F>(p0, staged, c, cc - lo, k)];
                     continue;
                 }
                 // the reference's `part` image at (cc, row): the last column (or a 1-pixel-wide frame) copies the edge
@@ -178,13 +264,12 @@ static __global__ void __launch_bounds__(RS_THREADS) k_resize_frames(const unsig
                 }
                 const float ndx = __fsub_rn(1.f, dx), ndy = __fsub_rn(1.f, dy);
                 for (int k = 0; k < c; ++k) {
-                    const int ia = xa * c + k;
-                    float part0 = unit[p0[ia]];
-                    if (!edge) part0 = __fadd_rn(__fmul_rn(ndx, part0), __fmul_rn(dx, unit[p0[ia + c]]));
+                    float part0 = unit[rs_px<F>(p0, staged, c, xa, k)];
+                    if (!edge) part0 = __fadd_rn(__fmul_rn(ndx, part0), __fmul_rn(dx, unit[rs_px<F>(p0, staged, c, xa + 1, k)]));
                     float val = __fmul_rn(ndy, part0);
                     if (two) {
-                        float part1 = unit[p1[ia]];
-                        if (!edge) part1 = __fadd_rn(__fmul_rn(ndx, part1), __fmul_rn(dx, unit[p1[ia + c]]));
+                        float part1 = unit[rs_px<F>(p1, staged, c, xa, k)];
+                        if (!edge) part1 = __fadd_rn(__fmul_rn(ndx, part1), __fmul_rn(dx, unit[rs_px<F>(p1, staged, c, xa + 1, k)]));
                         val = __fadd_rn(val, __fmul_rn(dy, part1));
                     }
                     o[k * plane] = val;
