@@ -285,6 +285,12 @@ int  yb_network_set_option(yb_network *net, const char *name, int value);
 /* Engine facts (builds the engine if needed): "launches", "tc_layers" (convolutions on the tensor cores),
    "act_bytes" (device memory of the activation buffers).  -1: unknown key. */
 long yb_network_get_info(yb_network *net, int quantized, const char *key);
+/* The tensor-core plan of layer `layer` (builds the engine if needed), read-only: up to n of {kernel (0 k_conv_tc,
+ * 1 k_conv_tc_reg, 2 k_stem_tc, 3 k_stem_s2_tc), kind (0 bf16, 1 int8, 2 xnor, 3 tf32), TW, TH, BN, BK, nt, bstat, stages,
+ * sps, grid, num_work, tma_epi, jshift, out_ldc (output pixel stride, elements; 0: no NHWC output)} into fields; -1 in a
+ * field that does not apply to the kernel (the stems' fixed tiles).  Returns the number written: 0 for a layer without a
+ * tensor-core plan, -1 on error. */
+int  yb_network_tc_plan(yb_network *net, int quantized, int layer, int *fields, int n);
 /* Raw integer results of conv layer i (NCHW, batch-major) when "keep_counts" is on; returns the element count. */
 int  yb_network_fetch_counts(yb_network *net, int i, int quantized, int32_t *dst, size_t count);
 int  yb_network_layer_outputs(const yb_network *net, int i);   /* layer.outputs (per image) */

@@ -1,0 +1,900 @@
+"""The tensor-core convolutions bit for bit, on data on which they are exact.
+
+Activations are a/8 (a in [-8, 8]; stem images a/16, a in [0, 16]), weights b/64 (b in [-8, 8]), biases c/512.  Every
+product is then exact in bf16 / tf32, every partial sum a multiple of the product grid, and while sum |x| |w| over a dot
+product stays below 2^20 grid units every partial sum is an exact f32 number in any summation order, whatever the tensor
+core's alignment of its addends and with or without FMA contraction.  The accumulator is the float64 dot product; the
+epilogue is a few IEEE f32 operations (bias add, leaky, residual add, second leaky, round to bf16) that numpy float32
+repeats bit for bit.  So every output is known to the bit, and a single wrong element -- a stale ring stage, a wrong
+bias column, a tile row stored in the wrong place -- fails the comparison, where a rel-L2 bound over the tensor would not
+notice it.  `premise` checks these conditions on the host for every convolution before anything runs.
+
+A layer under test that writes bf16 needs a consumer (a convolution without one writes f32): a one-hot 3x3 convolution
+(bias 0, linear, one weight of 1 per filter) whose filters see the tested output through every tap, border included.  Its
+output is a set of exactly shifted copies of the tested output, so a value stored into a zero border or into a pad row of a
+merged-row tile shows up bitwise.  Each case names the edge of the tile planner it is for and asserts it through
+Network.tc_plan.
+
+The helpers and the case table run on the CPU; the tests that need a GPU are marked."""
+import os
+import struct
+
+import numpy as np
+import pytest
+
+import ybtest_util as util
+from test_gpu_tc import bf16_round
+from yolo2_light_b200 import cfgs
+
+LINEAR, LEAKY = "linear", "leaky"
+BOUND_UNITS = 2 ** 20          # |partial sums| in product-grid units: 4 bits below f32's 24-bit significand
+F32_01 = np.float32(0.1)
+
+
+# ---- data ---------------------------------------------------------------------------------------------------------------
+def grid_acts(rng, shape, den=8, lo=-8, hi=8):
+    return (rng.integers(lo, hi + 1, shape) / den).astype(np.float32)
+
+
+def grid_weights(rng, n, c, k):
+    return (rng.integers(-8, 9, (n, c, k, k)) / 64).astype(np.float32)
+
+
+def grid_bias(rng, n, den=512, lim=512):
+    return (rng.integers(-lim, lim + 1, n) / den).astype(np.float32)
+
+
+def onehot(n, c, k, pairs):
+    """n filters, filter j reads channel pairs[j][0] through tap pairs[j][1] (ky * k + kx) with weight 1"""
+    w = np.zeros((n, c, k, k), np.float32)
+    for j, (ch, t) in enumerate(pairs):
+        w[j, ch, t // k, t % k] = 1.0
+    return w
+
+
+def consumer_pairs(c):
+    """(channel, tap) of every filter of a one-hot 3x3 consumer over c channels: all 9 taps of every channel (9 c filters)"""
+    return [(j % c, (j // c + j % c) % 9) for j in range(9 * c)]
+
+
+class Net:
+    """A small network under construction: cfg sections, the weights of each convolution and what each is expected to
+    run on ("reg" k_conv_tc_reg, "tc" k_conv_tc, "stem" k_stem_tc, "stem_s2" k_stem_s2_tc, "simt" the CUDA cores)."""
+
+    def __init__(self, c, h, w, batch, seed, calib=None):
+        net = cfgs._net(w, h, calib)
+        net[1]["channels"] = str(c)
+        self.secs = [net]
+        self.rng = np.random.default_rng(seed)
+        self.batch, self.c, self.h, self.w = batch, c, h, w
+        self.params = {}     # layer -> (weights [n][c][k][k], bias)
+        self.kern = {}       # layer -> expected kernel
+        self.edges = []      # (layer, description, predicate on the plan)
+        self.env = {}
+        self.quantized = 0
+        self.fuse = 1
+        self.x = None        # the input images, when a case sets them
+
+    @property
+    def n(self):
+        return len(self.secs) - 1
+
+    def shapes(self):
+        return cfgs.conv_shapes(self.secs)
+
+    def conv(self, n, size=3, stride=1, act=LEAKY, kern="reg", w=None, b=None, **extra):
+        self.secs.append(cfgs._conv(n, size, stride, bn=False, act=act, **extra))
+        c = self.shapes()[-1]["c"]
+        w = grid_weights(self.rng, n, c, size) if w is None else w
+        b = grid_bias(self.rng, n) if b is None else b
+        i = self.n - 1
+        self.params[i] = (np.asarray(w, np.float32), np.asarray(b, np.float32))
+        self.kern[i] = kern
+        return i
+
+    def preserve(self, kern="reg"):
+        """grid-preserving 1x1 layer: one-hot weights over a permutation of the channels, a bias on the activation grid,
+        linear -- its output stays exactly on the activation grid"""
+        c = self.shapes()[-1]["out_c"] if self.n else self.c
+        perm = self.rng.permutation(c)
+        w = onehot(c, c, 1, [(int(perm[j]), 0) for j in range(c)])
+        return self.conv(c, 1, 1, LINEAR, kern, w=w, b=grid_acts(self.rng, c, 8, -4, 4))
+
+    def consume(self):
+        """one-hot 3x3 consumer of the last layer's output (f32 out when it is the last layer): k_conv_tc where its channels
+        fill whole 32-byte bf16 rows, else the CUDA cores"""
+        c = self.shapes()[-1]["out_c"]
+        pairs = consumer_pairs(c)
+        kern = "tc" if c % 16 == 0 else "simt"
+        return self.conv(len(pairs), 3, 1, LINEAR, kern, w=onehot(len(pairs), c, 3, pairs), b=np.zeros(len(pairs), np.float32))
+
+    def add(self, name, **opts):
+        self.secs.append((name, {k: str(v) for k, v in opts.items()}))
+        return self.n - 1
+
+    def edge(self, layer, what, pred):
+        self.edges.append((layer, what, pred))
+        return self
+
+    def images(self, den=8, lo=-8, hi=8):
+        return grid_acts(np.random.default_rng(self.rng.integers(1 << 30)), (self.batch, self.c, self.h, self.w), den, lo, hi)
+
+
+def write_weights(net, path):
+    """The convolutions' weights in the reference's .weights format (cfgs.write_weights), no batch norm: biases[n], then
+    weights[n][c][k][k] per convolution in cfg order"""
+    with open(path, "wb") as f:
+        f.write(struct.pack("<iiiQ", 0, 2, 0, 0))
+        for i in sorted(net.params):
+            w, b = net.params[i]
+            b.astype("<f4").tofile(f)
+            w.astype("<f4").tofile(f)
+    return path
+
+
+# ---- reference ----------------------------------------------------------------------------------------------------------
+def conv_acc(x, w, stride, pad):
+    """float64 accumulators of a convolution over NHWC x: one matmul per tap"""
+    x = np.asarray(x, np.float64)
+    B, H, W, C = x.shape
+    n, _, k, _ = w.shape
+    OH, OW = (H + 2 * pad - k) // stride + 1, (W + 2 * pad - k) // stride + 1
+    xp = np.zeros((B, H + 2 * pad, W + 2 * pad, C))
+    xp[:, pad:pad + H, pad:pad + W] = x
+    acc = np.zeros((B, OH, OW, n))
+    w = np.asarray(w, np.float64)
+    for ky in range(k):
+        for kx in range(k):
+            xs = xp[:, ky:ky + stride * (OH - 1) + 1:stride, kx:kx + stride * (OW - 1) + 1:stride, :]
+            acc += xs @ w[:, :, ky, kx].T
+    return acc
+
+
+def grid_step(a):
+    """the coarsest power of two 2^-e (e <= 40) of which every element of a is a multiple"""
+    a = np.asarray(a, np.float64)
+    for e in range(41):
+        s = a * 2.0 ** e
+        if np.array_equal(s, np.round(s)):
+            return 2.0 ** -e
+    raise AssertionError("data off every binary grid")
+
+
+def premise(x, w, b, stride, pad):
+    """every partial sum of the convolution, and the bias add, is exact in f32 in any order; returns the largest
+    sum |x| |w| + |b| in units of the grid of those sums (0 for one-hot filters)"""
+    nz = w != 0
+    if np.all(nz.reshape(len(w), -1).sum(1) <= 1) and np.all(np.abs(w[nz]) == 1):
+        # one-hot filters: a single product per output, then the bias add, which must be exact itself
+        acc = conv_acc(x, w, stride, pad) + 0.0
+        s = acc.astype(np.float32) + b.astype(np.float32)
+        assert np.array_equal(s.astype(np.float64), acc + np.asarray(b, np.float64)), "one-hot layer: bias add rounds"
+        return 0.0
+    g = min(grid_step(x) * grid_step(w), grid_step(b))     # every partial sum and the bias add are multiples of g
+    units = (conv_acc(np.abs(x), np.abs(w), stride, pad) + np.abs(b)).max() / g
+    assert units < BOUND_UNITS, f"sum |x||w| = {units:.3g} grid units >= 2^20"
+    return units
+
+
+def leaky_tc(a):
+    """fmaxf(a, 0.1f * a): the epilogues of k_conv_tc_reg, k_conv_tc, k_stem_tc and k_stem_s2_tc"""
+    return np.maximum(a, F32_01 * a)
+
+
+def leaky_exact(a):
+    """act_exact: a > 0 ? a : (float)(0.1 * (double)a), the CUDA-core kernels (the reference's activate())"""
+    return np.where(a > 0, a, (0.1 * a.astype(np.float64)).astype(np.float32)).astype(np.float32)
+
+
+def epilogue(acc, b, act, kern, res=None, act2=LINEAR, bf16=True):
+    a = (acc + 0.0).astype(np.float32) + b.astype(np.float32)
+    act_f = leaky_exact if kern == "simt" else leaky_tc
+    if act == LEAKY:
+        a = act_f(a)
+    if res is not None:
+        a = a + res.astype(np.float32)
+        if act2 == LEAKY:
+            a = act_f(a)
+    return bf16_round(a) if bf16 else a.astype(np.float32)
+
+
+def run_reference(net, x, adt_bf16=True):
+    """Host model of the engine on these networks: every layer's output as stored (NHWC f32 values; bf16-rounded where the
+    engine keeps bf16), the [yolo] layers' raw head values, and the premise of every convolution.  Follows the engine's
+    layer plan: bf16 outputs unless a convolution has no consumer or only detection layers read it; conv + same-shape
+    shortcut fused when `fuse` is on, the conv is stride 1 and the shortcut its sole reader."""
+    shapes = net.shapes()
+    secs = net.secs[1:]
+    cons = {i: [] for i in range(len(secs))}
+    for i, L in enumerate(shapes):
+        t = L["type"]
+        if t == "route":
+            for j in L["layers"]:
+                cons[j].append(i)
+        elif t == "shortcut":
+            cons[i - 1].append(i); cons[L["index"]].append(i)
+        elif i > 0:
+            cons[i - 1].append(i)
+    outs, units = {}, {}
+    cur = np.ascontiguousarray(x.transpose(0, 2, 3, 1))
+    if net.kern.get(0, "").startswith("stem"):
+        cur = bf16_round(cur) if adt_bf16 else cur
+    fused_res = {}
+    for i, L in enumerate(shapes):
+        t = L["type"]
+        if t == "convolutional":
+            w, b = net.params[i]
+            units[i] = premise(cur, w, b, L["stride"], L["pad"])
+            acc = conv_acc(cur, w, L["stride"], L["pad"])
+            heads_only = bool(cons[i]) and all(shapes[r]["type"] in ("yolo", "region") for r in cons[i])
+            bf16 = adt_bf16 and bool(cons[i]) and not heads_only
+            nxt = shapes[i + 1] if i + 1 < len(shapes) else None
+            if (net.fuse and nxt is not None and nxt["type"] == "shortcut" and cons[i] == [i + 1] and L["stride"] == 1
+                    and nxt["index"] != i):
+                fused_res[i + 1] = (acc, b, L["activation"], net.kern[i])
+                outs[i] = None
+                continue
+            cur = epilogue(acc, b, L["activation"], net.kern[i], bf16=bf16)
+        elif t == "shortcut":
+            res = outs[L["index"]]
+            act2 = secs[i][1].get("activation", LINEAR)
+            if i in fused_res:
+                acc, b, act, kern = fused_res[i]
+                cur = epilogue(acc, b, act, kern, res=res, act2=act2, bf16=adt_bf16)
+            else:
+                a = cur + res
+                cur = leaky_exact(a) if act2 == LEAKY else a
+                cur = bf16_round(cur) if adt_bf16 else cur
+        elif t == "route":
+            cur = np.concatenate([outs[j] for j in L["layers"]], axis=3)
+        elif t == "yolo":
+            pass   # the head's f32 values stay in `cur`; the test applies the logistic
+        else:
+            raise NotImplementedError(t)
+        outs[i] = cur
+    return outs, units
+
+
+def shifted_copies(t, pairs):
+    """the one-hot 3x3 consumer's output: filter j = t[..., c_j] shifted by tap t_j, zero border (NHWC)"""
+    B, H, W, C = t.shape
+    tp = np.zeros((B, H + 2, W + 2, C), np.float32)
+    tp[:, 1:H + 1, 1:W + 1] = t
+    return np.stack([tp[:, tap // 3:tap // 3 + H, tap % 3:tap % 3 + W, c] for c, tap in pairs], axis=3)
+
+
+# ---- the case table -----------------------------------------------------------------------------------------------------
+def c_bk(C, bk):
+    n = Net(C, 9, 11, 2, 100 + C)
+    i = n.conv(64)
+    n.consume()
+    return n.edge(i, f"BK {bk} at C = {C}", lambda p: p["BK"] == bk)
+
+
+def c_filters(nf, bn=None):
+    n = Net(32, 7, 5, 3, 200 + nf)
+    i = n.conv(nf)
+    n.consume()
+    if bn:
+        n.env["YB_TC_BN"] = str(bn)
+    n.edge(i, f"n = {nf} not a multiple of BN", lambda p: nf % p["BN"] != 0 and p["nt"] == -(-nf // p["BN"]))
+    if bn:
+        n.edge(i, "two or more filter tiles", lambda p: p["nt"] >= 2)
+    return n
+
+
+def c_f32(nf, size=3):
+    n = Net(64, 13, 7, 2, 300 + nf)
+    i = n.conv(nf, size, act=LEAKY if nf != 255 else LINEAR, kern="tc")
+    return n.edge(i, f"f32 output, n = {nf}", lambda p: p["kernel"] == "k_conv_tc" and p["kind"] == "bf16")
+
+
+def c_width(h, w):
+    n = Net(32, h, w, 3, 400 + 7 * h + w)
+    i = n.conv(64)
+    n.consume()
+    return n.edge(i, f"OW {w} < TW, OW % TW != 0, or one-pixel tiles",
+                  lambda p: w < p["TW"] or w % p["TW"] != 0 or p["TW"] == w == 1)
+
+
+def c_tw128(w, batch):
+    n = Net(16, 1, w, batch, 500 + w)
+    i = n.conv(32)
+    n.consume()
+    return n.edge(i, "TW = 128: a k_conv_tc_reg half tile is half a pixel row", lambda p: p["TW"] == 128)
+
+
+def c_many_images_s1():
+    n = Net(32, 2, 2, 33, 601)
+    i = n.conv(32)
+    n.consume()
+    return n.edge(i, "one tile spans 8+ images (stride 1: 4 merged rows each)", lambda p: p["TH"] >= 8 * 4)
+
+
+def c_many_images_s2():
+    n = Net(32, 4, 6, 17, 602)
+    i = n.conv(64, 3, 2)
+    n.consume()
+    return n.edge(i, "one tile spans 3+ images (stride 2: 3 merged half rows each)", lambda p: p["TH"] >= 3 * 3)
+
+
+def c_straddle(h, w, batch):
+    n = Net(32, h, w, batch, 700 + h + w)
+    i = n.conv(64, 3, 2)
+    n.consume()
+    # merged half rows: OH + 1 per image; a half tile of TH / 2 rows straddles two images unless it divides them
+    return n.edge(i, "stride-2 half tiles straddle images",
+                  lambda p: max(p["TH"] // 2, 1) > 1 and (h // 2 + 1) % max(p["TH"] // 2, 1) != 0)
+
+
+def c_bump():
+    n = Net(32, 30, 2, 5, 801)
+    i = n.conv(32, 3, 2)
+    n.consume()
+    n.env["YB_TC_BN"] = "32"
+    return n.edge(i, "stride 2, BN 32: TW 1 -> 2", lambda p: p["BN"] == 32 and p["TW"] == 2)
+
+
+def c_knobs(bn=None, no_bstat=False, grid=None, stride=1):
+    n = Net(64, 12, 10, 2, 900 + (bn or 0) + 7 * (grid or 0) + stride)
+    i = n.conv(256, 3, stride)
+    n.consume()
+    if bn:
+        n.env["YB_TC_BN"] = str(bn)
+        n.edge(i, f"BN {bn}", lambda p: p["BN"] == bn)
+    if no_bstat:
+        n.env["YB_TC_NO_BSTAT"] = "1"
+        n.edge(i, "filter tiles streamed", lambda p: p["bstat"] == 0)
+    if grid:
+        n.env["YB_TC_GRID"] = str(grid)
+        n.edge(i, f"{grid} CTAs, several work items each", lambda p: p["grid"] == grid and p["num_work"] > grid)
+    return n
+
+
+def c_shortcut(act2, fuse):
+    n = Net(64, 10, 6, 3, 1000 + fuse + (act2 == LEAKY))
+    n.preserve()
+    i = n.conv(64)
+    n.add("shortcut", **{"from": "-2", "activation": act2})
+    n.consume()
+    n.fuse = fuse
+    return n.edge(i, f"shortcut act2 {act2}, fuse {fuse}", lambda p: p["kernel"] == "k_conv_tc_reg")
+
+
+def c_concat(first):
+    """two tested layers write channel slices of one [route] buffer, each beside the other"""
+    n = Net(32, 8, 6, 2, 1100 + first)
+    n.preserve()
+    a = n.conv(40)                        # 1
+    n.add("route", layers="-2")           # 2: alias of layer 0
+    b = n.conv(24)                        # 3
+    n.add("route", layers="-3, -1" if first else "-1, -3")
+    n.consume()
+    pos = "first" if first else "second"
+    # a channel slice: the output's pixel stride is the concat's 64 channels, not the layer's own
+    n.edge(a, f"layer 1 writes the {pos} slice", lambda p: p["kernel"] == "k_conv_tc_reg" and p["out_ldc"] == 64)
+    return n.edge(b, "layer 3 writes the other slice", lambda p: p["kernel"] == "k_conv_tc_reg" and p["out_ldc"] == 64)
+
+
+def c_yolo(tf32):
+    n = Net(64, 6, 10, 2, 1200 + tf32, calib=[16] * 4 if tf32 else None)
+    i = n.conv(255, 1, act=LINEAR, kern="tc")
+    n.secs.append(cfgs._yolo("0,1,2", cfgs.COCO_ANCHORS, 9))
+    n.quantized = tf32
+    kind = "tf32" if tf32 else "bf16"
+    return n.edge(i, f"fused [yolo], {kind}", lambda p: p["kind"] == kind and p["kernel"] == "k_conv_tc")
+
+
+def c_refused(size):
+    n = Net(8, 6, 10, 2, 1300 + size)
+    n.conv(16, size, 2 if size == 1 else 1, kern="simt")
+    n.consume()
+    return n
+
+
+def c_stem(nf, h, w, batch):
+    n = Net(3, h, w, batch, 1400 + nf + h)
+    i = n.conv(nf, kern="stem", w=(n.rng.integers(-8, 9, (nf, 3, 3, 3)) / 64).astype(np.float32))
+    n.consume()
+    n.env["YB_NO_STEM_S2_FUSE"] = "1"
+    return n.edge(i, f"k_stem_tc, n = {nf}", lambda p: p["kernel"] == "k_stem_tc")
+
+
+def c_stem_s2(h, w, batch):
+    n = Net(3, h, w, batch, 1500 + h + w)
+    # linear stem, small weights: its bf16 output (layer 1's input) stays on a grid fine enough for the bound
+    n.conv(32, act=LINEAR, kern="stem_s2", w=(n.rng.integers(-2, 3, (32, 3, 3, 3)) / 64).astype(np.float32),
+           b=grid_bias(n.rng, 32, 512, 64))
+    i = n.conv(64, 3, 2, kern="stem_s2", w=(n.rng.integers(-2, 3, (64, 32, 3, 3)) / 64).astype(np.float32))
+    n.consume()
+    return n.edge(i, "k_stem_s2_tc: stem + layer 1", lambda p: p["kernel"] == "k_stem_s2_tc")
+
+
+def c_calibration():
+    """the largest K (3x3x1024) at the largest sums: images of 7/8 and 1 (on the 1/8 grid), a filter of +1/8 weights and one
+    of -1/8 weights: |sum| ~ 1080 = 2^19.08 units of the 2^-9 product grid at every interior pixel; the other filters mix
+    large and small addends.  f32 output: the accumulator itself, not rounded to bf16."""
+    n = Net(1024, 5, 5, 2, 1600)
+    w = grid_weights(n.rng, 32, 1024, 3)
+    w[0] = 8 / 64
+    w[1] = -8 / 64
+    w[2] = np.where(n.rng.random((1024, 3, 3)) < 0.5, 8 / 64, 1 / 64)
+    i = n.conv(32, act=LINEAR, kern="tc", w=w)
+    n.x = (n.rng.integers(7, 9, (2, 1024, 5, 5)) / 8).astype(np.float32)
+    return n.edge(i, "K = 9216 at 2^19 product-grid units", lambda p: p["BK"] == 64)
+
+
+CASES = {
+    "calibration": c_calibration,
+    **{f"bk{bk}_c{C}": (lambda C=C, bk=bk: c_bk(C, bk)) for C, bk in [(16, 16), (48, 16), (80, 16), (112, 16), (96, 32),
+                                                                       (32, 32), (192, 64)]},
+    **{f"n{nf}": (lambda nf=nf: c_filters(nf)) for nf in (8, 24, 40, 72, 136, 264)},
+    "n520_bn128": lambda: c_filters(520, 128),
+    "n136_bn64": lambda: c_filters(136, 64),
+    **{f"f32_n{nf}": (lambda nf=nf: c_f32(nf, 1 if nf == 255 else 3)) for nf in (9, 18, 75, 255)},
+    **{f"w{w}_h{h}": (lambda h=h, w=w: c_width(h, w)) for h, w in [(5, 1), (3, 3), (9, 7), (11, 13), (7, 19), (3, 37)]},
+    "tw128_w256": lambda: c_tw128(256, 1),
+    "tw128_w200_b3": lambda: c_tw128(200, 3),
+    "images_s1_b33": c_many_images_s1,
+    "images_s2_b17": c_many_images_s2,
+    "straddle_6x10": lambda: c_straddle(6, 10, 3),
+    "straddle_38x38": lambda: c_straddle(38, 38, 3),
+    "s2_bn32_tw_bump": c_bump,
+    **{f"bn{bn}": (lambda bn=bn: c_knobs(bn=bn)) for bn in (32, 64, 128, 256)},
+    "bn64_s2": lambda: c_knobs(bn=64, stride=2),
+    "streamed": lambda: c_knobs(bn=64, no_bstat=True),
+    "streamed_s2": lambda: c_knobs(bn=128, no_bstat=True, stride=2),
+    "grid1": lambda: c_knobs(grid=1),
+    "grid3": lambda: c_knobs(bn=32, grid=3),
+    "grid3_s2": lambda: c_knobs(bn=64, grid=3, stride=2),
+    **{f"shortcut_{a}_fuse{f}": (lambda a=a, f=f: c_shortcut(a, f)) for a in (LINEAR, LEAKY) for f in (0, 1)},
+    "concat_first": lambda: c_concat(True),
+    "concat_second": lambda: c_concat(False),
+    "yolo_bf16": lambda: c_yolo(0),
+    "yolo_tf32": lambda: c_yolo(1),
+    "refused_c8_1x1s2": lambda: c_refused(1),
+    "refused_c8_3x3": lambda: c_refused(3),
+    "stem16": lambda: c_stem(16, 10, 14, 3),
+    "stem32": lambda: c_stem(32, 7, 9, 2),
+    **{f"stem_s2_{h}x{w}_b{b}": (lambda h=h, w=w, b=b: c_stem_s2(h, w, b)) for h, w, b in [(16, 16, 2), (38, 22, 3), (64, 48, 1)]},
+}
+
+
+def build_case(name):
+    net = CASES[name]()
+    if net.x is not None:
+        return net, net.x
+    stem = net.kern.get(0, "").startswith("stem")
+    x = net.images(16, 0, 16) if stem else net.images()
+    return net, x
+
+
+def logistic_bound(v):
+    """|__fdividef(1, 1 + __expf(-v)) - 1 / (1 + exp(-v))| bound (CUDA C Programming Guide, intrinsic functions): __expf(x)
+    is within 2 + floor(|1.173 x|) ulp, __fdividef within 2 ulp for a divisor in [2^-126, 2^126]; the 1 + e add rounds
+    once more (1/2 ulp).  The relative error of 1 + e is at most that of e, so the result is within
+    (2 + floor(|1.173 v|) + 0.5 + 2) ulp of an f32 value, relative to the result."""
+    return (4.5 + np.floor(np.abs(1.173 * v))) * 2.0 ** -23
+
+
+# ---- CPU tests ----------------------------------------------------------------------------------------------------------
+def test_calibration_case_reaches_the_top_of_the_bound():
+    """the calibration case holds the accumulator between 2^19 and 2^20 units of its product grid (2^-9)"""
+    net, x = build_case("calibration")
+    w, b = net.params[0]
+    assert grid_step(x) * grid_step(w) == 2.0 ** -9 and grid_step(b) >= 2.0 ** -9
+    _, units = run_reference(net, x, adt_bf16=True)
+    assert 2 ** 19 <= units[0] < BOUND_UNITS, units[0]
+
+
+@pytest.mark.parametrize("name", sorted(CASES))
+def test_case_premise(name):
+    """every convolution of every case is exact on the tensor cores: on the grid and below 2^20 product-grid units"""
+    net, x = build_case(name)
+    _, units = run_reference(net, x, adt_bf16=not net.quantized)
+    assert units and max(units.values()) < BOUND_UNITS
+
+
+@pytest.mark.parametrize("shape", [(16, 5, 7, 24, 3, 1, 2), (48, 6, 4, 40, 3, 2, 3), (64, 3, 9, 9, 1, 1, 2),
+                                   (192, 4, 4, 32, 3, 1, 1), (32, 1, 37, 72, 3, 1, 3)])
+def test_reference_equals_oracle_on_grid_data(shape):
+    """float64 per-tap matmul + the f32 epilogue == the oracle's f32 convolution (which sums in k order -- also exact on grid
+    data), bit for bit, linear activation"""
+    from oracle import port
+    C, H, W, n, k, s, B = shape
+    rng = np.random.default_rng(C + H + n)
+    x = grid_acts(rng, (B, C, H, W))
+    w = grid_weights(rng, n, C, k)
+    b = grid_bias(rng, n)
+    premise(x.transpose(0, 2, 3, 1), w, b, s, k // 2)
+    ref = epilogue(conv_acc(x.transpose(0, 2, 3, 1), w, s, k // 2), b, LINEAR, "reg", bf16=False)
+    exp = port.conv_fp32(x, w, b, n, k, s, k // 2, 3)
+    assert util.bits_equal(ref.transpose(0, 3, 1, 2), exp)
+
+
+def test_leaky_emulations_differ_where_the_kernels_do():
+    """fmaxf(a, 0.1f a) and (float)(0.1 (double) a) are different functions: the two epilogue emulations are not
+    interchangeable"""
+    a = -(np.arange(1, 4097, dtype=np.float32) / 512)
+    assert not np.array_equal(leaky_tc(a), leaky_exact(a))
+
+
+def _tested_layers(net):
+    one_hot = lambda w: np.all((w != 0).reshape(len(w), -1).sum(1) <= 1)
+    return [i for i, (w, _) in net.params.items() if not one_hot(w)]
+
+
+@pytest.mark.parametrize("name", sorted(CASES))
+def test_case_sensitivity(name):
+    """a kernel that skips a K-block or misindexes a bias cannot pass by luck: dropping any single (tap, 16-channel group)
+    of a tested layer's weights, or moving one filter's bias by one grid step, changes at least one expected output"""
+    net, x = build_case(name)
+    outs, _ = run_reference(net, x, adt_bf16=not net.quantized)
+    shapes = net.shapes()
+    for i in _tested_layers(net):
+        L = shapes[i]
+        cur = np.ascontiguousarray(x.transpose(0, 2, 3, 1)) if i == 0 else outs[i - 1]
+        if net.kern[i].startswith("stem") and i == 0:
+            cur = bf16_round(cur)
+        w, b = net.params[i]
+        bf16 = not net.quantized and shapes[i + 1]["type"] != "yolo" if i + 1 < len(shapes) else False
+        act = L["activation"]
+        base = epilogue(conv_acc(cur, w, L["stride"], L["pad"]), b, act, net.kern[i], bf16=bf16)
+        C, k = w.shape[1], w.shape[2]
+        for t in range(k * k):
+            for g in range(0, C, 16):
+                w2 = w.copy()
+                w2[:, g:g + 16, t // k, t % k] = 0
+                if not np.any(conv_acc(cur, w - w2, L["stride"], L["pad"])):
+                    continue   # nothing to drop: zero weights, or a tap that only ever reads the zero border
+                e = epilogue(conv_acc(cur, w2, L["stride"], L["pad"]), b, act, net.kern[i], bf16=bf16)
+                assert not np.array_equal(e, base), (name, i, "tap", t, "channels", g)
+        acc = conv_acc(cur, w, L["stride"], L["pad"])
+        for f in range(len(b)):
+            b2 = b.copy()
+            b2[f] += np.float32(1 / 512)
+            e = epilogue(acc[..., f:f + 1], b2[f:f + 1], act, net.kern[i], bf16=bf16)
+            assert not np.array_equal(e, base[..., f:f + 1]), (name, i, "bias", f)
+
+
+# ---- GPU tests ----------------------------------------------------------------------------------------------------------
+KERNEL_OF = {"reg": "k_conv_tc_reg", "tc": "k_conv_tc", "stem": "k_stem_tc", "stem_s2": "k_stem_s2_tc"}
+
+
+def _load(net, workdir, name):
+    import yolo2_light_b200 as yb
+    cfg = cfgs.write_cfg(net.secs, os.path.join(workdir, name + ".cfg"))
+    wts = write_weights(net, os.path.join(workdir, name + ".weights"))
+    m = yb.load_network(cfg, wts, batch=net.batch, quantized=net.quantized)
+    m.set_option("fuse", net.fuse)
+    return m
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name", sorted(CASES))
+def test_tc_exact(name, workdir, monkeypatch):
+    net, x = build_case(name)
+    exp, _ = run_reference(net, x, adt_bf16=not net.quantized)
+    for k, v in net.env.items():
+        monkeypatch.setenv(k, v)
+    m = _load(net, workdir, name)
+    q = bool(net.quantized)
+    # the plan of every convolution is the one the case is for
+    for i, kern in net.kern.items():
+        p = m.tc_plan(i, quantized=q)
+        if kern == "simt":
+            assert p == {}, (name, i, p)
+        else:
+            assert p.get("kernel") == KERNEL_OF[kern], (name, i, p)
+    for i, what, pred in net.edges:
+        p = m.tc_plan(i, quantized=q)
+        assert pred(p), (name, what, p)
+    m.predict(x, quantized=q)
+    shapes = net.shapes()
+    checked = 0
+    for i, L in enumerate(shapes):
+        e = exp.get(i)
+        if L["type"] == "yolo":
+            got = m.detection_outputs()[i]
+            v = exp[i - 1].transpose(0, 3, 1, 2)        # head values, NCHW
+            per = 4 + 80 + 1
+            raw = np.isin(np.arange(v.shape[1]) % per, (2, 3))
+            assert util.bits_equal(got[:, raw], v[:, raw]), name
+            sg = 1.0 / (1.0 + np.exp(-v[:, ~raw].astype(np.float64)))
+            err = np.abs(got[:, ~raw] - sg) / sg
+            assert np.all(err <= logistic_bound(v[:, ~raw])), (name, float(err.max()))
+            checked += 1
+            continue
+        if e is None or (L["type"] == "convolutional" and i + 1 < len(shapes) and shapes[i + 1]["type"] == "yolo"):
+            continue
+        if net.kern.get(0) == "stem_s2" and i == 0:
+            continue   # k_stem_s2_tc never writes the stem output
+        got = m.fetch_layer(i, quantized=q).transpose(0, 2, 3, 1)
+        assert got.shape == e.shape, (name, i)
+        bad = np.argwhere(got.view(np.uint32) != np.ascontiguousarray(e).view(np.uint32))
+        assert len(bad) == 0, (name, i, len(bad), bad[:5].tolist())
+        checked += 1
+    last = len(shapes) - 1
+    if shapes[last]["type"] == "convolutional" and net.params[last][0].shape[2] == 3 and _is_consumer(net, last):
+        # the consumer against shifted copies of its input, computed independently of run_reference
+        pairs = [(int(c), int(ky * 3 + kx)) for _, c, ky, kx in np.argwhere(net.params[last][0] == 1)]   # ordered by filter
+        src = m.fetch_layer(last - 1, quantized=q).transpose(0, 2, 3, 1)
+        got = m.fetch_layer(last, quantized=q).transpose(0, 2, 3, 1)
+        assert util.bits_equal(got, shifted_copies(src, pairs)), name
+    assert checked >= 1, name
+
+
+def _is_consumer(net, i):
+    w, b = net.params[i]
+    return not np.any(b) and np.all((w != 0).reshape(len(w), -1).sum(1) == 1) and np.all(w[w != 0] == 1)
+
+
+# ---- integer kinds at the edge shapes: bit for bit against the oracle on the fetched input ---------------------------
+def _int_net(workdir, name, secs, batch, quantized, seed):
+    import yolo2_light_b200 as yb
+    cfg = cfgs.write_cfg(secs, os.path.join(workdir, name + ".cfg"))
+    wts = cfgs.write_weights(secs, os.path.join(workdir, name + ".weights"), seed=seed)
+    return yb.load_network(cfg, wts, batch=batch, quantized=quantized)
+
+
+def _int_secs(C, h, w, quantized):
+    net = cfgs._net(w, h, [16] * 8 if quantized else None)
+    return [net, cfgs._conv(C, 3)]     # layer 0: f32 (the INT8 rule starts at layer 1), leaky
+
+
+def _int_ref(l, x, quantized):
+    from oracle import port
+    if quantized:
+        return port.conv_int8(x, l["weights_int8"], l["biases"], l["input_quant_multipler"], l["weights_quant_multipler"],
+                              l["n"], l["size"], l["stride"], l["pad"], l["activation"], want_acc=True)
+    return port.conv_xnor(x, l["weights"], l["biases"], l["mean_arr"], l["n"], l["size"], l["activation"], want_counts=True)
+
+
+INT_SHAPES = [   # kind, C, n, h, w, stride, batch: padded channels (C % 32 != 0), n % 4 != 0, odd sizes, stride 2
+    ("s8", 8, 8, 7, 9, 1, 3), ("s8", 24, 30, 9, 5, 1, 2), ("s8", 40, 40, 11, 13, 1, 1), ("s8", 100, 264, 5, 7, 1, 2),
+    ("s8", 24, 30, 10, 14, 2, 3), ("s8", 40, 264, 6, 10, 2, 1), ("s8", 8, 40, 2, 2, 2, 5),
+    ("xnor", 16, 8, 7, 9, 1, 3), ("xnor", 48, 40, 5, 3, 1, 2), ("xnor", 80, 264, 9, 11, 1, 1), ("xnor", 16, 30, 1, 13, 1, 3),
+]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("kind,C,n,h,w,stride,batch", INT_SHAPES)
+def test_integer_kinds_exact(kind, C, n, h, w, stride, batch, workdir):
+    q = kind == "s8"
+    secs = _int_secs(C, h, w, q)
+    secs.append(cfgs._conv(n, 3, stride, **({} if q else {"xnor": 1, "bin_output": 1})))
+    m = _int_net(workdir, f"int_{kind}_{C}_{n}_{h}x{w}s{stride}", secs, batch, int(q), C + n)
+    m.set_option("keep_counts", 1)
+    p = m.tc_plan(1, quantized=q)
+    assert p.get("kind") == kind and p["kernel"] == "k_conv_tc", p
+    assert p["tma_epi"] == 0, p    # keep_counts: the raw accumulators go through the LSU stores
+    m.predict(cfgs.synthetic_images(batch, 3, h, w, seed=C), quantized=q)
+    exp, acc = _int_ref(m.layers[1], m.fetch_layer(0, quantized=q), q)
+    assert np.array_equal(m.fetch_counts(1, quantized=q), acc)
+    assert util.bits_equal(m.fetch_layer(1, quantized=q), exp)
+    # and without the raw-accumulator dump: the TMA epilogue at stride 1, the LSU stores at stride 2
+    m.set_option("keep_counts", 0)
+    p = m.tc_plan(1, quantized=q)
+    assert (p["tma_epi"] == 0) == (stride == 2), p
+    m.predict(cfgs.synthetic_images(batch, 3, h, w, seed=C), quantized=q)
+    assert util.bits_equal(m.fetch_layer(1, quantized=q), exp)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("kind,h,w,batch", [("s8", 2, 2, 3), ("s8", 6, 10, 1), ("xnor", 2, 2, 3), ("xnor", 6, 10, 1)])
+def test_pool_fused_epilogue_exact(kind, h, w, batch, workdir):
+    """the 2x2/2 max-pool and the next layer's input conversion in the integer epilogue (mode 1: s8, mode 2: +-1 bytes) at
+    the smallest and odd-batch shapes it takes"""
+    from oracle import port
+    q = kind == "s8"
+    extra = {} if q else {"xnor": 1, "bin_output": 1}
+    secs = _int_secs(32, h, w, q) + [cfgs._conv(32, 3, **extra), ("maxpool", {"size": "2", "stride": "2"}),
+                                      cfgs._conv(32, 3, **extra)]
+    m = _int_net(workdir, f"pool_{kind}_{h}x{w}", secs, batch, int(q), 7 + h)
+    p = m.tc_plan(1, quantized=q)
+    assert p.get("kind") == kind and p["jshift"] == 1 and p["TW"] == 8, p    # pool fused: 8 x 16 tiles, one row down
+    m.predict(cfgs.synthetic_images(batch, 3, h, w, seed=h), quantized=q)
+    L = m.layers
+    y1, _ = _int_ref(L[1], m.fetch_layer(0, quantized=q), q)
+    y3, _ = _int_ref(L[3], port.maxpool(y1, L[2]["size"], L[2]["stride"], L[2]["pad"]), q)
+    assert util.bits_equal(m.fetch_layer(3, quantized=q), y3)
+
+
+@pytest.mark.gpu
+def test_int8_slice_store_leaves_the_next_slice(workdir):
+    """An INT8 stride-2 layer with n = 30 writes channels 0..29 of a [route] buffer whose channels 30.. belong to layer 1,
+    which ran earlier (on the CUDA cores: its f32 slice is not 16-byte aligned).  The f32 LSU store of the tensor-core
+    epilogue must stop at filter n, not at the next whole float4 group."""
+    from oracle import port
+    secs = _int_secs(16, 6, 10, True) + [cfgs._conv(16, 3),                       # 1: INT8, second slice
+                                          ("upsample", {"stride": "2"}),            # 2
+                                          cfgs._conv(30, 3, 2),                     # 3: INT8 stride 2, first slice
+                                          ("route", {"layers": "-1, -3"}),          # 4: [layer 3, layer 1]
+                                          cfgs._conv(16, 1)]
+    m = _int_net(workdir, "slice_spill", secs, 2, 1, 5)
+    assert m.tc_plan(1, quantized=True) == {}
+    p = m.tc_plan(3, quantized=True)
+    assert p.get("kind") == "s8" and p["tma_epi"] == 0, p
+    m.predict(cfgs.synthetic_images(2, 3, 6, 10, seed=3), quantized=True)
+    L = m.layers
+    y1, _ = _int_ref(L[1], m.fetch_layer(0, quantized=True), True)
+    y3, _ = _int_ref(L[3], port.upsample(y1, 2), True)
+    got = m.fetch_layer(4, quantized=True)
+    assert util.bits_equal(got[:, :30], y3)
+    assert util.bits_equal(got[:, 30:], y1), "layer 3 overwrote layer 1's channels"
+
+
+# ---- production shapes: every distinct convolution of yolov3-608 and yolov3-spp-608 at batch 16, with its fusion ----------
+def production_shapes():
+    """(C, H, W, n, size, stride, fusion) of every distinct convolution of the two networks at 608 x 608.  fusion: "stem_s2"
+    (the stem and layer 1, one kernel), "shortcut" (3x3 + fused residual), "yolo" (head + fused [yolo]), "slice" (writes a
+    channel slice of a [route] buffer) or "none"."""
+    keys = []
+    for secs in (cfgs.yolov3(608, 608), cfgs.yolov3_spp(608, 608)):
+        L = cfgs.conv_shapes(secs)
+        slices = {j for l in L if l["type"] == "route" and len(l["layers"]) > 1 for j in l["layers"]}
+        for i, l in enumerate(L):
+            if l["type"] != "convolutional" or i == 1:
+                continue
+            nxt = L[i + 1]["type"] if i + 1 < len(L) else None
+            fusion = ("stem_s2" if i == 0 else "shortcut" if nxt == "shortcut" and l["stride"] == 1 else
+                      "yolo" if nxt == "yolo" else "slice" if i in slices else "none")
+            k = (l["c"], l["h"], l["w"], l["n"], l["size"], l["stride"], fusion)
+            if k not in keys:
+                keys.append(k)
+    return keys
+
+
+PRODUCTION = production_shapes()
+
+
+def test_torch_reference_equals_numpy_reference():
+    """the GPU-side float64 reference of the production shapes is the same function as conv_acc (run here on the CPU)"""
+    import torch
+    rng = np.random.default_rng(3)
+    for C, n, k, s in ((32, 24, 3, 1), (48, 40, 3, 2), (64, 16, 1, 1)):
+        x = grid_acts(rng, (2, 9, 7, C)).astype(np.float64)
+        w = grid_weights(rng, n, C, k)
+        got = _t_conv_acc(torch.as_tensor(x), w, s, k // 2).numpy()
+        assert np.array_equal(got, conv_acc(x, w, s, k // 2))
+
+
+def test_production_shapes_cover_both_networks():
+    fusions = {k[-1] for k in PRODUCTION}
+    assert fusions == {"stem_s2", "shortcut", "yolo", "slice", "none"}, fusions
+    assert (1024, 19, 19, 512, 1, 1, "none") in PRODUCTION and (2048, 19, 19, 512, 1, 1, "none") in PRODUCTION
+
+
+def production_net(key, batch=16):
+    """the single-layer case of one production shape, with the fusion the network uses there; returns (net, tested layer)"""
+    C, H, W, n, k, s, fusion = key
+    seed = C * 7 + n + H + k + s
+    if fusion == "stem_s2":
+        net = Net(3, H, W, batch, seed)
+        net.conv(32, act=LINEAR, kern="stem_s2", w=(net.rng.integers(-2, 3, (32, 3, 3, 3)) / 64).astype(np.float32),
+                 b=grid_bias(net.rng, 32, 512, 64))
+        i = net.conv(64, 3, 2, kern="stem_s2", w=(net.rng.integers(-2, 3, (64, 32, 3, 3)) / 64).astype(np.float32))
+        net.add("route", layers="-1")
+        return net, i
+    if fusion == "shortcut":
+        # grid-preserving n -> n (the residual), a one-hot n -> C selection, the tested 3x3 C -> n, shortcut from layer 0
+        net = Net(n, H, W, batch, seed)
+        net.preserve()
+        perm = net.rng.permutation(n)[:C]
+        net.conv(C, 1, 1, LINEAR, w=onehot(C, n, 1, [(int(c), 0) for c in perm]), b=grid_acts(net.rng, C, 8, -4, 4))
+        i = net.conv(n, k, s)
+        net.add("shortcut", **{"from": "-3", "activation": LINEAR})
+        net.add("route", layers="-1")
+        return net, i
+    net = Net(C, H, W, batch, seed)
+    if fusion == "yolo":
+        i = net.conv(n, k, s, act=LINEAR, kern="tc")
+        net.secs.append(cfgs._yolo("0,1,2", cfgs.COCO_ANCHORS, 9))
+        return net, i
+    i = net.conv(n, k, s)
+    if fusion == "slice":      # as in the SPP block: max-pools of the layer, concatenated with it
+        net.add("maxpool", size=5, stride=1)
+        net.add("route", layers="-1, -2")
+    else:
+        net.add("route", layers="-1")
+    return net, i
+
+
+def _t_conv_acc(x, w, stride, pad):
+    """conv_acc with torch float64 on the GPU: exact on grid data in any summation order"""
+    import torch
+    B, H, W, C = x.shape
+    n, _, k, _ = w.shape
+    OH, OW = (H + 2 * pad - k) // stride + 1, (W + 2 * pad - k) // stride + 1
+    xp = torch.nn.functional.pad(x, (0, 0, pad, pad, pad, pad))
+    wt = torch.as_tensor(w, dtype=torch.float64, device=x.device)
+    acc = torch.zeros((B, OH, OW, n), dtype=torch.float64, device=x.device)
+    for ky in range(k):
+        for kx in range(k):
+            xs = xp[:, ky:ky + stride * (OH - 1) + 1:stride, kx:kx + stride * (OW - 1) + 1:stride, :]
+            acc += xs @ wt[:, :, ky, kx].T
+    return acc
+
+
+def _t_grid_step(a):
+    import torch
+    for e in range(41):
+        s = a * 2.0 ** e
+        if bool(torch.equal(s, torch.round(s))):
+            return 2.0 ** -e
+    raise AssertionError("data off every binary grid")
+
+
+def _t_layer(x, w, b, L, kern, res=None, act2=LINEAR, bf16=True):
+    """premise and expected output of one convolution over NHWC float64 x on the GPU, as stored (float32)"""
+    import torch
+    nz = w != 0
+    if not (np.all(nz.reshape(len(w), -1).sum(1) <= 1) and np.all(np.abs(w[nz]) == 1)):
+        g = min(_t_grid_step(x) * grid_step(w), grid_step(b))
+        units = float((_t_conv_acc(x.abs(), np.abs(w), L["stride"], L["pad"]).amax() + float(np.abs(b).max())) / g)
+        assert units < BOUND_UNITS, units
+    acc = _t_conv_acc(x, w, L["stride"], L["pad"])
+    bt = torch.as_tensor(b, device=x.device)
+    a = (acc + 0.0).float() + bt
+    f01 = torch.tensor(F32_01, device=x.device)
+    assert kern != "simt"
+    if L["activation"] == LEAKY:
+        a = torch.maximum(a, f01 * a)
+    if res is not None:
+        a = a + res
+        if act2 == LEAKY:
+            a = torch.maximum(a, f01 * a)
+    return a.to(torch.bfloat16).float() if bf16 else a
+
+
+def _t_bits_equal(got_nchw, exp_nhwc):
+    import torch
+    g = torch.as_tensor(np.ascontiguousarray(got_nchw), device=exp_nhwc.device).permute(0, 2, 3, 1)
+    return g.shape == exp_nhwc.shape and bool(torch.equal(g.contiguous().view(torch.int32), exp_nhwc.contiguous().view(torch.int32)))
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("key", PRODUCTION, ids=lambda k: "{}x{}x{}-n{}-k{}s{}-{}".format(*k))
+def test_production_shape_exact(key, workdir):
+    import torch
+    net, i = production_net(key)
+    stem = key[-1] == "stem_s2"
+    x = net.images(16, 0, 16) if stem else net.images()
+    m = _load(net, workdir, "prod_{}x{}x{}_n{}_k{}s{}_{}".format(*key))
+    p = m.tc_plan(i)
+    assert p.get("kernel") == KERNEL_OF[net.kern[i]] and p["kind"] == "bf16", (key, p)
+    if net.kern[i] == "reg":
+        assert p["BN"] >= min(64, key[3]), (key, p)     # the production tiles: 64 to 256 filters (32 at n = 32)
+    if key[-1] == "slice":
+        assert p["out_ldc"] == 2 * key[3], (key, p)
+    for j, kern in net.kern.items():
+        assert m.tc_plan(j).get("kernel") == KERNEL_OF[kern], (key, j)
+    # the expected outputs, each convolution's premise checked, before the network runs
+    dev = torch.device("cuda")
+    cur = torch.as_tensor(x, device=dev).permute(0, 2, 3, 1).double()
+    shapes = net.shapes()
+    outs = {}
+    for j in sorted(net.params):
+        w, b = net.params[j]
+        if stem and j == 0:
+            cur = cur.to(torch.bfloat16).double()
+        res = outs[0] if key[-1] == "shortcut" and j == i else None
+        outs[j] = _t_layer(cur, w, b, shapes[j], net.kern[j], res=res, bf16=key[-1] != "yolo")
+        cur = outs[j].double()
+    del cur
+    m.predict(x)
+    for j, out in outs.items():
+        if key[-1] == "yolo":
+            got = torch.as_tensor(m.detection_outputs()[j + 1], device=dev)
+            v = out.permute(0, 3, 1, 2)
+            raw = torch.as_tensor(np.isin(np.arange(v.shape[1]) % 85, (2, 3)), device=dev)
+            assert torch.equal(got[:, raw].contiguous().view(torch.int32), v[:, raw].contiguous().view(torch.int32)), key
+            vs = v[:, ~raw].double()
+            sg = torch.sigmoid(vs)
+            assert bool(((got[:, ~raw].double() - sg).abs() / sg <= (4.5 + torch.floor((1.173 * vs).abs())) * 2.0 ** -23).all()), key
+        elif key[-1] == "shortcut" and j == i:
+            assert _t_bits_equal(m.fetch_layer(j + 1), out), key      # the fused shortcut's output
+        elif not (stem and j == 0):                                   # k_stem_s2_tc never writes the stem output
+            assert _t_bits_equal(m.fetch_layer(j), out), (key, j)
+    del m
+    torch.cuda.empty_cache()

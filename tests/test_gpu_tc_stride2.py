@@ -16,6 +16,7 @@ from yolo2_light_b200 import cfgs
 pytestmark = pytest.mark.gpu
 
 SHAPES = [((152, 152), 3), ((232, 136), 3)]
+TW = {(152, 152): (16, 1, 2), (232, 136): (4, 2, 4)}   # the tile width of stride-2 layers 1, 3 and 5
 
 
 def s2chain():
@@ -56,6 +57,10 @@ def test_tc_stride2_reg_every_layer_vs_oracle(hw, batch, bn, workdir, monkeypatc
         kinds.setdefault(li, []).append(kind)
     layers = net.layers
     got = [net.fetch_layer(i) for i in range(net.n)]
+    for i, tw in zip((1, 3, 5), TW[hw]):
+        p = net.tc_plan(i)
+        # BN 32 with TW 1 takes TW 2: a one-row store of a straddling half tile must start 128-byte aligned
+        assert p["kernel"] == "k_conv_tc_reg" and p["TW"] == (2 if tw == 1 and p["BN"] == 32 else tw), (hw, bn, i, p)
     for i in range(1, 7):
         assert "conv_tc" in kinds.get(i, []), (i, kinds.get(i))
         l = layers[i]

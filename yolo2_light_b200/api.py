@@ -98,6 +98,7 @@ def lib():
         "yb_network_set_precision": (C.c_int, [vp, C.c_int]),
         "yb_network_set_option": (C.c_int, [vp, C.c_char_p, C.c_int]),
         "yb_network_get_info": (C.c_long, [vp, C.c_int, C.c_char_p]),
+        "yb_network_tc_plan": (C.c_int, [vp, C.c_int, C.c_int, ip, C.c_int]),
         "yb_network_calibrate": (C.c_int, [vp, vp, vp, C.c_int]),
         "yb_entropy_calibration": (C.c_float, [vp, C.c_size_t, C.c_float, C.c_int]),
         "yb_network_input_histogram": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, vp]),
@@ -152,7 +153,7 @@ EXPORTED_SYMBOLS = [
     "yb_fuse_conv_batchnorm", "yb_calculate_binary_weights", "yb_quantinization_and_get_multipliers",
     "yb_network_from_layers", "yb_free_network", "yb_network_num_layers", "yb_network_dims", "yb_network_layer",
     "yb_network_layer_outputs", "yb_network_input_calibration", "yb_set_batch_network", "yb_network_set_device",
-    "yb_network_set_precision", "yb_network_set_option", "yb_network_get_info", "yb_network_detect", "yb_network_calibrate", "yb_entropy_calibration",
+    "yb_network_set_precision", "yb_network_set_option", "yb_network_get_info", "yb_network_tc_plan", "yb_network_detect", "yb_network_calibrate", "yb_entropy_calibration",
     "yb_network_input_histogram", "yb_map_evaluate", "yb_network_predict", "yb_network_predict_quantized",
     "yb_network_predict_image_u8", "yb_network_fetch_input", "yb_network_submit", "yb_network_collect", "yb_network_layer_output", "yb_network_forward_device", "yb_network_sync_outputs", "yb_network_fetch_layer",
     "yb_network_fetch_counts", "yb_forward_convolutional_layer", "yb_network_weight_arena",
@@ -162,6 +163,12 @@ EXPORTED_SYMBOLS = [
     "yb_network_detect_frames", "yb_network_submit_frames_u8", "yb_network_predict_device_frames",
     "yb_network_submit_device_frames",
 ]
+
+
+TC_PLAN_FIELDS = ("kernel", "kind", "TW", "TH", "BN", "BK", "nt", "bstat", "stages", "sps", "grid", "num_work", "tma_epi",
+                  "jshift", "out_ldc")
+TC_PLAN_KERNELS = ("k_conv_tc", "k_conv_tc_reg", "k_stem_tc", "k_stem_s2_tc")
+TC_PLAN_KINDS = ("bf16", "s8", "xnor", "tf32")
 
 
 def _check(ok: bool):
@@ -250,6 +257,19 @@ class Network:
 
     def get_info(self, key: str, quantized: bool = False) -> int:
         return int(lib().yb_network_get_info(self._h, int(quantized), key.encode()))
+
+    def tc_plan(self, i: int, quantized: bool = False) -> dict:
+        """The tensor-core plan of layer i (see yb_network_tc_plan): kernel and kind by name, the tile parameters as ints
+        (-1: does not apply to that kernel); {} for a layer without one."""
+        f = (C.c_int * len(TC_PLAN_FIELDS))()
+        r = lib().yb_network_tc_plan(self._h, int(quantized), i, f, len(f))
+        _check(r >= 0)
+        if r == 0:
+            return {}
+        d = dict(zip(TC_PLAN_FIELDS, list(f)[:r]))
+        d["kernel"] = TC_PLAN_KERNELS[d["kernel"]]
+        d["kind"] = TC_PLAN_KINDS[d["kind"]]
+        return d
 
     # -- forward -------------------------------------------------------------------------------------
     def _out_shape(self, i: int):

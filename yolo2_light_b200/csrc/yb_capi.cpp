@@ -235,6 +235,12 @@ long yb_network_get_info(yb_network *n, int quantized, const char *key) {
     YB_CATCH(-1)
 }
 
+int yb_network_tc_plan(yb_network *n, int quantized, int layer, int *fields, int count) {
+    YB_TRY
+    return engine_tc_plan(get_engine(n, quantized), layer, fields, count);
+    YB_CATCH(-1)
+}
+
 static float *predict_common(yb_network *n, const float *input, int quantized) {
     Engine *e = get_engine(n, quantized);
     engine_upload_input(e, input, nullptr);

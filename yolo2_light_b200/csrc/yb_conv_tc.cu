@@ -92,7 +92,7 @@ struct TcParams {
     signed char *pool_out; long pool_ldc; int pool_Hp, pool_Wp;   // next layer's s8 input: padded NHWC, bytes
     int sps;                                  // K-blocks per pipeline stage (amortises the per-stage barrier round trip)
     uint32_t desc_hi;         // high word of the wgmma shared-memory descriptors (SBO, swizzle mode)
-    char *out; long out_ldc; int n, n_store;
+    char *out; long out_ldc; int n;
     const char *res;          // fused shortcut operand (bf16, k_conv_tc_reg at stride 1 only), or null
     const float *bias; int act, act2;
     unsigned long long *stats; // YB_TC_STATS=1: per-CTA cycle counters [grid][16] (diagnostic)
@@ -566,7 +566,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
 
             // ---- f32 output (detection heads) of one 32-column slab, one row per thread
             auto finish_f32 = [&](const uint32_t (&v)[32], int f0) {
-                if (!valid || (n0 + f0) >= p.n_store) return;
+                if (!valid || (n0 + f0) >= p.n) return;
                 float x[32];
 #pragma unroll
                 for (int j = 0; j < 32; ++j) {
@@ -592,8 +592,10 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                     float4 *op = reinterpret_cast<float4 *>(orow + (size_t)(n0 + f0) * 4);
 #pragma unroll
                     for (int g = 0; g < 8; ++g) {
-                        if (n0 + f0 + g * 4 >= p.n_store) break;
-                        op[g] = make_float4(x[g * 4 + 0], x[g * 4 + 1], x[g * 4 + 2], x[g * 4 + 3]);
+                        const int left = p.n - (n0 + f0 + g * 4);   // the output may be a channel slice: nothing past filter n
+                        if (left <= 0) break;
+                        if (left >= 4) op[g] = make_float4(x[g * 4 + 0], x[g * 4 + 1], x[g * 4 + 2], x[g * 4 + 3]);
+                        else for (int e = 0; e < left; ++e) reinterpret_cast<float *>(op + g)[e] = x[g * 4 + e];
                     }
                 }
             };
@@ -621,8 +623,15 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                     uint32_t w0, w1, w2, w3;
                     asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(w0), "=r"(w1), "=r"(w2), "=r"(w3)
                                  : "r"(stg + (uint32_t)row * 128u + (uint32_t)((schunk ^ (row & 7)) << 4)) : "memory");
-                    if (ok && (n0 + f0 + schunk * 4) < p.n_store)
-                        *(reinterpret_cast<uint4 *>(op + (size_t)(n0 + f0) * 4) + schunk) = make_uint4(w0, w1, w2, w3);
+                    const int left = p.n - (n0 + f0 + schunk * 4);   // the output may be a channel slice: nothing past filter n
+                    uint4 *dst = reinterpret_cast<uint4 *>(op + (size_t)(n0 + f0) * 4) + schunk;
+                    if (ok && left >= 4) *dst = make_uint4(w0, w1, w2, w3);
+                    else if (ok && left > 0) {
+                        uint32_t *d1 = reinterpret_cast<uint32_t *>(dst);
+                        d1[0] = w0;
+                        if (left > 1) d1[1] = w1;
+                        if (left > 2) d1[2] = w2;
+                    }
                 }
                 __syncwarp();
             };
@@ -1592,8 +1601,6 @@ void plan_epilogue(TcParams &p, const TcConv &c, bool reg) {
     p.acc_pitch = p.BN + 4;
     p.out = c.out.base; p.out_ldc = c.out.ldc;
     p.n = l.n;
-    // f32: whole float4 groups, within the output's pixel stride (a fused [yolo] head has no NHWC output)
-    p.n_store = c.out_bf16 ? l.n : c.out.base ? std::min<int>((l.n + 3) / 4 * 4, c.out.ldc) : (l.n + 3) / 4 * 4;
     p.res = c.res.base;
     p.bias = c.bias; p.act = l.activation; p.act2 = c.act2;
     p.alpha1 = c.alpha1;
@@ -1808,6 +1815,30 @@ void tc_stem_launch_u8(void *vp, const unsigned char *d_in_hwc, cudaStream_t s) 
     else k_stem_tc<true><<<sp->grid, 128, 0, s>>>(p);
 }
 void tc_stem_free_plan(void *vp) { delete reinterpret_cast<StemPlan *>(vp); }
+
+namespace {
+int copy_fields(const int (&f)[TC_PLAN_NFIELDS], int *fields, int n) {
+    const int k = std::max(0, std::min(n, (int)TC_PLAN_NFIELDS));
+    for (int i = 0; i < k; ++i) fields[i] = f[i];
+    return k;
+}
+}  // namespace
+
+int tc_plan_fields(const void *vp, int *fields, int n) {
+    const TcPlan &plan = *reinterpret_cast<const TcPlan *>(vp);
+    const TcParams &p = plan.p;
+    const int f[TC_PLAN_NFIELDS] = {plan.threads == TCR_THREADS ? TC_PLAN_CONV_REG : TC_PLAN_CONV, p.kind, p.TW, p.TH, p.BN, p.BK,
+                                    p.nt, p.bstat, p.stages, p.sps, plan.grid, p.num_work, p.tma_epi, p.jshift,
+                                    p.out ? (int)p.out_ldc : 0};
+    return copy_fields(f, fields, n);
+}
+
+int tc_stem_plan_fields(const void *vp, int *fields, int n) {
+    const StemPlan &sp = *reinterpret_cast<const StemPlan *>(vp);
+    const int f[TC_PLAN_NFIELDS] = {sp.s2 ? TC_PLAN_STEM_S2 : TC_PLAN_STEM, TC_BF16, sp.s2 ? S2_TW : -1, sp.s2 ? S2_TH : -1,
+                                    sp.s2 ? 64 : -1, -1, -1, -1, -1, -1, sp.grid, sp.p.ntiles, -1, -1, (int)sp.p.out_ldc};
+    return copy_fields(f, fields, n);
+}
 
 void tc_launch(void *vp, cudaStream_t s) {
     TcPlan *plan = reinterpret_cast<TcPlan *>(vp);

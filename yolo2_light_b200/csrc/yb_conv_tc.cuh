@@ -58,4 +58,12 @@ void tc_stem_launch(void *plan, const float *d_in_nchw, cudaStream_t s);
 void tc_stem_launch_u8(void *plan, const unsigned char *d_in_hwc, cudaStream_t s);   // frames already of the network size
 void tc_stem_free_plan(void *plan);
 
+// What a plan decided, for tests (read-only): up to n of {kernel (TC_PLAN_*), kind (TcKind), TW, TH, BN, BK, nt, bstat,
+// stages, sps, grid, num_work, tma_epi, jshift, out_ldc (the output's pixel stride in elements, 0 without an NHWC output)}
+// into fields; returns how many were written.  The stem plans report kernel, kind, grid, num_work (tiles) and out_ldc, and
+// k_stem_s2_tc its S2_TW x S2_TH tiles of layer-1 pixels and its 64 filters as TW, TH, BN; every other field is -1.
+enum { TC_PLAN_CONV = 0, TC_PLAN_CONV_REG = 1, TC_PLAN_STEM = 2, TC_PLAN_STEM_S2 = 3, TC_PLAN_NFIELDS = 15 };
+int tc_plan_fields(const void *plan, int *fields, int n);
+int tc_stem_plan_fields(const void *plan, int *fields, int n);
+
 }  // namespace yb

@@ -92,6 +92,7 @@ struct Engine {
     cudaGraphExec_t graph_exec = nullptr;
     bool graph_failed = false;
     std::vector<void *> tc_plans;      // opaque per-layer state of the tensor-core path (tensor maps)
+    std::vector<int> tc_plan_layer;    // the layer of each of tc_plans
     // device-side decode + NMS workspace (engine_detect), sized for det_cap rows per image
     int n_tc = 0;
     std::function<void(const float *, cudaStream_t)> first_op;   // consumes the caller's NCHW images (pointer varies per call)
@@ -720,6 +721,7 @@ struct Builder {
     void push_tc_plan(int kind, int i) {
         void *plan = tc_make_plan(tc_conv(i, true, L[i].pool_mode));
         e.tc_plans.push_back(plan);
+        e.tc_plan_layer.push_back(i);
         if (kind == OP_CONV_TC || kind == OP_CONV_TC_TF32) ++e.n_tc;
         push(kind, i, [plan](cudaStream_t s) { tc_launch(plan, s); });
     }
@@ -1741,6 +1743,14 @@ long engine_info(Engine *e, const char *key) {
     if (!strcmp(key, "tc_layers")) return e->n_tc;
     if (!strcmp(key, "act_bytes")) return (long)e->act_bytes;
     return -1;
+}
+
+int engine_tc_plan(Engine *e, int layer, int *fields, int n) {
+    for (size_t k = 0; k < e->tc_plans.size(); ++k)
+        if (e->tc_plan_layer[k] == layer) return tc_plan_fields(e->tc_plans[k], fields, n);
+    // the stem plan runs layer 0, and layer 1 too when k_stem_s2_tc fuses it
+    if (e->stem_plan && (layer == 0 || layer == e->first_layer)) return tc_stem_plan_fields(e->stem_plan, fields, n);
+    return 0;
 }
 
 int engine_profile(Engine *e, const void *d_input, int *layer_idx, int *op_kind, float *ms, int max) {

@@ -65,6 +65,8 @@ constexpr int DET_MAX_ROWS = 16384;
 void engine_input_histogram(Engine *e, Network *net, int layer, int img, float bin_width, int max_bin, uint32_t *hist);
 int engine_num_launches(Engine *e);
 long engine_info(Engine *e, const char *key);   // "launches", "tc_layers", "act_bytes"; -1 unknown
+// the tensor-core plan of a layer (tc_plan_fields / tc_stem_plan_fields); 0 fields for a layer without one
+int engine_tc_plan(Engine *e, int layer, int *fields, int n);
 int engine_profile(Engine *e, const void *d_input, int *layer_idx, int *op_kind, float *ms, int max);
 void *engine_stream(Engine *e);
 const char *op_kind_name(int k);
