@@ -33,21 +33,24 @@ static void report(const std::string &msg) {
     catch (const yb::Error &e) { report(e.msg); return; }                      \
     catch (const std::exception &e) { report(e.what()); return; }
 
+// The options of an engine of `net` on `device`; upload == false leaves its weight arena to a broadcast.
+static EngineOptions engine_options(const Network &net, int quantized, int device, bool upload) {
+    EngineOptions opt;
+    opt.device = device;
+    opt.precision = net.precision;
+    opt.qrule = quantized != 0;
+    opt.upload = upload;
+    const char *nf = getenv("YB_NO_FUSE");
+    opt.fuse = !(nf && nf[0] == '1') && net.fuse;
+    opt.keep_counts = net.keep_counts;
+    opt.q_index_offset = net.q_index_offset;
+    return opt;
+}
+
 static Engine *get_engine(yb_network *n, int quantized, bool upload = true) {
     Network &net = n->net;
     const int slot = quantized ? 1 : 0;
-    if (!net.engine[slot]) {
-        EngineOptions opt;
-        opt.device = net.device;
-        opt.precision = net.precision;
-        opt.qrule = quantized != 0;
-        opt.upload = upload;
-        const char *nf = getenv("YB_NO_FUSE");
-        opt.fuse = !(nf && nf[0] == '1') && net.fuse;
-        opt.keep_counts = net.keep_counts;
-        opt.q_index_offset = net.q_index_offset;
-        net.engine[slot] = build_engine(&net, opt);
-    }
+    if (!net.engine[slot]) net.engine[slot] = build_engine(&net, engine_options(net, quantized, net.device, upload));
     return net.engine[slot].get();
 }
 
@@ -518,13 +521,8 @@ static std::vector<Engine *> get_replicas(yb_network *n, int quantized, int ngpu
     std::vector<std::shared_ptr<Engine>> &reps = n->replicas[slot];
     bool built = false;
     while ((int)reps.size() < ngpus - 1) {
-        EngineOptions opt;
-        opt.device = n->devices[reps.size() + 1];
-        opt.precision = n->net.precision; opt.qrule = quantized != 0; opt.upload = false;   // weights arrive by the broadcast
-        const char *nf = getenv("YB_NO_FUSE");
-        opt.fuse = !(nf && nf[0] == '1') && n->net.fuse;
-        opt.keep_counts = n->net.keep_counts; opt.q_index_offset = n->net.q_index_offset;
-        reps.push_back(build_engine(&n->net, opt));
+        const int device = n->devices[reps.size() + 1];
+        reps.push_back(build_engine(&n->net, engine_options(n->net, quantized, device, false)));   // weights arrive by the broadcast
         built = true;
     }
     std::vector<Engine *> all{e0};

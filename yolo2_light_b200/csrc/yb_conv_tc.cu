@@ -38,6 +38,7 @@
 #include <vector>
 
 #include "yb_conv_tc.cuh"
+#include "yb_cuda.h"
 
 namespace yb {
 
@@ -1464,6 +1465,8 @@ EncodeTiledFn encode_fn() {
     return fn;
 }
 
+}  // namespace
+
 struct TcPlan {
     CUtensorMap tmA, tmB, tmO, tmO1, tmR;   // activation, filters; TMA epilogue: output, its one-row view (stride 2), residual
     TcParams p;
@@ -1471,7 +1474,10 @@ struct TcPlan {
     int threads;                      // TC_THREADS (k_conv_tc) or TCR_THREADS (k_conv_tc_reg)
     size_t smem;
     char desc[96];
+    DevBuf<unsigned long long> stats;   // p.stats (YB_TC_STATS)
 };
+
+namespace {
 
 int sm_count() {
     int dev = 0, sms = 132;
@@ -1719,10 +1725,10 @@ int tc_conv_supported(const TcConv &c) {
     return 1;
 }
 
-void *tc_make_plan(const TcConv &c) {
+TcPlanPtr tc_make_plan(const TcConv &c) {
     const Layer &l = *c.l;
     if (!tc_conv_supported(c)) fatal_throw("tc plan: convolution not supported by the tensor-core kernels");
-    std::unique_ptr<TcPlan> plan(new TcPlan());
+    TcPlanPtr plan(new TcPlan());
     TcParams &p = plan->p;
     const bool reg = c.kind == TC_BF16 && c.out_bf16;   // bf16 NHWC output: the register-accumulator kernel with its TMA epilogue
     const int sms = sm_count();
@@ -1746,10 +1752,11 @@ void *tc_make_plan(const TcConv &c) {
         if (cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
             fatal_throw("cudaFuncSetAttribute(k_conv_tc) failed");
     if (getenv("YB_TC_STATS")) {
-        cudaMalloc(&p.stats, sizeof(unsigned long long) * 16 * plan->grid);
+        plan->stats.ensure(16 * (size_t)plan->grid);
+        p.stats = plan->stats.get();
         cudaMemset(p.stats, 0, sizeof(unsigned long long) * 16 * plan->grid);
     }
-    return plan.release();
+    return plan;
 }
 
 struct StemPlan { StemTcP p; int grid; bool s2; };   // s2: k_stem_s2_tc (stem + layer 1)
@@ -1759,9 +1766,8 @@ int tc_stem_supported(const Layer &l, const TV &out) {
            (reinterpret_cast<uintptr_t>(out.base) & 15) == 0;
 }
 // d_w: device buffer of 32*32 bf16 ([filter][k], k = (ky,kx,c), zero padded), d_bias: device f32[>= n]
-void *tc_stem_make_plan(const Layer &l, const TV &out, const void *d_w, const float *d_bias) {
-    StemPlan *sp = new StemPlan();
-    memset(sp, 0, sizeof(*sp));
+StemPlanPtr tc_stem_make_plan(const Layer &l, const TV &out, const void *d_w, const float *d_bias) {
+    StemPlanPtr sp(new StemPlan());
     StemTcP &p = sp->p;
     p.out = out.base; p.out_ldc = out.ldc; p.w = reinterpret_cast<const __nv_bfloat16 *>(d_w); p.bias = d_bias;
     p.N = out.N; p.H = l.h; p.W = l.w; p.OHp = out.Hp; p.OWp = out.Wp; p.nf = l.n; p.act = l.activation;
@@ -1777,10 +1783,9 @@ int tc_stem_s2_supported(const Layer &l0, const Layer &l1, const TV &out1) {
            out1.H == l0.h / 2 && out1.W == l0.w / 2 && out1.ldc % 8 == 0 && (reinterpret_cast<uintptr_t>(out1.base) & 15) == 0;
 }
 // d_w1: layer 1's bf16 [64][9 * 32] filter matrix (K ordered (ky, kx, c)), d_bias1: its f32 bias
-void *tc_stem_s2_make_plan(const Layer &l0, const Layer &l1, const TV &out1, const void *d_w, const float *d_bias, const void *d_w1,
-                           const float *d_bias1) {
-    StemPlan *sp = new StemPlan();
-    memset(sp, 0, sizeof(*sp));
+StemPlanPtr tc_stem_s2_make_plan(const Layer &l0, const Layer &l1, const TV &out1, const void *d_w, const float *d_bias,
+                                 const void *d_w1, const float *d_bias1) {
+    StemPlanPtr sp(new StemPlan());
     sp->s2 = true;
     StemTcP &p = sp->p;
     p.out = out1.base; p.out_ldc = out1.ldc; p.w = reinterpret_cast<const __nv_bfloat16 *>(d_w); p.bias = d_bias;
@@ -1799,22 +1804,19 @@ void *tc_stem_s2_make_plan(const Layer &l0, const Layer &l1, const TV &out1, con
     }
     return sp;
 }
-void tc_stem_launch(void *vp, const float *d_in_nchw, cudaStream_t s) {
-    StemPlan *sp = reinterpret_cast<StemPlan *>(vp);
-    StemTcP p = sp->p;
+void tc_stem_launch(const StemPlan &sp, const float *d_in_nchw, cudaStream_t s) {
+    StemTcP p = sp.p;
     p.in = d_in_nchw;
-    if (sp->s2) k_stem_s2_tc<false><<<sp->grid, 256, S2_SMEM, s>>>(p);
-    else k_stem_tc<false><<<sp->grid, 128, 0, s>>>(p);
+    if (sp.s2) k_stem_s2_tc<false><<<sp.grid, 256, S2_SMEM, s>>>(p);
+    else k_stem_tc<false><<<sp.grid, 128, 0, s>>>(p);
 }
 // 8-bit HWC frames of exactly the network size (3 channels): no planar-float staging
-void tc_stem_launch_u8(void *vp, const unsigned char *d_in_hwc, cudaStream_t s) {
-    StemPlan *sp = reinterpret_cast<StemPlan *>(vp);
-    StemTcP p = sp->p;
+void tc_stem_launch_u8(const StemPlan &sp, const unsigned char *d_in_hwc, cudaStream_t s) {
+    StemTcP p = sp.p;
     p.in8 = d_in_hwc;
-    if (sp->s2) k_stem_s2_tc<true><<<sp->grid, 256, S2_SMEM, s>>>(p);
-    else k_stem_tc<true><<<sp->grid, 128, 0, s>>>(p);
+    if (sp.s2) k_stem_s2_tc<true><<<sp.grid, 256, S2_SMEM, s>>>(p);
+    else k_stem_tc<true><<<sp.grid, 128, 0, s>>>(p);
 }
-void tc_stem_free_plan(void *vp) { delete reinterpret_cast<StemPlan *>(vp); }
 
 namespace {
 int copy_fields(const int (&f)[TC_PLAN_NFIELDS], int *fields, int n) {
@@ -1824,8 +1826,7 @@ int copy_fields(const int (&f)[TC_PLAN_NFIELDS], int *fields, int n) {
 }
 }  // namespace
 
-int tc_plan_fields(const void *vp, int *fields, int n) {
-    const TcPlan &plan = *reinterpret_cast<const TcPlan *>(vp);
+int tc_plan_fields(const TcPlan &plan, int *fields, int n) {
     const TcParams &p = plan.p;
     const int f[TC_PLAN_NFIELDS] = {plan.threads == TCR_THREADS ? TC_PLAN_CONV_REG : TC_PLAN_CONV, p.kind, p.TW, p.TH, p.BN, p.BK,
                                     p.nt, p.bstat, p.stages, p.sps, plan.grid, p.num_work, p.tma_epi, p.jshift,
@@ -1833,26 +1834,23 @@ int tc_plan_fields(const void *vp, int *fields, int n) {
     return copy_fields(f, fields, n);
 }
 
-int tc_stem_plan_fields(const void *vp, int *fields, int n) {
-    const StemPlan &sp = *reinterpret_cast<const StemPlan *>(vp);
+int tc_stem_plan_fields(const StemPlan &sp, int *fields, int n) {
     const int f[TC_PLAN_NFIELDS] = {sp.s2 ? TC_PLAN_STEM_S2 : TC_PLAN_STEM, TC_BF16, sp.s2 ? S2_TW : -1, sp.s2 ? S2_TH : -1,
                                     sp.s2 ? 64 : -1, -1, -1, -1, -1, -1, sp.grid, sp.p.ntiles, -1, -1, (int)sp.p.out_ldc};
     return copy_fields(f, fields, n);
 }
 
-void tc_launch(void *vp, cudaStream_t s) {
-    TcPlan *plan = reinterpret_cast<TcPlan *>(vp);
+void tc_launch(const TcPlan &P, cudaStream_t s) {
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)plan->grid); cfg.blockDim = dim3((unsigned)plan->threads);
-    cfg.dynamicSmemBytes = plan->smem; cfg.stream = s;
+    cfg.gridDim = dim3((unsigned)P.grid); cfg.blockDim = dim3((unsigned)P.threads);
+    cfg.dynamicSmemBytes = P.smem; cfg.stream = s;
     cudaLaunchAttribute attr[1];   // programmatic dependent launch: this kernel's prologue runs while the previous kernel drains
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
-    const bool st = plan->p.stats != nullptr;   // role counters: a separate instantiation (YB_TC_STATS=1)
-    const TcPlan &P = *plan;
+    const bool st = P.p.stats != nullptr;   // role counters: a separate instantiation (YB_TC_STATS=1)
 #define YB_TC_LAUNCH(KERNEL) cudaLaunchKernelEx(&cfg, KERNEL, P.tmA, P.tmB, P.tmO, P.p)
-    if (plan->threads == TCR_THREADS) {
+    if (P.threads == TCR_THREADS) {
         if (st) cudaLaunchKernelEx(&cfg, k_conv_tc_reg<true>, P.tmA, P.tmB, P.tmO, P.tmO1, P.tmR, P.p);
         else cudaLaunchKernelEx(&cfg, k_conv_tc_reg<false>, P.tmA, P.tmB, P.tmO, P.tmO1, P.tmR, P.p);
     }
@@ -1861,9 +1859,8 @@ void tc_launch(void *vp, cudaStream_t s) {
 #undef YB_TC_LAUNCH
 }
 
-void tc_free_plan(void *vp) {
-    TcPlan *plan = reinterpret_cast<TcPlan *>(vp);
-    if (plan && plan->p.stats) {   // diagnostic dump: mean cycles per CTA of the LAST launch
+void TcPlanDelete::operator()(TcPlan *plan) const {
+    if (plan->p.stats) {   // diagnostic dump: mean cycles per CTA of the LAST launch
         std::vector<unsigned long long> h(16 * (size_t)plan->grid);
         cudaDeviceSynchronize();
         cudaMemcpy(h.data(), plan->p.stats, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
@@ -1875,9 +1872,9 @@ void tc_free_plan(void *vp) {
             fprintf(stderr, "consumers: wait_full %.0f wait_ready %.0f (first item %.0f) total %.0f | store: wait_full %.0f wait_read %.0f\n",
                     m[2], m[8], m[3], m[6], m[4], m[5]);
         else fprintf(stderr, "consumers: wait_full %.0f total %.0f\n", m[2], m[6]);
-        cudaFree(plan->p.stats);
     }
     delete plan;
 }
+void TcPlanDelete::operator()(StemPlan *plan) const { delete plan; }
 
 }  // namespace yb

@@ -3,6 +3,8 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <memory>
+
 #include "yb_kernels.cuh"
 #include "yb_model.h"
 
@@ -39,31 +41,39 @@ struct TcConv {
     TV pool_next{};                // the next integer layer's s8 input
 };
 
+// The launch state of a tensor-core convolution (TMA tensor maps, tile schedule) and of a tensor-core stem
+struct TcPlan;
+struct StemPlan;
+struct TcPlanDelete {
+    void operator()(TcPlan *plan) const;     // with YB_TC_STATS set, prints the plan's cycle counters first
+    void operator()(StemPlan *plan) const;
+};
+using TcPlanPtr = std::unique_ptr<TcPlan, TcPlanDelete>;
+using StemPlanPtr = std::unique_ptr<StemPlan, TcPlanDelete>;
+
 // non-zero if the tensor-core kernels take this convolution, fusions included
 int tc_conv_supported(const TcConv &c);
-// builds the launch state (TMA tensor maps, tile schedule) of a supported convolution; throws yb::Error on failure
-void *tc_make_plan(const TcConv &c);
-void tc_launch(void *plan, cudaStream_t s);
-void tc_free_plan(void *plan);
+// builds the plan of a supported convolution; throws yb::Error on failure
+TcPlanPtr tc_make_plan(const TcConv &c);
+void tc_launch(const TcPlan &plan, cudaStream_t s);
 
 // tensor-core stem (3-channel 3x3 from the caller's NCHW f32 image, bf16 NHWC out)
 int tc_stem_supported(const Layer &l, const TV &out);
-void *tc_stem_make_plan(const Layer &l, const TV &out, const void *d_w_32x32_bf16, const float *d_bias);
+StemPlanPtr tc_stem_make_plan(const Layer &l, const TV &out, const void *d_w_32x32_bf16, const float *d_bias);
 // the tensor-core stem fused with layer 1, a 3x3 / stride-2 convolution 32 -> 64 filters (bf16 out1): the stem output never
-// reaches HBM.  The plan takes the same launch / free calls as the stem's.
+// reaches HBM.  The plan takes the same launch calls as the stem's.
 int tc_stem_s2_supported(const Layer &l0, const Layer &l1, const TV &out1);
-void *tc_stem_s2_make_plan(const Layer &l0, const Layer &l1, const TV &out1, const void *d_w_32x32_bf16, const float *d_bias,
-                           const void *d_w1_bf16, const float *d_bias1);
-void tc_stem_launch(void *plan, const float *d_in_nchw, cudaStream_t s);
-void tc_stem_launch_u8(void *plan, const unsigned char *d_in_hwc, cudaStream_t s);   // frames already of the network size
-void tc_stem_free_plan(void *plan);
+StemPlanPtr tc_stem_s2_make_plan(const Layer &l0, const Layer &l1, const TV &out1, const void *d_w_32x32_bf16,
+                                 const float *d_bias, const void *d_w1_bf16, const float *d_bias1);
+void tc_stem_launch(const StemPlan &plan, const float *d_in_nchw, cudaStream_t s);
+void tc_stem_launch_u8(const StemPlan &plan, const unsigned char *d_in_hwc, cudaStream_t s);   // frames already of the network size
 
 // What a plan decided, for tests (read-only): up to n of {kernel (TC_PLAN_*), kind (TcKind), TW, TH, BN, BK, nt, bstat,
 // stages, sps, grid, num_work, tma_epi, jshift, out_ldc (the output's pixel stride in elements, 0 without an NHWC output)}
 // into fields; returns how many were written.  The stem plans report kernel, kind, grid, num_work (tiles) and out_ldc, and
 // k_stem_s2_tc its S2_TW x S2_TH tiles of layer-1 pixels and its 64 filters as TW, TH, BN; every other field is -1.
 enum { TC_PLAN_CONV = 0, TC_PLAN_CONV_REG = 1, TC_PLAN_STEM = 2, TC_PLAN_STEM_S2 = 3, TC_PLAN_NFIELDS = 15 };
-int tc_plan_fields(const void *plan, int *fields, int n);
-int tc_stem_plan_fields(const void *plan, int *fields, int n);
+int tc_plan_fields(const TcPlan &plan, int *fields, int n);
+int tc_stem_plan_fields(const StemPlan &plan, int *fields, int n);
 
 }  // namespace yb

@@ -16,18 +16,11 @@
 #include <cstring>
 
 #include "yb_conv_tc.cuh"
+#include "yb_cuda.h"
 #include "yb_kernels.cuh"
 #include "yb_detect.cuh"
 
 namespace yb {
-
-#define CUDA_OK(call)                                                                                   \
-    do {                                                                                                \
-        cudaError_t _e = (call);                                                                        \
-        if (_e != cudaSuccess)                                                                          \
-            fatal_throw(std::string("CUDA error: ") + cudaGetErrorString(_e) + " at " + __FILE__ + ":" + \
-                        std::to_string(__LINE__) + " (" #call ")");                                     \
-    } while (0)
 
 const char *op_kind_name(int k) {
     static const char *names[] = {"input", "conv_simt", "conv_tc", "binarize", "conv_xnor", "quantize",
@@ -75,107 +68,62 @@ struct Engine {
     Switches sw{};
     int batch = 0;
     int act_dt = DT_F32;
-    cudaStream_t stream = nullptr;
-    char *act_arena = nullptr; size_t act_bytes = 0;
-    char *w_arena = nullptr;   size_t w_bytes = 0;
-    float *d_input = nullptr;  size_t input_count = 0;
+    Stream stream;
+    DevBuf<char> act_arena, w_arena;
+    DevBuf<float> d_input;             // staging of the caller's images
     std::vector<TV> out_tv;            // per layer (base == nullptr: no NHWC output, or one that exists only in a fused form)
     std::vector<int> out_dt;
-    std::vector<float *> d_final;      // yolo / region device outputs
-    std::vector<float *> h_final;      // pinned host mirrors
-    std::vector<size_t> final_count;
-    std::vector<int32_t *> d_counts;   // optional raw integer results per conv layer
-    std::vector<size_t> counts_count;
+    struct Final { DevBuf<float> d; PinnedBuf<float> h; };   // a layer's f32 NCHW output and its pinned host mirror
+    std::vector<Final> finals;         // per layer: the yolo / region outputs and the last layer's (empty for the others)
+    std::vector<DevBuf<int32_t>> counts;   // per layer: optional raw integer results of a convolution
     std::vector<Op> ops;
     TV in0{};                          // NHWC copy of the caller's images (base == nullptr: the stem reads them directly)
     int in0_dt = DT_F32;
-    cudaGraphExec_t graph_exec = nullptr;
+    GraphExec graph_exec;
     bool graph_failed = false;
-    std::vector<void *> tc_plans;      // opaque per-layer state of the tensor-core path (tensor maps)
-    std::vector<int> tc_plan_layer;    // the layer of each of tc_plans
-    // device-side decode + NMS workspace (engine_detect), sized for det_cap rows per image
+    std::vector<std::pair<int, TcPlanPtr>> tc_plans;   // (layer, its tensor-core plan)
     int n_tc = 0;
     std::function<void(const float *, cudaStream_t)> first_op;   // consumes the caller's NCHW images (pointer varies per call)
     std::function<void(const unsigned char *, cudaStream_t)> first_op_u8;   // same from 8-bit HWC frames of the network size (if set)
     int first_kind = OP_INPUT, first_layer = -1;
-    void *stem_plan = nullptr;
+    StemPlanPtr stem_plan;
     struct FrameStage {                 // the caller's 8-bit frames of one batch on the device, packed back to back
-        unsigned char *buf = nullptr; size_t bytes = 0;
-        ImageGeo *d_geo = nullptr, *h_geo = nullptr;   // per-image table (batch entries) and its pinned host twin
+        DevBuf<unsigned char> buf;
+        DevBuf<ImageGeo> d_geo; PinnedBuf<ImageGeo> h_geo;   // per-image table (batch entries) and its pinned host twin
     };
     FrameStage u8;                      // device-side input pipeline + decode geometry of the synchronous calls
-    float *d_unit = nullptr;            // byte value -> float /255. (k_resize_frames)
+    DevBuf<float> d_unit;               // byte value -> float /255. (k_resize_frames)
     // hand-off of the caller's device frames: produced on the caller's stream (ev_frames_ready) / read (ev_frames_read)
-    cudaEvent_t ev_frames_ready = nullptr, ev_frames_read = nullptr;
+    Event ev_frames_ready, ev_frames_read;
     // ---- pipelined end-to-end path: H2D(k+1) | compute(k) | D2H(k-1) on three streams -----------------
-    struct DetWs {                      // decode + NMS workspace for `cap` candidate rows per image
-        float *rows = nullptr; unsigned *mask = nullptr; int *blkcnt = nullptr, *counts = nullptr;
-        int cap = 0, stride = 0, nblk = 0;
+    struct DetWs {                      // decode + NMS workspace for `cap` candidate rows of `stride` floats per image
+        DevBuf<float> rows; DevBuf<unsigned> mask; DevBuf<int> blkcnt, counts;
+        int cap = 0, stride = 0;
     };
     struct Slot {
-        float *d_in = nullptr;
-        std::vector<float *> d_out, h_out;
-        cudaEvent_t ev_in = nullptr, ev_comp = nullptr, ev_done = nullptr, ev_det = nullptr;
+        DevBuf<float> d_in;
+        std::vector<Final> out;         // raw tensors (mode 0), made by the first engine_submit on this slot
+        Event ev_in, ev_comp, ev_done, ev_det;
         bool busy = false;
         // device-side input pipeline + decode of the pipelined detection path (engine_submit_frames)
         FrameStage u8;
         DetWs det;
-        float *h_rows = nullptr; size_t h_rows_bytes = 0; int *h_counts = nullptr;
+        PinnedBuf<float> h_rows; PinnedBuf<int> h_counts;
         int mode = 0;                   // 0: raw tensors (engine_submit), 1: detections (engine_submit_frames)
         int nimg = 0;                   // images of the batch in this slot (mode 1)
     };
     std::vector<Slot> slots;
-    cudaStream_t s_in = nullptr, s_out = nullptr, s_det = nullptr;
+    Stream s_in, s_out, s_det;
     int next_slot = 0;
     DetWs det;                          // workspace of the synchronous engine_detect
     ~Engine();
 };
 
-static void free_stage(Engine::FrameStage &st) {
-    if (st.buf) cudaFree(st.buf);
-    if (st.d_geo) cudaFree(st.d_geo);
-    if (st.h_geo) cudaFreeHost(st.h_geo);
-}
-
+// Work may still be queued for uncollected tickets, or on a caller's stream (engine_forward); the members free themselves
+// once it has finished.
 Engine::~Engine() {
     cudaSetDevice(opt.device);
-    if (graph_exec) cudaGraphExecDestroy(graph_exec);
-    for (float *p : h_final) if (p) cudaFreeHost(p);
-    for (float *p : d_final) if (p) cudaFree(p);
-    for (int32_t *p : d_counts) if (p) cudaFree(p);
-    for (void *p : tc_plans) tc_free_plan(p);
-    if (stem_plan) tc_stem_free_plan(stem_plan);
-    if (det.rows) cudaFree(det.rows);
-    if (det.mask) cudaFree(det.mask);
-    if (det.blkcnt) cudaFree(det.blkcnt);
-    if (det.counts) cudaFree(det.counts);
-    free_stage(u8);
-    if (d_unit) cudaFree(d_unit);
-    if (ev_frames_ready) cudaEventDestroy(ev_frames_ready);
-    if (ev_frames_read) cudaEventDestroy(ev_frames_read);
-    for (Slot &sl : slots) {
-        free_stage(sl.u8);
-        if (sl.det.rows) cudaFree(sl.det.rows);
-        if (sl.det.mask) cudaFree(sl.det.mask);
-        if (sl.det.blkcnt) cudaFree(sl.det.blkcnt);
-        if (sl.det.counts) cudaFree(sl.det.counts);
-        if (sl.h_rows) cudaFreeHost(sl.h_rows);
-        if (sl.h_counts) cudaFreeHost(sl.h_counts);
-        if (sl.ev_det) cudaEventDestroy(sl.ev_det);
-        if (sl.d_in) cudaFree(sl.d_in);
-        for (float *p : sl.d_out) if (p) cudaFree(p);
-        for (float *p : sl.h_out) if (p) cudaFreeHost(p);
-        if (sl.ev_in) cudaEventDestroy(sl.ev_in);
-        if (sl.ev_comp) cudaEventDestroy(sl.ev_comp);
-        if (sl.ev_done) cudaEventDestroy(sl.ev_done);
-    }
-    if (s_in) cudaStreamDestroy(s_in);
-    if (s_out) cudaStreamDestroy(s_out);
-    if (s_det) cudaStreamDestroy(s_det);
-    if (act_arena) cudaFree(act_arena);
-    if (w_arena) cudaFree(w_arena);
-    if (d_input) cudaFree(d_input);
-    if (stream) cudaStreamDestroy(stream);
+    cudaDeviceSynchronize();
 }
 
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
@@ -347,7 +295,7 @@ struct Builder {
         if (L[i].side == SIDE_S8) return make_tv(base, B, l.h, l.w, l.c, ld, P, DT_S8, 0);
         return make_tv(base, B, l.h, l.w, ld, ld, P, DT_BITS, 0);
     }
-    TV side_placed(int i) const { return side_view(i, e.act_arena + side_off[i]); }
+    TV side_placed(int i) const { return side_view(i, e.act_arena.get() + side_off[i]); }
     static float alpha1(const Layer &l) { return 32 / (l.input_quant_multipler * l.weights_quant_multipler); }   // ALPHA1, ..._quantized.c:598
 
     // Convolution i as a tensor-core convolution (the kind follows the variant and the activation type), with the shortcut and
@@ -377,14 +325,14 @@ struct Builder {
         }
         if (!placed) return c;
         // filters: [ldn][K] bf16, f32 (K-major copy) or s8 / +-1 bytes ([taps][cpad] per filter)
-        c.w = e.w_arena + (c.kind == TC_BF16 ? cw[i].w_bf16 : c.kind == TC_TF32 ? cw[i].w_f32km : cw[i].w_s8);
+        c.w = e.w_arena.get() + (c.kind == TC_BF16 ? cw[i].w_bf16 : c.kind == TC_TF32 ? cw[i].w_f32km : cw[i].w_s8);
         c.ldn = cw[i].ldn;
         c.bias = bias(i);
         if (c.kind == TC_S8) c.alpha1 = alpha1(l);
-        if (c.kind == TC_XNOR) c.mean = reinterpret_cast<const float *>(e.w_arena + cw[i].mean);
-        c.acc_out = e.d_counts[i];
+        if (c.kind == TC_XNOR) c.mean = reinterpret_cast<const float *>(e.w_arena.get() + cw[i].mean);
+        c.acc_out = e.counts[i].get();
         if (p.yolo_fused) {
-            c.yolo_out = e.d_final[i + 1];
+            c.yolo_out = e.finals[i + 1].d.get();
             c.yolo_classes = layer(i + 1).classes;
         }
         return c;
@@ -605,36 +553,31 @@ struct Builder {
             const int sdt = L[i].side == SIDE_PM1_F32 ? DT_F32 : L[i].side == SIDE_S8 ? DT_S8 : DT_BITS;
             if (L[i].side != SIDE_NONE) side_off[i] = take(tv_bytes(B, l.h, l.w, L[i].side_ld, P, sdt));
         }
-        e.act_bytes = total;
-        CUDA_OK(cudaMalloc(&e.act_arena, total));
-        CUDA_OK(cudaMemsetAsync(e.act_arena, 0, total, e.stream));   // zero borders, once
+        e.act_arena.ensure(total);
+        CUDA_OK(cudaMemsetAsync(e.act_arena.get(), 0, total, e.stream));   // zero borders, once
         for (int i = 0; i < nl; ++i)   // +-1 activation buffers: borders are -1 (out-of-image taps count as -1, SURVEY F9)
             if (L[i].variant == 1 && L[i].side == SIDE_S8)
-                CUDA_OK(cudaMemsetAsync(e.act_arena + side_off[i], 0xFF, tv_bytes(B, layer(i).h, layer(i).w, L[i].side_ld, P, DT_S8), e.stream));
-        e.in0 = first == FIRST_NHWC ? in0_view(e.act_arena + in0_off) : TV{};
+                CUDA_OK(cudaMemsetAsync(e.act_arena.get() + side_off[i], 0xFF, tv_bytes(B, layer(i).h, layer(i).w, L[i].side_ld, P, DT_S8), e.stream));
+        e.in0 = first == FIRST_NHWC ? in0_view(e.act_arena.get() + in0_off) : TV{};
         e.in0_dt = ADT;
         e.act_dt = ADT;
         e.out_tv.assign(nl, TV{});
         e.out_dt.assign(nl, ADT);
         for (int i = 0; i < nl; ++i) {
             e.out_dt[i] = L[i].out_dt;
-            if (L[i].materialised) e.out_tv[i] = out_view(i, [&](int j) { return e.act_arena + buf_off[j]; });
+            if (L[i].materialised) e.out_tv[i] = out_view(i, [&](int j) { return e.act_arena.get() + buf_off[j]; });
         }
     }
 
     // detection-layer outputs, and the last layer's output whatever its type (the reference returns it)
     void place_finals() {
-        e.d_final.assign(nl, nullptr);
-        e.h_final.assign(nl, nullptr);
-        e.final_count.assign(nl, 0);
-        e.d_counts.assign(nl, nullptr);
-        e.counts_count.assign(nl, 0);
+        e.finals.resize(nl);
+        e.counts.resize(nl);
         for (int i = 0; i < nl; ++i) {
             const Layer &l = layer(i);
             if (!(l.type == YB_YOLO || l.type == YB_REGION || (i == nl - 1 && l.outputs > 0))) continue;
-            e.final_count[i] = (size_t)l.outputs * B;
-            CUDA_OK(cudaMalloc(&e.d_final[i], e.final_count[i] * sizeof(float)));
-            CUDA_OK(cudaHostAlloc(&e.h_final[i], e.final_count[i] * sizeof(float), cudaHostAllocDefault));
+            e.finals[i].d.ensure((size_t)l.outputs * B);
+            e.finals[i].h.ensure((size_t)l.outputs * B);
         }
     }
 
@@ -707,31 +650,28 @@ struct Builder {
             const Layer &l0 = layer(0);
             for_each_weight(l0, [&](int f, int c, int t, size_t k) { dst[f * 32 + t * 3 + c] = __float2bfloat16_rn(l0.weights[k]); });
         }
-        e.w_bytes = align_up(std::max<size_t>(hostw.size(), 1024), 1024);
-        CUDA_OK(cudaMalloc(&e.w_arena, e.w_bytes));
-        if (opt.upload) CUDA_OK(cudaMemcpyAsync(e.w_arena, hostw.data(), hostw.size(), cudaMemcpyHostToDevice, e.stream));
+        e.w_arena.ensure(align_up(std::max<size_t>(hostw.size(), 1024), 1024));
+        if (opt.upload) CUDA_OK(cudaMemcpyAsync(e.w_arena.get(), hostw.data(), hostw.size(), cudaMemcpyHostToDevice, e.stream));
         CUDA_OK(cudaStreamSynchronize(e.stream));   // hostw goes out of scope below
     }
 
     // ---- pass 4: op emission ---------------------------------------------------------------------------------------------
-    const float *bias(int i) const { return reinterpret_cast<const float *>(e.w_arena + cw[i].bias); }
+    const float *bias(int i) const { return reinterpret_cast<const float *>(e.w_arena.get() + cw[i].bias); }
     void push(int kind, int i, std::function<void(cudaStream_t)> f) { e.ops.push_back(Op{kind, i, std::move(f)}); }
 
     // the tensor-core plan of layer i, with the [yolo] layer or the max-pool the layer plan fuses
     void push_tc_plan(int kind, int i) {
-        void *plan = tc_make_plan(tc_conv(i, true, L[i].pool_mode));
-        e.tc_plans.push_back(plan);
-        e.tc_plan_layer.push_back(i);
+        e.tc_plans.emplace_back(i, tc_make_plan(tc_conv(i, true, L[i].pool_mode)));
+        const TcPlan *plan = e.tc_plans.back().second.get();
         if (kind == OP_CONV_TC || kind == OP_CONV_TC_TF32) ++e.n_tc;
-        push(kind, i, [plan](cudaStream_t s) { tc_launch(plan, s); });
+        push(kind, i, [plan](cudaStream_t s) { tc_launch(*plan, s); });
     }
 
     int32_t *counts_buffer(int i) {   // raw XNOR popcounts / INT8 accumulators (keep_counts)
         if (!opt.keep_counts) return nullptr;
         const Layer &l = layer(i);
-        e.counts_count[i] = (size_t)B * l.n * l.out_h * l.out_w;
-        CUDA_OK(cudaMalloc(&e.d_counts[i], e.counts_count[i] * sizeof(int32_t)));
-        return e.d_counts[i];
+        e.counts[i].ensure((size_t)B * l.n * l.out_h * l.out_w);
+        return e.counts[i].get();
     }
 
     void emit_first() {
@@ -756,17 +696,17 @@ struct Builder {
                 else k_stem_pool<2, ACT_LINEAR><<<grid, 128, 0, s>>>(din, q, w16, act, H, W, mult);
             };
         } else if (first == FIRST_STEM_TC || first == FIRST_STEM_S2) {
-            void *sp = first == FIRST_STEM_S2
-                ? tc_stem_s2_make_plan(l0, layer(1), e.out_tv[1], e.w_arena + stem_w_off, bias(0), e.w_arena + cw[1].w_bf16, bias(1))
-                : tc_stem_make_plan(l0, e.out_tv[0], e.w_arena + stem_w_off, bias(0));
-            e.stem_plan = sp;
+            e.stem_plan = first == FIRST_STEM_S2
+                ? tc_stem_s2_make_plan(l0, layer(1), e.out_tv[1], e.w_arena.get() + stem_w_off, bias(0), e.w_arena.get() + cw[1].w_bf16, bias(1))
+                : tc_stem_make_plan(l0, e.out_tv[0], e.w_arena.get() + stem_w_off, bias(0));
+            const StemPlan *sp = e.stem_plan.get();
             e.first_kind = OP_CONV_TC;
             if (first == FIRST_STEM_S2) {
                 e.first_layer = 1;
                 ++e.n_tc;
             }
-            e.first_op = [sp](const float *din, cudaStream_t s) { tc_stem_launch(sp, din, s); };
-            if (!sw.no_stem_u8) e.first_op_u8 = [sp](const unsigned char *d8, cudaStream_t s) { tc_stem_launch_u8(sp, d8, s); };
+            e.first_op = [sp](const float *din, cudaStream_t s) { tc_stem_launch(*sp, din, s); };
+            if (!sw.no_stem_u8) e.first_op_u8 = [sp](const unsigned char *d8, cudaStream_t s) { tc_stem_launch_u8(*sp, d8, s); };
         } else if (first == FIRST_STEM_SIMT) {
             const TV tout = e.out_tv[0];
             const int nf = l0.n, odt = L[0].out_dt;
@@ -832,7 +772,7 @@ struct Builder {
         const long M = (long)B * l.out_h * l.out_w;
         ConvP cp{};
         cp.in = tin; cp.out = tout; cp.res = res;
-        cp.w = e.w_arena + cw[i].w_f32;
+        cp.w = e.w_arena.get() + cw[i].w_f32;
         cp.bias = bias(i);
         cp.n = l.n; cp.ldw = cw[i].ldw; cp.size = l.size; cp.stride = l.stride; cp.pad = l.pad;
         cp.act = l.activation; cp.act2 = act2; cp.K = l.size * l.size * l.c; cp.M = M;
@@ -863,7 +803,7 @@ struct Builder {
             push(OP_BINARIZE, i, [tin, pm1, gb](cudaStream_t s) { k_binarize_pm1<<<gb, 256, 0, s>>>(tin, pm1); });
             ConvP cp{};
             cp.in = pm1; cp.out = tout; cp.res = TV{};
-            cp.w = e.w_arena + cw[i].w_f32;
+            cp.w = e.w_arena.get() + cw[i].w_f32;
             cp.bias = bias(i);
             cp.n = l.n; cp.ldw = cw[i].ldw; cp.size = l.size; cp.stride = l.stride; cp.pad = l.pad;
             cp.act = l.activation; cp.act2 = ACT_LINEAR; cp.K = l.size * l.size * l.c; cp.M = M;
@@ -880,7 +820,7 @@ struct Builder {
             return;
         }
         const int CW = p.side_ld;
-        const TV bits = make_tv(e.act_arena + side_off[i], B, l.h, l.w, CW, CW, P, DT_BITS, 0);
+        const TV bits = make_tv(e.act_arena.get() + side_off[i], B, l.h, l.w, CW, CW, P, DT_BITS, 0);
         if (!p.prefilled) {
             if (vec4_view(tin)) {
                 const int g = grid_for((long)B * l.h * l.w * CW);
@@ -892,8 +832,8 @@ struct Builder {
         }
         XnorP xp{};
         xp.bits = bits; xp.out = tout;
-        xp.w = reinterpret_cast<const uint32_t *>(e.w_arena + cw[i].w_bits);
-        xp.mean = reinterpret_cast<const float *>(e.w_arena + cw[i].mean);
+        xp.w = reinterpret_cast<const uint32_t *>(e.w_arena.get() + cw[i].w_bits);
+        xp.mean = reinterpret_cast<const float *>(e.w_arena.get() + cw[i].mean);
         xp.bias = bias(i);
         xp.n = l.n; xp.size = l.size; xp.pad = l.pad; xp.K = l.size * l.size * l.c;
         xp.padbits = (CW * 32 - l.c) * l.size * l.size;
@@ -942,7 +882,7 @@ struct Builder {
         const long M = (long)B * l.out_h * l.out_w;
         Int8P ip{};
         ip.q = q; ip.out = tout;
-        ip.w = reinterpret_cast<const uint32_t *>(e.w_arena + cw[i].w_s8);
+        ip.w = reinterpret_cast<const uint32_t *>(e.w_arena.get() + cw[i].w_s8);
         ip.bias = bias(i);
         ip.alpha1 = alpha1(l);
         ip.n = l.n; ip.size = l.size; ip.stride = l.stride; ip.pad = l.pad; ip.act = l.activation;
@@ -1064,7 +1004,7 @@ struct Builder {
         case YB_YOLO: {
             if (p.yolo_fused) break;   // written by the head convolution's epilogue
             need_input(i);
-            float *dst = e.d_final[i];
+            float *dst = e.finals[i].d.get();
             const int classes = l.classes;
             const int gy = grid_for((long)B * ((l.h * l.w + 31) / 32) * ((l.c + 31) / 32) * 256);
             const int fast = (ADT == DT_BF16) ? 1 : 0;
@@ -1076,7 +1016,7 @@ struct Builder {
         }
         case YB_REGION: {
             need_input(i);
-            float *dst = e.d_final[i];
+            float *dst = e.finals[i].d.get();
             const int n = l.n, classes = l.classes, coords = l.coords, softmax = l.softmax;
             const int gr = grid_for((long)B * l.h * l.w * l.n);
             push(OP_REGION, i, [tin, dst, n, classes, coords, softmax, gr, dt](cudaStream_t s) {
@@ -1094,11 +1034,11 @@ struct Builder {
     void emit_last_copy() {
         const int last = nl - 1;
         const Layer &l = layer(last);
-        if (l.type == YB_YOLO || l.type == YB_REGION || !e.d_final[last]) return;
+        if (l.type == YB_YOLO || l.type == YB_REGION || !e.finals[last].d) return;
         const int src = L[last].fused_into >= 0 ? L[last].fused_into : last;
         const TV t = e.out_tv[src];
         if (!t.base) return;
-        float *dst = e.d_final[last];
+        float *dst = e.finals[last].d.get();
         const int dt = L[src].out_dt;
         const int g = grid_for((long)B * l.outputs);
         push(OP_YOLO, last, [t, dst, g, dt](cudaStream_t s) {
@@ -1136,41 +1076,37 @@ std::shared_ptr<Engine> build_engine(Network *net, const EngineOptions &opt) {
     e->opt = opt;
     e->batch = net->batch;
     e->sw = Switches::read();
-    CUDA_OK(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
+    e->stream = make_stream();
 
     Builder b(*net, opt, *e);
     b.plan_layers();
     b.place();
     b.place_finals();
     b.pack_weights();
-    e->input_count = (size_t)net->batch * net->c * net->h * net->w;   // staging of the caller's images
-    CUDA_OK(cudaMalloc(&e->d_input, e->input_count * sizeof(float)));
+    e->d_input.ensure((size_t)net->batch * net->c * net->h * net->w);
     b.emit_ops();
     CUDA_OK(cudaStreamSynchronize(e->stream));
     CUDA_OK(cudaGetLastError());
     return e;
 }
 
-static void launch_input(Engine *e, const float *d_in, cudaStream_t s) { e->first_op(d_in, s); }
 static void engine_forward_impl(Engine *e, const void *d_input, const unsigned char *d_u8_frames, void *stream);
 void engine_forward(Engine *e, const void *d_input, void *stream) { engine_forward_impl(e, d_input, nullptr, stream); }
 
 void engine_upload_input(Engine *e, const float *host_input, void *stream) {
-    cudaStream_t s = stream ? (cudaStream_t)stream : e->stream;
+    cudaStream_t s = stream ? (cudaStream_t)stream : (cudaStream_t)e->stream;
     CUDA_OK(cudaSetDevice(e->opt.device));
-    CUDA_OK(cudaMemcpyAsync(e->d_input, host_input, e->input_count * sizeof(float), cudaMemcpyHostToDevice, s));
+    CUDA_OK(cudaMemcpyAsync(e->d_input.get(), host_input, e->d_input.count() * sizeof(float), cudaMemcpyHostToDevice, s));
 }
 
 // The per-image table: frame sizes, the resize's scales, and the size correct_yolo_boxes (additionally.c:4287-4296) embeds each image at -- the
 // network size, or with `letter` the reference's integer letterbox size of that image.  Entries nimg .. batch-1 are zero.
 static void fill_geo(Engine *e, Engine::FrameStage &st, const Network *net, const int *w, const int *h, int nimg, int letter) {
     const int B = e->batch;
-    if (!st.h_geo) {
-        CUDA_OK(cudaHostAlloc(&st.h_geo, (size_t)B * sizeof(ImageGeo), cudaHostAllocDefault));
-        CUDA_OK(cudaMalloc(&st.d_geo, (size_t)B * sizeof(ImageGeo)));
-    }
+    st.h_geo.ensure(B);
+    st.d_geo.ensure(B);
     for (int b = 0; b < B; ++b) {
-        ImageGeo &g = st.h_geo[b];
+        ImageGeo &g = st.h_geo.get()[b];
         g = ImageGeo{};
         if (b >= nimg) continue;
         g.w = w[b]; g.h = h[b]; g.new_w = net->w; g.new_h = net->h;
@@ -1200,20 +1136,17 @@ static bool stage_frames(Engine *e, Engine::FrameStage &st, const Network *net, 
     }
     // room for a zero tail of network-size frames (the 8-bit stem reads whole batches)
     const size_t need = std::max(total, net_size ? (size_t)B * net->w * net->h * c : 0);
-    if (need > st.bytes) {
-        if (st.buf) cudaFree(st.buf);
-        CUDA_OK(cudaMalloc(&st.buf, need));
-        st.bytes = need;
-    }
-    for (int b = 0; b < nimg; ++b) { st.h_geo[b].src = st.buf + off[b]; st.h_geo[b].pitch = w[b] * c; }
+    st.buf.ensure(need);
+    ImageGeo *geo = st.h_geo.get();
+    for (int b = 0; b < nimg; ++b) { geo[b].src = st.buf.get() + off[b]; geo[b].pitch = w[b] * c; }
     for (int b = 0; b < nimg;) {
         size_t run = (size_t)w[b] * h[b] * c;
         int nb = b + 1;
         while (nb < nimg && frames[nb] == frames[b] + run) run += (size_t)w[nb] * h[nb] * c, ++nb;
-        CUDA_OK(cudaMemcpyAsync(st.buf + off[b], frames[b], run, cudaMemcpyHostToDevice, s));
+        CUDA_OK(cudaMemcpyAsync(st.buf.get() + off[b], frames[b], run, cudaMemcpyHostToDevice, s));
         b = nb;
     }
-    CUDA_OK(cudaMemcpyAsync(st.d_geo, st.h_geo, (size_t)B * sizeof(ImageGeo), cudaMemcpyHostToDevice, s));
+    CUDA_OK(cudaMemcpyAsync(st.d_geo.get(), geo, (size_t)B * sizeof(ImageGeo), cudaMemcpyHostToDevice, s));
     return net_size;
 }
 
@@ -1224,10 +1157,10 @@ static void stage_device_frames(Engine *e, Engine::FrameStage &st, const Network
     for (int b = 0; b < nimg; ++b) { w[b] = frames[b].w; h[b] = frames[b].h; }
     fill_geo(e, st, net, w.data(), h.data(), nimg, letter);
     for (int b = 0; b < nimg; ++b) {
-        ImageGeo &g = st.h_geo[b];
+        ImageGeo &g = st.h_geo.get()[b];
         g.src = frames[b].data; g.chroma = frames[b].chroma; g.pitch = frames[b].pitch; g.plane = frames[b].plane_stride;
     }
-    CUDA_OK(cudaMemcpyAsync(st.d_geo, st.h_geo, (size_t)e->batch * sizeof(ImageGeo), cudaMemcpyHostToDevice, s));
+    CUDA_OK(cudaMemcpyAsync(st.d_geo.get(), st.h_geo.get(), (size_t)e->batch * sizeof(ImageGeo), cudaMemcpyHostToDevice, s));
 }
 
 // frames described by st.d_geo, of format fmt -> the network's planar f32 input; images nimg .. batch-1 are zero
@@ -1236,13 +1169,14 @@ static void launch_resize(Engine *e, const Engine::FrameStage &st, const Network
     if (!e->d_unit) {   // load_image_stb's conversion, additionally.c:3093-3103
         float unit[256];
         for (int v = 0; v < 256; ++v) unit[v] = (float)((double)(float)v / 255.);
-        CUDA_OK(cudaMalloc(&e->d_unit, sizeof(unit)));
-        CUDA_OK(cudaMemcpy(e->d_unit, unit, sizeof(unit), cudaMemcpyHostToDevice));
+        DevBuf<float> d_unit(256);
+        CUDA_OK(cudaMemcpy(d_unit.get(), unit, sizeof(unit), cudaMemcpyHostToDevice));
+        e->d_unit = std::move(d_unit);
     }
     const dim3 grid((unsigned)((net->h + RS_ROWS - 1) / RS_ROWS), (unsigned)nimg);
     auto *k = fmt == YB_FRAME_BGR ? k_resize_frames<YB_FRAME_BGR> : fmt == YB_FRAME_RGB_PLANAR ? k_resize_frames<YB_FRAME_RGB_PLANAR>
             : fmt == YB_FRAME_NV12 ? k_resize_frames<YB_FRAME_NV12> : k_resize_frames<YB_FRAME_RGB>;
-    k<<<grid, RS_THREADS, 0, s>>>(st.d_geo, e->d_unit, net->c, dst, net->w, net->h);
+    k<<<grid, RS_THREADS, 0, s>>>(st.d_geo.get(), e->d_unit.get(), net->c, dst, net->w, net->h);
     const size_t per = (size_t)net->c * net->h * net->w;
     if (nimg < e->batch) CUDA_OK(cudaMemsetAsync(dst + nimg * per, 0, (e->batch - nimg) * per * sizeof(float), s));
 }
@@ -1253,10 +1187,8 @@ static void launch_resize(Engine *e, const Engine::FrameStage &st, const Network
 // at once, so each call may reuse them.
 static void resize_device_frames(Engine *e, Engine::FrameStage &st, const Network *net, const yb_device_frame *frames,
                                  int nimg, int fmt, int letter, float *dst, cudaStream_t s, cudaStream_t user) {
-    if (!e->ev_frames_ready) {
-        CUDA_OK(cudaEventCreateWithFlags(&e->ev_frames_ready, cudaEventDisableTiming));
-        CUDA_OK(cudaEventCreateWithFlags(&e->ev_frames_read, cudaEventDisableTiming));
-    }
+    if (!e->ev_frames_ready) e->ev_frames_ready = make_event();
+    if (!e->ev_frames_read) e->ev_frames_read = make_event();
     stage_device_frames(e, st, net, frames, nimg, letter, s);
     CUDA_OK(cudaEventRecord(e->ev_frames_ready, user));
     CUDA_OK(cudaStreamWaitEvent(s, e->ev_frames_ready, 0));
@@ -1269,13 +1201,13 @@ static void resize_device_frames(Engine *e, Engine::FrameStage &st, const Networ
 void engine_upload_frames(Engine *e, Network *net, const unsigned char *const *frames, const int *w, const int *h, int nimg) {
     CUDA_OK(cudaSetDevice(e->opt.device));
     stage_frames(e, e->u8, net, frames, w, h, nimg, 0, e->stream);
-    launch_resize(e, e->u8, net, nimg, YB_FRAME_RGB, e->d_input, e->stream);
+    launch_resize(e, e->u8, net, nimg, YB_FRAME_RGB, e->d_input.get(), e->stream);
     CUDA_OK(cudaGetLastError());
 }
 
 void engine_upload_device_frames(Engine *e, Network *net, const yb_device_frame *frames, int nimg, int fmt, void *stream) {
     CUDA_OK(cudaSetDevice(e->opt.device));
-    resize_device_frames(e, e->u8, net, frames, nimg, fmt, 0, e->d_input, e->stream, (cudaStream_t)stream);
+    resize_device_frames(e, e->u8, net, frames, nimg, fmt, 0, e->d_input.get(), e->stream, (cudaStream_t)stream);
     CUDA_OK(cudaGetLastError());
 }
 
@@ -1301,11 +1233,11 @@ void check_frame_memory(int device, const char *fn, const yb_device_frame *frame
 void *engine_stream(Engine *e) { return e->stream; }
 
 static void engine_forward_impl(Engine *e, const void *d_input, const unsigned char *d_u8_frames, void *stream) {
-    cudaStream_t s = stream ? (cudaStream_t)stream : e->stream;
+    cudaStream_t s = stream ? (cudaStream_t)stream : (cudaStream_t)e->stream;
     CUDA_OK(cudaSetDevice(e->opt.device));   // thread identity may change per call (SURVEY 8b, threading)
-    const float *din = d_input ? reinterpret_cast<const float *>(d_input) : e->d_input;
+    const float *din = d_input ? reinterpret_cast<const float *>(d_input) : e->d_input.get();
     if (d_u8_frames) e->first_op_u8(d_u8_frames, s);   // stem straight from the 8-bit frames
-    else launch_input(e, din, s);
+    else e->first_op(din, s);
     if (!e->graph_exec && !e->graph_failed && e->sw.no_graph) e->graph_failed = true;   // profiling aid
     if (!e->graph_exec && !e->graph_failed) {
         // capture everything after the input conversion once
@@ -1315,15 +1247,13 @@ static void engine_forward_impl(Engine *e, const void *d_input, const unsigned c
             for (size_t k = 1; k < e->ops.size(); ++k) e->ops[k].launch(s);
             st = cudaStreamEndCapture(s, &graph);
         }
+        cudaGraphExec_t exec = nullptr;
         if (st == cudaSuccess && graph) {
-            st = cudaGraphInstantiate(&e->graph_exec, graph, 0);
+            st = cudaGraphInstantiate(&exec, graph, 0);
             cudaGraphDestroy(graph);
         }
-        if (st != cudaSuccess || !e->graph_exec) {
-            e->graph_failed = true;
-            e->graph_exec = nullptr;
-            cudaGetLastError();
-        }
+        e->graph_exec = GraphExec(st == cudaSuccess ? exec : nullptr);
+        if (!e->graph_exec) { e->graph_failed = true; cudaGetLastError(); }
     }
     if (e->graph_exec) {
         CUDA_OK(cudaGraphLaunch(e->graph_exec, s));
@@ -1334,66 +1264,86 @@ static void engine_forward_impl(Engine *e, const void *d_input, const unsigned c
 }
 
 void engine_download_outputs(Engine *e, Network *net, void *stream) {
-    cudaStream_t s = stream ? (cudaStream_t)stream : e->stream;
+    cudaStream_t s = stream ? (cudaStream_t)stream : (cudaStream_t)e->stream;
     CUDA_OK(cudaSetDevice(e->opt.device));
-    for (size_t i = 0; i < e->d_final.size(); ++i) {
-        if (!e->d_final[i]) continue;
-        CUDA_OK(cudaMemcpyAsync(e->h_final[i], e->d_final[i], e->final_count[i] * sizeof(float), cudaMemcpyDeviceToHost, s));
-        net->layers[i].output = e->h_final[i];
-        net->layers[i].output_count = e->final_count[i];
+    for (size_t i = 0; i < e->finals.size(); ++i) {
+        const Engine::Final &f = e->finals[i];
+        if (!f.d) continue;
+        CUDA_OK(cudaMemcpyAsync(f.h.get(), f.d.get(), f.d.count() * sizeof(float), cudaMemcpyDeviceToHost, s));
+        net->layers[i].output = f.h.get();
+        net->layers[i].output_count = f.d.count();
     }
     CUDA_OK(cudaStreamSynchronize(s));
 }
 
-static void ensure_slots(Engine *e) {
-    if (!e->slots.empty()) return;
-    const int NS = 3;
-    CUDA_OK(cudaStreamCreateWithFlags(&e->s_in, cudaStreamNonBlocking));
-    CUDA_OK(cudaStreamCreateWithFlags(&e->s_out, cudaStreamNonBlocking));
-    e->slots.resize(NS);
-    for (auto &sl : e->slots) {
-        CUDA_OK(cudaMalloc(&sl.d_in, e->input_count * sizeof(float)));
-        sl.d_out.assign(e->d_final.size(), nullptr);
-        sl.h_out.assign(e->d_final.size(), nullptr);
-        for (size_t i = 0; i < e->d_final.size(); ++i) {
-            if (!e->d_final[i]) continue;
-            CUDA_OK(cudaMalloc(&sl.d_out[i], e->final_count[i] * sizeof(float)));
-            CUDA_OK(cudaHostAlloc(&sl.h_out[i], e->final_count[i] * sizeof(float), cudaHostAllocDefault));
+// ---- the pipeline of the submit / collect calls: three slots, one batch in flight in each ------------------------------
+// Takes the next slot for a submit and returns its ticket.  The slots are published only once all three are built; a slot
+// whose ticket is still out is refused; the copy-in stream waits until the forward that last read the slot's input is done.
+static int acquire_slot(Engine *e) {
+    CUDA_OK(cudaSetDevice(e->opt.device));
+    if (e->slots.empty()) {
+        e->s_in = make_stream(); e->s_out = make_stream(); e->s_det = make_stream();
+        std::vector<Engine::Slot> slots(3);
+        for (Engine::Slot &sl : slots) {
+            sl.d_in.ensure(e->d_input.count());
+            sl.ev_in = make_event(); sl.ev_comp = make_event(); sl.ev_done = make_event(); sl.ev_det = make_event();
         }
-        CUDA_OK(cudaEventCreateWithFlags(&sl.ev_in, cudaEventDisableTiming));
-        CUDA_OK(cudaEventCreateWithFlags(&sl.ev_comp, cudaEventDisableTiming));
-        CUDA_OK(cudaEventCreateWithFlags(&sl.ev_done, cudaEventDisableTiming));
-        CUDA_OK(cudaEventCreateWithFlags(&sl.ev_det, cudaEventDisableTiming));
+        e->slots = std::move(slots);
     }
-    CUDA_OK(cudaStreamCreateWithFlags(&e->s_det, cudaStreamNonBlocking));
+    const int k = e->next_slot;
+    Engine::Slot &sl = e->slots[k];
+    if (sl.busy) fatal_throw("submit: pipeline full (3 batches in flight) -- collect the oldest ticket first");
+    e->next_slot = (k + 1) % (int)e->slots.size();
+    CUDA_OK(cudaStreamWaitEvent(e->s_in, sl.ev_comp, 0));
+    return k;
+}
+
+// Runs the forward on the compute stream once the input staged on the copy-in stream is there: from the network-size 8-bit
+// frames u8 when given, else from the slot's input.  Then the compute stream waits until the slot's previous outputs have
+// been read out (D2H of the raw tensors, or NMS and counts copy), so that what it enqueues next may overwrite them.
+static void forward_slot(Engine *e, Engine::Slot &sl, const unsigned char *u8) {
+    CUDA_OK(cudaEventRecord(sl.ev_in, e->s_in));
+    CUDA_OK(cudaStreamWaitEvent(e->stream, sl.ev_in, 0));
+    engine_forward_impl(e, sl.d_in.get(), u8, e->stream);
+    CUDA_OK(cudaStreamWaitEvent(e->stream, sl.ev_done, 0));
+    CUDA_OK(cudaStreamWaitEvent(e->stream, sl.ev_det, 0));
+}
+
+// The slot of a ticket of `mode` once its results have reached the host, marked free; any other ticket throws
+// "<fn>: bad ticket".
+static Engine::Slot &release_slot(Engine *e, int ticket, int mode, const char *fn) {
+    if (ticket < 0 || ticket >= (int)e->slots.size() || !e->slots[ticket].busy || e->slots[ticket].mode != mode)
+        fatal_throw(std::string(fn) + ": bad ticket");
+    CUDA_OK(cudaSetDevice(e->opt.device));
+    Engine::Slot &sl = e->slots[ticket];
+    CUDA_OK(cudaEventSynchronize(mode == 0 ? sl.ev_done : sl.ev_det));
+    sl.busy = false;
+    return sl;
 }
 
 // Enqueue one batch: H2D on the copy-in stream, forward on the compute stream, D2H on the copy-out stream.
 // Returns the ticket to pass to engine_collect.  Up to 3 batches may be in flight.
 int engine_submit(Engine *e, const float *host_input) {
-    CUDA_OK(cudaSetDevice(e->opt.device));
-    ensure_slots(e);
-    const int k = e->next_slot;
+    const int k = acquire_slot(e);
     Engine::Slot &sl = e->slots[k];
-    if (sl.busy) fatal_throw("submit: pipeline full (3 batches in flight) -- collect the oldest ticket first");
-    e->next_slot = (k + 1) % (int)e->slots.size();
-    // the previous forward that read d_in[k] must have finished before it is overwritten
-    CUDA_OK(cudaStreamWaitEvent(e->s_in, sl.ev_comp, 0));
-    CUDA_OK(cudaMemcpyAsync(sl.d_in, host_input, e->input_count * sizeof(float), cudaMemcpyHostToDevice, e->s_in));
-    CUDA_OK(cudaEventRecord(sl.ev_in, e->s_in));
-    CUDA_OK(cudaStreamWaitEvent(e->stream, sl.ev_in, 0));
-    engine_forward(e, sl.d_in, e->stream);
-    // the previous D2H out of d_out[k] (or decode of it) must have finished before it is overwritten
-    CUDA_OK(cudaStreamWaitEvent(e->stream, sl.ev_done, 0));
-    CUDA_OK(cudaStreamWaitEvent(e->stream, sl.ev_det, 0));
-    for (size_t i = 0; i < e->d_final.size(); ++i)
-        if (e->d_final[i])
-            CUDA_OK(cudaMemcpyAsync(sl.d_out[i], e->d_final[i], e->final_count[i] * sizeof(float), cudaMemcpyDeviceToDevice, e->stream));
+    if (sl.out.empty()) {
+        std::vector<Engine::Final> out(e->finals.size());
+        for (size_t i = 0; i < out.size(); ++i) {
+            out[i].d.ensure(e->finals[i].d.count());
+            out[i].h.ensure(e->finals[i].d.count());
+        }
+        sl.out = std::move(out);
+    }
+    CUDA_OK(cudaMemcpyAsync(sl.d_in.get(), host_input, sl.d_in.count() * sizeof(float), cudaMemcpyHostToDevice, e->s_in));
+    forward_slot(e, sl, nullptr);
+    for (size_t i = 0; i < e->finals.size(); ++i)
+        if (e->finals[i].d)
+            CUDA_OK(cudaMemcpyAsync(sl.out[i].d.get(), e->finals[i].d.get(), e->finals[i].d.count() * sizeof(float),
+                                    cudaMemcpyDeviceToDevice, e->stream));
     CUDA_OK(cudaEventRecord(sl.ev_comp, e->stream));
     CUDA_OK(cudaStreamWaitEvent(e->s_out, sl.ev_comp, 0));
-    for (size_t i = 0; i < e->d_final.size(); ++i)
-        if (e->d_final[i])
-            CUDA_OK(cudaMemcpyAsync(sl.h_out[i], sl.d_out[i], e->final_count[i] * sizeof(float), cudaMemcpyDeviceToHost, e->s_out));
+    for (const Engine::Final &o : sl.out)
+        if (o.d) CUDA_OK(cudaMemcpyAsync(o.h.get(), o.d.get(), o.d.count() * sizeof(float), cudaMemcpyDeviceToHost, e->s_out));
     CUDA_OK(cudaEventRecord(sl.ev_done, e->s_out));
     sl.busy = true; sl.mode = 0;
     return k;
@@ -1402,19 +1352,9 @@ int engine_submit(Engine *e, const float *host_input) {
 // ptrs[i] = pinned host copy of layer i's output for this ticket (nullptr where the layer has none); valid until the slot
 // is reused.  The form the multi-GPU batch call uses: several engines feed ONE host model.
 void engine_collect_ptrs(Engine *e, int ticket, std::vector<const float *> &ptrs, std::vector<size_t> &counts) {
-    if (ticket < 0 || ticket >= (int)e->slots.size() || !e->slots[ticket].busy || e->slots[ticket].mode != 0)
-        fatal_throw("collect: bad ticket");
-    CUDA_OK(cudaSetDevice(e->opt.device));
-    Engine::Slot &sl = e->slots[ticket];
-    CUDA_OK(cudaEventSynchronize(sl.ev_done));
-    ptrs.assign(e->d_final.size(), nullptr);
-    counts.assign(e->d_final.size(), 0);
-    for (size_t i = 0; i < e->d_final.size(); ++i) {
-        if (!e->d_final[i]) continue;
-        ptrs[i] = sl.h_out[i];
-        counts[i] = e->final_count[i];
-    }
-    sl.busy = false;
+    const Engine::Slot &sl = release_slot(e, ticket, 0, "collect");
+    ptrs.clear(); counts.clear();
+    for (const Engine::Final &o : sl.out) { ptrs.push_back(o.h.get()); counts.push_back(o.h.count()); }
 }
 
 void engine_collect(Engine *e, Network *net, int ticket) {
@@ -1432,8 +1372,8 @@ void engine_collect(Engine *e, Network *net, int ticket) {
 // list with repeats, which NCCL refuses -- falls back to peer copies out of replica 0.
 const char *engine_broadcast_arena(const std::vector<Engine *> &reps) {
     if (reps.size() < 2) return "single";
-    const size_t bytes = reps[0]->w_bytes;
-    for (Engine *r : reps) if (r->w_bytes != bytes) fatal_throw("broadcast: replicas disagree on the arena size");
+    const size_t bytes = reps[0]->w_arena.count();
+    for (Engine *r : reps) if (r->w_arena.count() != bytes) fatal_throw("broadcast: replicas disagree on the arena size");
     bool distinct = true;
     for (size_t a = 0; a < reps.size(); ++a)
         for (size_t b = a + 1; b < reps.size(); ++b) distinct &= reps[a]->opt.device != reps[b]->opt.device;
@@ -1455,7 +1395,7 @@ const char *engine_broadcast_arena(const std::vector<Engine *> &reps) {
                 int rc = gstart();
                 for (size_t k = 0; k < reps.size() && rc == 0; ++k) {
                     CUDA_OK(cudaSetDevice(reps[k]->opt.device));
-                    rc = bcast(reps[k]->w_arena, reps[k]->w_arena, bytes, /*ncclChar*/ 0, /*root*/ 0, comms[k], reps[k]->stream);
+                    rc = bcast(reps[k]->w_arena.get(), reps[k]->w_arena.get(), bytes, /*ncclChar*/ 0, /*root*/ 0, comms[k], reps[k]->stream);
                 }
                 rc |= gend();
                 for (Engine *r : reps) { CUDA_OK(cudaSetDevice(r->opt.device)); CUDA_OK(cudaStreamSynchronize(r->stream)); }
@@ -1466,7 +1406,7 @@ const char *engine_broadcast_arena(const std::vector<Engine *> &reps) {
     }
     for (size_t k = 1; k < reps.size(); ++k) {
         CUDA_OK(cudaSetDevice(reps[0]->opt.device));
-        CUDA_OK(cudaMemcpyPeer(reps[k]->w_arena, reps[k]->opt.device, reps[0]->w_arena, reps[0]->opt.device, bytes));
+        CUDA_OK(cudaMemcpyPeer(reps[k]->w_arena.get(), reps[k]->opt.device, reps[0]->w_arena.get(), reps[0]->opt.device, bytes));
     }
     CUDA_OK(cudaDeviceSynchronize());
     return "peer-copy";
@@ -1477,81 +1417,78 @@ void engine_fetch_layer(Engine *e, Network *net, int layer, float *dst) {
     CUDA_OK(cudaSetDevice(e->opt.device));
     const Layer &l = net->layers[layer];
     const size_t count = (size_t)l.outputs * e->batch;
-    if (e->d_final[layer] && (l.type == YB_YOLO || l.type == YB_REGION)) {
-        CUDA_OK(cudaMemcpy(dst, e->d_final[layer], count * sizeof(float), cudaMemcpyDeviceToHost));
+    if (e->finals[layer].d && (l.type == YB_YOLO || l.type == YB_REGION)) {
+        CUDA_OK(cudaMemcpy(dst, e->finals[layer].d.get(), count * sizeof(float), cudaMemcpyDeviceToHost));
         return;
     }
     const TV t = e->out_tv[layer];
     if (!t.base) fatal_throw("fetch_layer: layer " + std::to_string(layer) + " has no materialised output "
                              "(fused or aliased away; build the engine with fusion off)");
-    float *tmp = nullptr;
-    CUDA_OK(cudaMalloc(&tmp, count * sizeof(float)));
+    DevBuf<float> tmp(count);
     const int g = grid_for((long)count);
-    if (e->out_dt[layer] == DT_F32) k_nhwc_to_nchw_f32<float><<<g, 256, 0, e->stream>>>(t, tmp);
-    else k_nhwc_to_nchw_f32<__nv_bfloat16><<<g, 256, 0, e->stream>>>(t, tmp);
-    CUDA_OK(cudaMemcpyAsync(dst, tmp, count * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
+    if (e->out_dt[layer] == DT_F32) k_nhwc_to_nchw_f32<float><<<g, 256, 0, e->stream>>>(t, tmp.get());
+    else k_nhwc_to_nchw_f32<__nv_bfloat16><<<g, 256, 0, e->stream>>>(t, tmp.get());
+    CUDA_OK(cudaMemcpyAsync(dst, tmp.get(), count * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
     CUDA_OK(cudaStreamSynchronize(e->stream));
-    cudaFree(tmp);
 }
 
 void engine_fetch_input(Engine *e, float *dst) {
     CUDA_OK(cudaSetDevice(e->opt.device));
     CUDA_OK(cudaStreamSynchronize(e->stream));
-    CUDA_OK(cudaMemcpy(dst, e->d_input, e->input_count * sizeof(float), cudaMemcpyDeviceToHost));
+    CUDA_OK(cudaMemcpy(dst, e->d_input.get(), e->d_input.count() * sizeof(float), cudaMemcpyDeviceToHost));
 }
 
 int engine_fetch_counts(Engine *e, int layer, int32_t *dst, size_t count) {
-    if (layer < 0 || layer >= (int)e->d_counts.size() || !e->d_counts[layer]) return -1;
-    if (count < e->counts_count[layer]) return -2;
+    if (layer < 0 || layer >= (int)e->counts.size() || !e->counts[layer]) return -1;
+    const DevBuf<int32_t> &c = e->counts[layer];
+    if (count < c.count()) return -2;
     CUDA_OK(cudaSetDevice(e->opt.device));
-    CUDA_OK(cudaMemcpy(dst, e->d_counts[layer], e->counts_count[layer] * sizeof(int32_t), cudaMemcpyDeviceToHost));
-    return (int)e->counts_count[layer];
+    CUDA_OK(cudaMemcpy(dst, c.get(), c.count() * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    return (int)c.count();
 }
 
-void engine_weight_arena(Engine *e, void **ptr, size_t *bytes) { *ptr = e->w_arena; *bytes = e->w_bytes; }
+void engine_weight_arena(Engine *e, void **ptr, size_t *bytes) { *ptr = e->w_arena.get(); *bytes = e->w_arena.count(); }
 // INT8 input calibration (SURVEY 8f row 3): |x| histogram of the INPUT of layer `layer` (image `img` of the batch) after a
 // forward, binned like the reference's entropy_calibration.  hist: host uint32[max_bin].
 void engine_input_histogram(Engine *e, Network *net, int layer, int img, float bin_width, int max_bin, uint32_t *hist) {
     CUDA_OK(cudaSetDevice(e->opt.device));
     if (max_bin < 129 || max_bin > 4096) fatal_throw("calibrate: max_bin must be in 129..4096");
     if (img < 0 || img >= e->batch) fatal_throw("calibrate: image index out of range");
-    unsigned *d_hist = nullptr;
-    CUDA_OK(cudaMalloc(&d_hist, (size_t)max_bin * sizeof(unsigned)));
-    CUDA_OK(cudaMemsetAsync(d_hist, 0, (size_t)max_bin * sizeof(unsigned), e->stream));
+    DevBuf<unsigned> d_hist(max_bin);
+    CUDA_OK(cudaMemsetAsync(d_hist.get(), 0, (size_t)max_bin * sizeof(unsigned), e->stream));
     if (layer == 0) {
         const long n = (long)net->c * net->h * net->w;
-        k_abs_hist_flat<<<grid_for(n), 256, 0, e->stream>>>(e->d_input + (size_t)img * n, n, bin_width, max_bin, d_hist);
+        k_abs_hist_flat<<<grid_for(n), 256, 0, e->stream>>>(e->d_input.get() + (size_t)img * n, n, bin_width, max_bin, d_hist.get());
     } else {
         const TV t = e->out_tv[layer - 1];
-        if (!t.base) { cudaFree(d_hist); fatal_throw("calibrate: the input of layer " + std::to_string(layer) +
-                                                     " is not materialised (fused away; set option fuse=0)"); }
+        if (!t.base) fatal_throw("calibrate: the input of layer " + std::to_string(layer) +
+                                 " is not materialised (fused away; set option fuse=0)");
         const long n = (long)t.C * t.H * t.W;
-        if (e->out_dt[layer - 1] == DT_F32) k_abs_hist<float><<<grid_for(n), 256, 0, e->stream>>>(t, img, bin_width, max_bin, d_hist);
-        else k_abs_hist<__nv_bfloat16><<<grid_for(n), 256, 0, e->stream>>>(t, img, bin_width, max_bin, d_hist);
+        if (e->out_dt[layer - 1] == DT_F32) k_abs_hist<float><<<grid_for(n), 256, 0, e->stream>>>(t, img, bin_width, max_bin, d_hist.get());
+        else k_abs_hist<__nv_bfloat16><<<grid_for(n), 256, 0, e->stream>>>(t, img, bin_width, max_bin, d_hist.get());
     }
-    CUDA_OK(cudaMemcpyAsync(hist, d_hist, (size_t)max_bin * sizeof(unsigned), cudaMemcpyDeviceToHost, e->stream));
+    CUDA_OK(cudaMemcpyAsync(hist, d_hist.get(), (size_t)max_bin * sizeof(unsigned), cudaMemcpyDeviceToHost, e->stream));
     CUDA_OK(cudaStreamSynchronize(e->stream));
-    cudaFree(d_hist);
 }
 
 // ---- batched decode + NMS on the device (yb_detect.cuh) ---------------------------------------------------------
 // geometry: P.geo, set by the caller
-static DetParams det_params(Engine *e, Network *net, const std::vector<float *> &finals, float thresh, float nms,
-                            int relative, int max_rows) {
+static DetParams det_params(Network *net, const std::vector<Engine::Final> &finals, float thresh, float nms, int relative,
+                            int max_rows) {
     if (max_rows <= 0 || max_rows > DET_MAX_ROWS) fatal_throw("detect: max_rows must be in 1.." + std::to_string(DET_MAX_ROWS));
     DetParams P{};
     int total = 0;
     for (size_t i = 0; i < net->layers.size(); ++i) {
         const Layer &l = net->layers[i];
         if (l.type != YB_YOLO && l.type != YB_REGION) continue;
-        if (!finals[i]) fatal_throw("detect: detection layer has no device output");
+        if (!finals[i].d) fatal_throw("detect: detection layer has no device output");
         if (P.nl == DET_MAX_LAYERS) fatal_throw("detect: too many detection layers");
         if (l.n > DET_MAX_ANCHORS) fatal_throw("detect: too many anchors per layer");
         if (P.nl && l.classes != P.classes) fatal_throw("detect: detection layers disagree on the class count");
         if ((l.type == YB_YOLO && (int)l.mask.size() < l.n) || (int)l.anchors.size() < 2 * l.n)
             fatal_throw("detect: detection layer without mask / anchors");
         DetLayer &d = P.L[P.nl++];
-        d.p = finals[i]; d.type = l.type; d.w = l.w; d.h = l.h; d.n = l.n; d.classes = l.classes; d.outputs = l.outputs;
+        d.p = finals[i].d.get(); d.type = l.type; d.w = l.w; d.h = l.h; d.n = l.n; d.classes = l.classes; d.outputs = l.outputs;
         d.base = total; d.nbox = l.w * l.h * l.n; total += d.nbox;
         for (int a = 0; a < l.n; ++a) {
             const int k = (l.type == YB_YOLO) ? l.mask[a] : a;
@@ -1562,41 +1499,36 @@ static DetParams det_params(Engine *e, Network *net, const std::vector<float *> 
     if (!P.nl) fatal_throw("detect: the network has no yolo / region layer");
     P.total = total; P.netw = net->w; P.neth = net->h; P.relative = relative;
     P.thresh = thresh; P.nms = nms; P.max_rows = max_rows; P.nblk = (total + 255) / 256;
-    (void)e;
     return P;
 }
 
+// pitch == cap == max_rows: the NMS sees exactly the rows the caller asked for
 static void det_ws_ensure(Engine::DetWs &ws, int B, const DetParams &P) {
     const int stride = 5 + P.classes, words = (P.max_rows + 31) / 32;
-    if (ws.cap == P.max_rows && ws.stride == stride && ws.nblk >= P.nblk) return;   // pitch == cap == max_rows: the NMS sees
-                                                                                    // exactly the rows the caller asked for
-    if (ws.rows) cudaFree(ws.rows);
-    if (ws.mask) cudaFree(ws.mask);
-    if (ws.blkcnt) cudaFree(ws.blkcnt);
-    if (ws.counts) cudaFree(ws.counts);
-    CUDA_OK(cudaMalloc(&ws.rows, (size_t)B * P.max_rows * stride * sizeof(float)));
-    CUDA_OK(cudaMalloc(&ws.mask, (size_t)B * P.max_rows * words * sizeof(unsigned)));
-    CUDA_OK(cudaMalloc(&ws.blkcnt, (size_t)B * P.nblk * sizeof(int)));
-    CUDA_OK(cudaMalloc(&ws.counts, (size_t)B * sizeof(int)));
-    ws.cap = P.max_rows; ws.stride = stride; ws.nblk = P.nblk;
+    ws.rows.ensure((size_t)B * P.max_rows * stride);
+    ws.mask.ensure((size_t)B * P.max_rows * words);
+    ws.blkcnt.ensure((size_t)B * P.nblk);
+    ws.counts.ensure(B);
+    ws.cap = P.max_rows; ws.stride = stride;
 }
 
 // decode of the first nimg images; counts[b] = 0 for the others
 static void det_launch_count_emit(const DetParams &P, Engine::DetWs &ws, int B, int nimg, cudaStream_t s) {
-    k_det_count<<<dim3((unsigned)P.nblk, (unsigned)nimg), 256, 0, s>>>(P, ws.blkcnt);
-    k_det_emit<<<dim3((unsigned)P.nblk, (unsigned)nimg), 256, 0, s>>>(P, ws.blkcnt, ws.rows, ws.counts);
-    if (nimg < B) CUDA_OK(cudaMemsetAsync(ws.counts + nimg, 0, (size_t)(B - nimg) * sizeof(int), s));
+    k_det_count<<<dim3((unsigned)P.nblk, (unsigned)nimg), 256, 0, s>>>(P, ws.blkcnt.get());
+    k_det_emit<<<dim3((unsigned)P.nblk, (unsigned)nimg), 256, 0, s>>>(P, ws.blkcnt.get(), ws.rows.get(), ws.counts.get());
+    if (nimg < B) CUDA_OK(cudaMemsetAsync(ws.counts.get() + nimg, 0, (size_t)(B - nimg) * sizeof(int), s));
 }
 // nmax: upper bound of the candidates of any image (the kernels read the true counts on the device and idle beyond them)
 static void det_launch_nms(const DetParams &P, Engine::DetWs &ws, int nimg, int nmax, cudaStream_t s) {
     if (!(P.nms > 0.f) || nmax <= 0) return;
     const int capw = (ws.cap + 31) / 32;
-    k_det_iou<<<dim3((unsigned)((capw + 127) / 128), (unsigned)std::min(nmax, 256), (unsigned)nimg), 128, 0, s>>>(P, ws.rows, ws.counts, ws.mask);
+    k_det_iou<<<dim3((unsigned)((capw + 127) / 128), (unsigned)std::min(nmax, 256), (unsigned)nimg), 128, 0, s>>>(
+        P, ws.rows.get(), ws.counts.get(), ws.mask.get());
     int P2 = 1; while (P2 < nmax) P2 <<= 1;
     const size_t smem = (size_t)P2 * 8 + (size_t)capw * 4;
     if (smem > 48 * 1024)
         CUDA_OK(cudaFuncSetAttribute(k_det_nms, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_det_nms<<<dim3((unsigned)P.classes, (unsigned)nimg), 256, smem, s>>>(P, ws.rows, ws.counts, ws.mask, P2);
+    k_det_nms<<<dim3((unsigned)P.classes, (unsigned)nimg), 256, smem, s>>>(P, ws.rows.get(), ws.counts.get(), ws.mask.get(), P2);
 }
 
 // Synchronous form.  Image b's boxes are corrected for a w[b] x h[b] frame.  rows: [batch][max_rows][5 + classes];
@@ -1604,16 +1536,16 @@ static void det_launch_nms(const DetParams &P, Engine::DetWs &ws, int nimg, int 
 int engine_detect(Engine *e, Network *net, const int *w, const int *h, int nimg, float thresh, float nms, int relative,
                   int letter, float *rows, int max_rows, int *counts) {
     CUDA_OK(cudaSetDevice(e->opt.device));
-    DetParams P = det_params(e, net, e->d_final, thresh, nms, relative, max_rows);
+    DetParams P = det_params(net, e->finals, thresh, nms, relative, max_rows);
     const int B = e->batch, stride = 5 + P.classes;
     det_ws_ensure(e->det, B, P);
     cudaStream_t s = e->stream;
     fill_geo(e, e->u8, net, w, h, nimg, letter);
-    CUDA_OK(cudaMemcpyAsync(e->u8.d_geo, e->u8.h_geo, (size_t)B * sizeof(ImageGeo), cudaMemcpyHostToDevice, s));
-    P.geo = e->u8.d_geo;
+    CUDA_OK(cudaMemcpyAsync(e->u8.d_geo.get(), e->u8.h_geo.get(), (size_t)B * sizeof(ImageGeo), cudaMemcpyHostToDevice, s));
+    P.geo = e->u8.d_geo.get();
     det_launch_count_emit(P, e->det, B, nimg, s);
     std::vector<int> hc(B);
-    CUDA_OK(cudaMemcpyAsync(hc.data(), e->det.counts, B * sizeof(int), cudaMemcpyDeviceToHost, s));
+    CUDA_OK(cudaMemcpyAsync(hc.data(), e->det.counts.get(), B * sizeof(int), cudaMemcpyDeviceToHost, s));
     CUDA_OK(cudaStreamSynchronize(s));
     int nmax = 0;
     for (int b = 0; b < B; ++b) { counts[b] = hc[b]; nmax = std::max(nmax, std::min(hc[b], max_rows)); }
@@ -1621,7 +1553,7 @@ int engine_detect(Engine *e, Network *net, const int *w, const int *h, int nimg,
     for (int b = 0; b < nimg; ++b) {
         const int n = std::min(hc[b], max_rows);
         if (n > 0)
-            CUDA_OK(cudaMemcpyAsync(rows + (size_t)b * max_rows * stride, e->det.rows + (size_t)b * max_rows * stride,
+            CUDA_OK(cudaMemcpyAsync(rows + (size_t)b * max_rows * stride, e->det.rows.get() + (size_t)b * max_rows * stride,
                                     (size_t)n * stride * sizeof(float), cudaMemcpyDeviceToHost, s));
     }
     CUDA_OK(cudaStreamSynchronize(s));
@@ -1640,49 +1572,28 @@ int engine_detect(Engine *e, Network *net, const int *w, const int *h, int nimg,
 // table and either resizes into sl.d_in (returns nullptr) or returns 8-bit frames of the network size for the stem to read.
 static int submit_detections(Engine *e, Network *net, int nimg, float thresh, float nms, int relative, int max_rows,
                              const std::function<const unsigned char *(Engine::Slot &)> &stage) {
-    CUDA_OK(cudaSetDevice(e->opt.device));
-    ensure_slots(e);
-    const int k = e->next_slot;
+    DetParams P = det_params(net, e->finals, thresh, nms, relative, max_rows);
+    const int B = e->batch, stride = 5 + P.classes;
+    const int k = acquire_slot(e);
     Engine::Slot &sl = e->slots[k];
-    if (sl.busy) fatal_throw("submit: pipeline full (3 batches in flight) -- collect the oldest ticket first");
-    const DetParams P0 = det_params(e, net, sl.d_out, thresh, nms, relative, max_rows);
-    const int B = e->batch, stride = 5 + P0.classes;
-    det_ws_ensure(sl.det, B, P0);
-    const size_t rows_bytes = (size_t)B * max_rows * stride * sizeof(float);
-    if (sl.h_rows_bytes < rows_bytes) {
-        if (sl.h_rows) cudaFreeHost(sl.h_rows);
-        CUDA_OK(cudaHostAlloc(&sl.h_rows, rows_bytes, cudaHostAllocDefault));
-        sl.h_rows_bytes = rows_bytes;
-    }
-    if (!sl.h_counts) CUDA_OK(cudaHostAlloc(&sl.h_counts, (size_t)B * sizeof(int), cudaHostAllocDefault));
-    e->next_slot = (k + 1) % (int)e->slots.size();
-    // the previous forward that read d_in[k] must have finished before it is overwritten
-    CUDA_OK(cudaStreamWaitEvent(e->s_in, sl.ev_comp, 0));
+    det_ws_ensure(sl.det, B, P);
+    sl.h_rows.ensure((size_t)B * max_rows * stride);
+    sl.h_counts.ensure(B);
     // The slot's frames and geometry table go on s_in.  The decode below reads the table on the compute stream behind ev_in,
-    // and the next submit to this slot rewrites it only after waiting for ev_comp (above) -- and only once this ticket has
-    // been collected, which waits for ev_det, so the pinned host table is no longer being copied either.
-    const unsigned char *direct = stage(sl);
-    CUDA_OK(cudaEventRecord(sl.ev_in, e->s_in));
-    CUDA_OK(cudaStreamWaitEvent(e->stream, sl.ev_in, 0));
-    engine_forward_impl(e, sl.d_in, direct, e->stream);
+    // and the next submit to this slot rewrites it only after waiting for ev_comp (acquire_slot) -- and only once this ticket
+    // has been collected, which waits for ev_det, so the pinned host table is no longer being copied either.
+    forward_slot(e, sl, stage(sl));
     // Candidate selection + box decode (k_det_count / k_det_emit: they read the objectness planes and, for the few candidates,
     // their class scores) run right behind the forward on the compute stream, straight on the engine's yolo tensors -- the next
     // forward overwrites those, so this is the only part that must not slip.  What follows (IoU matrix + per-class NMS) works on
     // the slot's own candidate rows and goes to the side stream, where it overlaps the next batch's forward.  (Copying the
     // 124 MB of yolo tensors into the slot first, as the raw-tensor path does, cost more than the decode itself.)
-    CUDA_OK(cudaStreamWaitEvent(e->stream, sl.ev_det, 0));     // the slot's previous NMS / counts copy are done with its workspace
-    DetParams P1 = P0;
-    P1.geo = sl.u8.d_geo;
-    {
-        int k2 = 0;
-        for (size_t i = 0; i < net->layers.size(); ++i)
-            if (net->layers[i].type == YB_YOLO || net->layers[i].type == YB_REGION) P1.L[k2++].p = e->d_final[i];
-    }
-    det_launch_count_emit(P1, sl.det, B, nimg, e->stream);
+    P.geo = sl.u8.d_geo.get();
+    det_launch_count_emit(P, sl.det, B, nimg, e->stream);
     CUDA_OK(cudaEventRecord(sl.ev_comp, e->stream));
     CUDA_OK(cudaStreamWaitEvent(e->s_det, sl.ev_comp, 0));
-    CUDA_OK(cudaMemcpyAsync(sl.h_counts, sl.det.counts, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, e->s_det));
-    det_launch_nms(P0, sl.det, nimg, max_rows, e->s_det);   // no host round trip: grids sized for the cap, kernels read the counts
+    CUDA_OK(cudaMemcpyAsync(sl.h_counts.get(), sl.det.counts.get(), (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, e->s_det));
+    det_launch_nms(P, sl.det, nimg, max_rows, e->s_det);   // no host round trip: grids sized for the cap, kernels read the counts
     CUDA_OK(cudaEventRecord(sl.ev_det, e->s_det));
     CUDA_OK(cudaGetLastError());
     sl.busy = true; sl.mode = 1; sl.nimg = nimg;
@@ -1695,10 +1606,10 @@ int engine_submit_frames(Engine *e, Network *net, const unsigned char *const *fr
         const bool net_size = stage_frames(e, sl.u8, net, frames, w, h, nimg, letter, e->s_in);
         if (e->first_op_u8 && net_size && net->c == 3) {   // frames of the network size: no staging
             const size_t frame = (size_t)net->w * net->h * net->c;
-            if (nimg < e->batch) CUDA_OK(cudaMemsetAsync(sl.u8.buf + nimg * frame, 0, (e->batch - nimg) * frame, e->s_in));
-            return sl.u8.buf;
+            if (nimg < e->batch) CUDA_OK(cudaMemsetAsync(sl.u8.buf.get() + nimg * frame, 0, (e->batch - nimg) * frame, e->s_in));
+            return sl.u8.buf.get();
         }
-        launch_resize(e, sl.u8, net, nimg, YB_FRAME_RGB, sl.d_in, e->s_in);
+        launch_resize(e, sl.u8, net, nimg, YB_FRAME_RGB, sl.d_in.get(), e->s_in);
         return nullptr;
     });
 }
@@ -1706,7 +1617,7 @@ int engine_submit_frames(Engine *e, Network *net, const unsigned char *const *fr
 int engine_submit_device_frames(Engine *e, Network *net, const yb_device_frame *frames, int nimg, int fmt, float thresh,
                                 float nms, int relative, int letter, int max_rows, void *stream) {
     return submit_detections(e, net, nimg, thresh, nms, relative, max_rows, [&](Engine::Slot &sl) -> const unsigned char * {
-        resize_device_frames(e, sl.u8, net, frames, nimg, fmt, letter, sl.d_in, e->s_in, (cudaStream_t)stream);
+        resize_device_frames(e, sl.u8, net, frames, nimg, fmt, letter, sl.d_in.get(), e->s_in, (cudaStream_t)stream);
         return nullptr;
     });
 }
@@ -1714,26 +1625,21 @@ int engine_submit_device_frames(Engine *e, Network *net, const yb_device_frame *
 // rows: pinned [batch][max_rows][5 + classes] (valid until the slot is reused), counts[batch] (0 beyond the ticket's images);
 // returns 5 + classes.
 int engine_collect_detections(Engine *e, int ticket, const float **rows, const int **counts, size_t *d2h_bytes) {
-    if (ticket < 0 || ticket >= (int)e->slots.size() || !e->slots[ticket].busy || e->slots[ticket].mode != 1)
-        fatal_throw("collect_detections: bad ticket");
-    CUDA_OK(cudaSetDevice(e->opt.device));
-    Engine::Slot &sl = e->slots[ticket];
-    CUDA_OK(cudaEventSynchronize(sl.ev_det));
+    const Engine::Slot &sl = release_slot(e, ticket, 1, "collect_detections");
     const int B = e->batch, cap = sl.det.cap, stride = sl.det.stride;
     size_t moved = (size_t)B * sizeof(int);
     for (int b = 0; b < sl.nimg; ++b) {
-        const int n = std::min(sl.h_counts[b], cap);
+        const int n = std::min(sl.h_counts.get()[b], cap);
         if (n > 0) {
-            CUDA_OK(cudaMemcpyAsync(sl.h_rows + (size_t)b * cap * stride, sl.det.rows + (size_t)b * cap * stride,
+            CUDA_OK(cudaMemcpyAsync(sl.h_rows.get() + (size_t)b * cap * stride, sl.det.rows.get() + (size_t)b * cap * stride,
                                     (size_t)n * stride * sizeof(float), cudaMemcpyDeviceToHost, e->s_out));
             moved += (size_t)n * stride * sizeof(float);
         }
     }
     CUDA_OK(cudaStreamSynchronize(e->s_out));
-    if (rows) *rows = sl.h_rows;
-    if (counts) *counts = sl.h_counts;
+    if (rows) *rows = sl.h_rows.get();
+    if (counts) *counts = sl.h_counts.get();
     if (d2h_bytes) *d2h_bytes = moved;
-    sl.busy = false;
     return stride;
 }
 
@@ -1741,29 +1647,29 @@ int engine_num_launches(Engine *e) { return (int)e->ops.size(); }
 long engine_info(Engine *e, const char *key) {
     if (!strcmp(key, "launches")) return (long)e->ops.size();
     if (!strcmp(key, "tc_layers")) return e->n_tc;
-    if (!strcmp(key, "act_bytes")) return (long)e->act_bytes;
+    if (!strcmp(key, "act_bytes")) return (long)e->act_arena.count();
     return -1;
 }
 
 int engine_tc_plan(Engine *e, int layer, int *fields, int n) {
-    for (size_t k = 0; k < e->tc_plans.size(); ++k)
-        if (e->tc_plan_layer[k] == layer) return tc_plan_fields(e->tc_plans[k], fields, n);
+    for (const auto &[plan_layer, plan] : e->tc_plans)
+        if (plan_layer == layer) return tc_plan_fields(*plan, fields, n);
     // the stem plan runs layer 0, and layer 1 too when k_stem_s2_tc fuses it
-    if (e->stem_plan && (layer == 0 || layer == e->first_layer)) return tc_stem_plan_fields(e->stem_plan, fields, n);
+    if (e->stem_plan && (layer == 0 || layer == e->first_layer)) return tc_stem_plan_fields(*e->stem_plan, fields, n);
     return 0;
 }
 
 int engine_profile(Engine *e, const void *d_input, int *layer_idx, int *op_kind, float *ms, int max) {
     CUDA_OK(cudaSetDevice(e->opt.device));
     cudaStream_t s = e->stream;
-    const float *din = d_input ? reinterpret_cast<const float *>(d_input) : e->d_input;
+    const float *din = d_input ? reinterpret_cast<const float *>(d_input) : e->d_input.get();
     const int n = (int)e->ops.size();
-    std::vector<cudaEvent_t> ev(n + 1);
-    for (auto &x : ev) CUDA_OK(cudaEventCreate(&x));
+    std::vector<Event> ev;
+    for (int k = 0; k <= n; ++k) ev.push_back(make_event(cudaEventDefault));
     for (int rep = 0; rep < 2; ++rep) {   // second pass is the measured one
         CUDA_OK(cudaEventRecord(ev[0], s));
         for (int k = 0; k < n; ++k) {
-            if (k == 0) launch_input(e, din, s);
+            if (k == 0) e->first_op(din, s);
             else e->ops[k].launch(s);
             CUDA_OK(cudaEventRecord(ev[k + 1], s));
         }
@@ -1774,7 +1680,6 @@ int engine_profile(Engine *e, const void *d_input, int *layer_idx, int *op_kind,
         op_kind[k] = e->ops[k].kind;
         CUDA_OK(cudaEventElapsedTime(&ms[k], ev[k], ev[k + 1]));
     }
-    for (auto &x : ev) cudaEventDestroy(x);
     return n;
 }
 
