@@ -50,6 +50,19 @@ constexpr int TC_THREADS = 32 * TC_EPI_WARPS + 32;
 constexpr int TC_PRODUCER_WARP = TC_EPI_WARPS;
 constexpr int TC_ACC_BAR = 3;                // named barrier of the 256 consumer threads (1, 2: the TMA-epilogue groups)
 
+// Where the regions of a plan's dynamic shared memory lie: byte offsets from the kernel's 1024-byte aligned base, placed by
+// tc_smem_layout.  The resident filter matrix (bstat_bytes) starts at offset 0.
+struct TcSmem {
+    uint32_t ring;                  // operand ring: stages x stage_bytes
+    uint32_t full, empty;           // mbarriers per ring stage: its K-blocks have landed / the consumers are done with them
+    uint32_t bstat_bar;             // mbarrier: the resident filter matrix has landed
+    uint32_t stg_full, stg_ready;   // k_conv_tc_reg's mbarriers per consumer warpgroup g: stg_full[g][slab], stg_ready[g]
+    uint32_t bias;                  // f32 bias of all nt * BN filters
+    uint32_t ymask;                 // k_conv_tc: fused [yolo] mask, one bit per filter
+    uint32_t stg;                   // epilogue staging or TMA-epilogue tiles (stg_bytes)
+    uint32_t acc;                   // k_conv_tc: [128][acc_pitch] 32-bit accumulator tile
+};
+
 struct TcParams {
     int N;                    // images
     int TW, TWlog2, TH;       // tile = TW x TH output pixels (TW*TH == 128)
@@ -92,6 +105,7 @@ struct TcParams {
     float pool_mult;
     signed char *pool_out; long pool_ldc; int pool_Hp, pool_Wp;   // next layer's s8 input: padded NHWC, bytes
     int sps;                                  // K-blocks per pipeline stage (amortises the per-stage barrier round trip)
+    TcSmem sm;
     uint32_t desc_hi;         // high word of the wgmma shared-memory descriptors (SBO, swizzle mode)
     char *out; long out_ldc; int n;
     const char *res;          // fused shortcut operand (bf16, k_conv_tc_reg at stride 1 only), or null
@@ -329,15 +343,18 @@ __device__ __forceinline__ void acc_store_frag(uint32_t acc, int pitch, int row0
     }
 }
 
-// Shared-memory barriers of both kernels: full[stages], empty[stages], then the resident-filter barrier.
-__device__ __forceinline__ uint32_t full_bar(uint32_t bars, int s) { return bars + 8u * (uint32_t)s; }
-__device__ __forceinline__ uint32_t empty_bar(uint32_t bars, int stages, int s) { return bars + 8u * (uint32_t)(stages + s); }
+// The aligned base of the dynamic shared memory: 128B swizzle atoms are 1024-byte aligned.  Every region lies at an offset
+// from it (TcParams::sm).
+__device__ __forceinline__ uint32_t smem_base(const void *smem_raw) { return (smem_u32(smem_raw) + 1023u) & ~1023u; }
+__device__ __forceinline__ void *smem_ptr(uint32_t addr) { return __cvta_shared_to_generic(addr); }
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
 
-// TMA producer (one elected thread): walks the consumers' work items and keeps the ring full.  smemB: resident filter matrix
-// (p.bstat), smem0: the ring.
+// TMA producer (one elected thread): walks the consumers' work items and keeps the ring full (base: the aligned shared memory)
 template <bool ST>
-__device__ __forceinline__ void tc_produce(const CUtensorMap *tmA, const CUtensorMap *tmB, const TcParams &p, uint32_t smemB,
-                                           uint32_t smem0, uint32_t bars, int w_first, int w_step) {
+__device__ __forceinline__ void tc_produce(const CUtensorMap *tmA, const CUtensorMap *tmB, const TcParams &p, uint32_t base,
+                                           int w_first, int w_step) {
     int stage = 0; uint32_t phase = 0;
     long long w_empty = 0, w_tma = 0; const long long t_begin = ST ? clock64() : 0;
     // loop-invariant parameters in registers; the (tap, channel-block) walk is incremental (no integer divisions per
@@ -346,7 +363,7 @@ __device__ __forceinline__ void tc_produce(const CUtensorMap *tmA, const CUtenso
     const int xoff = p.xoff, yoff = p.yoff, stride2 = p.stride2, nt = p.nt, xt = p.xt;
     const uint32_t a_bytes = p.a_bytes, b_bytes = p.b_bytes, stage_bytes = p.stage_bytes;
     const uint32_t b_off = (uint32_t)sps * a_bytes;
-    const uint32_t bstat_bar = bars + 16u * (uint32_t)stages;
+    const uint32_t smemB = base, smem0 = base + p.sm.ring, bstat_bar = base + p.sm.bstat_bar;
     const int bstat = p.bstat;
     if (bstat) {   // resident filter matrix: kblocks boxes of [BN filters][BK], once
         mbar_arrive_expect_tx(bstat_bar, p.bstat_bytes);
@@ -362,9 +379,9 @@ __device__ __forceinline__ void tc_produce(const CUtensorMap *tmA, const CUtenso
         int cb = 0, ky = 0, kx = 0, kcol = 0;
         for (int kb0 = 0; kb0 < kblocks; kb0 += sps) {
             const int nsub = min(sps, kblocks - kb0);
-            if constexpr (ST) { const long long c0 = clock64(); mbar_wait(empty_bar(bars, stages, stage), phase ^ 1u); w_empty += clock64() - c0; }
-            else mbar_wait(empty_bar(bars, stages, stage), phase ^ 1u);
-            const uint32_t fb = full_bar(bars, stage);
+            if constexpr (ST) { const long long c0 = clock64(); mbar_wait(base + p.sm.empty + 8u * (uint32_t)stage, phase ^ 1u); w_empty += clock64() - c0; }
+            else mbar_wait(base + p.sm.empty + 8u * (uint32_t)stage, phase ^ 1u);
+            const uint32_t fb = base + p.sm.full + 8u * (uint32_t)stage;
             const uint32_t a_dst = smem0 + (uint32_t)stage * stage_bytes;
             const uint32_t b_dst = a_dst + b_off;
             if (p.dbg & 1) {
@@ -396,22 +413,24 @@ __device__ __forceinline__ void tc_produce(const CUtensorMap *tmA, const CUtenso
 // accumulators while wgmmas are in flight, and every batch is the same KK wgmmas: ptxas then inserts no fences of its own
 // and serializes nothing (the -Xptxas -v log has no C75xx notes).
 template <int KIND, int BN, int KK, bool ST, typename T>
-__device__ __forceinline__ void tc_mma_loop(T (&d)[BN / 2], const TcParams &p, uint32_t smemB, uint32_t smem0, uint32_t bars,
-                                            int wg, int lane, int &stage, uint32_t &phase, long long &w_full) {
+__device__ __forceinline__ void tc_mma_loop(T (&d)[BN / 2], const TcParams &p, uint32_t base, int wg, int lane, int &stage,
+                                            uint32_t &phase, long long &w_full) {
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) d[i] = T(0);
     wg_fence_operand(d);
     const int sps = p.sps, stages = p.stages, kblocks = p.kblocks;
     const uint32_t a_bytes = p.a_bytes, b_bytes = p.b_bytes, stage_bytes = p.stage_bytes, hi = p.desc_hi;
     const uint32_t b_off = (uint32_t)sps * a_bytes, a_wg = (uint32_t)wg * (a_bytes >> 1);
-    auto release = [&](int s) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar(bars, stages, s)); };
+    const uint32_t smemB = base, smem0 = base + p.sm.ring;   // resident filter matrix, ring
+    const uint32_t full = base + p.sm.full, empty = base + p.sm.empty;   // the ring's mbarriers, 8 bytes per stage
+    auto release = [&](int s) { __syncwarp(); if (lane == 0) mbar_arrive(empty + 8u * (uint32_t)s); };
     // one commit group per K-block; a stage (sps K-blocks, fewer at the end of the work item) is released once the group of
     // its last K-block has retired, which wgmma.wait_group 1 shows one K-block later
     int pend = -1, jj = 0;
     for (int kb = 0; kb < kblocks; ++kb) {
         if (jj == 0) {
-            if constexpr (ST) { const long long c0 = clock64(); mbar_wait(full_bar(bars, stage), phase); w_full += clock64() - c0; }
-            else mbar_wait(full_bar(bars, stage), phase);
+            if constexpr (ST) { const long long c0 = clock64(); mbar_wait(full + 8u * (uint32_t)stage, phase); w_full += clock64() - c0; }
+            else mbar_wait(full + 8u * (uint32_t)stage, phase);
         }
         const uint32_t st_base = smem0 + (uint32_t)stage * stage_bytes;
         const uint32_t a_kb = st_base + a_wg + (uint32_t)jj * a_bytes;
@@ -456,16 +475,14 @@ __device__ __forceinline__ float int_epilogue(const TcParams &p, int kind, int a
 // contain no clock64() reads.
 // EPI: which epilogue family is compiled in -- 0: LSU stores, float kinds (f32 heads / fused [yolo]); 2: the integer
 // kinds (s8 requantising and XNOR-as-+-1 epilogues).  The bf16-output layers run k_conv_tc_reg.
+// tmO1, tmR: unused (the parameter list of k_conv_tc_reg, so that a plan launches either kernel the same way).
 template <bool ST, int EPI>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
-          const TcParams p) {
+          const __grid_constant__ CUtensorMap tmO1, const __grid_constant__ CUtensorMap tmR, const TcParams p) {
     extern __shared__ uint8_t smem_raw[];
-    const uint32_t smemB = (smem_u32(smem_raw) + 1023u) & ~1023u;   // 128B swizzle atoms are 1024B aligned
-    const uint32_t smem0 = smemB + p.bstat_bytes;                   // [resident filter matrix][pipeline ring]
-    const uint32_t bars = smem0 + (uint32_t)p.stages * p.stage_bytes;
-    const uint32_t bstat_bar = bars + 8u * (uint32_t)(2 * p.stages);
-    const uint32_t misc = (bstat_bar + 24u + 15u) & ~15u;
+    const uint32_t base = smem_base(smem_raw);
+    const uint32_t bstat_bar = base + p.sm.bstat_bar;
 
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
     const int lane = threadIdx.x & 31;
@@ -475,25 +492,26 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
         // full: one arrival (the producer's expect_tx); empty: one arrival per consumer warp
-        for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar(bars, s), 1); mbar_init(empty_bar(bars, p.stages, s), TC_EPI_WARPS); }
+        for (int s = 0; s < p.stages; ++s) { mbar_init(base + p.sm.full + 8u * s, 1); mbar_init(base + p.sm.empty + 8u * s, TC_EPI_WARPS); }
         mbar_init(bstat_bar, 1);
         if (p.tma_epi) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmO) : "memory");
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     // bias (folded batch-norm) for all filter tiles -> shared memory, once per CTA
-    float *bias_s = reinterpret_cast<float *>(smem_raw + (misc - smem_u32(smem_raw)));
+    const float *bias_s = reinterpret_cast<const float *>(smem_ptr(base + p.sm.bias));
     // fused [yolo]: one bit per filter, set where the entry is a box width/height (no logistic)
-    uint32_t *ymask_s = reinterpret_cast<uint32_t *>(bias_s + p.nt * p.BN);
+    const uint32_t *ymask_s = reinterpret_cast<const uint32_t *>(smem_ptr(base + p.sm.ymask));
     // 4 KB of staging per epilogue warp (32 rows x 128 B, XOR-swizzled) for the coalescing transposes, or the TMA-epilogue tiles
-    const uint32_t stg_align = p.tma_epi ? 1023u : 127u;     // TMA epilogue tiles are swizzled: 1024-byte aligned
-    const uint32_t stg_base = ((misc + 4u * (uint32_t)(p.nt * p.BN) + (uint32_t)(p.nt * p.BN / 8)) + stg_align) & ~stg_align;
-    const uint32_t acc_base = stg_base + p.stg_bytes;        // [128 rows][acc_pitch] 32-bit accumulators of the current tile
-    for (int i = threadIdx.x; i < p.nt * p.BN; i += TC_THREADS) bias_s[i] = (i < p.n) ? __ldg(p.bias + i) : 0.f;
+    const uint32_t stg_base = base + p.sm.stg;
+    const uint32_t acc_base = base + p.sm.acc;               // [128 rows][acc_pitch] 32-bit accumulators of the current tile
+    // (filled through shared-window addresses: EPI 2 spills more when the generic pointers are live from here on)
+    for (int i = threadIdx.x; i < p.nt * p.BN; i += TC_THREADS)
+        st_shared_u32(base + p.sm.bias + 4u * (uint32_t)i, __float_as_uint((i < p.n) ? __ldg(p.bias + i) : 0.f));
     if (p.yolo_out) {
         for (int wd = threadIdx.x; wd < p.nt * p.BN / 32; wd += TC_THREADS) {
             uint32_t m = 0;
             for (int j = 0; j < 32; ++j) { const int e = (wd * 32 + j) % p.yolo_per; if (e == 2 || e == 3) m |= 1u << j; }
-            ymask_s[wd] = m;
+            st_shared_u32(base + p.sm.ymask + 4u * (uint32_t)wd, m);
         }
     }
     __syncthreads();
@@ -504,7 +522,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
 
     if (warp == TC_PRODUCER_WARP) {
         // ======================= TMA producer =======================
-        if (elect_one()) tc_produce<ST>(&tmA, &tmB, p, smemB, smem0, bars, w_first, w_step);
+        if (elect_one()) tc_produce<ST>(&tmA, &tmB, p, base, w_first, w_step);
     } else {
         // ======================= consumers (warps 0..7): wgmma main loop, then the epilogue of the same tile =======================
         const int ew = warp;                      // consumer warp; warpgroup ew >> 2 computes accumulator rows 64 * (ew >> 2) .. + 63
@@ -520,7 +538,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
             constexpr int KK = decltype(kk_c)::value;   // wgmmas per K-block
             using T = typename std::conditional<KIND == 1 || KIND == 2, uint32_t, float>::type;
             T d[BN / 2];
-            tc_mma_loop<KIND, BN, KK, ST>(d, p, smemB, smem0, bars, wg, lane, stage, phase, w_full);
+            tc_mma_loop<KIND, BN, KK, ST>(d, p, base, wg, lane, stage, phase, w_full);
             named_bar_sync(TC_ACC_BAR, 32 * TC_EPI_WARPS);   // every warp is done with the previous tile's accumulators
             acc_store_frag(acc_base, p.acc_pitch, wg * 64, d);
             named_bar_sync(TC_ACC_BAR, 32 * TC_EPI_WARPS);   // the whole 128 x BN tile is in place
@@ -865,17 +883,14 @@ __global__ void __launch_bounds__(TCR_THREADS, 1)
 k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
               const __grid_constant__ CUtensorMap tmO1, const __grid_constant__ CUtensorMap tmR, const TcParams p) {
     extern __shared__ uint8_t smem_raw[];
-    const uint32_t smemB = (smem_u32(smem_raw) + 1023u) & ~1023u;   // [resident filter matrix][pipeline ring][barriers][bias][staging]
-    const uint32_t smem0 = smemB + p.bstat_bytes;
-    const uint32_t bars = smem0 + (uint32_t)p.stages * p.stage_bytes;
-    const uint32_t bstat_bar = bars + 8u * (uint32_t)(2 * p.stages);
-    // per consumer warpgroup g: stg_full for each of up to TCR_MAX_SLABS slabs, then stg_ready
-    auto stg_full = [&](int g, int s) { return bstat_bar + 8u + 8u * (uint32_t)(g * TCR_MAX_SLABS + s); };
-    auto stg_ready = [&](int g) { return bstat_bar + 8u + 8u * (uint32_t)(2 * TCR_MAX_SLABS + g); };
-    const uint32_t misc = (bstat_bar + 8u * (uint32_t)(2 * TCR_MAX_SLABS + 3) + 15u) & ~15u;
-    float *bias_s = reinterpret_cast<float *>(smem_raw + (misc - smem_u32(smem_raw)));
-    // staging buffers of warpgroups 0 and 1, 64 * BN bf16 each (1024-byte aligned for the swizzle)
-    const uint32_t stg_base = (misc + 4u * (uint32_t)(p.nt * p.BN) + (uint32_t)(p.nt * p.BN / 8) + 1023u) & ~1023u;
+    const uint32_t base = smem_base(smem_raw);
+    const uint32_t bstat_bar = base + p.sm.bstat_bar;
+    // per consumer warpgroup g: stg_full for each of up to TCR_MAX_SLABS slabs, and stg_ready
+    auto stg_full = [&](int g, int s) { return base + p.sm.stg_full + 8u * (uint32_t)(g * TCR_MAX_SLABS + s); };
+    auto stg_ready = [&](int g) { return base + p.sm.stg_ready + 8u * (uint32_t)g; };
+    float *bias_s = reinterpret_cast<float *>(smem_ptr(base + p.sm.bias));
+    // staging buffers of warpgroups 0 and 1, 64 * BN bf16 each
+    const uint32_t stg_base = base + p.sm.stg;
 
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
     const int lane = threadIdx.x & 31;
@@ -889,7 +904,7 @@ k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmO) : "memory");
         if (p.stride2) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmO1) : "memory");
         if (p.res) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmR) : "memory");
-        for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar(bars, s), 1); mbar_init(empty_bar(bars, p.stages, s), TC_EPI_WARPS); }
+        for (int s = 0; s < p.stages; ++s) { mbar_init(base + p.sm.full + 8u * s, 1); mbar_init(base + p.sm.empty + 8u * s, TC_EPI_WARPS); }
         mbar_init(bstat_bar, 1);
         for (int g = 0; g < 2; ++g) {
             for (int s = 0; s < TCR_MAX_SLABS; ++s) mbar_init(stg_full(g, s), 4);
@@ -906,7 +921,7 @@ k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     if (wg == 2) {
         asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(TCR_PRODUCER_REGS));
         if (warp == 8) {
-            if (elect_one()) tc_produce<ST>(&tmA, &tmB, p, smemB, smem0, bars, w_first, w_step);
+            if (elect_one()) tc_produce<ST>(&tmA, &tmB, p, base, w_first, w_step);
         } else if (warp < TCR_STORE_WARP + 2 && epi_mem) {
             const int g = warp - TCR_STORE_WARP;
             if (elect_one()) tcr_store<ST>(&tmO, &tmO1, &tmR, p, stg_base + (uint32_t)g * 128u * (uint32_t)p.BN, stg_full(g, 0), stg_ready(g), g, w_first, w_step);
@@ -940,7 +955,7 @@ k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
         };
         for (int w = w_first; w < p.num_work; w += w_step) {
             float d[BN / 2];
-            tc_mma_loop<0, BN, KK, ST>(d, p, smemB, smem0, bars, wg, lane, stage, phase, w_full);
+            tc_mma_loop<0, BN, KK, ST>(d, p, base, wg, lane, stage, phase, w_full);
             if (!epi_mem) continue;
             const int n0 = (w % p.nt) * BN, m = w / p.nt;
             const int x0 = (m % p.xt) * p.TW, J0 = (m / p.xt) * p.TH + p.jshift;
@@ -1467,12 +1482,16 @@ EncodeTiledFn encode_fn() {
 
 }  // namespace
 
+// Both kernel families take the same parameters
+using TcKernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, TcParams);
+
 struct TcPlan {
     CUtensorMap tmA, tmB, tmO, tmO1, tmR;   // activation, filters; TMA epilogue: output, its one-row view (stride 2), residual
     TcParams p;
+    TcKernel kernel;                  // the instantiation the plan runs
+    bool reg;                         // kernel is a k_conv_tc_reg (TCR_THREADS), else a k_conv_tc (TC_THREADS)
     int grid;
-    int threads;                      // TC_THREADS (k_conv_tc) or TCR_THREADS (k_conv_tc_reg)
-    size_t smem;
+    size_t smem;                      // dynamic shared memory per CTA (tc_smem_layout)
     char desc[96];
     DevBuf<unsigned long long> stats;   // p.stats (YB_TC_STATS)
 };
@@ -1620,22 +1639,69 @@ void plan_epilogue(TcParams &p, const TcConv &c, bool reg) {
     p.pool_Hp = c.pool_next.Hp; p.pool_Wp = c.pool_next.Wp;
 }
 
-// The operand ring: K-blocks per stage and stages, in what is left of 227 KB beside the epilogue's tiles (acc_bytes: k_conv_tc's
-// accumulator tile)
-void plan_ring(TcParams &p, size_t acc_bytes) {
-    // 5 KB: barriers, alignment slack
-    const size_t ring_budget = (size_t)(227 - 5) * 1024 - p.stg_bytes - acc_bytes;
+// Sizes of the epilogue's regions of shared memory (see tc_smem_layout).  reg: k_conv_tc_reg runs the plan.
+struct TcEpiBytes {
+    size_t bias, ymask, stg, acc;
+    size_t sum() const { return bias + ymask + stg + acc; }
+};
+TcEpiBytes epi_bytes(const TcParams &p, bool reg) {
+    const size_t f = (size_t)p.nt * p.BN;
+    return {sizeof(float) * f,                                     // f32 bias of every filter tile
+            reg ? 0 : f / 8,                                       // k_conv_tc's fused [yolo] mask: one bit per filter
+            p.stg_bytes,                                           // epilogue staging or TMA-epilogue tiles
+            reg ? 0 : (size_t)TC_BM * p.acc_pitch * sizeof(float)};   // k_conv_tc's accumulator tile (k_conv_tc_reg: registers)
+}
+
+// The operand ring: K-blocks per stage and stages, in what is left of 222 KB beside the resident filter matrix and the epilogue's
+// regions.  The other 5 KB of the 227 KB cover the barriers and the alignment padding of tc_smem_layout.
+void plan_ring(TcParams &p, bool reg) {
+    const size_t ring_budget = (size_t)(227 - 5) * 1024 - epi_bytes(p, reg).sum();
     // several K-blocks per stage when they are small: fewer barrier round trips per K
     const uint32_t ring_blk = p.a_bytes + (p.bstat ? 0u : p.b_bytes);
     p.sps = (int)std::max<uint32_t>(1, std::min<uint32_t>(4, 32u * 1024u / std::max(ring_blk, 1u)));
     p.sps = std::min(p.sps, p.kblocks);
-    const size_t fixed_smem = sizeof(float) * (size_t)p.nt * p.BN + (size_t)p.nt * p.BN / 8;
-    if (ring_budget < p.bstat_bytes + fixed_smem + 2 * (size_t)ring_blk) fatal_throw("tc plan: tile does not fit shared memory");
-    const size_t avail = ring_budget - p.bstat_bytes - fixed_smem;
+    if (ring_budget < p.bstat_bytes + 2 * (size_t)ring_blk) fatal_throw("tc plan: tile does not fit shared memory");
+    const size_t avail = ring_budget - p.bstat_bytes;
     while (p.sps > 1 && avail / ((size_t)p.sps * ring_blk) < 3) --p.sps;   // keep the ring at least 3 stages deep
     p.stage_bytes = (uint32_t)p.sps * ring_blk;
     p.stages = (int)std::min<size_t>(8, avail / p.stage_bytes);
     if (p.stages < 2) fatal_throw("tc plan: tile does not fit shared memory");
+}
+
+// The dynamic shared memory of a plan whose sizes are decided: places every region (TcParams::sm) at its alignment, in this
+// order, and returns the bytes the launch asks for -- the regions plus 1024 bytes of slack for aligning the kernel's base.
+//   resident filter matrix   bstat_bytes                  1024 (128B swizzle atoms)
+//   operand ring             stages x stage_bytes         1024
+//   mbarriers                full[stages], empty[stages], the resident-filter barrier; k_conv_tc_reg:
+//                            stg_full[2][TCR_MAX_SLABS], stg_ready[2]            8
+//   bias, [yolo] mask        epi_bytes                    16, 4
+//   staging                  stg_bytes                    1024 with the TMA epilogue (swizzled tiles), else 128
+//   accumulator tile         epi_bytes                    16
+size_t tc_smem_layout(TcParams &p, bool reg) {
+    const TcEpiBytes epi = epi_bytes(p, reg);
+    size_t top = 0;
+    auto place = [&](size_t bytes, size_t align) {
+        const size_t off = (top + align - 1) / align * align;
+        top = off + bytes;
+        return (uint32_t)off;
+    };
+    // the A and B boxes of every ring stage, and the filter matrix's boxes, are swizzled tiles: they keep the 1024-byte alignment
+    if (p.a_bytes % 1024 || p.b_bytes % 1024) fatal_throw("tc plan: operand tiles break the 1024-byte swizzle alignment");
+    place(p.bstat_bytes, 1024);
+    p.sm.ring = place((size_t)p.stages * p.stage_bytes, 1024);
+    const int nbars = 2 * p.stages + 1 + (reg ? 2 * TCR_MAX_SLABS + 2 : 0);
+    p.sm.full = place(8 * (size_t)nbars, 8);
+    p.sm.empty = p.sm.full + 8u * (uint32_t)p.stages;
+    p.sm.bstat_bar = p.sm.empty + 8u * (uint32_t)p.stages;
+    p.sm.stg_full = reg ? p.sm.bstat_bar + 8u : 0u;
+    p.sm.stg_ready = reg ? p.sm.stg_full + 8u * 2u * TCR_MAX_SLABS : 0u;
+    p.sm.bias = place(epi.bias, 16);
+    p.sm.ymask = reg ? 0u : place(epi.ymask, 4);
+    p.sm.stg = place(epi.stg, p.tma_epi ? 1024 : 128);
+    p.sm.acc = reg ? 0u : place(epi.acc, 16);
+    const size_t smem = 1024 + top;
+    if (smem > 227 * 1024) fatal_throw("tc plan: shared memory budget exceeded");
+    return smem;
 }
 
 // The tensor maps: activation boxes of a K-block, filter boxes and, for the TMA epilogue, the output and residual slabs
@@ -1734,24 +1800,22 @@ TcPlanPtr tc_make_plan(const TcConv &c) {
     const int sms = sm_count();
     plan_tiles(p, c, reg, sms);
     plan_epilogue(p, c, reg);
-    const size_t acc_bytes = reg ? 0 : (size_t)TC_BM * p.acc_pitch * 4;   // k_conv_tc_reg keeps the accumulators in registers
-    plan_ring(p, acc_bytes);
+    plan_ring(p, reg);
+    plan->smem = tc_smem_layout(p, reg);
     p.dbg = getenv("YB_TC_DBG") ? atoi(getenv("YB_TC_DBG")) : 0;
     snprintf(plan->desc, sizeof(plan->desc), "%dx%dx%d -> n%d k%d s%d%s", l.c, l.h, l.w, l.n, l.size, l.stride, reg ? " reg" : "");
     encode_maps(*plan, c, reg);
     plan->grid = std::min(p.num_work, grid_cap(sms));
-    plan->threads = reg ? TCR_THREADS : TC_THREADS;
-    // barriers: full / empty per stage, the resident-filter barrier, k_conv_tc_reg's stg_full / stg_ready per consumer warpgroup
-    plan->smem = 1024 /*alignment slack*/ + p.bstat_bytes + (size_t)p.stages * p.stage_bytes + 8 * (2 * p.stages + 11) + 16 +
-                 sizeof(float) * (size_t)p.nt * p.BN /*bias*/ + (size_t)p.nt * p.BN / 8 /*yolo mask*/ +
-                 (p.tma_epi ? 1024 : 128) + p.stg_bytes /*epilogue staging or TMA-epilogue tiles*/ +
-                 acc_bytes /*accumulator tile*/;
-    if (plan->smem > 227 * 1024) fatal_throw("tc plan: shared memory budget exceeded");
-    for (const void *f : {(const void *)k_conv_tc<false, 0>, (const void *)k_conv_tc_reg<false>, (const void *)k_conv_tc<false, 2>,
-                          (const void *)k_conv_tc<true, 0>, (const void *)k_conv_tc_reg<true>, (const void *)k_conv_tc<true, 2>})
-        if (cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
-            fatal_throw("cudaFuncSetAttribute(k_conv_tc) failed");
-    if (getenv("YB_TC_STATS")) {
+    // the integer kinds compile EPI 2, the float kinds EPI 0; YB_TC_STATS=1 runs the role-counter instantiations
+    const bool st = getenv("YB_TC_STATS") != nullptr;
+    plan->reg = reg;
+    if (reg) plan->kernel = st ? k_conv_tc_reg<true> : k_conv_tc_reg<false>;
+    else if (is_integer(c.kind)) plan->kernel = st ? k_conv_tc<true, 2> : k_conv_tc<false, 2>;
+    else plan->kernel = st ? k_conv_tc<true, 0> : k_conv_tc<false, 0>;
+    // the largest any plan may ask for: other plans of the same kernel rely on it
+    if (cudaFuncSetAttribute((const void *)plan->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
+        fatal_throw("cudaFuncSetAttribute(k_conv_tc) failed");
+    if (st) {
         plan->stats.ensure(16 * (size_t)plan->grid);
         p.stats = plan->stats.get();
         cudaMemset(p.stats, 0, sizeof(unsigned long long) * 16 * plan->grid);
@@ -1828,7 +1892,7 @@ int copy_fields(const int (&f)[TC_PLAN_NFIELDS], int *fields, int n) {
 
 int tc_plan_fields(const TcPlan &plan, int *fields, int n) {
     const TcParams &p = plan.p;
-    const int f[TC_PLAN_NFIELDS] = {plan.threads == TCR_THREADS ? TC_PLAN_CONV_REG : TC_PLAN_CONV, p.kind, p.TW, p.TH, p.BN, p.BK,
+    const int f[TC_PLAN_NFIELDS] = {plan.reg ? TC_PLAN_CONV_REG : TC_PLAN_CONV, p.kind, p.TW, p.TH, p.BN, p.BK,
                                     p.nt, p.bstat, p.stages, p.sps, plan.grid, p.num_work, p.tma_epi, p.jshift,
                                     p.out ? (int)p.out_ldc : 0};
     return copy_fields(f, fields, n);
@@ -1842,21 +1906,13 @@ int tc_stem_plan_fields(const StemPlan &sp, int *fields, int n) {
 
 void tc_launch(const TcPlan &P, cudaStream_t s) {
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)P.grid); cfg.blockDim = dim3((unsigned)P.threads);
+    cfg.gridDim = dim3((unsigned)P.grid); cfg.blockDim = dim3((unsigned)(P.reg ? TCR_THREADS : TC_THREADS));
     cfg.dynamicSmemBytes = P.smem; cfg.stream = s;
     cudaLaunchAttribute attr[1];   // programmatic dependent launch: this kernel's prologue runs while the previous kernel drains
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
-    const bool st = P.p.stats != nullptr;   // role counters: a separate instantiation (YB_TC_STATS=1)
-#define YB_TC_LAUNCH(KERNEL) cudaLaunchKernelEx(&cfg, KERNEL, P.tmA, P.tmB, P.tmO, P.p)
-    if (P.threads == TCR_THREADS) {
-        if (st) cudaLaunchKernelEx(&cfg, k_conv_tc_reg<true>, P.tmA, P.tmB, P.tmO, P.tmO1, P.tmR, P.p);
-        else cudaLaunchKernelEx(&cfg, k_conv_tc_reg<false>, P.tmA, P.tmB, P.tmO, P.tmO1, P.tmR, P.p);
-    }
-    else if (P.p.kind == 1 || P.p.kind == 2) { if (st) YB_TC_LAUNCH((k_conv_tc<true, 2>)); else YB_TC_LAUNCH((k_conv_tc<false, 2>)); }
-    else { if (st) YB_TC_LAUNCH((k_conv_tc<true, 0>)); else YB_TC_LAUNCH((k_conv_tc<false, 0>)); }
-#undef YB_TC_LAUNCH
+    cudaLaunchKernelEx(&cfg, P.kernel, P.tmA, P.tmB, P.tmO, P.tmO1, P.tmR, P.p);
 }
 
 void TcPlanDelete::operator()(TcPlan *plan) const {
@@ -1868,7 +1924,7 @@ void TcPlanDelete::operator()(TcPlan *plan) const {
         for (int b = 0; b < plan->grid; ++b) for (int k = 0; k < 16; ++k) m[k] += (double)h[16 * b + k] / plan->grid;
         fprintf(stderr, "TCSTATS %-28s tiles/cta %.1f kb %d sps %d BN %d | producer: wait_empty %.0f tma_issue %.0f total %.0f | ",
                 plan->desc, (double)plan->p.num_work / plan->grid, plan->p.kblocks, plan->p.sps, plan->p.BN, m[0], m[7], m[1]);
-        if (plan->threads == TCR_THREADS)   // k_conv_tc_reg: the consumers' wait on stg_ready (first work item apart) and the store warps
+        if (plan->reg)   // k_conv_tc_reg: the consumers' wait on stg_ready (first work item apart) and the store warps
             fprintf(stderr, "consumers: wait_full %.0f wait_ready %.0f (first item %.0f) total %.0f | store: wait_full %.0f wait_read %.0f\n",
                     m[2], m[8], m[3], m[6], m[4], m[5]);
         else fprintf(stderr, "consumers: wait_full %.0f total %.0f\n", m[2], m[6]);
