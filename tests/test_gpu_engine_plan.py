@@ -1,9 +1,11 @@
 """The engine's op sequence, pinned per model, precision and fusion setting (tests/golden/engine_plans.json, recorded with
 tests/golden/make_engine_plans.py): the same ops in the same order on the same layers, the same launch and tensor-core counts.
 Activation memory holds only outputs some op writes: every layer whose fetch_layer raises has no buffer, the NHWC input copy
-exists only when the first op makes it, and a detection head whose [yolo] layer runs in its epilogue raises too."""
+exists only when the first op makes it, and a detection head whose [yolo] layer runs in its epilogue raises too.
+Networks the op list cannot express fail when the engine is built, with the layer plan's message."""
 import json
 import os
+import re
 import sys
 
 import pytest
@@ -68,3 +70,30 @@ def test_engine_plan_matches_pinned(model, workdir):
         fused_heads = {i - 1 for i, l in enumerate(net.layers) if l["type_name"] == "YOLO" and i not in ops_layers}
         assert set(got["raises"]) == set(case["raises"]) | fused_heads, what
         assert got["act_bytes"] == case["act_bytes"] - _freed_bytes(net, prec, case, got["raises"]), what
+
+
+def _edit(descs, i, **fields):
+    for k, v in fields.items():
+        setattr(descs[i], k, v)
+    return descs
+
+
+# (case, model, edit of its layer descriptors, message)
+REJECTED = [
+    ("reverse_upsample", "tiny64", lambda d: _edit(d, 19, reverse=1), "engine: reverse upsample (downsample) is not supported"),
+    ("reverse_reorg", "v2voc32", lambda d: _edit(d, 27, reverse=1), "engine: reverse reorg is not supported"),
+    ("conv_input_shape", "tiny64", lambda d: _edit(d, 2, h=31, w=31), "engine: conv input shape mismatch"),
+    ("upsample_behind_yolo", "tiny64", lambda d: d[:17] + [d[19]], "engine: layer 17 has no image input"),
+    ("route_sizes", "tiny64", lambda d: _edit(d, 20, out_h=0),
+     "engine: route over layers of different spatial size is not supported"),
+]
+
+
+@pytest.mark.parametrize("case,model,edit,msg", REJECTED, ids=[r[0] for r in REJECTED])
+def test_engine_rejects_unsupported_network(case, model, edit, msg, workdir):
+    import yolo2_light_b200 as yb
+    cfg, wts = util.model_files(model, workdir)
+    src = yb.load_network(cfg, wts, batch=2)
+    net = yb.network_from_layers(edit([src.layer_desc(i) for i in range(src.n)]), 2, src.h, src.w, src.c)
+    with pytest.raises(yb.YbError, match=re.escape(msg)):
+        net.predict(util.images(model, 2))

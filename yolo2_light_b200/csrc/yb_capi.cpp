@@ -40,8 +40,7 @@ static EngineOptions engine_options(const Network &net, int quantized, int devic
     opt.precision = net.precision;
     opt.qrule = quantized != 0;
     opt.upload = upload;
-    const char *nf = getenv("YB_NO_FUSE");
-    opt.fuse = !(nf && nf[0] == '1') && net.fuse;
+    opt.fuse = net.fuse;
     opt.keep_counts = net.keep_counts;
     opt.q_index_offset = net.q_index_offset;
     return opt;

@@ -1532,13 +1532,13 @@ int pick_bn(int n) { return n <= 32 ? 32 : n <= 64 ? 64 : 128; }
 // A K-block of a 128 x BN tile feeds 128 activation rows and BN filter rows for BN columns of MMA work: the + 64 charges the
 // activation tile's share of the feed, 2 * BN the register epilogue.  E.g. 1x1 512 -> 256 at 38x38, batch 16: 380 work items
 // at BN = 128 (3 waves) against 190 at BN = 256 (2 waves of double-length tiles), and BN = 128 is cheaper.
-// YB_TC_BN=32/64/128/256 takes that width instead (capped at the filters' width; A/B experiments).
-int pick_bn_reg(int n, long m_tiles, int kblocks, int sms) {
+// forced > 0 (YB_TC_BN) takes that width instead (capped at the filters' width; A/B experiments).
+int pick_bn_reg(int n, long m_tiles, int kblocks, int sms, int forced) {
     int cap = 32;
     while (cap < n && cap < 256) cap *= 2;
-    if (const char *e = getenv("YB_TC_BN")) {
+    if (forced > 0) {
         int bn = 32;
-        while (bn * 2 <= std::min(atoi(e), cap)) bn *= 2;
+        while (bn * 2 <= std::min(forced, cap)) bn *= 2;
         return bn;
     }
     int best = 32; double best_cost = 1e300;
@@ -1550,12 +1550,9 @@ int pick_bn_reg(int n, long m_tiles, int kblocks, int sms) {
     return best;
 }
 
-// Persistent grid size of the tensor-core plans: one CTA per SM, or fewer under YB_TC_GRID=n (tests: several work items per CTA
-// reuse the epilogue buffers and flip the barrier phases many times on small layers).
-int grid_cap(int sms) {
-    const char *e = getenv("YB_TC_GRID");
-    return (e && atoi(e) > 0) ? std::min(sms, atoi(e)) : sms;
-}
+// Persistent grid size of the tensor-core plans: one CTA per SM, or at most max_grid > 0 (YB_TC_GRID; tests: several work items
+// per CTA reuse the epilogue buffers and flip the barrier phases many times on small layers).
+int grid_cap(int sms, int max_grid) { return max_grid > 0 ? std::min(sms, max_grid) : sms; }
 
 // Geometry, K-blocks, tile shape, filter tile width and the resident filter matrix.  reg: k_conv_tc_reg runs the plan.
 void plan_tiles(TcParams &p, const TcConv &c, bool reg, int sms) {
@@ -1602,7 +1599,7 @@ void plan_tiles(TcParams &p, const TcConv &c, bool reg, int sms) {
         p.jt = (int)((rows - p.jshift + p.TH - 1) / p.TH);
     };
     set_tw(tw);
-    p.BN = reg ? pick_bn_reg(l.n, (long)p.xt * p.jt, p.kblocks, sms) : pick_bn(l.n);
+    p.BN = reg ? pick_bn_reg(l.n, (long)p.xt * p.jt, p.kblocks, sms, c.sw.bn) : pick_bn(l.n);
     // k_conv_tc_reg stores straddling stride-2 half tiles one tile row at a time, from byte t * TW * 2 SW of a slab: with
     // 64-byte slab rows (SW = 32) and TW = 1 that is not 128-byte aligned, as bulk tensor copies need
     if (reg && s2 && p.BN == 32 && p.TW == 1) set_tw(2);
@@ -1611,7 +1608,7 @@ void plan_tiles(TcParams &p, const TcConv &c, bool reg, int sms) {
     p.a_bytes = (uint32_t)(TC_BM * p.BK * esz);
     p.b_bytes = (uint32_t)(p.BN * p.BK * esz);
     // small filter matrices stay resident in shared memory for the whole kernel (one TMA pass per CTA)
-    p.bstat = (p.nt == 1 && (size_t)p.kblocks * p.b_bytes <= 48 * 1024 && !getenv("YB_TC_NO_BSTAT")) ? 1 : 0;
+    p.bstat = (p.nt == 1 && (size_t)p.kblocks * p.b_bytes <= 48 * 1024 && !c.sw.no_bstat) ? 1 : 0;
     p.bstat_bytes = p.bstat ? (uint32_t)p.kblocks * p.b_bytes : 0u;
 }
 
@@ -1802,12 +1799,12 @@ TcPlanPtr tc_make_plan(const TcConv &c) {
     plan_epilogue(p, c, reg);
     plan_ring(p, reg);
     plan->smem = tc_smem_layout(p, reg);
-    p.dbg = getenv("YB_TC_DBG") ? atoi(getenv("YB_TC_DBG")) : 0;
+    p.dbg = c.sw.dbg;
     snprintf(plan->desc, sizeof(plan->desc), "%dx%dx%d -> n%d k%d s%d%s", l.c, l.h, l.w, l.n, l.size, l.stride, reg ? " reg" : "");
     encode_maps(*plan, c, reg);
-    plan->grid = std::min(p.num_work, grid_cap(sms));
-    // the integer kinds compile EPI 2, the float kinds EPI 0; YB_TC_STATS=1 runs the role-counter instantiations
-    const bool st = getenv("YB_TC_STATS") != nullptr;
+    plan->grid = std::min(p.num_work, grid_cap(sms, c.sw.grid));
+    // the integer kinds compile EPI 2, the float kinds EPI 0; YB_TC_STATS runs the role-counter instantiations
+    const bool st = c.sw.stats;
     plan->reg = reg;
     if (reg) plan->kernel = st ? k_conv_tc_reg<true> : k_conv_tc_reg<false>;
     else if (is_integer(c.kind)) plan->kernel = st ? k_conv_tc<true, 2> : k_conv_tc<false, 2>;
@@ -1848,7 +1845,7 @@ int tc_stem_s2_supported(const Layer &l0, const Layer &l1, const TV &out1) {
 }
 // d_w1: layer 1's bf16 [64][9 * 32] filter matrix (K ordered (ky, kx, c)), d_bias1: its f32 bias
 StemPlanPtr tc_stem_s2_make_plan(const Layer &l0, const Layer &l1, const TV &out1, const void *d_w, const float *d_bias,
-                                 const void *d_w1, const float *d_bias1) {
+                                 const void *d_w1, const float *d_bias1, int max_grid) {
     StemPlanPtr sp(new StemPlan());
     sp->s2 = true;
     StemTcP &p = sp->p;
@@ -1860,7 +1857,7 @@ StemPlanPtr tc_stem_s2_make_plan(const Layer &l0, const Layer &l1, const TV &out
     const long ntiles = (long)p.N * p.xt * p.yt;
     if (ntiles >= INT_MAX) fatal_throw("stem plan: too many tiles");
     p.ntiles = (int)ntiles;
-    sp->grid = std::min(p.ntiles, grid_cap(2 * sm_count()));
+    sp->grid = std::min(p.ntiles, grid_cap(2 * sm_count(), max_grid));
     for (const void *f : {(const void *)k_stem_s2_tc<false>, (const void *)k_stem_s2_tc<true>}) {
         if (cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S2_SMEM) != cudaSuccess ||
             cudaFuncSetAttribute(f, cudaFuncAttributePreferredSharedMemoryCarveout, 100) != cudaSuccess)

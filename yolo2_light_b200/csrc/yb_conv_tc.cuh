@@ -18,6 +18,15 @@ enum TcKind {
     TC_TF32 = 3,   // f32 operands read as tf32: the float detection heads of the exact (INT8 / XNOR) networks; f32 output
 };
 
+// The diagnostic switches of the tensor-core plans (DESIGN, appendix), read with the engine's
+struct TcSwitches {
+    int bn = 0;              // YB_TC_BN: k_conv_tc_reg filter-tile width, rounded down to a power of two >= 32; 0 unset
+    int grid = 0;            // YB_TC_GRID: at most this many CTAs per persistent grid; <= 0 no cap
+    bool no_bstat = false;   // YB_TC_NO_BSTAT: the ring streams the filter tiles, none stays resident
+    bool stats = false;      // YB_TC_STATS: run the role-counter instantiations, print their counters when the plan is freed
+    int dbg = 0;             // YB_TC_DBG: bit mask of bottleneck experiments
+};
+
 // One tensor-core convolution: the layer, its operands and what its epilogue fuses.  tc_conv_supported also takes views rooted
 // at any base with the activation arena's alignment, with the device pointers left null.
 struct TcConv {
@@ -39,6 +48,7 @@ struct TcConv {
     int pool_mode = 0;             // fused 2x2/2 max-pool + next integer layer's input conversion: 1 s8 quantised, 2 +-1 bytes; 0 none
     float pool_mult = 0.f;         // pool_mode 1: the next layer's input multiplier
     TV pool_next{};                // the next integer layer's s8 input
+    TcSwitches sw{};
 };
 
 // The launch state of a tensor-core convolution (TMA tensor maps, tile schedule) and of a tensor-core stem
@@ -61,10 +71,10 @@ void tc_launch(const TcPlan &plan, cudaStream_t s);
 int tc_stem_supported(const Layer &l, const TV &out);
 StemPlanPtr tc_stem_make_plan(const Layer &l, const TV &out, const void *d_w_32x32_bf16, const float *d_bias);
 // the tensor-core stem fused with layer 1, a 3x3 / stride-2 convolution 32 -> 64 filters (bf16 out1): the stem output never
-// reaches HBM.  The plan takes the same launch calls as the stem's.
+// reaches HBM.  The plan takes the same launch calls as the stem's.  max_grid > 0 caps its persistent grid (YB_TC_GRID).
 int tc_stem_s2_supported(const Layer &l0, const Layer &l1, const TV &out1);
 StemPlanPtr tc_stem_s2_make_plan(const Layer &l0, const Layer &l1, const TV &out1, const void *d_w_32x32_bf16,
-                                 const float *d_bias, const void *d_w1_bf16, const float *d_bias1);
+                                 const float *d_bias, const void *d_w1_bf16, const float *d_bias1, int max_grid);
 void tc_stem_launch(const StemPlan &plan, const float *d_in_nchw, cudaStream_t s);
 void tc_stem_launch_u8(const StemPlan &plan, const unsigned char *d_in_hwc, cudaStream_t s);   // frames already of the network size
 

@@ -31,11 +31,17 @@ const char *op_kind_name(int k) {
 
 enum { DT_F32 = 0, DT_BF16 = 1, DT_S8 = 2, DT_BITS = 3 };
 static inline size_t dt_size(int dt) { return dt == DT_F32 ? 4 : dt == DT_BF16 ? 2 : dt == DT_S8 ? 1 : 4; }
+// the <float> or <__nv_bfloat16> instantiation of kernel template k, for activations of dtype dt
+#define BY_DT(k, dt) ((dt) == DT_F32 ? k<float> : k<__nv_bfloat16>)
 
+// One launch of the op list.  `launch` is given the caller's NCHW images of the call, which only ops[0] reads: their pointer
+// changes per call, so ops[0] runs outside the CUDA graph.  ops[0] may also read 8-bit HWC frames of the network size instead
+// (`launch_u8`, when set).
 struct Op {
     int kind;
     int layer;
-    std::function<void(cudaStream_t)> launch;
+    std::function<void(const float *, cudaStream_t)> launch;
+    std::function<void(const unsigned char *, cudaStream_t)> launch_u8;
 };
 
 struct ConvWeights {   // offsets into the weight arena
@@ -47,19 +53,26 @@ struct ConvWeights {   // offsets into the weight arena
     int cpad = 0;     // padded channels of the s8 / bits / bf16 layouts
 };
 
-// The diagnostic YB_* switches of the engine (DESIGN, appendix), read once when an engine is built.
+// The diagnostic YB_* switches of the library (DESIGN, appendix), read once when an engine is built; nothing else reads the
+// environment.
 struct Switches {
     bool no_graph, no_nccl, no_tc, no_tf32, no_stem, no_stem_tc, no_stem_u8, no_stem_pool_fuse, no_stem_s2_fuse,
          no_conv_pool_fuse, no_pool_fuse, no_yolo_fuse;
+    bool no_fuse;       // YB_NO_FUSE=1: EngineOptions::fuse off
     bool xnor_tc;       // YB_XNOR_TC=0 puts every XNOR layer on the popcount kernels
     int xnor_tc_minc;   // narrowest XNOR layer on the tensor cores
+    TcSwitches tc;      // the tensor-core plans'
     static Switches read() {
         auto set = [](const char *name) { return getenv(name) != nullptr; };
-        const char *xtc = getenv("YB_XNOR_TC"), *minc = getenv("YB_XNOR_TC_MINC");
+        auto num = [](const char *name) { const char *v = getenv(name); return v ? atoi(v) : 0; };
+        const char *xtc = getenv("YB_XNOR_TC"), *minc = getenv("YB_XNOR_TC_MINC"), *nf = getenv("YB_NO_FUSE");
         return Switches{set("YB_NO_GRAPH"), set("YB_NO_NCCL"), set("YB_NO_TC"), set("YB_NO_TF32"), set("YB_NO_STEM"),
                         set("YB_NO_STEM_TC"), set("YB_NO_STEM_U8"), set("YB_NO_STEM_POOL_FUSE"), set("YB_NO_STEM_S2_FUSE"),
                         set("YB_NO_CONV_POOL_FUSE"), set("YB_NO_POOL_FUSE"), set("YB_NO_YOLO_FUSE"),
-                        !(xtc && xtc[0] == '0'), minc ? atoi(minc) : 16};
+                        nf && nf[0] == '1', !(xtc && xtc[0] == '0'), minc ? atoi(minc) : 16,
+                        // YB_TC_BN set to anything below 32 means 32
+                        TcSwitches{set("YB_TC_BN") ? std::max(num("YB_TC_BN"), 1) : 0, num("YB_TC_GRID"), set("YB_TC_NO_BSTAT"),
+                                   set("YB_TC_STATS"), num("YB_TC_DBG")}};
     }
 };
 
@@ -83,9 +96,6 @@ struct Engine {
     bool graph_failed = false;
     std::vector<std::pair<int, TcPlanPtr>> tc_plans;   // (layer, its tensor-core plan)
     int n_tc = 0;
-    std::function<void(const float *, cudaStream_t)> first_op;   // consumes the caller's NCHW images (pointer varies per call)
-    std::function<void(const unsigned char *, cudaStream_t)> first_op_u8;   // same from 8-bit HWC frames of the network size (if set)
-    int first_kind = OP_INPUT, first_layer = -1;
     StemPlanPtr stem_plan;
     struct FrameStage {                 // the caller's 8-bit frames of one batch on the device, packed back to back
         DevBuf<unsigned char> buf;
@@ -159,16 +169,13 @@ static std::vector<std::vector<int>> consumers_of(const Network &net) {
     return cons;
 }
 
-template <typename F>
-static void dispatch_dt(int dt, F &&f) {
-    if (dt == DT_F32) f((float *)nullptr);
-    else f((__nv_bfloat16 *)nullptr);
-}
+template <typename T> struct same_type { using type = T; };   // keeps a parameter out of template argument deduction
 
 // ---- engine build --------------------------------------------------------------------------------------------------------
 // Four passes, in this order: plan_layers decides every kernel path and fusion, each layer output's dtype and home, and which
-// outputs are materialised; place allocates the activation buffers that some op writes; pack_weights fills the weight arena;
-// the emit_* functions turn the plan into the op list in layer order, reading the plan only.
+// outputs are materialised, and rejects the networks the engine cannot run; place allocates the activation buffers that some op
+// writes; pack_weights fills the weight arena; the emit_* functions turn the plan into the op list in layer order, reading the
+// plan only: each picks its kernel instantiation and launch shape once, and the op repeats that launch.
 
 enum FirstOp { FIRST_NHWC, FIRST_STEM_SIMT, FIRST_STEM_TC, FIRST_STEM_S2, FIRST_STEM_POOL };
 enum ConvPath { CP_NONE, CP_TC, CP_TF32, CP_SIMT, CP_XNOR_FALLBACK, CP_XNOR_TC, CP_XNOR_SMALLK, CP_XNOR_GENERAL, CP_I8_TC, CP_I8_SIMT };
@@ -234,8 +241,8 @@ struct Builder {
     std::vector<ConvWeights> cw;
     size_t stem_w_off = (size_t)-1;
 
-    Builder(Network &n, const EngineOptions &o, Engine &en)
-        : net(n), opt(o), e(en), sw(en.sw), B(n.batch), nl((int)n.layers.size()), cons(consumers_of(n)), L(nl),
+    Builder(Network &n, Engine &en)
+        : net(n), opt(en.opt), e(en), sw(en.sw), B(n.batch), nl((int)n.layers.size()), cons(consumers_of(n)), L(nl),
           buf_off(nl, (size_t)-1), side_off(nl, (size_t)-1), cw(nl) {}
 
     const Layer &layer(int i) const { return net.layers[i]; }
@@ -323,6 +330,7 @@ struct Builder {
             c.pool_mult = pool_mode == 1 ? layer(i + 2).input_quant_multipler : 0.f;
             c.pool_next = side(i + 2);
         }
+        c.sw = sw.tc;
         if (!placed) return c;
         // filters: [ldn][K] bf16, f32 (K-major copy) or s8 / +-1 bytes ([taps][cpad] per filter)
         c.w = e.w_arena.get() + (c.kind == TC_BF16 ? cw[i].w_bf16 : c.kind == TC_TF32 ? cw[i].w_f32km : cw[i].w_s8);
@@ -422,6 +430,45 @@ struct Builder {
         plan_fusions();
         for (int i = 0; i < nl; ++i)
             if (is_alias(i)) L[i].materialised = L[i].has_out && L[layer(i).input_layers[0]].materialised;
+        reject_unsupported();
+    }
+
+    // the networks the op list cannot express, rejected before anything is allocated
+    void reject_unsupported() const {
+        for (int i = 0; i < nl; ++i) {
+            const Layer &l = layer(i);
+            const LayerPlan &p = L[i];
+            // a fused shortcut reads the output of the convolution in front of it as that convolution's accumulators
+            const bool reads_prev = l.type == YB_CONVOLUTIONAL || l.type == YB_MAXPOOL || l.type == YB_UPSAMPLE || l.type == YB_REORG ||
+                                    l.type == YB_YOLO || l.type == YB_REGION || (l.type == YB_SHORTCUT && !p.fused_sc);
+            if (reads_prev && i > 0 && !L[i - 1].has_out) fatal_throw("engine: layer " + std::to_string(i) + " has no image input");
+            switch (l.type) {
+            case YB_CONVOLUTIONAL: {
+                if (!L[p.fused_into >= 0 ? p.fused_into : i].has_out) fatal_throw("engine: conv output not placed");
+                const int in_c = i == 0 ? net.c : layer(i - 1).out_c, in_h = i == 0 ? net.h : layer(i - 1).out_h,
+                          in_w = i == 0 ? net.w : layer(i - 1).out_w;
+                if (in_c != l.c || in_h != l.h || in_w != l.w) fatal_throw("engine: conv input shape mismatch");
+                break;
+            }
+            case YB_UPSAMPLE:
+                if (l.reverse) fatal_throw("engine: reverse upsample (downsample) is not supported");
+                break;
+            case YB_REORG:
+                if (l.reverse) fatal_throw("engine: reverse reorg is not supported");
+                break;
+            case YB_SHORTCUT:
+                if (!L[l.index].materialised) fatal_throw("engine: shortcut source not placed");
+                break;
+            case YB_ROUTE:
+                if (!p.has_out) fatal_throw("engine: route over layers of different spatial size is not supported");
+                if (is_alias(i)) break;
+                for (int j : l.input_layers)
+                    if (L[j].owner != i && !L[j].materialised) fatal_throw("engine: route source not placed");
+                break;
+            default:
+                break;
+            }
+        }
     }
 
     int conv_path(int i) const {
@@ -657,14 +704,24 @@ struct Builder {
 
     // ---- pass 4: op emission ---------------------------------------------------------------------------------------------
     const float *bias(int i) const { return reinterpret_cast<const float *>(e.w_arena.get() + cw[i].bias); }
-    void push(int kind, int i, std::function<void(cudaStream_t)> f) { e.ops.push_back(Op{kind, i, std::move(f)}); }
+    void push(int kind, int i, std::function<void(const float *, cudaStream_t)> f) { e.ops.push_back(Op{kind, i, std::move(f), nullptr}); }
+    // an op that launches kernel k with these arguments, converted to the kernel's parameter types here
+    template <typename... A>
+    void push_kernel(int kind, int i, void (*k)(A...), dim3 grid, dim3 block, size_t smem, typename same_type<A>::type... args) {
+        push(kind, i, [=](const float *, cudaStream_t s) { k<<<grid, block, smem, s>>>(args...); });
+    }
+    // ops[0] as a kernel whose first argument is the caller's images
+    template <typename... A>
+    void push_input_kernel(int kind, int i, void (*k)(const float *, A...), dim3 grid, dim3 block, typename same_type<A>::type... args) {
+        push(kind, i, [=](const float *in, cudaStream_t s) { k<<<grid, block, 0, s>>>(in, args...); });
+    }
 
     // the tensor-core plan of layer i, with the [yolo] layer or the max-pool the layer plan fuses
     void push_tc_plan(int kind, int i) {
         e.tc_plans.emplace_back(i, tc_make_plan(tc_conv(i, true, L[i].pool_mode)));
         const TcPlan *plan = e.tc_plans.back().second.get();
         if (kind == OP_CONV_TC || kind == OP_CONV_TC_TF32) ++e.n_tc;
-        push(kind, i, [plan](cudaStream_t s) { tc_launch(*plan, s); });
+        push(kind, i, [plan](const float *, cudaStream_t s) { tc_launch(*plan, s); });
     }
 
     int32_t *counts_buffer(int i) {   // raw XNOR popcounts / INT8 accumulators (keep_counts)
@@ -674,101 +731,52 @@ struct Builder {
         return e.counts[i].get();
     }
 
+    // ops[0]: reads the caller's images
     void emit_first() {
         const Layer &l0 = layer(0);
         const int act = l0.activation, H = l0.h, W = l0.w;
-        e.first_kind = OP_CONV_SIMT;
-        e.first_layer = 0;
         if (first == FIRST_STEM_POOL) {
+            // by what layer 2 reads (s8, +-1 bytes, sign bits) and the stem's activation
+            decltype(&k_stem_pool<0, ACT_LEAKY>) const k[3][2] = {{k_stem_pool<0, ACT_LEAKY>, k_stem_pool<0, ACT_LINEAR>},
+                                                                  {k_stem_pool<1, ACT_LEAKY>, k_stem_pool<1, ACT_LINEAR>},
+                                                                  {k_stem_pool<2, ACT_LEAKY>, k_stem_pool<2, ACT_LINEAR>}};
             const Layer &c2 = layer(2);
-            const int v2 = L[2].variant;
-            const bool pm1 = v2 == 1 && L[2].side == SIDE_S8;   // next layer reads +-1 bytes
-            const TV q = side_placed(2);
-            const StemW<16> w16 = stem_weights<16>(l0);
-            const float mult = (v2 == 2) ? c2.input_quant_multipler : 0.f;
-            const int grid = (int)(((long)B * c2.h * c2.w + 127) / 128);
-            e.first_op = [=](const float *din, cudaStream_t s) {
-                if (v2 == 2 && act == ACT_LEAKY) k_stem_pool<0, ACT_LEAKY><<<grid, 128, 0, s>>>(din, q, w16, act, H, W, mult);
-                else if (v2 == 2) k_stem_pool<0, ACT_LINEAR><<<grid, 128, 0, s>>>(din, q, w16, act, H, W, mult);
-                else if (pm1 && act == ACT_LEAKY) k_stem_pool<1, ACT_LEAKY><<<grid, 128, 0, s>>>(din, q, w16, act, H, W, mult);
-                else if (pm1) k_stem_pool<1, ACT_LINEAR><<<grid, 128, 0, s>>>(din, q, w16, act, H, W, mult);
-                else if (act == ACT_LEAKY) k_stem_pool<2, ACT_LEAKY><<<grid, 128, 0, s>>>(din, q, w16, act, H, W, mult);
-                else k_stem_pool<2, ACT_LINEAR><<<grid, 128, 0, s>>>(din, q, w16, act, H, W, mult);
-            };
+            const int mode = L[2].variant == 2 ? 0 : L[2].side == SIDE_S8 ? 1 : 2;
+            push_input_kernel(OP_CONV_SIMT, 0, k[mode][act == ACT_LEAKY ? 0 : 1], (unsigned)(((long)B * c2.h * c2.w + 127) / 128), 128,
+                              side_placed(2), stem_weights<16>(l0), act, H, W, mode == 0 ? c2.input_quant_multipler : 0.f);
         } else if (first == FIRST_STEM_TC || first == FIRST_STEM_S2) {
-            e.stem_plan = first == FIRST_STEM_S2
-                ? tc_stem_s2_make_plan(l0, layer(1), e.out_tv[1], e.w_arena.get() + stem_w_off, bias(0), e.w_arena.get() + cw[1].w_bf16, bias(1))
-                : tc_stem_make_plan(l0, e.out_tv[0], e.w_arena.get() + stem_w_off, bias(0));
+            const bool s2 = first == FIRST_STEM_S2;
+            e.stem_plan = s2 ? tc_stem_s2_make_plan(l0, layer(1), e.out_tv[1], e.w_arena.get() + stem_w_off, bias(0),
+                                                    e.w_arena.get() + cw[1].w_bf16, bias(1), sw.tc.grid)
+                             : tc_stem_make_plan(l0, e.out_tv[0], e.w_arena.get() + stem_w_off, bias(0));
             const StemPlan *sp = e.stem_plan.get();
-            e.first_kind = OP_CONV_TC;
-            if (first == FIRST_STEM_S2) {
-                e.first_layer = 1;
-                ++e.n_tc;
-            }
-            e.first_op = [sp](const float *din, cudaStream_t s) { tc_stem_launch(*sp, din, s); };
-            if (!sw.no_stem_u8) e.first_op_u8 = [sp](const unsigned char *d8, cudaStream_t s) { tc_stem_launch_u8(*sp, d8, s); };
+            if (s2) ++e.n_tc;
+            push(OP_CONV_TC, s2 ? 1 : 0, [sp](const float *in, cudaStream_t s) { tc_stem_launch(*sp, in, s); });
+            if (!sw.no_stem_u8) e.ops[0].launch_u8 = [sp](const unsigned char *in, cudaStream_t s) { tc_stem_launch_u8(*sp, in, s); };
         } else if (first == FIRST_STEM_SIMT) {
-            const TV tout = e.out_tv[0];
-            const int nf = l0.n, odt = L[0].out_dt;
-            const StemW<32> w32 = nf == 32 ? stem_weights<32>(l0) : StemW<32>{};
-            const StemW<16> w16 = nf == 16 ? stem_weights<16>(l0) : StemW<16>{};
-            const int grid = (int)(((long)B * H * W + 127) / 128);
-            e.first_op = [=](const float *din, cudaStream_t s) {
-                if (nf == 32 && odt == DT_BF16) k_conv_stem<32, __nv_bfloat16><<<grid, 128, 0, s>>>(din, tout, w32, act, H, W);
-                else if (nf == 32) k_conv_stem<32, float, true><<<grid, 128, 0, s>>>(din, tout, w32, act, H, W);
-                else if (odt == DT_BF16) k_conv_stem<16, __nv_bfloat16><<<grid, 128, 0, s>>>(din, tout, w16, act, H, W);
-                else k_conv_stem<16, float, true><<<grid, 128, 0, s>>>(din, tout, w16, act, H, W);
-            };
+            const bool bf16 = L[0].out_dt == DT_BF16;
+            const unsigned grid = (unsigned)(((long)B * H * W + 127) / 128);
+            if (l0.n == 32)
+                push_input_kernel(OP_CONV_SIMT, 0, bf16 ? k_conv_stem<32, __nv_bfloat16> : k_conv_stem<32, float, true>, grid, 128,
+                                  e.out_tv[0], stem_weights<32>(l0), act, H, W);
+            else
+                push_input_kernel(OP_CONV_SIMT, 0, bf16 ? k_conv_stem<16, __nv_bfloat16> : k_conv_stem<16, float, true>, grid, 128,
+                                  e.out_tv[0], stem_weights<16>(l0), act, H, W);
         } else {
-            const TV in0 = e.in0;
-            const int dt = ADT;
-            const int g = grid_for((long)in0.N * in0.H * in0.W);
-            e.first_kind = OP_INPUT;
-            e.first_layer = -1;
-            e.first_op = [=](const float *din, cudaStream_t s) {
-                if (dt == DT_F32) k_input_nchw_to_nhwc<float><<<g, 256, 0, s>>>(din, in0);
-                else k_input_nchw_to_nhwc<__nv_bfloat16><<<g, 256, 0, s>>>(din, in0);
-            };
+            push_input_kernel(OP_INPUT, -1, BY_DT(k_input_nchw_to_nhwc, ADT), grid_for((long)e.in0.N * e.in0.H * e.in0.W), 256, e.in0);
         }
-        push(e.first_kind, e.first_layer, nullptr);   // launched specially: pointer varies per call
-    }
-
-    void need_input(int i) const {
-        if (i > 0 && !L[i - 1].has_out) fatal_throw("engine: layer " + std::to_string(i) + " has no image input");
     }
 
     void emit_conv(int i) {
-        const Layer &l = layer(i);
-        need_input(i);
-        const int tgt = L[i].fused_into >= 0 ? L[i].fused_into : i;
-        if (!L[tgt].has_out) fatal_throw("engine: conv output not placed");
-        const int in_c = i == 0 ? net.c : layer(i - 1).out_c, in_h = i == 0 ? net.h : layer(i - 1).out_h,
-                  in_w = i == 0 ? net.w : layer(i - 1).out_w;
-        if (in_c != l.c || in_h != l.h || in_w != l.w) fatal_throw("engine: conv input shape mismatch");
         const TV tin = i == 0 ? e.in0 : e.out_tv[i - 1];   // no base where the input is fused away
         if (L[i].variant == 0) emit_conv_fp32(i, tin);
         else if (L[i].variant == 1) emit_conv_xnor(i, tin);
         else emit_conv_int8(i, tin);
     }
 
-    void emit_conv_fp32(int i, const TV &tin) {
+    // k_conv_simt: the f32 [K][ldw] weights of convolution i
+    void push_conv_simt(int i, void (*k)(ConvP), const TV &tin, const TV &tout, const TV &res, int act2) {
         const Layer &l = layer(i);
-        const LayerPlan &p = L[i];
-        const int tgt = p.fused_into >= 0 ? p.fused_into : i;
-        const TV tout = e.out_tv[tgt];   // no base where the [yolo] layer is fused
-        const int odt = L[tgt].out_dt;
-        TV res{}; int rdt = DT_F32; int act2 = ACT_LINEAR;
-        if (p.fused_into >= 0) {
-            const Layer &s = layer(tgt);
-            res = e.out_tv[s.index];
-            rdt = L[s.index].out_dt;
-            act2 = s.activation;
-            if (!res.base) fatal_throw("engine: shortcut source not placed");
-        }
-        if (p.path == CP_TC || p.path == CP_TF32) {
-            push_tc_plan(p.path == CP_TC ? OP_CONV_TC : OP_CONV_TC_TF32, i);
-            return;
-        }
         const long M = (long)B * l.out_h * l.out_w;
         ConvP cp{};
         cp.in = tin; cp.out = tout; cp.res = res;
@@ -776,20 +784,30 @@ struct Builder {
         cp.bias = bias(i);
         cp.n = l.n; cp.ldw = cw[i].ldw; cp.size = l.size; cp.stride = l.stride; cp.pad = l.pad;
         cp.act = l.activation; cp.act2 = act2; cp.K = l.size * l.size * l.c; cp.M = M;
-        dim3 grid((unsigned)((M + 63) / 64), (unsigned)((l.n + 63) / 64));
-        const int key = in_dt(i) * 4 + odt * 2 + rdt;
-        push(OP_CONV_SIMT, i, [cp, grid, key](cudaStream_t s) {
-            switch (key) {
-            case 0: k_conv_simt<float, float, float, true><<<grid, 256, 0, s>>>(cp); break;   // reference order, bit-exact
-            case 1: k_conv_simt<float, float, __nv_bfloat16><<<grid, 256, 0, s>>>(cp); break;
-            case 2: k_conv_simt<float, __nv_bfloat16, float><<<grid, 256, 0, s>>>(cp); break;
-            case 3: k_conv_simt<float, __nv_bfloat16, __nv_bfloat16><<<grid, 256, 0, s>>>(cp); break;
-            case 4: k_conv_simt<__nv_bfloat16, float, float><<<grid, 256, 0, s>>>(cp); break;
-            case 5: k_conv_simt<__nv_bfloat16, float, __nv_bfloat16><<<grid, 256, 0, s>>>(cp); break;
-            case 6: k_conv_simt<__nv_bfloat16, __nv_bfloat16, float><<<grid, 256, 0, s>>>(cp); break;
-            default: k_conv_simt<__nv_bfloat16, __nv_bfloat16, __nv_bfloat16><<<grid, 256, 0, s>>>(cp); break;
-            }
-        });
+        push_kernel(OP_CONV_SIMT, i, k, dim3((unsigned)((M + 63) / 64), (unsigned)((l.n + 63) / 64)), 256, 0, cp);
+    }
+
+    void emit_conv_fp32(int i, const TV &tin) {
+        const LayerPlan &p = L[i];
+        if (p.path == CP_TC || p.path == CP_TF32) {
+            push_tc_plan(p.path == CP_TC ? OP_CONV_TC : OP_CONV_TC_TF32, i);
+            return;
+        }
+        const int tgt = p.fused_into >= 0 ? p.fused_into : i;
+        TV res{}; int rdt = DT_F32; int act2 = ACT_LINEAR;
+        if (p.fused_into >= 0) {
+            const Layer &s = layer(tgt);
+            res = e.out_tv[s.index];
+            rdt = L[s.index].out_dt;
+            act2 = s.activation;
+        }
+        // by input, output and residual dtype; all f32 is the reference's summation order, bit-exact
+        void (*const k[2][2][2])(ConvP) = {
+            {{k_conv_simt<float, float, float, true>, k_conv_simt<float, float, __nv_bfloat16>},
+             {k_conv_simt<float, __nv_bfloat16, float>, k_conv_simt<float, __nv_bfloat16, __nv_bfloat16>}},
+            {{k_conv_simt<__nv_bfloat16, float, float>, k_conv_simt<__nv_bfloat16, float, __nv_bfloat16>},
+             {k_conv_simt<__nv_bfloat16, __nv_bfloat16, float>, k_conv_simt<__nv_bfloat16, __nv_bfloat16, __nv_bfloat16>}}};
+        push_conv_simt(i, k[in_dt(i)][L[tgt].out_dt][rdt], tin, e.out_tv[tgt], res, act2);
     }
 
     void emit_conv_xnor(int i, const TV &tin) {
@@ -799,36 +817,23 @@ struct Builder {
         const long M = (long)B * l.out_h * l.out_w;
         if (p.path == CP_XNOR_FALLBACK) {
             const TV pm1 = side_placed(i);
-            const int gb = grid_for((long)B * l.h * l.w * l.c);
-            push(OP_BINARIZE, i, [tin, pm1, gb](cudaStream_t s) { k_binarize_pm1<<<gb, 256, 0, s>>>(tin, pm1); });
-            ConvP cp{};
-            cp.in = pm1; cp.out = tout; cp.res = TV{};
-            cp.w = e.w_arena.get() + cw[i].w_f32;
-            cp.bias = bias(i);
-            cp.n = l.n; cp.ldw = cw[i].ldw; cp.size = l.size; cp.stride = l.stride; cp.pad = l.pad;
-            cp.act = l.activation; cp.act2 = ACT_LINEAR; cp.K = l.size * l.size * l.c; cp.M = M;
-            dim3 grid((unsigned)((M + 63) / 64), (unsigned)((l.n + 63) / 64));
-            push(OP_CONV_SIMT, i, [cp, grid](cudaStream_t s) { k_conv_simt<float, float, float, true><<<grid, 256, 0, s>>>(cp); });
+            push_kernel(OP_BINARIZE, i, k_binarize_pm1, grid_for((long)B * l.h * l.w * l.c), 256, 0, tin, pm1);
+            push_conv_simt(i, k_conv_simt<float, float, float, true>, pm1, tout, TV{}, ACT_LINEAR);
             return;
         }
         int32_t *cnt_dbg = counts_buffer(i);
         if (p.path == CP_XNOR_TC) {
-            const TV q = side_placed(i);
-            const int g = grid_for((long)B * l.h * l.w * (l.c / 16));
-            if (!p.prefilled) push(OP_BINARIZE, i, [tin, q, g](cudaStream_t s) { k_binarize_s8<<<g, 256, 0, s>>>(tin, q); });
+            if (!p.prefilled)
+                push_kernel(OP_BINARIZE, i, k_binarize_s8, grid_for((long)B * l.h * l.w * (l.c / 16)), 256, 0, tin, side_placed(i));
             push_tc_plan(OP_CONV_TC_I8, i);
             return;
         }
         const int CW = p.side_ld;
         const TV bits = make_tv(e.act_arena.get() + side_off[i], B, l.h, l.w, CW, CW, P, DT_BITS, 0);
-        if (!p.prefilled) {
-            if (vec4_view(tin)) {
-                const int g = grid_for((long)B * l.h * l.w * CW);
-                push(OP_BINARIZE, i, [tin, bits, g](cudaStream_t s) { k_binarize_vec<float><<<g, 256, 0, s>>>(tin, bits); });
-            } else {
-                const int g = grid_for((long)B * l.h * l.w * CW * 32);
-                push(OP_BINARIZE, i, [tin, bits, g](cudaStream_t s) { k_binarize<float><<<g, 256, 0, s>>>(tin, bits); });
-            }
+        if (!p.prefilled) {   // a word of sign bits per thread, or per warp
+            const bool vec = vec4_view(tin);
+            push_kernel(OP_BINARIZE, i, vec ? k_binarize_vec<float> : k_binarize<float>,
+                        grid_for((long)B * l.h * l.w * CW * (vec ? 1 : 32)), 256, 0, tin, bits);
         }
         XnorP xp{};
         xp.bits = bits; xp.out = tout;
@@ -839,31 +844,22 @@ struct Builder {
         xp.padbits = (CW * 32 - l.c) * l.size * l.size;
         xp.act = l.activation; xp.M = M; xp.counts = cnt_dbg;
         if (p.path == CP_XNOR_GENERAL) {
-            dim3 grid((unsigned)((M + 63) / 64), (unsigned)((l.n + 63) / 64));
-            push(OP_CONV_XNOR, i, [xp, grid](cudaStream_t s) { k_conv_xnor<<<grid, 256, 0, s>>>(xp); });
+            push_kernel(OP_CONV_XNOR, i, k_conv_xnor, dim3((unsigned)((M + 63) / 64), (unsigned)((l.n + 63) / 64)), 256, 0, xp);
             return;
         }
         const size_t smem = (size_t)l.n * 9 * CW * 4;
         if (const int pm = p.pool_mode) {
             // the 2x2 max-pool behind this layer and the next XNOR layer's sign extraction run in this kernel, which reads only
-            // the shape of the output it does not write
+            // the shape of the output it does not write.  By sign words per tap and what the next layer reads (+-1 bytes, bits).
+            void (*const k[2][2])(XnorP, TV) = {{k_conv_xnor_smallk_pool<1, 2>, k_conv_xnor_smallk_pool<1, 3>},
+                                                {k_conv_xnor_smallk_pool<2, 2>, k_conv_xnor_smallk_pool<2, 3>}};
             xp.out = make_tv(nullptr, B, l.out_h, l.out_w, l.n, L[i].ldc, P, DT_F32, 0);
             const Layer &c2 = layer(i + 2);
-            const TV qn = side_placed(i + 2);
-            const unsigned gp = (unsigned)(((long)B * c2.h * c2.w + 127) / 128);
-            push(OP_CONV_XNOR, i, [xp, qn, gp, smem, CW, pm](cudaStream_t s) {
-                if (CW == 1 && pm == 2) k_conv_xnor_smallk_pool<1, 2><<<gp, 128, smem, s>>>(xp, qn);
-                else if (CW == 1) k_conv_xnor_smallk_pool<1, 3><<<gp, 128, smem, s>>>(xp, qn);
-                else if (pm == 2) k_conv_xnor_smallk_pool<2, 2><<<gp, 128, smem, s>>>(xp, qn);
-                else k_conv_xnor_smallk_pool<2, 3><<<gp, 128, smem, s>>>(xp, qn);
-            });
+            push_kernel(OP_CONV_XNOR, i, k[CW - 1][pm - 2], (unsigned)(((long)B * c2.h * c2.w + 127) / 128), 128, smem, xp,
+                        side_placed(i + 2));
             return;
         }
-        const unsigned gsm = (unsigned)((M + 127) / 128);
-        push(OP_CONV_XNOR, i, [xp, gsm, smem, CW](cudaStream_t s) {
-            if (CW == 1) k_conv_xnor_smallk<1><<<gsm, 128, smem, s>>>(xp);
-            else k_conv_xnor_smallk<2><<<gsm, 128, smem, s>>>(xp);
-        });
+        push_kernel(OP_CONV_XNOR, i, CW == 1 ? k_conv_xnor_smallk<1> : k_conv_xnor_smallk<2>, (unsigned)((M + 127) / 128), 128, smem, xp);
     }
 
     void emit_conv_int8(int i, const TV &tin) {
@@ -871,9 +867,9 @@ struct Builder {
         const LayerPlan &p = L[i];
         const TV tout = e.out_tv[i];   // no base where the max-pool behind it is fused
         const TV q = side_placed(i);
-        const float mult = l.input_quant_multipler;
-        const int g = grid_for((long)B * l.h * l.w * (p.side_ld / 4));
-        if (!p.prefilled) push(OP_QUANTIZE, i, [tin, q, mult, g](cudaStream_t s) { k_quantize<float><<<g, 256, 0, s>>>(tin, q, mult); });
+        if (!p.prefilled)
+            push_kernel(OP_QUANTIZE, i, k_quantize<float>, grid_for((long)B * l.h * l.w * (p.side_ld / 4)), 256, 0, tin, q,
+                        l.input_quant_multipler);
         int *acc_dbg = counts_buffer(i);
         if (p.path == CP_I8_TC) {
             push_tc_plan(OP_CONV_TC_I8, i);
@@ -887,8 +883,7 @@ struct Builder {
         ip.alpha1 = alpha1(l);
         ip.n = l.n; ip.size = l.size; ip.stride = l.stride; ip.pad = l.pad; ip.act = l.activation;
         ip.CW = p.side_ld / 4; ip.M = M; ip.acc_out = acc_dbg;
-        dim3 grid((unsigned)((M + 63) / 64), (unsigned)((l.n + 63) / 64));
-        push(OP_CONV_INT8, i, [ip, grid](cudaStream_t s) { k_conv_int8_simt<<<grid, 256, 0, s>>>(ip); });
+        push_kernel(OP_CONV_INT8, i, k_conv_int8_simt, dim3((unsigned)((M + 63) / 64), (unsigned)((l.n + 63) / 64)), 256, 0, ip);
     }
 
     // max-pool, upsample, shortcut, route, reorg, yolo, region
@@ -902,129 +897,72 @@ struct Builder {
         switch (l.type) {
         case YB_MAXPOOL: {
             if (p.pool_in_conv) break;    // done in the epilogue of the integer convolution in front of it
-            need_input(i);
-            const int size = l.size, stride = l.stride, pad = l.pad;
             if (p.pool_to_side) {
+                // by what layer i+1 reads: s8 quantised (with its multiplier), +-1 bytes, or sign bits
+                void (*const k[3])(TV, TV, int, int, int, float) = {k_maxpool_fused<0>, k_maxpool_fused<1>, k_maxpool_fused<2>};
                 const Layer &c = layer(i + 1);
                 const TV q = side_placed(i + 1);
-                const float mult = c.input_quant_multipler;
-                if (L[i + 1].side == SIDE_BITS) {
-                    const int gb = grid_for((long)B * c.h * c.w * q.ldc);
-                    push(OP_MAXPOOL, i, [tin, q, size, stride, pad, gb](cudaStream_t s) {
-                        k_maxpool_fused<2><<<gb, 256, 0, s>>>(tin, q, size, stride, pad, 0.f); });
-                } else {
-                    const int gq = grid_for((long)B * c.h * c.w * (q.ldc / 4));
-                    if (L[i + 1].variant == 2)
-                        push(OP_MAXPOOL, i, [tin, q, size, stride, pad, mult, gq](cudaStream_t s) {
-                            k_maxpool_fused<0><<<gq, 256, 0, s>>>(tin, q, size, stride, pad, mult); });
-                    else
-                        push(OP_MAXPOOL, i, [tin, q, size, stride, pad, gq](cudaStream_t s) {
-                            k_maxpool_fused<1><<<gq, 256, 0, s>>>(tin, q, size, stride, pad, 0.f); });
-                }
+                const int mode = L[i + 1].side == SIDE_BITS ? 2 : L[i + 1].variant == 2 ? 0 : 1;
+                push_kernel(OP_MAXPOOL, i, k[mode], grid_for((long)B * c.h * c.w * (mode == 2 ? q.ldc : q.ldc / 4)), 256, 0, tin, q,
+                            l.size, l.stride, l.pad, mode == 0 ? c.input_quant_multipler : 0.f);
                 break;
             }
             const int esz = (int)dt_size(dt);
             const bool vec = (l.out_c * esz) % 16 == 0 && (tin.ldc * esz) % 16 == 0 && (tout.ldc * esz) % 16 == 0 &&
                              (reinterpret_cast<uintptr_t>(tin.base) & 15) == 0 && (reinterpret_cast<uintptr_t>(tout.base) & 15) == 0;
             const int gv = grid_for((long)B * l.out_h * l.out_w * ((l.out_c * esz) / 16 + 1));
-            push(OP_MAXPOOL, i, [tin, tout, size, stride, pad, g, dt, vec, gv](cudaStream_t s) {
-                if (vec && dt == DT_F32) k_maxpool_vec<float><<<gv, 256, 0, s>>>(tin, tout, size, stride, pad);
-                else if (vec) k_maxpool_vec<__nv_bfloat16><<<gv, 256, 0, s>>>(tin, tout, size, stride, pad);
-                else if (dt == DT_F32) k_maxpool<float><<<g, 256, 0, s>>>(tin, tout, size, stride, pad);
-                else k_maxpool<__nv_bfloat16><<<g, 256, 0, s>>>(tin, tout, size, stride, pad);
-            });
+            push_kernel(OP_MAXPOOL, i, vec ? BY_DT(k_maxpool_vec, dt) : BY_DT(k_maxpool, dt), vec ? gv : g, 256, 0, tin, tout, l.size,
+                        l.stride, l.pad);
             break;
         }
         case YB_UPSAMPLE: {
-            need_input(i);
-            if (l.reverse) fatal_throw("engine: reverse upsample (downsample) is not supported");
-            const int stride = l.stride; const float scale = l.scale;
             const int esz = (int)dt_size(dt);
-            const bool vec = scale == 1.f && (l.out_c * esz) % 16 == 0 && (tin.ldc * esz) % 16 == 0 && (tout.ldc * esz) % 16 == 0 &&
+            const bool vec = l.scale == 1.f && (l.out_c * esz) % 16 == 0 && (tin.ldc * esz) % 16 == 0 && (tout.ldc * esz) % 16 == 0 &&
                              (reinterpret_cast<uintptr_t>(tin.base) & 15) == 0 && (reinterpret_cast<uintptr_t>(tout.base) & 15) == 0;
-            const int gv = grid_for((long)B * l.out_h * l.out_w * ((l.out_c * esz) / 16 + 1));
-            push(OP_UPSAMPLE, i, [tin, tout, stride, scale, g, dt, vec, gv, esz](cudaStream_t s) {
-                if (vec) k_upsample_vec16<<<gv, 256, 0, s>>>(tin, tout, stride, esz);
-                else if (dt == DT_F32) k_upsample<float><<<g, 256, 0, s>>>(tin, tout, stride, scale);
-                else k_upsample<__nv_bfloat16><<<g, 256, 0, s>>>(tin, tout, stride, scale);
-            });
+            if (vec)
+                push_kernel(OP_UPSAMPLE, i, k_upsample_vec16, grid_for((long)B * l.out_h * l.out_w * ((l.out_c * esz) / 16 + 1)), 256, 0,
+                            tin, tout, l.stride, esz);
+            else
+                push_kernel(OP_UPSAMPLE, i, BY_DT(k_upsample, dt), g, 256, 0, tin, tout, l.stride, l.scale);
             break;
         }
         case YB_SHORTCUT: {
             if (p.fused_sc) break;
-            need_input(i);
-            const TV from = e.out_tv[l.index];
-            if (!from.base) fatal_throw("engine: shortcut source not placed");
-            if (L[l.index].out_dt != dt) fatal_throw("engine: shortcut dtype mismatch");
             // shortcut_cpu(batch, w1=l.w, h1=l.h, c1=l.c (from), add, w2=l.out_w, ...): yolov2_forward_network.c:410
             const int stride = std::max(l.w / l.out_w, 1), sample = std::max(l.out_w / l.w, 1);
             const int minw = std::min(l.w, l.out_w), minh = std::min(l.h, l.out_h), minc = std::min(l.c, l.out_c);
-            const int act = l.activation;
-            push(OP_SHORTCUT, i, [=](cudaStream_t s) {
-                if (dt == DT_F32) k_shortcut<float><<<g, 256, 0, s>>>(tin, from, tout, stride, sample, minw, minh, minc, act);
-                else k_shortcut<__nv_bfloat16><<<g, 256, 0, s>>>(tin, from, tout, stride, sample, minw, minh, minc, act);
-            });
+            push_kernel(OP_SHORTCUT, i, BY_DT(k_shortcut, dt), g, 256, 0, tin, e.out_tv[l.index], tout, stride, sample, minw, minh,
+                        minc, l.activation);
             break;
         }
         case YB_ROUTE: {
-            if (!p.has_out) fatal_throw("engine: route over layers of different spatial size is not supported");
             if (is_alias(i)) break;
             int off = 0;
-            for (int k = 0; k < l.n; ++k) {
-                const int j = l.input_layers[k];
+            for (int j : l.input_layers) {
                 const Layer &src = layer(j);
                 if (L[j].owner != i) {
-                    const TV tsrc = e.out_tv[j];
-                    if (!tsrc.base) fatal_throw("engine: route source not placed");
-                    if (L[j].out_dt != p.out_dt) fatal_throw("engine: route dtype mismatch");
                     TV slice = tout;
                     slice.base += (size_t)off * dt_size(p.out_dt);
                     slice.C = src.out_c;
-                    const int gs = grid_for((long)B * src.out_h * src.out_w * src.out_c);
-                    const int odt = p.out_dt;
-                    push(OP_ROUTE_COPY, i, [tsrc, slice, gs, odt](cudaStream_t s) {
-                        if (odt == DT_F32) k_copy_channels<float><<<gs, 256, 0, s>>>(tsrc, slice);
-                        else k_copy_channels<__nv_bfloat16><<<gs, 256, 0, s>>>(tsrc, slice);
-                    });
+                    push_kernel(OP_ROUTE_COPY, i, BY_DT(k_copy_channels, p.out_dt),
+                                grid_for((long)B * src.out_h * src.out_w * src.out_c), 256, 0, e.out_tv[j], slice);
                 }
                 off += src.out_c;
             }
             break;
         }
-        case YB_REORG: {
-            need_input(i);
-            if (l.reverse) fatal_throw("engine: reverse reorg is not supported");
-            const int stride = l.stride;
-            push(OP_REORG, i, [tin, tout, stride, g, dt](cudaStream_t s) {
-                if (dt == DT_F32) k_reorg<float><<<g, 256, 0, s>>>(tin, tout, stride);
-                else k_reorg<__nv_bfloat16><<<g, 256, 0, s>>>(tin, tout, stride);
-            });
+        case YB_REORG:
+            push_kernel(OP_REORG, i, BY_DT(k_reorg, dt), g, 256, 0, tin, tout, l.stride);
             break;
-        }
-        case YB_YOLO: {
+        case YB_YOLO:
             if (p.yolo_fused) break;   // written by the head convolution's epilogue
-            need_input(i);
-            float *dst = e.finals[i].d.get();
-            const int classes = l.classes;
-            const int gy = grid_for((long)B * ((l.h * l.w + 31) / 32) * ((l.c + 31) / 32) * 256);
-            const int fast = (ADT == DT_BF16) ? 1 : 0;
-            push(OP_YOLO, i, [tin, dst, classes, gy, dt, fast](cudaStream_t s) {
-                if (dt == DT_F32) k_yolo<float><<<gy, 256, 0, s>>>(tin, dst, classes, fast);
-                else k_yolo<__nv_bfloat16><<<gy, 256, 0, s>>>(tin, dst, classes, fast);
-            });
+            push_kernel(OP_YOLO, i, BY_DT(k_yolo, dt), grid_for((long)B * ((l.h * l.w + 31) / 32) * ((l.c + 31) / 32) * 256), 256, 0,
+                        tin, e.finals[i].d.get(), l.classes, ADT == DT_BF16 ? 1 : 0);
             break;
-        }
-        case YB_REGION: {
-            need_input(i);
-            float *dst = e.finals[i].d.get();
-            const int n = l.n, classes = l.classes, coords = l.coords, softmax = l.softmax;
-            const int gr = grid_for((long)B * l.h * l.w * l.n);
-            push(OP_REGION, i, [tin, dst, n, classes, coords, softmax, gr, dt](cudaStream_t s) {
-                if (dt == DT_F32) k_region<float><<<gr, 256, 0, s>>>(tin, dst, n, classes, coords, softmax);
-                else k_region<__nv_bfloat16><<<gr, 256, 0, s>>>(tin, dst, n, classes, coords, softmax);
-            });
+        case YB_REGION:
+            push_kernel(OP_REGION, i, BY_DT(k_region, dt), grid_for((long)B * l.h * l.w * l.n), 256, 0, tin, e.finals[i].d.get(), l.n,
+                        l.classes, l.coords, l.softmax);
             break;
-        }
         default:
             break;
         }
@@ -1038,13 +976,8 @@ struct Builder {
         const int src = L[last].fused_into >= 0 ? L[last].fused_into : last;
         const TV t = e.out_tv[src];
         if (!t.base) return;
-        float *dst = e.finals[last].d.get();
-        const int dt = L[src].out_dt;
-        const int g = grid_for((long)B * l.outputs);
-        push(OP_YOLO, last, [t, dst, g, dt](cudaStream_t s) {
-            if (dt == DT_F32) k_nhwc_to_nchw_f32<float><<<g, 256, 0, s>>>(t, dst);
-            else k_nhwc_to_nchw_f32<__nv_bfloat16><<<g, 256, 0, s>>>(t, dst);
-        });
+        push_kernel(OP_YOLO, last, BY_DT(k_nhwc_to_nchw_f32, L[src].out_dt), grid_for((long)B * l.outputs), 256, 0, t,
+                    e.finals[last].d.get());
     }
 
     void emit_ops() {
@@ -1076,9 +1009,10 @@ std::shared_ptr<Engine> build_engine(Network *net, const EngineOptions &opt) {
     e->opt = opt;
     e->batch = net->batch;
     e->sw = Switches::read();
+    e->opt.fuse = opt.fuse && !e->sw.no_fuse;
     e->stream = make_stream();
 
-    Builder b(*net, opt, *e);
+    Builder b(*net, *e);
     b.plan_layers();
     b.place();
     b.place_finals();
@@ -1236,15 +1170,15 @@ static void engine_forward_impl(Engine *e, const void *d_input, const unsigned c
     cudaStream_t s = stream ? (cudaStream_t)stream : (cudaStream_t)e->stream;
     CUDA_OK(cudaSetDevice(e->opt.device));   // thread identity may change per call (SURVEY 8b, threading)
     const float *din = d_input ? reinterpret_cast<const float *>(d_input) : e->d_input.get();
-    if (d_u8_frames) e->first_op_u8(d_u8_frames, s);   // stem straight from the 8-bit frames
-    else e->first_op(din, s);
+    if (d_u8_frames) e->ops[0].launch_u8(d_u8_frames, s);   // stem straight from the 8-bit frames
+    else e->ops[0].launch(din, s);
     if (!e->graph_exec && !e->graph_failed && e->sw.no_graph) e->graph_failed = true;   // profiling aid
     if (!e->graph_exec && !e->graph_failed) {
-        // capture everything after the input conversion once
+        // capture everything after ops[0] once
         cudaGraph_t graph = nullptr;
         cudaError_t st = cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal);
         if (st == cudaSuccess) {
-            for (size_t k = 1; k < e->ops.size(); ++k) e->ops[k].launch(s);
+            for (size_t k = 1; k < e->ops.size(); ++k) e->ops[k].launch(din, s);
             st = cudaStreamEndCapture(s, &graph);
         }
         cudaGraphExec_t exec = nullptr;
@@ -1258,7 +1192,7 @@ static void engine_forward_impl(Engine *e, const void *d_input, const unsigned c
     if (e->graph_exec) {
         CUDA_OK(cudaGraphLaunch(e->graph_exec, s));
     } else {
-        for (size_t k = 1; k < e->ops.size(); ++k) e->ops[k].launch(s);
+        for (size_t k = 1; k < e->ops.size(); ++k) e->ops[k].launch(din, s);
     }
     CUDA_OK(cudaGetLastError());
 }
@@ -1425,9 +1359,8 @@ void engine_fetch_layer(Engine *e, Network *net, int layer, float *dst) {
     if (!t.base) fatal_throw("fetch_layer: layer " + std::to_string(layer) + " has no materialised output "
                              "(fused or aliased away; build the engine with fusion off)");
     DevBuf<float> tmp(count);
-    const int g = grid_for((long)count);
-    if (e->out_dt[layer] == DT_F32) k_nhwc_to_nchw_f32<float><<<g, 256, 0, e->stream>>>(t, tmp.get());
-    else k_nhwc_to_nchw_f32<__nv_bfloat16><<<g, 256, 0, e->stream>>>(t, tmp.get());
+    auto *k = BY_DT(k_nhwc_to_nchw_f32, e->out_dt[layer]);
+    k<<<grid_for((long)count), 256, 0, e->stream>>>(t, tmp.get());
     CUDA_OK(cudaMemcpyAsync(dst, tmp.get(), count * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
     CUDA_OK(cudaStreamSynchronize(e->stream));
 }
@@ -1463,9 +1396,8 @@ void engine_input_histogram(Engine *e, Network *net, int layer, int img, float b
         const TV t = e->out_tv[layer - 1];
         if (!t.base) fatal_throw("calibrate: the input of layer " + std::to_string(layer) +
                                  " is not materialised (fused away; set option fuse=0)");
-        const long n = (long)t.C * t.H * t.W;
-        if (e->out_dt[layer - 1] == DT_F32) k_abs_hist<float><<<grid_for(n), 256, 0, e->stream>>>(t, img, bin_width, max_bin, d_hist.get());
-        else k_abs_hist<__nv_bfloat16><<<grid_for(n), 256, 0, e->stream>>>(t, img, bin_width, max_bin, d_hist.get());
+        auto *k = BY_DT(k_abs_hist, e->out_dt[layer - 1]);
+        k<<<grid_for((long)t.C * t.H * t.W), 256, 0, e->stream>>>(t, img, bin_width, max_bin, d_hist.get());
     }
     CUDA_OK(cudaMemcpyAsync(hist, d_hist.get(), (size_t)max_bin * sizeof(unsigned), cudaMemcpyDeviceToHost, e->stream));
     CUDA_OK(cudaStreamSynchronize(e->stream));
@@ -1604,7 +1536,7 @@ int engine_submit_frames(Engine *e, Network *net, const unsigned char *const *fr
                          float thresh, float nms, int relative, int letter, int max_rows) {
     return submit_detections(e, net, nimg, thresh, nms, relative, max_rows, [&](Engine::Slot &sl) -> const unsigned char * {
         const bool net_size = stage_frames(e, sl.u8, net, frames, w, h, nimg, letter, e->s_in);
-        if (e->first_op_u8 && net_size && net->c == 3) {   // frames of the network size: no staging
+        if (e->ops[0].launch_u8 && net_size && net->c == 3) {   // frames of the network size: no staging
             const size_t frame = (size_t)net->w * net->h * net->c;
             if (nimg < e->batch) CUDA_OK(cudaMemsetAsync(sl.u8.buf.get() + nimg * frame, 0, (e->batch - nimg) * frame, e->s_in));
             return sl.u8.buf.get();
@@ -1655,7 +1587,7 @@ int engine_tc_plan(Engine *e, int layer, int *fields, int n) {
     for (const auto &[plan_layer, plan] : e->tc_plans)
         if (plan_layer == layer) return tc_plan_fields(*plan, fields, n);
     // the stem plan runs layer 0, and layer 1 too when k_stem_s2_tc fuses it
-    if (e->stem_plan && (layer == 0 || layer == e->first_layer)) return tc_stem_plan_fields(*e->stem_plan, fields, n);
+    if (e->stem_plan && (layer == 0 || layer == e->ops[0].layer)) return tc_stem_plan_fields(*e->stem_plan, fields, n);
     return 0;
 }
 
@@ -1669,8 +1601,7 @@ int engine_profile(Engine *e, const void *d_input, int *layer_idx, int *op_kind,
     for (int rep = 0; rep < 2; ++rep) {   // second pass is the measured one
         CUDA_OK(cudaEventRecord(ev[0], s));
         for (int k = 0; k < n; ++k) {
-            if (k == 0) e->first_op(din, s);
-            else e->ops[k].launch(s);
+            e->ops[k].launch(din, s);
             CUDA_OK(cudaEventRecord(ev[k + 1], s));
         }
         CUDA_OK(cudaStreamSynchronize(s));
