@@ -143,16 +143,32 @@ float *yb_network_predict_quantized(yb_network *net, const float *input);
  * The bilinear resize to the network size is bit-identical to the reference's (scalar build).  The one-size case of
  * yb_network_predict_frames_u8. */
 float *yb_network_predict_image_u8(yb_network *net, const unsigned char *images_hwc, int w, int h, int quantized);
+
+/* Letterboxing of the frame calls (off by default).  Off, every call below that resizes frames (predict_image_u8,
+ * predict_frames_u8, submit_u8, submit_frames_u8, predict_device_frames, submit_device_frames) stretches each frame to the
+ * network size W x H.  On, it letterboxes each frame as darknet's letterbox_image does: a w x h frame is resized
+ * (resize_image, bit-identical to the reference) to its letterbox size nw x nh -- nw = W, nh = (h * W) / w when
+ * (float)W / w < (float)H / h, else nh = H, nw = (w * H) / h (correct_yolo_boxes' expression, src/additionally.c:4287-4294)
+ * -- and embedded at ((W - nw) / 2, (H - nh) / 2) in an input filled with 0.5.  A frame of the network's aspect ratio is
+ * the same input either way.  The switch takes effect at the next call, without an engine rebuild; a submitted ticket
+ * keeps the geometry it was submitted with.  The float-input calls are not affected.
+ * `letter` of the detection calls still only chooses the box correction: pass letter = 1 with letterboxing on to get boxes
+ * in frame coordinates (letter = 0 with it off).  With it on, a frame whose letterbox size has a side below 2 pixels (a
+ * 640 x 10 frame in a 64 x 64 network) is rejected before any device work, with the frame's index and letterbox size. */
+int yb_network_set_letterbox(yb_network *net, int on);
+
 /* 1 <= nimg <= net.batch 8-bit HWC frames (net.c channels), frame b is w[b] x h[b]; each is converted and resized exactly as
- * load_image_stb + resize_image do it (src/additionally.c:3021-3103), as the reference app does per image (src/main.c:188-229).
+ * load_image_stb + resize_image do it (src/additionally.c:3021-3103), as the reference app does per image (src/main.c:188-229),
+ * or letterboxed (yb_network_set_letterbox).
  * Batch items nimg .. batch-1 are zero images.  Each frame is copied to the device on its own (frames that lie back to back
  * in host memory in one copy); the copies overlap other work only when the frames are in pinned memory (yb_alloc_pinned),
  * pageable frames work but each copy then serialises.  Rejected before any device work: nimg outside 1..net.batch, a null
- * frames / w / h array or frame, w[b] < 1 or h[b] < 1, a frame of more than INT_MAX bytes. */
+ * frames / w / h array or frame, w[b] < 1 or h[b] < 1, a frame of more than INT_MAX bytes, and with letterboxing on a frame
+ * whose letterbox size has a side below 2. */
 float *yb_network_predict_frames_u8(yb_network *net, const unsigned char *const *frames, const int *w, const int *h,
                                     int nimg, int quantized);
 /* Diagnostic: the planar float input (batch*c*h*w) the device pipeline produced for the last predict_image_u8 /
- * predict_frames_u8 / predict_device_frames call. */
+ * predict_frames_u8 / predict_device_frames call (letterboxed when yb_network_set_letterbox is on). */
 int    yb_network_fetch_input(yb_network *net, int quantized, float *dst);
 
 /* Pipelined form of the two calls above for throughput serving: yb_network_submit enqueues one batch (H2D of
@@ -178,8 +194,9 @@ int yb_network_submit_u8(yb_network *net, const unsigned char *images_hwc, int w
 int yb_network_collect_detections(yb_network *net, int ticket, int quantized, const float **rows, const int **counts,
                                   size_t *d2h_bytes);
 /* The same serving loop for frames of different sizes and partial batches: 1 <= nimg <= net.batch frames, frame b is
- * w[b] x h[b], each resized as load_image + resize_image do it and its boxes corrected for its own size (correct_yolo_boxes
- * src/additionally.c:4281-4315), per image as in src/main.c:188-229.  Same slots, streams and ticket rules as
+ * w[b] x h[b], each resized as load_image + resize_image do it, or letterboxed (yb_network_set_letterbox, then pass
+ * letter = 1), and its boxes corrected for its own size (correct_yolo_boxes src/additionally.c:4281-4315), per image as in
+ * src/main.c:188-229.  Same slots, streams and ticket rules as
  * yb_network_submit_u8 (which is its one-size case); collected with yb_network_collect_detections, whose counts[b] is 0 for
  * b >= nimg.  When all nimg frames have the network size the stem reads the 8-bit frames directly.  Frames as in
  * yb_network_predict_frames_u8 (pinned memory for overlapped copies; untouched until the ticket is collected), same argument
@@ -200,7 +217,8 @@ int yb_network_submit_frames_u8(yb_network *net, const unsigned char *const *fra
  *                        half = 1 << 19:  R = clamp((yy + half + 1673527 v) >> 20),
  *                        G = clamp((yy + half - 852492 v - 409993 u) >> 20), B = clamp((yy + half + 2116026 u) >> 20),
  *                        clamped to 0..255.
- * Device frames are always resized by the kernel, also at the network size.  One format per call, 3-channel networks only. */
+ * Device frames are always resized by the kernel, also at the network size, and letterboxed like host frames when
+ * yb_network_set_letterbox is on.  One format per call, 3-channel networks only. */
 enum { YB_FRAME_RGB = 0, YB_FRAME_BGR = 1, YB_FRAME_RGB_PLANAR = 2, YB_FRAME_NV12 = 3 };
 
 typedef struct yb_device_frame {
@@ -229,8 +247,8 @@ float *yb_network_predict_device_frames(yb_network *net, const yb_device_frame *
  *
  * Rejected before any device work: nimg outside 1..net.batch, a null frames array, a null data (or, for NV12, chroma)
  * pointer, w < 1 or h < 1, an odd w or h for NV12, a pitch or plane_stride below its minimum, an unknown format, a
- * network whose input does not have 3 channels, a frame whose addressed span exceeds INT_MAX bytes, max_rows outside
- * 1..16384.  Then a frame that is not device or managed memory of the network's device (host, pinned host, or another
+ * network whose input does not have 3 channels, a frame whose addressed span exceeds INT_MAX bytes, with letterboxing on a
+ * frame whose letterbox size has a side below 2, max_rows outside 1..16384.  Then a frame that is not device or managed memory of the network's device (host, pinned host, or another
  * GPU's memory; cudaPointerGetAttributes) is rejected. */
 int yb_network_submit_device_frames(yb_network *net, const yb_device_frame *frames, int nimg, int format, int quantized,
                                     float thresh, float nms, int relative, int letter, int max_rows, void *stream);

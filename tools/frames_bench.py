@@ -11,7 +11,11 @@ stream that cycles 640x480 / 1280x720 / 1920x1080 (so every batch mixes three si
       sheet figure) as the time floor;
   (d) the card's name and power limit, read in the same run.
 
-  python tools/frames_bench.py [--batches 30] [--out result.json]
+With --letterbox it measures letterboxing instead (yb_network_set_letterbox): the same mixed stream through
+submit_frames_u8 with letterboxing on (letter = 1) against off (letter = 0), alternated for three pairs, and
+k_resize_frames' device time per mixed batch for each, in profiler passes of their own.
+
+  python tools/frames_bench.py [--batches 30] [--letterbox] [--out result.json]
 """
 import argparse
 import json
@@ -52,6 +56,7 @@ def run_pipeline(submit, collect, batches):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batches", type=int, default=30, help="mixed batches per timed pass (a multiple of 3)")
+    ap.add_argument("--letterbox", action="store_true", help="letterbox on against off instead of (a) - (c)")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     nb = max(3, a.batches // 3 * 3)
@@ -96,6 +101,12 @@ def main():
     def sub_grouped(b):
         return net.submit_u8(b, thresh, 0.45, max_rows=cap)
 
+    if a.letterbox:
+        res = letterbox_leg(net, mixed, thresh, cap, collect, nimg, nb)
+        res["card"] = card()
+        emit(res, a.out)
+        return
+
     run_pipeline(sub_mixed, collect, mixed[:6])          # warm-up: engine, slots, buffers, both paths
     run_pipeline(sub_grouped, collect, grouped[:6])
     ta, tb = [], []
@@ -104,14 +115,7 @@ def main():
         tb.append(run_pipeline(sub_grouped, collect, grouped))
 
     # (c) resize kernel time: its own pass under the profiler
-    import torch
-    from torch.profiler import ProfilerActivity, profile
-    torch.cuda.init()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        run_pipeline(sub_mixed, collect, mixed[:12])
-        torch.cuda.synchronize()
-    ks = [e for e in prof.events() if "k_resize_frames" in e.name]
-    dev_us = [e.device_time if hasattr(e, "device_time") else e.cuda_time for e in ks]
+    dev_us = resize_times(sub_mixed, collect, mixed[:12])
     resize_us = float(np.mean(dev_us)) if dev_us else float("nan")
     bytes_per_batch = sum(f.size for b in mixed for f in b) / nb + 12 * NET * NET * BATCH
     floor_us = bytes_per_batch / HBM_BPS * 1e6
@@ -130,11 +134,60 @@ def main():
         "c_resize_hbm_floor_us": round(floor_us, 1),
         "c_resize_share_of_hbm_floor": round(floor_us / resize_us, 3) if dev_us else None,
     }
+    emit(res, a.out)
+
+
+def resize_times(submit, collect, batches):
+    """k_resize_frames' device time (us) of each launch of one pipelined pass, under torch.profiler."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    torch.cuda.init()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        run_pipeline(submit, collect, batches)
+        torch.cuda.synchronize()
+    ks = [e for e in prof.events() if "k_resize_frames" in e.name]
+    return [e.device_time if hasattr(e, "device_time") else e.cuda_time for e in ks]
+
+
+def letterbox_leg(net, mixed, thresh, cap, collect, nimg, nb):
+    """The mixed stream letterboxed (letter = 1) against stretched (letter = 0), alternated; then k_resize_frames per batch
+    for each in a profiler pass of its own."""
+    def submitter(on):
+        def sub(b):
+            net.set_letterbox(on)
+            return net.submit_frames_u8(b, thresh, 0.45, letter=int(on), max_rows=cap)
+        return sub
+
+    sub_on, sub_off = submitter(True), submitter(False)
+    run_pipeline(sub_on, collect, mixed[:6])            # warm-up both
+    run_pipeline(sub_off, collect, mixed[:6])
+    t_on, t_off = [], []
+    for _ in range(3):
+        t_off.append(run_pipeline(sub_off, collect, mixed))
+        t_on.append(run_pipeline(sub_on, collect, mixed))
+    us_off = resize_times(sub_off, collect, mixed[:12])
+    us_on = resize_times(sub_on, collect, mixed[:12])
+    net.set_letterbox(False)
+    return {
+        "workload": f"yolov3-{NET} b{BATCH} bf16, pinned 8-bit frames cycling "
+                    + " / ".join(f"{w}x{h}" for w, h in SIZES) + ", three tickets in flight, letterbox on vs off",
+        "images_per_pass": nimg,
+        "batches_per_pass": nb,
+        "det_thresh": thresh,
+        "stretched_submit_frames_u8_img_s": [round(nimg / t, 1) for t in t_off],
+        "letterboxed_submit_frames_u8_img_s": [round(nimg / t, 1) for t in t_on],
+        "resize_launches_profiled": [len(us_off), len(us_on)],
+        "stretched_resize_us_per_batch": round(float(np.mean(us_off)), 1) if us_off else None,
+        "letterboxed_resize_us_per_batch": round(float(np.mean(us_on)), 1) if us_on else None,
+    }
+
+
+def emit(res, out):
     line = json.dumps(res)
     print(line)
-    if a.out:
-        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-        open(a.out, "w").write(line + "\n")
+    if out:
+        os.makedirs(os.path.dirname(os.path.abspath(out)), exist_ok=True)
+        open(out, "w").write(line + "\n")
 
 
 if __name__ == "__main__":

@@ -97,6 +97,7 @@ def lib():
         "yb_network_set_device": (C.c_int, [vp, C.c_int]),
         "yb_network_set_precision": (C.c_int, [vp, C.c_int]),
         "yb_network_set_option": (C.c_int, [vp, C.c_char_p, C.c_int]),
+        "yb_network_set_letterbox": (C.c_int, [vp, C.c_int]),
         "yb_network_get_info": (C.c_long, [vp, C.c_int, C.c_char_p]),
         "yb_network_tc_plan": (C.c_int, [vp, C.c_int, C.c_int, ip, C.c_int]),
         "yb_network_calibrate": (C.c_int, [vp, vp, vp, C.c_int]),
@@ -161,7 +162,7 @@ EXPORTED_SYMBOLS = [
     "yb_free_pinned", "yb_network_submit_u8", "yb_network_collect_detections", "yb_network_set_devices",
     "yb_network_predict_batch", "yb_network_batch_output", "yb_network_replication", "yb_network_predict_frames_u8",
     "yb_network_detect_frames", "yb_network_submit_frames_u8", "yb_network_predict_device_frames",
-    "yb_network_submit_device_frames",
+    "yb_network_submit_device_frames", "yb_network_set_letterbox",
 ]
 
 
@@ -254,6 +255,11 @@ class Network:
 
     def set_option(self, name: str, value: int):
         _check(lib().yb_network_set_option(self._h, name.encode(), value) == 0)
+
+    def set_letterbox(self, on: bool):
+        """Letterbox frames instead of stretching them in every frame call (``yb_network_set_letterbox``); pass
+        ``letter=1`` to the detection calls to get boxes in frame coordinates.  Takes effect at the next call."""
+        _check(lib().yb_network_set_letterbox(self._h, int(bool(on))) == 0)
 
     def get_info(self, key: str, quantized: bool = False) -> int:
         return int(lib().yb_network_get_info(self._h, int(quantized), key.encode()))

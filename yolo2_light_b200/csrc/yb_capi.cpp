@@ -231,6 +231,11 @@ int yb_network_set_option(yb_network *n, const char *name, int value) {
     return 0;
 }
 
+int yb_network_set_letterbox(yb_network *n, int on) {
+    n->net.letterbox = on != 0;   // read by each frame call when it fills its geometry table: no engine rebuild
+    return 0;
+}
+
 long yb_network_get_info(yb_network *n, int quantized, const char *key) {
     YB_TRY
     return engine_info(get_engine(n, quantized), key);
@@ -277,6 +282,18 @@ int yb_network_collect(yb_network *n, int ticket, int quantized) {
 
 }  // extern "C"
 
+// With letterboxing on, a frame whose letterbox size has a side below 2 is refused: resize_image divides by that side
+// minus 1 (additionally.c:3027-3028).
+static void check_letterbox(const Network &net, const std::string &fb, int w, int h) {
+    if (!net.letterbox) return;
+    int nw, nh;
+    letterbox_size(net.w, net.h, w, h, &nw, &nh);
+    if (nw < 2 || nh < 2)
+        fatal_throw(fb + " (" + std::to_string(w) + "x" + std::to_string(h) + ") letterboxes to " + std::to_string(nw) + "x" +
+                    std::to_string(nh) + " in the " + std::to_string(net.w) + "x" + std::to_string(net.h) +
+                    " network; letterboxing needs at least 2 pixels on each side");
+}
+
 // Argument checks of the frame entry points, all before any device work.  frames_call false: the decode-only call, which
 // takes sizes alone.
 static void check_sizes(const Network &net, const char *fn, const int *w, const int *h, int nimg, bool frames_call,
@@ -293,6 +310,7 @@ static void check_sizes(const Network &net, const char *fn, const int *w, const 
         // the resize indexes within a frame in 32 bits
         if (frames_call && (long long)w[b] * h[b] * net.c > INT_MAX)
             fatal_throw(f + ": frame " + std::to_string(b) + " has more than INT_MAX bytes");
+        if (frames_call) check_letterbox(net, f + ": frame " + std::to_string(b), w[b], h[b]);
     }
 }
 static void check_max_rows(const char *fn, int max_rows) {
@@ -328,6 +346,7 @@ static void check_device_frames(const Network &net, const char *fn, const yb_dev
             span += 2 * d.plane_stride;
         }
         if (span > INT_MAX) fatal_throw(fb + " addresses more than INT_MAX bytes");
+        check_letterbox(net, fb, d.w, d.h);
     }
 }
 

@@ -1033,8 +1033,10 @@ void engine_upload_input(Engine *e, const float *host_input, void *stream) {
     CUDA_OK(cudaMemcpyAsync(e->d_input.get(), host_input, e->d_input.count() * sizeof(float), cudaMemcpyHostToDevice, s));
 }
 
-// The per-image table: frame sizes, the resize's scales, and the size correct_yolo_boxes (additionally.c:4287-4296) embeds each image at -- the
-// network size, or with `letter` the reference's integer letterbox size of that image.  Entries nimg .. batch-1 are zero.
+// The per-image table: frame sizes; the resize target, its offset and the resize's scales -- the network size at (0, 0), or
+// with net->letterbox the letterbox size, centred (embed_image's integer offsets); and the size correct_yolo_boxes
+// (additionally.c:4287-4296) embeds each image at -- the network size, or with `letter` the letterbox size.  Entries
+// nimg .. batch-1 are zero.
 static void fill_geo(Engine *e, Engine::FrameStage &st, const Network *net, const int *w, const int *h, int nimg, int letter) {
     const int B = e->batch;
     st.h_geo.ensure(B);
@@ -1043,13 +1045,14 @@ static void fill_geo(Engine *e, Engine::FrameStage &st, const Network *net, cons
         ImageGeo &g = st.h_geo.get()[b];
         g = ImageGeo{};
         if (b >= nimg) continue;
-        g.w = w[b]; g.h = h[b]; g.new_w = net->w; g.new_h = net->h;
-        g.w_scale = (float)(g.w - 1) / (float)(net->w - 1);   // resize_image, additionally.c:3027-3028
-        g.h_scale = (float)(g.h - 1) / (float)(net->h - 1);
-        if (letter) {
-            if (((float)net->w / g.w) < ((float)net->h / g.h)) { g.new_w = net->w; g.new_h = (g.h * net->w) / g.w; }
-            else { g.new_h = net->h; g.new_w = (g.w * net->h) / g.h; }
-        }
+        g.w = w[b]; g.h = h[b];
+        int lw, lh;
+        letterbox_size(net->w, net->h, g.w, g.h, &lw, &lh);
+        g.new_w = letter ? lw : net->w; g.new_h = letter ? lh : net->h;
+        g.nw = net->letterbox ? lw : net->w; g.nh = net->letterbox ? lh : net->h;
+        g.dx = (net->w - g.nw) / 2; g.dy = (net->h - g.nh) / 2;
+        g.w_scale = (float)(g.w - 1) / (float)(g.nw - 1);   // resize_image, additionally.c:3027-3028
+        g.h_scale = (float)(g.h - 1) / (float)(g.nh - 1);
     }
 }
 

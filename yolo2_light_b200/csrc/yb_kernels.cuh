@@ -95,6 +95,11 @@ __global__ void k_nhwc_to_nchw_f32(TV in, float *__restrict__ out) {
 // the chroma span of each source row and converts them to RGB bytes in shared memory, once per source pixel, with
 // BT.601 limited-range fixed-point arithmetic (OpenCV's COLOR_YUV2RGB_NV12 constants).  The interpolation that follows
 // is the same for every format, so a device frame gives bit-for-bit what its RGB equivalent gives through the host path.
+//
+// Letterboxing (darknet's letterbox_image: resize to the letterbox size, fill_image(.5), embed_image): each image resizes
+// to its target nw x nh (ImageGeo), placed at (dx, dy) of the out_w x out_h input.  Rows outside [dy, dy + nh) are 0.5 in
+// every channel and stage nothing; inside, the columns outside [dx, dx + nw) are 0.5.  Without letterboxing the target is
+// the whole input at (0, 0), and the kernel computes exactly the stretched resize.
 // ------------------------------------------------------------------------------------------------------
 struct ImageGeo {               // one image of a batch (device table, uploaded with the frames)
     const unsigned char *src;   // RGB / BGR: first pixel; planar: the R plane; NV12: the Y plane
@@ -102,8 +107,10 @@ struct ImageGeo {               // one image of a batch (device table, uploaded 
     long long plane;            // planar: bytes from one plane to the next
     int pitch;                  // bytes from one row to the next
     int w, h;                   // frame size
-    int new_w, new_h;           // correct_yolo_boxes' embedded size (the network size unless letterboxed)
-    float w_scale, h_scale;     // resize_image's (w - 1) / (out_w - 1), (h - 1) / (out_h - 1): IEEE float divides, made
+    int new_w, new_h;           // correct_yolo_boxes' embedded size (the network size unless `letter`)
+    int nw, nh, dx, dy;         // resize target and its offset in the network input: the network size at (0, 0), or with
+                                // letterboxing on the letterbox size at ((W - nw) / 2, (H - nh) / 2)
+    float w_scale, h_scale;     // resize_image's (w - 1) / (nw - 1), (h - 1) / (nh - 1): IEEE float divides, made
                                 // on the host so that the kernel has no divide
 };
 
@@ -168,31 +175,43 @@ static __global__ void __launch_bounds__(RS_THREADS) k_resize_frames(const Image
     const int c = F == YB_FRAME_RGB ? c_ : 3;
     const int n = blockIdx.y;
     const ImageGeo g = geo[n];
-    const int w = g.w, h = g.h;
+    const int w = g.w, h = g.h, tw = g.nw, th = g.nh;   // frame and resize target
     float *out = dst + (size_t)n * c * out_h * out_w;
     const size_t plane = (size_t)out_h * out_w;
-    const bool same = (out_w == w && out_h == h);
+    const bool same = (tw == w && th == h);
     const float w_scale = g.w_scale, h_scale = g.h_scale;
-    const int r_end = min(out_h, (int)(blockIdx.x + 1) * RS_ROWS);
-    for (int r = blockIdx.x * RS_ROWS; r < r_end; ++r) {
-        int iy = r;
+    const int r0 = blockIdx.x * RS_ROWS, r_end = min(out_h, r0 + RS_ROWS);
+    // letterbox: 0.5 in the bands above and below the image and in the columns left and right of it (none when stretched)
+    for (int r = r0; r < r_end; ++r) {
+        const bool band = r < g.dy || r >= g.dy + th;
+        const int nfill = band ? out_w : out_w - tw;
+        for (int cc = threadIdx.x; cc < nfill; cc += RS_THREADS) {
+            const int x = band || cc < g.dx ? cc : cc + tw;
+#pragma unroll 1
+            for (int k = 0; k < c; ++k) out[k * plane + (size_t)r * out_w + x] = 0.5f;
+        }
+    }
+    for (int r = max(r0, g.dy), r1 = min(r_end, g.dy + th); r < r1; ++r) {   // the image's rows
+        const int tr = r - g.dy;                            // row of the target
+        float *orow = out + (size_t)r * out_w + g.dx;
+        int iy = tr;
         float dy = 0.f;
         bool two = false;
         if (!same) {
-            const float sy = __fmul_rn((float)r, h_scale);
+            const float sy = __fmul_rn((float)tr, h_scale);
             iy = (int)sy;
             dy = __fsub_rn(sy, (float)iy);
-            two = !(r == out_h - 1 || h == 1);
+            two = !(tr == th - 1 || h == 1);
         }
-        for (int cc0 = 0; cc0 < out_w; cc0 += RS_COLS) {
-            const int cc1 = min(out_w, cc0 + RS_COLS) - 1;      // last column of this chunk
+        for (int cc0 = 0; cc0 < tw; cc0 += RS_COLS) {
+            const int cc1 = min(tw, cc0 + RS_COLS) - 1;         // last column of this chunk
             // source columns the chunk reads: ix(cc0) .. ix(cc1) + 1, or the last column
             int lo, hi;
             if (same) { lo = cc0; hi = cc1; }
             else if (w == 1) { lo = hi = 0; }
             else {
-                lo = cc0 == out_w - 1 ? w - 1 : (int)__fmul_rn((float)cc0, w_scale);
-                hi = cc1 == out_w - 1 ? w - 1 : (int)__fmul_rn((float)cc1, w_scale) + 1;
+                lo = cc0 == tw - 1 ? w - 1 : (int)__fmul_rn((float)cc0, w_scale);
+                hi = cc1 == tw - 1 ? w - 1 : (int)__fmul_rn((float)cc1, w_scale) + 1;
             }
             const int npix = hi - lo + 1, len = npix * c;
             const unsigned char *row[2] = {g.src + (size_t)iy * g.pitch, g.src + (size_t)(iy + two) * g.pitch};
@@ -247,13 +266,13 @@ static __global__ void __launch_bounds__(RS_THREADS) k_resize_frames(const Image
             }
             const RsSrc &p0 = src[0], &p1 = src[1];
             for (int cc = cc0 + threadIdx.x; cc <= cc1; cc += RS_THREADS) {
-                float *o = out + (size_t)r * out_w + cc;
+                float *o = orow + cc;
                 if (same) {
                     for (int k = 0; k < c; ++k) o[k * plane] = unit[rs_px<F>(p0, staged, c, cc - lo, k)];
                     continue;
                 }
                 // the reference's `part` image at (cc, row): the last column (or a 1-pixel-wide frame) copies the edge
-                const bool edge = cc == out_w - 1 || w == 1;
+                const bool edge = cc == tw - 1 || w == 1;
                 int xa = w - 1 - lo;
                 float dx = 0.f;
                 if (!edge) {

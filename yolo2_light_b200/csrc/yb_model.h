@@ -51,7 +51,15 @@ struct Network {
     bool fuse = true;          // conv+shortcut fusion / route aliasing (diagnostic switch)
     bool keep_counts = false;  // keep raw XNOR popcounts / INT8 accumulators (tests)
     int q_index_offset = 0;    // see EngineOptions
+    bool letterbox = false;    // frame calls letterbox instead of stretching (yb_network_set_letterbox); read per call
 };
+
+// The integer size darknet's letterbox gives a w x h frame in a netw x neth network (correct_yolo_boxes,
+// additionally.c:4287-4294): the side that limits the scale takes the network's size, the other keeps the aspect ratio.
+inline void letterbox_size(int netw, int neth, int w, int h, int *nw, int *nh) {
+    if (((float)netw / w) < ((float)neth / h)) { *nw = netw; *nh = (h * netw) / w; }
+    else { *nh = neth; *nw = (w * neth) / h; }
+}
 
 // error plumbing shared by all translation units
 [[noreturn]] void fatal_throw(const std::string &msg);   // throws yb::Error
