@@ -294,71 +294,108 @@ static void check_letterbox(const Network &net, const std::string &fb, int w, in
                     " network; letterboxing needs at least 2 pixels on each side");
 }
 
-// Argument checks of the frame entry points, all before any device work.  frames_call false: the decode-only call, which
-// takes sizes alone.
-static void check_sizes(const Network &net, const char *fn, const int *w, const int *h, int nimg, bool frames_call,
-                        const unsigned char *const *frames) {
-    const std::string f(fn);
+// Argument checks of the frame entry points, all before any device work.
+static void check_nimg(const Network &net, const std::string &f, int nimg) {
     if (nimg < 1 || nimg > net.batch)
         fatal_throw(f + ": nimg " + std::to_string(nimg) + " outside 1.." + std::to_string(net.batch) + " (net.batch)");
+}
+// The decode-only call, which takes sizes alone.
+static void check_sizes(const Network &net, const char *fn, const int *w, const int *h, int nimg) {
+    const std::string f(fn);
+    check_nimg(net, f, nimg);
     if (!w || !h) fatal_throw(f + ": null w / h array");
-    if (frames_call && !frames) fatal_throw(f + ": null frames array");
-    for (int b = 0; b < nimg; ++b) {
-        if (frames_call && !frames[b]) fatal_throw(f + ": frame " + std::to_string(b) + " is null");
+    for (int b = 0; b < nimg; ++b)
         if (w[b] < 1 || h[b] < 1)
             fatal_throw(f + ": frame " + std::to_string(b) + " has size " + std::to_string(w[b]) + "x" + std::to_string(h[b]));
-        // the resize indexes within a frame in 32 bits
-        if (frames_call && (long long)w[b] * h[b] * net.c > INT_MAX)
-            fatal_throw(f + ": frame " + std::to_string(b) + " has more than INT_MAX bytes");
-        if (frames_call) check_letterbox(net, f + ": frame " + std::to_string(b), w[b], h[b]);
-    }
 }
 static void check_max_rows(const char *fn, int max_rows) {
     if (max_rows <= 0 || max_rows > DET_MAX_ROWS)
         fatal_throw(std::string(fn) + ": max_rows must be in 1.." + std::to_string(DET_MAX_ROWS));
 }
-// The device-frame calls: everything but the memory kind (check_frame_memory), without touching the device.
-static void check_device_frames(const Network &net, const char *fn, const yb_device_frame *frames, int nimg, int format) {
+// The frame calls: everything but the memory kind of device frames (check_frame_memory), without touching the device.
+static void check_frames(const Network &net, const char *fn, const FrameBatch &batch) {
     const std::string f(fn);
-    if (nimg < 1 || nimg > net.batch)
-        fatal_throw(f + ": nimg " + std::to_string(nimg) + " outside 1.." + std::to_string(net.batch) + " (net.batch)");
-    if (!frames) fatal_throw(f + ": null frames array");
+    check_nimg(net, f, batch.nimg);
+    if (!batch.frames) fatal_throw(f + ": null frames array");
+    const int format = batch.fmt;
     if (format < YB_FRAME_RGB || format > YB_FRAME_NV12) fatal_throw(f + ": unknown frame format " + std::to_string(format));
-    if (net.c != 3)
+    if (!batch.host && net.c != 3)
         fatal_throw(f + ": device frames have 3 channels, the network's input has " + std::to_string(net.c));
     const bool nv12 = format == YB_FRAME_NV12;
-    for (int b = 0; b < nimg; ++b) {
-        const yb_device_frame &d = frames[b];
+    for (int b = 0; b < batch.nimg; ++b) {
+        const yb_device_frame &d = batch.frames[b];
         const std::string fb = f + ": frame " + std::to_string(b);
         if (!d.data) fatal_throw(fb + " is null");
         if (nv12 && !d.chroma) fatal_throw(fb + " has a null chroma plane");
         if (d.w < 1 || d.h < 1) fatal_throw(fb + " has size " + std::to_string(d.w) + "x" + std::to_string(d.h));
         if (nv12 && (d.w % 2 || d.h % 2))
             fatal_throw(fb + " has size " + std::to_string(d.w) + "x" + std::to_string(d.h) + ", NV12 needs an even width and height");
-        const long long row = format == YB_FRAME_RGB || format == YB_FRAME_BGR ? 3LL * d.w : d.w;
-        if (d.pitch < row)
-            fatal_throw(fb + " has pitch " + std::to_string(d.pitch) + " below its row of " + std::to_string(row) + " bytes");
-        long long span = (long long)(d.h - 1) * d.pitch + row;   // the resize indexes within a frame in 32 bits
+        // net.c bytes per packed pixel: 3 for device frames
+        const long long row = format == YB_FRAME_RGB || format == YB_FRAME_BGR ? (long long)net.c * d.w : d.w;
+        const long long pitch = batch.host ? row : d.pitch;   // host frames are packed (host_frame)
+        if (pitch < row)
+            fatal_throw(fb + " has pitch " + std::to_string(pitch) + " below its row of " + std::to_string(row) + " bytes");
+        long long span = (d.h - 1) * pitch + row;   // the resize indexes within a frame in 32 bits
         if (format == YB_FRAME_RGB_PLANAR) {
-            if (d.plane_stride < (long long)d.pitch * d.h)
+            if (d.plane_stride < pitch * d.h)
                 fatal_throw(fb + " has plane_stride " + std::to_string(d.plane_stride) + " below pitch * h = " +
-                            std::to_string((long long)d.pitch * d.h));
+                            std::to_string(pitch * d.h));
             span += 2 * d.plane_stride;
         }
-        if (span > INT_MAX) fatal_throw(fb + " addresses more than INT_MAX bytes");
+        if (span > INT_MAX) fatal_throw(fb + (batch.host ? " has" : " addresses") + " more than INT_MAX bytes");
         check_letterbox(net, fb, d.w, d.h);
     }
 }
 
-// net.batch frames of one size, stacked: the uniform case of the frame entry points
-struct Uniform {
-    std::vector<const unsigned char *> frames;
-    std::vector<int> w, h;
-    Uniform(const Network &net, const unsigned char *images_hwc, int w_, int h_)
-        : frames(net.batch), w(net.batch, w_), h(net.batch, h_) {
-        for (int b = 0; b < net.batch; ++b) frames[b] = images_hwc + (size_t)b * w_ * h_ * net.c;
+// A host frame of w x h pixels of net.c bytes as an RGB frame of pitch w * net.c.  A frame whose pitch is not an int is
+// refused by check_frames (by its size or its span); its pitch is left 0.
+static yb_device_frame host_frame(const Network &net, const unsigned char *data, int w, int h) {
+    const long long pitch = (long long)w * net.c;
+    return yb_device_frame{data, nullptr, w, h, pitch > 0 && pitch <= INT_MAX ? (int)pitch : 0, 0};
+}
+
+// The frames of a host frame call as a batch
+struct HostFrames {
+    std::vector<yb_device_frame> table;
+    FrameBatch batch{};
+    // nimg frames, frame b w[b] x h[b]; the arrays are read once nimg, w and h have passed, and a null frames array is left
+    // to check_frames
+    HostFrames(const Network &net, const char *fn, const unsigned char *const *frames, const int *w, const int *h, int nimg) {
+        check_nimg(net, fn, nimg);
+        if (!w || !h) fatal_throw(std::string(fn) + ": null w / h array");
+        for (int b = 0; frames && b < nimg; ++b) table.push_back(host_frame(net, frames[b], w[b], h[b]));
+        batch = FrameBatch{frames ? table.data() : nullptr, nimg, YB_FRAME_RGB, true};
+    }
+    // net.batch frames of one size, stacked
+    HostFrames(const Network &net, const unsigned char *images_hwc, int w, int h) {
+        for (int b = 0; b < net.batch; ++b) table.push_back(host_frame(net, images_hwc + (size_t)b * w * h * net.c, w, h));
+        batch = FrameBatch{table.data(), net.batch, YB_FRAME_RGB, true};
     }
 };
+
+// The synchronous and the pipelined frame call: checks, then the resize and the forward (+ decode and NMS).
+static float *predict_frames(yb_network *n, const char *fn, const FrameBatch &b, int quantized, void *stream) {
+    Network &net = n->net;
+    check_frames(net, fn, b);
+    if (!b.host) check_frame_memory(net.device, fn, b);
+    Engine *e = get_engine(n, quantized);
+    engine_upload_frames(e, &net, b, stream);
+    engine_forward(e, nullptr, nullptr);
+    engine_download_outputs(e, &net, nullptr);
+    net.last_launches = engine_num_launches(e) + 1;   // + resize
+    return net.layers.back().output;
+}
+static int submit_frames(yb_network *n, const char *fn, const FrameBatch &b, int quantized, float thresh, float nms,
+                         int relative, int letter, int max_rows, void *stream) {
+    Network &net = n->net;
+    check_frames(net, fn, b);
+    check_max_rows(fn, max_rows);
+    if (!b.host) check_frame_memory(net.device, fn, b);
+    Engine *e = get_engine(n, quantized);
+    const int t = engine_submit_frames(e, &net, b, thresh, nms, relative, letter, max_rows, stream);
+    net.last_launches = engine_num_launches(e) + 5;   // + resize, count, emit, iou, nms
+    return t;
+}
 
 extern "C" {
 
@@ -366,20 +403,15 @@ int yb_network_submit_u8(yb_network *n, const unsigned char *images_hwc, int w, 
                          int relative, int letter, int max_rows) {
     YB_TRY
     if (w <= 0 || h <= 0 || !images_hwc) fatal_throw("submit_u8: bad image");
-    const Uniform u(n->net, images_hwc, w, h);
-    return yb_network_submit_frames_u8(n, u.frames.data(), u.w.data(), u.h.data(), n->net.batch, quantized, thresh, nms,
-                                       relative, letter, max_rows);
+    const HostFrames u(n->net, images_hwc, w, h);
+    return submit_frames(n, "submit_frames_u8", u.batch, quantized, thresh, nms, relative, letter, max_rows, nullptr);
     YB_CATCH(-1)
 }
 int yb_network_submit_frames_u8(yb_network *n, const unsigned char *const *frames, const int *w, const int *h, int nimg,
                                 int quantized, float thresh, float nms, int relative, int letter, int max_rows) {
     YB_TRY
-    check_sizes(n->net, "submit_frames_u8", w, h, nimg, true, frames);
-    check_max_rows("submit_frames_u8", max_rows);
-    Engine *e = get_engine(n, quantized);
-    const int t = engine_submit_frames(e, &n->net, frames, w, h, nimg, thresh, nms, relative, letter, max_rows);
-    n->net.last_launches = engine_num_launches(e) + 5;   // + resize, count, emit, iou, nms
-    return t;
+    const HostFrames hf(n->net, "submit_frames_u8", frames, w, h, nimg);
+    return submit_frames(n, "submit_frames_u8", hf.batch, quantized, thresh, nms, relative, letter, max_rows, nullptr);
     YB_CATCH(-1)
 }
 int yb_network_collect_detections(yb_network *n, int ticket, int quantized, const float **rows, const int **counts,
@@ -392,47 +424,28 @@ int yb_network_collect_detections(yb_network *n, int ticket, int quantized, cons
 float *yb_network_predict_image_u8(yb_network *n, const unsigned char *images_hwc, int w, int h, int quantized) {
     YB_TRY
     if (w <= 0 || h <= 0) fatal_throw("predict_image_u8: bad image size");
-    const Uniform u(n->net, images_hwc, w, h);
-    return yb_network_predict_frames_u8(n, u.frames.data(), u.w.data(), u.h.data(), n->net.batch, quantized);
+    const HostFrames u(n->net, images_hwc, w, h);
+    return predict_frames(n, "predict_frames_u8", u.batch, quantized, nullptr);
     YB_CATCH(nullptr)
 }
 float *yb_network_predict_frames_u8(yb_network *n, const unsigned char *const *frames, const int *w, const int *h, int nimg,
                                     int quantized) {
     YB_TRY
-    Network &net = n->net;
-    check_sizes(net, "predict_frames_u8", w, h, nimg, true, frames);
-    Engine *e = get_engine(n, quantized);
-    engine_upload_frames(e, &net, frames, w, h, nimg);
-    engine_forward(e, nullptr, nullptr);
-    engine_download_outputs(e, &net, nullptr);
-    net.last_launches = engine_num_launches(e) + 1;
-    return net.layers.back().output;
+    const HostFrames hf(n->net, "predict_frames_u8", frames, w, h, nimg);
+    return predict_frames(n, "predict_frames_u8", hf.batch, quantized, nullptr);
     YB_CATCH(nullptr)
 }
 float *yb_network_predict_device_frames(yb_network *n, const yb_device_frame *frames, int nimg, int format, int quantized,
                                         void *stream) {
     YB_TRY
-    Network &net = n->net;
-    check_device_frames(net, "predict_device_frames", frames, nimg, format);
-    check_frame_memory(net.device, "predict_device_frames", frames, nimg, format);
-    Engine *e = get_engine(n, quantized);
-    engine_upload_device_frames(e, &net, frames, nimg, format, stream);
-    engine_forward(e, nullptr, nullptr);
-    engine_download_outputs(e, &net, nullptr);
-    net.last_launches = engine_num_launches(e) + 1;
-    return net.layers.back().output;
+    return predict_frames(n, "predict_device_frames", FrameBatch{frames, nimg, format, false}, quantized, stream);
     YB_CATCH(nullptr)
 }
 int yb_network_submit_device_frames(yb_network *n, const yb_device_frame *frames, int nimg, int format, int quantized,
                                     float thresh, float nms, int relative, int letter, int max_rows, void *stream) {
     YB_TRY
-    check_device_frames(n->net, "submit_device_frames", frames, nimg, format);
-    check_max_rows("submit_device_frames", max_rows);
-    check_frame_memory(n->net.device, "submit_device_frames", frames, nimg, format);
-    Engine *e = get_engine(n, quantized);
-    const int t = engine_submit_device_frames(e, &n->net, frames, nimg, format, thresh, nms, relative, letter, max_rows, stream);
-    n->net.last_launches = engine_num_launches(e) + 5;   // + resize, count, emit, iou, nms
-    return t;
+    return submit_frames(n, "submit_device_frames", FrameBatch{frames, nimg, format, false}, quantized, thresh, nms, relative,
+                         letter, max_rows, stream);
     YB_CATCH(-1)
 }
 /* diagnostic: the resized planar float images the device pipeline produced for the last predict_image_u8 */
@@ -638,7 +651,7 @@ int yb_network_detect(yb_network *n, int quantized, int w, int h, float thresh, 
 int yb_network_detect_frames(yb_network *n, int quantized, const int *w, const int *h, int nimg, float thresh, float nms,
                              int relative, int letter, float *rows, int max_rows, int *counts) {
     YB_TRY
-    check_sizes(n->net, "detect_frames", w, h, nimg, false, nullptr);
+    check_sizes(n->net, "detect_frames", w, h, nimg);
     check_max_rows("detect_frames", max_rows);
     return engine_detect(get_engine(n, quantized), &n->net, w, h, nimg, thresh, nms, relative, letter, rows, max_rows, counts);
     YB_CATCH(-1)

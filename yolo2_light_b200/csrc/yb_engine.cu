@@ -1056,50 +1056,6 @@ static void fill_geo(Engine *e, Engine::FrameStage &st, const Network *net, cons
     }
 }
 
-// Enqueues on `s` the copies of nimg host frames (frame b: w[b] x h[b] x c bytes) into st.buf, packed back to back, and of the
-// per-image table.  Frames that lie back to back in host memory go in one copy (a stacked batch is one copy); each copy
-// overlaps other work only from pinned memory.  Returns true when every frame has the network size.
-static bool stage_frames(Engine *e, Engine::FrameStage &st, const Network *net, const unsigned char *const *frames,
-                         const int *w, const int *h, int nimg, int letter, cudaStream_t s) {
-    const int B = e->batch, c = net->c;
-    fill_geo(e, st, net, w, h, nimg, letter);
-    std::vector<size_t> off(nimg);
-    size_t total = 0;
-    bool net_size = true;
-    for (int b = 0; b < nimg; ++b) {
-        off[b] = total;
-        total += (size_t)w[b] * h[b] * c;
-        net_size &= w[b] == net->w && h[b] == net->h;
-    }
-    // room for a zero tail of network-size frames (the 8-bit stem reads whole batches)
-    const size_t need = std::max(total, net_size ? (size_t)B * net->w * net->h * c : 0);
-    st.buf.ensure(need);
-    ImageGeo *geo = st.h_geo.get();
-    for (int b = 0; b < nimg; ++b) { geo[b].src = st.buf.get() + off[b]; geo[b].pitch = w[b] * c; }
-    for (int b = 0; b < nimg;) {
-        size_t run = (size_t)w[b] * h[b] * c;
-        int nb = b + 1;
-        while (nb < nimg && frames[nb] == frames[b] + run) run += (size_t)w[nb] * h[nb] * c, ++nb;
-        CUDA_OK(cudaMemcpyAsync(st.buf.get() + off[b], frames[b], run, cudaMemcpyHostToDevice, s));
-        b = nb;
-    }
-    CUDA_OK(cudaMemcpyAsync(st.d_geo.get(), geo, (size_t)B * sizeof(ImageGeo), cudaMemcpyHostToDevice, s));
-    return net_size;
-}
-
-// The table of nimg caller's device frames (each entry points at the frame where it lies), enqueued on `s`.
-static void stage_device_frames(Engine *e, Engine::FrameStage &st, const Network *net, const yb_device_frame *frames,
-                                int nimg, int letter, cudaStream_t s) {
-    std::vector<int> w(nimg), h(nimg);
-    for (int b = 0; b < nimg; ++b) { w[b] = frames[b].w; h[b] = frames[b].h; }
-    fill_geo(e, st, net, w.data(), h.data(), nimg, letter);
-    for (int b = 0; b < nimg; ++b) {
-        ImageGeo &g = st.h_geo.get()[b];
-        g.src = frames[b].data; g.chroma = frames[b].chroma; g.pitch = frames[b].pitch; g.plane = frames[b].plane_stride;
-    }
-    CUDA_OK(cudaMemcpyAsync(st.d_geo.get(), st.h_geo.get(), (size_t)e->batch * sizeof(ImageGeo), cudaMemcpyHostToDevice, s));
-}
-
 // frames described by st.d_geo, of format fmt -> the network's planar f32 input; images nimg .. batch-1 are zero
 static void launch_resize(Engine *e, const Engine::FrameStage &st, const Network *net, int nimg, int fmt, float *dst,
                           cudaStream_t s) {
@@ -1118,42 +1074,66 @@ static void launch_resize(Engine *e, const Engine::FrameStage &st, const Network
     if (nimg < e->batch) CUDA_OK(cudaMemsetAsync(dst + nimg * per, 0, (e->batch - nimg) * per * sizeof(float), s));
 }
 
-// The caller's device frames -> dst, on the engine stream `s`: the table goes up, `s` waits for the work enqueued on the
-// caller's stream `user` before the call (the frames' producer), the resize reads the frames, and `user` waits for that
-// resize, so that the caller's later writes into the frames come after it.  The engine's events are recorded and waited on
-// at once, so each call may reuse them.
-static void resize_device_frames(Engine *e, Engine::FrameStage &st, const Network *net, const yb_device_frame *frames,
-                                 int nimg, int fmt, int letter, float *dst, cudaStream_t s, cudaStream_t user) {
-    if (!e->ev_frames_ready) e->ev_frames_ready = make_event();
-    if (!e->ev_frames_read) e->ev_frames_read = make_event();
-    stage_device_frames(e, st, net, frames, nimg, letter, s);
-    CUDA_OK(cudaEventRecord(e->ev_frames_ready, user));
-    CUDA_OK(cudaStreamWaitEvent(s, e->ev_frames_ready, 0));
-    launch_resize(e, st, net, nimg, fmt, dst, s);
-    CUDA_OK(cudaEventRecord(e->ev_frames_read, s));
-    CUDA_OK(cudaStreamWaitEvent(user, e->ev_frames_read, 0));
+// Batch b, on the engine stream `s`: fills st's per-image table (fill_geo, and where each frame lies) and uploads it, then
+// resizes the frames into dst -- or, with dst == nullptr (host frames of the network size), leaves them in st.buf for the
+// 8-bit stem, zero frames after the nimg-th.
+// Host frames are first copied into st.buf, packed back to back.  Frames that lie back to back in host memory go in one copy
+// (a stacked batch is one copy); each copy overlaps other work only from pinned memory.
+// Device frames are read where they lie: `s` waits for the work enqueued on the caller's stream `user` before the call (the
+// frames' producer), the resize reads the frames, and `user` waits for that resize, so that the caller's later writes into
+// the frames come after it.  The engine's events are recorded and waited on at once, so each call may reuse them.  Host
+// frames have no caller stream: nothing is recorded on `user` or made to wait for it.
+static void stage_frames(Engine *e, Engine::FrameStage &st, const Network *net, const FrameBatch &b, int letter, float *dst,
+                         cudaStream_t s, cudaStream_t user) {
+    const int B = e->batch;
+    const size_t frame = (size_t)net->w * net->h * net->c;
+    std::vector<int> w(b.nimg), h(b.nimg);
+    for (int i = 0; i < b.nimg; ++i) { w[i] = b.frames[i].w; h[i] = b.frames[i].h; }
+    fill_geo(e, st, net, w.data(), h.data(), b.nimg, letter);
+    ImageGeo *geo = st.h_geo.get();
+    for (int i = 0; i < b.nimg; ++i) {
+        const yb_device_frame &f = b.frames[i];
+        geo[i].src = f.data; geo[i].chroma = f.chroma; geo[i].pitch = f.pitch; geo[i].plane = f.plane_stride;
+    }
+    if (b.host) {
+        std::vector<size_t> off(b.nimg + 1, 0);   // frame i's bytes at off[i] .. off[i + 1] of st.buf
+        for (int i = 0; i < b.nimg; ++i) off[i + 1] = off[i] + (size_t)b.frames[i].pitch * b.frames[i].h;
+        st.buf.ensure(std::max(off[b.nimg], dst ? 0 : B * frame));   // the 8-bit stem reads whole batches
+        for (int i = 0; i < b.nimg; ++i) geo[i].src = st.buf.get() + off[i];
+        for (int i = 0; i < b.nimg;) {
+            int j = i + 1;
+            while (j < b.nimg && b.frames[j].data == b.frames[i].data + (off[j] - off[i])) ++j;
+            CUDA_OK(cudaMemcpyAsync(st.buf.get() + off[i], b.frames[i].data, off[j] - off[i], cudaMemcpyHostToDevice, s));
+            i = j;
+        }
+    }
+    CUDA_OK(cudaMemcpyAsync(st.d_geo.get(), geo, (size_t)B * sizeof(ImageGeo), cudaMemcpyHostToDevice, s));
+    if (!b.host) {
+        if (!e->ev_frames_ready) e->ev_frames_ready = make_event();
+        if (!e->ev_frames_read) e->ev_frames_read = make_event();
+        CUDA_OK(cudaEventRecord(e->ev_frames_ready, user));
+        CUDA_OK(cudaStreamWaitEvent(s, e->ev_frames_ready, 0));
+    }
+    if (dst) launch_resize(e, st, net, b.nimg, b.fmt, dst, s);
+    else if (b.nimg < B) CUDA_OK(cudaMemsetAsync(st.buf.get() + b.nimg * frame, 0, (B - b.nimg) * frame, s));
+    if (!b.host) {
+        CUDA_OK(cudaEventRecord(e->ev_frames_read, s));
+        CUDA_OK(cudaStreamWaitEvent(user, e->ev_frames_read, 0));
+    }
 }
 
-// nimg u8 HWC frames of their own sizes -> resized planar float in the engine's input staging buffer
-void engine_upload_frames(Engine *e, Network *net, const unsigned char *const *frames, const int *w, const int *h, int nimg) {
+void engine_upload_frames(Engine *e, Network *net, const FrameBatch &b, void *stream) {
     CUDA_OK(cudaSetDevice(e->opt.device));
-    stage_frames(e, e->u8, net, frames, w, h, nimg, 0, e->stream);
-    launch_resize(e, e->u8, net, nimg, YB_FRAME_RGB, e->d_input.get(), e->stream);
-    CUDA_OK(cudaGetLastError());
-}
-
-void engine_upload_device_frames(Engine *e, Network *net, const yb_device_frame *frames, int nimg, int fmt, void *stream) {
-    CUDA_OK(cudaSetDevice(e->opt.device));
-    resize_device_frames(e, e->u8, net, frames, nimg, fmt, 0, e->d_input.get(), e->stream, (cudaStream_t)stream);
+    stage_frames(e, e->u8, net, b, 0, e->d_input.get(), e->stream, (cudaStream_t)stream);
     CUDA_OK(cudaGetLastError());
 }
 
 // Throws unless every frame's memory (data, and chroma for NV12) is device or managed memory of `device`.
-void check_frame_memory(int device, const char *fn, const yb_device_frame *frames, int nimg, int fmt) {
-    for (int b = 0; b < nimg; ++b) {
-        for (int p = 0; p < (fmt == YB_FRAME_NV12 ? 2 : 1); ++p) {
+void check_frame_memory(int device, const char *fn, const FrameBatch &fb) {
+    for (int b = 0; b < fb.nimg; ++b) {
+        for (int p = 0; p < (fb.fmt == YB_FRAME_NV12 ? 2 : 1); ++p) {
             cudaPointerAttributes a{};
-            const cudaError_t r = cudaPointerGetAttributes(&a, p ? frames[b].chroma : frames[b].data);
+            const cudaError_t r = cudaPointerGetAttributes(&a, p ? fb.frames[b].chroma : fb.frames[b].data);
             if (r != cudaSuccess) cudaGetLastError();
             const char *kind = r != cudaSuccess ? "unknown" : a.type == cudaMemoryTypeHost ? "pinned host memory"
                              : a.type == cudaMemoryTypeDevice ? "device memory" : a.type == cudaMemoryTypeManaged ? "managed memory"
@@ -1410,7 +1390,6 @@ void engine_input_histogram(Engine *e, Network *net, int layer, int img, float b
 // geometry: P.geo, set by the caller
 static DetParams det_params(Network *net, const std::vector<Engine::Final> &finals, float thresh, float nms, int relative,
                             int max_rows) {
-    if (max_rows <= 0 || max_rows > DET_MAX_ROWS) fatal_throw("detect: max_rows must be in 1.." + std::to_string(DET_MAX_ROWS));
     DetParams P{};
     int total = 0;
     for (size_t i = 0; i < net->layers.size(); ++i) {
@@ -1501,12 +1480,10 @@ int engine_detect(Engine *e, Network *net, const int *w, const int *h, int nimg,
 // reference's resize on the copy-in stream, the forward on the compute stream, decode + NMS on a side stream (under the
 // forward of the NEXT batch), and returns a ticket.  engine_collect_detections waits for that batch and copies back exactly
 // the candidate rows.  Host traffic per batch: the u8 frames in (a quarter of the float images), counts + rows out (a few
-// hundred KB instead of the 124 MB of yolo tensors).
-//
-// `stage` enqueues on the copy-in stream what makes the slot's input, host or device frames: it fills the slot's geometry
-// table and either resizes into sl.d_in (returns nullptr) or returns 8-bit frames of the network size for the stem to read.
-static int submit_detections(Engine *e, Network *net, int nimg, float thresh, float nms, int relative, int max_rows,
-                             const std::function<const unsigned char *(Engine::Slot &)> &stage) {
+// hundred KB instead of the 124 MB of yolo tensors).  Device frames are resized the same way, read in order with the caller's
+// `stream`.
+int engine_submit_frames(Engine *e, Network *net, const FrameBatch &b, float thresh, float nms, int relative, int letter,
+                         int max_rows, void *stream) {
     DetParams P = det_params(net, e->finals, thresh, nms, relative, max_rows);
     const int B = e->batch, stride = 5 + P.classes;
     const int k = acquire_slot(e);
@@ -1514,47 +1491,29 @@ static int submit_detections(Engine *e, Network *net, int nimg, float thresh, fl
     det_ws_ensure(sl.det, B, P);
     sl.h_rows.ensure((size_t)B * max_rows * stride);
     sl.h_counts.ensure(B);
+    // host frames that all have the network size need no resize when the stem reads 8-bit frames
+    bool u8_stem = b.host && e->ops[0].launch_u8 && net->c == 3;
+    for (int i = 0; i < b.nimg; ++i) u8_stem &= b.frames[i].w == net->w && b.frames[i].h == net->h;
     // The slot's frames and geometry table go on s_in.  The decode below reads the table on the compute stream behind ev_in,
     // and the next submit to this slot rewrites it only after waiting for ev_comp (acquire_slot) -- and only once this ticket
     // has been collected, which waits for ev_det, so the pinned host table is no longer being copied either.
-    forward_slot(e, sl, stage(sl));
+    stage_frames(e, sl.u8, net, b, letter, u8_stem ? nullptr : sl.d_in.get(), e->s_in, (cudaStream_t)stream);
+    forward_slot(e, sl, u8_stem ? sl.u8.buf.get() : nullptr);
     // Candidate selection + box decode (k_det_count / k_det_emit: they read the objectness planes and, for the few candidates,
     // their class scores) run right behind the forward on the compute stream, straight on the engine's yolo tensors -- the next
     // forward overwrites those, so this is the only part that must not slip.  What follows (IoU matrix + per-class NMS) works on
     // the slot's own candidate rows and goes to the side stream, where it overlaps the next batch's forward.  (Copying the
     // 124 MB of yolo tensors into the slot first, as the raw-tensor path does, cost more than the decode itself.)
     P.geo = sl.u8.d_geo.get();
-    det_launch_count_emit(P, sl.det, B, nimg, e->stream);
+    det_launch_count_emit(P, sl.det, B, b.nimg, e->stream);
     CUDA_OK(cudaEventRecord(sl.ev_comp, e->stream));
     CUDA_OK(cudaStreamWaitEvent(e->s_det, sl.ev_comp, 0));
     CUDA_OK(cudaMemcpyAsync(sl.h_counts.get(), sl.det.counts.get(), (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, e->s_det));
-    det_launch_nms(P, sl.det, nimg, max_rows, e->s_det);   // no host round trip: grids sized for the cap, kernels read the counts
+    det_launch_nms(P, sl.det, b.nimg, max_rows, e->s_det);  // no host round trip: grids sized for the cap, kernels read the counts
     CUDA_OK(cudaEventRecord(sl.ev_det, e->s_det));
     CUDA_OK(cudaGetLastError());
-    sl.busy = true; sl.mode = 1; sl.nimg = nimg;
+    sl.busy = true; sl.mode = 1; sl.nimg = b.nimg;
     return k;
-}
-
-int engine_submit_frames(Engine *e, Network *net, const unsigned char *const *frames, const int *w, const int *h, int nimg,
-                         float thresh, float nms, int relative, int letter, int max_rows) {
-    return submit_detections(e, net, nimg, thresh, nms, relative, max_rows, [&](Engine::Slot &sl) -> const unsigned char * {
-        const bool net_size = stage_frames(e, sl.u8, net, frames, w, h, nimg, letter, e->s_in);
-        if (e->ops[0].launch_u8 && net_size && net->c == 3) {   // frames of the network size: no staging
-            const size_t frame = (size_t)net->w * net->h * net->c;
-            if (nimg < e->batch) CUDA_OK(cudaMemsetAsync(sl.u8.buf.get() + nimg * frame, 0, (e->batch - nimg) * frame, e->s_in));
-            return sl.u8.buf.get();
-        }
-        launch_resize(e, sl.u8, net, nimg, YB_FRAME_RGB, sl.d_in.get(), e->s_in);
-        return nullptr;
-    });
-}
-
-int engine_submit_device_frames(Engine *e, Network *net, const yb_device_frame *frames, int nimg, int fmt, float thresh,
-                                float nms, int relative, int letter, int max_rows, void *stream) {
-    return submit_detections(e, net, nimg, thresh, nms, relative, max_rows, [&](Engine::Slot &sl) -> const unsigned char * {
-        resize_device_frames(e, sl.u8, net, frames, nimg, fmt, letter, sl.d_in.get(), e->s_in, (cudaStream_t)stream);
-        return nullptr;
-    });
 }
 
 // rows: pinned [batch][max_rows][5 + classes] (valid until the slot is reused), counts[batch] (0 beyond the ticket's images);

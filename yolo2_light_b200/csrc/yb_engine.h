@@ -28,13 +28,23 @@ struct EngineOptions {
     bool keep_counts = false;  // keep raw XNOR popcounts / INT8 accumulators (tests)
 };
 
+// The caller's 8-bit frames of one call: nimg (1..batch) frames of one YB_FRAME_* format.  Device frames (3-channel networks)
+// lie in device memory and are read in order with the caller's stream; host frames are YB_FRAME_RGB frames of net.c bytes
+// per pixel with pitch w * net.c.  The engine calls take a batch that has passed the argument checks.
+struct FrameBatch {
+    const yb_device_frame *frames;
+    int nimg;
+    int fmt;
+    bool host;
+};
+
 struct Engine;
 std::shared_ptr<Engine> build_engine(Network *net, const EngineOptions &opt);
 // d_input == nullptr: use the engine's staging buffer (filled by engine_upload_input)
 void engine_upload_input(Engine *e, const float *host_input, void *stream);
-// nimg (1..batch) host u8 HWC frames, frame b w[b] x h[b] -> the reference's resize into the staging buffer (images
-// nimg .. batch-1 zero)
-void engine_upload_frames(Engine *e, Network *net, const unsigned char *const *frames, const int *w, const int *h, int nimg);
+// frames -> the reference's resize into the staging buffer (images nimg .. batch-1 zero); `stream`: the caller's stream of
+// device frames
+void engine_upload_frames(Engine *e, Network *net, const FrameBatch &b, void *stream);
 void engine_forward(Engine *e, const void *d_input, void *stream);
 void engine_download_outputs(Engine *e, Network *net, void *stream);   // async D2H into pinned, then sync
 int engine_submit(Engine *e, const float *host_input);
@@ -42,22 +52,19 @@ void engine_collect(Engine *e, Network *net, int ticket);
 void engine_collect_ptrs(Engine *e, int ticket, std::vector<const float *> &ptrs, std::vector<size_t> &counts);
 const char *engine_broadcast_arena(const std::vector<Engine *> &replicas);   // "nccl" | "peer-copy" | "single"
 int engine_device_count();
-// pipelined u8 frames -> detections (device-side resize, forward, decode + NMS; only candidate rows come back)
-int engine_submit_frames(Engine *e, Network *net, const unsigned char *const *frames, const int *w, const int *h, int nimg,
-                         float thresh, float nms, int relative, int letter, int max_rows);
+// pipelined frames -> detections (device-side resize, forward, decode + NMS; only candidate rows come back); max_rows in
+// 1..DET_MAX_ROWS
+int engine_submit_frames(Engine *e, Network *net, const FrameBatch &b, float thresh, float nms, int relative, int letter,
+                         int max_rows, void *stream);
 int engine_collect_detections(Engine *e, int ticket, const float **rows, const int **counts, size_t *d2h_bytes);
-// the caller's device frames (one YB_FRAME_* format, 3-channel networks), read in order with the caller's `stream`:
-// resize into the staging buffer (synchronous calls), or the pipelined path of engine_submit_frames
-void engine_upload_device_frames(Engine *e, Network *net, const yb_device_frame *frames, int nimg, int fmt, void *stream);
-int engine_submit_device_frames(Engine *e, Network *net, const yb_device_frame *frames, int nimg, int fmt, float thresh,
-                                float nms, int relative, int letter, int max_rows, void *stream);
-// throws unless the frames' memory is device or managed memory of `device`
-void check_frame_memory(int device, const char *fn, const yb_device_frame *frames, int nimg, int fmt);
+// throws unless the memory of the device frames of `b` is device or managed memory of `device`
+void check_frame_memory(int device, const char *fn, const FrameBatch &b);
 void engine_fetch_layer(Engine *e, Network *net, int layer, float *dst);
 void engine_fetch_input(Engine *e, float *dst);
 int engine_fetch_counts(Engine *e, int layer, int32_t *dst, size_t count);
 void engine_weight_arena(Engine *e, void **ptr, size_t *bytes);
-// device-side decode + NMS of the first nimg images, image b's boxes corrected for a w[b] x h[b] frame
+// device-side decode + NMS of the first nimg images, image b's boxes corrected for a w[b] x h[b] frame; max_rows in
+// 1..DET_MAX_ROWS
 int engine_detect(Engine *e, Network *net, const int *w, const int *h, int nimg, float thresh, float nms, int relative,
                   int letter, float *rows, int max_rows, int *counts);
 // the per-(class, image) sort of the decode lives in shared memory: 8 B per (power-of-two) row
