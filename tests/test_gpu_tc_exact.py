@@ -283,9 +283,11 @@ def c_filters(nf, bn=None):
     return n
 
 
-def c_f32(nf, size=3):
+def c_f32(nf, size=3, stats=False):
     n = Net(64, 13, 7, 2, 300 + nf)
     i = n.conv(nf, size, act=LEAKY if nf != 255 else LINEAR, kern="tc")
+    if stats:
+        n.env["YB_TC_STATS"] = "1"
     return n.edge(i, f"f32 output, n = {nf}", lambda p: p["kernel"] == "k_conv_tc" and p["kind"] == "bf16")
 
 
@@ -335,8 +337,8 @@ def c_bump():
     return n.edge(i, "stride 2, BN 32: TW 1 -> 2", lambda p: p["BN"] == 32 and p["TW"] == 2)
 
 
-def c_knobs(bn=None, no_bstat=False, grid=None, stride=1):
-    n = Net(64, 12, 10, 2, 900 + (bn or 0) + 7 * (grid or 0) + stride)
+def c_knobs(bn=None, no_bstat=False, grid=None, stride=1, stats=False):
+    n = Net(64, 12, 10, 2, 900 + (bn or 0) + 7 * (grid or 0) + stride + 3 * stats)
     i = n.conv(256, 3, stride)
     n.consume()
     if bn:
@@ -348,6 +350,8 @@ def c_knobs(bn=None, no_bstat=False, grid=None, stride=1):
     if grid:
         n.env["YB_TC_GRID"] = str(grid)
         n.edge(i, f"{grid} CTAs, several work items each", lambda p: p["grid"] == grid and p["num_work"] > grid)
+    if stats:   # the role-counter instantiations compute the same bits
+        n.env["YB_TC_STATS"] = "1"
     return n
 
 
@@ -447,6 +451,9 @@ CASES = {
     "grid1": lambda: c_knobs(grid=1),
     "grid3": lambda: c_knobs(bn=32, grid=3),
     "grid3_s2": lambda: c_knobs(bn=64, grid=3, stride=2),
+    "stats_grid3": lambda: c_knobs(bn=128, grid=3, stats=True),
+    "stats_grid3_s2": lambda: c_knobs(bn=64, grid=3, stride=2, stats=True),
+    "stats_f32_n75": lambda: c_f32(75, stats=True),
     **{f"shortcut_{a}_fuse{f}": (lambda a=a, f=f: c_shortcut(a, f)) for a in (LINEAR, LEAKY) for f in (0, 1)},
     "concat_first": lambda: c_concat(True),
     "concat_second": lambda: c_concat(False),
@@ -678,6 +685,29 @@ def test_integer_kinds_exact(kind, C, n, h, w, stride, batch, workdir):
     assert (p["tma_epi"] == 0) == (stride == 2), p
     m.predict(cfgs.synthetic_images(batch, 3, h, w, seed=C), quantized=q)
     assert util.bits_equal(m.fetch_layer(1, quantized=q), exp)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("kind", ["s8", "xnor"])
+def test_integer_kinds_role_counters(kind, workdir, monkeypatch, capfd):
+    """YB_TC_STATS=1 runs the role-counter instantiation of the integer epilogue: the same bits as the oracle, and a TCSTATS
+    line per plan when the network is freed"""
+    import gc
+    monkeypatch.setenv("YB_TC_STATS", "1")
+    monkeypatch.setenv("YB_TC_GRID", "2")   # several work items per CTA
+    q = kind == "s8"
+    secs = _int_secs(40 if q else 48, 11, 13, q) + [cfgs._conv(40, 3, **({} if q else {"xnor": 1, "bin_output": 1}))]
+    m = _int_net(workdir, f"stats_{kind}", secs, 2, int(q), 11)
+    p = m.tc_plan(1, quantized=q)
+    assert p.get("kind") == kind and p["kernel"] == "k_conv_tc" and p["num_work"] > p["grid"], p
+    m.predict(cfgs.synthetic_images(2, 3, 11, 13, seed=4), quantized=q)
+    exp, _ = _int_ref(m.layers[1], m.fetch_layer(0, quantized=q), q)
+    assert util.bits_equal(m.fetch_layer(1, quantized=q), exp)
+    capfd.readouterr()
+    del m
+    gc.collect()
+    lines = [l for l in capfd.readouterr().err.splitlines() if l.startswith("TCSTATS")]
+    assert lines and all("producer: wait_empty" in l and "consumers: wait_full" in l for l in lines), lines
 
 
 @pytest.mark.gpu

@@ -68,9 +68,9 @@ struct TcParams {
     int TW, TWlog2, TH;       // tile = TW x TH output pixels (TW*TH == 128)
     int xt, jt, nt;           // #tiles along x, merged rows, filters
     int num_work;             // tiles = work items of the persistent loop (xt * jt * nt)
-    int kind;                 // 0: bf16 x bf16 -> f32;  1: s8 x s8 -> s32, exact requantising epilogue;
-                              // 2: XNOR layer as +-1 s8 on the s8 wgmma (dot = 2*count - K exactly), reference float epilogue;
-                              // 3: f32 operands read as tf32 (K = 8 per MMA) -> f32: float heads of the exact nets
+    int kind;                 // TcKind: TC_BF16 bf16 x bf16 -> f32;  TC_S8 s8 x s8 -> s32, exact requantising epilogue;
+                              // TC_XNOR XNOR layer as +-1 s8 on the s8 wgmma (dot = 2*count - K exactly), reference float epilogue;
+                              // TC_TF32 f32 operands read as tf32 (K = 8 per MMA) -> f32: float heads of the exact nets
     int kk;                   // MMAs per K-block (BK bytes / 32)
     float alpha1;             // INT8: R_MULT / (input_mult * weights_mult)
     const float *mean;        // kind 2 (XNOR as +-1 s8): per-filter mean |w|; out = (float)dot * mean + bias
@@ -110,7 +110,7 @@ struct TcParams {
     char *out; long out_ldc; int n;
     const char *res;          // fused shortcut operand (bf16, k_conv_tc_reg at stride 1 only), or null
     const float *bias; int act, act2;
-    unsigned long long *stats; // YB_TC_STATS=1: per-CTA cycle counters [grid][16] (diagnostic)
+    unsigned long long *stats; // YB_TC_STATS=1: per-CTA cycle counters [grid][TC_NSTATS] (diagnostic)
     int dbg;                  // YB_TC_DBG bit mask for bottleneck experiments: 1 no TMA, 4 no epilogue memory ops
 };
 
@@ -188,6 +188,14 @@ __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bu
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+__device__ __forceinline__ void prefetch_tmap(const CUtensorMap *tm) { asm volatile("prefetch.tensormap [%0];" ::"l"(tm) : "memory"); }
+__device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+// Programmatic dependent launch: the prologue before this (barrier init, tensor-map prefetch, bias -> smem: weights only)
+// overlapped the tail of the previous kernel; from here on the kernel touches activations it wrote.
+__device__ __forceinline__ void pdl_wait_and_launch() {
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+}
 
 // --- wgmma (sm_90a) ----------------------------------------------------------------------------------------------------
 // Shared-memory matrix descriptor: start address >> 4 (bits 0-13), LBO = 1 (unused by the swizzled K-major layouts), high word
@@ -211,9 +219,9 @@ __device__ __forceinline__ void wg_fence_operand(T (&d)[N]) {
 }
 
 // One M=64 x N x (32 bytes of K) wgmma per call; d: this thread's accumulator fragment (N/2 values).  scale_d == 0 overwrites.
-// KIND 0: bf16 -> f32, 1 (and 2): s8 -> s32, 3: tf32 -> f32.
-template <int KIND, int N> struct Wg;
-template <> struct Wg<0, 32> {
+// TC_BF16: bf16 -> f32, TC_S8 (and TC_XNOR): s8 -> s32, TC_TF32: tf32 -> f32.
+template <TcKind KIND, int N> struct Wg;
+template <> struct Wg<TC_BF16, 32> {
     static __device__ __forceinline__ void mma(float (&d)[16], uint64_t a, uint64_t b, uint32_t scale_d) {
         asm volatile(
             "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
@@ -223,7 +231,7 @@ template <> struct Wg<0, 32> {
             : "l"(a), "l"(b), "r"(scale_d) : "memory");
     }
 };
-template <> struct Wg<0, 64> {
+template <> struct Wg<TC_BF16, 64> {
     static __device__ __forceinline__ void mma(float (&d)[32], uint64_t a, uint64_t b, uint32_t scale_d) {
         asm volatile(
             "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
@@ -233,7 +241,7 @@ template <> struct Wg<0, 64> {
             : "l"(a), "l"(b), "r"(scale_d) : "memory");
     }
 };
-template <> struct Wg<0, 128> {
+template <> struct Wg<TC_BF16, 128> {
     static __device__ __forceinline__ void mma(float (&d)[64], uint64_t a, uint64_t b, uint32_t scale_d) {
         asm volatile(
             "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
@@ -243,7 +251,7 @@ template <> struct Wg<0, 128> {
             : "l"(a), "l"(b), "r"(scale_d) : "memory");
     }
 };
-template <> struct Wg<0, 256> {
+template <> struct Wg<TC_BF16, 256> {
     static __device__ __forceinline__ void mma(float (&d)[128], uint64_t a, uint64_t b, uint32_t scale_d) {
         asm volatile(
             "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
@@ -253,7 +261,7 @@ template <> struct Wg<0, 256> {
             : "l"(a), "l"(b), "r"(scale_d) : "memory");
     }
 };
-template <> struct Wg<1, 32> {
+template <> struct Wg<TC_S8, 32> {
     static __device__ __forceinline__ void mma(uint32_t (&d)[16], uint64_t a, uint64_t b, uint32_t scale_d) {
         asm volatile(
             "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
@@ -263,7 +271,7 @@ template <> struct Wg<1, 32> {
             : "l"(a), "l"(b), "r"(scale_d) : "memory");
     }
 };
-template <> struct Wg<1, 64> {
+template <> struct Wg<TC_S8, 64> {
     static __device__ __forceinline__ void mma(uint32_t (&d)[32], uint64_t a, uint64_t b, uint32_t scale_d) {
         asm volatile(
             "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
@@ -273,7 +281,7 @@ template <> struct Wg<1, 64> {
             : "l"(a), "l"(b), "r"(scale_d) : "memory");
     }
 };
-template <> struct Wg<1, 128> {
+template <> struct Wg<TC_S8, 128> {
     static __device__ __forceinline__ void mma(uint32_t (&d)[64], uint64_t a, uint64_t b, uint32_t scale_d) {
         asm volatile(
             "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
@@ -283,7 +291,7 @@ template <> struct Wg<1, 128> {
             : "l"(a), "l"(b), "r"(scale_d) : "memory");
     }
 };
-template <> struct Wg<3, 32> {
+template <> struct Wg<TC_TF32, 32> {
     static __device__ __forceinline__ void mma(float (&d)[16], uint64_t a, uint64_t b, uint32_t scale_d) {
         asm volatile(
             "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
@@ -293,7 +301,7 @@ template <> struct Wg<3, 32> {
             : "l"(a), "l"(b), "r"(scale_d) : "memory");
     }
 };
-template <> struct Wg<3, 64> {
+template <> struct Wg<TC_TF32, 64> {
     static __device__ __forceinline__ void mma(float (&d)[32], uint64_t a, uint64_t b, uint32_t scale_d) {
         asm volatile(
             "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
@@ -303,7 +311,7 @@ template <> struct Wg<3, 64> {
             : "l"(a), "l"(b), "r"(scale_d) : "memory");
     }
 };
-template <> struct Wg<3, 128> {
+template <> struct Wg<TC_TF32, 128> {
     static __device__ __forceinline__ void mma(float (&d)[64], uint64_t a, uint64_t b, uint32_t scale_d) {
         asm volatile(
             "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
@@ -313,7 +321,7 @@ template <> struct Wg<3, 128> {
             : "l"(a), "l"(b), "r"(scale_d) : "memory");
     }
 };
-template <int N> struct Wg<2, N> : Wg<1, N> {};
+template <int N> struct Wg<TC_XNOR, N> : Wg<TC_S8, N> {};
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
     __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
@@ -351,16 +359,91 @@ __device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
     asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
 }
 
+// --- The pipeline both kernels share: work items, the operand ring, the role counters ------------------------------------
+// Work item w: filter tile w % nt (first filter n0) of pixel tile w / nt, whose first pixel is column x0 of merged row J0.  The
+// producer, the consumers and k_conv_tc_reg's store threads walk the same items, w = blockIdx.x, + gridDim.x, ...
+// BN: p.BN, or the same width as a compile-time constant.
+struct TcItem { int n0, x0, J0; };
+__device__ __forceinline__ TcItem tc_item(const TcParams &p, int w, int BN) {
+    const int m = w / p.nt;
+    return {(w % p.nt) * BN, (m % p.xt) * p.TW, (m / p.xt) * p.TH + p.jshift};
+}
+// The output pixel of accumulator row r of item t's tile.  A row that falls on a border or padding row of the merged-row
+// tiling, past the batch or past the output's width is no output pixel (valid() is false).
+struct TcPixel {
+    int img, oy, ox;
+    __device__ __forceinline__ bool valid(const TcParams &p) const { return img < p.N && oy >= 0 && oy < p.OH && ox < p.OW; }
+};
+__device__ __forceinline__ TcPixel tc_pixel(const TcParams &p, const TcItem &t, int r) {
+    const int J = t.J0 + (r >> p.TWlog2);
+    const int img = J / p.PR;
+    return {img, J - img * p.PR - p.row_off, t.x0 + (r & (p.TW - 1))};
+}
+
+// Position in the operand ring: the stage and the parity of its barriers' current phase.  The producer and every consumer
+// warp step through the stages in the same order.
+struct TcRing {
+    int stage = 0;
+    uint32_t phase = 0;
+    __device__ __forceinline__ void advance(int stages) { if (++stage == stages) { stage = 0; phase ^= 1u; } }
+};
+// The ring's barriers and the resident filter matrix's, by one thread before the block's first barrier: full[s] and bstat_bar
+// complete on the producer's arrive.expect_tx and the bytes of its loads; empty[s] on one arrival per consumer warp
+// (tc_mma_loop's release).
+__device__ __forceinline__ void tc_init_ring(const TcParams &p, uint32_t base) {
+    for (int s = 0; s < p.stages; ++s) { mbar_init(base + p.sm.full + 8u * s, 1); mbar_init(base + p.sm.empty + 8u * s, TC_EPI_WARPS); }
+    mbar_init(base + p.sm.bstat_bar, 1);
+}
+
+// Runs f(BN, KK) with the plan's filter-tile width and wgmmas per K-block as std::integral_constants.  BN_MAX: the kernel's
+// widest filter tile.
+template <int BN_MAX, typename F>
+__device__ __forceinline__ void tc_dispatch(const TcParams &p, F &&f) {
+    auto by_kk = [&](auto bn_c) {
+        if (p.kk == 4) f(bn_c, std::integral_constant<int, 4>{});
+        else if (p.kk == 2) f(bn_c, std::integral_constant<int, 2>{});
+        else f(bn_c, std::integral_constant<int, 1>{});
+    };
+    if constexpr (BN_MAX == 256) {
+        if (p.BN == 256) { by_kk(std::integral_constant<int, 256>{}); return; }
+    }
+    if (p.BN == 128) by_kk(std::integral_constant<int, 128>{});
+    else if (p.BN == 64) by_kk(std::integral_constant<int, 64>{});
+    else by_kk(std::integral_constant<int, 32>{});
+}
+
+// Role counters of the ST instantiations (YB_TC_STATS=1): cycles of one CTA, p.stats[blockIdx.x * TC_NSTATS + slot].  The
+// consumer slots are warp 0's, the store slots the store thread's of consumer warpgroup 0.
+enum TcStat {
+    STAT_PROD_WAIT_EMPTY,    // producer: waiting for free ring stages
+    STAT_PROD_TMA_ISSUE,     // producer: issuing TMA loads
+    STAT_PROD_TOTAL,         // producer: all of its work items
+    STAT_CONS_WAIT_FULL,     // consumer: waiting for loaded ring stages
+    STAT_CONS_WAIT_READY,    // k_conv_tc_reg consumer: waiting on stg_ready, the first work item apart
+    STAT_CONS_FIRST_READY,   // k_conv_tc_reg consumer: waiting on stg_ready before the first work item's epilogue
+    STAT_CONS_TOTAL,         // consumer: all of its work items
+    STAT_STORE_WAIT_FULL,    // k_conv_tc_reg store thread: waiting on stg_full
+    STAT_STORE_WAIT_READ,    // k_conv_tc_reg store thread: waiting for its bulk stores to read shared memory
+    TC_NSTATS = 16           // slots per CTA, padded to a power of two: with a multiply in its index, k_conv_tc_reg<true> spills more
+};
+__device__ __forceinline__ unsigned long long &tc_stat(const TcParams &p, TcStat s) { return p.stats[blockIdx.x * TC_NSTATS + s]; }
+// Runs f(); the ST instantiations add the cycles it took to cycles, the others read no clock
+template <bool ST, typename F>
+__device__ __forceinline__ void timed(long long &cycles, F &&f) {
+    if constexpr (ST) { const long long c0 = clock64(); f(); cycles += clock64() - c0; }
+    else f();
+}
+
 // TMA producer (one elected thread): walks the consumers' work items and keeps the ring full (base: the aligned shared memory)
 template <bool ST>
 __device__ __forceinline__ void tc_produce(const CUtensorMap *tmA, const CUtensorMap *tmB, const TcParams &p, uint32_t base,
                                            int w_first, int w_step) {
-    int stage = 0; uint32_t phase = 0;
+    TcRing ring;
     long long w_empty = 0, w_tma = 0; const long long t_begin = ST ? clock64() : 0;
     // loop-invariant parameters in registers; the (tap, channel-block) walk is incremental (no integer divisions per
     // K-block in this single thread)
     const int sps = p.sps, kblocks = p.kblocks, cblocks = p.cblocks, BK = p.BK, fsize = p.size, stages = p.stages;
-    const int xoff = p.xoff, yoff = p.yoff, stride2 = p.stride2, nt = p.nt, xt = p.xt;
+    const int xoff = p.xoff, yoff = p.yoff, stride2 = p.stride2;
     const uint32_t a_bytes = p.a_bytes, b_bytes = p.b_bytes, stage_bytes = p.stage_bytes;
     const uint32_t b_off = (uint32_t)sps * a_bytes;
     const uint32_t smemB = base, smem0 = base + p.sm.ring, bstat_bar = base + p.sm.bstat_bar;
@@ -370,41 +453,39 @@ __device__ __forceinline__ void tc_produce(const CUtensorMap *tmA, const CUtenso
         for (int kb = 0; kb < kblocks; ++kb) tma_load_2d(smemB + (uint32_t)kb * b_bytes, tmB, bstat_bar, kb * BK, 0);
     }
     for (int w = w_first; w < p.num_work; w += w_step) {
-        const int n_idx = w % nt;
-        const int m = w / nt;
-        const int x0 = (m % xt) * p.TW;
-        const int J0 = (m / xt) * p.TH + p.jshift;
-        const int n0 = n_idx * p.BN;
+        const TcItem it = tc_item(p, w, p.BN);
         // channel block, tap x/y, K column of the weight matrix
         int cb = 0, ky = 0, kx = 0, kcol = 0;
         for (int kb0 = 0; kb0 < kblocks; kb0 += sps) {
             const int nsub = min(sps, kblocks - kb0);
-            if constexpr (ST) { const long long c0 = clock64(); mbar_wait(base + p.sm.empty + 8u * (uint32_t)stage, phase ^ 1u); w_empty += clock64() - c0; }
-            else mbar_wait(base + p.sm.empty + 8u * (uint32_t)stage, phase ^ 1u);
-            const uint32_t fb = base + p.sm.full + 8u * (uint32_t)stage;
-            const uint32_t a_dst = smem0 + (uint32_t)stage * stage_bytes;
+            timed<ST>(w_empty, [&] { mbar_wait(base + p.sm.empty + 8u * (uint32_t)ring.stage, ring.phase ^ 1u); });
+            const uint32_t fb = base + p.sm.full + 8u * (uint32_t)ring.stage;
+            const uint32_t a_dst = smem0 + (uint32_t)ring.stage * stage_bytes;
             const uint32_t b_dst = a_dst + b_off;
             if (p.dbg & 1) {
                 mbar_arrive(fb);
-                if (++stage == stages) { stage = 0; phase ^= 1u; }
+                ring.advance(stages);
                 continue;
             }
             mbar_arrive_expect_tx(fb, (uint32_t)nsub * (a_bytes + (bstat ? 0u : b_bytes)));
-            const long long ct0 = ST ? clock64() : 0;
-            for (int j = 0; j < nsub; ++j) {
-                const uint32_t ad = a_dst + (uint32_t)j * a_bytes, bd = b_dst + (uint32_t)j * b_bytes;
-                const int c0 = cb * BK;
-                if (stride2) tma_load_5d(ad, tmA, fb, c0, kx & 1, x0 + (kx >> 1), ky & 1, J0 + (ky >> 1));
-                else tma_load_3d(ad, tmA, fb, c0, x0 + kx + xoff, J0 + ky + yoff);
-                if (!bstat) tma_load_2d(bd, tmB, fb, kcol, n0);
-                kcol += BK;
-                if (++cb == cblocks) { cb = 0; if (++kx == fsize) { kx = 0; ++ky; } }
-            }
-            if constexpr (ST) w_tma += clock64() - ct0;
-            if (++stage == stages) { stage = 0; phase ^= 1u; }
+            timed<ST>(w_tma, [&] {
+                for (int j = 0; j < nsub; ++j) {
+                    const uint32_t ad = a_dst + (uint32_t)j * a_bytes, bd = b_dst + (uint32_t)j * b_bytes;
+                    const int c0 = cb * BK;
+                    if (stride2) tma_load_5d(ad, tmA, fb, c0, kx & 1, it.x0 + (kx >> 1), ky & 1, it.J0 + (ky >> 1));
+                    else tma_load_3d(ad, tmA, fb, c0, it.x0 + kx + xoff, it.J0 + ky + yoff);
+                    if (!bstat) tma_load_2d(bd, tmB, fb, kcol, it.n0);
+                    kcol += BK;
+                    if (++cb == cblocks) { cb = 0; if (++kx == fsize) { kx = 0; ++ky; } }
+                }
+            });
+            ring.advance(stages);
         }
     }
-    if (ST && p.stats) { p.stats[blockIdx.x * 16 + 0] = (unsigned long long)w_empty; p.stats[blockIdx.x * 16 + 1] = (unsigned long long)(clock64() - t_begin); p.stats[blockIdx.x * 16 + 7] = (unsigned long long)w_tma; }
+    if (ST && p.stats) {
+        tc_stat(p, STAT_PROD_WAIT_EMPTY) = w_empty; tc_stat(p, STAT_PROD_TMA_ISSUE) = w_tma;
+        tc_stat(p, STAT_PROD_TOTAL) = clock64() - t_begin;
+    }
 }
 
 // The K-blocks of the current work item into warpgroup wg's accumulator fragment d (rows 64 wg .. + 63
@@ -412,9 +493,9 @@ __device__ __forceinline__ void tc_produce(const CUtensorMap *tmA, const CUtenso
 // one stage behind the issue (wgmma.wait_group 1) so that the tensor pipe never drains.  Nothing but wgmmas touches the
 // accumulators while wgmmas are in flight, and every batch is the same KK wgmmas: ptxas then inserts no fences of its own
 // and serializes nothing (the -Xptxas -v log has no C75xx notes).
-template <int KIND, int BN, int KK, bool ST, typename T>
-__device__ __forceinline__ void tc_mma_loop(T (&d)[BN / 2], const TcParams &p, uint32_t base, int wg, int lane, int &stage,
-                                            uint32_t &phase, long long &w_full) {
+template <TcKind KIND, int BN, int KK, bool ST, typename T>
+__device__ __forceinline__ void tc_mma_loop(T (&d)[BN / 2], const TcParams &p, uint32_t base, int wg, int lane, TcRing &ring,
+                                            long long &w_full) {
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) d[i] = T(0);
     wg_fence_operand(d);
@@ -423,16 +504,14 @@ __device__ __forceinline__ void tc_mma_loop(T (&d)[BN / 2], const TcParams &p, u
     const uint32_t b_off = (uint32_t)sps * a_bytes, a_wg = (uint32_t)wg * (a_bytes >> 1);
     const uint32_t smemB = base, smem0 = base + p.sm.ring;   // resident filter matrix, ring
     const uint32_t full = base + p.sm.full, empty = base + p.sm.empty;   // the ring's mbarriers, 8 bytes per stage
+    // one arrival per consumer warp (tc_init_ring)
     auto release = [&](int s) { __syncwarp(); if (lane == 0) mbar_arrive(empty + 8u * (uint32_t)s); };
     // one commit group per K-block; a stage (sps K-blocks, fewer at the end of the work item) is released once the group of
     // its last K-block has retired, which wgmma.wait_group 1 shows one K-block later
     int pend = -1, jj = 0;
     for (int kb = 0; kb < kblocks; ++kb) {
-        if (jj == 0) {
-            if constexpr (ST) { const long long c0 = clock64(); mbar_wait(full + 8u * (uint32_t)stage, phase); w_full += clock64() - c0; }
-            else mbar_wait(full + 8u * (uint32_t)stage, phase);
-        }
-        const uint32_t st_base = smem0 + (uint32_t)stage * stage_bytes;
+        if (jj == 0) timed<ST>(w_full, [&] { mbar_wait(full + 8u * (uint32_t)ring.stage, ring.phase); });
+        const uint32_t st_base = smem0 + (uint32_t)ring.stage * stage_bytes;
         const uint32_t a_kb = st_base + a_wg + (uint32_t)jj * a_bytes;
         const uint32_t b_kb = p.bstat ? smemB + (uint32_t)kb * b_bytes : st_base + b_off + (uint32_t)jj * b_bytes;
         wg_fence();
@@ -444,8 +523,8 @@ __device__ __forceinline__ void tc_mma_loop(T (&d)[BN / 2], const TcParams &p, u
         wg_wait<1>();
         if (pend >= 0) { release(pend); pend = -1; }
         if (++jj == sps || kb + 1 == kblocks) {
-            pend = stage; jj = 0;
-            if (++stage == stages) { stage = 0; phase ^= 1u; }
+            pend = ring.stage; jj = 0;
+            ring.advance(stages);
         }
     }
     wg_wait<0>();
@@ -454,13 +533,13 @@ __device__ __forceinline__ void tc_mma_loop(T (&d)[BN / 2], const TcParams &p, u
 }
 
 // The reference's float epilogue of the integer kinds, with its operations in its order (bit-exact results):
-//   kind 1, INT8 (yolov2_forward_network_quantized.c:474-490, :598-627): q16 = clamp(+-32767, acc / 32) [C truncating
+//   TC_S8, INT8 (yolov2_forward_network_quantized.c:474-490, :598-627): q16 = clamp(+-32767, acc / 32) [C truncating
 //     division]; y = (float)q16 * ALPHA1; y += bias; leaky: y / 10.
-//   kind 2, XNOR as +-1 s8 (acc == 2*count - K exactly): y = act((float)acc * mean + bias) (additionally.c:1531,
+//   TC_XNOR, XNOR as +-1 s8 (acc == 2*count - K exactly): y = act((float)acc * mean + bias) (additionally.c:1531,
 //     yolov2_forward_network.c:243-261).
-// f: filter index (kind 2 reads its mean |w|).
+// f: filter index (TC_XNOR reads its mean |w|).
 __device__ __forceinline__ float int_epilogue(const TcParams &p, int kind, int acc, int f, float bias) {
-    if (kind == 1) {
+    if (kind == TC_S8) {
         int q16 = acc / 32;
         q16 = q16 > 32767 ? 32767 : (q16 < -32767 ? -32767 : q16);
         const float t = __fadd_rn(__fmul_rn((float)q16, p.alpha1), bias);
@@ -482,20 +561,17 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
           const __grid_constant__ CUtensorMap tmO1, const __grid_constant__ CUtensorMap tmR, const TcParams p) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = smem_base(smem_raw);
-    const uint32_t bstat_bar = base + p.sm.bstat_bar;
 
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
     const int lane = threadIdx.x & 31;
     const int w_first = (int)blockIdx.x, w_step = (int)gridDim.x;
 
     if (warp == TC_PRODUCER_WARP && elect_one()) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-        // full: one arrival (the producer's expect_tx); empty: one arrival per consumer warp
-        for (int s = 0; s < p.stages; ++s) { mbar_init(base + p.sm.full + 8u * s, 1); mbar_init(base + p.sm.empty + 8u * s, TC_EPI_WARPS); }
-        mbar_init(bstat_bar, 1);
-        if (p.tma_epi) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmO) : "memory");
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        prefetch_tmap(&tmA);
+        prefetch_tmap(&tmB);
+        tc_init_ring(p, base);
+        if (p.tma_epi) prefetch_tmap(&tmO);
+        fence_mbar_init();
     }
     // bias (folded batch-norm) for all filter tiles -> shared memory, once per CTA
     const float *bias_s = reinterpret_cast<const float *>(smem_ptr(base + p.sm.bias));
@@ -515,10 +591,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
         }
     }
     __syncthreads();
-    // Programmatic dependent launch: everything above (barrier init, tensor-map prefetch, bias -> smem: weights only)
-    // overlapped the tail of the previous kernel; from here on we touch activations it wrote.
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    pdl_wait_and_launch();
 
     if (warp == TC_PRODUCER_WARP) {
         // ======================= TMA producer =======================
@@ -527,36 +600,29 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
         // ======================= consumers (warps 0..7): wgmma main loop, then the epilogue of the same tile =======================
         const int ew = warp;                      // consumer warp; warpgroup ew >> 2 computes accumulator rows 64 * (ew >> 2) .. + 63
         const int wg = ew >> 2;
-        int stage = 0; uint32_t phase = 0;
+        TcRing ring;
         long long w_full = 0;
-        if (p.bstat) mbar_wait(bstat_bar, 0);
+        if (p.bstat) mbar_wait(base + p.sm.bstat_bar, 0);
         // The K-blocks of the current work item into this warpgroup's registers, then both warpgroups' accumulators into the
         // shared-memory tile.
-        auto mainloop = [&](auto kind_c, auto bn_c, auto kk_c) {
-            constexpr int KIND = decltype(kind_c)::value;
-            constexpr int BN = decltype(bn_c)::value;
-            constexpr int KK = decltype(kk_c)::value;   // wgmmas per K-block
-            using T = typename std::conditional<KIND == 1 || KIND == 2, uint32_t, float>::type;
-            T d[BN / 2];
-            tc_mma_loop<KIND, BN, KK, ST>(d, p, base, wg, lane, stage, phase, w_full);
-            named_bar_sync(TC_ACC_BAR, 32 * TC_EPI_WARPS);   // every warp is done with the previous tile's accumulators
-            acc_store_frag(acc_base, p.acc_pitch, wg * 64, d);
-            named_bar_sync(TC_ACC_BAR, 32 * TC_EPI_WARPS);   // the whole 128 x BN tile is in place
+        auto mainloop = [&](auto kind_c) {
+            tc_dispatch<128>(p, [&](auto bn_c, auto kk_c) {
+                constexpr TcKind KIND = decltype(kind_c)::value;
+                constexpr int BN = decltype(bn_c)::value;
+                constexpr int KK = decltype(kk_c)::value;   // wgmmas per K-block
+                using T = typename std::conditional<KIND == TC_S8 || KIND == TC_XNOR, uint32_t, float>::type;
+                T d[BN / 2];
+                tc_mma_loop<KIND, BN, KK, ST>(d, p, base, wg, lane, ring, w_full);
+                named_bar_sync(TC_ACC_BAR, 32 * TC_EPI_WARPS);   // every warp is done with the previous tile's accumulators
+                acc_store_frag(acc_base, p.acc_pitch, wg * 64, d);
+                named_bar_sync(TC_ACC_BAR, 32 * TC_EPI_WARPS);   // the whole 128 x BN tile is in place
+            });
         };
         auto run_mainloop = [&]() {
-            auto by_kk = [&](auto kind_c, auto bn_c) {
-                if (p.kk == 4) mainloop(kind_c, bn_c, std::integral_constant<int, 4>{});
-                else if (p.kk == 2) mainloop(kind_c, bn_c, std::integral_constant<int, 2>{});
-                else mainloop(kind_c, bn_c, std::integral_constant<int, 1>{});
-            };
-            auto by_bn = [&](auto kind_c) {
-                if (p.BN == 128) by_kk(kind_c, std::integral_constant<int, 128>{});
-                else if (p.BN == 64) by_kk(kind_c, std::integral_constant<int, 64>{});
-                else by_kk(kind_c, std::integral_constant<int, 32>{});
-            };
-            if constexpr (EPI == 2) by_bn(std::integral_constant<int, 1>{});
-            else if (p.kind == 0) by_bn(std::integral_constant<int, 0>{});
-            else by_bn(std::integral_constant<int, 3>{});
+            // EPI 2: TC_XNOR runs the same s8 wgmma as TC_S8
+            if constexpr (EPI == 2) mainloop(std::integral_constant<TcKind, TC_S8>{});
+            else if (p.kind == TC_BF16) mainloop(std::integral_constant<TcKind, TC_BF16>{});
+            else mainloop(std::integral_constant<TcKind, TC_TF32>{});
         };
 
         // Epilogue.  Per slab: read the accumulator row(s) and the residual first, then the math and the stores.
@@ -565,20 +631,15 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
         const int cbeg = (p.BN >= 64) ? half * (p.BN >> 1) : 0;
         const int cend = (p.BN >= 64) ? cbeg + (p.BN >> 1) : (half == 0 ? p.BN : 0);
         const int r = q * 32 + lane;              // accumulator row == pixel within the tile
-        const int tx = r & (p.TW - 1), ty = r >> p.TWlog2;
         const bool leaky = p.act == ACT_LEAKY;
         const uint32_t taddr = acc_base + 4u * (uint32_t)(r * p.acc_pitch);
         const long long t_begin = ST ? clock64() : 0;
         for (int w = w_first; w < p.num_work; w += w_step) {
             run_mainloop();
-            const int n_idx = w % p.nt;
-            const int m = w / p.nt;
-            const int ox = (m % p.xt) * p.TW + tx;
-            const int J = (m / p.xt) * p.TH + p.jshift + ty;
-            const int n0 = n_idx * p.BN;
-            const int img = J / p.PR;
-            const int oy = J - img * p.PR - p.row_off;
-            const bool valid = (img < p.N) && (oy >= 0) && (oy < p.OH) && (ox < p.OW) && !(p.dbg & 4);
+            const TcItem it = tc_item(p, w, p.BN);
+            const TcPixel px = tc_pixel(p, it, r);
+            const int n0 = it.n0, img = px.img, oy = px.oy, ox = px.ox;
+            const bool valid = px.valid(p) && !(p.dbg & 4);
             const long pix = ((long)(img * p.OHp + oy + 1) * p.OWp + ox + 1);
             char *orow = p.out + pix * p.out_ldc * 4;
             const float *bs = bias_s + n0;
@@ -614,7 +675,11 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                         const int left = p.n - (n0 + f0 + g * 4);   // the output may be a channel slice: nothing past filter n
                         if (left <= 0) break;
                         if (left >= 4) op[g] = make_float4(x[g * 4 + 0], x[g * 4 + 1], x[g * 4 + 2], x[g * 4 + 3]);
-                        else for (int e = 0; e < left; ++e) reinterpret_cast<float *>(op + g)[e] = x[g * 4 + e];
+                        else {   // bounded and unrolled: a runtime index into x would put it in local memory
+#pragma unroll
+                            for (int e = 0; e < 3; ++e)
+                                if (e < left) reinterpret_cast<float *>(op + g)[e] = x[g * 4 + e];
+                        }
                     }
                 }
             };
@@ -688,9 +753,9 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                     if (f >= p.n) b8 = 0;
                     if (j < 4) w0 |= (uint32_t)(b8 & 0xff) << (8 * j); else w1 |= (uint32_t)(b8 & 0xff) << (8 * (j - 4));
                 }
-                const int oye = oy & ~1, oxe = ox & ~1;                  // the window's origin: the same pooled pixel in all four lanes
-                if (img < p.N && oye >= 0 && oye < p.OH && oxe < p.OW && !(p.dbg & 4)) {
-                    signed char *dst = p.pool_out + ((size_t)(img * p.pool_Hp + (oye >> 1) + 1) * p.pool_Wp + (oxe >> 1) + 1) * (size_t)p.pool_ldc + n0 + cbase;
+                const TcPixel o{img, oy & ~1, ox & ~1};                 // the window's origin: the same pooled pixel in all four lanes
+                if (o.valid(p) && !(p.dbg & 4)) {
+                    signed char *dst = p.pool_out + ((size_t)(img * p.pool_Hp + (o.oy >> 1) + 1) * p.pool_Wp + (o.ox >> 1) + 1) * (size_t)p.pool_ldc + n0 + cbase;
                     *reinterpret_cast<uint2 *>(dst) = make_uint2(w0, w1);
                 }
             };
@@ -715,7 +780,8 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
                 named_bar_sync(1 + g, 128);
                 if (boss) {
-                    tma_store_3d(&tmO, out_tile, n0 + f0, (m % p.xt) * p.TW + 1, (m / p.xt) * p.TH + p.jshift);
+                    const TcItem t = tc_item(p, w, p.BN);   // decoded again here: EPI 2 spills when `it` stays live
+                    tma_store_3d(&tmO, out_tile, n0 + f0, t.x0 + 1, t.J0);
                     tma_store_commit();
                 }
             };
@@ -723,7 +789,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
             if constexpr (EPI == 2) {
                 // ---- integer kinds: the exact float epilogue per 32-column slab (or the fused max-pool), f32 stores
                 auto int_slabs = [&](auto kind_c) {
-                    constexpr int KIND = decltype(kind_c)::value;
+                    constexpr TcKind KIND = decltype(kind_c)::value;
                     for (int f0 = cbeg; f0 < cend; f0 += 32) {
                         uint32_t v0[32];
                         acc_ld32(taddr + 4u * (uint32_t)f0, v0);
@@ -738,12 +804,12 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                         for (int j = 0; j < 32; ++j) {
                             const int f = n0 + f0 + j;
                             // raw results: the INT8 accumulator; XNOR: the reference's popcount, (dot + K) / 2
-                            if (f < p.n) p.acc_out[(((size_t)img * p.n + f) * p.OH + oy) * p.OW + ox] = KIND == 2 ? ((int)v0[j] + p.xK) / 2 : (int)v0[j];
+                            if (f < p.n) p.acc_out[(((size_t)img * p.n + f) * p.OH + oy) * p.OW + ox] = KIND == TC_XNOR ? ((int)v0[j] + p.xK) / 2 : (int)v0[j];
                         }
                     }
                 };
-                if (p.kind == 2) int_slabs(std::integral_constant<int, 2>{});
-                else int_slabs(std::integral_constant<int, 1>{});
+                if (p.kind == TC_XNOR) int_slabs(std::integral_constant<TcKind, TC_XNOR>{});
+                else int_slabs(std::integral_constant<TcKind, TC_S8>{});
             } else {
                 for (int f0 = cbeg; f0 < cend; f0 += 64) {
                     if (cend - f0 >= 64) {
@@ -761,7 +827,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
             }
         }
         if (EPI == 2 && p.tma_epi && q == 0 && lane == 0) tma_store_wait_all();   // this group's bulk stores have completed
-        if (ST && p.stats && ew == 0 && lane == 0) { p.stats[blockIdx.x * 16 + 2] = (unsigned long long)w_full; p.stats[blockIdx.x * 16 + 6] = (unsigned long long)(clock64() - t_begin); }
+        if (ST && p.stats && ew == 0 && lane == 0) { tc_stat(p, STAT_CONS_WAIT_FULL) = w_full; tc_stat(p, STAT_CONS_TOTAL) = clock64() - t_begin; }
     }
 }
 
@@ -799,8 +865,8 @@ constexpr int TCR_STORE_WARP = 9;                                // store warps 
 constexpr int TCR_MAX_SLABS = 4;                                 // BN / SW <= 256 / 64
 
 // Store thread of consumer warpgroup g: walks the consumers' work items (see k_conv_tc_reg).  buf: the warpgroup's staging buffer,
-// stg_full: its first per-slab barrier.  ST: cycles spent waiting on stg_full and in cp.async.bulk.wait_group.read go to stats
-// slots 4 and 5 (warpgroup 0's thread).
+// stg_full: its first per-slab barrier.  ST: cycles spent waiting on stg_full and in cp.async.bulk.wait_group.read go to
+// STAT_STORE_WAIT_FULL and STAT_STORE_WAIT_READ (warpgroup 0's thread).
 template <bool ST>
 __device__ __forceinline__ void tcr_store(const CUtensorMap *tmO, const CUtensorMap *tmO1, const CUtensorMap *tmR, const TcParams &p,
                                           uint32_t buf, uint32_t stg_full, uint32_t stg_ready, int g, int w_first, int w_step) {
@@ -814,8 +880,8 @@ __device__ __forceinline__ void tcr_store(const CUtensorMap *tmO, const CUtensor
     // image (rows past the batch fall outside the tensor), y = -1 - J0 for one that straddles two images (stored row by row;
     // J0: merged row of its first tile row).
     auto item = [&](int w, int &n0, int &x, int &y) {
-        const int m = w / p.nt;
-        n0 = (w % p.nt) * BN; x = (m % p.xt) * p.TW + 1 + hx; y = (m / p.xt) * p.TH + p.jshift + hy;
+        const TcItem it = tc_item(p, w, BN);
+        n0 = it.n0; x = it.x0 + 1 + hx; y = it.J0 + hy;
         if (p.stride2) {
             const int i0 = y / p.PR, i1 = min((y + max(p.TH >> 1, 1) - 1) / p.PR, p.N - 1);
             y = i0 == i1 ? y + i0 + 1 : -1 - y;
@@ -832,10 +898,7 @@ __device__ __forceinline__ void tcr_store(const CUtensorMap *tmO, const CUtensor
             src += (uint32_t)(p.TW * 2 * SW);
         }
     };
-    auto wait_read = [&]() {   // the bulk stores issued so far have read shared memory
-        if constexpr (ST) { const long long c0 = clock64(); tma_store_wait_read0(); w_read += clock64() - c0; }
-        else tma_store_wait_read0();
-    };
+    auto wait_read = [&]() { timed<ST>(w_read, tma_store_wait_read0); };   // the bulk stores issued so far have read shared memory
     auto load_res = [&](int s, int n0, int x, int y) {
         tma_load_3d_hint(buf + (uint32_t)s * tile, tmR, stg_ready, n0 + s * SW, x, y, l2_policy_evict_first());
     };
@@ -858,8 +921,7 @@ __device__ __forceinline__ void tcr_store(const CUtensorMap *tmO, const CUtensor
         const int nsn = next ? item(w + w_step, n0n, xn, yn) : 0;
         for (int s = 0; s < ns; ++s) {
             const uint32_t fb = stg_full + 8u * (uint32_t)s;
-            if constexpr (ST) { const long long c0 = clock64(); mbar_wait(fb, (phases >> s) & 1u); w_full += clock64() - c0; }
-            else mbar_wait(fb, (phases >> s) & 1u);
+            timed<ST>(w_full, [&] { mbar_wait(fb, (phases >> s) & 1u); });
             phases ^= 1u << s;
             // the consumers are past this item's stg_ready: its phase is complete and the next item's may begin
             if (s == 0 && res_next) mbar_arrive_expect_tx(stg_ready, (uint32_t)nsn * tile);
@@ -875,7 +937,7 @@ __device__ __forceinline__ void tcr_store(const CUtensorMap *tmO, const CUtensor
         }
     }
     tma_store_wait_all();   // bulk groups are per thread: these are this warpgroup's stores only
-    if (ST && p.stats && g == 0) { p.stats[blockIdx.x * 16 + 4] = (unsigned long long)w_full; p.stats[blockIdx.x * 16 + 5] = (unsigned long long)w_read; }
+    if (ST && p.stats && g == 0) { tc_stat(p, STAT_STORE_WAIT_FULL) = w_full; tc_stat(p, STAT_STORE_WAIT_READ) = w_read; }
 }
 
 template <bool ST>
@@ -884,7 +946,6 @@ k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
               const __grid_constant__ CUtensorMap tmO1, const __grid_constant__ CUtensorMap tmR, const TcParams p) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = smem_base(smem_raw);
-    const uint32_t bstat_bar = base + p.sm.bstat_bar;
     // per consumer warpgroup g: stg_full for each of up to TCR_MAX_SLABS slabs, and stg_ready
     auto stg_full = [&](int g, int s) { return base + p.sm.stg_full + 8u * (uint32_t)(g * TCR_MAX_SLABS + s); };
     auto stg_ready = [&](int g) { return base + p.sm.stg_ready + 8u * (uint32_t)g; };
@@ -898,29 +959,26 @@ k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     const int w_first = (int)blockIdx.x, w_step = (int)gridDim.x;
     const bool epi_mem = !(p.dbg & 4);
 
-    if (warp == 8 && elect_one()) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmO) : "memory");
-        if (p.stride2) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmO1) : "memory");
-        if (p.res) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmR) : "memory");
-        for (int s = 0; s < p.stages; ++s) { mbar_init(base + p.sm.full + 8u * s, 1); mbar_init(base + p.sm.empty + 8u * s, TC_EPI_WARPS); }
-        mbar_init(bstat_bar, 1);
+    if (warp == TC_PRODUCER_WARP && elect_one()) {
+        prefetch_tmap(&tmA);
+        prefetch_tmap(&tmB);
+        prefetch_tmap(&tmO);
+        if (p.stride2) prefetch_tmap(&tmO1);
+        if (p.res) prefetch_tmap(&tmR);
+        tc_init_ring(p, base);
         for (int g = 0; g < 2; ++g) {
             for (int s = 0; s < TCR_MAX_SLABS; ++s) mbar_init(stg_full(g, s), 4);
             mbar_init(stg_ready(g), 1);
         }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        fence_mbar_init();
     }
     for (int i = threadIdx.x; i < p.nt * p.BN; i += TCR_THREADS) bias_s[i] = (i < p.n) ? __ldg(p.bias + i) : 0.f;
     __syncthreads();
-    // Programmatic dependent launch: everything above overlapped the tail of the previous kernel
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    pdl_wait_and_launch();
 
     if (wg == 2) {
         asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(TCR_PRODUCER_REGS));
-        if (warp == 8) {
+        if (warp == TC_PRODUCER_WARP) {
             if (elect_one()) tc_produce<ST>(&tmA, &tmB, p, base, w_first, w_step);
         } else if (warp < TCR_STORE_WARP + 2 && epi_mem) {
             const int g = warp - TCR_STORE_WARP;
@@ -935,14 +993,14 @@ k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     const int rl = 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);
     const bool leaky = p.act == ACT_LEAKY, leaky2 = p.act2 == ACT_LEAKY;
     const bool has_res = p.res != nullptr;
-    int stage = 0; uint32_t phase = 0;
+    TcRing ring;
     uint32_t stg_phase = 0;
     // w_ready: waits on stg_ready after the first work item (the first item's, whose residual fetch overlaps only one main loop,
-    // goes to stats slot 3 right away)
+    // goes to STAT_CONS_FIRST_READY right away)
     long long w_full = 0, w_ready = 0; const long long t_begin = ST ? clock64() : 0;
-    if (p.bstat) mbar_wait(bstat_bar, 0);
+    if (p.bstat) mbar_wait(base + p.sm.bstat_bar, 0);
 
-    auto run = [&](auto bn_c, auto kk_c) {
+    tc_dispatch<256>(p, [&](auto bn_c, auto kk_c) {
         constexpr int BN = decltype(bn_c)::value;
         constexpr int KK = decltype(kk_c)::value;
         constexpr int SW = BN >= 64 ? 64 : 32;             // slab width (columns); rows of 128 B (128B swizzle) or 64 B (64B swizzle)
@@ -955,28 +1013,20 @@ k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
         };
         for (int w = w_first; w < p.num_work; w += w_step) {
             float d[BN / 2];
-            tc_mma_loop<0, BN, KK, ST>(d, p, base, wg, lane, stage, phase, w_full);
+            tc_mma_loop<TC_BF16, BN, KK, ST>(d, p, base, wg, lane, ring, w_full);
             if (!epi_mem) continue;
-            const int n0 = (w % p.nt) * BN, m = w / p.nt;
-            const int x0 = (m % p.xt) * p.TW, J0 = (m / p.xt) * p.TH + p.jshift;
+            const TcItem it = tc_item(p, w, BN);
+            const int n0 = it.n0;
             bool valid[2];
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {                  // border / padding rows of the merged-row tiling are stored as zeros
-                const int r = 64 * wg + rl + 8 * h;
-                const int ox = x0 + (r & (p.TW - 1)), J = J0 + (r >> p.TWlog2);
-                const int img = J / p.PR, oy = J - img * p.PR - p.row_off;
-                valid[h] = img < p.N && oy >= 0 && oy < p.OH && ox < p.OW;
-            }
+            for (int h = 0; h < 2; ++h)                    // border / padding rows of the merged-row tiling are stored as zeros
+                valid[h] = tc_pixel(p, it, 64 * wg + rl + 8 * h).valid(p);
             const int nslab = (min(BN, p.n - n0) + SW - 1) / SW;   // slabs holding filters < n
             // the buffer is back from the store thread: the previous item's bulk stores have read it, this item's residual is in it
-            if constexpr (ST) {
-                const long long c0 = clock64();
-                mbar_wait(stg_ready(wg), stg_phase);
-                const long long dt = clock64() - c0;
-                if (w != w_first) w_ready += dt;
-                else if (p.stats && warp == 0 && lane == 0) p.stats[blockIdx.x * 16 + 3] = (unsigned long long)dt;
-            }
-            else mbar_wait(stg_ready(wg), stg_phase);
+            long long dt = 0;
+            timed<ST>(dt, [&] { mbar_wait(stg_ready(wg), stg_phase); });
+            if (w != w_first) w_ready += dt;
+            else if (ST && p.stats && warp == 0 && lane == 0) tc_stat(p, STAT_CONS_FIRST_READY) = dt;
             stg_phase ^= 1u;
 #pragma unroll
             for (int s = 0; s < BN / SW; ++s) {
@@ -1027,18 +1077,11 @@ k_conv_tc_reg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
                 if (lane == 0) mbar_arrive(stg_full(wg, s));
             }
         }
-    };
-    auto by_kk = [&](auto bn_c) {
-        if (p.kk == 4) run(bn_c, std::integral_constant<int, 4>{});
-        else if (p.kk == 2) run(bn_c, std::integral_constant<int, 2>{});
-        else run(bn_c, std::integral_constant<int, 1>{});
-    };
-    if (p.BN == 256) by_kk(std::integral_constant<int, 256>{});
-    else if (p.BN == 128) by_kk(std::integral_constant<int, 128>{});
-    else if (p.BN == 64) by_kk(std::integral_constant<int, 64>{});
-    else by_kk(std::integral_constant<int, 32>{});
-    if (ST && p.stats && warp == 0 && lane == 0) { p.stats[blockIdx.x * 16 + 2] = (unsigned long long)w_full; p.stats[blockIdx.x * 16 + 6] = (unsigned long long)(clock64() - t_begin);
-                                                    p.stats[blockIdx.x * 16 + 8] = (unsigned long long)w_ready; }
+    });
+    if (ST && p.stats && warp == 0 && lane == 0) {
+        tc_stat(p, STAT_CONS_WAIT_FULL) = w_full; tc_stat(p, STAT_CONS_WAIT_READY) = w_ready;
+        tc_stat(p, STAT_CONS_TOTAL) = clock64() - t_begin;
+    }
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -1166,8 +1209,8 @@ __global__ void __launch_bounds__(128) k_stem_tc(StemTcP p) {
 #pragma unroll
             for (int k = 0; k < 2; ++k) {
                 const uint64_t bdesc = wg_desc(b_addr + 32u * k, hi);
-                Wg<0, 32>::mma(d0, wg_desc(a_addr + 32u * k, hi), bdesc, (uint32_t)k);            // pixels 0..63
-                Wg<0, 32>::mma(d1, wg_desc(a_addr + 64u * 64u + 32u * k, hi), bdesc, (uint32_t)k);  // pixels 64..127
+                Wg<TC_BF16, 32>::mma(d0, wg_desc(a_addr + 32u * k, hi), bdesc, (uint32_t)k);            // pixels 0..63
+                Wg<TC_BF16, 32>::mma(d1, wg_desc(a_addr + 64u * 64u + 32u * k, hi), bdesc, (uint32_t)k);  // pixels 64..127
             }
             wg_commit();
             wg_wait<0>();
@@ -1366,7 +1409,7 @@ __global__ void __launch_bounds__(256, 2) k_stem_s2_tc(StemTcP p) {
         for (int c = 0; c < 5; ++c)
 #pragma unroll
             for (int k = 0; k < 2; ++k)
-                Wg<0, 32>::mma(ds[c], wg_desc(U + (uint32_t)(5 * wg + c) * 4096u + 32u * k, hi), wg_desc(base + S2_BS + 32u * k, hi), (uint32_t)k);
+                Wg<TC_BF16, 32>::mma(ds[c], wg_desc(U + (uint32_t)(5 * wg + c) * 4096u + 32u * k, hi), wg_desc(base + S2_BS + 32u * k, hi), (uint32_t)k);
         wg_commit();
         wg_wait<0>();
 #pragma unroll
@@ -1421,7 +1464,7 @@ __global__ void __launch_bounds__(256, 2) k_stem_s2_tc(StemTcP p) {
             const uint32_t b = base + S2_B1 + (uint32_t)r * 4096u;
 #pragma unroll
             for (int k = 0; k < 2; ++k)
-                Wg<0, 64>::mma(d, wg_desc(a + 32u * k, hi), wg_desc(b + 32u * k, hi), (r > 0 || k > 0) ? 1u : 0u);
+                Wg<TC_BF16, 64>::mma(d, wg_desc(a + 32u * k, hi), wg_desc(b + 32u * k, hi), (r > 0 || k > 0) ? 1u : 0u);
         }
         wg_commit();
         wg_wait<0>();
@@ -1813,9 +1856,9 @@ TcPlanPtr tc_make_plan(const TcConv &c) {
     if (cudaFuncSetAttribute((const void *)plan->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
         fatal_throw("cudaFuncSetAttribute(k_conv_tc) failed");
     if (st) {
-        plan->stats.ensure(16 * (size_t)plan->grid);
+        plan->stats.ensure(TC_NSTATS * (size_t)plan->grid);
         p.stats = plan->stats.get();
-        cudaMemset(p.stats, 0, sizeof(unsigned long long) * 16 * plan->grid);
+        cudaMemset(p.stats, 0, sizeof(unsigned long long) * TC_NSTATS * plan->grid);
     }
     return plan;
 }
@@ -1914,17 +1957,19 @@ void tc_launch(const TcPlan &P, cudaStream_t s) {
 
 void TcPlanDelete::operator()(TcPlan *plan) const {
     if (plan->p.stats) {   // diagnostic dump: mean cycles per CTA of the LAST launch
-        std::vector<unsigned long long> h(16 * (size_t)plan->grid);
+        std::vector<unsigned long long> h(TC_NSTATS * (size_t)plan->grid);
         cudaDeviceSynchronize();
         cudaMemcpy(h.data(), plan->p.stats, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
-        double m[16] = {0};
-        for (int b = 0; b < plan->grid; ++b) for (int k = 0; k < 16; ++k) m[k] += (double)h[16 * b + k] / plan->grid;
+        double m[TC_NSTATS] = {0};
+        for (int b = 0; b < plan->grid; ++b) for (int k = 0; k < TC_NSTATS; ++k) m[k] += (double)h[TC_NSTATS * b + k] / plan->grid;
         fprintf(stderr, "TCSTATS %-28s tiles/cta %.1f kb %d sps %d BN %d | producer: wait_empty %.0f tma_issue %.0f total %.0f | ",
-                plan->desc, (double)plan->p.num_work / plan->grid, plan->p.kblocks, plan->p.sps, plan->p.BN, m[0], m[7], m[1]);
+                plan->desc, (double)plan->p.num_work / plan->grid, plan->p.kblocks, plan->p.sps, plan->p.BN,
+                m[STAT_PROD_WAIT_EMPTY], m[STAT_PROD_TMA_ISSUE], m[STAT_PROD_TOTAL]);
         if (plan->reg)   // k_conv_tc_reg: the consumers' wait on stg_ready (first work item apart) and the store warps
             fprintf(stderr, "consumers: wait_full %.0f wait_ready %.0f (first item %.0f) total %.0f | store: wait_full %.0f wait_read %.0f\n",
-                    m[2], m[8], m[3], m[6], m[4], m[5]);
-        else fprintf(stderr, "consumers: wait_full %.0f total %.0f\n", m[2], m[6]);
+                    m[STAT_CONS_WAIT_FULL], m[STAT_CONS_WAIT_READY], m[STAT_CONS_FIRST_READY], m[STAT_CONS_TOTAL],
+                    m[STAT_STORE_WAIT_FULL], m[STAT_STORE_WAIT_READ]);
+        else fprintf(stderr, "consumers: wait_full %.0f total %.0f\n", m[STAT_CONS_WAIT_FULL], m[STAT_CONS_TOTAL]);
     }
     delete plan;
 }
