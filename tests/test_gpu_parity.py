@@ -372,7 +372,7 @@ def test_int8_calibration_on_device(name, workdir):
 
 @pytest.mark.parametrize("name,q", [("tiny64", 1), ("xnor64", 0), ("tinyvoc64", 1), ("tiny_w96_h64", 1)])
 def test_maxpool_fused_with_quantise_or_binarise_is_bit_exact(name, q, workdir):
-    """fuse=1 lets a max-pool write the s8 / sign input of the integer convolution that follows (k_maxpool_fused):
+    """fuse=1 lets a max-pool write the s8 / sign input of the integer convolution that follows (k_int_input):
     the same values in the same order as max-pool + quantise / binarise, so everything downstream is bit-identical."""
     import yolo2_light_b200 as yb
     B = 3
@@ -460,7 +460,7 @@ def test_fused_stem_pool_is_bit_identical_to_the_three_kernels(builder, w, h, q,
     for i, o in a.detection_outputs().items():
         assert util.rel_l2(o, b.layer_output(i)) <= 1e-5, (builder.__name__, i)
     # production configuration (no raw-accumulator dump): the max-pools behind the integer convolutions run in their epilogues
-    # (TcConv::pool_mode) -- every integer layer that is still materialised is bit-identical to the unfused plan
+    # (TcConv::pool_fmt) -- every integer layer that is still materialised is bit-identical to the unfused plan
     c = yb.load_network(cfg, wts, batch=B, quantized=q)
     c.predict(x, quantized=bool(q))
     assert c.last_launches() < b.last_launches()

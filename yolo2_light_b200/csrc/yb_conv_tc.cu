@@ -97,11 +97,11 @@ struct TcParams {
     uint32_t stg_bytes;       // epilogue staging / TMA-epilogue tiles
     int acc_pitch;            // words per row of the shared-memory accumulator tile (BN + 4: conflict-free row reads)
     // Fused 2x2 / stride-2 max-pool + input conversion of the NEXT integer layer (integer kinds, tiles of 8 x 16 pixels):
-    // the epilogue reduces every 2x2 window inside the warp (lane ^ 1 = x neighbour, lane ^ 8 = y neighbour), quantises (pool_mode
-    // 1: quant_i8 with pool_mult) or takes the sign (pool_mode 2: +-1 bytes) and writes bytes straight into the next layer's s8
-    // input: the f32 activation and the pooled f32 tensor never reach HBM.  jshift = 1 moves every tile down one merged row so
+    // the epilogue reduces every 2x2 window inside the warp (lane ^ 1 = x neighbour, lane ^ 8 = y neighbour), converts it into
+    // the next layer's side format pool_fmt (SIDE_S8 with pool_mult, or SIDE_PM1_S8) and writes bytes straight into that layer's
+    // input: the f32 activation and the pooled f32 tensor never reach HBM.  pool_fmt SIDE_NONE: no fused max-pool.  jshift = 1 moves every tile down one merged row so
     // that window rows (oy even, oy + 1) fall into the same tile (the padded layout puts oy = 0 on an odd merged row).
-    int pool_mode, jshift;
+    int pool_fmt, jshift;     // SideFmt
     float pool_mult;
     signed char *pool_out; long pool_ldc; int pool_Hp, pool_Wp;   // next layer's s8 input: padded NHWC, bytes
     int sps;                                  // K-blocks per pipeline stage (amortises the per-stage barrier round trip)
@@ -532,21 +532,11 @@ __device__ __forceinline__ void tc_mma_loop(T (&d)[BN / 2], const TcParams &p, u
     if (pend >= 0) release(pend);
 }
 
-// The reference's float epilogue of the integer kinds, with its operations in its order (bit-exact results):
-//   TC_S8, INT8 (yolov2_forward_network_quantized.c:474-490, :598-627): q16 = clamp(+-32767, acc / 32) [C truncating
-//     division]; y = (float)q16 * ALPHA1; y += bias; leaky: y / 10.
-//   TC_XNOR, XNOR as +-1 s8 (acc == 2*count - K exactly): y = act((float)acc * mean + bias) (additionally.c:1531,
-//     yolov2_forward_network.c:243-261).
-// f: filter index (TC_XNOR reads its mean |w|).
+// The reference's float epilogue of the integer kinds (bit-exact): TC_S8 int8_epilogue; TC_XNOR xnor_epilogue, where the s8
+// wgmma's acc is dot = 2*count - K exactly.  f: filter index (TC_XNOR reads its mean |w|).
 __device__ __forceinline__ float int_epilogue(const TcParams &p, int kind, int acc, int f, float bias) {
-    if (kind == TC_S8) {
-        int q16 = acc / 32;
-        q16 = q16 > 32767 ? 32767 : (q16 < -32767 ? -32767 : q16);
-        const float t = __fadd_rn(__fmul_rn((float)q16, p.alpha1), bias);
-        return (p.act == ACT_LEAKY) ? ((t > 0.f) ? t : __fdiv_rn(t, 10.f)) : t;
-    }
-    const float t = __fadd_rn(__fmul_rn((float)acc, (f < p.n) ? __ldg(p.mean + f) : 0.f), bias);
-    return act_exact(t, p.act);
+    if (kind == TC_S8) return int8_epilogue(acc, p.alpha1, bias, p.act);
+    return xnor_epilogue(acc, (f < p.n) ? __ldg(p.mean + f) : 0.f, bias, p.act);
 }
 
 // One CTA per 128-pixel x BN-filter tile, persistent over the tiles (grid <= #SMs, one CTA per SM).
@@ -720,7 +710,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                 __syncwarp();
             };
 
-            // ---- fused 2x2/2 max-pool + conversion to the next integer layer's input (TcParams::pool_mode).  Both epilogue functions
+            // ---- fused 2x2/2 max-pool + conversion to the next integer layer's input (TcParams::pool_fmt).  Both epilogue functions
             // are monotone non-decreasing in the s32 accumulator (truncating /32, clamp, x positive ALPHA1, + bias, leaky; resp.
             // x mean >= 0, + bias, leaky), so max over the window commutes with them EXACTLY: the window maximum is taken on the raw
             // accumulators and the float epilogue runs once per pooled value.  Window = lanes {l, l^1, l^8, l^9} (tile rows are 8
@@ -749,9 +739,9 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                 for (int j = 0; j < 8; ++j) {
                     const int f = n0 + cbase + j;
                     const float t = int_epilogue(p, p.kind, h8[j], f, bs[cbase + j]);
-                    int b8 = (p.pool_mode == 1) ? quant_i8(t, p.pool_mult) : (t > 0.f ? 1 : -1);
+                    uint32_t b8 = (p.pool_fmt == SIDE_S8) ? side_code<SIDE_S8>(t, p.pool_mult) : side_code<SIDE_PM1_S8>(t, 0.f);
                     if (f >= p.n) b8 = 0;
-                    if (j < 4) w0 |= (uint32_t)(b8 & 0xff) << (8 * j); else w1 |= (uint32_t)(b8 & 0xff) << (8 * (j - 4));
+                    if (j < 4) w0 |= side_place<SIDE_S8>(b8, j); else w1 |= side_place<SIDE_S8>(b8, j - 4);
                 }
                 const TcPixel o{img, oy & ~1, ox & ~1};                 // the window's origin: the same pooled pixel in all four lanes
                 if (o.valid(p) && !(p.dbg & 4)) {
@@ -793,7 +783,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                     for (int f0 = cbeg; f0 < cend; f0 += 32) {
                         uint32_t v0[32];
                         acc_ld32(taddr + 4u * (uint32_t)f0, v0);
-                        if (p.pool_mode) { pool_store_raw(v0, f0); continue; }
+                        if (p.pool_fmt != SIDE_NONE) { pool_store_raw(v0, f0); continue; }
                         float y[32];
 #pragma unroll
                         for (int j = 0; j < 32; ++j) y[j] = int_epilogue(p, KIND, (int)v0[j], n0 + f0 + j, bs[f0 + j]);
@@ -1633,8 +1623,8 @@ void plan_tiles(TcParams &p, const TcConv &c, bool reg, int sms) {
     }
     // a fused 2x2 max-pool needs 8 x 16 tiles that start one merged row down -- row 0 is a border row, and 2x2 windows then
     // never straddle tiles
-    if (c.pool_mode) tw = 8;
-    p.jshift = c.pool_mode ? 1 : 0;
+    if (c.pool_fmt != SIDE_NONE) tw = 8;
+    p.jshift = c.pool_fmt != SIDE_NONE ? 1 : 0;
     auto set_tw = [&](int t) {
         p.TW = t; p.TH = 128 / t;
         p.TWlog2 = 0; while ((1 << p.TWlog2) < p.TW) ++p.TWlog2;
@@ -1674,7 +1664,7 @@ void plan_epilogue(TcParams &p, const TcConv &c, bool reg) {
     p.acc_out = c.acc_out;
     p.yolo_out = c.yolo_out;
     p.yolo_per = c.yolo_out ? 4 + c.yolo_classes + 1 : 0;
-    p.pool_mode = c.pool_mode; p.pool_mult = c.pool_mult;
+    p.pool_fmt = c.pool_fmt; p.pool_mult = c.pool_mult;
     p.pool_out = reinterpret_cast<signed char *>(c.pool_next.base); p.pool_ldc = c.pool_next.ldc;
     p.pool_Hp = c.pool_next.Hp; p.pool_Wp = c.pool_next.Wp;
 }
@@ -1815,7 +1805,7 @@ int tc_conv_supported(const TcConv &c) {
     if (channel_row(operand_channels(c), elem_size(c.kind)) == 0 || c.in.P != 1 || !aligned(c.in, elem_size(c.kind))) return 0;
     // bf16 output: the bf16 kind only, whole 16-byte filter groups
     if (c.out_bf16 && (c.kind != TC_BF16 || l.n % 8 != 0)) return 0;
-    if (c.out.base ? (c.out.P != 1 || !aligned(c.out, c.out_bf16 ? 2 : 4)) : !(c.yolo_out || c.pool_mode)) return 0;
+    if (c.out.base ? (c.out.P != 1 || !aligned(c.out, c.out_bf16 ? 2 : 4)) : !(c.yolo_out || c.pool_fmt != SIDE_NONE)) return 0;
     // fused shortcut: k_conv_tc_reg at stride 1
     if (c.res.base && !(c.kind == TC_BF16 && c.out_bf16 && l.stride == 1 && c.res.H == l.out_h && c.res.W == l.out_w &&
                         c.res.C == l.n && aligned(c.res, 2)))
@@ -1824,7 +1814,7 @@ int tc_conv_supported(const TcConv &c) {
     if (c.yolo_out && (integer || c.out_bf16)) return 0;
     // fused max-pool: the 8 x 16 tiles of the stride-1 3x3 integer layers start one merged row down, so 2x2 windows never
     // straddle tiles when the padded height and the output size are even; the epilogue writes whole 32-filter groups of bytes
-    if (c.pool_mode && !(integer && (c.pool_mode == 1 || c.pool_mode == 2) && !c.acc_out && l.size == 3 && l.stride == 1 &&
+    if (c.pool_fmt != SIDE_NONE && !(integer && (c.pool_fmt == SIDE_S8 || c.pool_fmt == SIDE_PM1_S8) && !c.acc_out && l.size == 3 && l.stride == 1 &&
                          l.h % 2 == 0 && l.out_h % 2 == 0 && l.out_w % 2 == 0 && l.n % 32 == 0 &&
                          c.pool_next.H == l.out_h / 2 && c.pool_next.W == l.out_w / 2 && aligned(c.pool_next, 1)))
         return 0;

@@ -5,18 +5,10 @@
 
 #include <memory>
 
-#include "yb_kernels.cuh"
+#include "yb_device.cuh"
 #include "yb_model.h"
 
 namespace yb {
-
-// Operand types of a tensor-core convolution
-enum TcKind {
-    TC_BF16 = 0,   // bf16 x bf16 -> f32; bf16 or f32 output
-    TC_S8 = 1,     // INT8: s8 x s8 -> s32, the reference's exact requantising epilogue; f32 output
-    TC_XNOR = 2,   // XNOR layer as +-1 s8 on the s8 wgmma (dot = 2*count - K exactly); f32 output
-    TC_TF32 = 3,   // f32 operands read as tf32: the float detection heads of the exact (INT8 / XNOR) networks; f32 output
-};
 
 // The diagnostic switches of the tensor-core plans (DESIGN, appendix), read with the engine's
 struct TcSwitches {
@@ -45,9 +37,9 @@ struct TcConv {
     int *acc_out = nullptr;        // integer kinds: raw s32 accumulators / popcounts, NCHW (tests), or null
     float *yolo_out = nullptr;     // fused [yolo] layer: its NCHW f32 output, or null
     int yolo_classes = 0;
-    int pool_mode = 0;             // fused 2x2/2 max-pool + next integer layer's input conversion: 1 s8 quantised, 2 +-1 bytes; 0 none
-    float pool_mult = 0.f;         // pool_mode 1: the next layer's input multiplier
-    TV pool_next{};                // the next integer layer's s8 input
+    SideFmt pool_fmt = SIDE_NONE;  // fused 2x2/2 max-pool + the next integer layer's input conversion into this format; SIDE_NONE: none
+    float pool_mult = 0.f;         // SIDE_S8: the next layer's input multiplier
+    TV pool_next{};                // the next integer layer's input
     TcSwitches sw{};
 };
 

@@ -1,0 +1,139 @@
+// yb_device.cuh -- what the SIMT kernels (yb_kernels.cuh) and the tensor-core kernels (yb_conv_tc.cu) share: the tensor view,
+// the activations, the operand kinds and, defined once, the integer layers' arithmetic -- the conversion of an f32 activation
+// into an integer convolution's input and the reference's float epilogues of the XNOR and INT8 convolutions.  Every kernel
+// that converts or finishes an integer layer calls these, so all of them stay bit-identical to the reference together.
+#pragma once
+#include <cuda_bf16.h>
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+namespace yb {
+
+struct TV {            // tensor view (POD, passed by value to kernels)
+    char *base;        // address of channel 0 of padded pixel (n=0, y=-P, x=-P)
+    int N, H, W, C;
+    int ldc;           // elements per pixel in the underlying buffer
+    int P;             // border
+    int Hp, Wp;        // H+2P, W+2P
+};
+
+template <typename T>
+__device__ __forceinline__ T *tv_px(const TV &t, int n, int y, int x) {
+    return reinterpret_cast<T *>(t.base) + ((size_t)(n * t.Hp + y + t.P) * t.Wp + (x + t.P)) * (size_t)t.ldc;
+}
+
+// an f32 view whose every 4-channel group can be read with one 16-byte load
+__host__ __device__ __forceinline__ bool vec4_view(const TV &t) {
+    return t.ldc % 4 == 0 && (reinterpret_cast<uintptr_t>(t.base) & 15) == 0;
+}
+
+__device__ __forceinline__ float to_f32(float v) { return v; }
+__device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
+template <typename T> __device__ __forceinline__ T from_f32(float v);
+template <> __device__ __forceinline__ float from_f32<float>(float v) { return v; }
+template <> __device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+
+enum { ACT_LOGISTIC = 0, ACT_RELU = 1, ACT_LINEAR = 3, ACT_LEAKY = 7 };
+
+// activate(), reference additionally.h:126-157 (scalar build): leaky = x>0 ? x : (float)(.1 * (double)x),
+// logistic = (float)(1./(1.+exp(-x))) in double.  Used by the "exact" paths.
+__device__ __forceinline__ float act_exact(float x, int a) {
+    if (a == ACT_LEAKY) return (x > 0.f) ? x : (float)(0.1 * (double)x);
+    if (a == ACT_LINEAR) return x;
+    if (a == ACT_LOGISTIC) return (float)(1.0 / (1.0 + exp(-(double)x)));
+    if (a == ACT_RELU) return x * (x > 0.f);
+    return x;
+}
+
+// Operand types of a tensor-core convolution
+enum TcKind {
+    TC_BF16 = 0,   // bf16 x bf16 -> f32; bf16 or f32 output
+    TC_S8 = 1,     // INT8: s8 x s8 -> s32, the reference's exact requantising epilogue; f32 output
+    TC_XNOR = 2,   // XNOR layer as +-1 s8 on the s8 wgmma (dot = 2*count - K exactly); f32 output
+    TC_TF32 = 3,   // f32 operands read as tf32: the float detection heads of the exact (INT8 / XNOR) networks; f32 output
+};
+
+// The converted ("side") input of an integer convolution, padded NHWC.  The three integer formats are what the kernels write;
+// SIDE_NONE and SIDE_PM1_F32 occur only in the engine's layer plan.
+enum SideFmt {
+    SIDE_NONE = 0,   // no converted input (f32 convolutions); as a fusion: none
+    SIDE_PM1_F32,    // +-1 floats (k_binarize_pm1): the XNOR layers that take the reference's float-GEMM fallback
+    SIDE_S8,         // s8 quant_i8(x, the layer's input multiplier): INT8 convolutions
+    SIDE_PM1_S8,     // +-1 bytes, +1 where x > 0: XNOR layers on the s8 wgmma
+    SIDE_BITS,       // sign bits, bit = (x > 0), 32 channels per 32-bit word: XNOR layers on the popcount kernels
+};
+
+// channels per 32-bit word of an integer side format
+__host__ __device__ constexpr int side_per_word(SideFmt f) { return f == SIDE_BITS ? 32 : 4; }
+// the formats the kernels write: everything but the plan-only SIDE_NONE and SIDE_PM1_F32
+__host__ __device__ constexpr bool side_int(SideFmt f) { return f == SIDE_S8 || f == SIDE_PM1_S8 || f == SIDE_BITS; }
+
+// INT8 input quantisation (reference yolov2_forward_network_quantized.c:527-631): xq = clamp(+-127, (int16_t)(x * input_mult))
+// with x86 float->int16 semantics (cvttss2si, low 16 bits, indefinite -> 0).  NaN and -inf give 0, and so does -FLT_MAX for
+// every multiplier >= 2^-97.
+__device__ __forceinline__ int quant_i8(float x, float mult) {
+    const float v = __fmul_rn(x, mult);
+    int i;
+    if (!(v > -2147483648.0f && v < 2147483648.0f)) i = (int)0x80000000;
+    else i = __float2int_rz(v);
+    int s = (int)(short)(i & 0xffff);
+    if (s > 127) s = 127;
+    if (s < -127) s = -127;
+    return s;
+}
+
+// One f32 value in side format F: the s8 byte (mult: the layer's input multiplier), the +-1 byte or the sign bit, in the low
+// bits of the result.  The sign is x > 0 (binarize_cpu, float_to_bit): NaN, -inf and -FLT_MAX give -1 / 0 alike.
+template <SideFmt F>
+__device__ __forceinline__ uint32_t side_code(float x, float mult) {
+    static_assert(F == SIDE_S8 || F == SIDE_PM1_S8 || F == SIDE_BITS, "integer side formats only");
+    if constexpr (F == SIDE_S8) return (uint32_t)quant_i8(x, mult) & 0xffu;
+    else if constexpr (F == SIDE_PM1_S8) return x > 0.f ? 0x01u : 0xFFu;
+    else return x > 0.f ? 1u : 0u;
+}
+
+// code of channel j (0 <= j < side_per_word(F)) at its place in the word: byte j or bit j
+template <SideFmt F>
+__device__ __forceinline__ uint32_t side_place(uint32_t code, int j) { return code << (F == SIDE_BITS ? j : 8 * j); }
+
+// the word of channels v[0 .. N) in side format F (N <= side_per_word(F))
+template <SideFmt F, int N = side_per_word(F)>
+__device__ __forceinline__ uint32_t side_word(const float *v, float mult) {
+    uint32_t w = 0;
+#pragma unroll
+    for (int j = 0; j < N; ++j) w |= side_place<F>(side_code<F>(v[j], mult), j);
+    return w;
+}
+
+// 16 channels v[0 .. 16) in an s8 side format: four words, one 16-byte store
+template <SideFmt F>
+__device__ __forceinline__ uint4 side_word4(const float *v, float mult) {
+    return make_uint4(side_word<F>(v, mult), side_word<F>(v + 4, mult), side_word<F>(v + 8, mult), side_word<F>(v + 12, mult));
+}
+
+// the 32-bit words of pixel (n, y, x) of a side tensor (s8 formats: ldc in bytes, a multiple of 4; sign bits: ldc in words)
+template <SideFmt F>
+__device__ __forceinline__ uint32_t *side_px(const TV &q, int n, int y, int x) {
+    if constexpr (F == SIDE_BITS) return tv_px<uint32_t>(q, n, y, x);
+    else return reinterpret_cast<uint32_t *>(tv_px<int8_t>(q, n, y, x));
+}
+
+// XNOR epilogue, dot = 2*count - K: act((float)dot * mean + bias) in the reference's float operation order -- one multiply,
+// one add, no FMA contraction (additionally.c:1531, yolov2_forward_network.c:243-261).
+__device__ __forceinline__ float xnor_epilogue(int dot, float mean, float bias, int act) {
+    return act_exact(__fadd_rn(__fmul_rn((float)dot, mean), bias), act);
+}
+
+// INT8 requantising epilogue (yolov2_forward_network_quantized.c:474-490, :598-627): q16 = clamp(+-32767, acc / 32) [C truncating
+// division]; y = (float)q16 * alpha1; y += bias; leaky: y > 0 ? y : y / 10.
+__device__ __forceinline__ float int8_epilogue(int acc, float alpha1, float bias, int act) {
+    int q = acc / 32;
+    if (q > 32767) q = 32767;
+    if (q < -32767) q = -32767;
+    float y = __fmul_rn((float)q, alpha1);
+    y = __fadd_rn(y, bias);
+    if (act == ACT_LEAKY) y = (y > 0.f) ? y : __fdiv_rn(y, 10.f);
+    return y;
+}
+
+}  // namespace yb

@@ -179,7 +179,6 @@ template <typename T> struct same_type { using type = T; };   // keeps a paramet
 
 enum FirstOp { FIRST_NHWC, FIRST_STEM_SIMT, FIRST_STEM_TC, FIRST_STEM_S2, FIRST_STEM_POOL };
 enum ConvPath { CP_NONE, CP_TC, CP_TF32, CP_SIMT, CP_XNOR_FALLBACK, CP_XNOR_TC, CP_XNOR_SMALLK, CP_XNOR_GENERAL, CP_I8_TC, CP_I8_SIMT };
-enum SideFmt { SIDE_NONE, SIDE_PM1_F32, SIDE_S8, SIDE_BITS };   // a convolution's converted input
 
 struct LayerPlan {
     int variant = 0;            // convolutions: 0 fp32, 1 xnor, 2 int8
@@ -187,13 +186,14 @@ struct LayerPlan {
     int fused_into = -1;        // conv + shortcut: this convolution writes the shortcut's output
     bool fused_sc = false;      // shortcut computed in the epilogue of the convolution in front of it
     bool yolo_fused = false;    // conv: writes the [yolo] layer behind it from its epilogue; [yolo]: written that way
-    int pool_mode = 0;          // conv: runs the max-pool behind it and layer i+2's input conversion (1 s8, 2 +-1 bytes, 3 sign bits)
+    SideFmt pool = SIDE_NONE;   // conv: runs the max-pool behind it and writes layer i+2's converted input (in its side format)
     bool pool_in_conv = false;  // max-pool: runs in the epilogue of the convolution in front of it
     bool pool_to_side = false;  // max-pool: writes the next convolution's converted input instead of its own output
     bool prefilled = false;     // conv: its converted input is written by the op in front of it
     bool in_first_op = false;   // computed by the op that reads the caller's images
     int out_dt = DT_F32;
-    int side = SIDE_NONE, side_ld = 0;   // converted input of a convolution and its pixel stride
+    SideFmt side = SIDE_NONE;   // converted input of a convolution ...
+    int side_ld = 0;            // ... and its pixel stride
     bool has_out = false;       // has an NHWC output: own buffer, channel slice of a route's buffer, or alias
     bool materialised = false;  // ... and some op writes it
     int owner = -1, coff = 0;   // channel slice at `coff` of route `owner`'s buffer (owner -1: own buffer or alias)
@@ -203,8 +203,6 @@ struct LayerPlan {
 // Stands in for the activation arena while the plan is made.  Every buffer starts 1024-byte aligned in the arena, so the
 // predicates that check a view's alignment answer the same for views rooted here as for the placed ones.
 static char *const kLayoutBase = reinterpret_cast<char *>(uintptr_t(1) << 40);
-
-static bool vec4_view(const TV &t) { return t.ldc % 4 == 0 && (reinterpret_cast<uintptr_t>(t.base) & 15) == 0; }
 
 // calls put(filter, channel, tap, index into l.weights) for every weight of convolution l
 template <typename F>
@@ -268,18 +266,14 @@ struct Builder {
     // not -1.  Same here: k_binarize_pm1 + the exact-order float convolution.
     static bool xnor_fallback(const Layer &l) { return l.xnor && !(l.stride == 1 && l.pad == 1); }
 
-    // integer conv i -> 2x2/2 max-pool i+1 -> integer conv i+2, nothing else reading i or i+1: the pool and the next layer's
-    // input conversion may run in conv i's epilogue.  Returns the mode (1 s8 quantised, 2 +-1 bytes, 3 sign bits) or 0.
-    int conv_pool_mode(int i) const {
-        if (!opt.fuse || opt.keep_counts || sw.no_conv_pool_fuse || i + 2 >= nl) return 0;
-        const Layer &mp = layer(i + 1), &c2 = layer(i + 2);
-        if (mp.type != YB_MAXPOOL || mp.size != 2 || mp.stride != 2 || mp.pad != 1 || c2.type != YB_CONVOLUTIONAL) return 0;
-        if (!sole_reader(i, i + 1) || !sole_reader(i + 1, i + 2)) return 0;
-        const int v2 = L[i + 2].variant;
-        if (v2 == 2) return 1;
-        if (v2 == 1 && xnor_on_tc(c2) && !xnor_fallback(c2)) return 2;
-        if (v2 == 1 && !xnor_fallback(c2)) return 3;     // next XNOR layer reads sign bits (popcount kernels)
-        return 0;
+    // conv i -> 2x2/2 max-pool i+1 -> integer conv i+2, nothing else reading i or i+1: the pool and the next layer's input
+    // conversion may run in conv i's epilogue.  Returns layer i+2's side format, or SIDE_NONE.
+    SideFmt conv_pool_fmt(int i) const {
+        if (!opt.fuse || opt.keep_counts || sw.no_conv_pool_fuse || i + 2 >= nl) return SIDE_NONE;
+        const Layer &mp = layer(i + 1);
+        if (mp.type != YB_MAXPOOL || mp.size != 2 || mp.stride != 2 || mp.pad != 1 || !is_conv(i + 2)) return SIDE_NONE;
+        if (!sole_reader(i, i + 1) || !sole_reader(i + 1, i + 2)) return SIDE_NONE;
+        return side_int(L[i + 2].side) ? L[i + 2].side : SIDE_NONE;
     }
 
     // layer i's NHWC output view; buf(j) is the start of layer j's own buffer
@@ -299,17 +293,19 @@ struct Builder {
         const Layer &l = layer(i);
         const int ld = L[i].side_ld;
         if (L[i].side == SIDE_PM1_F32) return make_tv(base, B, l.h, l.w, l.c, ld, P, DT_F32, 0);
-        if (L[i].side == SIDE_S8) return make_tv(base, B, l.h, l.w, l.c, ld, P, DT_S8, 0);
-        return make_tv(base, B, l.h, l.w, ld, ld, P, DT_BITS, 0);
+        if (L[i].side == SIDE_BITS) return make_tv(base, B, l.h, l.w, ld, ld, P, DT_BITS, 0);
+        return make_tv(base, B, l.h, l.w, l.c, ld, P, DT_S8, 0);
     }
     TV side_placed(int i) const { return side_view(i, e.act_arena.get() + side_off[i]); }
+    // the multiplier of layer i's side conversion: the input multiplier of an INT8 layer, unused otherwise
+    float side_mult(int i) const { return L[i].side == SIDE_S8 ? layer(i).input_quant_multipler : 0.f; }
     static float alpha1(const Layer &l) { return 32 / (l.input_quant_multipler * l.weights_quant_multipler); }   // ALPHA1, ..._quantized.c:598
 
     // Convolution i as a tensor-core convolution (the kind follows the variant and the activation type), with the shortcut and
-    // [yolo] fusions of its plan and the max-pool fusion `pool_mode`.  placed == false: views rooted at kLayoutBase and no
-    // device pointers, for the queries of the layer plan; true: the placed buffers, the packed weights and the raw-count
-    // buffer (keep_counts) that counts_buffer made.
-    TcConv tc_conv(int i, bool placed, int pool_mode) const {
+    // [yolo] fusions of its plan and the max-pool fusion `pool` (layer i+2's side format, or SIDE_NONE).  placed == false: views
+    // rooted at kLayoutBase and no device pointers, for the queries of the layer plan; true: the placed buffers, the packed
+    // weights and the raw-count buffer (keep_counts) that counts_buffer made.
+    TcConv tc_conv(int i, bool placed, SideFmt pool) const {
         const Layer &l = layer(i);
         const LayerPlan &p = L[i];
         const int tgt = p.fused_into >= 0 ? p.fused_into : i;
@@ -325,9 +321,9 @@ struct Builder {
             c.res = out(layer(tgt).index);
             c.act2 = layer(tgt).activation;
         }
-        c.pool_mode = pool_mode;
-        if (pool_mode) {
-            c.pool_mult = pool_mode == 1 ? layer(i + 2).input_quant_multipler : 0.f;
+        c.pool_fmt = pool;
+        if (pool != SIDE_NONE) {
+            c.pool_mult = side_mult(i + 2);
             c.pool_next = side(i + 2);
         }
         c.sw = sw.tc;
@@ -419,7 +415,7 @@ struct Builder {
             const Layer &l = layer(i);
             LayerPlan &p = L[i];
             if (p.variant == 1 && xnor_fallback(l)) { p.side = SIDE_PM1_F32; p.side_ld = l.c; }
-            else if (p.variant == 1 && xnor_on_tc(l)) { p.side = SIDE_S8; p.side_ld = (int)align_up(l.c, 32); }   // pad channels meet zero weights
+            else if (p.variant == 1 && xnor_on_tc(l)) { p.side = SIDE_PM1_S8; p.side_ld = (int)align_up(l.c, 32); }   // pad channels meet zero weights
             else if (p.variant == 1) { p.side = SIDE_BITS; p.side_ld = (l.c + 31) / 32; }
             else if (p.variant == 2) { p.side = SIDE_S8; p.side_ld = (int)align_up(l.c, 32); }   // every INT8 layer fits the s8 wgmma tile
         }
@@ -477,7 +473,7 @@ struct Builder {
         const int tgt = p.fused_into >= 0 ? p.fused_into : i;
         const TV tin = layout_in(i), tout = layout_view(tgt);
         const int idt = in_dt(i), odt = L[tgt].out_dt;
-        const TcConv tc_query = tc_conv(i, false, 0);
+        const TcConv tc_query = tc_conv(i, false, SIDE_NONE);
         if (p.variant == 0) {
             int tc = (ADT == DT_BF16 && idt == DT_BF16) ? tc_conv_supported(tc_query) : 0;
             // float detection heads of the INT8 / XNOR networks (default precision): tf32 wgmma.  Only layers whose every
@@ -553,15 +549,15 @@ struct Builder {
             LayerPlan &p = L[i];
             if (!is_conv(i) || p.in_first_op) continue;
             // max-pool i+1 and layer i+2's input conversion in the epilogue
-            const int pm = conv_pool_mode(i);
+            const SideFmt pf = conv_pool_fmt(i);
             bool pool = false;
             if (p.path == CP_XNOR_TC || p.path == CP_I8_TC) {
-                pool = pm != 0 && tc_conv_supported(tc_conv(i, false, pm));
+                pool = pf != SIDE_NONE && tc_conv_supported(tc_conv(i, false, pf));
             } else if (p.path == CP_XNOR_SMALLK) {
-                pool = pm == 2 || pm == 3;
+                pool = pf == SIDE_PM1_S8 || pf == SIDE_BITS;
             }
             if (pool) {
-                p.pool_mode = pm;
+                p.pool = pf;
                 L[i + 1].pool_in_conv = L[i + 2].prefilled = true;
                 p.materialised = L[i + 1].materialised = false;
             }
@@ -597,13 +593,13 @@ struct Builder {
         }
         for (int i = 0; i < nl; ++i) {
             const Layer &l = layer(i);
-            const int sdt = L[i].side == SIDE_PM1_F32 ? DT_F32 : L[i].side == SIDE_S8 ? DT_S8 : DT_BITS;
+            const int sdt = L[i].side == SIDE_PM1_F32 ? DT_F32 : L[i].side == SIDE_BITS ? DT_BITS : DT_S8;
             if (L[i].side != SIDE_NONE) side_off[i] = take(tv_bytes(B, l.h, l.w, L[i].side_ld, P, sdt));
         }
         e.act_arena.ensure(total);
         CUDA_OK(cudaMemsetAsync(e.act_arena.get(), 0, total, e.stream));   // zero borders, once
         for (int i = 0; i < nl; ++i)   // +-1 activation buffers: borders are -1 (out-of-image taps count as -1, SURVEY F9)
-            if (L[i].variant == 1 && L[i].side == SIDE_S8)
+            if (L[i].side == SIDE_PM1_S8)
                 CUDA_OK(cudaMemsetAsync(e.act_arena.get() + side_off[i], 0xFF, tv_bytes(B, layer(i).h, layer(i).w, L[i].side_ld, P, DT_S8), e.stream));
         e.in0 = first == FIRST_NHWC ? in0_view(e.act_arena.get() + in0_off) : TV{};
         e.in0_dt = ADT;
@@ -718,7 +714,7 @@ struct Builder {
 
     // the tensor-core plan of layer i, with the [yolo] layer or the max-pool the layer plan fuses
     void push_tc_plan(int kind, int i) {
-        e.tc_plans.emplace_back(i, tc_make_plan(tc_conv(i, true, L[i].pool_mode)));
+        e.tc_plans.emplace_back(i, tc_make_plan(tc_conv(i, true, L[i].pool)));
         const TcPlan *plan = e.tc_plans.back().second.get();
         if (kind == OP_CONV_TC || kind == OP_CONV_TC_TF32) ++e.n_tc;
         push(kind, i, [plan](const float *, cudaStream_t s) { tc_launch(*plan, s); });
@@ -736,14 +732,15 @@ struct Builder {
         const Layer &l0 = layer(0);
         const int act = l0.activation, H = l0.h, W = l0.w;
         if (first == FIRST_STEM_POOL) {
-            // by what layer 2 reads (s8, +-1 bytes, sign bits) and the stem's activation
-            decltype(&k_stem_pool<0, ACT_LEAKY>) const k[3][2] = {{k_stem_pool<0, ACT_LEAKY>, k_stem_pool<0, ACT_LINEAR>},
-                                                                  {k_stem_pool<1, ACT_LEAKY>, k_stem_pool<1, ACT_LINEAR>},
-                                                                  {k_stem_pool<2, ACT_LEAKY>, k_stem_pool<2, ACT_LINEAR>}};
+            // by layer 2's side format (SIDE_S8, SIDE_PM1_S8, SIDE_BITS) and the stem's activation
+            decltype(&k_stem_pool<SIDE_S8, ACT_LEAKY>) const k[3][2] = {
+                {k_stem_pool<SIDE_S8, ACT_LEAKY>, k_stem_pool<SIDE_S8, ACT_LINEAR>},
+                {k_stem_pool<SIDE_PM1_S8, ACT_LEAKY>, k_stem_pool<SIDE_PM1_S8, ACT_LINEAR>},
+                {k_stem_pool<SIDE_BITS, ACT_LEAKY>, k_stem_pool<SIDE_BITS, ACT_LINEAR>}};
             const Layer &c2 = layer(2);
-            const int mode = L[2].variant == 2 ? 0 : L[2].side == SIDE_S8 ? 1 : 2;
-            push_input_kernel(OP_CONV_SIMT, 0, k[mode][act == ACT_LEAKY ? 0 : 1], (unsigned)(((long)B * c2.h * c2.w + 127) / 128), 128,
-                              side_placed(2), stem_weights<16>(l0), act, H, W, mode == 0 ? c2.input_quant_multipler : 0.f);
+            push_input_kernel(OP_CONV_SIMT, 0, k[L[2].side - SIDE_S8][act == ACT_LEAKY ? 0 : 1],
+                              (unsigned)(((long)B * c2.h * c2.w + 127) / 128), 128, side_placed(2), stem_weights<16>(l0), act, H, W,
+                              side_mult(2));
         } else if (first == FIRST_STEM_TC || first == FIRST_STEM_S2) {
             const bool s2 = first == FIRST_STEM_S2;
             e.stem_plan = s2 ? tc_stem_s2_make_plan(l0, layer(1), e.out_tv[1], e.w_arena.get() + stem_w_off, bias(0),
@@ -767,11 +764,24 @@ struct Builder {
         }
     }
 
+    // k_int_input: convolution j's converted input from tin, behind a size x size / stride max-pool (1 / 1 / 0: the conversion
+    // alone)
+    void push_int_input(int kind, int i, int j, const TV &tin, int size, int stride, int pad) {
+        const SideFmt f = L[j].side;   // SIDE_S8, SIDE_PM1_S8 or SIDE_BITS
+        void (*const k[3])(TV, TV, int, int, int, float) = {k_int_input<SIDE_S8>, k_int_input<SIDE_PM1_S8>, k_int_input<SIDE_BITS>};
+        const TV q = side_placed(j);
+        push_kernel(kind, i, k[f - SIDE_S8], grid_for((long)B * q.H * q.W * int_input_groups(f, tin.C)), 256, 0, tin, q, size, stride, pad,
+                    side_mult(j));
+    }
+
     void emit_conv(int i) {
         const TV tin = i == 0 ? e.in0 : e.out_tv[i - 1];   // no base where the input is fused away
+        const SideFmt f = L[i].side;
+        if (!L[i].prefilled && side_int(f))
+            push_int_input(f == SIDE_S8 ? OP_QUANTIZE : OP_BINARIZE, i, i, tin, 1, 1, 0);
         if (L[i].variant == 0) emit_conv_fp32(i, tin);
         else if (L[i].variant == 1) emit_conv_xnor(i, tin);
-        else emit_conv_int8(i, tin);
+        else emit_conv_int8(i);
     }
 
     // k_conv_simt: the f32 [K][ldw] weights of convolution i
@@ -823,20 +833,12 @@ struct Builder {
         }
         int32_t *cnt_dbg = counts_buffer(i);
         if (p.path == CP_XNOR_TC) {
-            if (!p.prefilled)
-                push_kernel(OP_BINARIZE, i, k_binarize_s8, grid_for((long)B * l.h * l.w * (l.c / 16)), 256, 0, tin, side_placed(i));
             push_tc_plan(OP_CONV_TC_I8, i);
             return;
         }
         const int CW = p.side_ld;
-        const TV bits = make_tv(e.act_arena.get() + side_off[i], B, l.h, l.w, CW, CW, P, DT_BITS, 0);
-        if (!p.prefilled) {   // a word of sign bits per thread, or per warp
-            const bool vec = vec4_view(tin);
-            push_kernel(OP_BINARIZE, i, vec ? k_binarize_vec<float> : k_binarize<float>,
-                        grid_for((long)B * l.h * l.w * CW * (vec ? 1 : 32)), 256, 0, tin, bits);
-        }
         XnorP xp{};
-        xp.bits = bits; xp.out = tout;
+        xp.bits = side_placed(i); xp.out = tout;
         xp.w = reinterpret_cast<const uint32_t *>(e.w_arena.get() + cw[i].w_bits);
         xp.mean = reinterpret_cast<const float *>(e.w_arena.get() + cw[i].mean);
         xp.bias = bias(i);
@@ -848,28 +850,26 @@ struct Builder {
             return;
         }
         const size_t smem = (size_t)l.n * 9 * CW * 4;
-        if (const int pm = p.pool_mode) {
+        if (p.pool != SIDE_NONE) {
             // the 2x2 max-pool behind this layer and the next XNOR layer's sign extraction run in this kernel, which reads only
-            // the shape of the output it does not write.  By sign words per tap and what the next layer reads (+-1 bytes, bits).
-            void (*const k[2][2])(XnorP, TV) = {{k_conv_xnor_smallk_pool<1, 2>, k_conv_xnor_smallk_pool<1, 3>},
-                                                {k_conv_xnor_smallk_pool<2, 2>, k_conv_xnor_smallk_pool<2, 3>}};
+            // the shape of the output it does not write.  By sign words per tap and the next layer's side format (SIDE_PM1_S8,
+            // SIDE_BITS).
+            void (*const k[2][2])(XnorP, TV) = {{k_conv_xnor_smallk_pool<1, SIDE_PM1_S8>, k_conv_xnor_smallk_pool<1, SIDE_BITS>},
+                                                {k_conv_xnor_smallk_pool<2, SIDE_PM1_S8>, k_conv_xnor_smallk_pool<2, SIDE_BITS>}};
             xp.out = make_tv(nullptr, B, l.out_h, l.out_w, l.n, L[i].ldc, P, DT_F32, 0);
             const Layer &c2 = layer(i + 2);
-            push_kernel(OP_CONV_XNOR, i, k[CW - 1][pm - 2], (unsigned)(((long)B * c2.h * c2.w + 127) / 128), 128, smem, xp,
+            push_kernel(OP_CONV_XNOR, i, k[CW - 1][p.pool - SIDE_PM1_S8], (unsigned)(((long)B * c2.h * c2.w + 127) / 128), 128, smem, xp,
                         side_placed(i + 2));
             return;
         }
         push_kernel(OP_CONV_XNOR, i, CW == 1 ? k_conv_xnor_smallk<1> : k_conv_xnor_smallk<2>, (unsigned)((M + 127) / 128), 128, smem, xp);
     }
 
-    void emit_conv_int8(int i, const TV &tin) {
+    void emit_conv_int8(int i) {
         const Layer &l = layer(i);
         const LayerPlan &p = L[i];
         const TV tout = e.out_tv[i];   // no base where the max-pool behind it is fused
         const TV q = side_placed(i);
-        if (!p.prefilled)
-            push_kernel(OP_QUANTIZE, i, k_quantize<float>, grid_for((long)B * l.h * l.w * (p.side_ld / 4)), 256, 0, tin, q,
-                        l.input_quant_multipler);
         int *acc_dbg = counts_buffer(i);
         if (p.path == CP_I8_TC) {
             push_tc_plan(OP_CONV_TC_I8, i);
@@ -898,13 +898,7 @@ struct Builder {
         case YB_MAXPOOL: {
             if (p.pool_in_conv) break;    // done in the epilogue of the integer convolution in front of it
             if (p.pool_to_side) {
-                // by what layer i+1 reads: s8 quantised (with its multiplier), +-1 bytes, or sign bits
-                void (*const k[3])(TV, TV, int, int, int, float) = {k_maxpool_fused<0>, k_maxpool_fused<1>, k_maxpool_fused<2>};
-                const Layer &c = layer(i + 1);
-                const TV q = side_placed(i + 1);
-                const int mode = L[i + 1].side == SIDE_BITS ? 2 : L[i + 1].variant == 2 ? 0 : 1;
-                push_kernel(OP_MAXPOOL, i, k[mode], grid_for((long)B * c.h * c.w * (mode == 2 ? q.ldc : q.ldc / 4)), 256, 0, tin, q,
-                            l.size, l.stride, l.pad, mode == 0 ? c.input_quant_multipler : 0.f);
+                push_int_input(OP_MAXPOOL, i, i + 1, tin, l.size, l.stride, l.pad);
                 break;
             }
             const int esz = (int)dt_size(dt);
