@@ -10,11 +10,13 @@ ap = argparse.ArgumentParser()
 ap.add_argument("--model", default="yolov3"); ap.add_argument("--size", type=int, default=608)
 ap.add_argument("--batch", type=int, default=16); ap.add_argument("--quantized", type=int, default=0)
 ap.add_argument("--reps", type=int, default=1); ap.add_argument("--list", action="store_true")
+ap.add_argument("--precision", choices=["bf16", "fp32"], default="bf16", help="fp32: YB_PREC_FP32, the exact f32 path")
 a = ap.parse_args()
 wd = tempfile.mkdtemp()
 secs = cfgs.MODELS[a.model](a.size, a.size)
 cfg = cfgs.write_cfg(secs, os.path.join(wd, "m.cfg")); wts = cfgs.write_weights(secs, os.path.join(wd, "m.weights"), seed=1)
 net = yb.load_network(cfg, wts, batch=a.batch, quantized=a.quantized)
+net.set_precision(yb.YB_PREC_FP32 if a.precision == "fp32" else yb.YB_PREC_BF16_TC)
 x = cfgs.synthetic_images(a.batch, 3, a.size, a.size)
 if a.list:
     net.predict(x, quantized=bool(a.quantized))

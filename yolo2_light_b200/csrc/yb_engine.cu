@@ -784,17 +784,36 @@ struct Builder {
         else emit_conv_int8(i);
     }
 
-    // k_conv_simt: the f32 [K][ldw] weights of convolution i
-    void push_conv_simt(int i, void (*k)(ConvP), const TV &tin, const TV &tout, const TV &res, int act2) {
+    // k_conv_simt<V>: convolution i as the CUDA-core implicit GEMM, over the f32 [K][ldw] weights or, for an XNOR or INT8 layer
+    // reading sign bits or s8 values, over the 32-bit words of its side input and weights
+    void push_conv_simt(int kind, int i, void (*k)(SimtP), const TV &tin, const TV &tout, const TV &res = TV{}, int act2 = ACT_LINEAR) {
         const Layer &l = layer(i);
+        const LayerPlan &p = L[i];
+        const int taps = l.size * l.size;
         const long M = (long)B * l.out_h * l.out_w;
-        ConvP cp{};
-        cp.in = tin; cp.out = tout; cp.res = res;
-        cp.w = e.w_arena.get() + cw[i].w_f32;
-        cp.bias = bias(i);
-        cp.n = l.n; cp.ldw = cw[i].ldw; cp.size = l.size; cp.stride = l.stride; cp.pad = l.pad;
-        cp.act = l.activation; cp.act2 = act2; cp.K = l.size * l.size * l.c; cp.M = M;
-        push_kernel(OP_CONV_SIMT, i, k, dim3((unsigned)((M + 63) / 64), (unsigned)((l.n + 63) / 64)), 256, 0, cp);
+        SimtP sp{};
+        sp.in = tin; sp.out = tout; sp.res = res;
+        sp.bias = bias(i);
+        sp.n = l.n; sp.size = l.size; sp.stride = l.stride; sp.pad = l.pad;
+        sp.act = l.activation; sp.act2 = act2; sp.M = M;
+        if (p.side == SIDE_BITS) {
+            sp.CW = p.side_ld;
+            sp.w = e.w_arena.get() + cw[i].w_bits;
+            sp.mean = reinterpret_cast<const float *>(e.w_arena.get() + cw[i].mean);
+            sp.bits = taps * l.c; sp.padbits = (sp.CW * 32 - l.c) * taps;
+        } else if (p.side == SIDE_S8) {
+            sp.CW = p.side_ld / 4;
+            sp.w = e.w_arena.get() + cw[i].w_s8;
+            sp.alpha1 = alpha1(l);
+        }
+        if (sp.CW) {
+            sp.K = taps * sp.CW;
+            sp.counts = counts_buffer(i);
+        } else {
+            sp.w = e.w_arena.get() + cw[i].w_f32;
+            sp.ldw = cw[i].ldw; sp.K = taps * l.c;
+        }
+        push_kernel(kind, i, k, dim3((unsigned)((M + 63) / 64), (unsigned)((l.n + 63) / 64)), 256, 0, sp);
     }
 
     void emit_conv_fp32(int i, const TV &tin) {
@@ -812,12 +831,12 @@ struct Builder {
             act2 = s.activation;
         }
         // by input, output and residual dtype; all f32 is the reference's summation order, bit-exact
-        void (*const k[2][2][2])(ConvP) = {
-            {{k_conv_simt<float, float, float, true>, k_conv_simt<float, float, __nv_bfloat16>},
-             {k_conv_simt<float, __nv_bfloat16, float>, k_conv_simt<float, __nv_bfloat16, __nv_bfloat16>}},
-            {{k_conv_simt<__nv_bfloat16, float, float>, k_conv_simt<__nv_bfloat16, float, __nv_bfloat16>},
-             {k_conv_simt<__nv_bfloat16, __nv_bfloat16, float>, k_conv_simt<__nv_bfloat16, __nv_bfloat16, __nv_bfloat16>}}};
-        push_conv_simt(i, k[in_dt(i)][L[tgt].out_dt][rdt], tin, e.out_tv[tgt], res, act2);
+        void (*const k[2][2][2])(SimtP) = {
+            {{k_conv_simt<SimtF32<float, float, float, true>>, k_conv_simt<SimtF32<float, float, __nv_bfloat16>>},
+             {k_conv_simt<SimtF32<float, __nv_bfloat16, float>>, k_conv_simt<SimtF32<float, __nv_bfloat16, __nv_bfloat16>>}},
+            {{k_conv_simt<SimtF32<__nv_bfloat16, float, float>>, k_conv_simt<SimtF32<__nv_bfloat16, float, __nv_bfloat16>>},
+             {k_conv_simt<SimtF32<__nv_bfloat16, __nv_bfloat16, float>>, k_conv_simt<SimtF32<__nv_bfloat16, __nv_bfloat16, __nv_bfloat16>>}}};
+        push_conv_simt(OP_CONV_SIMT, i, k[in_dt(i)][L[tgt].out_dt][rdt], tin, e.out_tv[tgt], res, act2);
     }
 
     void emit_conv_xnor(int i, const TV &tin) {
@@ -828,12 +847,16 @@ struct Builder {
         if (p.path == CP_XNOR_FALLBACK) {
             const TV pm1 = side_placed(i);
             push_kernel(OP_BINARIZE, i, k_binarize_pm1, grid_for((long)B * l.h * l.w * l.c), 256, 0, tin, pm1);
-            push_conv_simt(i, k_conv_simt<float, float, float, true>, pm1, tout, TV{}, ACT_LINEAR);
+            push_conv_simt(OP_CONV_SIMT, i, k_conv_simt<SimtF32<float, float, float, true>>, pm1, tout);
             return;
         }
         int32_t *cnt_dbg = counts_buffer(i);
         if (p.path == CP_XNOR_TC) {
             push_tc_plan(OP_CONV_TC_I8, i);
+            return;
+        }
+        if (p.path == CP_XNOR_GENERAL) {
+            push_conv_simt(OP_CONV_XNOR, i, k_conv_simt<SimtXnor>, side_placed(i), tout);
             return;
         }
         const int CW = p.side_ld;
@@ -842,13 +865,9 @@ struct Builder {
         xp.w = reinterpret_cast<const uint32_t *>(e.w_arena.get() + cw[i].w_bits);
         xp.mean = reinterpret_cast<const float *>(e.w_arena.get() + cw[i].mean);
         xp.bias = bias(i);
-        xp.n = l.n; xp.size = l.size; xp.pad = l.pad; xp.K = l.size * l.size * l.c;
+        xp.n = l.n; xp.K = l.size * l.size * l.c;
         xp.padbits = (CW * 32 - l.c) * l.size * l.size;
         xp.act = l.activation; xp.M = M; xp.counts = cnt_dbg;
-        if (p.path == CP_XNOR_GENERAL) {
-            push_kernel(OP_CONV_XNOR, i, k_conv_xnor, dim3((unsigned)((M + 63) / 64), (unsigned)((l.n + 63) / 64)), 256, 0, xp);
-            return;
-        }
         const size_t smem = (size_t)l.n * 9 * CW * 4;
         if (p.pool != SIDE_NONE) {
             // the 2x2 max-pool behind this layer and the next XNOR layer's sign extraction run in this kernel, which reads only
@@ -866,24 +885,9 @@ struct Builder {
     }
 
     void emit_conv_int8(int i) {
-        const Layer &l = layer(i);
-        const LayerPlan &p = L[i];
-        const TV tout = e.out_tv[i];   // no base where the max-pool behind it is fused
-        const TV q = side_placed(i);
-        int *acc_dbg = counts_buffer(i);
-        if (p.path == CP_I8_TC) {
-            push_tc_plan(OP_CONV_TC_I8, i);
-            return;
-        }
-        const long M = (long)B * l.out_h * l.out_w;
-        Int8P ip{};
-        ip.q = q; ip.out = tout;
-        ip.w = reinterpret_cast<const uint32_t *>(e.w_arena.get() + cw[i].w_s8);
-        ip.bias = bias(i);
-        ip.alpha1 = alpha1(l);
-        ip.n = l.n; ip.size = l.size; ip.stride = l.stride; ip.pad = l.pad; ip.act = l.activation;
-        ip.CW = p.side_ld / 4; ip.M = M; ip.acc_out = acc_dbg;
-        push_kernel(OP_CONV_INT8, i, k_conv_int8_simt, dim3((unsigned)((M + 63) / 64), (unsigned)((l.n + 63) / 64)), 256, 0, ip);
+        counts_buffer(i);   // allocated before the tensor-core plan, which takes its address
+        if (L[i].path == CP_I8_TC) push_tc_plan(OP_CONV_TC_I8, i);
+        else push_conv_simt(OP_CONV_INT8, i, k_conv_simt<SimtInt8>, side_placed(i), e.out_tv[i]);
     }
 
     // max-pool, upsample, shortcut, route, reorg, yolo, region

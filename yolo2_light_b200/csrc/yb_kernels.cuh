@@ -1,5 +1,5 @@
 // yb_kernels.cuh -- CUDA-core (SIMT) kernels of the engine: layout converters, the generic FP32 / XNOR / INT8
-// convolutions and all small layers.  sm_90a only.  The tensor-core (wgmma) convolutions live in
+// convolution and all small layers.  sm_90a only.  The tensor-core (wgmma) convolutions live in
 // yb_conv_tc.cuh.
 //
 // Device activation layout ("padded NHWC"): element (n, y, x, c) of a tensor with logical dims N,H,W,C lives at
@@ -269,86 +269,173 @@ static __global__ void __launch_bounds__(RS_THREADS) k_resize_frames(const Image
 }
 
 // ------------------------------------------------------------------------------------------------------
-// generic FP32 convolution on CUDA cores (implicit GEMM, 64 pixels x 64 filters per CTA, 4x4 per thread).
-// Semantics: forward_convolutional_layer_cpu FP32 branch (reference yolov2_forward_network.c:204-261):
-// out = act(sum_{c,ky,kx} w*in + bias) with zero padding; optional fused shortcut (reference :443-449):
-// out = act2(act(..) + residual).  Used for: validation precision (YB_PREC_FP32), the FP32 layers of
-// XNOR / INT8 networks, the 3-channel stem, and any shape the tensor-core kernel does not take.
-// Weights: [K][ldw] f32, K ordered (ky, kx, c), ldw = filters rounded up to 64.
+// The convolutions on CUDA cores: one implicit GEMM, 64 pixels x 64 filters per CTA, 256 threads, a 4x4 accumulator tile per
+// thread, K streamed through shared memory.  Taps outside the image read a zero element.  A policy V gives the K element, its
+// loaders, the multiply-accumulate and the epilogue:
+//   SimtF32<TIn, TOut, TRes, EXACT>  f32 values: forward_convolutional_layer_cpu FP32 branch (reference
+//       yolov2_forward_network.c:204-261), out = act(sum_{c,ky,kx} w*in + bias) with zero padding; optional fused shortcut
+//       (reference :443-449), out = act2(act(..) + residual).  Validation precision (YB_PREC_FP32), the FP32 layers of XNOR /
+//       INT8 networks, the bf16 layers the tensor cores refuse, and the XNOR layers of the float-GEMM fallback.
+//   SimtXnor  words of 32 sign bits (reference yolov2_forward_network.c:116-203): count = sum popc(~(a ^ w)) - (pad bits),
+//       out = xnor_epilogue(2*count - K, mean[f], bias[f]).  XNOR layers off the s8 wgmma with more than 2 words per tap.
+//   SimtInt8  words of 4 s8 values (reference yolov2_forward_network_quantized.c:527-631): acc32 = sum xq*wq (dp4a, exact),
+//       out = int8_epilogue(acc32).  INT8 layers the s8 wgmma tile refuses.
+// The integer inputs are written by k_int_input or by the fused kernels in front of the convolution.
 // ------------------------------------------------------------------------------------------------------
-struct ConvP {
-    TV in, out, res;           // res.base == nullptr: no residual
-    const void *w;
+struct SimtP {
+    TV in, out, res;           // in: f32 / bf16 activations or the integer side input; res.base == nullptr: no residual
+    const void *w;             // f32: [K][ldw], ldw = filters rounded up to 64; integer: [filters rounded up to 64][K] words
     const float *bias;
+    const float *mean;         // XNOR
+    float alpha1;              // INT8
     int n;                     // filters
     int ldw;
     int size, stride, pad;
     int act, act2;
-    int K;                     // size*size*C
+    int K;                     // GEMM depth: size*size*C f32 values, or size*size*CW words ordered (ky, kx, word)
+    int CW;                    // integer: words per input pixel
+    int bits, padbits;         // XNOR: true bit count size*size*C, and (CW*32 - C) * size*size
     long M;                    // N*out_h*out_w
+    int32_t *counts;           // integer: optional raw popcounts / s32 accumulators, NCHW (tests)
 };
+
+// the image and window origin of an A-loader's output pixel; valid = false past the last pixel
+struct SimtRow {
+    bool valid;
+    int n, iy0, ix0;
+};
+
+// (iy, ix): the input pixel of row r under tap t; false where it falls outside the image
+__device__ __forceinline__ bool simt_tap(const SimtP &p, const SimtRow &r, int tap, int &iy, int &ix) {
+    const int ky = tap / p.size, kx = tap - ky * p.size;
+    iy = r.iy0 + ky;
+    ix = r.ix0 + kx;
+    return iy >= 0 && iy < p.in.H && ix >= 0 && ix < p.in.W;
+}
 
 // EXACT = true (f32 activations: the exact nets and YB_PREC_FP32): K runs in the reference's own order (c, ky, kx) --
 // weights [K][ldw] stored in that order -- and every product and sum is rounded separately (__fmul_rn / __fadd_rn), i.e.
 // gemm_nn's `C[j] += A_PART * B[k][j]` of the scalar build (additionally.c:1272-1286): the result is bit-identical to the
-// reference, so a last-bit difference can never flip `x > 0` / `(int16)(x * m)` in a following integer layer.
-template <typename TIn, typename TOut, typename TRes, bool EXACT = false>
-__global__ void __launch_bounds__(256) k_conv_simt(ConvP p) {
-    constexpr int BM = 64, BN = 64, BK = 16;
-    __shared__ float As[BK][BM + 4];
-    __shared__ float Bs[BK][BN + 4];
-    const int tid = threadIdx.x;
-    const long m0 = (long)blockIdx.x * BM;
-    const int n0 = blockIdx.y * BN;
-    const int OH = p.out.H, OW = p.out.W, C = p.in.C;
-
-    // A-load role: thread -> (pixel tid/4, 4 consecutive k starting at (tid%4)*4)
-    const int lp = tid >> 2, lk = (tid & 3) * 4;
-    const long lm = m0 + lp;
-    const bool lvalid = lm < p.M;
-    int ln = 0, liy0 = 0, lix0 = 0;
-    if (lvalid) {
-        const int ox = (int)(lm % OW);
-        const int oy = (int)((lm / OW) % OH);
-        ln = (int)(lm / ((long)OW * OH));
-        liy0 = oy * p.stride - p.pad;
-        lix0 = ox * p.stride - p.pad;
-    }
-    // B-load role: thread -> (k row tid/16, 4 consecutive filters (tid%16)*4)
-    const int bk = tid >> 4, bn = (tid & 15) * 4;
-    const float *wptr = reinterpret_cast<const float *>(p.w);
-
-    const int tx = tid & 15, ty = tid >> 4;   // compute role: pixels ty*4.., filters tx*4..
-    float acc[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-
-    for (int k0 = 0; k0 < p.K; k0 += BK) {
+// reference, so a last-bit difference can never flip `x > 0` / `(int16)(x * m)` in a following integer layer.  Otherwise K
+// is ordered (ky, kx, c) and summed with fmaf.
+template <typename TIn, typename TOut_, typename TRes_, bool EXACT = false>
+struct SimtF32 {
+    using E = float;
+    using Acc = float;
+    using TOut = TOut_;
+    using TRes = TRes_;
+    static constexpr int BK = 16, SKEW = 4;
+    static constexpr bool RAW = false;
+    // A: pixel tid/4, 4 consecutive k from (tid%4)*4; B: k row tid/16, 4 consecutive filters (tid%16)*4 in one float4
+    static __device__ __forceinline__ void load(const SimtP &p, const SimtRow &r, E (*As)[64 + SKEW], E (*Bs)[64 + SKEW], int k0,
+                                                int n0) {
+        const int tid = threadIdx.x, lp = tid >> 2, lk = (tid & 3) * 4;
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
             const int k = k0 + lk + q;
             float v = 0.f;
-            if (lvalid && k < p.K) {
-                const int taps = p.size * p.size;
+            if (r.valid && k < p.K) {
+                const int taps = p.size * p.size, C = p.in.C;
                 const int tap = EXACT ? k % taps : k / C, ch = EXACT ? k / taps : k - tap * C;
-                const int ky = tap / p.size, kx = tap - ky * p.size;
-                const int iy = liy0 + ky, ix = lix0 + kx;
-                if (iy >= 0 && iy < p.in.H && ix >= 0 && ix < p.in.W) v = to_f32(tv_px<TIn>(p.in, ln, iy, ix)[ch]);
+                int iy, ix;
+                if (simt_tap(p, r, tap, iy, ix)) v = to_f32(tv_px<TIn>(p.in, r.n, iy, ix)[ch]);
             }
             As[lk + q][lp] = v;
         }
-        {
-            const int k = k0 + bk;
-            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (k < p.K) v = *reinterpret_cast<const float4 *>(wptr + (size_t)k * p.ldw + n0 + bn);
-            Bs[bk][bn + 0] = v.x; Bs[bk][bn + 1] = v.y; Bs[bk][bn + 2] = v.z; Bs[bk][bn + 3] = v.w;
+        const int bk = tid >> 4, bn = (tid & 15) * 4, k = k0 + bk;
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (k < p.K) v = *reinterpret_cast<const float4 *>(reinterpret_cast<const float *>(p.w) + (size_t)k * p.ldw + n0 + bn);
+        Bs[bk][bn + 0] = v.x; Bs[bk][bn + 1] = v.y; Bs[bk][bn + 2] = v.z; Bs[bk][bn + 3] = v.w;
+    }
+    static __device__ __forceinline__ void mac(float &acc, float a, float b) {
+        if constexpr (EXACT) acc = __fadd_rn(acc, __fmul_rn(b, a));
+        else acc = fmaf(a, b, acc);
+    }
+    static __device__ __forceinline__ float finish(const SimtP &p, float acc, int f, const TRes *r) {
+        float v = act_exact(__fadd_rn(acc, p.bias[f]), p.act);
+        if (r) v = act_exact(__fadd_rn(v, to_f32(r[f])), p.act2);
+        return v;
+    }
+};
+
+// the integer policies' shared part: 64 rows x 8 words per operand, 2 words per thread -- A: pixel tid/4 of the side input
+// (element type T), B: filter n0 + tid/4 of [ldn][K]; the K tail pads A with 0 and B with KPAD, which contribute nothing
+template <typename T, uint32_t KPAD>
+struct SimtWords {
+    using E = uint32_t;
+    using Acc = int;
+    using TOut = float;
+    using TRes = float;
+    static constexpr int BK = 8, SKEW = 1;
+    static constexpr bool RAW = true;
+    static __device__ __forceinline__ void load(const SimtP &p, const SimtRow &r, E (*As)[64 + SKEW], E (*Bs)[64 + SKEW], int k0,
+                                                int n0) {
+        const int lr = threadIdx.x >> 2, lw = (threadIdx.x & 3) * 2;
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+            const int k = k0 + lw + q;
+            uint32_t a = 0, b = KPAD;
+            if (k < p.K) {
+                const int tap = k / p.CW, wd = k - tap * p.CW;
+                int iy, ix;
+                if (r.valid && simt_tap(p, r, tap, iy, ix)) a = reinterpret_cast<const uint32_t *>(tv_px<T>(p.in, r.n, iy, ix))[wd];
+                b = reinterpret_cast<const uint32_t *>(p.w)[(size_t)(n0 + lr) * p.K + k];
+            }
+            As[lw + q][lr] = a;
+            Bs[lw + q][lr] = b;
         }
+    }
+};
+
+struct SimtXnor : SimtWords<uint32_t, 0xffffffffu> {   // a ^ b all ones in the tail: xnor counts 0
+    static __device__ __forceinline__ void mac(int &acc, uint32_t a, uint32_t b) { acc += __popc(~(a ^ b)); }
+    static __device__ __forceinline__ int raw(const SimtP &p, int acc) { return acc - p.padbits; }
+    static __device__ __forceinline__ float finish(const SimtP &p, int acc, int f, const float *) {
+        return xnor_epilogue(2 * raw(p, acc) - p.bits, p.mean[f], p.bias[f], p.act);
+    }
+};
+
+struct SimtInt8 : SimtWords<int8_t, 0u> {
+    static __device__ __forceinline__ void mac(int &acc, uint32_t a, uint32_t b) { acc = __dp4a((int)a, (int)b, acc); }
+    static __device__ __forceinline__ int raw(const SimtP &, int acc) { return acc; }
+    static __device__ __forceinline__ float finish(const SimtP &p, int acc, int f, const float *) {
+        return int8_epilogue(acc, p.alpha1, p.bias[f], p.act);
+    }
+};
+
+template <typename V>
+__global__ void __launch_bounds__(256) k_conv_simt(SimtP p) {
+    constexpr int BM = 64, BN = 64;
+    using E = typename V::E;
+    __shared__ E As[V::BK][BM + V::SKEW];
+    __shared__ E Bs[V::BK][BN + V::SKEW];
+    const int tid = threadIdx.x;
+    const long m0 = (long)blockIdx.x * BM;
+    const int n0 = blockIdx.y * BN;
+    const int OH = p.out.H, OW = p.out.W;
+
+    SimtRow row{m0 + (tid >> 2) < p.M, 0, 0, 0};   // A-load role: pixel tid/4
+    if (row.valid) {
+        const long m = m0 + (tid >> 2);
+        const int ox = (int)(m % OW);
+        const int oy = (int)((m / OW) % OH);
+        row.n = (int)(m / ((long)OW * OH));
+        row.iy0 = oy * p.stride - p.pad;
+        row.ix0 = ox * p.stride - p.pad;
+    }
+    const int tx = tid & 15, ty = tid >> 4;   // compute role: pixels ty*4.., filters tx*4..
+    typename V::Acc acc[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = 0;
+
+    for (int k0 = 0; k0 < p.K; k0 += V::BK) {
+        V::load(p, row, As, Bs, k0, n0);
         __syncthreads();
 #pragma unroll
-        for (int kk = 0; kk < BK; ++kk) {
-            float a[4], b[4];
+        for (int kk = 0; kk < V::BK; ++kk) {
+            E a[4], b[4];
 #pragma unroll
             for (int i = 0; i < 4; ++i) a[i] = As[kk][ty * 4 + i];
 #pragma unroll
@@ -356,10 +443,7 @@ __global__ void __launch_bounds__(256) k_conv_simt(ConvP p) {
 #pragma unroll
             for (int i = 0; i < 4; ++i)
 #pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    if constexpr (EXACT) acc[i][j] = __fadd_rn(acc[i][j], __fmul_rn(b[j], a[i]));
-                    else acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
-                }
+                for (int j = 0; j < 4; ++j) V::mac(acc[i][j], a[i], b[j]);
         }
         __syncthreads();
     }
@@ -370,15 +454,15 @@ __global__ void __launch_bounds__(256) k_conv_simt(ConvP p) {
         const int ox = (int)(m % OW);
         const int oy = (int)((m / OW) % OH);
         const int n = (int)(m / ((long)OW * OH));
-        TOut *o = tv_px<TOut>(p.out, n, oy, ox);
-        const TRes *r = p.res.base ? tv_px<TRes>(p.res, n, oy, ox) : nullptr;
+        typename V::TOut *o = tv_px<typename V::TOut>(p.out, n, oy, ox);
+        const typename V::TRes *r = p.res.base ? tv_px<typename V::TRes>(p.res, n, oy, ox) : nullptr;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const int f = n0 + tx * 4 + j;
             if (f >= p.n) continue;
-            float v = act_exact(__fadd_rn(acc[i][j], p.bias[f]), p.act);
-            if (r) v = act_exact(__fadd_rn(v, to_f32(r[f])), p.act2);
-            o[f] = from_f32<TOut>(v);
+            if constexpr (V::RAW)
+                if (p.counts) p.counts[(((size_t)n * p.n + f) * OH + oy) * OW + ox] = V::raw(p, acc[i][j]);
+            o[f] = from_f32<typename V::TOut>(V::finish(p, acc[i][j], f, r));
         }
     }
 }
@@ -487,13 +571,13 @@ static __global__ void k_binarize_pm1(TV in, TV out) {
     }
 }
 
-struct XnorP {
+struct XnorP {                // the small-K XNOR convolutions, 3x3 / stride 1 / pad 1
     TV bits;                  // input bits, C = words per pixel (CW)
     TV out;                   // f32
     const uint32_t *w;        // [ldn filters][9 taps][CW] sign bits
     const float *mean, *bias;
-    int n, size, pad;
-    int K;                    // true bit count size*size*C
+    int n;
+    int K;                   // true bit count size*size*C
     int padbits;              // (CW*32 - C) * size*size
     int act;
     long M;
@@ -586,191 +670,6 @@ __global__ void __launch_bounds__(128) k_conv_xnor_smallk(XnorP p) {
         }
         if (f0 + 3 < p.n) *reinterpret_cast<float4 *>(o + f0) = make_float4(r[0], r[1], r[2], r[3]);
         else for (int j = 0; j < 4 && f0 + j < p.n; ++j) o[f0 + j] = r[j];
-    }
-}
-
-// XNOR bit-GEMM convolution, 3x3 / stride 1 / pad 1: count = sum_taps popc(~(a ^ w)) - (pad bits), then
-// out = xnor_epilogue(2*count - K, mean[f], bias[f]).  64 pixels x 64 filters per CTA, 4x4 per thread,
-// K streamed through shared memory in 8-word slices with 128-bit loads.
-
-static __global__ void __launch_bounds__(256) k_conv_xnor(XnorP p) {
-    constexpr int BM = 64, BN = 64, BKW = 8;
-    __shared__ uint32_t As[BKW][BM + 1];
-    __shared__ uint32_t Bs[BKW][BN + 1];
-    const int tid = threadIdx.x;
-    const long m0 = (long)blockIdx.x * BM;
-    const int n0 = blockIdx.y * BN;
-    const int H = p.out.H, W = p.out.W, CW = p.bits.C;
-    const int taps = p.size * p.size;
-    const int KW = taps * CW;
-
-    // loader roles: 64 rows x 8 words = 512 words per operand, 2 per thread
-    const int lr = tid >> 2, lw = (tid & 3) * 2;
-    const long lm = m0 + lr;
-    const bool lvalid = lm < p.M;
-    int ln = 0, ly = 0, lx = 0;
-    if (lvalid) {
-        lx = (int)(lm % W);
-        ly = (int)((lm / W) % H);
-        ln = (int)(lm / ((long)W * H));
-    }
-    const int tx = tid & 15, ty = tid >> 4;
-    int acc[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = 0;
-
-    for (int k0 = 0; k0 < KW; k0 += BKW) {
-#pragma unroll
-        for (int q = 0; q < 2; ++q) {
-            const int k = k0 + lw + q;
-            uint32_t a = 0, b = 0;
-            if (k < KW) {
-                const int tap = k / CW, wd = k - tap * CW;
-                if (lvalid) {
-                    const int ky = tap / p.size, kx = tap - ky * p.size;
-                    const int iy = ly + ky - p.pad, ix = lx + kx - p.pad;
-                    // out-of-image taps read 0-bits (== -1): border for pad<=1, explicit otherwise
-                    if (iy >= -p.bits.P && iy < H + p.bits.P && ix >= -p.bits.P && ix < W + p.bits.P)
-                        a = tv_px<uint32_t>(p.bits, ln, iy, ix)[wd];
-                }
-                const int f = n0 + lr;
-                b = p.w[(size_t)f * KW + k];
-            } else {
-                a = 0; b = 0xffffffffu;   // a ^ b = all ones -> xnor contributes 0
-            }
-            As[lw + q][lr] = a;
-            Bs[lw + q][lr] = b;
-        }
-        __syncthreads();
-#pragma unroll
-        for (int kk = 0; kk < BKW; ++kk) {
-            uint32_t a[4], b[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) a[i] = As[kk][ty * 4 + i];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) b[j] = Bs[kk][tx * 4 + j];
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-                for (int j = 0; j < 4; ++j) acc[i][j] += __popc(~(a[i] ^ b[j]));
-        }
-        __syncthreads();
-    }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const long m = m0 + ty * 4 + i;
-        if (m >= p.M) continue;
-        const int x = (int)(m % W);
-        const int y = (int)((m / W) % H);
-        const int n = (int)(m / ((long)W * H));
-        float *o = tv_px<float>(p.out, n, y, x);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int f = n0 + tx * 4 + j;
-            if (f >= p.n) continue;
-            const int count = acc[i][j] - p.padbits;
-            if (p.counts) p.counts[(((size_t)n * p.n + f) * H + y) * W + x] = count;
-            o[f] = xnor_epilogue(2 * count - p.K, p.mean[f], p.bias[f], p.act);
-        }
-    }
-}
-
-// ------------------------------------------------------------------------------------------------------
-// INT8 path (reference yolov2_forward_network_quantized.c:527-631; SURVEY Appendix A).  The s8 input (quant_i8) is written by
-// k_int_input or by the fused kernels in front of the convolution.
-// ------------------------------------------------------------------------------------------------------
-
-// INT8 convolution on CUDA cores (dp4a): acc32 = sum xq*wq (exact), then the reference's requantisation epilogue
-// (int8_epilogue).  Weights: [ldn filters][taps][ldc_in/4 words] s8, K ordered (ky, kx, c) with zero channel padding.
-struct Int8P {
-    TV q;                     // s8 input, ldc % 4 == 0
-    TV out;                   // f32
-    const uint32_t *w;
-    const float *bias;
-    float alpha1;
-    int n, size, stride, pad, act;
-    int CW;                   // words per pixel = q.ldc/4
-    long M;
-    int32_t *acc_out;         // optional raw accumulators, NCHW (tests)
-};
-
-static __global__ void __launch_bounds__(256) k_conv_int8_simt(Int8P p) {
-    constexpr int BM = 64, BN = 64, BKW = 8;
-    __shared__ uint32_t As[BKW][BM + 1];
-    __shared__ uint32_t Bs[BKW][BN + 1];
-    const int tid = threadIdx.x;
-    const long m0 = (long)blockIdx.x * BM;
-    const int n0 = blockIdx.y * BN;
-    const int OH = p.out.H, OW = p.out.W, CW = p.CW;
-    const int KW = p.size * p.size * CW;
-    const int lr = tid >> 2, lw = (tid & 3) * 2;
-    const long lm = m0 + lr;
-    const bool lvalid = lm < p.M;
-    int ln = 0, liy0 = 0, lix0 = 0;
-    if (lvalid) {
-        const int ox = (int)(lm % OW);
-        const int oy = (int)((lm / OW) % OH);
-        ln = (int)(lm / ((long)OW * OH));
-        liy0 = oy * p.stride - p.pad;
-        lix0 = ox * p.stride - p.pad;
-    }
-    const int tx = tid & 15, ty = tid >> 4;
-    int acc[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = 0;
-
-    for (int k0 = 0; k0 < KW; k0 += BKW) {
-#pragma unroll
-        for (int q = 0; q < 2; ++q) {
-            const int k = k0 + lw + q;
-            uint32_t a = 0, b = 0;
-            if (k < KW) {
-                const int tap = k / CW, wd = k - tap * CW;
-                if (lvalid) {
-                    const int ky = tap / p.size, kx = tap - ky * p.size;
-                    const int iy = liy0 + ky, ix = lix0 + kx;
-                    if (iy >= 0 && iy < p.q.H && ix >= 0 && ix < p.q.W)
-                        a = reinterpret_cast<const uint32_t *>(tv_px<int8_t>(p.q, ln, iy, ix))[wd];
-                }
-                b = p.w[(size_t)(n0 + lr) * KW + k];
-            }
-            As[lw + q][lr] = a;
-            Bs[lw + q][lr] = b;
-        }
-        __syncthreads();
-#pragma unroll
-        for (int kk = 0; kk < BKW; ++kk) {
-            uint32_t a[4], b[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) a[i] = As[kk][ty * 4 + i];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) b[j] = Bs[kk][tx * 4 + j];
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-                for (int j = 0; j < 4; ++j) acc[i][j] = __dp4a((int)a[i], (int)b[j], acc[i][j]);
-        }
-        __syncthreads();
-    }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const long m = m0 + ty * 4 + i;
-        if (m >= p.M) continue;
-        const int ox = (int)(m % OW);
-        const int oy = (int)((m / OW) % OH);
-        const int n = (int)(m / ((long)OW * OH));
-        float *o = tv_px<float>(p.out, n, oy, ox);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int f = n0 + tx * 4 + j;
-            if (f >= p.n) continue;
-            if (p.acc_out) p.acc_out[(((size_t)n * p.n + f) * OH + oy) * OW + ox] = acc[i][j];
-            o[f] = int8_epilogue(acc[i][j], p.alpha1, p.bias[f], p.act);
-        }
     }
 }
 
