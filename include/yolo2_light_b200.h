@@ -313,6 +313,10 @@ int  yb_network_tc_plan(yb_network *net, int quantized, int layer, int *fields, 
 int  yb_network_fetch_counts(yb_network *net, int i, int quantized, int32_t *dst, size_t count);
 int  yb_network_layer_outputs(const yb_network *net, int i);   /* layer.outputs (per image) */
 const char *yb_op_kind_name(int kind);
+/* The engine's ops in launch order (builds the engine if needed), read-only: up to max of {layer index, op kind code, name
+ * of the kernel the op launches (cudaFuncGetName; NULL for a tensor-core convolution, which launches through its plan)}.
+ * Returns the number of ops, -1 on error. */
+int  yb_network_op_kernels(yb_network *net, int quantized, int *layer_idx, int *op_kind, const char **name, int max);
 
 /* Pinned host buffers for the end-to-end path (cudaHostAlloc / cudaFreeHost). */
 void *yb_alloc_pinned(size_t bytes);

@@ -26,7 +26,7 @@ import ybtest_util as util
 from test_gpu_tc import bf16_round
 from yolo2_light_b200 import cfgs
 
-LINEAR, LEAKY = "linear", "leaky"
+LINEAR, LEAKY, RELU, LOGISTIC = "linear", "leaky", "relu", "logistic"
 BOUND_UNITS = 2 ** 20          # |partial sums| in product-grid units: 4 bits below f32's 24-bit significand
 F32_01 = np.float32(0.1)
 
@@ -74,6 +74,7 @@ class Net:
         self.quantized = 0
         self.fuse = 1
         self.x = None        # the input images, when a case sets them
+        self.tol = {}        # layer -> bf16 ulps its output may differ by (the double-precision logistic), else 0
 
     @property
     def n(self):
@@ -186,15 +187,24 @@ def leaky_exact(a):
     return np.where(a > 0, a, (0.1 * a.astype(np.float64)).astype(np.float32)).astype(np.float32)
 
 
-def epilogue(acc, b, act, kern, res=None, act2=LINEAR, bf16=True):
-    a = (acc + 0.0).astype(np.float32) + b.astype(np.float32)
-    act_f = leaky_exact if kern == "simt" else leaky_tc
+def activate(a, act, kern):
+    """the epilogue's activation: leaky as leaky_exact on the CUDA cores and leaky_tc on the tensor cores; relu and logistic
+    only run on the CUDA cores (act_exact): x * (x > 0), which is -0 for x < 0, and (float)(1 / (1 + exp(-(double)x))), which
+    numpy's float64 exp reproduces to within one f32 ulp"""
     if act == LEAKY:
-        a = act_f(a)
+        return leaky_exact(a) if kern == "simt" else leaky_tc(a)
+    if act == RELU:
+        return a * (a > 0)
+    if act == LOGISTIC:
+        return (1.0 / (1.0 + np.exp(-a.astype(np.float64)))).astype(np.float32)
+    assert act == LINEAR, act
+    return a
+
+
+def epilogue(acc, b, act, kern, res=None, act2=LINEAR, bf16=True):
+    a = activate((acc + 0.0).astype(np.float32) + b.astype(np.float32), act, kern)
     if res is not None:
-        a = a + res.astype(np.float32)
-        if act2 == LEAKY:
-            a = act_f(a)
+        a = activate(a + res.astype(np.float32), act2, kern)
     return bf16_round(a) if bf16 else a.astype(np.float32)
 
 
@@ -256,10 +266,11 @@ def run_reference(net, x, adt_bf16=True):
 
 
 def shifted_copies(t, pairs):
-    """the one-hot 3x3 consumer's output: filter j = t[..., c_j] shifted by tap t_j, zero border (NHWC)"""
+    """the one-hot 3x3 consumer's output: filter j = t[..., c_j] shifted by tap t_j, zero border (NHWC); + 0 as the
+    consumer's accumulator, which starts at +0 and so turns a -0 input (relu) into +0"""
     B, H, W, C = t.shape
     tp = np.zeros((B, H + 2, W + 2, C), np.float32)
-    tp[:, 1:H + 1, 1:W + 1] = t
+    tp[:, 1:H + 1, 1:W + 1] = t + np.float32(0)
     return np.stack([tp[:, tap // 3:tap // 3 + H, tap % 3:tap % 3 + W, c] for c, tap in pairs], axis=3)
 
 
@@ -396,6 +407,35 @@ def c_refused(size):
     return n
 
 
+def c_simt_shortcut():
+    """12 filters: no whole 16-byte bf16 filter groups, so the CUDA cores run the layer, with the shortcut behind it fused
+    (k_conv_simt<SimtF32<bf16, bf16, bf16>>: bf16 input, output and residual)"""
+    n = Net(12, 7, 9, 3, 1700)
+    n.preserve(kern="simt")
+    i = n.conv(12, kern="simt")
+    n.add("shortcut", **{"from": "-2", "activation": LEAKY})
+    n.consume()
+    return n
+
+
+def c_simt_act(act):
+    """relu and logistic, which the tensor cores refuse; the consumer copies the logistic's bf16 values, so it inherits
+    their one-ulp tolerance"""
+    n = Net(16, 6, 10, 2, 1800 + len(act))
+    i = n.conv(16, act=act, kern="simt")
+    j = n.consume()
+    if act == LOGISTIC:
+        n.tol = {i: 1, j: 1}
+    return n
+
+
+def c_simt_n4():
+    n = Net(16, 7, 5, 3, 1900)
+    n.conv(4, kern="simt")
+    n.consume()
+    return n
+
+
 def c_stem(nf, h, w, batch):
     n = Net(3, h, w, batch, 1400 + nf + h)
     i = n.conv(nf, kern="stem", w=(n.rng.integers(-8, 9, (nf, 3, 3, 3)) / 64).astype(np.float32))
@@ -461,6 +501,10 @@ CASES = {
     "yolo_tf32": lambda: c_yolo(1),
     "refused_c8_1x1s2": lambda: c_refused(1),
     "refused_c8_3x3": lambda: c_refused(3),
+    "simt_n12_shortcut": c_simt_shortcut,
+    "simt_relu": lambda: c_simt_act(RELU),
+    "simt_logistic": lambda: c_simt_act(LOGISTIC),
+    "simt_n4": c_simt_n4,
     "stem16": lambda: c_stem(16, 10, 14, 3),
     "stem32": lambda: c_stem(32, 7, 9, 2),
     **{f"stem_s2_{h}x{w}_b{b}": (lambda h=h, w=w, b=b: c_stem_s2(h, w, b)) for h, w, b in [(16, 16, 2), (38, 22, 3), (64, 48, 1)]},
@@ -596,8 +640,20 @@ def test_tc_exact(name, workdir, monkeypatch):
     for i, what, pred in net.edges:
         p = m.tc_plan(i, quantized=q)
         assert pred(p), (name, what, p)
-    m.predict(x, quantized=q)
+    # the CUDA-core layers: one k_conv_simt launch each, the bf16 instantiation in a bf16 network, and no launch for a
+    # shortcut fused into one
+    # (the last layer's NCHW copy, k_nhwc_to_nchw_f32, is an op of that layer too)
+    ops = [op for op in m.op_kernels(quantized=q) if op[2] is None or "k_nhwc_to_nchw_f32" not in op[2]]
     shapes = net.shapes()
+    for i, kern in net.kern.items():
+        if kern != "simt":
+            continue
+        mine = [k for j, _, k in ops if j == i]
+        assert len(mine) == 1 and "k_conv_simt" in mine[0] and "SimtF32" in mine[0], (name, i, mine)
+        assert ("__nv_bfloat16" in mine[0]) == (not q), (name, i, mine)
+        if i + 1 < len(shapes) and shapes[i + 1]["type"] == "shortcut" and net.fuse and shapes[i]["stride"] == 1:
+            assert not [k for j, _, k in ops if j == i + 1], (name, i + 1, ops)
+    m.predict(x, quantized=q)
     checked = 0
     for i, L in enumerate(shapes):
         e = exp.get(i)
@@ -618,6 +674,11 @@ def test_tc_exact(name, workdir, monkeypatch):
             continue   # k_stem_s2_tc never writes the stem output
         got = m.fetch_layer(i, quantized=q).transpose(0, 2, 3, 1)
         assert got.shape == e.shape, (name, i)
+        if net.tol.get(i):
+            d = np.abs(got.view(np.int32).astype(np.int64) - np.ascontiguousarray(e).view(np.int32).astype(np.int64)) >> 16
+            assert np.all(got >= 0) and np.all(e >= 0) and d.max() <= net.tol[i], (name, i, int(d.max()))   # logistic > 0, border 0
+            checked += 1
+            continue
         bad = np.argwhere(got.view(np.uint32) != np.ascontiguousarray(e).view(np.uint32))
         assert len(bad) == 0, (name, i, len(bad), bad[:5].tolist())
         checked += 1

@@ -22,7 +22,8 @@ def _ref_and_port(name, workdir, quantized, batch=1):
 
 @pytest.mark.parametrize("name,quantized", [("tiny64", 0), ("tiny64", 1), ("xnor64", 0), ("v3_32", 0),
                                             ("spp32", 0), ("v2voc32", 0), ("tinyvoc64", 1), ("v3_32", 1),
-                                            ("tiny_w96_h64", 0), ("tiny_w96_h64", 1), ("v3_w64_h96", 0)])
+                                            ("tiny_w96_h64", 0), ("tiny_w96_h64", 1), ("v3_w64_h96", 0),
+                                            ("edges_yolo_w40_h24", 0), ("edges_region_w26_h22", 0)])
 def test_whole_network_bit_exact(name, quantized, workdir):
     """Same cfg, same generated .weights, same image -> every layer output of the restatement equals the
     reference's l.output bit-for-bit (FP32 conv: identical k-ascending float accumulation; XNOR / INT8: exact
@@ -42,6 +43,16 @@ def test_batch_two_fp32(workdir):
     for i, o in enumerate(outs):
         r = rnet.output(i)
         assert util.bits_equal(o.reshape(r.shape), r), i
+
+
+@pytest.mark.parametrize("name", ["edges_yolo_w40_h24", "edges_region_w26_h22"])
+def test_batch_three_edge_shapes(name, workdir):
+    """The edge geometries at batch 3, where the reference's reorg of a size its stride does not divide reads each image
+    from a flat offset inside the images before it (yolov2_forward_network.c:359-366)"""
+    rnet, outs = _ref_and_port(name, workdir, 0, batch=3)
+    for i, o in enumerate(outs):
+        r = rnet.output(i)
+        assert util.bits_equal(o.reshape(r.shape), r), (name, i, rnet.layers[i]["type_name"])
 
 
 def test_quantize_input_matches_reference_cast():

@@ -133,6 +133,7 @@ def lib():
         "yb_network_last_launches": (C.c_int, [vp]),
         "yb_network_profile": (C.c_int, [vp, C.c_int, vp, ip, ip, fp, C.c_int]),
         "yb_op_kind_name": (C.c_char_p, [C.c_int]),
+        "yb_network_op_kernels": (C.c_int, [vp, C.c_int, ip, ip, C.POINTER(C.c_char_p), C.c_int]),
         "yb_get_network_boxes": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_int, C.c_int,
                                            vp, C.c_int]),
         "yb_alloc_pinned": (vp, [C.c_size_t]),
@@ -158,7 +159,7 @@ EXPORTED_SYMBOLS = [
     "yb_network_input_histogram", "yb_map_evaluate", "yb_network_predict", "yb_network_predict_quantized",
     "yb_network_predict_image_u8", "yb_network_fetch_input", "yb_network_submit", "yb_network_collect", "yb_network_layer_output", "yb_network_forward_device", "yb_network_sync_outputs", "yb_network_fetch_layer",
     "yb_network_fetch_counts", "yb_forward_convolutional_layer", "yb_network_weight_arena",
-    "yb_network_last_launches", "yb_network_profile", "yb_op_kind_name", "yb_get_network_boxes", "yb_alloc_pinned",
+    "yb_network_last_launches", "yb_network_profile", "yb_op_kind_name", "yb_network_op_kernels", "yb_get_network_boxes", "yb_alloc_pinned",
     "yb_free_pinned", "yb_network_submit_u8", "yb_network_collect_detections", "yb_network_set_devices",
     "yb_network_predict_batch", "yb_network_batch_output", "yb_network_replication", "yb_network_predict_frames_u8",
     "yb_network_detect_frames", "yb_network_submit_frames_u8", "yb_network_predict_device_frames",
@@ -563,6 +564,15 @@ class Network:
         r = lib().yb_network_profile(self._h, int(quantized), C.c_void_p(d_input_ptr), li, kk, ms, n)
         _check(r >= 0)
         return [(li[i], lib().yb_op_kind_name(kk[i]).decode(), ms[i]) for i in range(min(r, n))]
+
+    def op_kernels(self, quantized: bool = False):
+        """The engine's ops in launch order: (layer, op kind, kernel name), the name as cudaFuncGetName gives it (None for
+        an op that launches through a tensor-core plan); layer -1 is the input conversion."""
+        n = lib().yb_network_op_kernels(self._h, int(quantized), None, None, None, 0)
+        _check(n >= 0)
+        li, kk, nm = (C.c_int * max(n, 1))(), (C.c_int * max(n, 1))(), (C.c_char_p * max(n, 1))()
+        _check(lib().yb_network_op_kernels(self._h, int(quantized), li, kk, nm, n) == n)
+        return [(li[i], lib().yb_op_kind_name(kk[i]).decode(), nm[i].decode() if nm[i] else None) for i in range(n)]
 
     def get_network_boxes(self, b: int, w: int, h: int, thresh: float, nms: float = 0.0, relative: int = 1,
                           letter: int = 0, max_rows: int = 200000) -> np.ndarray:

@@ -633,6 +633,12 @@ int yb_network_profile(yb_network *n, int quantized, const void *d_input, int *l
 }
 const char *yb_op_kind_name(int k) { return op_kind_name(k); }
 
+int yb_network_op_kernels(yb_network *n, int quantized, int *layer_idx, int *op_kind, const char **name, int max) {
+    YB_TRY
+    return engine_op_kernels(get_engine(n, quantized), layer_idx, op_kind, name, max);
+    YB_CATCH(-1)
+}
+
 int yb_get_network_boxes(const yb_network *n, int b, int w, int h, float thresh, float nms, int relative,
                          int letter, float *out, int max_rows) {
     YB_TRY

@@ -36,12 +36,13 @@ static inline size_t dt_size(int dt) { return dt == DT_F32 ? 4 : dt == DT_BF16 ?
 
 // One launch of the op list.  `launch` is given the caller's NCHW images of the call, which only ops[0] reads: their pointer
 // changes per call, so ops[0] runs outside the CUDA graph.  ops[0] may also read 8-bit HWC frames of the network size instead
-// (`launch_u8`, when set).
+// (`launch_u8`, when set).  `kernel` is the kernel an op launches directly (null for the ops that launch through a plan).
 struct Op {
     int kind;
     int layer;
     std::function<void(const float *, cudaStream_t)> launch;
     std::function<void(const unsigned char *, cudaStream_t)> launch_u8;
+    const void *kernel = nullptr;
 };
 
 struct ConvWeights {   // offsets into the weight arena
@@ -454,6 +455,16 @@ struct Builder {
                 break;
             case YB_SHORTCUT:
                 if (!L[l.index].materialised) fatal_throw("engine: shortcut source not placed");
+                // shortcut_cpu's asserts (yolov2_forward_network.c:414-415): the subsampling step taken from the widths must
+                // also be the one of the heights, or the rows read from `from` run past it
+                if (l.w / l.out_w != l.h / l.out_h || l.out_w / l.w != l.out_h / l.h)
+                    fatal_throw("engine: shortcut from layer " + std::to_string(l.index) + " (" + std::to_string(l.w) + "x" +
+                                std::to_string(l.h) + ") onto " + std::to_string(l.out_w) + "x" + std::to_string(l.out_h) +
+                                ": the two scale by different factors in width and height");
+                break;
+            case YB_REGION:
+                // the reference's forward and both decoders take the objectness at entry 4 and the classes from entry 5
+                if (l.coords != 4) fatal_throw("engine: [region] coords=" + std::to_string(l.coords) + " is not supported (only 4)");
                 break;
             case YB_ROUTE:
                 if (!p.has_out) fatal_throw("engine: route over layers of different spatial size is not supported");
@@ -700,16 +711,18 @@ struct Builder {
 
     // ---- pass 4: op emission ---------------------------------------------------------------------------------------------
     const float *bias(int i) const { return reinterpret_cast<const float *>(e.w_arena.get() + cw[i].bias); }
-    void push(int kind, int i, std::function<void(const float *, cudaStream_t)> f) { e.ops.push_back(Op{kind, i, std::move(f), nullptr}); }
+    void push(int kind, int i, std::function<void(const float *, cudaStream_t)> f, const void *kernel = nullptr) {
+        e.ops.push_back(Op{kind, i, std::move(f), nullptr, kernel});
+    }
     // an op that launches kernel k with these arguments, converted to the kernel's parameter types here
     template <typename... A>
     void push_kernel(int kind, int i, void (*k)(A...), dim3 grid, dim3 block, size_t smem, typename same_type<A>::type... args) {
-        push(kind, i, [=](const float *, cudaStream_t s) { k<<<grid, block, smem, s>>>(args...); });
+        push(kind, i, [=](const float *, cudaStream_t s) { k<<<grid, block, smem, s>>>(args...); }, reinterpret_cast<const void *>(k));
     }
     // ops[0] as a kernel whose first argument is the caller's images
     template <typename... A>
     void push_input_kernel(int kind, int i, void (*k)(const float *, A...), dim3 grid, dim3 block, typename same_type<A>::type... args) {
-        push(kind, i, [=](const float *in, cudaStream_t s) { k<<<grid, block, 0, s>>>(in, args...); });
+        push(kind, i, [=](const float *in, cudaStream_t s) { k<<<grid, block, 0, s>>>(in, args...); }, reinterpret_cast<const void *>(k));
     }
 
     // the tensor-core plan of layer i, with the [yolo] layer or the max-pool the layer plan fuses
@@ -1536,6 +1549,18 @@ int engine_collect_detections(Engine *e, int ticket, const float **rows, const i
 }
 
 int engine_num_launches(Engine *e) { return (int)e->ops.size(); }
+
+int engine_op_kernels(Engine *e, int *layer, int *kind, const char **name, int max) {
+    CUDA_OK(cudaSetDevice(e->opt.device));
+    const int n = (int)e->ops.size();
+    for (int k = 0; k < n && k < max; ++k) {
+        layer[k] = e->ops[k].layer;
+        kind[k] = e->ops[k].kind;
+        name[k] = nullptr;
+        if (e->ops[k].kernel) CUDA_OK(cudaFuncGetName(&name[k], e->ops[k].kernel));
+    }
+    return n;
+}
 long engine_info(Engine *e, const char *key) {
     if (!strcmp(key, "launches")) return (long)e->ops.size();
     if (!strcmp(key, "tc_layers")) return e->n_tc;

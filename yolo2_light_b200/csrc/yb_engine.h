@@ -71,6 +71,9 @@ int engine_detect(Engine *e, Network *net, const int *w, const int *h, int nimg,
 constexpr int DET_MAX_ROWS = 16384;
 void engine_input_histogram(Engine *e, Network *net, int layer, int img, float bin_width, int max_bin, uint32_t *hist);
 int engine_num_launches(Engine *e);
+// per op, in launch order: its layer, its OpKind and the name of the kernel it launches (nullptr: launched through a plan);
+// returns the number of ops, fills the first max
+int engine_op_kernels(Engine *e, int *layer, int *kind, const char **name, int max);
 long engine_info(Engine *e, const char *key);   // "launches", "tc_layers", "act_bytes"; -1 unknown
 // the tensor-core plan of a layer (tc_plan_fields / tc_stem_plan_fields); 0 fields for a layer without one
 int engine_tc_plan(Engine *e, int layer, int *fields, int n);

@@ -961,8 +961,10 @@ __global__ void k_copy_channels(TV in, TV out /* view of the slice: C == in.C */
 }
 
 // forward_reorg_layer_cpu (reference yolov2_forward_network.c:337-373), darknet's space-to-depth flavour:
-// out[k][j][i] = x_flat[ w2 + (out_w*stride) * (h2 + (out_h*stride) * c2) ] with the input tensor reinterpreted
-// as [in_c][out_h*stride][out_w*stride] where in_c = out_c/stride^2.
+// out[n][k][j][i] = x_flat[ w2 + (out_w*stride) * (h2 + (out_h*stride) * (c2 + in_c*n)) ] with the whole batch of the input
+// reinterpreted as [N][in_c][out_h*stride][out_w*stride] where in_c = out_c/stride^2.  When stride does not divide the input's
+// height or width, that view is smaller than an image, so image n > 0 reads from a flat offset inside the images before it, as
+// the reference does; the index stays below N*in.C*in.H*in.W.
 template <typename T>
 __global__ void k_reorg(TV in, TV out, int stride) {
     const long total = (long)out.N * out.H * out.W * out.C;
@@ -975,13 +977,14 @@ __global__ void k_reorg(TV in, TV out, int stride) {
         const int n = (int)(pxl / ((long)out.W * out.H));
         const int c2 = k % in_c, offset = k / in_c;
         const int w2 = x * stride + offset % stride, h2 = y * stride + offset / stride;
-        // flat index inside one image of the source viewed as [in_c][out.H*stride][out.W*stride]
-        const long flat = w2 + (long)out.W * stride * (h2 + (long)out.H * stride * c2);
-        // map the flat NCHW index back onto the real source dims [in.C][in.H][in.W]
+        // flat index into the batch viewed as [N][in_c][out.H*stride][out.W*stride]
+        const long flat = w2 + (long)out.W * stride * (h2 + (long)out.H * stride * (c2 + (long)in_c * n));
+        // map the flat NCHW index back onto the real source dims [N][in.C][in.H][in.W]
         const int sx = (int)(flat % in.W);
         const int sy = (int)((flat / in.W) % in.H);
-        const int sc = (int)(flat / ((long)in.W * in.H));
-        tv_px<T>(out, n, y, x)[k] = tv_px<T>(in, n, sy, sx)[sc];
+        const int sc = (int)((flat / ((long)in.W * in.H)) % in.C);
+        const int sn = (int)(flat / ((long)in.W * in.H * in.C));
+        tv_px<T>(out, n, y, x)[k] = tv_px<T>(in, sn, sy, sx)[sc];
     }
 }
 
