@@ -506,20 +506,25 @@ struct Builder {
             if (!tc_conv_supported(tc_query)) fatal_throw("engine: xnor tensor-core layer not supported by the i8 tile");
             return CP_XNOR_TC;
         }
-        // small K: one thread per pixel, all filters (weights broadcast from shared memory)
+        // small K: one thread per pixel, all filters (weights broadcast from shared memory).  It stores 4 filters per float4,
+        // so every pixel of its output must be 16-byte aligned: a channel slice of a route's buffer may not be.
         const int CW = p.side_ld;
-        if (CW <= 2 && l.size == 3 && (size_t)l.n * 9 * CW * 4 <= 40 * 1024 && tout.ldc % 4 == 0) return CP_XNOR_SMALLK;
+        if (CW <= 2 && l.size == 3 && (size_t)l.n * 9 * CW * 4 <= 40 * 1024 && vec4_view(tout)) return CP_XNOR_SMALLK;
         return CP_XNOR_GENERAL;
     }
 
     // ops[0] consumes the caller's NCHW f32 images.  Usually that is the stem convolution itself (3 input channels, 3x3/1/1),
-    // reading NCHW directly; otherwise a plain NCHW -> padded-NHWC conversion.
+    // reading NCHW directly; otherwise a plain NCHW -> padded-NHWC conversion.  The stems store whole 16-byte groups of
+    // filters (k_conv_stem: float4 / 8 bf16; k_stem_tc: 16-byte rows), so each output pixel must start 16-byte aligned; a stem
+    // writing a channel slice of a route's buffer at an unaligned offset runs as a plain convolution behind the conversion.
     void plan_first_op() {
         const Layer &l0 = layer(0);
         const TV out0 = layout_view(0);
+        const bool out_vec = L[0].out_dt == DT_F32 ? vec4_view(out0)
+                                                   : out0.ldc % 8 == 0 && (reinterpret_cast<uintptr_t>(out0.base) & 15) == 0;
         const bool stem_ok = l0.type == YB_CONVOLUTIONAL && L[0].variant == 0 && L[0].path == CP_SIMT && l0.c == 3 &&
                              l0.size == 3 && l0.stride == 1 && l0.pad == 1 && (l0.n == 16 || l0.n == 32) && L[0].fused_into < 0 &&
-                             L[0].has_out && !sw.no_stem && (L[0].out_dt == DT_F32 || out0.ldc % 8 == 0);
+                             L[0].has_out && !sw.no_stem && out_vec;
         // exact nets: stem + 2x2/2 max-pool + the integer layer's input conversion in one kernel (k_stem_pool): layers 0 and 1
         // are then never written to HBM
         bool pool_ok = stem_ok && opt.fuse && L[0].out_dt == DT_F32 && l0.n == 16 && nl > 2 && !sw.no_stem_pool_fuse &&

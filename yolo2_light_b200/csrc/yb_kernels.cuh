@@ -530,7 +530,7 @@ __global__ void __launch_bounds__(128) k_conv_stem(const float *__restrict__ in,
     }
     TOut *o = tv_px<TOut>(out, n, y, x);
     if constexpr (sizeof(TOut) == 2) {
-        uint4 *op = reinterpret_cast<uint4 *>(o);
+        uint4 *op = reinterpret_cast<uint4 *>(o);     // 8 filters per store: the layer plan checks a 16-byte aligned base, ldc % 8 == 0
 #pragma unroll
         for (int g = 0; g < NF / 8; ++g) {
             float t[8];
@@ -547,7 +547,7 @@ __global__ void __launch_bounds__(128) k_conv_stem(const float *__restrict__ in,
             op[g] = v;
         }
     } else {
-        float4 *op = reinterpret_cast<float4 *>(o);   // NF*4 bytes per pixel, 16-byte aligned (ldc % 4 == 0)
+        float4 *op = reinterpret_cast<float4 *>(o);   // NF*4 bytes per pixel, 16-byte aligned: the layer plan checks vec4_view(out)
 #pragma unroll
         for (int g = 0; g < NF / 4; ++g)
             op[g] = make_float4(act_exact(__fadd_rn(acc[g * 4 + 0], sw.b[g * 4 + 0]), act), act_exact(__fadd_rn(acc[g * 4 + 1], sw.b[g * 4 + 1]), act),
@@ -632,7 +632,8 @@ __global__ void __launch_bounds__(128) k_conv_xnor_smallk_pool(XnorP p, TV q /* 
 }
 
 // XNOR convolution for small K (one or two words per tap): one thread per output pixel keeps its 9 x CW input
-// words in registers and walks all filters, whose sign words sit in shared memory (broadcast reads).
+// words in registers and walks all filters, whose sign words sit in shared memory (broadcast reads).  Whole groups of 4
+// filters are stored as one float4: the output must be a vec4_view (16-byte aligned pixels), which the layer plan checks.
 template <int CW>
 __global__ void __launch_bounds__(128) k_conv_xnor_smallk(XnorP p) {
     extern __shared__ uint32_t wsm[];            // [n][9*CW]
