@@ -41,9 +41,38 @@ enum { YB_LOGISTIC = 0, YB_RELU = 1, YB_LINEAR = 3, YB_LEAKY = 7 };
 /* Arithmetic used for the FP32-variant convolutions (yolov2_forward_network.c:204-211).
  *  YB_PREC_BF16_TC : bf16 operands, f32 accumulation on the wgmma tensor cores, bf16 NHWC activations (default)
  *  YB_PREC_FP32    : f32 operands and accumulation on CUDA cores, f32 activations (validation / exact nets)
- * Networks that contain XNOR layers, and every network run through the -quantized rule, always keep f32
+ * Networks that contain XNOR layers, and every network run through an INT8 rule, always keep f32
  * activations so the integer paths see exactly the reference's inputs. */
 enum { YB_PREC_BF16_TC = 0, YB_PREC_FP32 = 1 };
+
+/* INT8 rules: what every `int quantized` argument below selects.  The reference has two INT8 forwards, and they compute
+ * different things; src/main.c:199-206 runs the GPU one when built with GPU and run with -quantized.
+ *  YB_QUANT_NONE (0) : no INT8 layer (network_predict_cpu / network_predict_gpu_cudnn).
+ *  YB_QUANT_CPU  (1) : network_predict_quantized, src/yolov2_forward_network_quantized.c:1160.  Every other non-zero value
+ *                      means this rule too.
+ *      layers: conv i is INT8 iff i >= 1 and its activation is not LINEAR (:1036);
+ *      input:  xq = clamp(+-127, (int16_t)(x * input_mult)) (x86 float->int16: wraps for |x * m| >= 32768);
+ *      output: y = (float)clamp(+-32767, acc / 32) * (32 / (input_mult * weights_mult)) + bias, leaky as y / 10 (:474-490).
+ *  YB_QUANT_GPU  (2) : network_predict_gpu_cudnn_quantized, src/yolov2_forward_network_gpu.cu:576.
+ *      layers: conv i is INT8 iff the parser's l.quantized is set (forward_network_gpu_cudnn_quantized :494-507,
+ *              init_gpu_int8x4 :603-611).  parse_convolutional sets it only for a cfg parsed with quantized = 1, and not
+ *              for index 0, LINEAR activations, stride > 1 at index > 1, or 1x1 layers (src/additionally.c:3557-3559); the
+ *              convolution whose next-but-one section is [yolo] switches it off for the rest of the net (:3996-4003).
+ *              Every other convolution is a float one (an XNOR layer keeps its XNOR path), so a network parsed with
+ *              quantized = 0 runs no INT8 layer.  yb_layer_desc.quantized carries the flag on the drop-in path.
+ *      input:  v = x * input_mult rounded once, converted to int as CUDA does (truncation, saturating at +-2^31, NaN -> 0),
+ *              clamped to +-127 (cuda_f32_to_int8 + max_abs, src/gpu.cu:730-739).  It agrees with the CPU rule's for
+ *              |v| < 32768 and saturates above (v = 40000: +127 here, -127 there).  v <= -2^31 (and -inf) gives -127 here:
+ *              max_abs read without overflow; what the reference binary makes of abs(INT_MIN) is its compiler's choice.
+ *      output: y = act((float)acc * (1 / (input_mult * weights_mult)) + bias) with the exact s32 accumulator and zero
+ *              padding (yolov2_forward_network_gpu.cu:184-229, :314): one rounded multiply, one rounded add, then the
+ *              activation as every f32 layer computes it.  No /32, no int16 clamp.  cuDNN may fuse the multiply and the add
+ *              (one rounding less); that difference cannot be checked without cuDNN.
+ *      Every other layer computes what yb_network_predict computes.  Activations between layers stay f32.  With
+ *      YB_PREC_FP32 the float convolutions are the reference's exact CPU arithmetic; at the default precision every float
+ *      convolution the tensor cores take runs on tf32 (the reference's are cuDNN convolutions, which no fixed summation
+ *      order reproduces). */
+enum { YB_QUANT_NONE = 0, YB_QUANT_CPU = 1, YB_QUANT_GPU = 2 };
 
 /* One layer of a prepared network: the subset of the reference's `struct layer` (src/additionally.h:409-684)
  * that the forward path reads (SURVEY 8a, a13).  All pointers are host pointers owned by the caller; the
@@ -57,7 +86,7 @@ typedef struct yb_layer_desc {
     int size, stride, pad;    /* conv/maxpool geometry (maxpool pad = cfg `padding`) (layer.size/stride/pad) */
     int out_h, out_w, out_c;  /* output tensor                                      (layer.out_*)       */
     int xnor;                 /* conv: BIT1-XNOR variant                            (layer.xnor)        */
-    int quantized;            /* conv: parser's per-layer INT8 flag (informational)  (layer.quantized)   */
+    int quantized;            /* conv: parser's per-layer INT8 flag; YB_QUANT_GPU's layers (layer.quantized) */
     int index;                /* shortcut: absolute index of the `from` layer        (layer.index)       */
     int classes, coords, softmax, total;   /* yolo/region                            (layer.classes ...) */
     int reverse;              /* upsample/reorg                                      (layer.reverse)     */
@@ -136,6 +165,10 @@ float *yb_network_predict(yb_network *net, const float *input);
  * INT8 rule of yolov2_forward_network_q (:1036): conv i uses the s8 x s8 -> s32 path iff i >= 1 and its
  * activation is not LINEAR; everything else as in yb_network_predict with f32 activations. */
 float *yb_network_predict_quantized(yb_network *net, const float *input);
+
+/* replaces network_predict_gpu_cudnn_quantized(network net, float *input)   src/yolov2_forward_network_gpu.cu:576
+ * The YB_QUANT_GPU rule (see there); outputs as in yb_network_predict. */
+float *yb_network_predict_cudnn_quantized(yb_network *net, const float *input);
 
 /* Input pipeline on the device (SURVEY 8f row 2): replaces load_image_stb's u8 -> float/255 conversion
  * (src/additionally.c:3080-3103) + resize_image (src/additionally.c:3021-3064) + network_predict_*.
@@ -267,10 +300,12 @@ int yb_network_sync_outputs(yb_network *net, int quantized, void *stream);   /* 
  * layout/dtype.  dst must hold batch*out_c*out_h*out_w floats (region: batch*outputs). */
 int yb_network_fetch_layer(yb_network *net, int i, int quantized, float *dst);
 
-/* replaces forward_convolutional_layer_cpu(layer l, network_state state)  src/yolov2_forward_network.c:30 and
- * forward_convolutional_layer_q(layer l, network_state state)  src/yolov2_forward_network_quantized.c:527.
+/* replaces forward_convolutional_layer_cpu(layer l, network_state state)  src/yolov2_forward_network.c:30,
+ * forward_convolutional_layer_q(layer l, network_state state)  src/yolov2_forward_network_quantized.c:527 and
+ * forward_convolutional_layer_gpu_cudnn_quantized(layer l, network_state state)  src/yolov2_forward_network_gpu.cu:143.
  * Runs conv layer `i` of net alone on `input` (host NCHW, batch*c*h*w) and writes host NCHW `output`
- * (batch*n*out_h*out_w).  variant: 0 = as yb_network_predict would run it, 1 = as the quantized rule would. */
+ * (batch*n*out_h*out_w).  variant: 0 = as yb_network_predict would run it, 1 = as the quantized rule would,
+ * 2 = by the YB_QUANT_GPU arithmetic, in INT8 whatever the layer's l.quantized (as that reference function does). */
 int yb_forward_convolutional_layer(yb_network *net, int i, int variant, const float *input, float *output);
 
 /* ---- multi-GPU batch extension (SURVEY 8b "Batch extension", 8e) ------------------------------------------------------
@@ -304,7 +339,7 @@ int  yb_network_set_option(yb_network *net, const char *name, int value);
    "act_bytes" (device memory of the activation buffers).  -1: unknown key. */
 long yb_network_get_info(yb_network *net, int quantized, const char *key);
 /* The tensor-core plan of layer `layer` (builds the engine if needed), read-only: up to n of {kernel (0 k_conv_tc,
- * 1 k_conv_tc_reg, 2 k_stem_tc, 3 k_stem_s2_tc), kind (0 bf16, 1 int8, 2 xnor, 3 tf32), TW, TH, BN, BK, nt, bstat, stages,
+ * 1 k_conv_tc_reg, 2 k_stem_tc, 3 k_stem_s2_tc), kind (0 bf16, 1 int8, 2 xnor, 3 tf32, 4 int8 of YB_QUANT_GPU), TW, TH, BN, BK, nt, bstat, stages,
  * sps, grid, num_work, tma_epi, jshift, out_ldc (output pixel stride, elements; 0: no NHWC output)} into fields; -1 in a
  * field that does not apply to the kernel (the stems' fixed tiles).  Returns the number written: 0 for a layer without a
  * tensor-core plan, -1 on error. */

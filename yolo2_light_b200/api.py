@@ -8,6 +8,10 @@ forward path (same names, argument meaning and call order as ``src/main.c:160-21
     quantinization_and_get_multipliers(net)               # yolov2_forward_network_quantized.c:1402 (if quantized)
     out = network_predict_b200(net, images)               # slot of network_predict_cpu / _gpu_cudnn
     out = network_predict_b200_quantized(net, images)     # slot of network_predict_quantized
+    out = network_predict_b200_cudnn_quantized(net, images)   # slot of network_predict_gpu_cudnn_quantized
+
+Every ``quantized`` argument selects an INT8 rule: 0 (or False) none, 1 (or True) the CPU build's, 2 the GPU build's
+(YB_QUANT_NONE / YB_QUANT_CPU / YB_QUANT_GPU of the C header).
 
 Everything heavy happens inside the shared library (CUDA, sm_90a); this module only marshals pointers.  There is
 no CPU fallback: if the library is missing or no sm_90 GPU (H100) is visible the calls raise.
@@ -27,6 +31,7 @@ YB_CONVOLUTIONAL, YB_MAXPOOL, YB_SOFTMAX, YB_ROUTE, YB_SHORTCUT = 0, 3, 4, 8, 13
 YB_REGION, YB_YOLO, YB_UPSAMPLE, YB_REORG, YB_BLANK = 21, 22, 23, 24, 25
 YB_LOGISTIC, YB_RELU, YB_LINEAR, YB_LEAKY = 0, 1, 3, 7
 YB_PREC_BF16_TC, YB_PREC_FP32 = 0, 1
+YB_QUANT_NONE, YB_QUANT_CPU, YB_QUANT_GPU = 0, 1, 2
 LAYER_NAMES = {0: "CONVOLUTIONAL", 3: "MAXPOOL", 4: "SOFTMAX", 8: "ROUTE", 13: "SHORTCUT", 21: "REGION", 22: "YOLO",
                23: "UPSAMPLE", 24: "REORG", 25: "BLANK"}
 
@@ -119,6 +124,7 @@ def lib():
         "yb_network_replication": (C.c_char_p, [vp]),
         "yb_network_predict": (fp, [vp, vp]),
         "yb_network_predict_quantized": (fp, [vp, vp]),
+        "yb_network_predict_cudnn_quantized": (fp, [vp, vp]),
         "yb_network_predict_image_u8": (fp, [vp, vp, C.c_int, C.c_int, C.c_int]),
         "yb_network_fetch_input": (C.c_int, [vp, C.c_int, vp]),
         "yb_network_submit": (C.c_int, [vp, vp, C.c_int]),
@@ -157,6 +163,7 @@ EXPORTED_SYMBOLS = [
     "yb_network_layer_outputs", "yb_network_input_calibration", "yb_set_batch_network", "yb_network_set_device",
     "yb_network_set_precision", "yb_network_set_option", "yb_network_get_info", "yb_network_tc_plan", "yb_network_detect", "yb_network_calibrate", "yb_entropy_calibration",
     "yb_network_input_histogram", "yb_map_evaluate", "yb_network_predict", "yb_network_predict_quantized",
+    "yb_network_predict_cudnn_quantized",
     "yb_network_predict_image_u8", "yb_network_fetch_input", "yb_network_submit", "yb_network_collect", "yb_network_layer_output", "yb_network_forward_device", "yb_network_sync_outputs", "yb_network_fetch_layer",
     "yb_network_fetch_counts", "yb_forward_convolutional_layer", "yb_network_weight_arena",
     "yb_network_last_launches", "yb_network_profile", "yb_op_kind_name", "yb_network_op_kernels", "yb_get_network_boxes", "yb_alloc_pinned",
@@ -170,7 +177,7 @@ EXPORTED_SYMBOLS = [
 TC_PLAN_FIELDS = ("kernel", "kind", "TW", "TH", "BN", "BK", "nt", "bstat", "stages", "sps", "grid", "num_work", "tma_epi",
                   "jshift", "out_ldc")
 TC_PLAN_KERNELS = ("k_conv_tc", "k_conv_tc_reg", "k_stem_tc", "k_stem_s2_tc")
-TC_PLAN_KINDS = ("bf16", "s8", "xnor", "tf32")
+TC_PLAN_KINDS = ("bf16", "s8", "xnor", "tf32", "s8_gpu")
 
 
 def _check(ok: bool):
@@ -289,7 +296,9 @@ class Network:
         x = np.ascontiguousarray(images, dtype=np.float32)
         if x.size != self.batch * self.c * self.h * self.w:
             raise YbError(f"input has {x.size} floats, network wants batch {self.batch} x {self.c}x{self.h}x{self.w}")
-        f = lib().yb_network_predict_quantized if quantized else lib().yb_network_predict
+        rule = int(quantized)
+        f = (lib().yb_network_predict_cudnn_quantized if rule == YB_QUANT_GPU else
+             lib().yb_network_predict_quantized if rule else lib().yb_network_predict)
         p = f(self._h, x.ctypes.data_as(C.c_void_p))
         _check(bool(p))
         return self.layer_output(self.n - 1)
@@ -702,6 +711,11 @@ def network_predict_b200(net: Network, images: np.ndarray) -> np.ndarray:
 
 def network_predict_b200_quantized(net: Network, images: np.ndarray) -> np.ndarray:
     return net.predict(images, quantized=True)
+
+
+def network_predict_b200_cudnn_quantized(net: Network, images: np.ndarray) -> np.ndarray:
+    """The reference's GPU INT8 mode (network_predict_gpu_cudnn_quantized): the INT8 layers are the parser's l.quantized."""
+    return net.predict(images, quantized=YB_QUANT_GPU)
 
 
 def load_network(cfg: str, weights: Optional[str], batch: int = 1, quantized: int = 0) -> Network:

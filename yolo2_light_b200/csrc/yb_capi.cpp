@@ -38,7 +38,7 @@ static EngineOptions engine_options(const Network &net, int quantized, int devic
     EngineOptions opt;
     opt.device = device;
     opt.precision = net.precision;
-    opt.qrule = quantized != 0;
+    opt.rule = quant_rule(quantized);
     opt.upload = upload;
     opt.fuse = net.fuse;
     opt.keep_counts = net.keep_counts;
@@ -48,7 +48,7 @@ static EngineOptions engine_options(const Network &net, int quantized, int devic
 
 static Engine *get_engine(yb_network *n, int quantized, bool upload = true) {
     Network &net = n->net;
-    const int slot = quantized ? 1 : 0;
+    const int slot = quant_rule(quantized);
     if (!net.engine[slot]) net.engine[slot] = build_engine(&net, engine_options(net, quantized, net.device, upload));
     return net.engine[slot].get();
 }
@@ -261,7 +261,10 @@ float *yb_network_predict(yb_network *n, const float *input) {
     YB_TRY return predict_common(n, input, 0); YB_CATCH(nullptr)
 }
 float *yb_network_predict_quantized(yb_network *n, const float *input) {
-    YB_TRY return predict_common(n, input, 1); YB_CATCH(nullptr)
+    YB_TRY return predict_common(n, input, YB_QUANT_CPU); YB_CATCH(nullptr)
+}
+float *yb_network_predict_cudnn_quantized(yb_network *n, const float *input) {
+    YB_TRY return predict_common(n, input, YB_QUANT_GPU); YB_CATCH(nullptr)
 }
 
 int yb_network_submit(yb_network *n, const float *input, int quantized) {
@@ -499,7 +502,8 @@ int yb_forward_convolutional_layer(yb_network *n, int i, int variant, const floa
     if (i < 0 || i >= (int)src.layers.size() || src.layers[i].type != YB_CONVOLUTIONAL)
         fatal_throw("yb_forward_convolutional_layer: not a convolutional layer");
     if (!input || !output) fatal_throw("yb_forward_convolutional_layer: null buffer");
-    const int key = 2 * i + (variant ? 1 : 0);
+    const int rule = quant_rule(variant);
+    const int key = 3 * i + rule;
     auto it = n->single.find(key);
     if (it == n->single.end() || it->second->net.batch != src.batch || it->second->net.device != src.device ||
         it->second->net.precision != src.precision) {
@@ -508,13 +512,15 @@ int yb_forward_convolutional_layer(yb_network *n, int i, int variant, const floa
         const Layer &l = src.layers[i];
         t.batch = src.batch; t.h = l.h; t.w = l.w; t.c = l.c; t.inputs = l.h * l.w * l.c;
         t.device = src.device; t.precision = src.precision; t.fuse = false;
-        t.q_index_offset = i + src.q_index_offset;   // the `i >= 1` half of the INT8 rule
+        t.q_index_offset = i + src.q_index_offset;   // the `i >= 1` half of the CPU INT8 rule
         t.layers.push_back(l);
+        // forward_convolutional_layer_gpu_cudnn_quantized runs the layer in INT8 whatever its l.quantized
+        if (rule == YB_QUANT_GPU) t.layers[0].quantized = 1;
         t.layers[0].output = nullptr; t.layers[0].output_count = 0;
         it = n->single.insert_or_assign(key, std::move(tmp)).first;
     }
     yb_network *one = it->second.get();
-    Engine *e = get_engine(one, variant);
+    Engine *e = get_engine(one, rule);
     engine_upload_input(e, input, nullptr);
     engine_forward(e, nullptr, nullptr);
     engine_fetch_layer(e, &one->net, 0, output);
@@ -530,22 +536,22 @@ int yb_network_set_devices(yb_network *n, const int *devices, int ndev) {
     for (int k = 0; k < ndev; ++k)
         if (devices[k] < 0 || devices[k] >= have) fatal_throw("set_devices: device " + std::to_string(devices[k]) + " does not exist");
     n->devices.assign(devices, devices + ndev);
-    n->replicas[0].clear(); n->replicas[1].clear();
+    for (auto &r : n->replicas) r.clear();
     if (ndev > 0 && n->net.device != devices[0]) { n->net.device = devices[0]; drop_engines(&n->net); }
     return 0;
     YB_CATCH(-1)
 }
 
 static std::vector<Engine *> get_replicas(yb_network *n, int quantized, int ngpus) {
-    const int slot = quantized ? 1 : 0;
+    const int slot = quant_rule(quantized);
     if (n->devices.empty() || (int)n->devices.size() < ngpus) {
         const int have = engine_device_count();
         if (ngpus > have) fatal_throw("predict_batch: " + std::to_string(ngpus) + " GPUs requested, " + std::to_string(have) + " visible");
         n->devices.resize(ngpus);
         for (int k = 0; k < ngpus; ++k) n->devices[k] = k;
-        n->replicas[0].clear(); n->replicas[1].clear();
+        for (auto &r : n->replicas) r.clear();
     }
-    if (n->net.device != n->devices[0]) { n->net.device = n->devices[0]; drop_engines(&n->net); n->replicas[0].clear(); n->replicas[1].clear(); }
+    if (n->net.device != n->devices[0]) { n->net.device = n->devices[0]; drop_engines(&n->net); for (auto &r : n->replicas) r.clear(); }
     const bool fresh0 = !n->net.engine[slot];
     Engine *e0 = get_engine(n, quantized);
     if (fresh0) n->replicas[slot].clear();           // replica 0 was rebuilt: the others hold stale plans

@@ -20,8 +20,8 @@
 //     bias (folded batch-norm), apply leaky-ReLU and store f32 for detection heads -- optionally with the following
 //     [yolo] layer applied (:453-472).  The producer warp keeps loading the next tile's stages meanwhile.
 //   * The same kernel runs the INT8 variant (s8 x s8 -> s32 wgmma, exact requantising epilogue,
-//     yolov2_forward_network_quantized.c:474-490), wide XNOR layers as +-1 bytes on the s8 wgmma, and the float heads
-//     of the exact networks on tf32 wgmma.
+//     yolov2_forward_network_quantized.c:474-490, or the GPU rule's unscaled one, yolov2_forward_network_gpu.cu:184-229),
+//     wide XNOR layers as +-1 bytes on the s8 wgmma, and the float heads of the exact networks on tf32 wgmma.
 //
 // Warp roles of k_conv_tc (288 threads): warps 0-7 = two consumer warpgroups (wgmma + epilogue), warp 8 = TMA producer.
 #include <cuda.h>
@@ -69,10 +69,11 @@ struct TcParams {
     int xt, jt, nt;           // #tiles along x, merged rows, filters
     int num_work;             // tiles = work items of the persistent loop (xt * jt * nt)
     int kind;                 // TcKind: TC_BF16 bf16 x bf16 -> f32;  TC_S8 s8 x s8 -> s32, exact requantising epilogue;
+                              // TC_S8_GPU the same GEMM, the GPU rule's unscaled epilogue;
                               // TC_XNOR XNOR layer as +-1 s8 on the s8 wgmma (dot = 2*count - K exactly), reference float epilogue;
                               // TC_TF32 f32 operands read as tf32 (K = 8 per MMA) -> f32: float heads of the exact nets
     int kk;                   // MMAs per K-block (BK bytes / 32)
-    float alpha1;             // INT8: R_MULT / (input_mult * weights_mult)
+    float alpha1;             // INT8: R_MULT / (input_mult * weights_mult); TC_S8_GPU: 1 / (input_mult * weights_mult)
     const float *mean;        // kind 2 (XNOR as +-1 s8): per-filter mean |w|; out = (float)dot * mean + bias
     int xK;                   // kind 2: true K (size*size*C) for the raw popcount dump: count = (dot + K) / 2
     int *acc_out;             // INT8: optional raw s32 accumulators, NCHW (tests)
@@ -98,7 +99,7 @@ struct TcParams {
     int acc_pitch;            // words per row of the shared-memory accumulator tile (BN + 4: conflict-free row reads)
     // Fused 2x2 / stride-2 max-pool + input conversion of the NEXT integer layer (integer kinds, tiles of 8 x 16 pixels):
     // the epilogue reduces every 2x2 window inside the warp (lane ^ 1 = x neighbour, lane ^ 8 = y neighbour), converts it into
-    // the next layer's side format pool_fmt (SIDE_S8 with pool_mult, or SIDE_PM1_S8) and writes bytes straight into that layer's
+    // the next layer's side format pool_fmt (SIDE_S8 or SIDE_S8_SAT with pool_mult, or SIDE_PM1_S8) and writes bytes straight into that layer's
     // input: the f32 activation and the pooled f32 tensor never reach HBM.  pool_fmt SIDE_NONE: no fused max-pool.  jshift = 1 moves every tile down one merged row so
     // that window rows (oy even, oy + 1) fall into the same tile (the padded layout puts oy = 0 on an odd merged row).
     int pool_fmt, jshift;     // SideFmt
@@ -532,10 +533,11 @@ __device__ __forceinline__ void tc_mma_loop(T (&d)[BN / 2], const TcParams &p, u
     if (pend >= 0) release(pend);
 }
 
-// The reference's float epilogue of the integer kinds (bit-exact): TC_S8 int8_epilogue; TC_XNOR xnor_epilogue, where the s8
-// wgmma's acc is dot = 2*count - K exactly.  f: filter index (TC_XNOR reads its mean |w|).
+// The reference's float epilogue of the integer kinds (bit-exact): TC_S8 int8_epilogue; TC_S8_GPU int8_gpu_epilogue; TC_XNOR
+// xnor_epilogue, where the s8 wgmma's acc is dot = 2*count - K exactly.  f: filter index (TC_XNOR reads its mean |w|).
 __device__ __forceinline__ float int_epilogue(const TcParams &p, int kind, int acc, int f, float bias) {
     if (kind == TC_S8) return int8_epilogue(acc, p.alpha1, bias, p.act);
+    if (kind == TC_S8_GPU) return int8_gpu_epilogue(acc, p.alpha1, bias, p.act);
     return xnor_epilogue(acc, (f < p.n) ? __ldg(p.mean + f) : 0.f, bias, p.act);
 }
 
@@ -543,7 +545,7 @@ __device__ __forceinline__ float int_epilogue(const TcParams &p, int kind, int a
 // ST: compiled with the per-role cycle counters of YB_TC_STATS=1 (diagnostic); the production instantiations (ST = false)
 // contain no clock64() reads.
 // EPI: which epilogue family is compiled in -- 0: LSU stores, float kinds (f32 heads / fused [yolo]); 2: the integer
-// kinds (s8 requantising and XNOR-as-+-1 epilogues).  The bf16-output layers run k_conv_tc_reg.
+// kinds (s8 requantising, s8 unscaled and XNOR-as-+-1 epilogues).  The bf16-output layers run k_conv_tc_reg.
 // tmO1, tmR: unused (the parameter list of k_conv_tc_reg, so that a plan launches either kernel the same way).
 template <bool ST, int EPI>
 __global__ void __launch_bounds__(TC_THREADS, 1)
@@ -609,7 +611,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
             });
         };
         auto run_mainloop = [&]() {
-            // EPI 2: TC_XNOR runs the same s8 wgmma as TC_S8
+            // EPI 2: TC_S8_GPU and TC_XNOR run the same s8 wgmma as TC_S8
             if constexpr (EPI == 2) mainloop(std::integral_constant<TcKind, TC_S8>{});
             else if (p.kind == TC_BF16) mainloop(std::integral_constant<TcKind, TC_BF16>{});
             else mainloop(std::integral_constant<TcKind, TC_TF32>{});
@@ -710,9 +712,10 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                 __syncwarp();
             };
 
-            // ---- fused 2x2/2 max-pool + conversion to the next integer layer's input (TcParams::pool_fmt).  Both epilogue functions
-            // are monotone non-decreasing in the s32 accumulator (truncating /32, clamp, x positive ALPHA1, + bias, leaky; resp.
-            // x mean >= 0, + bias, leaky), so max over the window commutes with them EXACTLY: the window maximum is taken on the raw
+            // ---- fused 2x2/2 max-pool + conversion to the next integer layer's input (TcParams::pool_fmt).  All three epilogue
+            // functions are monotone non-decreasing in the s32 accumulator (truncating /32, clamp, x positive ALPHA1, + bias, leaky;
+            // the GPU rule's (float)acc x positive ALPHA1, + bias, leaky; resp. x mean >= 0, + bias, leaky), each step rounding
+            // monotonically, so max over the window commutes with them EXACTLY: the window maximum is taken on the raw
             // accumulators and the float epilogue runs once per pooled value.  Window = lanes {l, l^1, l^8, l^9} (tile rows are 8
             // pixels wide).  The reduction is a reduce-scatter: lane^1 halves the 32 columns, lane^8 halves them again, every lane
             // ends up with the maxima of 8 columns of its window and finishes those -- a quarter of the float work per lane.
@@ -739,7 +742,8 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                 for (int j = 0; j < 8; ++j) {
                     const int f = n0 + cbase + j;
                     const float t = int_epilogue(p, p.kind, h8[j], f, bs[cbase + j]);
-                    uint32_t b8 = (p.pool_fmt == SIDE_S8) ? side_code<SIDE_S8>(t, p.pool_mult) : side_code<SIDE_PM1_S8>(t, 0.f);
+                    uint32_t b8 = (p.pool_fmt == SIDE_S8) ? side_code<SIDE_S8>(t, p.pool_mult)
+                                : (p.pool_fmt == SIDE_S8_SAT) ? side_code<SIDE_S8_SAT>(t, p.pool_mult) : side_code<SIDE_PM1_S8>(t, 0.f);
                     if (f >= p.n) b8 = 0;
                     if (j < 4) w0 |= side_place<SIDE_S8>(b8, j); else w1 |= side_place<SIDE_S8>(b8, j - 4);
                 }
@@ -799,6 +803,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                     }
                 };
                 if (p.kind == TC_XNOR) int_slabs(std::integral_constant<TcKind, TC_XNOR>{});
+                else if (p.kind == TC_S8_GPU) int_slabs(std::integral_constant<TcKind, TC_S8_GPU>{});
                 else int_slabs(std::integral_constant<TcKind, TC_S8>{});
             } else {
                 for (int f0 = cbeg; f0 < cend; f0 += 64) {
@@ -1538,7 +1543,7 @@ int sm_count() {
     return sms;
 }
 
-bool is_integer(int kind) { return kind == TC_S8 || kind == TC_XNOR; }
+bool is_integer(int kind) { return kind == TC_S8 || kind == TC_S8_GPU || kind == TC_XNOR; }
 int elem_size(int kind) { return kind == TC_TF32 ? 4 : is_integer(kind) ? 1 : 2; }   // operand element size
 // operand channels per pixel: the integer kinds read the s8 input's zero-padded channels (their weights are padded alike)
 int operand_channels(const TcConv &c) { return is_integer(c.kind) ? c.in.ldc : c.l->c; }
@@ -1814,7 +1819,7 @@ int tc_conv_supported(const TcConv &c) {
     if (c.yolo_out && (integer || c.out_bf16)) return 0;
     // fused max-pool: the 8 x 16 tiles of the stride-1 3x3 integer layers start one merged row down, so 2x2 windows never
     // straddle tiles when the padded height and the output size are even; the epilogue writes whole 32-filter groups of bytes
-    if (c.pool_fmt != SIDE_NONE && !(integer && (c.pool_fmt == SIDE_S8 || c.pool_fmt == SIDE_PM1_S8) && !c.acc_out && l.size == 3 && l.stride == 1 &&
+    if (c.pool_fmt != SIDE_NONE && !(integer && (side_s8(c.pool_fmt) || c.pool_fmt == SIDE_PM1_S8) && !c.acc_out && l.size == 3 && l.stride == 1 &&
                          l.h % 2 == 0 && l.out_h % 2 == 0 && l.out_w % 2 == 0 && l.n % 32 == 0 &&
                          c.pool_next.H == l.out_h / 2 && c.pool_next.W == l.out_w / 2 && aligned(c.pool_next, 1)))
         return 0;

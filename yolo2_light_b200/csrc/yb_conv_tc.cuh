@@ -32,13 +32,13 @@ struct TcConv {
     const void *w = nullptr;       // [ldn][K] filter matrix, K ordered (ky, kx, c); integer kinds: c padded to in.ldc
     int ldn = 0;
     const float *bias = nullptr;
-    float alpha1 = 0.f;            // TC_S8: R_MULT / (input_mult * weights_mult)
+    float alpha1 = 0.f;            // TC_S8: R_MULT / (input_mult * weights_mult); TC_S8_GPU: 1 / (input_mult * weights_mult)
     const float *mean = nullptr;   // TC_XNOR: per-filter mean |w|
     int *acc_out = nullptr;        // integer kinds: raw s32 accumulators / popcounts, NCHW (tests), or null
     float *yolo_out = nullptr;     // fused [yolo] layer: its NCHW f32 output, or null
     int yolo_classes = 0;
     SideFmt pool_fmt = SIDE_NONE;  // fused 2x2/2 max-pool + the next integer layer's input conversion into this format; SIDE_NONE: none
-    float pool_mult = 0.f;         // SIDE_S8: the next layer's input multiplier
+    float pool_mult = 0.f;         // SIDE_S8, SIDE_S8_SAT: the next layer's input multiplier
     TV pool_next{};                // the next integer layer's input
     TcSwitches sw{};
 };

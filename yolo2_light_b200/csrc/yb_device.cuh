@@ -50,10 +50,12 @@ enum TcKind {
     TC_BF16 = 0,   // bf16 x bf16 -> f32; bf16 or f32 output
     TC_S8 = 1,     // INT8: s8 x s8 -> s32, the reference's exact requantising epilogue; f32 output
     TC_XNOR = 2,   // XNOR layer as +-1 s8 on the s8 wgmma (dot = 2*count - K exactly); f32 output
-    TC_TF32 = 3,   // f32 operands read as tf32: the float detection heads of the exact (INT8 / XNOR) networks; f32 output
+    TC_TF32 = 3,   // f32 operands read as tf32: the float detection heads of the exact (INT8 / XNOR) networks, and every float
+                   // convolution of the GPU INT8 rule; f32 output
+    TC_S8_GPU = 4, // INT8 of the GPU rule: s8 x s8 -> s32, the unscaled epilogue int8_gpu_epilogue; f32 output
 };
 
-// The converted ("side") input of an integer convolution, padded NHWC.  The three integer formats are what the kernels write;
+// The converted ("side") input of an integer convolution, padded NHWC.  The four integer formats are what the kernels write;
 // SIDE_NONE and SIDE_PM1_F32 occur only in the engine's layer plan.
 enum SideFmt {
     SIDE_NONE = 0,   // no converted input (f32 convolutions); as a fusion: none
@@ -61,12 +63,15 @@ enum SideFmt {
     SIDE_S8,         // s8 quant_i8(x, the layer's input multiplier): INT8 convolutions
     SIDE_PM1_S8,     // +-1 bytes, +1 where x > 0: XNOR layers on the s8 wgmma
     SIDE_BITS,       // sign bits, bit = (x > 0), 32 channels per 32-bit word: XNOR layers on the popcount kernels
+    SIDE_S8_SAT,     // s8 quant_i8_sat(x, the layer's input multiplier): INT8 convolutions of the GPU rule
 };
 
 // channels per 32-bit word of an integer side format
 __host__ __device__ constexpr int side_per_word(SideFmt f) { return f == SIDE_BITS ? 32 : 4; }
 // the formats the kernels write: everything but the plan-only SIDE_NONE and SIDE_PM1_F32
-__host__ __device__ constexpr bool side_int(SideFmt f) { return f == SIDE_S8 || f == SIDE_PM1_S8 || f == SIDE_BITS; }
+__host__ __device__ constexpr bool side_int(SideFmt f) { return f == SIDE_S8 || f == SIDE_PM1_S8 || f == SIDE_BITS || f == SIDE_S8_SAT; }
+// the s8 formats of the INT8 layers: the byte is the quantised activation under the layer's input multiplier
+__host__ __device__ constexpr bool side_s8(SideFmt f) { return f == SIDE_S8 || f == SIDE_S8_SAT; }
 
 // INT8 input quantisation (reference yolov2_forward_network_quantized.c:527-631): xq = clamp(+-127, (int16_t)(x * input_mult))
 // with x86 float->int16 semantics (cvttss2si, low 16 bits, indefinite -> 0).  NaN and -inf give 0, and so does -FLT_MAX for
@@ -82,12 +87,23 @@ __device__ __forceinline__ int quant_i8(float x, float mult) {
     return s;
 }
 
+// INT8 input quantisation of the GPU rule (cuda_f32_to_int8 + max_abs, reference gpu.cu:730-739): v = x * input_mult rounded
+// once, converted to int as CUDA does it (truncation, saturating at +-2^31, NaN -> 0), then clamped to +-127.  It agrees with
+// quant_i8 for |v| < 32768; above that quant_i8 wraps through int16 and this saturates (v = 40000: -127 there, +127 here).
+// v <= -2^31 (and -inf) gives -127 here: max_abs read without overflow.  The reference evaluates abs(INT_MIN) there, whose
+// result its compiler decides; that case cannot be checked against the reference binary.
+__device__ __forceinline__ int quant_i8_sat(float x, float mult) {
+    const int i = __float2int_rz(__fmul_rn(x, mult));
+    return i > 127 ? 127 : i < -127 ? -127 : i;
+}
+
 // One f32 value in side format F: the s8 byte (mult: the layer's input multiplier), the +-1 byte or the sign bit, in the low
 // bits of the result.  The sign is x > 0 (binarize_cpu, float_to_bit): NaN, -inf and -FLT_MAX give -1 / 0 alike.
 template <SideFmt F>
 __device__ __forceinline__ uint32_t side_code(float x, float mult) {
-    static_assert(F == SIDE_S8 || F == SIDE_PM1_S8 || F == SIDE_BITS, "integer side formats only");
+    static_assert(side_int(F), "integer side formats only");
     if constexpr (F == SIDE_S8) return (uint32_t)quant_i8(x, mult) & 0xffu;
+    else if constexpr (F == SIDE_S8_SAT) return (uint32_t)quant_i8_sat(x, mult) & 0xffu;
     else if constexpr (F == SIDE_PM1_S8) return x > 0.f ? 0x01u : 0xFFu;
     else return x > 0.f ? 1u : 0u;
 }
@@ -134,6 +150,15 @@ __device__ __forceinline__ float int8_epilogue(int acc, float alpha1, float bias
     y = __fadd_rn(y, bias);
     if (act == ACT_LEAKY) y = (y > 0.f) ? y : __fdiv_rn(y, 10.f);
     return y;
+}
+
+// INT8 epilogue of the GPU rule (forward_convolutional_layer_gpu_cudnn_quantized, yolov2_forward_network_gpu.cu:184-229, :314):
+// y = act((float)acc * alpha1 + bias), alpha1 = 1 / (input_mult * weights_mult) -- no /32, no int16 clamp.  One rounded multiply,
+// one rounded add, then act_exact, the operation order of int8_epilogue and the activation of every other f32 layer.  cuDNN's
+// fused convolution-bias-activation may contract the multiply and the add (one rounding less); that cannot be checked here.
+// Monotone non-decreasing in acc for alpha1 > 0, as the fused max-pool needs.
+__device__ __forceinline__ float int8_gpu_epilogue(int acc, float alpha1, float bias, int act) {
+    return act_exact(__fadd_rn(__fmul_rn((float)acc, alpha1), bias), act);
 }
 
 }  // namespace yb

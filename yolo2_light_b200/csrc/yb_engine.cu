@@ -251,7 +251,10 @@ struct Builder {
 
     int conv_variant(int i) const {   // 0 fp32, 1 xnor, 2 int8
         const Layer &l = layer(i);
-        if (opt.qrule && (i + opt.q_index_offset) >= 1 && l.activation != YB_LINEAR) return 2;
+        // CPU rule: yolov2_forward_network_q (yolov2_forward_network_quantized.c:1036); GPU rule: the parser's l.quantized
+        // (forward_network_gpu_cudnn_quantized, yolov2_forward_network_gpu.cu:494-507), XNOR layers included
+        if (opt.rule == YB_QUANT_CPU && (i + opt.q_index_offset) >= 1 && l.activation != YB_LINEAR) return 2;
+        if (opt.rule == YB_QUANT_GPU && l.quantized) return 2;
         return l.xnor ? 1 : 0;
     }
     // XNOR layers with enough channels run on the tensor cores as +-1 int8 (dot == 2*count - K, exact); the small ones stay on
@@ -299,8 +302,11 @@ struct Builder {
     }
     TV side_placed(int i) const { return side_view(i, e.act_arena.get() + side_off[i]); }
     // the multiplier of layer i's side conversion: the input multiplier of an INT8 layer, unused otherwise
-    float side_mult(int i) const { return L[i].side == SIDE_S8 ? layer(i).input_quant_multipler : 0.f; }
-    static float alpha1(const Layer &l) { return 32 / (l.input_quant_multipler * l.weights_quant_multipler); }   // ALPHA1, ..._quantized.c:598
+    float side_mult(int i) const { return side_s8(L[i].side) ? layer(i).input_quant_multipler : 0.f; }
+    // ALPHA1 of the rule's INT8 epilogue: ..._quantized.c:598 (CPU), yolov2_forward_network_gpu.cu:200 (GPU, no R_MULT)
+    float alpha1(const Layer &l) const {
+        return (opt.rule == YB_QUANT_GPU ? 1 : 32) / (l.input_quant_multipler * l.weights_quant_multipler);
+    }
 
     // Convolution i as a tensor-core convolution (the kind follows the variant and the activation type), with the shortcut and
     // [yolo] fusions of its plan and the max-pool fusion `pool` (layer i+2's side format, or SIDE_NONE).  placed == false: views
@@ -313,7 +319,7 @@ struct Builder {
         auto out = [&](int j) { return placed ? e.out_tv[j] : layout_view(j); };
         auto side = [&](int j) { return placed ? side_placed(j) : side_view(j, kLayoutBase); };
         TcConv c;
-        c.kind = p.variant == 2 ? TC_S8 : p.variant == 1 ? TC_XNOR : ADT == DT_BF16 ? TC_BF16 : TC_TF32;
+        c.kind = p.variant == 2 ? (opt.rule == YB_QUANT_GPU ? TC_S8_GPU : TC_S8) : p.variant == 1 ? TC_XNOR : ADT == DT_BF16 ? TC_BF16 : TC_TF32;
         c.l = &l;
         c.in = p.variant != 0 ? side(i) : !placed ? layout_in(i) : i == 0 ? e.in0 : e.out_tv[i - 1];
         c.out = out(tgt);
@@ -333,7 +339,7 @@ struct Builder {
         c.w = e.w_arena.get() + (c.kind == TC_BF16 ? cw[i].w_bf16 : c.kind == TC_TF32 ? cw[i].w_f32km : cw[i].w_s8);
         c.ldn = cw[i].ldn;
         c.bias = bias(i);
-        if (c.kind == TC_S8) c.alpha1 = alpha1(l);
+        if (c.kind == TC_S8 || c.kind == TC_S8_GPU) c.alpha1 = alpha1(l);
         if (c.kind == TC_XNOR) c.mean = reinterpret_cast<const float *>(e.w_arena.get() + cw[i].mean);
         c.acc_out = e.counts[i].get();
         if (p.yolo_fused) {
@@ -346,20 +352,22 @@ struct Builder {
     // ---- pass 1: the layer plan ------------------------------------------------------------------------------------------
     void plan_layers() {
         bool any_xnor = false;
-        for (const Layer &l : net.layers) {
+        for (int i = 0; i < nl; ++i) {
+            const Layer &l = layer(i);
             if (l.type != YB_CONVOLUTIONAL) continue;
             if (l.batch_normalize) fatal_throw("engine: batch-norm not folded -- call yb_fuse_conv_batchnorm first");
+            L[i].variant = conv_variant(i);
             if (l.xnor) {
                 any_xnor = true;
                 if (!l.has_mean_arr) fatal_throw("engine: xnor layer without mean_arr -- call yb_calculate_binary_weights first");
             }
-            if (opt.qrule && !l.has_int8)
+            // the CPU rule reads every convolution's int8 weights (yolov2_forward_network_q), the GPU rule its INT8 layers'
+            if ((opt.rule == YB_QUANT_CPU || L[i].variant == 2) && !l.has_int8)
                 fatal_throw("engine: -quantized rule without int8 weights -- call yb_quantinization_and_get_multipliers first");
         }
-        // f32 activations whenever an integer path must see exactly the reference's inputs
-        ADT = (opt.qrule || any_xnor || opt.precision == YB_PREC_FP32) ? DT_F32 : DT_BF16;
-        for (int i = 0; i < nl; ++i)
-            if (is_conv(i)) L[i].variant = conv_variant(i);
+        // f32 activations whenever an integer path must see exactly the reference's inputs; the GPU rule keeps float tensors
+        // between layers as the reference's GPU build does
+        ADT = (opt.rule != YB_QUANT_NONE || any_xnor || opt.precision == YB_PREC_FP32) ? DT_F32 : DT_BF16;
 
         // conv i + same-shape shortcut i+1 whose only reader is that shortcut
         if (opt.fuse) {
@@ -418,7 +426,10 @@ struct Builder {
             if (p.variant == 1 && xnor_fallback(l)) { p.side = SIDE_PM1_F32; p.side_ld = l.c; }
             else if (p.variant == 1 && xnor_on_tc(l)) { p.side = SIDE_PM1_S8; p.side_ld = (int)align_up(l.c, 32); }   // pad channels meet zero weights
             else if (p.variant == 1) { p.side = SIDE_BITS; p.side_ld = (l.c + 31) / 32; }
-            else if (p.variant == 2) { p.side = SIDE_S8; p.side_ld = (int)align_up(l.c, 32); }   // every INT8 layer fits the s8 wgmma tile
+            else if (p.variant == 2) {   // every INT8 layer fits the s8 wgmma tile
+                p.side = opt.rule == YB_QUANT_GPU ? SIDE_S8_SAT : SIDE_S8;
+                p.side_ld = (int)align_up(l.c, 32);
+            }
         }
 
         for (int i = 0; i < nl; ++i)
@@ -488,12 +499,14 @@ struct Builder {
         if (p.variant == 0) {
             int tc = (ADT == DT_BF16 && idt == DT_BF16) ? tc_conv_supported(tc_query) : 0;
             // float detection heads of the INT8 / XNOR networks (default precision): tf32 wgmma.  Only layers whose every
-            // reader is a yolo / region layer -- nothing they compute can reach an integer layer.
+            // reader is a yolo / region layer -- nothing they compute can reach an integer layer, which stays bit-exact
+            // against the CPU reference.  The GPU rule's float layers are cuDNN convolutions in the reference, which no
+            // summation order reproduces bit for bit: all of them that the tensor cores take run on tf32.
             if (ADT == DT_F32 && opt.precision == YB_PREC_BF16_TC && idt == DT_F32 && odt == DT_F32 && p.fused_into < 0 &&
                 !cons[i].empty() && !sw.no_tf32) {
                 bool heads_only = true;
                 for (int r : cons[i]) heads_only &= layer(r).type == YB_YOLO || layer(r).type == YB_REGION;
-                if (heads_only && tc_conv_supported(tc_query)) tc = 2;
+                if ((heads_only || opt.rule == YB_QUANT_GPU) && tc_conv_supported(tc_query)) tc = 2;
             }
             if (sw.no_tc) tc = 0;
             return tc == 2 ? CP_TF32 : tc ? CP_TC : CP_SIMT;
@@ -750,11 +763,12 @@ struct Builder {
         const Layer &l0 = layer(0);
         const int act = l0.activation, H = l0.h, W = l0.w;
         if (first == FIRST_STEM_POOL) {
-            // by layer 2's side format (SIDE_S8, SIDE_PM1_S8, SIDE_BITS) and the stem's activation
-            decltype(&k_stem_pool<SIDE_S8, ACT_LEAKY>) const k[3][2] = {
+            // by layer 2's side format (SIDE_S8, SIDE_PM1_S8, SIDE_BITS, SIDE_S8_SAT) and the stem's activation
+            decltype(&k_stem_pool<SIDE_S8, ACT_LEAKY>) const k[4][2] = {
                 {k_stem_pool<SIDE_S8, ACT_LEAKY>, k_stem_pool<SIDE_S8, ACT_LINEAR>},
                 {k_stem_pool<SIDE_PM1_S8, ACT_LEAKY>, k_stem_pool<SIDE_PM1_S8, ACT_LINEAR>},
-                {k_stem_pool<SIDE_BITS, ACT_LEAKY>, k_stem_pool<SIDE_BITS, ACT_LINEAR>}};
+                {k_stem_pool<SIDE_BITS, ACT_LEAKY>, k_stem_pool<SIDE_BITS, ACT_LINEAR>},
+                {k_stem_pool<SIDE_S8_SAT, ACT_LEAKY>, k_stem_pool<SIDE_S8_SAT, ACT_LINEAR>}};
             const Layer &c2 = layer(2);
             push_input_kernel(OP_CONV_SIMT, 0, k[L[2].side - SIDE_S8][act == ACT_LEAKY ? 0 : 1],
                               (unsigned)(((long)B * c2.h * c2.w + 127) / 128), 128, side_placed(2), stem_weights<16>(l0), act, H, W,
@@ -785,8 +799,9 @@ struct Builder {
     // k_int_input: convolution j's converted input from tin, behind a size x size / stride max-pool (1 / 1 / 0: the conversion
     // alone)
     void push_int_input(int kind, int i, int j, const TV &tin, int size, int stride, int pad) {
-        const SideFmt f = L[j].side;   // SIDE_S8, SIDE_PM1_S8 or SIDE_BITS
-        void (*const k[3])(TV, TV, int, int, int, float) = {k_int_input<SIDE_S8>, k_int_input<SIDE_PM1_S8>, k_int_input<SIDE_BITS>};
+        const SideFmt f = L[j].side;   // SIDE_S8, SIDE_PM1_S8, SIDE_BITS or SIDE_S8_SAT
+        void (*const k[4])(TV, TV, int, int, int, float) = {k_int_input<SIDE_S8>, k_int_input<SIDE_PM1_S8>, k_int_input<SIDE_BITS>,
+                                                            k_int_input<SIDE_S8_SAT>};
         const TV q = side_placed(j);
         push_kernel(kind, i, k[f - SIDE_S8], grid_for((long)B * q.H * q.W * int_input_groups(f, tin.C)), 256, 0, tin, q, size, stride, pad,
                     side_mult(j));
@@ -796,7 +811,7 @@ struct Builder {
         const TV tin = i == 0 ? e.in0 : e.out_tv[i - 1];   // no base where the input is fused away
         const SideFmt f = L[i].side;
         if (!L[i].prefilled && side_int(f))
-            push_int_input(f == SIDE_S8 ? OP_QUANTIZE : OP_BINARIZE, i, i, tin, 1, 1, 0);
+            push_int_input(side_s8(f) ? OP_QUANTIZE : OP_BINARIZE, i, i, tin, 1, 1, 0);
         if (L[i].variant == 0) emit_conv_fp32(i, tin);
         else if (L[i].variant == 1) emit_conv_xnor(i, tin);
         else emit_conv_int8(i);
@@ -819,7 +834,7 @@ struct Builder {
             sp.w = e.w_arena.get() + cw[i].w_bits;
             sp.mean = reinterpret_cast<const float *>(e.w_arena.get() + cw[i].mean);
             sp.bits = taps * l.c; sp.padbits = (sp.CW * 32 - l.c) * taps;
-        } else if (p.side == SIDE_S8) {
+        } else if (side_s8(p.side)) {
             sp.CW = p.side_ld / 4;
             sp.w = e.w_arena.get() + cw[i].w_s8;
             sp.alpha1 = alpha1(l);
@@ -905,7 +920,8 @@ struct Builder {
     void emit_conv_int8(int i) {
         counts_buffer(i);   // allocated before the tensor-core plan, which takes its address
         if (L[i].path == CP_I8_TC) push_tc_plan(OP_CONV_TC_I8, i);
-        else push_conv_simt(OP_CONV_INT8, i, k_conv_simt<SimtInt8>, side_placed(i), e.out_tv[i]);
+        else push_conv_simt(OP_CONV_INT8, i, opt.rule == YB_QUANT_GPU ? k_conv_simt<SimtInt8Gpu> : k_conv_simt<SimtInt8>, side_placed(i),
+                            e.out_tv[i]);
     }
 
     // max-pool, upsample, shortcut, route, reorg, yolo, region

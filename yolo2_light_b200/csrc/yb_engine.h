@@ -21,10 +21,10 @@ enum OpKind {
 struct EngineOptions {
     int device = 0;
     int precision = YB_PREC_BF16_TC;
-    bool qrule = false;        // yolov2_forward_network_q layer rule
+    int rule = YB_QUANT_NONE;  // INT8 layer rule: none, the CPU build's (yolov2_forward_network_q) or the GPU build's (l.quantized)
     bool fuse = true;          // conv + shortcut fusion, route aliasing (YB_NO_FUSE=1 turns it off in every engine)
     bool upload = true;        // upload the weight arena (false on non-root ranks before the broadcast)
-    int q_index_offset = 0;    // added to the layer index in the `i >= 1` INT8 rule (single-layer runs)
+    int q_index_offset = 0;    // added to the layer index in the `i >= 1` INT8 rule of YB_QUANT_CPU (single-layer runs)
     bool keep_counts = false;  // keep raw XNOR popcounts / INT8 accumulators (tests)
 };
 

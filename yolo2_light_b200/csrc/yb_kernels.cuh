@@ -280,6 +280,7 @@ static __global__ void __launch_bounds__(RS_THREADS) k_resize_frames(const Image
 //       out = xnor_epilogue(2*count - K, mean[f], bias[f]).  XNOR layers off the s8 wgmma with more than 2 words per tap.
 //   SimtInt8  words of 4 s8 values (reference yolov2_forward_network_quantized.c:527-631): acc32 = sum xq*wq (dp4a, exact),
 //       out = int8_epilogue(acc32).  INT8 layers the s8 wgmma tile refuses.
+//   SimtInt8Gpu  the same GEMM, out = int8_gpu_epilogue(acc32): the INT8 layers of the GPU rule the s8 wgmma tile refuses.
 // The integer inputs are written by k_int_input or by the fused kernels in front of the convolution.
 // ------------------------------------------------------------------------------------------------------
 struct SimtP {
@@ -287,7 +288,7 @@ struct SimtP {
     const void *w;             // f32: [K][ldw], ldw = filters rounded up to 64; integer: [filters rounded up to 64][K] words
     const float *bias;
     const float *mean;         // XNOR
-    float alpha1;              // INT8
+    float alpha1;              // INT8: ALPHA1 of the rule's epilogue
     int n;                     // filters
     int ldw;
     int size, stride, pad;
@@ -400,6 +401,12 @@ struct SimtInt8 : SimtWords<int8_t, 0u> {
     static __device__ __forceinline__ int raw(const SimtP &, int acc) { return acc; }
     static __device__ __forceinline__ float finish(const SimtP &p, int acc, int f, const float *) {
         return int8_epilogue(acc, p.alpha1, p.bias[f], p.act);
+    }
+};
+
+struct SimtInt8Gpu : SimtInt8 {
+    static __device__ __forceinline__ float finish(const SimtP &p, int acc, int f, const float *) {
+        return int8_gpu_epilogue(acc, p.alpha1, p.bias[f], p.act);
     }
 };
 
@@ -825,7 +832,7 @@ __device__ __forceinline__ unsigned long long f2_add(unsigned long long a, unsig
 // output (709 MB at 416x416 batch 64) is written once and read once just to be reduced 4:1 and narrowed to one byte (or bit)
 // per value.  One thread per POOLED pixel: the 4x4x3 input window (48 loads), four stem outputs x 16 filters in the
 // reference's exact order (c, ky, kx; separately rounded products and sums: k_conv_stem<EXACT>), bias + activation, the
-// reference's max (forward_maxpool_layer_avx scalar semantics: -FLT_MAX start, strict >), then quant_i8 / sign exactly as
+// reference's max (forward_maxpool_layer_avx scalar semantics: -FLT_MAX start, strict >), then quant_i8 / quant_i8_sat / sign exactly as
 // k_int_input, in the side format F of the integer layer.  Bit-identical to the three separate kernels.  s8 formats: q.ldc bytes
 // per pixel, of which the first 16 are written; sign bits: one word per pixel.
 // ------------------------------------------------------------------------------------------------------

@@ -20,8 +20,7 @@ void fatal_throw(const std::string &msg) { throw Error{msg}; }
 // Every host `Layer::output` points into pinned memory owned by an Engine: whenever the engines go, those pointers go
 // with them (a stale non-null pointer would make get_boxes / yb_network_layer_output read freed memory).
 void drop_engines(Network *net) {
-    net->engine[0].reset();
-    net->engine[1].reset();
+    for (auto &e : net->engine) e.reset();
     for (Layer &l : net->layers) { l.output = nullptr; l.output_count = 0; }
 }
 

@@ -46,7 +46,7 @@ struct Network {
     std::vector<Layer> layers;
     int device = 0;
     int precision = YB_PREC_BF16_TC;
-    std::shared_ptr<Engine> engine[2];   // [0] fp32 rule, [1] -quantized rule
+    std::shared_ptr<Engine> engine[3];   // by INT8 rule: [YB_QUANT_NONE], [YB_QUANT_CPU], [YB_QUANT_GPU]
     int last_launches = 0;
     bool fuse = true;          // conv+shortcut fusion / route aliasing (diagnostic switch)
     bool keep_counts = false;  // keep raw XNOR popcounts / INT8 accumulators (tests)
@@ -72,7 +72,9 @@ void fuse_conv_batchnorm(Network *net);
 void calculate_binary_weights(Network *net);
 void quantinization_and_get_multipliers(Network *net);
 void set_batch(Network *net, int batch);
-void drop_engines(Network *net);   // resets both engines AND the host output pointers they own
+void drop_engines(Network *net);   // resets every rule's engine AND the host output pointers they own
+// the INT8 rule of a `quantized` argument: YB_QUANT_GPU for 2, YB_QUANT_CPU for any other non-zero value, else YB_QUANT_NONE
+inline int quant_rule(int quantized) { return quantized == YB_QUANT_GPU ? YB_QUANT_GPU : quantized ? YB_QUANT_CPU : YB_QUANT_NONE; }
 int get_boxes(const Network *net, int b, int w, int h, float thresh, float nms, int relative, int letter,
               float *out, int max_rows);
 
@@ -87,11 +89,11 @@ struct yb_network {
     yb::Network net;
     // multi-GPU batch extension (yb_network_predict_batch): replica engines [rule][k], k >= 1 (replica 0 is net.engine[rule]),
     // the device of every replica, and the gathered host outputs [layer] = nimg x layer.outputs floats
-    std::vector<std::shared_ptr<yb::Engine>> replicas[2];
+    std::vector<std::shared_ptr<yb::Engine>> replicas[3];
     std::vector<int> devices;
     std::string replication;                       // how the weights reached the replicas: "nccl" | "peer-copy" | "single"
     std::vector<std::vector<float>> batch_out;
     int batch_nimg = 0;
-    // single-layer networks of yb_forward_convolutional_layer, keyed by 2 * layer + variant (engines are built once)
+    // single-layer networks of yb_forward_convolutional_layer, keyed by 3 * layer + rule (engines are built once)
     std::map<int, std::unique_ptr<yb_network>> single;
 };
