@@ -8,6 +8,20 @@ import ctypes as C
 import numpy as np
 
 
+# (w, h) -> (nw, nh, dx, dy) in a 64 x 64 network: wide, tall, already its letterbox size, the network's aspect ratio,
+# an upscale with an odd margin, a target height of 2, and rows wider than the resize kernel stages in shared memory
+LETTERBOX_CASES = {
+    (640, 480): (64, 48, 0, 8),
+    (100, 300): (21, 64, 21, 0),
+    (64, 36): (64, 36, 0, 14),
+    (128, 128): (64, 64, 0, 0),
+    (35, 17): (64, 31, 0, 16),
+    (640, 20): (64, 2, 0, 31),
+    (4500, 400): (64, 5, 0, 29),
+}
+SIZES = list(LETTERBOX_CASES)
+
+
 def letterbox_size(netw, neth, w, h):
     """correct_yolo_boxes' integer letterbox size (additionally.c:4287-4294), the float compare done in float32 as C does."""
     if np.float32(netw) / np.float32(w) < np.float32(neth) / np.float32(h):

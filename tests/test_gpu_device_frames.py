@@ -7,7 +7,7 @@ import pytest
 
 import ybtest_util as util
 from device_frames_util import GOLDEN_NV12, LAYOUTS, device_frame, equivalent_host_frame, random_frame
-from test_gpu_frames import INPUT_SETS, _mixed_net
+from ybtest_util import INPUT_SETS, mixed_net
 
 pytestmark = pytest.mark.gpu
 
@@ -25,9 +25,7 @@ def _sets(fmt):
 @pytest.fixture(scope="module")
 def tiny(tmp_path_factory):
     import yolo2_light_b200 as yb
-    cfg, wts = util.model_files("tiny64", str(tmp_path_factory.mktemp("device_frames")))
-    net = yb.load_network(cfg, wts, batch=4)
-    net.set_precision(yb.YB_PREC_FP32)
+    net = util.load(*util.model_files("tiny64", str(tmp_path_factory.mktemp("device_frames"))), 4, precision=yb.YB_PREC_FP32)
     return net
 
 
@@ -67,7 +65,7 @@ DET_BATCHES = [[(120, 96), (64, 64), (32, 200)], [(300, 170)], [(64, 64), (2, 2)
 
 @pytest.mark.parametrize("kind", ["tiny64_fp32", "tiny64_bf16", "s2chain", "tiny64_q1", "xnor64"])
 def test_detections_equal_host_frames(kind, workdir):
-    net, q = _mixed_net(kind, workdir)
+    net, q = mixed_net(kind, workdir)
     rng = np.random.default_rng(17)
     total = 0
     for fmt in FORMATS:
@@ -97,7 +95,7 @@ def test_stream_ordering_with_the_producer(workdir):
     """The producer stream sleeps, writes the frames, submits them without synchronising and then overwrites them: the
     engine reads what was written before the call.  Device and host submits share the three slots of one network."""
     import torch
-    net, q = _mixed_net("s2chain", workdir)
+    net, q = mixed_net("s2chain", workdir)
     rng = np.random.default_rng(23)
     sizes = [(120, 96), (64, 64), (32, 200)]
     plan = ["rgb", "host", "nv12", "bgr", "host", "planar", "nv12"]

@@ -10,34 +10,18 @@ import numpy as np
 import pytest
 
 import ybtest_util as util
-from test_gpu_detect import _bigger, _sorted
-from test_gpu_tc import _files
-from test_gpu_tc_stride2 import s2chain
+from ybtest_util import INPUT_SETS, bigger, mixed_net, sorted_rows
 from yolo2_light_b200 import cfgs
 
 pytestmark = pytest.mark.gpu
-
-
-def _frames(sizes, seed):
-    rng = np.random.default_rng(seed)
-    return [rng.integers(0, 256, size=(h, w, 3), dtype=np.uint8) for w, h in sizes]
-
-
-# (w, h): 1 pixel wide, 1 pixel high, the network size (64), upscales, a >= 3x downscale, odd sizes, and a frame whose rows
-# are wider than the resize kernel stages in shared memory
-INPUT_SETS = [[(1, 40), (50, 1), (64, 64), (33, 17)],
-              [(200, 197), (97, 131), (4500, 5)],
-              [(7, 9)]]
 
 
 @pytest.mark.parametrize("k", range(len(INPUT_SETS)))
 def test_resized_input_equals_reference_resize(k, workdir):
     import yolo2_light_b200 as yb
     from oracle import port
-    cfg, wts = util.model_files("tiny64", workdir)
-    net = yb.load_network(cfg, wts, batch=4)
-    net.set_precision(yb.YB_PREC_FP32)
-    frames = _frames(INPUT_SETS[k], 100 + k)
+    net = util.load(*util.model_files("tiny64", workdir), 4, precision=yb.YB_PREC_FP32)
+    frames = util.frames(INPUT_SETS[k], 100 + k)
     net.predict_frames_u8(frames)
     got = net.fetch_input()
     for b, f in enumerate(frames):
@@ -47,27 +31,11 @@ def test_resized_input_equals_reference_resize(k, workdir):
     assert tail.size == 0 or np.array_equal(tail.view(np.uint32), np.zeros_like(tail.view(np.uint32)))
 
 
-def _mixed_net(kind, workdir):
-    import yolo2_light_b200 as yb
-    if kind == "s2chain":
-        secs = s2chain()
-        cfg, wts = _files(workdir, "frames_s2chain64", secs, 61)
-        net = yb.load_network(cfg, wts, batch=3)
-        net.set_precision(yb.YB_PREC_BF16_TC)
-        return net, False
-    name, q, prec = {"tiny64_fp32": ("tiny64", 0, yb.YB_PREC_FP32), "tiny64_bf16": ("tiny64", 0, yb.YB_PREC_BF16_TC),
-                     "tiny64_q1": ("tiny64", 1, yb.YB_PREC_BF16_TC), "xnor64": ("xnor64", 0, yb.YB_PREC_BF16_TC)}[kind]
-    cfg, wts = util.model_files(name, workdir)
-    net = yb.load_network(cfg, wts, batch=3, quantized=q)
-    net.set_precision(prec)
-    return net, bool(q)
-
-
 @pytest.mark.parametrize("kind", ["tiny64_fp32", "tiny64_bf16", "s2chain", "tiny64_q1", "xnor64"])
 def test_no_leakage_across_images(kind, workdir):
     """Image b of a mixed batch gives the detection tensors a batch of that frame alone gives."""
-    net, q = _mixed_net(kind, workdir)
-    frames = _frames([(120, 96), (64, 64), (31, 200)], 7)
+    net, q = mixed_net(kind, workdir)
+    frames = util.frames([(120, 96), (64, 64), (31, 200)], 7)
     net.predict_frames_u8(frames, quantized=q)
     mixed = {i: o.copy() for i, o in net.detection_outputs().items()}
     assert mixed
@@ -82,10 +50,8 @@ SIZES = [(640, 480), (1280, 720), (333, 999)]
 
 @pytest.mark.parametrize("relative,letter", [(0, 0), (0, 1), (1, 0), (1, 1)])
 def test_detect_frames_equals_host_decode_per_image(relative, letter, workdir):
-    import yolo2_light_b200 as yb
     B = 3
-    cfg, wts = _bigger("tiny", workdir, 160, 160)
-    net = yb.load_network(cfg, wts, batch=B)
+    net = util.load(*bigger("tiny", workdir, 160, 160), B)
     net.predict(cfgs.synthetic_images(B, 3, 160, 160, seed=43))
     for nimg in (3, 2):
         sizes = SIZES[:nimg]
@@ -94,7 +60,7 @@ def test_detect_frames_equals_host_decode_per_image(relative, letter, workdir):
         for b, (w, h) in enumerate(sizes):
             host = net.get_network_boxes(b, w, h, 0.2, 0.45, relative, letter)
             assert counts[b] == host.shape[0] > 0, (b, counts[b], host.shape)
-            a, e = _sorted(dets[b]), _sorted(host)
+            a, e = sorted_rows(dets[b]), sorted_rows(host)
             # boxes: double exp() on both sides, identical up to libm's last bit; probabilities: exact
             assert np.allclose(a[:, :4], e[:, :4], rtol=1e-6, atol=1e-7), b
             assert np.array_equal(a[:, 4:], e[:, 4:]), b
@@ -117,11 +83,10 @@ def test_detect_frames_vs_reference_per_image(workdir):
     test_gpu_detect.py::test_device_detect_vs_reference_boxes."""
     import yolo2_light_b200 as yb
     from oracle import ref
-    cfg, wts = _bigger("tiny", workdir, 160, 160)
-    net = yb.load_network(cfg, wts, batch=3)
-    net.set_precision(yb.YB_PREC_FP32)
+    cfg, wts = bigger("tiny", workdir, 160, 160)
+    net = util.load(cfg, wts, 3, precision=yb.YB_PREC_FP32)
     sizes = [(640, 480), (100, 300)]
-    frames = _frames(sizes, 45)
+    frames = util.frames(sizes, 45)
     net.predict_frames_u8(frames)
     dets, counts = net.detect_frames(sizes, 0.2, 0.45, max_rows=4096)
     rnet = ref.RefNet(cfg, wts, 1, 0, 7)
@@ -130,7 +95,7 @@ def test_detect_frames_vs_reference_per_image(workdir):
         theirs = np.delete(rnet.get_boxes(w, h, 0.2, 0.45), 5, axis=1)
         assert abs(int(counts[b]) - theirs.shape[0]) <= max(1, theirs.shape[0] // 100), (b, counts[b], theirs.shape)
         if counts[b] == theirs.shape[0] and theirs.shape[0]:
-            a, e = _sorted(dets[b]), _sorted(theirs)
+            a, e = sorted_rows(dets[b]), sorted_rows(theirs)
             assert np.allclose(a[:, :5], e[:, :5], rtol=1e-4, atol=1e-5)
             kept_a, kept_e = (a[:, 5:] > 0).sum(), (e[:, 5:] > 0).sum()
             assert abs(int(kept_a) - int(kept_e)) <= max(2, int(kept_e) // 50), (kept_a, kept_e)
@@ -144,9 +109,9 @@ PIPE_BATCHES = [[(120, 96), (64, 64), (31, 200)], [(64, 64)] * 3, [(300, 170)], 
 
 @pytest.mark.parametrize("kind", ["s2chain", "tiny64_q1"])
 def test_pipelined_frames_equal_sync_calls(kind, workdir):
-    net, q = _mixed_net(kind, workdir)
+    net, q = mixed_net(kind, workdir)
     thresh = 0.3
-    batches = [_frames(sizes, 200 + k) for k, sizes in enumerate(PIPE_BATCHES)]
+    batches = [util.frames(sizes, 200 + k) for k, sizes in enumerate(PIPE_BATCHES)]
     exp = []
     for fr in batches:
         net.predict_frames_u8(fr, quantized=q)
@@ -170,8 +135,8 @@ def test_pipelined_frames_equal_sync_calls(kind, workdir):
 
 @pytest.mark.parametrize("fw,fh", [(64, 64), (120, 96)])
 def test_uniform_frames_equal_submit_u8(fw, fh, workdir):
-    net, q = _mixed_net("s2chain", workdir)
-    stacked = np.stack(_frames([(fw, fh)] * net.batch, 9))
+    net, q = mixed_net("s2chain", workdir)
+    stacked = np.stack(util.frames([(fw, fh)] * net.batch, 9))
     t = net.submit_u8(stacked, 0.3, 0.45, relative=0, max_rows=2048)
     de, ce, me = net.collect_detections(t)
     t = net.submit_frames_u8(list(stacked), 0.3, 0.45, relative=0, max_rows=2048)
@@ -187,14 +152,12 @@ def test_map_mixed_sizes_equals_validate_detector_map(workdir):
     images at batch 2 take 4 forwards, not 7; TP / FP / FN and mAP as the reference's validate_detector_map."""
     import yolo2_light_b200 as yb
     from yolo2_light_b200 import dataset
-    from test_map import test_map_accounting_equals_reference
     cfg, wts = util.model_files("tiny64", workdir)
     root = os.path.join(workdir, "mapset_tiny64_50")
     if not os.path.exists(os.path.join(root, "ref_stdout.txt")):
-        test_map_accounting_equals_reference("tiny64", 0.5, workdir)
+        util.check_map_accounting("tiny64", 0.5, workdir)
     paths, names, truth = dataset.load_validation_set(os.path.join(root, "data.cfg"))
-    net = yb.load_network(cfg, wts, batch=2)
-    net.set_precision(yb.YB_PREC_FP32)
+    net = util.load(cfg, wts, 2, precision=yb.YB_PREC_FP32)
 
     class Counting:
         batch = net.batch

@@ -11,15 +11,6 @@ from yolo2_light_b200 import cfgs
 pytestmark = pytest.mark.gpu
 
 
-def _files(workdir, name, secs, seed=1):
-    cfg = os.path.join(workdir, name + ".cfg")
-    wts = os.path.join(workdir, name + ".weights")
-    if not os.path.exists(cfg):
-        cfgs.write_cfg(secs, cfg)
-        cfgs.write_weights(secs, wts, seed=seed)
-    return cfg, wts
-
-
 def _ref_outputs(cfg, wts, x, q, kind):
     from oracle import ref
     os.environ.setdefault("OMP_NUM_THREADS", str(min(os.cpu_count() or 1, 32)))
@@ -36,11 +27,10 @@ def test_yolov3_608_bf16_tensor_core_vs_reference(workdir):
     activated yolo tensors, SURVEY 7.3) against the reference CPU path on the same weights and images: on a stored seeded
     sample of every tensor (tests/golden/v3_608_sample.npz, tests/golden/make_golden.py), and on the whole tensors when the
     reference build is present."""
-    import yolo2_light_b200 as yb
     secs = cfgs.yolov3(608, 608)
-    cfg, wts = _files(workdir, "yolov3_608", secs)
+    cfg, wts = util.write_net(workdir, "yolov3_608", secs, 1)
     x = cfgs.synthetic_images(2, 3, 608, 608)
-    net = yb.load_network(cfg, wts, batch=2)
+    net = util.load(cfg, wts, 2)
     net.predict(x)
     outs = net.detection_outputs()
     g = np.load(os.path.join(util.GOLDEN, "v3_608_sample.npz"))
@@ -61,17 +51,16 @@ def test_yolov3_608_bf16_tensor_core_vs_reference(workdir):
 
 @pytest.mark.skipif(not util.have_ref(), reason="oracle/_ref not built")
 def test_yolov3_tiny_416_fp32_and_int8_vs_reference(workdir):
-    import yolo2_light_b200 as yb
     secs = cfgs.yolov3_tiny(416, 416)
-    cfg, wts = _files(workdir, "tiny_416", secs)
+    cfg, wts = util.write_net(workdir, "tiny_416", secs, 1)
     x = cfgs.synthetic_images(2, 3, 416, 416)
-    net = yb.load_network(cfg, wts, batch=2)
+    net = util.load(cfg, wts, 2)
     net.predict(x)
     exp = _ref_outputs(cfg, wts, x, 0, "fast")
     for i, o in net.detection_outputs().items():
         for b in range(2):
             assert util.rel_l2(o[b], exp[b][i].reshape(o[b].shape)) <= 1e-3, (i, b)
-    netq = yb.load_network(cfg, wts, batch=2, quantized=1)
+    netq = util.load(cfg, wts, 2, quantized=1)
     netq.predict(x, quantized=True)
     kinds = [k for _, k, _ in netq.profile(quantized=True)]
     assert kinds.count("conv_tc_i8") >= 8, kinds   # the s8 x s8 -> s32 wgmma path carries the INT8 layers
@@ -83,11 +72,10 @@ def test_yolov3_tiny_416_fp32_and_int8_vs_reference(workdir):
 
 @pytest.mark.skipif(not util.have_ref(), reason="oracle/_ref not built")
 def test_xnor_416_vs_reference(workdir):
-    import yolo2_light_b200 as yb
     secs = cfgs.tiny_yolo_obj_xnor(416, 416)
-    cfg, wts = _files(workdir, "xnor_416", secs, seed=2)
+    cfg, wts = util.write_net(workdir, "xnor_416", secs, 2)
     x = cfgs.synthetic_images(2, 3, 416, 416)
-    net = yb.load_network(cfg, wts, batch=2)
+    net = util.load(cfg, wts, 2)
     net.predict(x)
     exp = _ref_outputs(cfg, wts, x, 0, "scalar")
     for i, o in net.detection_outputs().items():
@@ -98,18 +86,17 @@ def test_xnor_416_vs_reference(workdir):
 def test_batch_invariance_and_determinism_at_full_size(workdir):
     """Images are independent: image k of a batch of 16 == the same image run in a batch of 1 (bit-for-bit: the
     kernels' reduction order does not depend on the batch), and two runs of the same batch are identical."""
-    import yolo2_light_b200 as yb
     secs = cfgs.yolov3(608, 608)
-    cfg, wts = _files(workdir, "yolov3_608", secs)
+    cfg, wts = util.write_net(workdir, "yolov3_608", secs, 1)
     x = cfgs.synthetic_images(16, 3, 608, 608)
-    net = yb.load_network(cfg, wts, batch=16)
+    net = util.load(cfg, wts, 16)
     net.predict(x)
     a = {i: o.copy() for i, o in net.detection_outputs().items()}
     net.predict(x)
     for i, o in net.detection_outputs().items():
         assert util.bits_equal(o, a[i])
         assert np.isfinite(o).all()
-    one = yb.load_network(cfg, wts, batch=1)
+    one = util.load(cfg, wts, 1)
     for k in (0, 7, 15):
         one.predict(x[k:k + 1])
         for i, o in one.detection_outputs().items():
@@ -121,12 +108,11 @@ def test_spp_608_runs_and_matches_f32_cuda_core_path(workdir):
     (which the slim-model tests pin to the oracle); covers the 5/9/13 max-pools and the 4-way concat at 19x19."""
     import yolo2_light_b200 as yb
     secs = cfgs.yolov3_spp(608, 608)
-    cfg, wts = _files(workdir, "spp_608", secs, seed=3)
+    cfg, wts = util.write_net(workdir, "spp_608", secs, 3)
     x = cfgs.synthetic_images(2, 3, 608, 608)
-    a = yb.load_network(cfg, wts, batch=2)
+    a = util.load(cfg, wts, 2)
     a.predict(x)
-    b = yb.load_network(cfg, wts, batch=2)
-    b.set_precision(yb.YB_PREC_FP32)
+    b = util.load(cfg, wts, 2, precision=yb.YB_PREC_FP32)
     b.predict(x)
     for i, o in a.detection_outputs().items():
         assert util.rel_l2(o, b.layer_output(i)) <= 1e-3, i
@@ -137,9 +123,9 @@ def test_pipelined_submit_collect_equals_predict(workdir):
     synchronous predict returns, batch after batch, including when slots are reused."""
     import yolo2_light_b200 as yb
     secs = cfgs.yolov3_tiny(416, 416)
-    cfg, wts = _files(workdir, "tiny_416", secs)
+    cfg, wts = util.write_net(workdir, "tiny_416", secs, 1)
     B = 4
-    net = yb.load_network(cfg, wts, batch=B)
+    net = util.load(cfg, wts, B)
     batches = [cfgs.synthetic_images(B, 3, 416, 416, seed=100 + 10 * k) for k in range(7)]
     expect = []
     for x in batches:
@@ -182,11 +168,9 @@ def test_c3_int8_layers_bit_exact_at_full_shape(layer, workdir):
     """yolov3-tiny 416 -quantized, batch 64 (BASELINE configs[2]): conv `layer` alone on the GPU at its real shape (K up to 4608,
     multi-wave tiles, several filter tiles) against the oracle on three images of the batch: s32 accumulators identical, float outputs
     bit-identical, including outputs that hit the int16 saturation."""
-    import yolo2_light_b200 as yb
     from oracle import port
     B = 64
-    cfg, wts = _files(workdir, "tiny_416", cfgs.yolov3_tiny(416, 416))
-    net = yb.load_network(cfg, wts, batch=B, quantized=1)
+    net = util.load(*util.write_net(workdir, "tiny_416", cfgs.yolov3_tiny(416, 416), 1), B, quantized=1)
     l = net.layers[layer]
     rng = np.random.default_rng(700 + layer)
     x = _saturating_input(l, B, rng, image=31)
@@ -210,11 +194,9 @@ def test_c3_int8_layers_bit_exact_at_full_shape(layer, workdir):
 def test_c4_xnor_layers_bit_exact_at_full_shape(layer, workdir):
     """tiny-yolo-obj_xnor 416, batch 64 (BASELINE configs[3]): every XNOR layer class at its real shape (K up to 9216) --
     popcount kernels for the narrow layers, +-1 on the s8 wgmma for the wide ones -- against the oracle on three images."""
-    import yolo2_light_b200 as yb
     from oracle import port
     B = 64
-    cfg, wts = _files(workdir, "xnor_416", cfgs.tiny_yolo_obj_xnor(416, 416))
-    net = yb.load_network(cfg, wts, batch=B)
+    net = util.load(*util.write_net(workdir, "xnor_416", cfgs.tiny_yolo_obj_xnor(416, 416), 2), B)
     l = net.layers[layer]
     assert l["xnor"]
     rng = np.random.default_rng(800 + layer)
@@ -229,13 +211,12 @@ def test_c4_xnor_layers_bit_exact_at_full_shape(layer, workdir):
 def test_c4_all_popcount_configuration(workdir, monkeypatch):
     """YB_XNOR_TC=0: every XNOR layer on the xor + __popc kernels (what north_star describes), whole network bit-identical to the
     default configuration (wide layers as +-1 on the tensor cores) on every XNOR layer's output."""
-    import yolo2_light_b200 as yb
-    cfg, wts = _files(workdir, "xnor_416", cfgs.tiny_yolo_obj_xnor(416, 416))
+    cfg, wts = util.write_net(workdir, "xnor_416", cfgs.tiny_yolo_obj_xnor(416, 416), 2)
     B = 4
     x = cfgs.synthetic_images(B, 3, 416, 416, seed=5)
-    a = yb.load_network(cfg, wts, batch=B); a.set_option("fuse", 0); a.predict(x)
+    a = util.load(cfg, wts, B, fuse=0); a.predict(x)
     monkeypatch.setenv("YB_XNOR_TC", "0")
-    b = yb.load_network(cfg, wts, batch=B); b.set_option("fuse", 0); b.predict(x)
+    b = util.load(cfg, wts, B, fuse=0); b.predict(x)
     kinds = {k for _, k, _ in b.profile()}
     assert "conv_xnor" in kinds and "conv_tc_i8" not in kinds
     assert "conv_tc_i8" in {k for _, k, _ in a.profile()}
@@ -259,11 +240,10 @@ def test_spp_608_against_scalar_reference(workdir):
     import yolo2_light_b200 as yb
     from oracle import ref
     secs = cfgs.yolov3_spp(608, 608)
-    cfg, wts = _files(workdir, "spp_608", secs)
+    cfg, wts = util.write_net(workdir, "spp_608", secs, 3)
     x = cfgs.synthetic_images(1, 3, 608, 608, seed=11)
-    net = yb.load_network(cfg, wts, batch=1)
-    net.set_precision(yb.YB_PREC_FP32)            # f32 engine: data-movement layers are then comparable bit for bit
-    net.set_option("fuse", 0)
+    # f32 engine: data-movement layers are then comparable bit for bit
+    net = util.load(cfg, wts, 1, precision=yb.YB_PREC_FP32, fuse=0)
     net.predict(x)
     rnet = ref.RefNet(cfg, wts, 1, 0, 7, kind="scalar")
     types = [L["type_name"] for L in rnet.layers]
@@ -284,7 +264,7 @@ def test_spp_608_against_scalar_reference(workdir):
     assert rnet.layers[first_pool + 5]["out_c"] == 2048
     # default precision (bf16 tensor cores), the whole network against the reference's scalar CPU path on the same image
     # (~1 minute of single-thread CPU): FP32-variant bar of north_star, <= 1e-3 rel on the activated detection tensors
-    fast = yb.load_network(cfg, wts, batch=1)
+    fast = util.load(cfg, wts, 1)
     fast.predict(x)
     rnet.predict(x)
     n = 0

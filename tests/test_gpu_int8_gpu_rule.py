@@ -2,8 +2,6 @@
 parser's l.quantized, with the saturating input conversion and the unscaled epilogue; everything else as in the float forward
 with f32 activations.  Checked bit for bit against the oracle's run_network_gpu (tests/gpu_rule_oracle.py) at YB_PREC_FP32, and against the
 oracle's INT8 convolution on the engine's own inputs at the default precision, where the float layers run on tf32.  GPU box only."""
-import os
-
 import numpy as np
 import pytest
 
@@ -15,45 +13,12 @@ pytestmark = pytest.mark.gpu
 Q = 2
 
 
-def _files(name, secs, workdir, seed):
-    cfg = cfgs.write_cfg(secs, os.path.join(workdir, name + ".cfg"))
-    wts = cfgs.write_weights(secs, os.path.join(workdir, name + ".weights"), seed=seed)
-    return cfg, wts
-
-
-def _load(cfg, wts, B, precision=None, **opts):
-    import yolo2_light_b200 as yb
-    net = yb.load_network(cfg, wts, batch=B, quantized=1)
-    if precision is not None:
-        net.set_precision(precision)
-    for k, v in opts.items():
-        net.set_option(k, int(v))
-    return net
-
-
 def _int8_layers(net):
     return [i for i, l in enumerate(net.layers) if l["type_name"] == "CONVOLUTIONAL" and l["quantized"]]
 
 
-def _conv_gpu(l, x, want_acc=False):
-    return gro.conv_int8_gpu(x, l["weights_int8"], l["biases"], l["input_quant_multipler"], l["weights_quant_multipler"],
-                              l["n"], l["size"], l["stride"], l["pad"], l["activation"], want_acc=want_acc)
-
-
-def _fetch_all(net):
-    """every layer output the engine materialises, by index"""
-    import yolo2_light_b200 as yb
-    got = {}
-    for i in range(net.n):
-        try:
-            got[i] = net.fetch_layer(i, quantized=Q)
-        except yb.YbError:
-            pass
-    return got
-
-
 def _assert_bit_exact(net, outs, need=()):
-    got = _fetch_all(net)
+    got = util.fetch_all(net, Q)
     for i in need:
         assert i in got, i
     for i, o in got.items():
@@ -66,7 +31,7 @@ def _assert_bit_exact(net, outs, need=()):
 @pytest.fixture(scope="module")
 def tiny416(tmp_path_factory):
     d = str(tmp_path_factory.mktemp("tiny416"))
-    cfg, wts = _files("tiny416", cfgs.yolov3_tiny(416, 416), d, 41)
+    cfg, wts = util.write_net(d, "tiny416", cfgs.yolov3_tiny(416, 416), 41)
     x = cfgs.synthetic_images(4, 3, 416, 416, seed=42)
     return cfg, wts, x
 
@@ -77,13 +42,13 @@ def test_yolov3_tiny_416_fp32_bit_exact(tiny416):
     import yolo2_light_b200 as yb
     from oracle import port
     cfg, wts, x = tiny416
-    net = _load(cfg, wts, 4, yb.YB_PREC_FP32, fuse=0, keep_counts=1)
+    net = util.load(cfg, wts, 4, quantized=1, precision=yb.YB_PREC_FP32, fuse=0, keep_counts=True)
     assert _int8_layers(net) == [2, 4, 6, 8, 10, 12]
     net.predict(x, quantized=Q)
     layers = net.layers
     outs = gro.run_network_gpu(layers, x)
     for i in _int8_layers(net):
-        _, acc = _conv_gpu(layers[i], outs[i - 1], want_acc=True)
+        _, acc = util.oracle_layer(layers[i], i, outs[i - 1], Q)
         assert np.array_equal(net.fetch_counts(i, quantized=Q), acc), i
     got = _assert_bit_exact(net, outs)
     assert len(got) >= 20
@@ -97,19 +62,20 @@ def test_yolov3_tiny_416_default_precision(tiny416):
     float convolution but the 3-channel stem runs on tf32; the yolo tensors stay within rel-L2 1e-3 of YB_PREC_FP32."""
     import yolo2_light_b200 as yb
     cfg, wts, x = tiny416
-    net = _load(cfg, wts, 4, fuse=0)
+    net = util.load(cfg, wts, 4, quantized=1, fuse=0)
     net.predict(x, quantized=Q)
     layers = net.layers
     for i in _int8_layers(net):
-        assert util.bits_equal(net.fetch_layer(i, quantized=Q), _conv_gpu(layers[i], net.fetch_layer(i - 1, quantized=Q))), i
+        exp, _ = util.oracle_layer(layers[i], i, net.fetch_layer(i - 1, quantized=Q), Q)
+        assert util.bits_equal(net.fetch_layer(i, quantized=Q), exp), i
         assert net.tc_plan(i, quantized=Q)["kind"] == "s8_gpu", i
     floats = [i for i, l in enumerate(layers) if l["type_name"] == "CONVOLUTIONAL" and not l["quantized"] and i > 0]
     assert floats == [13, 14, 15, 18, 21, 22]
     for i in floats:
         assert net.tc_plan(i, quantized=Q)["kind"] == "tf32", i
-    fused = _load(cfg, wts, 4)            # the production engine: every fusion on
+    fused = util.load(cfg, wts, 4, quantized=1)            # the production engine: every fusion on
     fused.predict(x, quantized=Q)
-    exact = _load(cfg, wts, 4, yb.YB_PREC_FP32)
+    exact = util.load(cfg, wts, 4, quantized=1, precision=yb.YB_PREC_FP32)
     exact.predict(x, quantized=Q)
     ref = exact.detection_outputs()
     for i, o in fused.detection_outputs().items():
@@ -138,7 +104,7 @@ def _edge_secs(calib):
 def edge_net(tmp_path_factory):
     d = str(tmp_path_factory.mktemp("edges"))
     # large images and multipliers: every INT8 layer's input has values with |x * m| >= 32768
-    cfg, wts = _files("gpu_rule_edges", _edge_secs([2048, 2048, 2 ** 20, 2 ** 20, 2 ** 20, 16, 16]), d, 43)
+    cfg, wts = util.write_net(d, "gpu_rule_edges", _edge_secs([2048, 2048, 2 ** 20, 2 ** 20, 2 ** 20, 16, 16]), 43)
     x = cfgs.synthetic_images(3, 3, 32, 32, seed=44) * np.float32(40)
     return cfg, wts, x
 
@@ -152,7 +118,7 @@ def test_edges_bit_exact(mode, edge_net, monkeypatch):
         monkeypatch.setenv("YB_NO_TC", "1")
     if mode == "grid2":
         monkeypatch.setenv("YB_TC_GRID", "2")
-    net = _load(cfg, wts, 3, yb.YB_PREC_FP32)
+    net = util.load(cfg, wts, 3, quantized=1, precision=yb.YB_PREC_FP32)
     assert _int8_layers(net) == [1, 2, 4, 5]
     net.predict(x, quantized=Q)
     layers = net.layers
@@ -178,10 +144,10 @@ def test_rules_coexist_on_one_network(workdir):
     """Predicting with rules 1, 2, 1 on one yb_network leaves rule 1's outputs bit-identical to a fresh network's."""
     cfg, wts = util.model_files("tiny64", workdir)
     x = util.images("tiny64", 2)
-    fresh = _load(cfg, wts, 2)
+    fresh = util.load(cfg, wts, 2, quantized=1)
     fresh.predict(x, quantized=1)
     ref = fresh.detection_outputs()
-    net = _load(cfg, wts, 2)
+    net = util.load(cfg, wts, 2, quantized=1)
     net.predict(x, quantized=1)
     net.predict(x, quantized=Q)
     two = net.detection_outputs()
@@ -195,7 +161,7 @@ def test_serving_and_multi_gpu(workdir):
     """submit_frames_u8 with rule 2 returns the rows of detect after predict_frames_u8 with rule 2; predict_batch over a
     repeated device list equals the one-GPU call."""
     cfg, wts = util.model_files("tiny64", workdir)
-    net = _load(cfg, wts, 2)
+    net = util.load(cfg, wts, 2, quantized=1)
     rng = np.random.default_rng(5)
     frames = [rng.integers(0, 256, (64, 64, 3), dtype=np.uint8), rng.integers(0, 256, (96, 80, 3), dtype=np.uint8)]
     net.predict_frames_u8(frames, quantized=Q)
@@ -207,9 +173,9 @@ def test_serving_and_multi_gpu(workdir):
         assert util.bits_equal(exp[b], got[b]), b
 
     x = cfgs.synthetic_images(5, 3, 64, 64, seed=8)
-    one = _load(cfg, wts, 2)
+    one = util.load(cfg, wts, 2, quantized=1)
     r1 = one.predict_batch(x, 1, quantized=Q)
-    rep = _load(cfg, wts, 2)
+    rep = util.load(cfg, wts, 2, quantized=1)
     rep.set_devices([0, 0])
     r2 = rep.predict_batch(x, 2, quantized=Q)
     assert r1.keys() == r2.keys()
@@ -225,13 +191,12 @@ def test_true_dropin_gpu_rule_behind_reference_host_code(workdir):
     the cfg is parsed with quantized = 2 -- the reference treats every non-zero value alike, and its l.quantized flags are
     those of a quantized = 1 parse.  The last layer's yolo tensor is the oracle's GPU rule within the tf32 bar: the glue runs
     the default precision, where the float layers behind the INT8 ones take tf32."""
-    import yolo2_light_b200 as yb
     from oracle import port, ref
     cfg, wts = util.model_files("tiny64", workdir)
     x = util.images("tiny64", 1)
     rnet = ref.RefNet(cfg, wts, 1, Q, 7, kind="dropin")
     assert rnet.layers[-1]["type_name"] == "YOLO"
-    mine = yb.load_network(cfg, wts, batch=1, quantized=1)
+    mine = util.load(cfg, wts, 1, quantized=1)
     assert [i for i, L in enumerate(rnet.layers) if L["type_name"] == "CONVOLUTIONAL" and L["quantized"]] == _int8_layers(mine)
     got = rnet.predict_b200_batch(x, 1)
     outs = gro.run_network_gpu(mine.layers, x)
@@ -247,9 +212,9 @@ def test_yolov3_608_batch2(tmp_path_factory):
     YB_PREC_FP32, within rel-L2 1e-3 of that at the default precision."""
     import yolo2_light_b200 as yb
     d = str(tmp_path_factory.mktemp("v3_608"))
-    cfg, wts = _files("v3_608", cfgs.yolov3(608, 608), d, 45)
+    cfg, wts = util.write_net(d, "v3_608", cfgs.yolov3(608, 608), 45)
     x = cfgs.synthetic_images(2, 3, 608, 608, seed=46)
-    exact = _load(cfg, wts, 2, yb.YB_PREC_FP32)
+    exact = util.load(cfg, wts, 2, quantized=1, precision=yb.YB_PREC_FP32)
     q = _int8_layers(exact)
     assert len(q) == 26 and q[0] == 1 and max(q) == 78
     exact.predict(x, quantized=Q)
@@ -257,7 +222,7 @@ def test_yolov3_608_batch2(tmp_path_factory):
     outs = gro.run_network_gpu(exact.layers, x)
     for i, o in ref_out.items():
         assert util.bits_equal(o, outs[i].reshape(o.shape)), i
-    fast = _load(cfg, wts, 2)
+    fast = util.load(cfg, wts, 2, quantized=1)
     fast.predict(x, quantized=Q)
     for i, o in fast.detection_outputs().items():
         err = util.rel_l2(o, ref_out[i])

@@ -1,11 +1,10 @@
 """The input conversion of an integer convolution (k_int_input) reading a channel slice of a route's buffer at an offset that is
 not a multiple of 4 floats: the view is not 16-byte aligned, so the kernel must take its scalar loads, standalone and behind a
 2x2 max-pool alike.  GPU box only."""
-import os
-
 import numpy as np
 import pytest
 
+import ybtest_util as util
 from yolo2_light_b200 import cfgs
 
 pytestmark = pytest.mark.gpu
@@ -26,20 +25,14 @@ def _secs(kind, pooled):
 @pytest.mark.parametrize("pooled", [False, True])
 @pytest.mark.parametrize("kind", ["int8", "xnor"])
 def test_int_input_of_an_unaligned_channel_slice(kind, pooled, workdir):
-    import yolo2_light_b200 as yb
     q = kind == "int8"
-    secs = _secs(kind, pooled)
-    name = f"int_side_{kind}_{int(pooled)}"
-    cfg = cfgs.write_cfg(secs, os.path.join(workdir, name + ".cfg"))
-    wts = cfgs.write_weights(secs, os.path.join(workdir, name + ".weights"), seed=31)
+    cfg, wts = util.write_net(workdir, f"int_side_{kind}_{int(pooled)}", _secs(kind, pooled), 31)
     B = 2
     x = cfgs.synthetic_images(B, 3, 16, 16, seed=32)
     ic = 3 if pooled else 2          # the integer convolution behind conv B
     res = []
     for fuse in (0, 1):
-        net = yb.load_network(cfg, wts, batch=B, quantized=int(q))
-        net.set_option("fuse", fuse)
-        net.set_option("keep_counts", 1)
+        net = util.load(cfg, wts, B, quantized=int(q), fuse=fuse, keep_counts=True)
         net.predict(x, quantized=q)
         ops = [(li, k) for li, k, _ in net.profile(quantized=q)]
         ints = [i for i, l in enumerate(net.layers)

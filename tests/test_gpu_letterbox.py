@@ -9,10 +9,8 @@ import pytest
 
 import ybtest_util as util
 from device_frames_util import device_frame, equivalent_host_frame, random_frame
-from letterbox_util import port_letterbox_u8, ref_boxes, ref_letterbox_u8
-from test_gpu_detect import _bigger, _sorted
-from test_gpu_frames import _frames, _mixed_net
-from test_letterbox_oracle import SIZES
+from letterbox_util import SIZES, port_letterbox_u8, ref_boxes, ref_letterbox_u8
+from ybtest_util import bigger, mixed_net, sorted_rows
 
 pytestmark = pytest.mark.gpu
 
@@ -29,9 +27,7 @@ EVEN_SETS = [[(640, 480), (100, 300), (64, 36), (128, 128)],
 @pytest.fixture(scope="module")
 def tiny(tmp_path_factory):
     import yolo2_light_b200 as yb
-    cfg, wts = util.model_files("tiny64", str(tmp_path_factory.mktemp("letterbox")))
-    net = yb.load_network(cfg, wts, batch=4)
-    net.set_precision(yb.YB_PREC_FP32)
+    net = util.load(*util.model_files("tiny64", str(tmp_path_factory.mktemp("letterbox"))), 4, precision=yb.YB_PREC_FP32)
     net.set_letterbox(True)
     return net
 
@@ -43,7 +39,7 @@ def test_size_list_covers_every_case():
 
 @pytest.mark.parametrize("k", range(len(HOST_SETS)))
 def test_letterboxed_input_equals_oracle(tiny, k):
-    frames = _frames(HOST_SETS[k], 500 + k)
+    frames = util.frames(HOST_SETS[k], 500 + k)
     tiny.predict_frames_u8(frames)
     got = tiny.fetch_input()
     for b, f in enumerate(frames):
@@ -54,7 +50,7 @@ def test_letterboxed_input_equals_oracle(tiny, k):
 
 
 def test_one_size_call_letterboxes(tiny):
-    frames = np.stack(_frames([(100, 300)] * tiny.batch, 77))
+    frames = np.stack(util.frames([(100, 300)] * tiny.batch, 77))
     tiny.predict_image_u8(frames)
     got = tiny.fetch_input()
     for b in range(tiny.batch):
@@ -83,8 +79,8 @@ ASPECT = [(64, 64), (128, 128), (32, 32)]
 def test_network_aspect_frames_unchanged_by_letterbox(kind, workdir):
     """Frames of the network's aspect ratio letterbox to the network size at (0, 0): the input, the detection tensors and
     the pipelined rows (the 8-bit stem reads network-size batches directly on s2chain) are those of the stretched path."""
-    net, q = _mixed_net(kind, workdir)
-    batches = [_frames(ASPECT, 31), _frames([(64, 64)] * 3, 32), _frames([(64, 64), (32, 32)], 33)]
+    net, q = mixed_net(kind, workdir)
+    batches = [util.frames(ASPECT, 31), util.frames([(64, 64)] * 3, 32), util.frames([(64, 64), (32, 32)], 33)]
     res = {}
     for on in (False, True):
         net.set_letterbox(on)
@@ -111,12 +107,11 @@ def test_letterboxed_detections_vs_reference_per_image(workdir):
     detect_frames(..., letter = 1); criteria of test_gpu_frames.py::test_detect_frames_vs_reference_per_image."""
     import yolo2_light_b200 as yb
     from oracle import ref
-    cfg, wts = _bigger("tiny", workdir, 160, 160)
-    net = yb.load_network(cfg, wts, batch=3)
-    net.set_precision(yb.YB_PREC_FP32)
+    cfg, wts = bigger("tiny", workdir, 160, 160)
+    net = util.load(cfg, wts, 3, precision=yb.YB_PREC_FP32)
     net.set_letterbox(True)
     sizes = [(640, 480), (100, 300)]
-    frames = _frames(sizes, 45)
+    frames = util.frames(sizes, 45)
     net.predict_frames_u8(frames)
     dets, counts = net.detect_frames(sizes, 0.2, 0.45, letter=1, max_rows=4096)
     rnet = ref.RefNet(cfg, wts, 1, 0, 7)
@@ -128,7 +123,7 @@ def test_letterboxed_detections_vs_reference_per_image(workdir):
         assert theirs.shape[0] > 0, b
         assert abs(int(counts[b]) - theirs.shape[0]) <= max(1, theirs.shape[0] // 100), (b, counts[b], theirs.shape)
         if counts[b] == theirs.shape[0] and theirs.shape[0]:
-            a, e = _sorted(dets[b]), _sorted(theirs)
+            a, e = sorted_rows(dets[b]), sorted_rows(theirs)
             assert np.allclose(a[:, :5], e[:, :5], rtol=1e-4, atol=1e-5)
             kept_a, kept_e = (a[:, 5:] > 0).sum(), (e[:, 5:] > 0).sum()
             assert abs(int(kept_a) - int(kept_e)) <= max(2, int(kept_e) // 50), (kept_a, kept_e)
@@ -143,7 +138,7 @@ PIPE_BATCHES = [[(120, 96), (64, 64), (32, 200)], [(64, 64)] * 3, [(300, 170)], 
 def test_pipelined_equal_sync_calls(kind, workdir):
     """submit_frames_u8 and submit_device_frames (formats in turn) with letterboxing on and letter = 1, three tickets in
     flight, against predict_frames_u8 / predict_device_frames + detect_frames."""
-    net, q = _mixed_net(kind, workdir)
+    net, q = mixed_net(kind, workdir)
     net.set_letterbox(True)
     thresh = 0.3
     rng = np.random.default_rng(41)
@@ -186,8 +181,8 @@ def test_pipelined_equal_sync_calls(kind, workdir):
 def test_ticket_keeps_its_geometry(workdir):
     """The switch changes later calls only: a ticket submitted with letterboxing on and collected after it was turned off
     holds the letterboxed detections, and the next ticket the stretched ones."""
-    net, q = _mixed_net("tiny64_q1", workdir)
-    fr = _frames([(640, 480), (100, 300)], 55)
+    net, q = mixed_net("tiny64_q1", workdir)
+    fr = util.frames([(640, 480), (100, 300)], 55)
     sizes = [(640, 480), (100, 300)]
     exp = {}
     for on in (True, False):

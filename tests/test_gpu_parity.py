@@ -16,35 +16,15 @@ from yolo2_light_b200 import cfgs
 pytestmark = pytest.mark.gpu
 
 
-def _load(name, workdir, batch, q, precision=None, fuse=None, keep_counts=False):
-    import yolo2_light_b200 as yb
-    cfg, wts = util.model_files(name, workdir)
-    net = yb.load_network(cfg, wts, batch=batch, quantized=q)
-    if precision is not None:
-        net.set_precision(precision)
-    if fuse is not None:
-        net.set_option("fuse", int(fuse))
-    if keep_counts:
-        net.set_option("keep_counts", 1)
-    return net
-
-
-def _oracle_outs(net, x, q):
-    from oracle import port
-    layers = net.layers
-    per_image = [port.run_network(layers, x[b:b + 1], quantized=bool(q)) for b in range(x.shape[0])]
-    return [np.concatenate([pi[i] for pi in per_image], axis=0) for i in range(len(layers))]
-
-
 # ---- exact f32 mode: every layer of every model family against the oracle ---------------------------------
 @pytest.mark.parametrize("name", ["tiny64", "v3_32", "spp32", "v2voc32", "tinyvoc64", "tiny_w96_h64", "v3_w64_h96"])
 def test_fp32_mode_every_layer(name, workdir):
     import yolo2_light_b200 as yb
     B = 2
-    net = _load(name, workdir, B, 0, precision=yb.YB_PREC_FP32, fuse=False)
+    net = util.load(*util.model_files(name, workdir), B, precision=yb.YB_PREC_FP32, fuse=False)
     x = util.images(name, B)
     net.predict(x)
-    outs = _oracle_outs(net, x, 0)
+    outs = util.oracle_outs(net, x, 0)
     for i, o in enumerate(outs):
         got = net.fetch_layer(i)
         t = net.layer(i)["type_name"]
@@ -65,8 +45,8 @@ def test_fp32_mode_fused_equals_unfused(name, workdir):
     import yolo2_light_b200 as yb
     B = 2
     x = util.images(name, B)
-    a = _load(name, workdir, B, 0, precision=yb.YB_PREC_FP32, fuse=False)
-    b = _load(name, workdir, B, 0, precision=yb.YB_PREC_FP32, fuse=True)
+    a = util.load(*util.model_files(name, workdir), B, precision=yb.YB_PREC_FP32, fuse=False)
+    b = util.load(*util.model_files(name, workdir), B, precision=yb.YB_PREC_FP32, fuse=True)
     a.predict(x); b.predict(x)
     assert b.last_launches() < a.last_launches()
     for i, oa in a.detection_outputs().items():
@@ -78,9 +58,9 @@ def test_xnor_counts_and_outputs_bit_exact_per_layer(workdir):
     """Each XNOR conv fed the oracle's own input: popcounts equal as integers, outputs equal bit-for-bit."""
     from oracle import port
     name, B = "xnor64", 2
-    net = _load(name, workdir, B, 0, fuse=False, keep_counts=True)
+    net = util.load(*util.model_files(name, workdir), B, fuse=False, keep_counts=True)
     x = util.images(name, B)
-    outs = _oracle_outs(net, x, 0)
+    outs = util.oracle_outs(net, x, 0)
     layers = net.layers
     n_x = 0
     for i, l in enumerate(layers):
@@ -100,10 +80,10 @@ def test_xnor_network_counts_bit_exact(workdir):
     layer sees exactly the reference's signs: ALL raw popcounts and every XNOR layer's float output are identical."""
     from oracle import port
     name, B = "xnor64", 2
-    net = _load(name, workdir, B, 0, fuse=False, keep_counts=True)
+    net = util.load(*util.model_files(name, workdir), B, fuse=False, keep_counts=True)
     x = util.images(name, B)
     net.predict(x)
-    outs = _oracle_outs(net, x, 0)
+    outs = util.oracle_outs(net, x, 0)
     layers = net.layers
     for i, l in enumerate(layers):
         if l["type_name"] == "CONVOLUTIONAL" and l["xnor"]:
@@ -123,9 +103,9 @@ def test_xnor_network_counts_bit_exact(workdir):
 def test_int8_accumulators_and_outputs_bit_exact_per_layer(name, workdir):
     from oracle import port
     B = 2
-    net = _load(name, workdir, B, 1, fuse=False)
+    net = util.load(*util.model_files(name, workdir), B, quantized=1, fuse=False)
     x = util.images(name, B)
-    outs = _oracle_outs(net, x, 1)
+    outs = util.oracle_outs(net, x, 1)
     layers = net.layers
     n_q = 0
     for i, l in enumerate(layers):
@@ -145,10 +125,10 @@ def test_int8_accumulators_and_outputs_bit_exact_per_layer(name, workdir):
 def test_int8_network_accumulators(workdir):
     from oracle import port
     name, B = "tiny64", 2
-    net = _load(name, workdir, B, 1, fuse=False, keep_counts=True)
+    net = util.load(*util.model_files(name, workdir), B, quantized=1, fuse=False, keep_counts=True)
     x = util.images(name, B)
     net.predict(x, quantized=True)
-    outs = _oracle_outs(net, x, 1)
+    outs = util.oracle_outs(net, x, 1)
     layers = net.layers
     for i, l in enumerate(layers):
         if l["type_name"] == "CONVOLUTIONAL" and i >= 1 and l["activation"] != 3:
@@ -171,7 +151,7 @@ def test_detection_outputs_vs_reference_golden(name, q, workdir):
     import yolo2_light_b200 as yb
     g = np.load(os.path.join(util.GOLDEN, f"{name}_q{q}.npz"))
     B = 2
-    net = _load(name, workdir, B, q, precision=yb.YB_PREC_FP32)
+    net = util.load(*util.model_files(name, workdir), B, quantized=q, precision=yb.YB_PREC_FP32)
     x = util.images(name, B)
     net.predict(x, quantized=bool(q))
     n = 0
@@ -251,10 +231,10 @@ def test_dropin_from_reference_prepared_layers(name, q, workdir):
 def test_non_square_inputs_default_precision(name, q, workdir):
     """H != W through the default (tensor-core where the shape allows) paths, batch 3 (odd)."""
     B = 3
-    net = _load(name, workdir, B, q)
+    net = util.load(*util.model_files(name, workdir), B, quantized=q)
     x = util.images(name, B)
     net.predict(x, quantized=bool(q))
-    outs = _oracle_outs(net, x, q)
+    outs = util.oracle_outs(net, x, q)
     for i, o in net.detection_outputs().items():
         assert util.rel_l2(o, outs[i].reshape(o.shape)) <= 3e-3, (name, q, i)
 
@@ -264,11 +244,11 @@ def test_empty_and_edge_inputs(workdir):
     import yolo2_light_b200 as yb
     name = "tiny64"
     for B in (1, 3):
-        net = _load(name, workdir, B, 0, precision=yb.YB_PREC_FP32)
+        net = util.load(*util.model_files(name, workdir), B, precision=yb.YB_PREC_FP32)
         for val in (0.0, 1.0):
             x = np.full((B, 3, 64, 64), val, np.float32)
             net.predict(x)
-            outs = _oracle_outs(net, x, 0)
+            outs = util.oracle_outs(net, x, 0)
             for i, o in net.detection_outputs().items():
                 assert util.rel_l2(o, outs[i].reshape(o.shape)) <= 1e-5
     with pytest.raises(yb.YbError):
@@ -314,7 +294,7 @@ def test_device_input_pipeline_bit_exact(src_hw, workdir):
     import yolo2_light_b200 as yb
     from oracle import port
     name, B = "tiny64", 2
-    net = _load(name, workdir, B, 0, precision=yb.YB_PREC_FP32)
+    net = util.load(*util.model_files(name, workdir), B, precision=yb.YB_PREC_FP32)
     rng = np.random.default_rng(7)
     imgs = rng.integers(0, 256, (B, src_hw[0], src_hw[1], 3), dtype=np.uint8)
     net.predict_image_u8(imgs)
@@ -336,10 +316,8 @@ def test_int8_calibration_on_device(name, workdir):
     B = 2
     cfg, wts = util.model_files(name, workdir)
     x = util.images(name, B)
-    net = yb.load_network(cfg, wts, batch=B)
-    net.set_precision(yb.YB_PREC_FP32)
     # (1) the histogram kernel counts exactly what the reference's binning counts
-    net.set_option("fuse", 0)
+    net = util.load(cfg, wts, B, precision=yb.YB_PREC_FP32, fuse=0)
     net.predict(x)
     convs = [i for i, l in enumerate(net.layers) if l["type_name"] == "CONVOLUTIONAL"]
     for i in convs[:6]:
@@ -379,9 +357,7 @@ def test_maxpool_fused_with_quantise_or_binarise_is_bit_exact(name, q, workdir):
     x = util.images(name, B)
     res = []
     for fuse in (0, 1):
-        net = _load(name, workdir, B, q, precision=yb.YB_PREC_FP32)
-        net.set_option("fuse", fuse)
-        net.set_option("keep_counts", 1)
+        net = util.load(*util.model_files(name, workdir), B, quantized=q, precision=yb.YB_PREC_FP32, fuse=fuse, keep_counts=True)
         net.predict(x, quantized=bool(q))
         kinds = [k for _, k, _ in net.profile(quantized=bool(q))]
         ints = [i for i, l in enumerate(net.layers)
@@ -401,17 +377,14 @@ def test_maxpool_fused_with_quantise_or_binarise_is_bit_exact(name, q, workdir):
 def test_xnor_stride_pad_fallback_matches_reference(workdir):
     """yolov2_forward_network.c:40-50 + :204: such layers binarise the input to +-1 floats, swap in +-mean weights and run the
     ordinary im2col + gemm_nn.  The engine does the same (k_binarize_pm1 + exact-order float conv): bit-identical."""
-    import yolo2_light_b200 as yb
     from oracle import ref
     secs = [cfgs._net(32, 32), cfgs._conv(8, 3), cfgs._conv(16, 3, 2, xnor=1), cfgs._conv(16, 1, xnor=1),
             cfgs._conv(16, 3, xnor=1),                      # an ordinary XNOR layer behind them
             cfgs._conv(18, 1, bn=False, act="linear"), cfgs._yolo("0,1,2", cfgs.COCO_ANCHORS, 9, classes=1)]
-    cfg = cfgs.write_cfg(secs, os.path.join(workdir, "xnor_fb.cfg"))
-    wts = cfgs.write_weights(secs, os.path.join(workdir, "xnor_fb.weights"), seed=23)
+    cfg, wts = util.write_net(workdir, "xnor_fb", secs, 23)
     B = 2
     x = cfgs.synthetic_images(B, 3, 32, 32, seed=24)
-    net = yb.load_network(cfg, wts, batch=B)
-    net.set_option("fuse", 0)
+    net = util.load(cfg, wts, B, fuse=0)
     net.predict(x)
     rnet = ref.RefNet(cfg, wts, 1, 0, 7)
     for b in range(B):
@@ -433,14 +406,11 @@ def test_fused_stem_pool_is_bit_identical_to_the_three_kernels(builder, w, h, q,
     import yolo2_light_b200 as yb
     B = 3
     secs = builder(w, h)
-    cfg = cfgs.write_cfg(secs, os.path.join(workdir, f"sp_{builder.__name__}_{w}x{h}.cfg"))
-    wts = cfgs.write_weights(secs, os.path.join(workdir, f"sp_{builder.__name__}_{w}x{h}.weights"), seed=61)
+    cfg, wts = util.write_net(workdir, f"sp_{builder.__name__}_{w}x{h}", secs, 61)
     x = cfgs.synthetic_images(B, 3, h, w, seed=62)
     nets = []
     for fuse in (0, 1):
-        net = yb.load_network(cfg, wts, batch=B, quantized=q)
-        net.set_option("fuse", fuse)
-        net.set_option("keep_counts", 1)
+        net = util.load(cfg, wts, B, quantized=q, fuse=fuse, keep_counts=True)
         net.predict(x, quantized=bool(q))
         nets.append(net)
     a, b = nets
@@ -461,16 +431,15 @@ def test_fused_stem_pool_is_bit_identical_to_the_three_kernels(builder, w, h, q,
         assert util.rel_l2(o, b.layer_output(i)) <= 1e-5, (builder.__name__, i)
     # production configuration (no raw-accumulator dump): the max-pools behind the integer convolutions run in their epilogues
     # (TcConv::pool_fmt) -- every integer layer that is still materialised is bit-identical to the unfused plan
-    c = yb.load_network(cfg, wts, batch=B, quantized=q)
+    c = util.load(cfg, wts, B, quantized=q)
     c.predict(x, quantized=bool(q))
     assert c.last_launches() < b.last_launches()
     n_cmp = n_gone = 0
     for i, l in enumerate(a.layers):
         if not (l["type_name"] == "CONVOLUTIONAL" and i >= 2 and (l["xnor"] or (q and l["activation"] != 3))):
             continue
-        try:
-            got = c.fetch_layer(i, quantized=bool(q))
-        except yb.YbError:
+        got = util.fetched(c, i, bool(q))
+        if got is None:
             n_gone += 1
             continue
         assert util.bits_equal(got, a.fetch_layer(i, quantized=bool(q))), i

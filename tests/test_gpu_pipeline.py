@@ -4,7 +4,6 @@ yb_network_collect_detections): both kinds interleaved on every slot, a full pip
 call, and a network freed with tickets still in flight.  Every result is compared bitwise with the synchronous calls on the
 same inputs."""
 import gc
-import os
 
 import numpy as np
 import pytest
@@ -19,21 +18,6 @@ B, W, H = 3, 160, 128
 DEPTH = 3                      # batches in flight
 THRESH, NMS, MAX_ROWS = 0.3, 0.45, 2048
 KINDS = ("raw", "u8", "frames", "device")
-
-
-def _files(workdir, builder, slim, tag):
-    secs = cfgs.slim(builder, slim, W, H)
-    cfg = os.path.join(workdir, f"pipe_{tag}.cfg")
-    wts = os.path.join(workdir, f"pipe_{tag}.weights")
-    if not os.path.exists(wts):
-        cfgs.write_cfg(secs, cfg)
-        cfgs.write_weights(secs, wts, seed=23)
-    return cfg, wts
-
-
-def _load(cfg, wts, q):
-    import yolo2_light_b200 as yb
-    return yb.load_network(cfg, wts, batch=B, quantized=q)
 
 
 def _job(net, kind, seed, q):
@@ -95,8 +79,7 @@ def _collect_and_check(net, job, ticket, q, what):
 
 @pytest.mark.parametrize("q", [0, 1])
 def test_raw_and_detection_tickets_interleave_on_every_slot(q, workdir):
-    cfg, wts = _files(workdir, cfgs.yolov3_tiny, 2, "tiny")
-    net = _load(cfg, wts, q)
+    net = util.load(*util.write_net(workdir, "pipe_tiny", cfgs.slim(cfgs.yolov3_tiny, 2, W, H), 23), B, quantized=q)
     # 16 batches cycling through the four kinds over three slots: every slot serves every kind, both after a ticket of
     # the same mode and after one of the other mode
     jobs = [_job(net, KINDS[k % len(KINDS)], 100 + k, bool(q)) for k in range(16)]
@@ -114,8 +97,7 @@ def test_raw_and_detection_tickets_interleave_on_every_slot(q, workdir):
 
 def test_full_pipeline_refuses_and_runs_on(workdir):
     import yolo2_light_b200 as yb
-    cfg, wts = _files(workdir, cfgs.yolov3_tiny, 2, "tiny")
-    net = _load(cfg, wts, 0)
+    net = util.load(*util.write_net(workdir, "pipe_tiny", cfgs.slim(cfgs.yolov3_tiny, 2, W, H), 23), B)
     jobs = [_job(net, KINDS[k % len(KINDS)], 200 + k, False) for k in range(7)]
     inflight = [(k, _submit(net, jobs[k], False)) for k in range(DEPTH)]
     for k in (DEPTH, DEPTH + 1):    # a fourth batch: device frames, then raw
@@ -136,8 +118,7 @@ def test_full_pipeline_refuses_and_runs_on(workdir):
 
 def test_ticket_collected_with_the_wrong_call(workdir):
     import yolo2_light_b200 as yb
-    cfg, wts = _files(workdir, cfgs.yolov3_tiny, 2, "tiny")
-    net = _load(cfg, wts, 0)
+    net = util.load(*util.write_net(workdir, "pipe_tiny", cfgs.slim(cfgs.yolov3_tiny, 2, W, H), 23), B)
     raw, det = _job(net, "raw", 300, False), _job(net, "frames", 301, False)
     t_raw, t_det = _submit(net, raw, False), _submit(net, det, False)
     with pytest.raises(yb.YbError, match="collect_detections: bad ticket"):
@@ -149,14 +130,14 @@ def test_ticket_collected_with_the_wrong_call(workdir):
 
 
 def test_network_freed_with_tickets_in_flight(workdir):
-    cfg, wts = _files(workdir, cfgs.yolov3, 4, "v3")
-    net = _load(cfg, wts, 0)
+    cfg, wts = util.write_net(workdir, "pipe_v3", cfgs.slim(cfgs.yolov3, 4, W, H), 23)
+    net = util.load(cfg, wts, B)
     jobs = [_job(net, kind, 400 + k, False) for k, kind in enumerate(("raw", "u8", "device"))]
     for job in jobs:
         _submit(net, job, False)
     del net     # three uncollected tickets, of both kinds
     gc.collect()
-    fresh = _load(cfg, wts, 0)
+    fresh = util.load(cfg, wts, B)
     tickets = [_submit(fresh, job, False) for job in jobs]
     for k, (job, t) in enumerate(zip(jobs, tickets)):
         _collect_and_check(fresh, job, t, False, k)

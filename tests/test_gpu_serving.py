@@ -18,23 +18,13 @@ pytestmark = pytest.mark.gpu
 ROOT = util.ROOT
 
 
-def _net(builder, slim, w, h, workdir, tag, batch, q=0, seed=51):
-    import yolo2_light_b200 as yb
-    secs = cfgs.slim(builder, slim, w, h)
-    cfg = os.path.join(workdir, f"srv_{tag}.cfg")
-    wts = os.path.join(workdir, f"srv_{tag}.weights")
-    cfgs.write_cfg(secs, cfg)
-    cfgs.write_weights(secs, wts, seed=seed)
-    return yb.load_network(cfg, wts, batch=batch, quantized=q), cfg, wts
-
-
 @pytest.mark.parametrize("builder,slim,q,thresh,fw,fh", [(cfgs.yolov3_tiny, 2, 0, 0.3, 120, 96), (cfgs.yolov3, 4, 0, 0.3, 120, 96),
                                                         (cfgs.yolov3_tiny, 2, 1, 0.3, 120, 96), (cfgs.tiny_yolo_obj_xnor, 2, 0, 0.05, 120, 96),
                                                         # frames of exactly the network size: the stem reads the 8-bit frames itself
                                                         (cfgs.yolov3, 4, 0, 0.3, 160, 128), (cfgs.yolov3_tiny, 2, 0, 0.3, 160, 128)])
 def test_pipelined_u8_detections_equal_sync_calls(builder, slim, q, thresh, fw, fh, workdir):
     B, W, H = 3, 160, 128
-    net, _, _ = _net(builder, slim, W, H, workdir, f"{builder.__name__}_{q}", B, q)
+    net = util.load(*util.write_net(workdir, f"srv_{builder.__name__}_{q}", cfgs.slim(builder, slim, W, H), 51), B, quantized=q)
     rng = np.random.default_rng(5)
     frames = [rng.integers(0, 256, size=(B, fh, fw, 3), dtype=np.uint8) for _ in range(5)]   # 120x96 frames are resized on the device
     # expected: the synchronous pair predict_image_u8 + detect, frame set by frame set
@@ -64,7 +54,7 @@ def test_pipelined_u8_detections_equal_sync_calls(builder, slim, q, thresh, fw, 
 def test_predict_batch_two_replicas_equals_single_gpu(workdir):
     import torch
     B, W, H = 2, 96, 96
-    net, _, _ = _net(cfgs.yolov3, 4, W, H, workdir, "pb_v3", B)
+    net = util.load(*util.write_net(workdir, "srv_pb_v3", cfgs.slim(cfgs.yolov3, 4, W, H), 51), B)
     nimg = 3 * 2 * B + 1      # three rounds over two replicas and a partial last shard
     x = cfgs.synthetic_images(nimg, 3, H, W, seed=77)
     exp = {}
@@ -97,7 +87,7 @@ def test_c_host_program_drives_two_replicas(builder, slim, q, workdir):
                                os.path.join(ROOT, "tests", "c", "batch_multi_gpu.c"), "-o", exe,
                                "-L", os.path.join(ROOT, "yolo2_light_b200"), "-lyolo2_light_b200",
                                "-Wl,-rpath," + os.path.join(ROOT, "yolo2_light_b200")])
-    _, cfg, wts = _net(builder, slim, 96, 64, workdir, f"c_{builder.__name__}_{q}", 1, q)
+    cfg, wts = util.write_net(workdir, f"srv_c_{builder.__name__}_{q}", cfgs.slim(builder, slim, 96, 64), 51)
     r = subprocess.run([exe, cfg, wts, "2", "9", str(q)], capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, r.stdout + r.stderr
     assert "bit-identical" in r.stdout

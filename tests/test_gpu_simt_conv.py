@@ -1,8 +1,6 @@
 """The CUDA-core implicit-GEMM convolution (k_conv_simt) on the layers only it takes: INT8 layers the s8 wgmma tile refuses, XNOR
 layers off the s8 wgmma with more than 2 sign words per tap, and bf16 layers the tensor cores refuse.  Each network's op list
 shows the path runs; the results are checked against the CPU oracle.  GPU box only."""
-import os
-
 import numpy as np
 import pytest
 
@@ -12,30 +10,6 @@ from yolo2_light_b200 import cfgs
 pytestmark = pytest.mark.gpu
 
 B = 2
-
-
-def _load(workdir, name, secs, seed, q=0, keep_counts=False):
-    import yolo2_light_b200 as yb
-    cfg = cfgs.write_cfg(secs, os.path.join(workdir, name + ".cfg"))
-    wts = cfgs.write_weights(secs, os.path.join(workdir, name + ".weights"), seed=seed)
-    net = yb.load_network(cfg, wts, batch=B, quantized=q)
-    net.set_option("fuse", 0)
-    if keep_counts:
-        net.set_option("keep_counts", 1)
-    return net
-
-
-def _kinds(net, q=False):
-    kinds = {}
-    for li, kind, _ in net.profile(quantized=q):
-        kinds.setdefault(li, []).append(kind)
-    return kinds
-
-
-def _oracle_outs(net, x, q):
-    from oracle import port
-    per_image = [port.run_network(net.layers, x[b:b + 1], quantized=q) for b in range(x.shape[0])]
-    return [np.concatenate([pi[i] for pi in per_image], axis=0) for i in range(net.n)]
 
 
 def test_int8_layers_outside_the_tensor_core_tile(workdir):
@@ -48,13 +22,13 @@ def test_int8_layers_outside_the_tensor_core_tile(workdir):
             c(32, 1, 2),     # 3: 1x1 / 2, 7 -> 4
             c(4, 3),         # 4: 4 filters
             c(18, 1, bn=False, act="linear")]
-    net = _load(workdir, "simt_int8", secs, 41, q=1, keep_counts=True)
+    net = util.load(*util.write_net(workdir, "simt_int8", secs, 41), B, quantized=1, fuse=0, keep_counts=True)
     x = cfgs.synthetic_images(B, 3, 26, 26, seed=42)
     net.predict(x, quantized=True)
-    kinds = _kinds(net, True)
+    kinds = util.profile_kinds(net, True)
     for i in (2, 3, 4):
         assert "conv_int8" in kinds[i], (i, kinds[i])
-    outs = _oracle_outs(net, x, True)
+    outs = util.oracle_outs(net, x, 1)
     for i in (2, 3, 4):
         l = net.layer(i)
         args = (l["weights_int8"], l["biases"], l["input_quant_multipler"], l["weights_quant_multipler"], l["n"], l["size"],
@@ -77,13 +51,13 @@ def test_xnor_layers_on_the_general_popcount_kernel(workdir):
             c(96, 3, **xn),  # 1: C = 72
             c(4, 3, **xn),   # 2: C = 96, 4 filters
             c(18, 1, bn=False, act="linear")]
-    net = _load(workdir, "simt_xnor", secs, 43, keep_counts=True)
+    net = util.load(*util.write_net(workdir, "simt_xnor", secs, 43), B, fuse=0, keep_counts=True)
     x = cfgs.synthetic_images(B, 3, 20, 20, seed=44)
     net.predict(x)
-    kinds = _kinds(net)
+    kinds = util.profile_kinds(net)
     for i in (1, 2):
         assert "conv_xnor" in kinds[i], (i, kinds[i])
-    outs = _oracle_outs(net, x, False)
+    outs = util.oracle_outs(net, x, 0)
     for i in (1, 2):
         l = net.layer(i)
         exp, cnt = port.conv_xnor(outs[i - 1], l["weights"], l["biases"], l["mean_arr"], l["n"], l["size"], l["activation"],
@@ -99,20 +73,18 @@ def test_bf16_layer_the_tensor_cores_refuse(workdir):
     """3x3 / stride 2 on 13 x 13 in a bf16 network runs on CUDA cores, between tensor-core layers"""
     import yolo2_light_b200 as yb
     from oracle import port
-    from test_gpu_tc import bf16_round
     c = cfgs._conv
     secs = [cfgs._net(26, 26), c(16, 3), ("maxpool", {"size": "2", "stride": "2"}),
             c(32, 3, 2),     # 2: 13 -> 7
             c(32, 3),        # 3
             c(255, 1, bn=False, act="linear"), cfgs._yolo("0,1,2", cfgs.COCO_ANCHORS, 9)]
-    net = _load(workdir, "simt_bf16", secs, 45)
-    net.set_precision(yb.YB_PREC_BF16_TC)
+    net = util.load(*util.write_net(workdir, "simt_bf16", secs, 45), B, precision=yb.YB_PREC_BF16_TC, fuse=0)
     x = cfgs.synthetic_images(B, 3, 26, 26, seed=46)
     net.predict(x)
-    kinds = _kinds(net)
+    kinds = util.profile_kinds(net)
     assert "conv_simt" in kinds[2] and "conv_tc" in kinds[3], kinds
     l = net.layer(2)
-    exp = bf16_round(port.conv_fp32(net.fetch_layer(1), l["weights"], l["biases"], l["n"], l["size"], l["stride"], l["pad"],
+    exp = util.bf16_round(port.conv_fp32(net.fetch_layer(1), l["weights"], l["biases"], l["n"], l["size"], l["stride"], l["pad"],
                                     l["activation"]))
     err = util.rel_l2(net.fetch_layer(2), exp)
     assert err <= 5e-4, err

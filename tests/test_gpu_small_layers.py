@@ -10,14 +10,11 @@ asserts, through Network.op_kernels, which kernel ran the layer: the channel cou
 the scalar and the 16-byte kernels of max-pool and upsample to work in each precision.
 
 The helpers and the case table run on the CPU; the tests that need a GPU are marked."""
-import os
-
 import numpy as np
 import pytest
 
 import ybtest_util as util
-from test_gpu_tc import bf16_round
-from test_gpu_tc_exact import logistic_bound
+from ybtest_util import bf16_round, kernel_is, logistic_bound, ulp_diff
 from yolo2_light_b200 import cfgs
 
 BATCH = 3
@@ -188,15 +185,6 @@ CASES = {
 
 
 # ---- comparisons --------------------------------------------------------------------------------------------------------
-def ulp_diff(a, b, bf16):
-    """distance in f32 (or, for bf16 values, bf16) units in the last place"""
-    def key(x):
-        i = np.ascontiguousarray(x, np.float32).view(np.int32).astype(np.int64)
-        return np.where(i < 0, -(i & 0x7FFFFFFF), i)
-    d = np.abs(key(a) - key(b))
-    return d >> 16 if bf16 else d
-
-
 def expf_bounds(softmax_n):
     """Bounds, relative to the exact value, on k_region's logistic 1 / (1 + expf(-v)) and on its softmax over softmax_n
     classes, from the CUDA C Programming Guide's maximum error of expf (2 ulp, full range) and IEEE rounding of +, / (u =
@@ -215,16 +203,14 @@ def check_layer(m, i, L, layers, bf16, q=False):
     got = m.fetch_layer(i, quantized=q)
     fetch = lambda j: m.fetch_layer(j, quantized=q)
     rnd = bf16_round if bf16 else (lambda a: a)
-    if t == "MAXPOOL":
-        assert util.bits_equal(got, port.maxpool(fetch(i - 1), L["size"], L["stride"], L["pad"])), i
+    if t in ("MAXPOOL", "REORG"):
+        assert util.bits_equal(got, util.oracle_layer(L, i, fetch(i - 1), int(q))[0]), i
     elif t == "UPSAMPLE":
-        assert util.bits_equal(got, rnd(port.upsample(fetch(i - 1), L["stride"], L["scale"]))), i
-    elif t == "REORG":
-        assert util.bits_equal(got, port.reorg(fetch(i - 1), L["stride"])), i
+        assert util.bits_equal(got, rnd(util.oracle_layer(L, i, fetch(i - 1), int(q))[0])), i
     elif t == "ROUTE":
         assert util.bits_equal(got, np.concatenate([fetch(int(j)) for j in L["input_layers"]], axis=1)), i
     elif t == "SHORTCUT":
-        exp = rnd(port.shortcut(fetch(i - 1), fetch(L["index"]), L["activation"]))
+        exp = rnd(util.oracle_layer(L, i, fetch(i - 1), int(q), frm=fetch(L["index"]))[0])
         d = ulp_diff(got, exp, bf16)
         assert d.max() <= (1 if L["activation"] == 0 else 0), (i, int(d.max()), int((d > 0).sum()))
     elif t == "YOLO":
@@ -265,11 +251,6 @@ def check_layer(m, i, L, layers, bf16, q=False):
     return t
 
 
-def kernel_is(name, base):
-    """name (mangled or not) is kernel `base`, not a longer kernel name that starts with it"""
-    return name is not None and base in name and base + "_" not in name
-
-
 # ---- CPU tests ----------------------------------------------------------------------------------------------------------
 def test_cases_run_both_kernels_of_maxpool_and_upsample():
     """in each precision, the table runs the scalar and the 16-byte kernel of max-pool and of upsample"""
@@ -298,23 +279,14 @@ def test_ulp_diff():
 
 
 # ---- GPU tests ----------------------------------------------------------------------------------------------------------
-def _load(case, name, dt, workdir):
-    import yolo2_light_b200 as yb
-    secs = case.sections()
-    cfg = cfgs.write_cfg(secs, os.path.join(workdir, f"small_{name}.cfg"))
-    wts = cfgs.write_weights(secs, os.path.join(workdir, f"small_{name}.weights"), seed=sum(map(ord, name)))
-    m = yb.load_network(cfg, wts, batch=BATCH)
-    m.set_precision(yb.YB_PREC_FP32 if dt == "f32" else yb.YB_PREC_BF16_TC)
-    m.set_option("fuse", case.fuse)
-    return m
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("dt", DTYPES)
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_small_layer(name, dt, workdir):
+    import yolo2_light_b200 as yb
     case = CASES[name]()
-    m = _load(case, name, dt, workdir)
+    m = util.load(*util.write_net(workdir, f"small_{name}", case.sections(), sum(map(ord, name))), BATCH,
+                  precision=yb.YB_PREC_FP32 if dt == "f32" else yb.YB_PREC_BF16_TC, fuse=case.fuse)
     ops = [op for op in m.op_kernels() if op[2] is None or "k_nhwc_to_nchw_f32" not in op[2]]   # not the last layer's NCHW copy
     for i, kern in case.kernels.items():
         mine = [k for (j, _, k) in ops if j == i]
@@ -341,9 +313,7 @@ def test_shortcut_whose_scales_differ_in_width_and_height_is_rejected(workdir):
     tensor; the reference asserts stride == h1 / h2 = 3 and stops.  The engine refuses the network in its layer plan."""
     import yolo2_light_b200 as yb
     secs = [cfgs._net(56, 50), conv(8), conv(8, 3, 2), conv(8, 3, 2), conv(8, 3, 2), upsample(2), shortcut(0)]
-    cfg = cfgs.write_cfg(secs, os.path.join(workdir, "shortcut_aspect.cfg"))
-    wts = cfgs.write_weights(secs, os.path.join(workdir, "shortcut_aspect.weights"), seed=1)
-    m = yb.load_network(cfg, wts, batch=2)
+    m = util.load(*util.write_net(workdir, "shortcut_aspect", secs, 1), 2)
     assert (m.layer(5)["out_w"], m.layer(5)["out_h"]) == (14, 14)
     for prec in (yb.YB_PREC_BF16_TC, yb.YB_PREC_FP32):
         m.set_precision(prec)
@@ -358,8 +328,6 @@ def test_region_with_coords_other_than_4_is_rejected(workdir):
     import yolo2_light_b200 as yb
     head = ("region", {"anchors": "1,1, 2,2", "classes": "3", "coords": "5", "num": "2", "softmax": "1"})
     secs = [cfgs._net(8, 6), conv(8), cfgs._conv(2 * (5 + 1 + 3), 1, bn=False, act="linear"), head]
-    cfg = cfgs.write_cfg(secs, os.path.join(workdir, "region_coords5.cfg"))
-    wts = cfgs.write_weights(secs, os.path.join(workdir, "region_coords5.weights"), seed=2)
-    m = yb.load_network(cfg, wts, batch=1)
+    m = util.load(*util.write_net(workdir, "region_coords5", secs, 2), 1)
     with pytest.raises(yb.YbError, match=r"\[region\] coords=5 is not supported"):
         m.op_kernels()

@@ -6,9 +6,7 @@ import numpy as np
 import pytest
 
 import ybtest_util as util
-from test_gpu_tc import _files, bf16_round
-from test_gpu_tc_stride2 import s2chain
-from test_gpu_tc_wide import widenet
+from ybtest_util import bf16_round, s2chain, widenet
 from yolo2_light_b200 import cfgs
 
 pytestmark = pytest.mark.gpu
@@ -23,7 +21,7 @@ def _files_for(workdir, name, hw):
     h, w = hw
     secs = NETS[name]()
     secs[0][1]["height"], secs[0][1]["width"] = str(h), str(w)
-    return _files(workdir, f"stems2_{name}{h}x{w}", secs, 51)
+    return util.write_net(workdir, f"stems2_{name}{h}x{w}", secs, 51)
 
 
 def _run(cfg, wts, batch, x, monkeypatch, fused, u8=False):
@@ -32,9 +30,7 @@ def _run(cfg, wts, batch, x, monkeypatch, fused, u8=False):
         monkeypatch.delenv("YB_NO_STEM_S2_FUSE", raising=False)
     else:
         monkeypatch.setenv("YB_NO_STEM_S2_FUSE", "1")
-    net = yb.load_network(cfg, wts, batch=batch)
-    net.set_precision(yb.YB_PREC_BF16_TC)
-    net.set_option("fuse", 1)
+    net = util.load(cfg, wts, batch, precision=yb.YB_PREC_BF16_TC, fuse=1)
     if u8:
         net.predict_image_u8(x)
     else:
@@ -42,18 +38,10 @@ def _run(cfg, wts, batch, x, monkeypatch, fused, u8=False):
     return net
 
 
-def _layer(net, i):
-    import yolo2_light_b200 as yb
-    try:
-        return net.fetch_layer(i)
-    except yb.YbError:
-        return None
-
-
 def _assert_bit_equal(ref, got, what):
     """got: fused; ref: unfused.  Only the stem output is missing from the fused run."""
     for i in range(ref.n):
-        r, g = _layer(ref, i), _layer(got, i)
+        r, g = util.fetched(ref, i), util.fetched(got, i)
         if i == 0:
             assert r is not None and g is None, what
             continue
@@ -86,7 +74,7 @@ def test_stem_s2_u8_frames_bit_equal(workdir, monkeypatch):
 
 def test_stem_s2_yolov3_608_bit_equal(workdir, monkeypatch):
     secs = cfgs.MODELS["yolov3"](608, 608)
-    cfg, wts = _files(workdir, "stems2_yolov3_608", secs, 1)
+    cfg, wts = util.write_net(workdir, "stems2_yolov3_608", secs, 1)
     x = cfgs.synthetic_images(2, 3, 608, 608, seed=63)
     ref = _run(cfg, wts, 2, x, monkeypatch, fused=False)
     got = _run(cfg, wts, 2, x, monkeypatch, fused=True)
@@ -117,7 +105,7 @@ def test_stem_s2_small_grids_bit_equal(workdir, monkeypatch):
         monkeypatch.setenv("YB_TC_GRID", grid)
         net = _run(cfg, wts, batch, x, monkeypatch, fused=True)
         for i in range(1, net.n):
-            r, g = _layer(full, i), _layer(net, i)
+            r, g = util.fetched(full, i), util.fetched(net, i)
             assert (r is None) == (g is None), (grid, i)
             if r is not None:
                 assert np.array_equal(r, g), (grid, i)
@@ -140,7 +128,6 @@ def test_stem_s2_engine_behaviour(workdir, monkeypatch):
     assert not [k for li, k, _ in prof if li == 0], prof
     # with fusion off (fuse = 0) the stem runs on its own and layer 0 stays readable
     monkeypatch.delenv("YB_NO_STEM_S2_FUSE", raising=False)
-    net = yb.load_network(cfg, wts, batch=batch)
-    net.set_option("fuse", 0)
+    net = util.load(cfg, wts, batch, fuse=0)
     net.predict(x)
     assert net.fetch_layer(0).shape[1] == 32

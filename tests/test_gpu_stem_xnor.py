@@ -18,20 +18,17 @@ integers.  bf16 networks run on the exactly representable data of test_gpu_tc_ex
 gives the same f32 value, and must equal its reference model (run_reference) to the bit; a logistic to within one bf16 ulp.
 
 The helpers and the case table run on the CPU; the tests that need a GPU are marked."""
-import os
-import re
-
 import numpy as np
 import pytest
 
+import exact_model
 import ybtest_util as util
-from test_gpu_tc import bf16_round
-from test_gpu_tc_exact import Net, consumer_pairs, onehot, run_reference, write_weights
+from exact_model import Net, consumer_pairs, onehot, run_reference
+from ybtest_util import kernel_inst
 from yolo2_light_b200 import cfgs
 
 LINEAR, LEAKY, RELU, LOGISTIC = "linear", "leaky", "relu", "logistic"
 XNOR = {"xnor": 1, "bin_output": 1}
-SIDES = {2: "SIDE_S8", 3: "SIDE_PM1_S8", 4: "SIDE_BITS"}      # yb::SideFmt values
 ACT_CODE = {LEAKY: 7, LINEAR: 3}                                # the ACT_* template argument of k_stem_pool
 SMALLK_SMEM = 40 * 1024                                         # conv_path: n * 9 * CW * 4 bytes of sign words at most
 
@@ -74,67 +71,6 @@ FAMILIES = {
     "k_conv_xnor_smallk_pool": {smallk_pool(cw, s) for cw in (1, 2) for s in ("SIDE_PM1_S8", "SIDE_BITS")},
 }
 TRACKED = set(FAMILIES) | {"k_conv_simt"}        # every launch of these is pinned by the case table
-
-_MANGLED_ARGS = [
-    (re.compile(r"Li(\d+)E"), lambda m: m[1]),
-    (re.compile(r"Lb([01])E"), lambda m: "true" if m[1] == "1" else "false"),
-    (re.compile(r"LN(?:S_|2yb)7SideFmtE(\d+)E"), lambda m: SIDES[int(m[1])]),
-    (re.compile(r"13__nv_bfloat16"), lambda m: "bf16"),
-    (re.compile(r"f"), lambda m: "float"),
-]
-_POLICY = re.compile(r"N(?:S_|2yb)(\d+)")
-
-
-def _demangled_arg(a):
-    a = a.strip()
-    m = re.fullmatch(r"\((?:yb::)?SideFmt\)(\d+)", a)
-    if m:
-        return SIDES[int(m[1])]
-    if a == "__nv_bfloat16":
-        return "bf16"
-    return re.sub(r"<.*", "", a.replace("yb::", "")).strip()     # a policy: its name only
-
-
-def kernel_inst(name):
-    """(kernel, template arguments) of a kernel name as cudaFuncGetName gives it: mangled, or demangled.  A policy type
-    argument (k_conv_simt's) is given by its name alone."""
-    if name.startswith("_Z"):
-        m = re.match(r"_ZN2ybL?(\d+)", name)
-        assert m, name
-        pos = m.end() + int(m[1])
-        base, args = name[m.end():pos], []
-        if name.startswith("I", pos):
-            pos += 1
-            while name[pos] != "E":
-                p = _POLICY.match(name, pos)
-                if p:
-                    args.append(name[p.end():p.end() + int(p[1])])
-                    break
-                for rx, val in _MANGLED_ARGS:
-                    a = rx.match(name, pos)
-                    if a:
-                        args.append(val(a))
-                        pos = a.end()
-                        break
-                else:
-                    raise ValueError(f"template argument at {pos} of {name}")
-        return base, tuple(args)
-    m = re.search(r"(k_\w+)(<?)", name)
-    assert m, name
-    base, args = m[1], []
-    if m[2]:
-        depth, cur = 1, ""
-        for ch in name[m.end():]:
-            depth += (ch == "<") - (ch == ">")
-            if depth == 0 or (depth == 1 and ch == ","):
-                args.append(_demangled_arg(cur))
-                cur = ""
-                if depth == 0:
-                    break
-            else:
-                cur += ch
-    return base, tuple(args)
-
 
 # ---- the case table -----------------------------------------------------------------------------------------------------
 class Case:
@@ -500,33 +436,6 @@ def test_grid_case_premise(name):
 
 
 # ---- GPU tests ----------------------------------------------------------------------------------------------------------
-def _load(case, name, workdir):
-    import yolo2_light_b200 as yb
-    cfg = cfgs.write_cfg(case.net.secs, os.path.join(workdir, f"sx_{name}.cfg"))
-    wts = write_weights(case.net, os.path.join(workdir, f"sx_{name}.weights"))
-    m = yb.load_network(cfg, wts, batch=case.batch, quantized=int(case.q))
-    m.set_precision(yb.YB_PREC_FP32 if case.prec == "f32" else yb.YB_PREC_BF16_TC)
-    m.set_option("fuse", case.fuse)
-    if case.keep_counts:
-        m.set_option("keep_counts", 1)
-    return m
-
-
-def port_layer(L, i, x, q):
-    """layer i of the oracle on x; returns (output, raw XNOR popcounts or INT8 accumulators, or None)"""
-    from oracle import port
-    t = L["type_name"]
-    if t == "MAXPOOL":
-        return port.maxpool(x, L["size"], L["stride"], L["pad"]), None
-    assert t == "CONVOLUTIONAL", t
-    if L["xnor"]:
-        return port.conv_xnor(x, L["weights"], L["biases"], L["mean_arr"], L["n"], L["size"], L["activation"], want_counts=True)
-    if q and i >= 1 and L["activation"] != port.LINEAR:
-        return port.conv_int8(x, L["weights_int8"], L["biases"], L["input_quant_multipler"], L["weights_quant_multipler"],
-                              L["n"], L["size"], L["stride"], L["pad"], L["activation"], want_acc=True)
-    return port.conv_fp32(x, L["weights"], L["biases"], L["n"], L["size"], L["stride"], L["pad"], L["activation"]), None
-
-
 def check_chains(case, m, x):
     q, bf16 = case.q, case.prec == "bf16"
     layers = m.layers
@@ -534,10 +443,10 @@ def check_chains(case, m, x):
         if layers[last]["type_name"] == "ROUTE":
             exp, cnt = np.concatenate([m.fetch_layer(int(j), quantized=q) for j in layers[last]["input_layers"]], axis=1), None
         else:
-            cur = (bf16_round(x) if bf16 else x) if first == 0 else m.fetch_layer(first - 1, quantized=q)
+            cur = (util.bf16_round(x) if bf16 else x) if first == 0 else m.fetch_layer(first - 1, quantized=q)
             for i in range(first, last + 1):
-                cur, cnt = port_layer(layers[i], i, cur, q)
-            exp = bf16_round(cur) if bf16 else cur
+                cur, cnt = util.oracle_layer(layers[i], i, cur, int(q))
+            exp = util.bf16_round(cur) if bf16 else cur
         got = m.fetch_layer(last, quantized=q)
         bad = np.argwhere(got.view(np.uint32) != np.ascontiguousarray(exp, np.float32).view(np.uint32))
         assert got.shape == exp.shape and len(bad) == 0, (first, last, len(bad), bad[:5].tolist())
@@ -553,8 +462,9 @@ def check_grid(case, m, x):
         assert got.shape == e.shape, i
         tol = case.net.tol.get(i, 0)
         if tol:
-            d = np.abs(got.view(np.int32).astype(np.int64) - e.view(np.int32).astype(np.int64)) >> 16
-            assert np.all(got >= 0) and np.all(e >= 0) and d.max() <= tol, (i, int(d.max()))
+            d = util.ulp_diff(got, e, True)
+            assert np.all(got >= 0) and np.all(e >= 0) and np.array_equal(np.signbit(got), np.signbit(e)) and d.max() <= tol, \
+                (i, int(d.max()))
         else:
             bad = np.argwhere(got.view(np.uint32) != e.view(np.uint32))
             assert len(bad) == 0, (i, len(bad), bad[:5].tolist())
@@ -567,7 +477,9 @@ def test_stem_xnor(name, workdir, monkeypatch):
     case = CASES[name]()
     for k, v in case.env.items():
         monkeypatch.setenv(k, v)
-    m = _load(case, name, workdir)
+    m = util.load(*exact_model.write_net(case.net, workdir, f"sx_{name}"), case.batch, quantized=int(case.q),
+                  precision=yb.YB_PREC_FP32 if case.prec == "f32" else yb.YB_PREC_BF16_TC, fuse=case.fuse,
+                  keep_counts=case.keep_counts)
     q = case.q
     ops = m.op_kernels(quantized=q)
     ran = {}

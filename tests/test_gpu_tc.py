@@ -1,60 +1,13 @@
 """Tensor-core (wgmma) FP32-variant convolution: per-layer against the CPU oracle fed the GPU's own bf16 inputs,
 then whole networks against the f32 oracle on the activated detection tensors (north_star: <= 1e-3 rel)."""
-import os
-
 import numpy as np
 import pytest
 
 import ybtest_util as util
+from ybtest_util import bf16_round, tcnet
 from yolo2_light_b200 import cfgs
 
 pytestmark = pytest.mark.gpu
-
-
-def bf16_round(a):
-    """round-to-nearest-even float32 -> bfloat16 -> float32"""
-    u = np.ascontiguousarray(a, np.float32).view(np.uint32).astype(np.uint64)
-    r = ((u + 0x7FFF + ((u >> 16) & 1)) >> 16) << 16
-    return (r & 0xFFFFFFFF).astype(np.uint32).view(np.float32).reshape(np.shape(a))
-
-
-def tcnet(size=64):
-    """Exercises every tile configuration of k_conv_tc: BK 16/32/64, BN 32/64/128/256, 3x3 s1, 3x3 s2, 1x1, fused
-    shortcut, concat slice output, f32 head with 255 filters."""
-    c = cfgs._conv
-    s = [cfgs._net(size, size),
-         c(16, 3),                   # 0 stem (CUDA cores, C=3)
-         c(32, 3, 2),                # 1 s2, BK16, BN32
-         c(64, 3),                   # 2 s1, BK32, BN64
-         c(32, 1),                   # 3 1x1, BK64, BN32
-         c(64, 3),                   # 4 3x3 + fused shortcut
-         ("shortcut", {"from": "-3", "activation": "linear"}),   # 5
-         c(128, 3, 2),               # 6 s2, BK64, BN128
-         c(64, 1),                   # 7
-         c(128, 3),                  # 8
-         ("shortcut", {"from": "-3", "activation": "linear"}),   # 9
-         c(256, 3, 2),               # 10 s2 BN256
-         c(128, 1),                  # 11
-         c(256, 3),                  # 12
-         c(320, 1),                  # 13 two filter tiles (256 + 64)
-         c(255, 1, bn=False, act="linear"),   # 14 head, f32 out, n=255
-         cfgs._yolo("0,1,2", cfgs.COCO_ANCHORS, 9),              # 15
-         ("route", {"layers": "-4"}),                            # 16 -> layer 12
-         c(64, 1),                   # 17
-         ("upsample", {"stride": "2"}),                          # 18 writes a concat slice
-         ("route", {"layers": "-1, 9"}),                         # 19 concat(64 + 128) = 192 channels
-         c(128, 3),                  # 20 reads the concat (C=192, BK64)
-         c(255, 1, bn=False, act="linear"),   # 21
-         cfgs._yolo("3,4,5", cfgs.COCO_ANCHORS, 9)]              # 22
-    return s
-
-
-def _files(workdir, name, secs, seed):
-    cfg = os.path.join(workdir, name + ".cfg")
-    wts = os.path.join(workdir, name + ".weights")
-    cfgs.write_cfg(secs, cfg)
-    cfgs.write_weights(secs, wts, seed=seed)
-    return cfg, wts
 
 
 @pytest.mark.parametrize("size,batch", [(64, 2), (96, 3), ((64, 160), 2), ((96, 32), 1)])
@@ -64,16 +17,10 @@ def test_tc_every_layer_vs_oracle_on_bf16_inputs(size, batch, workdir):
     h, w = size if isinstance(size, tuple) else (size, size)
     secs = tcnet(64)
     secs[0][1]["height"], secs[0][1]["width"] = str(h), str(w)    # non-square variants exercise H != W tiling
-    cfg, wts = _files(workdir, f"tcnet{h}x{w}", secs, 21)
-    net = yb.load_network(cfg, wts, batch=batch)
-    net.set_precision(yb.YB_PREC_BF16_TC)
-    net.set_option("fuse", 0)
+    net = util.load(*util.write_net(workdir, f"tcnet{h}x{w}", secs, 21), batch, precision=yb.YB_PREC_BF16_TC, fuse=0)
     x = cfgs.synthetic_images(batch, 3, h, w, seed=5)
     net.predict(x)
-    prof = net.profile()
-    kinds = {}
-    for li, kind, ms in prof:
-        kinds.setdefault(li, []).append(kind)
+    kinds = util.profile_kinds(net)
     layers = net.layers
     got = [None] * net.n
     for i in range(net.n):
@@ -116,12 +63,10 @@ def test_tc_stride2_vs_oracle(hw, batch, streamed, workdir, monkeypatch):
     h, w = hw
     secs = s2net()
     secs[0][1]["height"], secs[0][1]["width"] = str(h), str(w)
-    cfg, wts = _files(workdir, f"s2net{h}x{w}", secs, 31)
+    cfg, wts = util.write_net(workdir, f"s2net{h}x{w}", secs, 31)
     if streamed:
         monkeypatch.setenv("YB_TC_NO_BSTAT", "1")   # filter tiles streamed through the ring instead of resident (layer 1)
-    net = yb.load_network(cfg, wts, batch=batch)
-    net.set_precision(yb.YB_PREC_BF16_TC)
-    net.set_option("fuse", 0)
+    net = util.load(cfg, wts, batch, precision=yb.YB_PREC_BF16_TC, fuse=0)
     x = cfgs.synthetic_images(batch, 3, h, w, seed=9)
     net.predict(x)
     layers = net.layers
@@ -135,13 +80,11 @@ def test_tc_stride2_vs_oracle(hw, batch, streamed, workdir, monkeypatch):
 
 
 def test_tc_fused_equals_unfused(workdir):
-    import yolo2_light_b200 as yb
-    cfg, wts = _files(workdir, "tcnet64f", tcnet(64), 22)
+    cfg, wts = util.write_net(workdir, "tcnet64f", tcnet(64), 22)
     x = cfgs.synthetic_images(2, 3, 64, 64, seed=6)
     outs = []
     for fuse in (0, 1):
-        net = yb.load_network(cfg, wts, batch=2)
-        net.set_option("fuse", fuse)
+        net = util.load(cfg, wts, 2, fuse=fuse)
         net.predict(x)
         outs.append({i: o.copy() for i, o in net.detection_outputs().items()})
         launches = net.last_launches()
@@ -156,15 +99,14 @@ def test_bf16_network_vs_f32_oracle(name, workdir):
     """Whole network, default precision, against the f32 oracle: <= 1e-3 rel-L2 on the activated yolo tensors... for
     the slim test nets the bar is 3e-3 (few channels -> less averaging of the bf16 rounding noise); the full-size
     bar is asserted in test_gpu_fullsize.py."""
-    import yolo2_light_b200 as yb
     from oracle import port
     if name == "tcnet":
-        cfg, wts = _files(workdir, "tcnet64w", tcnet(64), 23)
+        cfg, wts = util.write_net(workdir, "tcnet64w", tcnet(64), 23)
         x = cfgs.synthetic_images(2, 3, 64, 64, seed=7)
     else:
         cfg, wts = util.model_files(name, workdir)
         x = util.images(name, 2)
-    net = yb.load_network(cfg, wts, batch=2)
+    net = util.load(cfg, wts, 2)
     net.predict(x)
     layers = net.layers
     exp = [port.run_network(layers, x[b:b + 1]) for b in range(2)]
@@ -200,12 +142,10 @@ def deepknet(h, w):
 def test_tc_deepknet_vs_f32_oracle(h, w, batch, fuse, workdir):
     """The deep-K network against the f32 oracle on the detection tensors, with the bar of the other slim nets (see
     test_bf16_network_vs_f32_oracle), fused and unfused, after repeated launches of the same engine."""
-    import yolo2_light_b200 as yb
     from oracle import port
-    cfg, wts = _files(workdir, f"deepk{h}x{w}", deepknet(h, w), 31)
+    cfg, wts = util.write_net(workdir, f"deepk{h}x{w}", deepknet(h, w), 31)
     x = cfgs.synthetic_images(batch, 3, h, w, seed=9)
-    net = yb.load_network(cfg, wts, batch=batch)
-    net.set_option("fuse", fuse)
+    net = util.load(cfg, wts, batch, fuse=fuse)
     for rep in range(3):
         net.predict(x)
     assert net.get_info("tc_layers") >= 9
@@ -226,12 +166,11 @@ def test_tf32_heads_of_exact_networks(name, q, workdir):
     cfg, wts = util.model_files(name, workdir)
     B = 3
     x = util.images(name, B)
-    fast = yb.load_network(cfg, wts, batch=B, quantized=q)
+    fast = util.load(cfg, wts, B, quantized=q)
     fast.predict(x, quantized=bool(q))
     kinds = [k for _, k, _ in fast.profile(quantized=bool(q))]
     assert "conv_tc_tf32" in kinds, kinds
-    exact = yb.load_network(cfg, wts, batch=B, quantized=q)
-    exact.set_precision(yb.YB_PREC_FP32)
+    exact = util.load(cfg, wts, B, quantized=q, precision=yb.YB_PREC_FP32)
     exact.predict(x, quantized=bool(q))
     assert "conv_tc_tf32" not in [k for _, k, _ in exact.profile(quantized=bool(q))]
     for i, o in fast.detection_outputs().items():

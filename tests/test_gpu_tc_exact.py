@@ -1,13 +1,6 @@
-"""The tensor-core convolutions bit for bit, on data on which they are exact.
-
-Activations are a/8 (a in [-8, 8]; stem images a/16, a in [0, 16]), weights b/64 (b in [-8, 8]), biases c/512.  Every
-product is then exact in bf16 / tf32, every partial sum a multiple of the product grid, and while sum |x| |w| over a dot
-product stays below 2^20 grid units every partial sum is an exact f32 number in any summation order, whatever the tensor
-core's alignment of its addends and with or without FMA contraction.  The accumulator is the float64 dot product; the
-epilogue is a few IEEE f32 operations (bias add, leaky, residual add, second leaky, round to bf16) that numpy float32
-repeats bit for bit.  So every output is known to the bit, and a single wrong element -- a stale ring stage, a wrong
-bias column, a tile row stored in the wrong place -- fails the comparison, where a rel-L2 bound over the tensor would not
-notice it.  `premise` checks these conditions on the host for every convolution before anything runs.
+"""The tensor-core convolutions bit for bit, on data on which they are exact (exact_model): every output is known to the
+bit, so a single wrong element -- a stale ring stage, a wrong bias column, a tile row stored in the wrong place -- fails the
+comparison, where a rel-L2 bound over the tensor would not notice it.
 
 A layer under test that writes bf16 needs a consumer (a convolution without one writes f32): a one-hot 3x3 convolution
 (bias 0, linear, one weight of 1 per filter) whose filters see the tested output through every tap, border included.  Its
@@ -16,262 +9,14 @@ merged-row tile shows up bitwise.  Each case names the edge of the tile planner 
 Network.tc_plan.
 
 The helpers and the case table run on the CPU; the tests that need a GPU are marked."""
-import os
-import struct
-
 import numpy as np
 import pytest
 
+import exact_model
 import ybtest_util as util
-from test_gpu_tc import bf16_round
+from exact_model import (BOUND_UNITS, F32_01, LEAKY, LINEAR, LOGISTIC, RELU, Net, conv_acc, epilogue, grid_acts, grid_bias,
+                         grid_step, grid_weights, leaky_exact, leaky_tc, onehot, premise, run_reference, shifted_copies)
 from yolo2_light_b200 import cfgs
-
-LINEAR, LEAKY, RELU, LOGISTIC = "linear", "leaky", "relu", "logistic"
-BOUND_UNITS = 2 ** 20          # |partial sums| in product-grid units: 4 bits below f32's 24-bit significand
-F32_01 = np.float32(0.1)
-
-
-# ---- data ---------------------------------------------------------------------------------------------------------------
-def grid_acts(rng, shape, den=8, lo=-8, hi=8):
-    return (rng.integers(lo, hi + 1, shape) / den).astype(np.float32)
-
-
-def grid_weights(rng, n, c, k):
-    return (rng.integers(-8, 9, (n, c, k, k)) / 64).astype(np.float32)
-
-
-def grid_bias(rng, n, den=512, lim=512):
-    return (rng.integers(-lim, lim + 1, n) / den).astype(np.float32)
-
-
-def onehot(n, c, k, pairs):
-    """n filters, filter j reads channel pairs[j][0] through tap pairs[j][1] (ky * k + kx) with weight 1"""
-    w = np.zeros((n, c, k, k), np.float32)
-    for j, (ch, t) in enumerate(pairs):
-        w[j, ch, t // k, t % k] = 1.0
-    return w
-
-
-def consumer_pairs(c):
-    """(channel, tap) of every filter of a one-hot 3x3 consumer over c channels: all 9 taps of every channel (9 c filters)"""
-    return [(j % c, (j // c + j % c) % 9) for j in range(9 * c)]
-
-
-class Net:
-    """A small network under construction: cfg sections, the weights of each convolution and what each is expected to
-    run on ("reg" k_conv_tc_reg, "tc" k_conv_tc, "stem" k_stem_tc, "stem_s2" k_stem_s2_tc, "simt" the CUDA cores)."""
-
-    def __init__(self, c, h, w, batch, seed, calib=None):
-        net = cfgs._net(w, h, calib)
-        net[1]["channels"] = str(c)
-        self.secs = [net]
-        self.rng = np.random.default_rng(seed)
-        self.batch, self.c, self.h, self.w = batch, c, h, w
-        self.params = {}     # layer -> (weights [n][c][k][k], bias)
-        self.kern = {}       # layer -> expected kernel
-        self.edges = []      # (layer, description, predicate on the plan)
-        self.env = {}
-        self.quantized = 0
-        self.fuse = 1
-        self.x = None        # the input images, when a case sets them
-        self.tol = {}        # layer -> bf16 ulps its output may differ by (the double-precision logistic), else 0
-
-    @property
-    def n(self):
-        return len(self.secs) - 1
-
-    def shapes(self):
-        return cfgs.conv_shapes(self.secs)
-
-    def conv(self, n, size=3, stride=1, act=LEAKY, kern="reg", w=None, b=None, **extra):
-        self.secs.append(cfgs._conv(n, size, stride, bn=False, act=act, **extra))
-        c = self.shapes()[-1]["c"]
-        w = grid_weights(self.rng, n, c, size) if w is None else w
-        b = grid_bias(self.rng, n) if b is None else b
-        i = self.n - 1
-        self.params[i] = (np.asarray(w, np.float32), np.asarray(b, np.float32))
-        self.kern[i] = kern
-        return i
-
-    def preserve(self, kern="reg"):
-        """grid-preserving 1x1 layer: one-hot weights over a permutation of the channels, a bias on the activation grid,
-        linear -- its output stays exactly on the activation grid"""
-        c = self.shapes()[-1]["out_c"] if self.n else self.c
-        perm = self.rng.permutation(c)
-        w = onehot(c, c, 1, [(int(perm[j]), 0) for j in range(c)])
-        return self.conv(c, 1, 1, LINEAR, kern, w=w, b=grid_acts(self.rng, c, 8, -4, 4))
-
-    def consume(self):
-        """one-hot 3x3 consumer of the last layer's output (f32 out when it is the last layer): k_conv_tc where its channels
-        fill whole 32-byte bf16 rows, else the CUDA cores"""
-        c = self.shapes()[-1]["out_c"]
-        pairs = consumer_pairs(c)
-        kern = "tc" if c % 16 == 0 else "simt"
-        return self.conv(len(pairs), 3, 1, LINEAR, kern, w=onehot(len(pairs), c, 3, pairs), b=np.zeros(len(pairs), np.float32))
-
-    def add(self, name, **opts):
-        self.secs.append((name, {k: str(v) for k, v in opts.items()}))
-        return self.n - 1
-
-    def edge(self, layer, what, pred):
-        self.edges.append((layer, what, pred))
-        return self
-
-    def images(self, den=8, lo=-8, hi=8):
-        return grid_acts(np.random.default_rng(self.rng.integers(1 << 30)), (self.batch, self.c, self.h, self.w), den, lo, hi)
-
-
-def write_weights(net, path):
-    """The convolutions' weights in the reference's .weights format (cfgs.write_weights), no batch norm: biases[n], then
-    weights[n][c][k][k] per convolution in cfg order"""
-    with open(path, "wb") as f:
-        f.write(struct.pack("<iiiQ", 0, 2, 0, 0))
-        for i in sorted(net.params):
-            w, b = net.params[i]
-            b.astype("<f4").tofile(f)
-            w.astype("<f4").tofile(f)
-    return path
-
-
-# ---- reference ----------------------------------------------------------------------------------------------------------
-def conv_acc(x, w, stride, pad):
-    """float64 accumulators of a convolution over NHWC x: one matmul per tap"""
-    x = np.asarray(x, np.float64)
-    B, H, W, C = x.shape
-    n, _, k, _ = w.shape
-    OH, OW = (H + 2 * pad - k) // stride + 1, (W + 2 * pad - k) // stride + 1
-    xp = np.zeros((B, H + 2 * pad, W + 2 * pad, C))
-    xp[:, pad:pad + H, pad:pad + W] = x
-    acc = np.zeros((B, OH, OW, n))
-    w = np.asarray(w, np.float64)
-    for ky in range(k):
-        for kx in range(k):
-            xs = xp[:, ky:ky + stride * (OH - 1) + 1:stride, kx:kx + stride * (OW - 1) + 1:stride, :]
-            acc += xs @ w[:, :, ky, kx].T
-    return acc
-
-
-def grid_step(a):
-    """the coarsest power of two 2^-e (e <= 40) of which every element of a is a multiple"""
-    a = np.asarray(a, np.float64)
-    for e in range(41):
-        s = a * 2.0 ** e
-        if np.array_equal(s, np.round(s)):
-            return 2.0 ** -e
-    raise AssertionError("data off every binary grid")
-
-
-def premise(x, w, b, stride, pad):
-    """every partial sum of the convolution, and the bias add, is exact in f32 in any order; returns the largest
-    sum |x| |w| + |b| in units of the grid of those sums (0 for one-hot filters)"""
-    nz = w != 0
-    if np.all(nz.reshape(len(w), -1).sum(1) <= 1) and np.all(np.abs(w[nz]) == 1):
-        # one-hot filters: a single product per output, then the bias add, which must be exact itself
-        acc = conv_acc(x, w, stride, pad) + 0.0
-        s = acc.astype(np.float32) + b.astype(np.float32)
-        assert np.array_equal(s.astype(np.float64), acc + np.asarray(b, np.float64)), "one-hot layer: bias add rounds"
-        return 0.0
-    g = min(grid_step(x) * grid_step(w), grid_step(b))     # every partial sum and the bias add are multiples of g
-    units = (conv_acc(np.abs(x), np.abs(w), stride, pad) + np.abs(b)).max() / g
-    assert units < BOUND_UNITS, f"sum |x||w| = {units:.3g} grid units >= 2^20"
-    return units
-
-
-def leaky_tc(a):
-    """fmaxf(a, 0.1f * a): the epilogues of k_conv_tc_reg, k_conv_tc, k_stem_tc and k_stem_s2_tc"""
-    return np.maximum(a, F32_01 * a)
-
-
-def leaky_exact(a):
-    """act_exact: a > 0 ? a : (float)(0.1 * (double)a), the CUDA-core kernels (the reference's activate())"""
-    return np.where(a > 0, a, (0.1 * a.astype(np.float64)).astype(np.float32)).astype(np.float32)
-
-
-def activate(a, act, kern):
-    """the epilogue's activation: leaky as leaky_exact on the CUDA cores and leaky_tc on the tensor cores; relu and logistic
-    only run on the CUDA cores (act_exact): x * (x > 0), which is -0 for x < 0, and (float)(1 / (1 + exp(-(double)x))), which
-    numpy's float64 exp reproduces to within one f32 ulp"""
-    if act == LEAKY:
-        return leaky_exact(a) if kern == "simt" else leaky_tc(a)
-    if act == RELU:
-        return a * (a > 0)
-    if act == LOGISTIC:
-        return (1.0 / (1.0 + np.exp(-a.astype(np.float64)))).astype(np.float32)
-    assert act == LINEAR, act
-    return a
-
-
-def epilogue(acc, b, act, kern, res=None, act2=LINEAR, bf16=True):
-    a = activate((acc + 0.0).astype(np.float32) + b.astype(np.float32), act, kern)
-    if res is not None:
-        a = activate(a + res.astype(np.float32), act2, kern)
-    return bf16_round(a) if bf16 else a.astype(np.float32)
-
-
-def run_reference(net, x, adt_bf16=True):
-    """Host model of the engine on these networks: every layer's output as stored (NHWC f32 values; bf16-rounded where the
-    engine keeps bf16), the [yolo] layers' raw head values, and the premise of every convolution.  Follows the engine's
-    layer plan: bf16 outputs unless a convolution has no consumer or only detection layers read it; conv + same-shape
-    shortcut fused when `fuse` is on, the conv is stride 1 and the shortcut its sole reader."""
-    shapes = net.shapes()
-    secs = net.secs[1:]
-    cons = {i: [] for i in range(len(secs))}
-    for i, L in enumerate(shapes):
-        t = L["type"]
-        if t == "route":
-            for j in L["layers"]:
-                cons[j].append(i)
-        elif t == "shortcut":
-            cons[i - 1].append(i); cons[L["index"]].append(i)
-        elif i > 0:
-            cons[i - 1].append(i)
-    outs, units = {}, {}
-    cur = np.ascontiguousarray(x.transpose(0, 2, 3, 1))
-    if net.kern.get(0, "").startswith("stem"):
-        cur = bf16_round(cur) if adt_bf16 else cur
-    fused_res = {}
-    for i, L in enumerate(shapes):
-        t = L["type"]
-        if t == "convolutional":
-            w, b = net.params[i]
-            units[i] = premise(cur, w, b, L["stride"], L["pad"])
-            acc = conv_acc(cur, w, L["stride"], L["pad"])
-            heads_only = bool(cons[i]) and all(shapes[r]["type"] in ("yolo", "region") for r in cons[i])
-            bf16 = adt_bf16 and bool(cons[i]) and not heads_only
-            nxt = shapes[i + 1] if i + 1 < len(shapes) else None
-            if (net.fuse and nxt is not None and nxt["type"] == "shortcut" and cons[i] == [i + 1] and L["stride"] == 1
-                    and nxt["index"] != i):
-                fused_res[i + 1] = (acc, b, L["activation"], net.kern[i])
-                outs[i] = None
-                continue
-            cur = epilogue(acc, b, L["activation"], net.kern[i], bf16=bf16)
-        elif t == "shortcut":
-            res = outs[L["index"]]
-            act2 = secs[i][1].get("activation", LINEAR)
-            if i in fused_res:
-                acc, b, act, kern = fused_res[i]
-                cur = epilogue(acc, b, act, kern, res=res, act2=act2, bf16=adt_bf16)
-            else:
-                a = cur + res
-                cur = leaky_exact(a) if act2 == LEAKY else a
-                cur = bf16_round(cur) if adt_bf16 else cur
-        elif t == "route":
-            cur = np.concatenate([outs[j] for j in L["layers"]], axis=3)
-        elif t == "yolo":
-            pass   # the head's f32 values stay in `cur`; the test applies the logistic
-        else:
-            raise NotImplementedError(t)
-        outs[i] = cur
-    return outs, units
-
-
-def shifted_copies(t, pairs):
-    """the one-hot 3x3 consumer's output: filter j = t[..., c_j] shifted by tap t_j, zero border (NHWC); + 0 as the
-    consumer's accumulator, which starts at +0 and so turns a -0 input (relu) into +0"""
-    B, H, W, C = t.shape
-    tp = np.zeros((B, H + 2, W + 2, C), np.float32)
-    tp[:, 1:H + 1, 1:W + 1] = t + np.float32(0)
-    return np.stack([tp[:, tap // 3:tap // 3 + H, tap % 3:tap % 3 + W, c] for c, tap in pairs], axis=3)
 
 
 # ---- the case table -----------------------------------------------------------------------------------------------------
@@ -520,14 +265,6 @@ def build_case(name):
     return net, x
 
 
-def logistic_bound(v):
-    """|__fdividef(1, 1 + __expf(-v)) - 1 / (1 + exp(-v))| bound (CUDA C Programming Guide, intrinsic functions): __expf(x)
-    is within 2 + floor(|1.173 x|) ulp, __fdividef within 2 ulp for a divisor in [2^-126, 2^126]; the 1 + e add rounds
-    once more (1/2 ulp).  The relative error of 1 + e is at most that of e, so the result is within
-    (2 + floor(|1.173 v|) + 0.5 + 2) ulp of an f32 value, relative to the result."""
-    return (4.5 + np.floor(np.abs(1.173 * v))) * 2.0 ** -23
-
-
 # ---- CPU tests ----------------------------------------------------------------------------------------------------------
 def test_calibration_case_reaches_the_top_of_the_bound():
     """the calibration case holds the accumulator between 2^19 and 2^20 units of its product grid (2^-9)"""
@@ -586,7 +323,7 @@ def test_case_sensitivity(name):
         L = shapes[i]
         cur = np.ascontiguousarray(x.transpose(0, 2, 3, 1)) if i == 0 else outs[i - 1]
         if net.kern[i].startswith("stem") and i == 0:
-            cur = bf16_round(cur)
+            cur = util.bf16_round(cur)
         w, b = net.params[i]
         bf16 = not net.quantized and shapes[i + 1]["type"] != "yolo" if i + 1 < len(shapes) else False
         act = L["activation"]
@@ -612,15 +349,6 @@ def test_case_sensitivity(name):
 KERNEL_OF = {"reg": "k_conv_tc_reg", "tc": "k_conv_tc", "stem": "k_stem_tc", "stem_s2": "k_stem_s2_tc"}
 
 
-def _load(net, workdir, name):
-    import yolo2_light_b200 as yb
-    cfg = cfgs.write_cfg(net.secs, os.path.join(workdir, name + ".cfg"))
-    wts = write_weights(net, os.path.join(workdir, name + ".weights"))
-    m = yb.load_network(cfg, wts, batch=net.batch, quantized=net.quantized)
-    m.set_option("fuse", net.fuse)
-    return m
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_tc_exact(name, workdir, monkeypatch):
@@ -628,7 +356,7 @@ def test_tc_exact(name, workdir, monkeypatch):
     exp, _ = run_reference(net, x, adt_bf16=not net.quantized)
     for k, v in net.env.items():
         monkeypatch.setenv(k, v)
-    m = _load(net, workdir, name)
+    m = util.load(*exact_model.write_net(net, workdir, name), net.batch, quantized=net.quantized, fuse=net.fuse)
     q = bool(net.quantized)
     # the plan of every convolution is the one the case is for
     for i, kern in net.kern.items():
@@ -665,7 +393,7 @@ def test_tc_exact(name, workdir, monkeypatch):
             assert util.bits_equal(got[:, raw], v[:, raw]), name
             sg = 1.0 / (1.0 + np.exp(-v[:, ~raw].astype(np.float64)))
             err = np.abs(got[:, ~raw] - sg) / sg
-            assert np.all(err <= logistic_bound(v[:, ~raw])), (name, float(err.max()))
+            assert np.all(err <= util.logistic_bound(v[:, ~raw])), (name, float(err.max()))
             checked += 1
             continue
         if e is None or (L["type"] == "convolutional" and i + 1 < len(shapes) and shapes[i + 1]["type"] == "yolo"):
@@ -675,8 +403,9 @@ def test_tc_exact(name, workdir, monkeypatch):
         got = m.fetch_layer(i, quantized=q).transpose(0, 2, 3, 1)
         assert got.shape == e.shape, (name, i)
         if net.tol.get(i):
-            d = np.abs(got.view(np.int32).astype(np.int64) - np.ascontiguousarray(e).view(np.int32).astype(np.int64)) >> 16
-            assert np.all(got >= 0) and np.all(e >= 0) and d.max() <= net.tol[i], (name, i, int(d.max()))   # logistic > 0, border 0
+            d = util.ulp_diff(got, e, True)
+            assert np.all(got >= 0) and np.all(e >= 0) and np.array_equal(np.signbit(got), np.signbit(e)) and \
+                d.max() <= net.tol[i], (name, i, int(d.max()))   # logistic > 0, border 0
             checked += 1
             continue
         bad = np.argwhere(got.view(np.uint32) != np.ascontiguousarray(e).view(np.uint32))
@@ -698,24 +427,9 @@ def _is_consumer(net, i):
 
 
 # ---- integer kinds at the edge shapes: bit for bit against the oracle on the fetched input ---------------------------
-def _int_net(workdir, name, secs, batch, quantized, seed):
-    import yolo2_light_b200 as yb
-    cfg = cfgs.write_cfg(secs, os.path.join(workdir, name + ".cfg"))
-    wts = cfgs.write_weights(secs, os.path.join(workdir, name + ".weights"), seed=seed)
-    return yb.load_network(cfg, wts, batch=batch, quantized=quantized)
-
-
 def _int_secs(C, h, w, quantized):
     net = cfgs._net(w, h, [16] * 8 if quantized else None)
     return [net, cfgs._conv(C, 3)]     # layer 0: f32 (the INT8 rule starts at layer 1), leaky
-
-
-def _int_ref(l, x, quantized):
-    from oracle import port
-    if quantized:
-        return port.conv_int8(x, l["weights_int8"], l["biases"], l["input_quant_multipler"], l["weights_quant_multipler"],
-                              l["n"], l["size"], l["stride"], l["pad"], l["activation"], want_acc=True)
-    return port.conv_xnor(x, l["weights"], l["biases"], l["mean_arr"], l["n"], l["size"], l["activation"], want_counts=True)
 
 
 INT_SHAPES = [   # kind, C, n, h, w, stride, batch: padded channels (C % 32 != 0), n % 4 != 0, odd sizes, stride 2
@@ -731,13 +445,13 @@ def test_integer_kinds_exact(kind, C, n, h, w, stride, batch, workdir):
     q = kind == "s8"
     secs = _int_secs(C, h, w, q)
     secs.append(cfgs._conv(n, 3, stride, **({} if q else {"xnor": 1, "bin_output": 1})))
-    m = _int_net(workdir, f"int_{kind}_{C}_{n}_{h}x{w}s{stride}", secs, batch, int(q), C + n)
+    m = util.load(*util.write_net(workdir, f"int_{kind}_{C}_{n}_{h}x{w}s{stride}", secs, C + n), batch, quantized=int(q))
     m.set_option("keep_counts", 1)
     p = m.tc_plan(1, quantized=q)
     assert p.get("kind") == kind and p["kernel"] == "k_conv_tc", p
     assert p["tma_epi"] == 0, p    # keep_counts: the raw accumulators go through the LSU stores
     m.predict(cfgs.synthetic_images(batch, 3, h, w, seed=C), quantized=q)
-    exp, acc = _int_ref(m.layers[1], m.fetch_layer(0, quantized=q), q)
+    exp, acc = util.oracle_layer(m.layers[1], 1, m.fetch_layer(0, quantized=q), int(q))
     assert np.array_equal(m.fetch_counts(1, quantized=q), acc)
     assert util.bits_equal(m.fetch_layer(1, quantized=q), exp)
     # and without the raw-accumulator dump: the TMA epilogue at stride 1, the LSU stores at stride 2
@@ -758,11 +472,11 @@ def test_integer_kinds_role_counters(kind, workdir, monkeypatch, capfd):
     monkeypatch.setenv("YB_TC_GRID", "2")   # several work items per CTA
     q = kind == "s8"
     secs = _int_secs(40 if q else 48, 11, 13, q) + [cfgs._conv(40, 3, **({} if q else {"xnor": 1, "bin_output": 1}))]
-    m = _int_net(workdir, f"stats_{kind}", secs, 2, int(q), 11)
+    m = util.load(*util.write_net(workdir, f"stats_{kind}", secs, 11), 2, quantized=int(q))
     p = m.tc_plan(1, quantized=q)
     assert p.get("kind") == kind and p["kernel"] == "k_conv_tc" and p["num_work"] > p["grid"], p
     m.predict(cfgs.synthetic_images(2, 3, 11, 13, seed=4), quantized=q)
-    exp, _ = _int_ref(m.layers[1], m.fetch_layer(0, quantized=q), q)
+    exp, _ = util.oracle_layer(m.layers[1], 1, m.fetch_layer(0, quantized=q), int(q))
     assert util.bits_equal(m.fetch_layer(1, quantized=q), exp)
     capfd.readouterr()
     del m
@@ -781,13 +495,13 @@ def test_pool_fused_epilogue_exact(kind, h, w, batch, workdir):
     extra = {} if q else {"xnor": 1, "bin_output": 1}
     secs = _int_secs(32, h, w, q) + [cfgs._conv(32, 3, **extra), ("maxpool", {"size": "2", "stride": "2"}),
                                       cfgs._conv(32, 3, **extra)]
-    m = _int_net(workdir, f"pool_{kind}_{h}x{w}", secs, batch, int(q), 7 + h)
+    m = util.load(*util.write_net(workdir, f"pool_{kind}_{h}x{w}", secs, 7 + h), batch, quantized=int(q))
     p = m.tc_plan(1, quantized=q)
     assert p.get("kind") == kind and p["jshift"] == 1 and p["TW"] == 8, p    # pool fused: 8 x 16 tiles, one row down
     m.predict(cfgs.synthetic_images(batch, 3, h, w, seed=h), quantized=q)
     L = m.layers
-    y1, _ = _int_ref(L[1], m.fetch_layer(0, quantized=q), q)
-    y3, _ = _int_ref(L[3], port.maxpool(y1, L[2]["size"], L[2]["stride"], L[2]["pad"]), q)
+    y1, _ = util.oracle_layer(L[1], 1, m.fetch_layer(0, quantized=q), int(q))
+    y3, _ = util.oracle_layer(L[3], 3, port.maxpool(y1, L[2]["size"], L[2]["stride"], L[2]["pad"]), int(q))
     assert util.bits_equal(m.fetch_layer(3, quantized=q), y3)
 
 
@@ -802,14 +516,14 @@ def test_int8_slice_store_leaves_the_next_slice(workdir):
                                           cfgs._conv(30, 3, 2),                     # 3: INT8 stride 2, first slice
                                           ("route", {"layers": "-1, -3"}),          # 4: [layer 3, layer 1]
                                           cfgs._conv(16, 1)]
-    m = _int_net(workdir, "slice_spill", secs, 2, 1, 5)
+    m = util.load(*util.write_net(workdir, "slice_spill", secs, 5), 2, quantized=1)
     assert m.tc_plan(1, quantized=True) == {}
     p = m.tc_plan(3, quantized=True)
     assert p.get("kind") == "s8" and p["tma_epi"] == 0, p
     m.predict(cfgs.synthetic_images(2, 3, 6, 10, seed=3), quantized=True)
     L = m.layers
-    y1, _ = _int_ref(L[1], m.fetch_layer(0, quantized=True), True)
-    y3, _ = _int_ref(L[3], port.upsample(y1, 2), True)
+    y1, _ = util.oracle_layer(L[1], 1, m.fetch_layer(0, quantized=True), 1)
+    y3, _ = util.oracle_layer(L[3], 3, port.upsample(y1, 2), 1)
     got = m.fetch_layer(4, quantized=True)
     assert util.bits_equal(got[:, :30], y3)
     assert util.bits_equal(got[:, 30:], y1), "layer 3 overwrote layer 1's channels"
@@ -951,7 +665,8 @@ def test_production_shape_exact(key, workdir):
     net, i = production_net(key)
     stem = key[-1] == "stem_s2"
     x = net.images(16, 0, 16) if stem else net.images()
-    m = _load(net, workdir, "prod_{}x{}x{}_n{}_k{}s{}_{}".format(*key))
+    m = util.load(*exact_model.write_net(net, workdir, "prod_{}x{}x{}_n{}_k{}s{}_{}".format(*key)), net.batch,
+                  quantized=net.quantized, fuse=net.fuse)
     p = m.tc_plan(i)
     assert p.get("kernel") == KERNEL_OF[net.kern[i]] and p["kind"] == "bf16", (key, p)
     if net.kern[i] == "reg":

@@ -6,8 +6,7 @@ import numpy as np
 import pytest
 
 import ybtest_util as util
-from test_gpu_tc import _files, tcnet
-from test_gpu_tc_wide import widenet
+from ybtest_util import tcnet, widenet
 from yolo2_light_b200 import cfgs
 
 pytestmark = pytest.mark.gpu
@@ -18,10 +17,9 @@ NETS = {"widenet": (widenet, 32, 31, 8), "tcnet": (lambda: tcnet(64), 64, 21, 5)
 @pytest.mark.parametrize("bn", ["32", "64", "128", "256"])
 @pytest.mark.parametrize("name", list(NETS))
 def test_tc_small_grid_bit_equal_to_full_grid(name, bn, workdir, monkeypatch):
-    import yolo2_light_b200 as yb
     from oracle import port
     build, size, wseed, xseed = NETS[name]
-    cfg, wts = _files(workdir, f"{name}_grid", build(), wseed)
+    cfg, wts = util.write_net(workdir, f"{name}_grid", build(), wseed)
     x = cfgs.synthetic_images(2, 3, size, size, seed=xseed)
     monkeypatch.setenv("YB_TC_BN", bn)
     exp = None
@@ -32,15 +30,11 @@ def test_tc_small_grid_bit_equal_to_full_grid(name, bn, workdir, monkeypatch):
                 monkeypatch.setenv("YB_TC_GRID", grid)
             else:
                 monkeypatch.delenv("YB_TC_GRID", raising=False)
-            net = yb.load_network(cfg, wts, batch=2)
-            net.set_option("fuse", fuse)
+            net = util.load(cfg, wts, 2, fuse=fuse)
             net.predict(x)
-            got = {}
-            for i in range(net.n):
-                try:
-                    got[i] = net.fetch_layer(i)
-                except yb.YbError:   # with fusion on, a conv fused into its shortcut has no output of its own
-                    assert fuse, i
+            got = util.fetch_all(net)
+            # with fusion on, a conv fused into its shortcut has no output of its own
+            assert fuse or len(got) == net.n, (fuse, sorted(got))
             dets = {i: o.copy() for i, o in net.detection_outputs().items()}
             if exp is None:
                 exp = [port.run_network(net.layers, x[b:b + 1]) for b in range(2)]

@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 
 import ybtest_util as util
-from test_gpu_tc import _files, bf16_round
+from ybtest_util import bf16_round, s2chain
 from yolo2_light_b200 import cfgs
 
 pytestmark = pytest.mark.gpu
@@ -19,29 +19,12 @@ SHAPES = [((152, 152), 3), ((232, 136), 3)]
 TW = {(152, 152): (16, 1, 2), (232, 136): (4, 2, 4)}   # the tile width of stride-2 layers 1, 3 and 5
 
 
-def s2chain():
-    c = cfgs._conv
-    return [cfgs._net(64, 64),
-            c(32, 3),                   # 0 stem
-            c(64, 3, 2),                # 1 s2, C=32
-            c(64, 3),                   # 2 s1 over layer 1's borders
-            c(128, 3, 2),               # 3 s2
-            c(128, 3),                  # 4
-            c(256, 3, 2),               # 5 s2, up to 256 filters per tile
-            c(256, 3),                  # 6
-            c(255, 1, bn=False, act="linear"),
-            cfgs._yolo("0,1,2", cfgs.COCO_ANCHORS, 9)]
-
-
 def _net(workdir, hw, batch, seed):
     import yolo2_light_b200 as yb
     h, w = hw
     secs = s2chain()
     secs[0][1]["height"], secs[0][1]["width"] = str(h), str(w)
-    cfg, wts = _files(workdir, f"s2chain{h}x{w}", secs, seed)
-    net = yb.load_network(cfg, wts, batch=batch)
-    net.set_precision(yb.YB_PREC_BF16_TC)
-    net.set_option("fuse", 0)
+    net = util.load(*util.write_net(workdir, f"s2chain{h}x{w}_{seed}", secs, seed), batch, precision=yb.YB_PREC_BF16_TC, fuse=0)
     return net, cfgs.synthetic_images(batch, 3, h, w, seed=seed + 1)
 
 
@@ -52,9 +35,7 @@ def test_tc_stride2_reg_every_layer_vs_oracle(hw, batch, bn, workdir, monkeypatc
     monkeypatch.setenv("YB_TC_BN", bn)
     net, x = _net(workdir, hw, batch, 41)
     net.predict(x)
-    kinds = {}
-    for li, kind, _ in net.profile():
-        kinds.setdefault(li, []).append(kind)
+    kinds = util.profile_kinds(net)
     layers = net.layers
     got = [net.fetch_layer(i) for i in range(net.n)]
     for i, tw in zip((1, 3, 5), TW[hw]):

@@ -5,7 +5,7 @@ import numpy as np
 import pytest
 
 import ybtest_util as util
-from test_gpu_tc import _files, bf16_round, tcnet
+from ybtest_util import bf16_round, tcnet, widenet
 from yolo2_light_b200 import cfgs
 
 pytestmark = pytest.mark.gpu
@@ -15,15 +15,10 @@ def test_tc_bn256_every_layer_vs_oracle(workdir, monkeypatch):
     import yolo2_light_b200 as yb
     from oracle import port
     monkeypatch.setenv("YB_TC_BN", "256")
-    cfg, wts = _files(workdir, "tcnet64bn256", tcnet(64), 21)
-    net = yb.load_network(cfg, wts, batch=2)
-    net.set_precision(yb.YB_PREC_BF16_TC)
-    net.set_option("fuse", 0)
+    net = util.load(*util.write_net(workdir, "tcnet64bn256", tcnet(64), 21), 2, precision=yb.YB_PREC_BF16_TC, fuse=0)
     x = cfgs.synthetic_images(2, 3, 64, 64, seed=5)
     net.predict(x)
-    kinds = {}
-    for li, kind, ms in net.profile():
-        kinds.setdefault(li, []).append(kind)
+    kinds = util.profile_kinds(net)
     layers = net.layers
     got = [net.fetch_layer(i) for i in range(net.n)]
     for i, l in enumerate(layers):
@@ -37,35 +32,16 @@ def test_tc_bn256_every_layer_vs_oracle(workdir, monkeypatch):
         assert util.rel_l2(got[i], exp) <= 5e-4, i
 
 
-def widenet():
-    """Fused shortcuts on 256-filter layers, a 1x1 and a 3x3, and a masked second filter tile."""
-    c = cfgs._conv
-    return [cfgs._net(32, 32),
-            c(32, 3),
-            c(64, 3, 2),
-            c(256, 1),                  # 2
-            c(128, 1),                  # 3
-            c(256, 3),                  # 4 + fused shortcut
-            ("shortcut", {"from": "-3", "activation": "linear"}),   # 5
-            c(256, 1),                  # 6 + fused shortcut (1x1)
-            ("shortcut", {"from": "-2", "activation": "linear"}),   # 7
-            c(320, 3),                  # 8
-            c(255, 1, bn=False, act="linear"),
-            cfgs._yolo("0,1,2", cfgs.COCO_ANCHORS, 9)]
-
-
 @pytest.mark.parametrize("bn", ["256", None])
 def test_tc_wide_fused_shortcut_vs_f32_oracle(bn, workdir, monkeypatch):
-    import yolo2_light_b200 as yb
     from oracle import port
     if bn:
         monkeypatch.setenv("YB_TC_BN", bn)
-    cfg, wts = _files(workdir, "widenet", widenet(), 31)
+    cfg, wts = util.write_net(workdir, "widenet", widenet(), 31)
     x = cfgs.synthetic_images(2, 3, 32, 32, seed=8)
     outs = []
     for fuse in (0, 1):
-        net = yb.load_network(cfg, wts, batch=2)
-        net.set_option("fuse", fuse)
+        net = util.load(cfg, wts, 2, fuse=fuse)
         net.predict(x)
         outs.append({i: o.copy() for i, o in net.detection_outputs().items()})
         if fuse:

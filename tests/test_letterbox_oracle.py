@@ -5,21 +5,9 @@ import numpy as np
 import pytest
 
 import ybtest_util as util
-from letterbox_util import letterbox_size, port_letterbox_u8, ref_letterbox_u8
+from letterbox_util import LETTERBOX_CASES, SIZES, letterbox_size, port_letterbox_u8, ref_letterbox_u8
 
 NET = 64
-# (w, h) -> (nw, nh, dx, dy) in a 64 x 64 network: wide, tall, already its letterbox size, the network's aspect ratio,
-# an upscale with an odd margin, a target height of 2, and rows wider than the resize kernel stages in shared memory
-LETTERBOX_CASES = {
-    (640, 480): (64, 48, 0, 8),
-    (100, 300): (21, 64, 21, 0),
-    (64, 36): (64, 36, 0, 14),
-    (128, 128): (64, 64, 0, 0),
-    (35, 17): (64, 31, 0, 16),
-    (640, 20): (64, 2, 0, 31),
-    (4500, 400): (64, 5, 0, 29),
-}
-SIZES = list(LETTERBOX_CASES)
 
 
 def _frame(w, h, seed):

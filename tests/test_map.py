@@ -12,85 +12,9 @@ import ybtest_util as util
 pytestmark = pytest.mark.skipif(not util.have_ref(), reason="reference build absent")
 
 
-def _write_bmp(path, img):   # img: u8 [h, w, 3] RGB
-    h, w, _ = img.shape
-    row = (3 * w + 3) // 4 * 4
-    data = bytearray()
-    for y in range(h - 1, -1, -1):
-        line = img[y, :, ::-1].tobytes()
-        data += line + b"\0" * (row - len(line))
-    hdr = b"BM" + (54 + len(data)).to_bytes(4, "little") + b"\0\0\0\0" + (54).to_bytes(4, "little")
-    dib = (40).to_bytes(4, "little") + w.to_bytes(4, "little") + h.to_bytes(4, "little") + (1).to_bytes(2, "little") + \
-        (24).to_bytes(2, "little") + (0).to_bytes(4, "little") + len(data).to_bytes(4, "little") + \
-        (2835).to_bytes(4, "little") * 2 + (0).to_bytes(4, "little") * 2
-    open(path, "wb").write(hdr + dib + bytes(data))
-
-
 @pytest.mark.parametrize("name,iou_thresh", [("tiny64", 0.5), ("v3_32", 0.5), ("tiny64", 0.75)])
 def test_map_accounting_equals_reference(name, iou_thresh, workdir):
-    import yolo2_light_b200 as yb
-    from oracle import ref
-    cfg, wts = util.model_files(name, workdir)
-    rnet = ref.RefNet(cfg, wts, 1, 0, 7)
-    classes = rnet.layers[-1]["classes"]
-    root = os.path.join(workdir, f"mapset_{name}_{int(iou_thresh * 100)}")
-    os.makedirs(os.path.join(root, "images"), exist_ok=True)
-    os.makedirs(os.path.join(root, "labels"), exist_ok=True)
-    rng = np.random.default_rng(11)
-    nimg = 7
-    rows, truth, paths = [], [], []
-    for k in range(nimg):
-        img = rng.integers(0, 256, size=(72 + 4 * k, 80, 3), dtype=np.uint8)
-        path = os.path.join(root, "images", f"img{k}.bmp")
-        _write_bmp(path, img)
-        paths.append(path)
-        x = ref.load_resize_u8(img, rnet.width, rnet.height)[None]      # what load_image + resize_image hand to the net
-        rnet.predict(x)
-        r = np.delete(rnet.get_boxes(1, 1, 0.005, 0.45), 5, axis=1)      # get_network_boxes(net, 1, 1, .005, ...) + NMS
-        rows.append(r)
-        # labels: some of the strongest detections (true positives), jittered copies (IoU near the threshold), strays
-        lab = []
-        if r.shape[0]:
-            best = np.argsort(-r[:, 5:].max(axis=1))[:4]
-            for j, i in enumerate(best):
-                cls = int(np.argmax(r[i, 5:]))
-                box = r[i, :4].astype(np.float64)
-                if j % 2:
-                    box = box * (1.0 + 0.08 * rng.standard_normal(4))
-                lab.append((cls, *[round(float(v), 4) for v in box]))
-        lab.append((int(rng.integers(0, classes)), 0.5, 0.5, 0.2, 0.3))
-        if k == 3:
-            lab = []                                                     # an image without labels (no file at all)
-        else:
-            with open(os.path.join(root, "labels", f"img{k}.txt"), "w") as f:
-                for cls, bx, by, bw, bh in lab:
-                    f.write(f"{cls} {bx:.4f} {by:.4f} {bw:.4f} {bh:.4f}\n")
-        for cls, bx, by, bw, bh in lab:
-            truth.append((k, cls, float(f"{bx:.4f}"), float(f"{by:.4f}"), float(f"{bw:.4f}"), float(f"{bh:.4f}")))
-    open(os.path.join(root, "valid.txt"), "w").write("\n".join(paths) + "\n")
-    open(os.path.join(root, "names.txt"), "w").write("\n".join(f"c{i}" for i in range(classes)) + "\n")
-    datacfg = os.path.join(root, "data.cfg")
-    open(datacfg, "w").write(f"classes = {classes}\nvalid = {root}/valid.txt\nnames = {root}/names.txt\n")
-
-    out = ref.validate_map(datacfg, cfg, wts, 0.24, 0, iou_thresh, os.path.join(root, "ref_stdout.txt"))
-    ap_ref = {int(m.group(1)): float(m.group(2)) for m in re.finditer(r"class_id = (\d+), name = \S+,\s+ap = ([0-9.]+) %", out)}
-    m = re.search(r"(?:mean average precision \(mAP\)|average precision \(AP\)) = ([0-9.]+)", out)
-    assert m and len(ap_ref) == classes, out[-400:]
-    map_ref = float(m.group(1))
-    tp, fp, fn, aiou = re.search(r"TP = (\d+), FP = (\d+), FN = (\d+), average IoU = ([0-9.]+) %", out).groups()
-    prf = re.search(r"precision = ([0-9.]+), recall = ([0-9.]+), F1-score = ([0-9.]+)", out).groups()
-    ndet = int(re.search(r"detections_count = (\d+), unique_truth_count = (\d+)", out).group(1))
-
-    mAP, ap, st = yb.api.map_evaluate(rows, np.array(truth, np.float32).reshape(-1, 6), classes, iou_thresh, 0.24)
-    assert int(st["detections"]) == ndet
-    assert (int(st["tp"]), int(st["fp"]), int(st["fn"])) == (int(tp), int(fp), int(fn))
-    assert abs(mAP - map_ref) < 5e-7, (mAP, map_ref)                      # the reference prints %f
-    for c in range(classes):
-        assert abs(ap[c] * 100 - ap_ref[c]) <= 0.00501, (c, ap[c], ap_ref[c])   # printed with %2.2f
-    assert abs(st["avg_iou"] * 100 - float(aiou)) <= 0.00501
-    for mine, theirs in zip((st["precision"], st["recall"], st["f1"]), prf):
-        assert abs(mine - float(theirs)) <= 0.00501 or (np.isnan(mine) and "nan" in theirs)
-    assert int(tp) > 0 and mAP > 0                                       # the dataset exercises the matching at all
+    util.check_map_accounting(name, iou_thresh, workdir)
 
 
 def test_dataset_reader_matches_what_the_reference_reads(workdir):
@@ -105,7 +29,7 @@ def test_dataset_reader_matches_what_the_reference_reads(workdir):
     for w, h in ((80, 72), (33, 50)):                       # a width whose rows need BMP padding, too
         img = rng.integers(0, 256, size=(h, w, 3), dtype=np.uint8)
         p = os.path.join(root, "images", f"i{w}.bmp")
-        _write_bmp(p, img)
+        util.write_bmp(p, img)
         assert np.array_equal(dataset.read_image_u8(p), img)
         ppm = os.path.join(root, "images", f"i{w}.ppm")
         open(ppm, "wb").write(b"P6\n# c\n%d %d\n255\n" % (w, h) + img.tobytes())
@@ -136,7 +60,7 @@ def test_map_driver_loop_equals_reference_end_to_end(workdir):
     classes = rnet.layers[-1]["classes"]
     root = os.path.join(workdir, "mapset_tiny64_50")          # written by test_map_accounting_equals_reference
     if not os.path.exists(os.path.join(root, "data.cfg")):
-        test_map_accounting_equals_reference(name, 0.5, workdir)
+        util.check_map_accounting(name, 0.5, workdir)
     paths, names, truth = dataset.load_validation_set(os.path.join(root, "data.cfg"))
     assert len(paths) == 7 and len(names) == classes and truth.shape[0] > 0
 
@@ -173,7 +97,7 @@ def test_map_driver_on_the_gpu_equals_validate_detector_map(precision, workdir):
     cfg, wts = util.model_files(name, workdir)
     root = os.path.join(workdir, "mapset_tiny64_50")          # written by test_map_accounting_equals_reference
     if not os.path.exists(os.path.join(root, "ref_stdout.txt")):
-        test_map_accounting_equals_reference(name, 0.5, workdir)
+        util.check_map_accounting(name, 0.5, workdir)
     paths, names, truth = dataset.load_validation_set(os.path.join(root, "data.cfg"))
     net = yb.load_network(cfg, wts, batch=2)                  # 7 images: exercises the padded last batch
     if precision == "fp32":
