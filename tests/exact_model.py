@@ -6,7 +6,11 @@ product is then exact in bf16 / tf32, every partial sum a multiple of the produc
 product stays below 2^20 grid units every partial sum is an exact f32 number in any summation order, whatever the tensor
 core's alignment of its addends and with or without FMA contraction.  The accumulator is the float64 dot product; the
 epilogue is a few IEEE f32 operations (bias add, leaky, residual add, second leaky, round to bf16) that numpy float32
-repeats bit for bit.  `premise` checks these conditions on the host for every convolution before anything runs."""
+repeats bit for bit.  `premise` checks these conditions on the host for every convolution before anything runs.
+
+Under the GPU INT8 rule (`quantized` = 2) the activations stay f32 and the float convolutions take the tf32 wgmma: grid
+data is exact in tf32 as well, so those layers are bit for bit too.  A layer behind one reads f32 values off the tf32 grid
+(leaky outputs); only one-hot consumers do, and `tf32_round` gives what they see."""
 import hashlib
 import struct
 
@@ -49,9 +53,11 @@ def consumer_pairs(c):
 
 class Net:
     """A small network under construction: cfg sections, the weights of each convolution and what each is expected to
-    run on ("reg" k_conv_tc_reg, "tc" k_conv_tc, "stem" k_stem_tc, "stem_s2" k_stem_s2_tc, "simt" the CUDA cores)."""
+    run on ("reg" k_conv_tc_reg, "tc" k_conv_tc, "stem" k_stem_tc, "stem_s2" k_stem_s2_tc, "s8_gpu" the GPU rule's INT8
+    tile, "simt" the CUDA cores).  `quantized` is the flag the cfg is parsed with, `rule` the INT8 rule it runs under: a
+    rule-2 network parsed with 0 has no INT8 layer, and every float convolution with a reader takes tf32."""
 
-    def __init__(self, c, h, w, batch, seed, calib=None):
+    def __init__(self, c, h, w, batch, seed, calib=None, rule=0):
         net = cfgs._net(w, h, calib)
         net[1]["channels"] = str(c)
         self.secs = [net]
@@ -62,6 +68,7 @@ class Net:
         self.edges = []      # (layer, description, predicate on the plan)
         self.env = {}
         self.quantized = 0
+        self.rule = rule
         self.fuse = 1
         self.x = None        # the input images, when a case sets them
         self.tol = {}        # layer -> bf16 ulps its output may differ by (the double-precision logistic), else 0
@@ -73,7 +80,9 @@ class Net:
     def shapes(self):
         return cfgs.conv_shapes(self.secs)
 
-    def conv(self, n, size=3, stride=1, act=LEAKY, kern="reg", w=None, b=None, **extra):
+    def conv(self, n, size=3, stride=1, act=LEAKY, kern=None, w=None, b=None, **extra):
+        """kern None: the tensor-core kernel of a float layer with a reader, k_conv_tc_reg (bf16) or k_conv_tc (tf32)"""
+        kern = kern or ("tc" if self.rule == 2 else "reg")
         self.secs.append(cfgs._conv(n, size, stride, bn=False, act=act, **extra))
         c = self.shapes()[-1]["c"]
         w = grid_weights(self.rng, n, c, size) if w is None else w
@@ -83,7 +92,7 @@ class Net:
         self.kern[i] = kern
         return i
 
-    def preserve(self, kern="reg"):
+    def preserve(self, kern=None):
         """grid-preserving 1x1 layer: one-hot weights over a permutation of the channels, a bias on the activation grid,
         linear -- its output stays exactly on the activation grid"""
         c = self.shapes()[-1]["out_c"] if self.n else self.c
@@ -93,11 +102,15 @@ class Net:
 
     def consume(self):
         """one-hot 3x3 consumer of the last layer's output (f32 out when it is the last layer): k_conv_tc where its channels
-        fill whole 32-byte bf16 rows, else the CUDA cores"""
+        fill whole 32-byte rows (16 bf16, 8 tf32 channels), else the CUDA cores.  Under rule 2 a convolution without a
+        reader runs on the CUDA cores, so a tf32 consumer is read by a [route] alias."""
         c = self.shapes()[-1]["out_c"]
         pairs = consumer_pairs(c)
-        kern = "tc" if c % 16 == 0 else "simt"
-        return self.conv(len(pairs), 3, 1, LINEAR, kern, w=onehot(len(pairs), c, 3, pairs), b=np.zeros(len(pairs), np.float32))
+        kern = "tc" if c % (8 if self.rule == 2 else 16) == 0 else "simt"
+        i = self.conv(len(pairs), 3, 1, LINEAR, kern, w=onehot(len(pairs), c, 3, pairs), b=np.zeros(len(pairs), np.float32))
+        if self.rule == 2 and kern == "tc":
+            self.add("route", layers="-1")
+        return i
 
     def add(self, name, **opts):
         self.secs.append((name, {k: str(v) for k, v in opts.items()}))
@@ -211,7 +224,9 @@ def run_reference(net, x, adt_bf16=True):
     """Host model of the engine on these networks: every layer's output as stored (NHWC f32 values; bf16-rounded where the
     engine keeps bf16), the [yolo] layers' raw head values, and the premise of every convolution.  Follows the engine's
     layer plan: bf16 outputs unless a convolution has no consumer or only detection layers read it; conv + same-shape
-    shortcut fused when `fuse` is on, the conv is stride 1 and the shortcut its sole reader."""
+    shortcut fused when `fuse` is on, the conv is stride 1 and the shortcut its sole reader.  An INT8 layer ("s8_gpu") is
+    not modelled: its output is None, and the test checks it against the oracle on its fetched input.  A tf32 consumer's
+    output is the copy of its input at full f32 precision, which the test replaces with tf32_round's."""
     shapes = net.shapes()
     secs = net.secs[1:]
     cons = {i: [] for i in range(len(secs))}
@@ -232,6 +247,9 @@ def run_reference(net, x, adt_bf16=True):
     for i, L in enumerate(shapes):
         t = L["type"]
         if t == "convolutional":
+            if net.kern[i] == "s8_gpu":
+                outs[i] = cur = None
+                continue
             w, b = net.params[i]
             units[i] = premise(cur, w, b, L["stride"], L["pad"])
             acc = conv_acc(cur, w, L["stride"], L["pad"])
@@ -262,6 +280,19 @@ def run_reference(net, x, adt_bf16=True):
             raise NotImplementedError(t)
         outs[i] = cur
     return outs, units
+
+
+def tf32_round(a, mode):
+    """f32 values as a tf32 operand: "rz" drops the 13 low significand bits, "rn" rounds to nearest even, "rna" to nearest
+    with ties away from zero (cvt.rna.tf32.f32).  The PTX ISA does not say which one the tf32 wgmma applies to f32 operands."""
+    u = np.ascontiguousarray(a, np.float32).view(np.uint32).astype(np.uint64)
+    if mode == "rn":
+        u = u + 0xFFF + ((u >> 13) & 1)
+    elif mode == "rna":
+        u = u + 0x1000
+    else:
+        assert mode == "rz", mode
+    return ((u >> 13) << 13 & 0xFFFFFFFF).astype(np.uint32).view(np.float32).reshape(np.shape(a))
 
 
 def shifted_copies(t, pairs):

@@ -1,10 +1,12 @@
-"""Records tests/golden/engine_plans.json: the op sequence and buffer facts of the engine the library builds for every model
+"""Records tests/golden/engine_plans*.json: the op sequence and buffer facts of the engine the library builds for every model
 of cfgs.MODELS (full width, 128 x 128, batch 2, seeded synthetic weights), in every precision the model supports, with fusion
-off and on, and with and without YB_NO_STEM_S2_FUSE.  Needs a GPU:
-    python tests/golden/make_engine_plans.py [OUT.json]
+off and on, and with and without YB_NO_STEM_S2_FUSE.  The precisions "int8" and "int8_gpu" are the CPU build's and the GPU
+build's INT8 rules (`quantized` = 1 and 2) on the same quantized parse.  Needs a GPU:
+    python tests/golden/make_engine_plans.py [OUT_DIR]
 
-Per case it stores the (layer, op kind) list of the profile, the engine's `launches`, `tc_layers` and `act_bytes`, and the
-layers whose fetch_layer raises.  tests/test_gpu_engine_plan.py rebuilds the same cases with record() and compares.
+Per case it stores the (layer, op kind) list of the profile, the engine's `launches`, `tc_layers` and `act_bytes`, the
+layers whose fetch_layer raises, and `placed_only`: the engine allocated only the outputs some op writes (cases recorded
+before it did lack the flag).  tests/test_gpu_engine_plan.py rebuilds the same cases with record() and compares.
 """
 import json
 import os
@@ -18,7 +20,10 @@ if ROOT not in sys.path:
 from yolo2_light_b200 import cfgs  # noqa: E402
 
 SIZE, BATCH, WSEED, XSEED = 128, 2, 91, 92
-PRECS = ("bf16", "fp32", "int8")
+PRECS = ("bf16", "fp32", "int8", "int8_gpu")
+# the pinned files (suffix of the stem) and the precisions each holds: the GPU INT8 rule's cases were recorded after the others,
+# and each file is written whole
+GOLDEN = {"": PRECS[:3], "_int8_gpu": PRECS[3:]}
 
 
 def model_files(model, workdir):
@@ -32,25 +37,69 @@ def model_files(model, workdir):
 
 
 def precisions(model):
-    """bf16 and fp32 for every model; the quantized rule for the models that ship input calibration."""
+    """bf16 and fp32 for every model; the two INT8 rules for the models that ship input calibration."""
     net_opts = cfgs.MODELS[model](SIZE, SIZE)[0][1]
     return PRECS if "input_calibration" in net_opts else PRECS[:2]
 
 
+def rule(prec):
+    """the INT8 rule (the `quantized` argument of a forward call) a precision runs under"""
+    return {"int8": 1, "int8_gpu": 2}.get(prec, 0)
+
+
 def cases():
-    return [(m, p, fuse, no_s2) for m in cfgs.MODELS for p in precisions(m) for fuse in (0, 1) for no_s2 in (0, 1)]
+    # YB_NO_STEM_S2_FUSE only switches off k_stem_s2_tc, which runs in bf16 networks: the GPU INT8 rule's cases, which keep f32
+    # activations, record the default alone
+    return [(m, p, fuse, no_s2) for m in cfgs.MODELS for p in precisions(m) for fuse in (0, 1)
+            for no_s2 in ((0,) if p == "int8_gpu" else (0, 1))]
+
+
+def load_pinned(stem):
+    """the recording of every pinned file of `stem` ("engine_plans" or "tc_plans"): their common header and all their cases"""
+    rec = None
+    for sfx in GOLDEN:
+        with open(os.path.join(HERE, f"{stem}{sfx}.json")) as f:
+            part = json.load(f)
+        if rec is None:
+            rec = part
+            continue
+        assert {k: v for k, v in part.items() if k != "cases"} == {k: v for k, v in rec.items() if k != "cases"}, sfx
+        rec["cases"] += part["cases"]
+    return rec
+
+
+def write_pinned(out_dir, stem, header, record_case):
+    """records every file of `stem` into out_dir: the header and, per case of the file's precisions, the case's key and
+    record_case(net, prec, fuse, no_s2), net being the case's network (one per model and parse)"""
+    import tempfile
+    wd = tempfile.mkdtemp()
+    for sfx, precs in GOLDEN.items():
+        rec = dict(header, cases=[])
+        nets = {}
+        for model, prec, fuse, no_s2 in cases():
+            if prec not in precs:
+                continue
+            key = (model, rule(prec) > 0)
+            if key not in nets:
+                nets.clear()
+                nets[key] = load(model, prec, wd)
+            rec["cases"].append(dict(model=model, prec=prec, fuse=fuse, no_s2=no_s2, **record_case(nets[key], prec, fuse, no_s2)))
+            print(stem + sfx, model, prec, fuse, no_s2, flush=True)
+        with open(os.path.join(out_dir, f"{stem}{sfx}.json"), "w") as f:
+            json.dump(rec, f, indent=None, separators=(",", ":"))
+            f.write("\n")
 
 
 def load(model, prec, workdir):
     import yolo2_light_b200 as yb
     cfg, wts = model_files(model, workdir)
-    return yb.load_network(cfg, wts, batch=BATCH, quantized=int(prec == "int8"))
+    return yb.load_network(cfg, wts, batch=BATCH, quantized=int(rule(prec) > 0))
 
 
 def record(net, prec, fuse, no_s2):
     """Builds and runs the engine of one case on `net` (loaded by load() for this precision) and returns its facts."""
     import yolo2_light_b200 as yb
-    q = prec == "int8"
+    q = rule(prec)
     net.set_precision(yb.YB_PREC_FP32 if prec == "fp32" else yb.YB_PREC_BF16_TC)
     net.set_option("fuse", fuse)   # drops the engine: the next call builds one under the switches below
     old = os.environ.pop("YB_NO_STEM_S2_FUSE", None)
@@ -76,22 +125,9 @@ def record(net, prec, fuse, no_s2):
 
 
 def main():
-    import tempfile
-    out = sys.argv[1] if len(sys.argv) > 1 else os.path.join(HERE, "engine_plans.json")
-    wd = tempfile.mkdtemp()
-    rec = {"size": SIZE, "batch": BATCH, "cases": []}
-    nets = {}
-    for model, prec, fuse, no_s2 in cases():
-        key = (model, prec == "int8")
-        if key not in nets:
-            nets.clear()
-            nets[key] = load(model, prec, wd)
-        r = record(nets[key], prec, fuse, no_s2)
-        rec["cases"].append(dict(model=model, prec=prec, fuse=fuse, no_s2=no_s2, **r))
-        print(model, prec, fuse, no_s2, r["launches"], r["tc_layers"], r["act_bytes"], r["raises"], flush=True)
-    with open(out, "w") as f:
-        json.dump(rec, f, indent=None, separators=(",", ":"))
-        f.write("\n")
+    out = sys.argv[1] if len(sys.argv) > 1 else HERE
+    write_pinned(out, "engine_plans", {"size": SIZE, "batch": BATCH},
+                 lambda net, prec, fuse, no_s2: dict(record(net, prec, fuse, no_s2), placed_only=1))
 
 
 if __name__ == "__main__":

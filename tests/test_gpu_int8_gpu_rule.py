@@ -227,3 +227,7 @@ def test_yolov3_608_batch2(tmp_path_factory):
     for i, o in fast.detection_outputs().items():
         err = util.rel_l2(o, ref_out[i])
         assert err <= 1e-3, (i, err)
+    # the 48 float convolutions but the stem run on tf32, and nothing else does
+    convs = [i for i, l in enumerate(fast.layers) if l["type_name"] == "CONVOLUTIONAL"]
+    tf32 = [i for i in convs if fast.tc_plan(i, quantized=Q).get("kind") == "tf32"]
+    assert tf32 == [i for i in convs if i > 0 and i not in q] and len(tf32) == 48, tf32

@@ -8,6 +8,10 @@ output is a set of exactly shifted copies of the tested output, so a value store
 merged-row tile shows up bitwise.  Each case names the edge of the tile planner it is for and asserts it through
 Network.tc_plan.
 
+The "tf32_" cases run the same edges under the GPU INT8 rule (`quantized` = 2), where every float convolution with a reader
+runs on the tf32 wgmma of k_conv_tc and stores f32.  Their consumers read the tested output as tf32 operands: the expected
+copies are exact_model.tf32_round of it, in the one conversion mode the whole output shows.
+
 The helpers and the case table run on the CPU; the tests that need a GPU are marked."""
 import numpy as np
 import pytest
@@ -15,27 +19,30 @@ import pytest
 import exact_model
 import ybtest_util as util
 from exact_model import (BOUND_UNITS, F32_01, LEAKY, LINEAR, LOGISTIC, RELU, Net, conv_acc, epilogue, grid_acts, grid_bias,
-                         grid_step, grid_weights, leaky_exact, leaky_tc, onehot, premise, run_reference, shifted_copies)
+                         grid_step, grid_weights, leaky_exact, leaky_tc, onehot, premise, run_reference, shifted_copies,
+                         tf32_round)
 from yolo2_light_b200 import cfgs
 
 
 # ---- the case table -----------------------------------------------------------------------------------------------------
-def c_bk(C, bk):
-    n = Net(C, 9, 11, 2, 100 + C)
+def c_bk(C, bk, rule=0):
+    n = Net(C, 9, 11, 2, 100 + C, rule=rule)
     i = n.conv(64)
     n.consume()
     return n.edge(i, f"BK {bk} at C = {C}", lambda p: p["BK"] == bk)
 
 
-def c_filters(nf, bn=None):
-    n = Net(32, 7, 5, 3, 200 + nf)
+def c_filters(nf, bn=None, rule=0):
+    n = Net(32, 7, 5, 3, 200 + nf, rule=rule)
     i = n.conv(nf)
     n.consume()
     if bn:
         n.env["YB_TC_BN"] = str(bn)
     n.edge(i, f"n = {nf} not a multiple of BN", lambda p: nf % p["BN"] != 0 and p["nt"] == -(-nf // p["BN"]))
-    if bn:
+    if bn or (rule == 2 and nf > 128):   # k_conv_tc: at most 128 filters per tile
         n.edge(i, "two or more filter tiles", lambda p: p["nt"] >= 2)
+    if rule == 2 and nf <= 32:
+        n.edge(i, "BN 32: the second warpgroup idles in the epilogue", lambda p: p["BN"] == 32)
     return n
 
 
@@ -47,37 +54,37 @@ def c_f32(nf, size=3, stats=False):
     return n.edge(i, f"f32 output, n = {nf}", lambda p: p["kernel"] == "k_conv_tc" and p["kind"] == "bf16")
 
 
-def c_width(h, w):
-    n = Net(32, h, w, 3, 400 + 7 * h + w)
+def c_width(h, w, rule=0):
+    n = Net(32, h, w, 3, 400 + 7 * h + w, rule=rule)
     i = n.conv(64)
     n.consume()
     return n.edge(i, f"OW {w} < TW, OW % TW != 0, or one-pixel tiles",
                   lambda p: w < p["TW"] or w % p["TW"] != 0 or p["TW"] == w == 1)
 
 
-def c_tw128(w, batch):
-    n = Net(16, 1, w, batch, 500 + w)
+def c_tw128(w, batch, rule=0):
+    n = Net(16, 1, w, batch, 500 + w, rule=rule)
     i = n.conv(32)
     n.consume()
     return n.edge(i, "TW = 128: a k_conv_tc_reg half tile is half a pixel row", lambda p: p["TW"] == 128)
 
 
-def c_many_images_s1():
-    n = Net(32, 2, 2, 33, 601)
+def c_many_images_s1(rule=0):
+    n = Net(32, 2, 2, 33, 601, rule=rule)
     i = n.conv(32)
     n.consume()
     return n.edge(i, "one tile spans 8+ images (stride 1: 4 merged rows each)", lambda p: p["TH"] >= 8 * 4)
 
 
-def c_many_images_s2():
-    n = Net(32, 4, 6, 17, 602)
+def c_many_images_s2(rule=0):
+    n = Net(32, 4, 6, 17, 602, rule=rule)
     i = n.conv(64, 3, 2)
     n.consume()
     return n.edge(i, "one tile spans 3+ images (stride 2: 3 merged half rows each)", lambda p: p["TH"] >= 3 * 3)
 
 
-def c_straddle(h, w, batch):
-    n = Net(32, h, w, batch, 700 + h + w)
+def c_straddle(h, w, batch, rule=0):
+    n = Net(32, h, w, batch, 700 + h + w, rule=rule)
     i = n.conv(64, 3, 2)
     n.consume()
     # merged half rows: OH + 1 per image; a half tile of TH / 2 rows straddles two images unless it divides them
@@ -93,12 +100,14 @@ def c_bump():
     return n.edge(i, "stride 2, BN 32: TW 1 -> 2", lambda p: p["BN"] == 32 and p["TW"] == 2)
 
 
-def c_knobs(bn=None, no_bstat=False, grid=None, stride=1, stats=False):
-    n = Net(64, 12, 10, 2, 900 + (bn or 0) + 7 * (grid or 0) + stride + 3 * stats)
-    i = n.conv(256, 3, stride)
+def c_knobs(bn=None, no_bstat=False, grid=None, stride=1, stats=False, rule=0, c=64, nf=256, batch=2):
+    """rule 2: k_conv_tc takes its filter tile width from n alone (YB_TC_BN is k_conv_tc_reg's), so nf picks BN"""
+    n = Net(c, 12, 10, batch, 900 + (bn or 0) + 7 * (grid or 0) + stride + 3 * stats, rule=rule)
+    i = n.conv(nf, 3, stride)
     n.consume()
     if bn:
-        n.env["YB_TC_BN"] = str(bn)
+        if rule == 0:
+            n.env["YB_TC_BN"] = str(bn)
         n.edge(i, f"BN {bn}", lambda p: p["BN"] == bn)
     if no_bstat:
         n.env["YB_TC_NO_BSTAT"] = "1"
@@ -111,19 +120,23 @@ def c_knobs(bn=None, no_bstat=False, grid=None, stride=1, stats=False):
     return n
 
 
-def c_shortcut(act2, fuse):
-    n = Net(64, 10, 6, 3, 1000 + fuse + (act2 == LEAKY))
+def c_shortcut(act2, fuse, rule=0):
+    """rule 2: the fused conv + shortcut runs on the CUDA cores (f32 in, out and residual); unfused, the conv runs on tf32
+    and k_shortcut adds the residual"""
+    n = Net(64, 10, 6, 3, 1000 + fuse + (act2 == LEAKY), rule=rule)
     n.preserve()
-    i = n.conv(64)
+    i = n.conv(64, kern="simt" if rule == 2 and fuse else None)
     n.add("shortcut", **{"from": "-2", "activation": act2})
     n.consume()
     n.fuse = fuse
+    if rule == 2:
+        return n.edge(i, f"shortcut act2 {act2}, fuse 0", lambda p: p["kind"] == "tf32") if not fuse else n
     return n.edge(i, f"shortcut act2 {act2}, fuse {fuse}", lambda p: p["kernel"] == "k_conv_tc_reg")
 
 
-def c_concat(first):
+def c_concat(first, rule=0):
     """two tested layers write channel slices of one [route] buffer, each beside the other"""
-    n = Net(32, 8, 6, 2, 1100 + first)
+    n = Net(32, 8, 6, 2, 1100 + first, rule=rule)
     n.preserve()
     a = n.conv(40)                        # 1
     n.add("route", layers="-2")           # 2: alias of layer 0
@@ -132,16 +145,34 @@ def c_concat(first):
     n.consume()
     pos = "first" if first else "second"
     # a channel slice: the output's pixel stride is the concat's 64 channels, not the layer's own
-    n.edge(a, f"layer 1 writes the {pos} slice", lambda p: p["kernel"] == "k_conv_tc_reg" and p["out_ldc"] == 64)
-    return n.edge(b, "layer 3 writes the other slice", lambda p: p["kernel"] == "k_conv_tc_reg" and p["out_ldc"] == 64)
+    kern = "k_conv_tc" if rule == 2 else "k_conv_tc_reg"
+    n.edge(a, f"layer 1 writes the {pos} slice", lambda p: p["kernel"] == kern and p["out_ldc"] == 64)
+    return n.edge(b, "layer 3 writes the other slice", lambda p: p["kernel"] == kern and p["out_ldc"] == 64)
 
 
-def c_yolo(tf32):
-    n = Net(64, 6, 10, 2, 1200 + tf32, calib=[16] * 4 if tf32 else None)
+def c_slice_input():
+    """rule 2: a tf32 layer reads a channel slice of a [route] buffer through a single-input route: its input's pixel
+    stride is the concat's 64 channels, its own channels the slice's 40"""
+    n = Net(32, 8, 6, 2, 1150, rule=2)
+    n.preserve()
+    # 1: a one-hot 1x1 selection, linear, grid bias: layer 6 reads values on the activation grid
+    n.conv(40, 1, 1, LINEAR, w=onehot(40, 32, 1, [(int(c), 0) for c in n.rng.integers(0, 32, 40)]), b=grid_acts(n.rng, 40, 8, -4, 4))
+    n.add("route", layers="-2")               # 2: alias of layer 0
+    n.conv(24)                                # 3
+    n.add("route", layers="-3, -1")           # 4: [layer 1, layer 3]
+    n.add("route", layers="-4")               # 5: alias of layer 1, a slice of layer 4's buffer
+    i = n.conv(32)                            # 6
+    n.consume()
+    return n.edge(1, "layer 1 writes the first slice", lambda p: p["out_ldc"] == 64).edge(i, "C = 40: BK 8", lambda p: p["BK"] == 8)
+
+
+def c_yolo(rule):
+    """rule 1: the tf32 head of an INT8 network (parsed quantized); rule 2: parsed without INT8 layers"""
+    n = Net(64, 6, 10, 2, 1200 + rule, calib=[16] * 4 if rule == 1 else None, rule=rule)
     i = n.conv(255, 1, act=LINEAR, kern="tc")
     n.secs.append(cfgs._yolo("0,1,2", cfgs.COCO_ANCHORS, 9))
-    n.quantized = tf32
-    kind = "tf32" if tf32 else "bf16"
+    n.quantized = int(rule == 1)
+    kind = "tf32" if rule else "bf16"
     return n.edge(i, f"fused [yolo], {kind}", lambda p: p["kind"] == kind and p["kernel"] == "k_conv_tc")
 
 
@@ -150,6 +181,24 @@ def c_refused(size):
     n.conv(16, size, 2 if size == 1 else 1, kern="simt")
     n.consume()
     return n
+
+
+def c_odd_s2():
+    """rule 2: a stride-2 layer on an odd-sized input, which the tile's (half, parity) view cannot express: the CUDA cores"""
+    n = Net(32, 7, 9, 2, 1350, rule=2)
+    n.conv(64, 3, 2, kern="simt")
+    n.consume()
+    return n
+
+
+def c_tf32_into_s8():
+    """parsed quantized = 1, run under rule 2: a tf32 1x1 layer (index 0: float) feeds an INT8 3x3 layer; the INT8 layer is
+    checked against the GPU rule's oracle on the tf32 layer's fetched output"""
+    n = Net(32, 9, 7, 3, 1360, calib=[16] * 4, rule=2)
+    i = n.conv(32, 1)
+    j = n.conv(40, kern="s8_gpu")
+    n.quantized = 1
+    return n.edge(i, "tf32 1x1 into INT8", lambda p: p["kind"] == "tf32").edge(j, "s8_gpu", lambda p: p["kind"] == "s8_gpu")
 
 
 def c_simt_shortcut():
@@ -199,18 +248,21 @@ def c_stem_s2(h, w, batch):
     return n.edge(i, "k_stem_s2_tc: stem + layer 1", lambda p: p["kernel"] == "k_stem_s2_tc")
 
 
-def c_calibration():
+def c_calibration(rule=0):
     """the largest K (3x3x1024) at the largest sums: images of 7/8 and 1 (on the 1/8 grid), a filter of +1/8 weights and one
     of -1/8 weights: |sum| ~ 1080 = 2^19.08 units of the 2^-9 product grid at every interior pixel; the other filters mix
-    large and small addends.  f32 output: the accumulator itself, not rounded to bf16."""
-    n = Net(1024, 5, 5, 2, 1600)
+    large and small addends.  f32 output: the accumulator itself, not rounded to bf16.  Rule 2: the same sums on the tf32
+    wgmma, read by a [route] alias (a convolution without a reader runs on the CUDA cores)."""
+    n = Net(1024, 5, 5, 2, 1600, rule=rule)
     w = grid_weights(n.rng, 32, 1024, 3)
     w[0] = 8 / 64
     w[1] = -8 / 64
     w[2] = np.where(n.rng.random((1024, 3, 3)) < 0.5, 8 / 64, 1 / 64)
     i = n.conv(32, act=LINEAR, kern="tc", w=w)
     n.x = (n.rng.integers(7, 9, (2, 1024, 5, 5)) / 8).astype(np.float32)
-    return n.edge(i, "K = 9216 at 2^19 product-grid units", lambda p: p["BK"] == 64)
+    if rule == 2:
+        n.add("route", layers="-1")
+    return n.edge(i, "K = 9216 at 2^19 product-grid units", lambda p: p["BK"] == (32 if rule == 2 else 64))
 
 
 CASES = {
@@ -253,6 +305,33 @@ CASES = {
     "stem16": lambda: c_stem(16, 10, 14, 3),
     "stem32": lambda: c_stem(32, 7, 9, 2),
     **{f"stem_s2_{h}x{w}_b{b}": (lambda h=h, w=w, b=b: c_stem_s2(h, w, b)) for h, w, b in [(16, 16, 2), (38, 22, 3), (64, 48, 1)]},
+    # the GPU INT8 rule's float layers: k_conv_tc on the tf32 wgmma, f32 out.  BK 8 / 16 / 32: 1, 2, 4 wgmmas per K-block
+    "tf32_calibration": lambda: c_calibration(2),
+    **{f"tf32_bk{bk}_c{C}": (lambda C=C, bk=bk: c_bk(C, bk, 2)) for C, bk in [(8, 8), (24, 8), (40, 8), (16, 16), (48, 16),
+                                                                             (80, 16), (32, 32), (96, 32)]},
+    **{f"tf32_n{nf}": (lambda nf=nf: c_filters(nf, rule=2)) for nf in (8, 9, 24, 40, 72, 75, 136, 264)},
+    **{f"tf32_w{w}_h{h}": (lambda h=h, w=w: c_width(h, w, 2)) for h, w in [(5, 1), (3, 3), (9, 7), (11, 13), (7, 19), (3, 37)]},
+    "tf32_tw128_w256": lambda: c_tw128(256, 1, 2),
+    "tf32_tw128_w200_b3": lambda: c_tw128(200, 3, 2),
+    "tf32_images_s1_b33": lambda: c_many_images_s1(2),
+    "tf32_images_s2_b17": lambda: c_many_images_s2(2),
+    "tf32_straddle_6x10": lambda: c_straddle(6, 10, 3, 2),
+    "tf32_straddle_38x38": lambda: c_straddle(38, 38, 3, 2),
+    "tf32_odd_s2": c_odd_s2,
+    **{f"tf32_s2_bn{bn}": (lambda bn=bn, nf=nf: c_knobs(bn=bn, stride=2, rule=2, nf=nf)) for bn, nf in [(32, 24), (64, 40), (128, 136)]},
+    "tf32_streamed": lambda: c_knobs(no_bstat=True, rule=2, c=16, nf=24),
+    "tf32_streamed_s2": lambda: c_knobs(no_bstat=True, stride=2, rule=2, c=16, nf=40),
+    "tf32_grid1": lambda: c_knobs(grid=1, rule=2, nf=72),
+    "tf32_grid3": lambda: c_knobs(grid=3, rule=2, nf=136),
+    "tf32_grid3_s2": lambda: c_knobs(grid=3, stride=2, rule=2, nf=136, batch=8),
+    "tf32_stats_grid3": lambda: c_knobs(grid=3, stats=True, rule=2, nf=136),
+    "tf32_stats_grid3_s2": lambda: c_knobs(grid=3, stride=2, stats=True, rule=2, nf=136, batch=8),
+    **{f"tf32_shortcut_{a}_fuse{f}": (lambda a=a, f=f: c_shortcut(a, f, 2)) for a in (LINEAR, LEAKY) for f in (0, 1)},
+    "tf32_concat_first": lambda: c_concat(True, 2),
+    "tf32_concat_second": lambda: c_concat(False, 2),
+    "tf32_slice_input": c_slice_input,
+    "tf32_yolo": lambda: c_yolo(2),
+    "tf32_into_s8_gpu": c_tf32_into_s8,
 }
 
 
@@ -267,19 +346,20 @@ def build_case(name):
 
 # ---- CPU tests ----------------------------------------------------------------------------------------------------------
 def test_calibration_case_reaches_the_top_of_the_bound():
-    """the calibration case holds the accumulator between 2^19 and 2^20 units of its product grid (2^-9)"""
-    net, x = build_case("calibration")
-    w, b = net.params[0]
-    assert grid_step(x) * grid_step(w) == 2.0 ** -9 and grid_step(b) >= 2.0 ** -9
-    _, units = run_reference(net, x, adt_bf16=True)
-    assert 2 ** 19 <= units[0] < BOUND_UNITS, units[0]
+    """the calibration cases (bf16 and tf32) hold the accumulator between 2^19 and 2^20 units of its product grid (2^-9)"""
+    for name in ("calibration", "tf32_calibration"):
+        net, x = build_case(name)
+        w, b = net.params[0]
+        assert grid_step(x) * grid_step(w) == 2.0 ** -9 and grid_step(b) >= 2.0 ** -9
+        _, units = run_reference(net, x, adt_bf16=not net.rule)
+        assert 2 ** 19 <= units[0] < BOUND_UNITS, (name, units[0])
 
 
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_case_premise(name):
     """every convolution of every case is exact on the tensor cores: on the grid and below 2^20 product-grid units"""
     net, x = build_case(name)
-    _, units = run_reference(net, x, adt_bf16=not net.quantized)
+    _, units = run_reference(net, x, adt_bf16=not net.rule)
     assert units and max(units.values()) < BOUND_UNITS
 
 
@@ -308,16 +388,19 @@ def test_leaky_emulations_differ_where_the_kernels_do():
 
 
 def _tested_layers(net):
+    """the float layers the cases test (an INT8 layer is checked against the oracle instead)"""
     one_hot = lambda w: np.all((w != 0).reshape(len(w), -1).sum(1) <= 1)
-    return [i for i, (w, _) in net.params.items() if not one_hot(w)]
+    return [i for i, (w, _) in net.params.items() if not one_hot(w) and net.kern[i] != "s8_gpu"]
 
 
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_case_sensitivity(name):
-    """a kernel that skips a K-block or misindexes a bias cannot pass by luck: dropping any single (tap, 16-channel group)
-    of a tested layer's weights, or moving one filter's bias by one grid step, changes at least one expected output"""
+    """a kernel that skips a K-block or misindexes a bias cannot pass by luck: dropping any single (tap, channel group) of
+    a tested layer's weights -- 16 channels, 8 under rule 2, the narrowest K-block of each kind -- or moving one filter's
+    bias by one grid step, changes at least one expected output"""
     net, x = build_case(name)
-    outs, _ = run_reference(net, x, adt_bf16=not net.quantized)
+    outs, _ = run_reference(net, x, adt_bf16=not net.rule)
+    group = 8 if net.rule == 2 else 16
     shapes = net.shapes()
     for i in _tested_layers(net):
         L = shapes[i]
@@ -325,14 +408,14 @@ def test_case_sensitivity(name):
         if net.kern[i].startswith("stem") and i == 0:
             cur = util.bf16_round(cur)
         w, b = net.params[i]
-        bf16 = not net.quantized and shapes[i + 1]["type"] != "yolo" if i + 1 < len(shapes) else False
+        bf16 = not net.rule and shapes[i + 1]["type"] != "yolo" if i + 1 < len(shapes) else False
         act = L["activation"]
         base = epilogue(conv_acc(cur, w, L["stride"], L["pad"]), b, act, net.kern[i], bf16=bf16)
         C, k = w.shape[1], w.shape[2]
         for t in range(k * k):
-            for g in range(0, C, 16):
+            for g in range(0, C, group):
                 w2 = w.copy()
-                w2[:, g:g + 16, t // k, t % k] = 0
+                w2[:, g:g + group, t // k, t % k] = 0
                 if not np.any(conv_acc(cur, w - w2, L["stride"], L["pad"])):
                     continue   # nothing to drop: zero weights, or a tap that only ever reads the zero border
                 e = epilogue(conv_acc(cur, w2, L["stride"], L["pad"]), b, act, net.kern[i], bf16=bf16)
@@ -346,18 +429,19 @@ def test_case_sensitivity(name):
 
 
 # ---- GPU tests ----------------------------------------------------------------------------------------------------------
-KERNEL_OF = {"reg": "k_conv_tc_reg", "tc": "k_conv_tc", "stem": "k_stem_tc", "stem_s2": "k_stem_s2_tc"}
+KERNEL_OF = {"reg": "k_conv_tc_reg", "tc": "k_conv_tc", "stem": "k_stem_tc", "stem_s2": "k_stem_s2_tc", "s8_gpu": "k_conv_tc"}
+TF32_MODES = ("rz", "rn", "rna")
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_tc_exact(name, workdir, monkeypatch):
     net, x = build_case(name)
-    exp, _ = run_reference(net, x, adt_bf16=not net.quantized)
+    exp, _ = run_reference(net, x, adt_bf16=not net.rule)
     for k, v in net.env.items():
         monkeypatch.setenv(k, v)
     m = util.load(*exact_model.write_net(net, workdir, name), net.batch, quantized=net.quantized, fuse=net.fuse)
-    q = bool(net.quantized)
+    q = net.rule
     # the plan of every convolution is the one the case is for
     for i, kern in net.kern.items():
         p = m.tc_plan(i, quantized=q)
@@ -365,6 +449,8 @@ def test_tc_exact(name, workdir, monkeypatch):
             assert p == {}, (name, i, p)
         else:
             assert p.get("kernel") == KERNEL_OF[kern], (name, i, p)
+            if q == 2:
+                assert p["kind"] == ("s8_gpu" if kern == "s8_gpu" else "tf32"), (name, i, p)
     for i, what, pred in net.edges:
         p = m.tc_plan(i, quantized=q)
         assert pred(p), (name, what, p)
@@ -382,8 +468,18 @@ def test_tc_exact(name, workdir, monkeypatch):
         if i + 1 < len(shapes) and shapes[i + 1]["type"] == "shortcut" and net.fuse and shapes[i]["stride"] == 1:
             assert not [k for j, _, k in ops if j == i + 1], (name, i + 1, ops)
     m.predict(x, quantized=q)
+    # the one-hot consumer and what reads it: checked against shifted copies below (on tf32 they are not run_reference's)
+    last = max(i for i, L in enumerate(shapes) if L["type"] == "convolutional")
+    consumer = last if net.params[last][0].shape[2] == 3 and _is_consumer(net, last) else None
     checked = 0
     for i, L in enumerate(shapes):
+        if net.kern.get(i) == "s8_gpu":   # the INT8 layer against the GPU rule's oracle on its fetched input
+            e, _ = util.oracle_layer(m.layers[i], i, m.fetch_layer(i - 1, quantized=q), q)
+            assert util.bits_equal(m.fetch_layer(i, quantized=q), e), (name, i)
+            checked += 1
+            continue
+        if consumer is not None and i >= consumer and net.kern[consumer] == "tc" and q == 2:
+            continue
         e = exp.get(i)
         if L["type"] == "yolo":
             got = m.detection_outputs()[i]
@@ -411,13 +507,23 @@ def test_tc_exact(name, workdir, monkeypatch):
         bad = np.argwhere(got.view(np.uint32) != np.ascontiguousarray(e).view(np.uint32))
         assert len(bad) == 0, (name, i, len(bad), bad[:5].tolist())
         checked += 1
-    last = len(shapes) - 1
-    if shapes[last]["type"] == "convolutional" and net.params[last][0].shape[2] == 3 and _is_consumer(net, last):
-        # the consumer against shifted copies of its input, computed independently of run_reference
-        pairs = [(int(c), int(ky * 3 + kx)) for _, c, ky, kx in np.argwhere(net.params[last][0] == 1)]   # ordered by filter
-        src = m.fetch_layer(last - 1, quantized=q).transpose(0, 2, 3, 1)
-        got = m.fetch_layer(last, quantized=q).transpose(0, 2, 3, 1)
-        assert util.bits_equal(got, shifted_copies(src, pairs)), name
+    if consumer is not None:
+        # the consumer against shifted copies of its input, computed independently of run_reference: every tap that reads
+        # the border gives +0, so a value stored into a border or a pad row fails here
+        pairs = [(int(c), int(ky * 3 + kx)) for _, c, ky, kx in np.argwhere(net.params[consumer][0] == 1)]   # ordered by filter
+        src = m.fetch_layer(consumer - 1, quantized=q).transpose(0, 2, 3, 1)
+        got = m.fetch_layer(consumer, quantized=q).transpose(0, 2, 3, 1)
+        if q == 2 and net.kern[consumer] == "tc":
+            # tf32 operands: every element follows one conversion of f32 to tf32, and the modes differ on this input
+            exps = {mode: shifted_copies(tf32_round(src, mode), pairs) for mode in TF32_MODES}
+            assert not util.bits_equal(exps["rz"], exps["rn"]), name
+            modes = [mode for mode in TF32_MODES if util.bits_equal(got, exps[mode])]
+            bad = {mode: int(np.sum(got.view(np.uint32) != e.view(np.uint32))) for mode, e in exps.items()}
+            assert modes, (name, "elements off each conversion mode", bad)
+            print(name, "tf32 operand conversion:", modes)
+            checked += 1
+        else:
+            assert util.bits_equal(got, shifted_copies(src, pairs)), name
     assert checked >= 1, name
 
 
@@ -427,8 +533,11 @@ def _is_consumer(net, i):
 
 
 # ---- integer kinds at the edge shapes: bit for bit against the oracle on the fetched input ---------------------------
-def _int_secs(C, h, w, quantized):
-    net = cfgs._net(w, h, [16] * 8 if quantized else None)
+RULE_OF = {"s8": 1, "s8_gpu": 2, "xnor": 0}    # the INT8 rule each integer kind runs under
+
+
+def _int_secs(C, h, w, quantized, calib=16):
+    net = cfgs._net(w, h, [calib] * 8 if quantized else None)
     return [net, cfgs._conv(C, 3)]     # layer 0: f32 (the INT8 rule starts at layer 1), leaky
 
 
@@ -436,47 +545,58 @@ INT_SHAPES = [   # kind, C, n, h, w, stride, batch: padded channels (C % 32 != 0
     ("s8", 8, 8, 7, 9, 1, 3), ("s8", 24, 30, 9, 5, 1, 2), ("s8", 40, 40, 11, 13, 1, 1), ("s8", 100, 264, 5, 7, 1, 2),
     ("s8", 24, 30, 10, 14, 2, 3), ("s8", 40, 264, 6, 10, 2, 1), ("s8", 8, 40, 2, 2, 2, 5),
     ("xnor", 16, 8, 7, 9, 1, 3), ("xnor", 48, 40, 5, 3, 1, 2), ("xnor", 80, 264, 9, 11, 1, 1), ("xnor", 16, 30, 1, 13, 1, 3),
+    ("s8_gpu", 8, 8, 7, 9, 1, 3), ("s8_gpu", 24, 30, 9, 5, 1, 2), ("s8_gpu", 40, 40, 11, 13, 1, 1),
+    ("s8_gpu", 100, 264, 5, 7, 1, 2), ("s8_gpu", 24, 30, 10, 14, 2, 3), ("s8_gpu", 40, 264, 6, 10, 2, 1),
+    ("s8_gpu", 8, 40, 2, 2, 2, 5),
 ]
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("kind,C,n,h,w,stride,batch", INT_SHAPES)
 def test_integer_kinds_exact(kind, C, n, h, w, stride, batch, workdir):
-    q = kind == "s8"
-    secs = _int_secs(C, h, w, q)
-    secs.append(cfgs._conv(n, 3, stride, **({} if q else {"xnor": 1, "bin_output": 1})))
-    m = util.load(*util.write_net(workdir, f"int_{kind}_{C}_{n}_{h}x{w}s{stride}", secs, C + n), batch, quantized=int(q))
-    m.set_option("keep_counts", 1)
-    p = m.tc_plan(1, quantized=q)
-    assert p.get("kind") == kind and p["kernel"] == "k_conv_tc", p
-    assert p["tma_epi"] == 0, p    # keep_counts: the raw accumulators go through the LSU stores
-    m.predict(cfgs.synthetic_images(batch, 3, h, w, seed=C), quantized=q)
-    exp, acc = util.oracle_layer(m.layers[1], 1, m.fetch_layer(0, quantized=q), int(q))
-    assert np.array_equal(m.fetch_counts(1, quantized=q), acc)
-    assert util.bits_equal(m.fetch_layer(1, quantized=q), exp)
-    # and without the raw-accumulator dump: the TMA epilogue at stride 1, the LSU stores at stride 2
-    m.set_option("keep_counts", 0)
-    p = m.tc_plan(1, quantized=q)
-    assert (p["tma_epi"] == 0) == (stride == 2), p
-    m.predict(cfgs.synthetic_images(batch, 3, h, w, seed=C), quantized=q)
-    assert util.bits_equal(m.fetch_layer(1, quantized=q), exp)
+    """s8_gpu: also with input multipliers of 2^20, where the GPU rule's conversion saturates at +-127"""
+    import gpu_rule_oracle as gro
+    q = RULE_OF[kind]
+    for calib in (16, 2 ** 20) if q == 2 else (16,):
+        secs = _int_secs(C, h, w, q, calib)
+        secs.append(cfgs._conv(n, 3, stride, **({} if q else {"xnor": 1, "bin_output": 1})))
+        name = f"int_{kind}_{C}_{n}_{h}x{w}s{stride}" + ("_sat" if calib != 16 else "")
+        m = util.load(*util.write_net(workdir, name, secs, C + n), batch, quantized=int(q > 0))
+        m.set_option("keep_counts", 1)
+        p = m.tc_plan(1, quantized=q)
+        assert p.get("kind") == kind and p["kernel"] == "k_conv_tc", p
+        assert p["tma_epi"] == 0, p    # keep_counts: the raw accumulators go through the LSU stores
+        m.predict(cfgs.synthetic_images(batch, 3, h, w, seed=C), quantized=q)
+        x = m.fetch_layer(0, quantized=q)
+        if calib != 16:
+            xq = gro.quantize_input_gpu(x, m.layers[1]["input_quant_multipler"])
+            assert np.any(xq == 127) and np.any(xq == -127), (x.min(), x.max())
+        exp, acc = util.oracle_layer(m.layers[1], 1, x, q)
+        assert np.array_equal(m.fetch_counts(1, quantized=q), acc)
+        assert util.bits_equal(m.fetch_layer(1, quantized=q), exp)
+        # and without the raw-accumulator dump: the TMA epilogue at stride 1, the LSU stores at stride 2
+        m.set_option("keep_counts", 0)
+        p = m.tc_plan(1, quantized=q)
+        assert (p["tma_epi"] == 0) == (stride == 2), p
+        m.predict(cfgs.synthetic_images(batch, 3, h, w, seed=C), quantized=q)
+        assert util.bits_equal(m.fetch_layer(1, quantized=q), exp)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("kind", ["s8", "xnor"])
+@pytest.mark.parametrize("kind", ["s8", "xnor", "s8_gpu"])
 def test_integer_kinds_role_counters(kind, workdir, monkeypatch, capfd):
     """YB_TC_STATS=1 runs the role-counter instantiation of the integer epilogue: the same bits as the oracle, and a TCSTATS
     line per plan when the network is freed"""
     import gc
     monkeypatch.setenv("YB_TC_STATS", "1")
     monkeypatch.setenv("YB_TC_GRID", "2")   # several work items per CTA
-    q = kind == "s8"
+    q = RULE_OF[kind]
     secs = _int_secs(40 if q else 48, 11, 13, q) + [cfgs._conv(40, 3, **({} if q else {"xnor": 1, "bin_output": 1}))]
-    m = util.load(*util.write_net(workdir, f"stats_{kind}", secs, 11), 2, quantized=int(q))
+    m = util.load(*util.write_net(workdir, f"stats_{kind}", secs, 11), 2, quantized=int(q > 0))
     p = m.tc_plan(1, quantized=q)
     assert p.get("kind") == kind and p["kernel"] == "k_conv_tc" and p["num_work"] > p["grid"], p
     m.predict(cfgs.synthetic_images(2, 3, 11, 13, seed=4), quantized=q)
-    exp, _ = util.oracle_layer(m.layers[1], 1, m.fetch_layer(0, quantized=q), int(q))
+    exp, _ = util.oracle_layer(m.layers[1], 1, m.fetch_layer(0, quantized=q), q)
     assert util.bits_equal(m.fetch_layer(1, quantized=q), exp)
     capfd.readouterr()
     del m
@@ -486,22 +606,23 @@ def test_integer_kinds_role_counters(kind, workdir, monkeypatch, capfd):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("kind,h,w,batch", [("s8", 2, 2, 3), ("s8", 6, 10, 1), ("xnor", 2, 2, 3), ("xnor", 6, 10, 1)])
+@pytest.mark.parametrize("kind,h,w,batch", [("s8", 2, 2, 3), ("s8", 6, 10, 1), ("xnor", 2, 2, 3), ("xnor", 6, 10, 1),
+                                            ("s8_gpu", 2, 2, 3), ("s8_gpu", 6, 10, 1)])
 def test_pool_fused_epilogue_exact(kind, h, w, batch, workdir):
-    """the 2x2/2 max-pool and the next layer's input conversion in the integer epilogue (mode 1: s8, mode 2: +-1 bytes) at
-    the smallest and odd-batch shapes it takes"""
+    """the 2x2/2 max-pool and the next layer's input conversion in the integer epilogue (s8, the GPU rule's saturating s8,
+    +-1 bytes) at the smallest and odd-batch shapes it takes"""
     from oracle import port
-    q = kind == "s8"
+    q = RULE_OF[kind]
     extra = {} if q else {"xnor": 1, "bin_output": 1}
     secs = _int_secs(32, h, w, q) + [cfgs._conv(32, 3, **extra), ("maxpool", {"size": "2", "stride": "2"}),
                                       cfgs._conv(32, 3, **extra)]
-    m = util.load(*util.write_net(workdir, f"pool_{kind}_{h}x{w}", secs, 7 + h), batch, quantized=int(q))
+    m = util.load(*util.write_net(workdir, f"pool_{kind}_{h}x{w}", secs, 7 + h), batch, quantized=int(q > 0))
     p = m.tc_plan(1, quantized=q)
     assert p.get("kind") == kind and p["jshift"] == 1 and p["TW"] == 8, p    # pool fused: 8 x 16 tiles, one row down
     m.predict(cfgs.synthetic_images(batch, 3, h, w, seed=h), quantized=q)
     L = m.layers
-    y1, _ = util.oracle_layer(L[1], 1, m.fetch_layer(0, quantized=q), int(q))
-    y3, _ = util.oracle_layer(L[3], 3, port.maxpool(y1, L[2]["size"], L[2]["stride"], L[2]["pad"]), int(q))
+    y1, _ = util.oracle_layer(L[1], 1, m.fetch_layer(0, quantized=q), q)
+    y3, _ = util.oracle_layer(L[3], 3, port.maxpool(y1, L[2]["size"], L[2]["stride"], L[2]["pad"]), q)
     assert util.bits_equal(m.fetch_layer(3, quantized=q), y3)
 
 
@@ -530,16 +651,32 @@ def test_int8_slice_store_leaves_the_next_slice(workdir):
 
 
 # ---- production shapes: every distinct convolution of yolov3-608 and yolov3-spp-608 at batch 16, with its fusion ----------
-def production_shapes():
+def gpu_rule_floats(secs):
+    """the convolutions a network parsed with quantized = 1 keeps float (l.quantized == 0): index 0, linear and 1x1 layers,
+    stride-2 layers past index 1, and every convolution from the one whose second successor is a [yolo] layer on"""
+    L = cfgs.conv_shapes(secs)
+    floats, latched = [], False
+    for i, l in enumerate(L):
+        if l["type"] != "convolutional":
+            continue
+        latched |= i + 2 < len(L) and L[i + 2]["type"] == "yolo"
+        if latched or i == 0 or l["activation"] == LINEAR or (i > 1 and l["stride"] > 1) or l["size"] == 1:
+            floats.append(i)
+    return floats
+
+
+def production_shapes(rule=0, nets=None):
     """(C, H, W, n, size, stride, fusion) of every distinct convolution of the two networks at 608 x 608.  fusion: "stem_s2"
     (the stem and layer 1, one kernel), "shortcut" (3x3 + fused residual), "yolo" (head + fused [yolo]), "slice" (writes a
-    channel slice of a [route] buffer) or "none"."""
+    channel slice of a [route] buffer) or "none".  rule 2: the float convolutions of the GPU INT8 rule but the stem, the
+    layers that run on tf32."""
     keys = []
-    for secs in (cfgs.yolov3(608, 608), cfgs.yolov3_spp(608, 608)):
+    for secs in nets or (cfgs.yolov3(608, 608), cfgs.yolov3_spp(608, 608)):
         L = cfgs.conv_shapes(secs)
         slices = {j for l in L if l["type"] == "route" and len(l["layers"]) > 1 for j in l["layers"]}
+        tested = [i for i in gpu_rule_floats(secs) if i > 0] if rule == 2 else [i for i in range(len(L)) if i != 1]
         for i, l in enumerate(L):
-            if l["type"] != "convolutional" or i == 1:
+            if l["type"] != "convolutional" or i not in tested:
                 continue
             nxt = L[i + 1]["type"] if i + 1 < len(L) else None
             fusion = ("stem_s2" if i == 0 else "shortcut" if nxt == "shortcut" and l["stride"] == 1 else
@@ -551,6 +688,7 @@ def production_shapes():
 
 
 PRODUCTION = production_shapes()
+PRODUCTION_TF32 = production_shapes(2)
 
 
 def test_torch_reference_equals_numpy_reference():
@@ -570,7 +708,30 @@ def test_production_shapes_cover_both_networks():
     assert (1024, 19, 19, 512, 1, 1, "none") in PRODUCTION and (2048, 19, 19, 512, 1, 1, "none") in PRODUCTION
 
 
-def production_net(key, batch=16):
+def test_production_tf32_shapes():
+    """the GPU rule's tf32 layers: 19 distinct shapes in yolov3-608 (48 layers), two more in yolov3-spp-608 (the 1x1
+    2048 -> 512 and the 1x1 that writes the SPP block's [route] slice); the four 3x3/2 downsampling layers among them"""
+    v3 = cfgs.yolov3(608, 608)
+    assert len(gpu_rule_floats(v3)) == 49 and len(production_shapes(2, [v3])) == 19
+    assert len(PRODUCTION_TF32) == 21, len(PRODUCTION_TF32)
+    assert {k[-1] for k in PRODUCTION_TF32} == {"none", "yolo", "slice"}
+    assert [k for k in PRODUCTION_TF32 if k[5] == 2] == [(64, 304, 304, 128, 3, 2, "none"), (128, 152, 152, 256, 3, 2, "none"),
+                                                         (256, 76, 76, 512, 3, 2, "none"), (512, 38, 38, 1024, 3, 2, "none")]
+    assert (2048, 19, 19, 512, 1, 1, "none") in PRODUCTION_TF32 and (1024, 19, 19, 512, 1, 1, "slice") in PRODUCTION_TF32
+
+
+def test_gpu_rule_floats_are_the_parsers():
+    """gpu_rule_floats restates the parser's layer rule: the same float convolutions as yb.parse_network_cfg(quantized = 1)"""
+    import tempfile
+    import yolo2_light_b200 as yb
+    d = tempfile.mkdtemp()
+    for name, secs in (("v3", cfgs.yolov3(608, 608)), ("spp", cfgs.yolov3_spp(608, 608))):
+        net = yb.parse_network_cfg(cfgs.write_cfg(secs, f"{d}/{name}.cfg"), 1, 1)
+        assert gpu_rule_floats(secs) == [i for i, l in enumerate(net.layers)
+                                         if l["type_name"] == "CONVOLUTIONAL" and not l["quantized"]], name
+
+
+def production_net(key, batch=16, rule=0):
     """the single-layer case of one production shape, with the fusion the network uses there; returns (net, tested layer)"""
     C, H, W, n, k, s, fusion = key
     seed = C * 7 + n + H + k + s
@@ -591,7 +752,7 @@ def production_net(key, batch=16):
         net.add("shortcut", **{"from": "-3", "activation": LINEAR})
         net.add("route", layers="-1")
         return net, i
-    net = Net(C, H, W, batch, seed)
+    net = Net(C, H, W, batch, seed, rule=rule)
     if fusion == "yolo":
         i = net.conv(n, k, s, act=LINEAR, kern="tc")
         net.secs.append(cfgs._yolo("0,1,2", cfgs.COCO_ANCHORS, 9))
@@ -659,22 +820,24 @@ def _t_bits_equal(got_nchw, exp_nhwc):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("key", PRODUCTION, ids=lambda k: "{}x{}x{}-n{}-k{}s{}-{}".format(*k))
-def test_production_shape_exact(key, workdir):
+@pytest.mark.parametrize("key,rule", [pytest.param(k, 0, id="{}x{}x{}-n{}-k{}s{}-{}".format(*k)) for k in PRODUCTION] +
+                         [pytest.param(k, 2, id="{}x{}x{}-n{}-k{}s{}-{}-tf32".format(*k)) for k in PRODUCTION_TF32])
+def test_production_shape_exact(key, rule, workdir):
+    """rule 0: the bf16 engine; rule 2: the GPU INT8 rule's tf32 layers, f32 in and out"""
     import torch
-    net, i = production_net(key)
+    net, i = production_net(key, rule=rule)
     stem = key[-1] == "stem_s2"
     x = net.images(16, 0, 16) if stem else net.images()
-    m = util.load(*exact_model.write_net(net, workdir, "prod_{}x{}x{}_n{}_k{}s{}_{}".format(*key)), net.batch,
+    m = util.load(*exact_model.write_net(net, workdir, "prod{}_{}x{}x{}_n{}_k{}s{}_{}".format(rule or "", *key)), net.batch,
                   quantized=net.quantized, fuse=net.fuse)
-    p = m.tc_plan(i)
-    assert p.get("kernel") == KERNEL_OF[net.kern[i]] and p["kind"] == "bf16", (key, p)
+    p = m.tc_plan(i, quantized=rule)
+    assert p.get("kernel") == KERNEL_OF[net.kern[i]] and p["kind"] == ("tf32" if rule else "bf16"), (key, p)
     if net.kern[i] == "reg":
         assert p["BN"] >= min(64, key[3]), (key, p)     # the production tiles: 64 to 256 filters (32 at n = 32)
     if key[-1] == "slice":
         assert p["out_ldc"] == 2 * key[3], (key, p)
     for j, kern in net.kern.items():
-        assert m.tc_plan(j).get("kernel") == KERNEL_OF[kern], (key, j)
+        assert m.tc_plan(j, quantized=rule).get("kernel") == KERNEL_OF[kern], (key, j)
     # the expected outputs, each convolution's premise checked, before the network runs
     dev = torch.device("cuda")
     cur = torch.as_tensor(x, device=dev).permute(0, 2, 3, 1).double()
@@ -685,10 +848,10 @@ def test_production_shape_exact(key, workdir):
         if stem and j == 0:
             cur = cur.to(torch.bfloat16).double()
         res = outs[0] if key[-1] == "shortcut" and j == i else None
-        outs[j] = _t_layer(cur, w, b, shapes[j], net.kern[j], res=res, bf16=key[-1] != "yolo")
+        outs[j] = _t_layer(cur, w, b, shapes[j], net.kern[j], res=res, bf16=not rule and key[-1] != "yolo")
         cur = outs[j].double()
     del cur
-    m.predict(x)
+    m.predict(x, quantized=rule)
     for j, out in outs.items():
         if key[-1] == "yolo":
             got = torch.as_tensor(m.detection_outputs()[j + 1], device=dev)
@@ -701,6 +864,6 @@ def test_production_shape_exact(key, workdir):
         elif key[-1] == "shortcut" and j == i:
             assert _t_bits_equal(m.fetch_layer(j + 1), out), key      # the fused shortcut's output
         elif not (stem and j == 0):                                   # k_stem_s2_tc never writes the stem output
-            assert _t_bits_equal(m.fetch_layer(j), out), (key, j)
+            assert _t_bits_equal(m.fetch_layer(j, quantized=rule), out), (key, j)
     del m
     torch.cuda.empty_cache()

@@ -1,9 +1,7 @@
-"""The tensor-core plans, pinned per model, precision and fusion setting (tests/golden/tc_plans.json, recorded with
+"""The tensor-core plans, pinned per model, precision and fusion setting (tests/golden/tc_plans*.json, recorded with
 tests/golden/make_tc_plans.py): every layer with a plan keeps its kernel, kind, tile shape, filter tile width, resident filter
 matrix, ring depth, K-blocks per stage, grid, work items, TMA epilogue, row shift and output pitch.  The filter tile width and
 the grid depend on the SM count: the comparison needs a card with the SM count of the recording."""
-import json
-import os
 import sys
 
 import pytest
@@ -16,8 +14,7 @@ import make_tc_plans as tc_plans  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
-with open(os.path.join(util.GOLDEN, "tc_plans.json")) as _f:
-    PINNED = json.load(_f)
+PINNED = plans.load_pinned("tc_plans")
 MODELS = sorted({c["model"] for c in PINNED["cases"]})
 
 
@@ -34,7 +31,7 @@ def test_tc_plans_match_pinned(model, workdir, monkeypatch):
     nets = {}
     for case in cases:
         prec, fuse, no_s2 = case["prec"], case["fuse"], case["no_s2"]
-        q = prec == "int8"
+        q = plans.rule(prec) > 0    # the two INT8 rules run on one quantized parse
         if q not in nets:
             nets[q] = plans.load(model, prec, workdir)
         got = tc_plans.record(nets[q], prec, fuse, no_s2)
