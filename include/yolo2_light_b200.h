@@ -250,6 +250,10 @@ int yb_network_submit_frames_u8(yb_network *net, const unsigned char *const *fra
  *                        half = 1 << 19:  R = clamp((yy + half + 1673527 v) >> 20),
  *                        G = clamp((yy + half - 852492 v - 409993 u) >> 20), B = clamp((yy + half + 2116026 u) >> 20),
  *                        clamped to 0..255.
+ *                        The opposite direction, which yb_network_submit_device_frames_draw writes with: an 8-bit R, G, B
+ *                        becomes Y = ((66 R + 129 G + 25 B + 128) >> 8) + 16, U = ((-38 R - 74 G + 112 B + 128) >> 8) + 128,
+ *                        V = ((112 R - 94 G - 18 B + 128) >> 8) + 128 (BT.601 limited range, arithmetic shifts; Y in
+ *                        16..235, U and V in 16..240).
  * Device frames are always resized by the kernel, also at the network size, and letterboxed like host frames when
  * yb_network_set_letterbox is on.  One format per call, 3-channel networks only. */
 enum { YB_FRAME_RGB = 0, YB_FRAME_BGR = 1, YB_FRAME_RGB_PLANAR = 2, YB_FRAME_NV12 = 3 };
@@ -285,6 +289,47 @@ float *yb_network_predict_device_frames(yb_network *net, const yb_device_frame *
  * GPU's memory; cudaPointerGetAttributes) is rejected. */
 int yb_network_submit_device_frames(yb_network *net, const yb_device_frame *frames, int nimg, int format, int quantized,
                                     float thresh, float nms, int relative, int letter, int max_rows, void *stream);
+
+/* The detector's drawing (test_detector, src/main.c:188-229, which draws with draw_detections_v3, main.c:80-148, and no
+ * alphabet, so without text labels) into the device frames themselves.  yb_network_submit_device_frames_draw does what
+ * yb_network_submit_device_frames does with relative = 1 -- same slots, tickets, argument checks, rows and counts -- and
+ * then, on the engine's side stream behind the NMS of the batch, draws image b's selected detections into frame b, in place
+ * and in the frame's own format.  The library writes through `data` (and `chroma`) of these frames: they must be writable
+ * device memory of the network's device.  Two frames with the same `data` pointer are rejected before any device work (their
+ * draws would race), and networks of more than 17395 classes (the reference's colour index, cls * 123457, would overflow).
+ *
+ * What is drawn, for image b, on its first min(counts[b], max_rows) post-NMS candidate rows:
+ *   selection   (get_actual_detections, main.c:38-62): the best class is the first j, in class order, with prob[j] > best,
+ *               best starting at thresh; a row is selected iff there is one (a probability equal to thresh is not);
+ *   list order  (compare_by_lefts, main.c:65-70): ascending float x - w / 2 (NaN as +inf), equal keys by candidate position;
+ *   draw order  (compare_by_probs, main.c:73-78): ascending prob[cls], equal keys by candidate position; a later detection
+ *               overwrites an earlier one wherever they share pixels;
+ *   geometry    (main.c:109-143): width = (int)(h * .006), at least 1; left = (int)((x - w / 2.) * frame w), right, top and
+ *               bot likewise, in double, where a NaN or out-of-int value converts to INT_MIN as on x86; then left, top >= 0,
+ *               right <= frame w - 1, bot <= frame h - 1; draw_box_width's `width` nested draw_box rectangles
+ *               (additionally.c:2945-2988: each corner clamped into the frame, rows top and bot, columns left and right);
+ *   colour      (get_color, additionally.c:3247, offset = cls * 123457 % classes): red, green, blue as floats, written as
+ *               the bytes (unsigned char)(255 * c) that save_image_png (additionally.c:3226) writes;
+ *   formats     RGB: those bytes; BGR: reversed; RGB_PLANAR: one per plane; NV12: each drawn pixel's Y, and the U, V pair
+ *               of every 2x2 block with a drawn pixel, from the colour of the last detection in draw order that covers a
+ *               pixel of the block (the RGB -> YUV rule above).  Row padding and pixels that no box covers are never written.
+ * An RGB frame so drawn is byte for byte the reference's predictions.png of that frame and those rows.
+ *
+ * Ordering: as for yb_network_submit_device_frames, except that `stream` is made to wait on an event recorded after the
+ * draw, so the work the caller enqueues on `stream` after the call (an encoder reading the frames, the decoder's next write
+ * into them) sees the drawn frames.
+ *
+ * yb_network_collect_detections collects these tickets as any other (same rows and counts) and also copies the selected
+ * list, whose bytes *d2h_bytes includes.  Then yb_network_selected_detections gives that list, valid as long as the rows:
+ * *dets = pinned yb_detection[batch][max_rows] in list order, *counts = int[batch] selected detections per image (0 for
+ * b >= nimg); `row` is the detection's index among the ticket's candidate rows of its image, prob = prob[cls].  It returns
+ * 0, or -1 (without an error) for a ticket that is not a drawing ticket, has not been collected, or whose slot has been
+ * taken by a later submit. */
+typedef struct yb_detection { float x, y, w, h; float prob; int cls; int row; } yb_detection;
+
+int yb_network_submit_device_frames_draw(yb_network *net, const yb_device_frame *frames, int nimg, int format,
+                                         int quantized, float thresh, float nms, int letter, int max_rows, void *stream);
+int yb_network_selected_detections(yb_network *net, int ticket, const yb_detection **dets, const int **counts);
 
 /* Host output (NCHW for yolo, HWC-flattened for region, as the reference lays them out) of layer i after a
  * predict call; only YOLO/REGION layers (and the last layer) are kept on the host. */

@@ -66,6 +66,16 @@ class DeviceFrame(C.Structure):
                 ("plane_stride", C.c_longlong)]
 
 
+class Detection(C.Structure):
+    """``yb_detection`` (include/yolo2_light_b200.h): one selected detection of a drawing ticket."""
+    _fields_ = [("x", C.c_float), ("y", C.c_float), ("w", C.c_float), ("h", C.c_float), ("prob", C.c_float),
+                ("cls", C.c_int), ("row", C.c_int)]
+
+
+# the same record as a numpy dtype
+DETECTION_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("w", "<f4"), ("h", "<f4"), ("prob", "<f4"), ("cls", "<i4"),
+                            ("row", "<i4")])
+
 # ``YB_FRAME_*``: the layouts of device frames
 FRAME_FORMATS = {"rgb": 0, "bgr": 1, "planar": 2, "nv12": 3}
 
@@ -118,6 +128,9 @@ def lib():
         "yb_network_predict_device_frames": (fp, [vp, vp, C.c_int, C.c_int, C.c_int, vp]),
         "yb_network_submit_device_frames": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_int,
                                                       C.c_int, C.c_int, vp]),
+        "yb_network_submit_device_frames_draw": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_int,
+                                                           C.c_int, vp]),
+        "yb_network_selected_detections": (C.c_int, [vp, C.c_int, C.POINTER(C.POINTER(Detection)), C.POINTER(ip)]),
         "yb_network_set_devices": (C.c_int, [vp, ip, C.c_int]),
         "yb_network_predict_batch": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int]),
         "yb_network_batch_output": (fp, [vp, C.c_int, ip]),
@@ -170,7 +183,8 @@ EXPORTED_SYMBOLS = [
     "yb_free_pinned", "yb_network_submit_u8", "yb_network_collect_detections", "yb_network_set_devices",
     "yb_network_predict_batch", "yb_network_batch_output", "yb_network_replication", "yb_network_predict_frames_u8",
     "yb_network_detect_frames", "yb_network_submit_frames_u8", "yb_network_predict_device_frames",
-    "yb_network_submit_device_frames", "yb_network_set_letterbox",
+    "yb_network_submit_device_frames", "yb_network_set_letterbox", "yb_network_submit_device_frames_draw",
+    "yb_network_selected_detections",
 ]
 
 
@@ -474,6 +488,32 @@ class Network:
         self._inflight[("u8", t)] = (keep, max_rows, len(keep))
         return t
 
+    def submit_device_frames_draw(self, frames, thresh: float, fmt: str = "rgb", nms: float = 0.45, letter: int = 0,
+                                  max_rows: int = 2048, quantized: bool = False, stream: Optional[int] = None) -> int:
+        """submit_device_frames with relative boxes, which then draws each image's selected detections into its frame, in
+        place, as the reference's test_detector draws them (``yb_network_submit_device_frames_draw``).  The frames must be
+        writable device memory and distinct; `stream` waits for the draw.  Collect with collect_detections, then read the
+        selected list with selected_detections."""
+        keep, arr, F = self._device_frames(frames, fmt, "submit_device_frames_draw")
+        self._inflight = getattr(self, "_inflight", {})
+        t = lib().yb_network_submit_device_frames_draw(self._h, arr, len(keep), F, int(quantized), thresh, nms, letter,
+                                                       max_rows, C.c_void_p(stream or 0))
+        _check(t >= 0)
+        self._inflight[("u8", t)] = (keep, max_rows, len(keep))
+        return t
+
+    def selected_detections(self, ticket: int):
+        """The selected list of a collected drawing ticket (``yb_network_selected_detections``): one DETECTION_DTYPE array
+        per image of the ticket, in list order (ascending left edge); None for any other ticket."""
+        dets, counts = C.POINTER(Detection)(), C.POINTER(C.c_int)()
+        if lib().yb_network_selected_detections(self._h, ticket, C.byref(dets), C.byref(counts)) != 0:
+            return None
+        max_rows, nimg = getattr(self, "_collected", {})[ticket]
+        cnt = np.ctypeslib.as_array(counts, shape=(self.batch,))
+        buf = (C.c_char * (self.batch * max_rows * DETECTION_DTYPE.itemsize)).from_address(C.addressof(dets.contents))
+        alld = np.frombuffer(buf, DETECTION_DTYPE).reshape(self.batch, max_rows)
+        return [alld[b, :int(cnt[b])].copy() for b in range(nimg)]
+
     def collect_detections(self, ticket: int, quantized: bool = False, copy: bool = True):
         """Returns (list of [n_b, 5 + classes] arrays, counts int32, bytes moved device -> host) for the ticket's images:
         batch of them for submit_u8, nimg for submit_frames_u8 and submit_device_frames."""
@@ -483,6 +523,8 @@ class Network:
         _, max_rows, nimg = getattr(self, "_inflight", {}).pop(("u8", ticket), (None, None, None))
         if max_rows is None:
             raise YbError("collect_detections: unknown ticket")
+        self._collected = getattr(self, "_collected", {})
+        self._collected[ticket] = (max_rows, nimg)
         cnt = np.ctypeslib.as_array(counts, shape=(self.batch,))[:nimg].copy()
         allrows = np.ctypeslib.as_array(rows, shape=(self.batch, max_rows, stride))
         out = [allrows[b, :min(int(cnt[b]), max_rows)] for b in range(nimg)]

@@ -388,15 +388,27 @@ static float *predict_frames(yb_network *n, const char *fn, const FrameBatch &b,
     net.last_launches = engine_num_launches(e) + 1;   // + resize
     return net.layers.back().output;
 }
+// The drawing call's own checks: frames drawn in place must be distinct, and the colour index of every class must fit an int.
+static void check_draw(const Network &net, const char *fn, const FrameBatch &b) {
+    const std::string f(fn);
+    for (int i = 0; i < b.nimg; ++i)
+        for (int j = 0; j < i; ++j)
+            if (b.frames[i].data == b.frames[j].data)
+                fatal_throw(f + ": frames " + std::to_string(j) + " and " + std::to_string(i) + " share their data pointer");
+    for (const Layer &l : net.layers)
+        if ((l.type == YB_YOLO || l.type == YB_REGION) && l.classes > 17395)
+            fatal_throw(f + ": " + std::to_string(l.classes) + " classes, drawing takes at most 17395 (cls * 123457 must fit an int)");
+}
 static int submit_frames(yb_network *n, const char *fn, const FrameBatch &b, int quantized, float thresh, float nms,
-                         int relative, int letter, int max_rows, void *stream) {
+                         int relative, int letter, int max_rows, void *stream, bool draw = false) {
     Network &net = n->net;
     check_frames(net, fn, b);
     check_max_rows(fn, max_rows);
+    if (draw) check_draw(net, fn, b);
     if (!b.host) check_frame_memory(net.device, fn, b);
     Engine *e = get_engine(n, quantized);
-    const int t = engine_submit_frames(e, &net, b, thresh, nms, relative, letter, max_rows, stream);
-    net.last_launches = engine_num_launches(e) + 5;   // + resize, count, emit, iou, nms
+    const int t = engine_submit_frames(e, &net, b, thresh, nms, relative, letter, max_rows, stream, draw);
+    net.last_launches = engine_num_launches(e) + 5 + (draw ? 2 : 0);   // + resize, count, emit, iou, nms (+ select, draw)
     return t;
 }
 
@@ -449,6 +461,28 @@ int yb_network_submit_device_frames(yb_network *n, const yb_device_frame *frames
     YB_TRY
     return submit_frames(n, "submit_device_frames", FrameBatch{frames, nimg, format, false}, quantized, thresh, nms, relative,
                          letter, max_rows, stream);
+    YB_CATCH(-1)
+}
+int yb_network_submit_device_frames_draw(yb_network *n, const yb_device_frame *frames, int nimg, int format, int quantized,
+                                         float thresh, float nms, int letter, int max_rows, void *stream) {
+    YB_TRY
+    return submit_frames(n, "submit_device_frames_draw", FrameBatch{frames, nimg, format, false}, quantized, thresh, nms, 1,
+                         letter, max_rows, stream, true);
+    YB_CATCH(-1)
+}
+// The list of the drawing ticket most recently collected under this number, of whichever engine collected it.
+int yb_network_selected_detections(yb_network *n, int ticket, const yb_detection **dets, const int **counts) {
+    YB_TRY
+    unsigned long long best = 0;
+    for (const std::shared_ptr<Engine> &e : n->net.engine) {
+        const yb_detection *d = nullptr; const int *c = nullptr; unsigned long long seq = 0;
+        if (e && engine_selected_detections(e.get(), ticket, &d, &c, &seq) == 0 && seq > best) {
+            best = seq;
+            if (dets) *dets = d;
+            if (counts) *counts = c;
+        }
+    }
+    return best ? 0 : -1;
     YB_CATCH(-1)
 }
 /* diagnostic: the resized planar float images the device pipeline produced for the last predict_image_u8 */

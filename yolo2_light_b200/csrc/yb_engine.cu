@@ -11,6 +11,7 @@
 #include <dlfcn.h>
 
 #include <algorithm>
+#include <atomic>
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
@@ -104,8 +105,9 @@ struct Engine {
     };
     FrameStage u8;                      // device-side input pipeline + decode geometry of the synchronous calls
     DevBuf<float> d_unit;               // byte value -> float /255. (k_resize_frames)
-    // hand-off of the caller's device frames: produced on the caller's stream (ev_frames_ready) / read (ev_frames_read)
-    Event ev_frames_ready, ev_frames_read;
+    // hand-off of the caller's device frames: produced on the caller's stream (ev_frames_ready) / read (ev_frames_read) /
+    // drawn into (ev_frames_drawn)
+    Event ev_frames_ready, ev_frames_read, ev_frames_drawn;
     // ---- pipelined end-to-end path: H2D(k+1) | compute(k) | D2H(k-1) on three streams -----------------
     struct DetWs {                      // decode + NMS workspace for `cap` candidate rows of `stride` floats per image
         DevBuf<float> rows; DevBuf<unsigned> mask; DevBuf<int> blkcnt, counts;
@@ -122,6 +124,12 @@ struct Engine {
         PinnedBuf<float> h_rows; PinnedBuf<int> h_counts;
         int mode = 0;                   // 0: raw tensors (engine_submit), 1: detections (engine_submit_frames)
         int nimg = 0;                   // images of the batch in this slot (mode 1)
+        // drawing tickets (mode 1 with draw): the selected list in list order and the boxes in draw order (k_det_select),
+        // and the list's pinned host copy, valid from the collect (collect_seq) until the slot is taken again
+        bool draw = false;
+        DevBuf<yb_detection> d_sel; DevBuf<DetDraw> d_draw; DevBuf<int> d_nsel;
+        PinnedBuf<yb_detection> h_sel; PinnedBuf<int> h_nsel;
+        unsigned long long collect_seq = 0;   // 0: no collected list
     };
     std::vector<Slot> slots;
     Stream s_in, s_out, s_det;
@@ -1243,6 +1251,7 @@ static int acquire_slot(Engine *e) {
     Engine::Slot &sl = e->slots[k];
     if (sl.busy) fatal_throw("submit: pipeline full (3 batches in flight) -- collect the oldest ticket first");
     e->next_slot = (k + 1) % (int)e->slots.size();
+    sl.collect_seq = 0;
     CUDA_OK(cudaStreamWaitEvent(e->s_in, sl.ev_comp, 0));
     return k;
 }
@@ -1507,6 +1516,28 @@ int engine_detect(Engine *e, Network *net, const int *w, const int *h, int nimg,
     return stride;
 }
 
+// Selection and drawing of the batch in slot sl (device frames b, geometry table P.geo) on the side stream s, behind its NMS;
+// then `user` waits for the draw.  The counts of selected detections go to the host here, the list itself at the collect.
+static void det_launch_draw(Engine *e, const DetParams &P, Engine::Slot &sl, const FrameBatch &b, cudaStream_t s,
+                            cudaStream_t user) {
+    const int B = e->batch;
+    sl.d_sel.ensure((size_t)B * P.max_rows); sl.d_draw.ensure((size_t)B * P.max_rows); sl.d_nsel.ensure(B);
+    sl.h_sel.ensure((size_t)B * P.max_rows); sl.h_nsel.ensure(B);
+    int P2 = 1; while (P2 < P.max_rows) P2 <<= 1;
+    const size_t smem = (size_t)P2 * 12;   // set every time: with the kernel's static shared memory, 4096 rows pass 48 KB
+    CUDA_OK(cudaFuncSetAttribute(k_det_select, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_det_select<<<(unsigned)b.nimg, 256, smem, s>>>(P, sl.det.rows.get(), sl.det.counts.get(), sl.d_sel.get(), sl.d_nsel.get(),
+                                                      sl.d_draw.get(), P2);
+    auto *k = b.fmt == YB_FRAME_BGR ? k_det_draw<YB_FRAME_BGR> : b.fmt == YB_FRAME_RGB_PLANAR ? k_det_draw<YB_FRAME_RGB_PLANAR>
+            : b.fmt == YB_FRAME_NV12 ? k_det_draw<YB_FRAME_NV12> : k_det_draw<YB_FRAME_RGB>;
+    k<<<dim3((unsigned)b.nimg, DET_DRAW_BANDS), 256, 0, s>>>(P.geo, sl.d_draw.get(), sl.d_nsel.get(), P.max_rows);
+    if (b.nimg < B) CUDA_OK(cudaMemsetAsync(sl.d_nsel.get() + b.nimg, 0, (size_t)(B - b.nimg) * sizeof(int), s));
+    CUDA_OK(cudaMemcpyAsync(sl.h_nsel.get(), sl.d_nsel.get(), (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, s));
+    if (!e->ev_frames_drawn) e->ev_frames_drawn = make_event();
+    CUDA_OK(cudaEventRecord(e->ev_frames_drawn, s));
+    CUDA_OK(cudaStreamWaitEvent(user, e->ev_frames_drawn, 0));
+}
+
 // ---- pipelined detection path (SURVEY 8f rows 1 + 2 in the serving loop) -----------------------------------------
 // One call enqueues, for one batch of nimg 8-bit frames of any sizes: H2D of the frames and of their geometry table + the
 // reference's resize on the copy-in stream, the forward on the compute stream, decode + NMS on a side stream (under the
@@ -1514,8 +1545,10 @@ int engine_detect(Engine *e, Network *net, const int *w, const int *h, int nimg,
 // the candidate rows.  Host traffic per batch: the u8 frames in (a quarter of the float images), counts + rows out (a few
 // hundred KB instead of the 124 MB of yolo tensors).  Device frames are resized the same way, read in order with the caller's
 // `stream`.
+// With `draw`, the side stream then selects each image's detections (k_det_select) and draws them into its device frame
+// (k_det_draw), and the caller's `stream` waits for that draw.
 int engine_submit_frames(Engine *e, Network *net, const FrameBatch &b, float thresh, float nms, int relative, int letter,
-                         int max_rows, void *stream) {
+                         int max_rows, void *stream, bool draw) {
     DetParams P = det_params(net, e->finals, thresh, nms, relative, max_rows);
     const int B = e->batch, stride = 5 + P.classes;
     const int k = acquire_slot(e);
@@ -1542,16 +1575,17 @@ int engine_submit_frames(Engine *e, Network *net, const FrameBatch &b, float thr
     CUDA_OK(cudaStreamWaitEvent(e->s_det, sl.ev_comp, 0));
     CUDA_OK(cudaMemcpyAsync(sl.h_counts.get(), sl.det.counts.get(), (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, e->s_det));
     det_launch_nms(P, sl.det, b.nimg, max_rows, e->s_det);  // no host round trip: grids sized for the cap, kernels read the counts
+    if (draw) det_launch_draw(e, P, sl, b, e->s_det, (cudaStream_t)stream);
     CUDA_OK(cudaEventRecord(sl.ev_det, e->s_det));
     CUDA_OK(cudaGetLastError());
-    sl.busy = true; sl.mode = 1; sl.nimg = b.nimg;
+    sl.busy = true; sl.mode = 1; sl.nimg = b.nimg; sl.draw = draw;
     return k;
 }
 
 // rows: pinned [batch][max_rows][5 + classes] (valid until the slot is reused), counts[batch] (0 beyond the ticket's images);
-// returns 5 + classes.
+// returns 5 + classes.  A drawing ticket's selected list comes back too (engine_selected_detections).
 int engine_collect_detections(Engine *e, int ticket, const float **rows, const int **counts, size_t *d2h_bytes) {
-    const Engine::Slot &sl = release_slot(e, ticket, 1, "collect_detections");
+    Engine::Slot &sl = release_slot(e, ticket, 1, "collect_detections");
     const int B = e->batch, cap = sl.det.cap, stride = sl.det.stride;
     size_t moved = (size_t)B * sizeof(int);
     for (int b = 0; b < sl.nimg; ++b) {
@@ -1562,11 +1596,38 @@ int engine_collect_detections(Engine *e, int ticket, const float **rows, const i
             moved += (size_t)n * stride * sizeof(float);
         }
     }
+    if (sl.draw) {
+        moved += (size_t)B * sizeof(int);
+        for (int b = 0; b < sl.nimg; ++b) {
+            const int n = sl.h_nsel.get()[b];
+            if (n > 0) {
+                CUDA_OK(cudaMemcpyAsync(sl.h_sel.get() + (size_t)b * cap, sl.d_sel.get() + (size_t)b * cap,
+                                        (size_t)n * sizeof(yb_detection), cudaMemcpyDeviceToHost, e->s_out));
+                moved += (size_t)n * sizeof(yb_detection);
+            }
+        }
+    }
     CUDA_OK(cudaStreamSynchronize(e->s_out));
+    if (sl.draw) {
+        static std::atomic<unsigned long long> seq{0};
+        sl.collect_seq = ++seq;
+    }
     if (rows) *rows = sl.h_rows.get();
     if (counts) *counts = sl.h_counts.get();
     if (d2h_bytes) *d2h_bytes = moved;
     return stride;
+}
+
+// The selected list of a collected drawing ticket: 0 and *dets / *counts, with *seq the collect's place among all collects of
+// drawing tickets (so that of several engines the most recent one can be chosen); -1 for any other ticket.
+int engine_selected_detections(Engine *e, int ticket, const yb_detection **dets, const int **counts, unsigned long long *seq) {
+    if (ticket < 0 || ticket >= (int)e->slots.size()) return -1;
+    const Engine::Slot &sl = e->slots[ticket];
+    if (sl.busy || sl.mode != 1 || !sl.draw || !sl.collect_seq) return -1;
+    if (dets) *dets = sl.h_sel.get();
+    if (counts) *counts = sl.h_nsel.get();
+    if (seq) *seq = sl.collect_seq;
+    return 0;
 }
 
 int engine_num_launches(Engine *e) { return (int)e->ops.size(); }

@@ -53,10 +53,12 @@ void engine_collect_ptrs(Engine *e, int ticket, std::vector<const float *> &ptrs
 const char *engine_broadcast_arena(const std::vector<Engine *> &replicas);   // "nccl" | "peer-copy" | "single"
 int engine_device_count();
 // pipelined frames -> detections (device-side resize, forward, decode + NMS; only candidate rows come back); max_rows in
-// 1..DET_MAX_ROWS
+// 1..DET_MAX_ROWS.  draw (device frames): then select each image's detections and draw them into its frame
 int engine_submit_frames(Engine *e, Network *net, const FrameBatch &b, float thresh, float nms, int relative, int letter,
-                         int max_rows, void *stream);
+                         int max_rows, void *stream, bool draw = false);
 int engine_collect_detections(Engine *e, int ticket, const float **rows, const int **counts, size_t *d2h_bytes);
+// the selected list of a collected drawing ticket (yb_network_selected_detections); -1 for any other ticket
+int engine_selected_detections(Engine *e, int ticket, const yb_detection **dets, const int **counts, unsigned long long *seq);
 // throws unless the memory of the device frames of `b` is device or managed memory of `device`
 void check_frame_memory(int device, const char *fn, const FrameBatch &b);
 void engine_fetch_layer(Engine *e, Network *net, int layer, float *dst);

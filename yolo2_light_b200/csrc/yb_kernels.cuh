@@ -116,6 +116,14 @@ __device__ __forceinline__ int nv12_ch(int Y, int U, int V, int k) {
     return nv12_clamp((k == 0 ? yy + 1673527 * v : k == 1 ? yy - 852492 * v - 409993 * u : yy + 2116026 * u) >> 20);
 }
 
+// 8-bit RGB -> BT.601 limited-range Y, U, V, integer form with 8 fractional bits (the direction opposite to nv12_ch; the
+// rule of include/yolo2_light_b200.h, YB_FRAME_NV12).  >> is an arithmetic shift; the results lie in 16..235 / 16..240.
+__device__ __forceinline__ void rgb_to_yuv601(int R, int G, int B, unsigned char *yuv) {
+    yuv[0] = (unsigned char)(((66 * R + 129 * G + 25 * B + 128) >> 8) + 16);
+    yuv[1] = (unsigned char)(((-38 * R - 74 * G + 112 * B + 128) >> 8) + 128);
+    yuv[2] = (unsigned char)(((112 * R - 94 * G - 18 * B + 128) >> 8) + 128);
+}
+
 struct RsSrc {                  // one source row of a chunk; index 0 is column `lo`
     const unsigned char *q[3];  // RGB / BGR / NV12 staged (converted): q[0]; planar: the three planes; NV12 read
                                 // directly: the Y row (q[0]) and the chroma row from column lo & ~1 (q[1])
