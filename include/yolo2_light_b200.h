@@ -58,7 +58,7 @@ enum { YB_PREC_BF16_TC = 0, YB_PREC_FP32 = 1 };
  *              init_gpu_int8x4 :603-611).  parse_convolutional sets it only for a cfg parsed with quantized = 1, and not
  *              for index 0, LINEAR activations, stride > 1 at index > 1, or 1x1 layers (src/additionally.c:3557-3559); the
  *              convolution whose next-but-one section is [yolo] switches it off for the rest of the net (:3996-4003).
- *              Every other convolution is a float one (an XNOR layer keeps its XNOR path), so a network parsed with
+ *              Every other convolution is a float one (an XNOR layer keeps its XNOR path, by the XNOR rule below), so a network parsed with
  *              quantized = 0 runs no INT8 layer.  yb_layer_desc.quantized carries the flag on the drop-in path.
  *      input:  v = x * input_mult rounded once, converted to int as CUDA does (truncation, saturating at +-2^31, NaN -> 0),
  *              clamped to +-127 (cuda_f32_to_int8 + max_abs, src/gpu.cu:730-739).  It agrees with the CPU rule's for
@@ -73,6 +73,34 @@ enum { YB_PREC_BF16_TC = 0, YB_PREC_FP32 = 1 };
  *      convolution the tensor cores take runs on tf32 (the reference's are cuDNN convolutions, which no fixed summation
  *      order reproduces). */
 enum { YB_QUANT_NONE = 0, YB_QUANT_CPU = 1, YB_QUANT_GPU = 2 };
+
+/* XNOR rules (yb_network_set_xnor_rule): which of the reference's two XNOR forwards an XNOR layer ([convolutional] xnor=1)
+ * computes.  The default keeps every result as it was.
+ *  YB_XNOR_CPU (0) : the CPU build's (forward_convolutional_layer_cpu, yolov2_forward_network.c:116-261): input bit x > 0,
+ *      out-of-image taps -1, y = act((float)dot * mean + bias) with a rounded multiply and a rounded add; a layer with
+ *      stride != 1 or pad != 1 is the float convolution of +-1 inputs (zero padding) and +-mean weights.
+ *  YB_XNOR_GPU (1) : the GPU build's (forward_convolutional_layer_gpu_cudnn, yolov2_forward_network_gpu.cu:23-139).  With
+ *      quantized = 0 it replaces network_predict_gpu_cudnn; with quantized = 2 (YB_QUANT_GPU) it completes
+ *      network_predict_gpu_cudnn_quantized, whose l.quantized XNOR layers run in INT8.  quantized = 1 fails: no reference
+ *      binary runs that combination.  mean is the layer's mean_arr[f].
+ *    A. c % 32 == 0, any size, stride and pad: the bit GEMM.  Input bit x > 0, out-of-image taps -1, dot = 2*count - K
+ *       exactly as on the CPU.  y = fmaf((float)dot, mean, bias) -- nvcc contracts the reference's `count * mean + bias` to
+ *       one FFMA (gpu.cu:1981) -- then leaky as `y >= 0 ? y : 0.1f*y` (a float product), any other activation after it.
+ *       A [shortcut] right behind the layer with w == out_w, h == out_h and c == out_c is folded into the GEMM
+ *       (additionally.c:326-338): its output is from + v, with v the layer's leaky-only value, and neither the shortcut's
+ *       activation nor any later one is applied to the sum.
+ *    B. c < 32: the convolution of b(x) = x >= 0 ? +1 : -1 (note >=) and sign(w) * mean, out-of-image taps 0, as the exact
+ *       integer sum s: y = act(s * mean + bias) with a rounded multiply and a rounded add.  The reference runs cuDNN there,
+ *       whose summation order is not reproduced: this is the correctly rounded convolution.
+ *    Leaky is the reference GPU build's `.1f * x`; relu and linear are exact; logistic is the double-precision one of
+ *    every other layer, which may differ from the reference's float `1.f/(1.f+expf(-x))` in the last bit.
+ *    Rejected when the engine is built, with a message: an XNOR layer with c >= 32 and c % 32 != 0 (the reference
+ *    computes no convolution there); a same-shape [shortcut] behind an XNOR layer of path B or one that runs in INT8
+ *    (the reference never writes its output); and one behind a path-A layer whose activation is neither leaky nor linear.
+ *    Batch: the reference's bit GEMM computes image 0 of a batch only; here every image is computed as image 0 would be.
+ *    Do not check this rule against a reference binary built for sm_90: there its XOR bmma becomes an AND-popcount one, so
+ *    it no longer computes the XNOR count.  Non-XNOR layers compute what they compute under YB_XNOR_CPU. */
+enum { YB_XNOR_CPU = 0, YB_XNOR_GPU = 1 };
 
 /* One layer of a prepared network: the subset of the reference's `struct layer` (src/additionally.h:409-684)
  * that the forward path reads (SURVEY 8a, a13).  All pointers are host pointers owned by the caller; the
@@ -152,6 +180,12 @@ void yb_set_batch_network(yb_network *net, int batch);
 /* Select the device (cuda_set_device, src/gpu.cu:97) and the FP32-conv arithmetic for engines built later. */
 int  yb_network_set_device(yb_network *net, int device);
 int  yb_network_set_precision(yb_network *net, int precision /* YB_PREC_* */);
+/* The XNOR rule (YB_XNOR_*) of the engines built after this call; drops the network's engines.  -1 on a bad value.
+ * A network starts with the rule the environment variable YB_XNOR_RULE names when it is created (yb_parse_network_cfg,
+ * yb_network_from_layers): "0" YB_XNOR_CPU, "1" YB_XNOR_GPU; unset means YB_XNOR_CPU, any other value fails the creation.
+ * So a host whose networks are built by code it does not change -- the drop-in glue of a reference binary -- can run the
+ * GPU build's XNOR arithmetic. */
+int  yb_network_set_xnor_rule(yb_network *net, int rule /* YB_XNOR_* */);
 
 /* replaces network_predict_cpu(network net, float *input)   src/yolov2_forward_network.c:632
  * (same slot as network_predict_gpu_cudnn, src/yolov2_forward_network_gpu.cu:547).
@@ -381,10 +415,10 @@ int  yb_network_last_launches(const yb_network *net);
  * unknown name. */
 int  yb_network_set_option(yb_network *net, const char *name, int value);
 /* Engine facts (builds the engine if needed): "launches", "tc_layers" (convolutions on the tensor cores),
-   "act_bytes" (device memory of the activation buffers).  -1: unknown key. */
+   "act_bytes" (device memory of the activation buffers), "xnor_rule" (the engine's YB_XNOR_*).  -1: unknown key. */
 long yb_network_get_info(yb_network *net, int quantized, const char *key);
 /* The tensor-core plan of layer `layer` (builds the engine if needed), read-only: up to n of {kernel (0 k_conv_tc,
- * 1 k_conv_tc_reg, 2 k_stem_tc, 3 k_stem_s2_tc), kind (0 bf16, 1 int8, 2 xnor, 3 tf32, 4 int8 of YB_QUANT_GPU), TW, TH, BN, BK, nt, bstat, stages,
+ * 1 k_conv_tc_reg, 2 k_stem_tc, 3 k_stem_s2_tc), kind (0 bf16, 1 int8, 2 xnor, 3 tf32, 4 int8 of YB_QUANT_GPU, 5 xnor and 6 zero-padded +-1 of YB_XNOR_GPU), TW, TH, BN, BK, nt, bstat, stages,
  * sps, grid, num_work, tma_epi, jshift, out_ldc (output pixel stride, elements; 0: no NHWC output)} into fields; -1 in a
  * field that does not apply to the kernel (the stems' fixed tiles).  Returns the number written: 0 for a layer without a
  * tensor-core plan, -1 on error. */

@@ -16,6 +16,12 @@
  *                                                 images over the GPUs of the box from this one C process)
  *     detection *get_network_boxes_nms_b200(network *net, int w, int h, float thresh, float nms, int relative, int *num,
  *                                           int letter);      (optional: decode + NMS on the device)
+ *     void   network_b200_set_xnor_rule(int rule);    (YB_XNOR_CPU / YB_XNOR_GPU for the handles built after the call: with
+ *                                                 YB_XNOR_GPU, network_predict_b200 computes what network_predict_gpu_cudnn
+ *                                                 computes on an XNOR network, and network_predict_b200_cudnn_quantized
+ *                                                 what network_predict_gpu_cudnn_quantized does.  Until it is called, a
+ *                                                 handle keeps the library's initial rule: YB_XNOR_RULE in the
+ *                                                 environment, else YB_XNOR_CPU)
  *
  * Call sites to switch: src/main.c:199-219, src/main.c:394-414, src/additionally.c:4639-4659.
  * Preconditions are the reference's own (main.c:160-171): parse_network_cfg, load_weights_upto_cpu,
@@ -34,8 +40,15 @@
 #include "yolo2_light_b200.h"
 
 #define YB_GLUE_MAX_NETS 16
-static struct { layer *key; int quantized; yb_network *h; unsigned long stamp; } g_nets[YB_GLUE_MAX_NETS];
+static struct { layer *key; int quantized, xnor_rule; yb_network *h; unsigned long stamp; } g_nets[YB_GLUE_MAX_NETS];
 static unsigned long g_stamp;   /* which handle of a net ran last: the decode must read THAT engine's tensors */
+static int g_xnor_rule = -1;   /* the XNOR rule of the handles built from now on; -1: the library's initial rule */
+
+void network_b200_set_xnor_rule(int rule)
+{
+    if (rule != YB_XNOR_CPU && rule != YB_XNOR_GPU) { fprintf(stderr, "network_b200_set_xnor_rule: bad rule %d\n", rule); exit(1); }
+    g_xnor_rule = rule;
+}
 
 static yb_network *glue_build(network net, int quantized)
 {
@@ -69,6 +82,7 @@ static yb_network *glue_build(network net, int quantized)
     yb_network *h = yb_network_from_layers(d, net.n, net.batch, net.h, net.w, net.c, quantized);
     free(d);
     if (h && net.gpu_index >= 0) yb_network_set_device(h, net.gpu_index);
+    if (h && g_xnor_rule >= 0) yb_network_set_xnor_rule(h, g_xnor_rule);
     return h;
 }
 
@@ -76,14 +90,17 @@ static yb_network *glue_handle(network net, int quantized)
 {
     int k;
     for (k = 0; k < YB_GLUE_MAX_NETS; ++k)
-        if (g_nets[k].h && g_nets[k].key == net.layers && g_nets[k].quantized == quantized) { g_nets[k].stamp = ++g_stamp; return g_nets[k].h; }
+        if (g_nets[k].h && g_nets[k].key == net.layers && g_nets[k].quantized == quantized && g_nets[k].xnor_rule == g_xnor_rule) {
+            g_nets[k].stamp = ++g_stamp;
+            return g_nets[k].h;
+        }
     for (k = 0; k < YB_GLUE_MAX_NETS; ++k)
         if (!g_nets[k].h) {
             g_nets[k].h = glue_build(net, quantized);
-            g_nets[k].key = net.layers; g_nets[k].quantized = quantized; g_nets[k].stamp = ++g_stamp;
+            g_nets[k].key = net.layers; g_nets[k].quantized = quantized; g_nets[k].xnor_rule = g_xnor_rule; g_nets[k].stamp = ++g_stamp;
             return g_nets[k].h;
         }
-    fprintf(stderr, "yolo2_light_b200 glue: more than %d (network, rule) pairs -- raise YB_GLUE_MAX_NETS\n", YB_GLUE_MAX_NETS);
+    fprintf(stderr, "yolo2_light_b200 glue: more than %d (network, rules) triples -- raise YB_GLUE_MAX_NETS\n", YB_GLUE_MAX_NETS);
     exit(1);   /* the reference's error convention: message + exit */
 }
 

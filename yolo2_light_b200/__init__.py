@@ -5,7 +5,7 @@ mirror plus generators for the model definitions / synthetic weights used by the
 """
 from . import cfgs  # noqa: F401
 from .api import (  # noqa: F401
-    YB_PREC_BF16_TC, YB_PREC_FP32, YB_QUANT_CPU, YB_QUANT_GPU, YB_QUANT_NONE, LayerDesc, Network, PinnedBuffer, YbError,
+    YB_PREC_BF16_TC, YB_PREC_FP32, YB_QUANT_CPU, YB_QUANT_GPU, YB_QUANT_NONE, YB_XNOR_CPU, YB_XNOR_GPU, LayerDesc, Network, PinnedBuffer, YbError,
     calculate_binary_weights, lib, load_network, load_weights_upto_cpu, network_from_layers,
     network_predict_b200, network_predict_b200_cudnn_quantized, network_predict_b200_quantized, parse_network_cfg,
     quantinization_and_get_multipliers, yolov2_fuse_conv_batchnorm,

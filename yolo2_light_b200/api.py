@@ -32,6 +32,7 @@ YB_REGION, YB_YOLO, YB_UPSAMPLE, YB_REORG, YB_BLANK = 21, 22, 23, 24, 25
 YB_LOGISTIC, YB_RELU, YB_LINEAR, YB_LEAKY = 0, 1, 3, 7
 YB_PREC_BF16_TC, YB_PREC_FP32 = 0, 1
 YB_QUANT_NONE, YB_QUANT_CPU, YB_QUANT_GPU = 0, 1, 2
+YB_XNOR_CPU, YB_XNOR_GPU = 0, 1
 LAYER_NAMES = {0: "CONVOLUTIONAL", 3: "MAXPOOL", 4: "SOFTMAX", 8: "ROUTE", 13: "SHORTCUT", 21: "REGION", 22: "YOLO",
                23: "UPSAMPLE", 24: "REORG", 25: "BLANK"}
 
@@ -111,6 +112,7 @@ def lib():
         "yb_set_batch_network": (None, [vp, C.c_int]),
         "yb_network_set_device": (C.c_int, [vp, C.c_int]),
         "yb_network_set_precision": (C.c_int, [vp, C.c_int]),
+        "yb_network_set_xnor_rule": (C.c_int, [vp, C.c_int]),
         "yb_network_set_option": (C.c_int, [vp, C.c_char_p, C.c_int]),
         "yb_network_set_letterbox": (C.c_int, [vp, C.c_int]),
         "yb_network_get_info": (C.c_long, [vp, C.c_int, C.c_char_p]),
@@ -174,7 +176,7 @@ EXPORTED_SYMBOLS = [
     "yb_fuse_conv_batchnorm", "yb_calculate_binary_weights", "yb_quantinization_and_get_multipliers",
     "yb_network_from_layers", "yb_free_network", "yb_network_num_layers", "yb_network_dims", "yb_network_layer",
     "yb_network_layer_outputs", "yb_network_input_calibration", "yb_set_batch_network", "yb_network_set_device",
-    "yb_network_set_precision", "yb_network_set_option", "yb_network_get_info", "yb_network_tc_plan", "yb_network_detect", "yb_network_calibrate", "yb_entropy_calibration",
+    "yb_network_set_precision", "yb_network_set_xnor_rule", "yb_network_set_option", "yb_network_get_info", "yb_network_tc_plan", "yb_network_detect", "yb_network_calibrate", "yb_entropy_calibration",
     "yb_network_input_histogram", "yb_map_evaluate", "yb_network_predict", "yb_network_predict_quantized",
     "yb_network_predict_cudnn_quantized",
     "yb_network_predict_image_u8", "yb_network_fetch_input", "yb_network_submit", "yb_network_collect", "yb_network_layer_output", "yb_network_forward_device", "yb_network_sync_outputs", "yb_network_fetch_layer",
@@ -191,7 +193,7 @@ EXPORTED_SYMBOLS = [
 TC_PLAN_FIELDS = ("kernel", "kind", "TW", "TH", "BN", "BK", "nt", "bstat", "stages", "sps", "grid", "num_work", "tma_epi",
                   "jshift", "out_ldc")
 TC_PLAN_KERNELS = ("k_conv_tc", "k_conv_tc_reg", "k_stem_tc", "k_stem_s2_tc")
-TC_PLAN_KINDS = ("bf16", "s8", "xnor", "tf32", "s8_gpu")
+TC_PLAN_KINDS = ("bf16", "s8", "xnor", "tf32", "s8_gpu", "xnor_gpu", "pm1z_gpu")
 
 
 def _check(ok: bool):
@@ -274,6 +276,11 @@ class Network:
 
     def set_precision(self, precision: int):
         _check(lib().yb_network_set_precision(self._h, precision) == 0)
+
+    def set_xnor_rule(self, rule: int):
+        """The XNOR arithmetic of the engines built after this call (``yb_network_set_xnor_rule``): ``YB_XNOR_CPU``
+        (default), the reference CPU build's, or ``YB_XNOR_GPU``, its GPU build's."""
+        _check(lib().yb_network_set_xnor_rule(self._h, rule) == 0)
 
     def set_option(self, name: str, value: int):
         _check(lib().yb_network_set_option(self._h, name.encode(), value) == 0)

@@ -39,6 +39,7 @@ static EngineOptions engine_options(const Network &net, int quantized, int devic
     opt.device = device;
     opt.precision = net.precision;
     opt.rule = quant_rule(quantized);
+    opt.xnor_rule = net.xnor_rule;
     opt.upload = upload;
     opt.fuse = net.fuse;
     opt.keep_counts = net.keep_counts;
@@ -59,11 +60,23 @@ void yb_set_abort_on_error(int on) { g_abort_on_error = on; }
 const char *yb_last_error(void) { return g_last_error.c_str(); }
 const char *yb_version(void) { return "yolo2_light_b200 0.1 (sm_90a)"; }
 
+// The XNOR rule a new network starts with: YB_XNOR_RULE (0 or 1) when set, else YB_XNOR_CPU.  It lets a host program that
+// builds its networks through unchanged code, such as the drop-in glue, choose the GPU build's XNOR arithmetic.
+static int initial_xnor_rule() {
+    const char *v = getenv("YB_XNOR_RULE");
+    if (!v) return YB_XNOR_CPU;
+    if (!strcmp(v, "0")) return YB_XNOR_CPU;
+    if (!strcmp(v, "1")) return YB_XNOR_GPU;
+    fatal_throw(std::string("YB_XNOR_RULE=") + v + ": must be 0 (YB_XNOR_CPU) or 1 (YB_XNOR_GPU)");
+}
+
 yb_network *yb_parse_network_cfg(const char *filename, int batch, int quantized) {
     YB_TRY
+    const int xnor_rule = initial_xnor_rule();
     Network *net = parse_network_cfg(filename, batch, quantized);
     yb_network *h = new yb_network();
     h->net = std::move(*net);
+    h->net.xnor_rule = xnor_rule;
     delete net;
     return h;
     YB_CATCH(nullptr)
@@ -90,6 +103,7 @@ yb_network *yb_network_from_layers(const yb_layer_desc *layers, int n_layers, in
     yb_network *hnd = hold.get();
     Network &net = hnd->net;
     net.batch = batch; net.h = h; net.w = w; net.c = c; net.inputs = h * w * c; net.quantized = quantized;
+    net.xnor_rule = initial_xnor_rule();
     net.layers.resize(n_layers);
     for (int i = 0; i < n_layers; ++i) {
         const yb_layer_desc &d = layers[i];
@@ -217,6 +231,12 @@ int yb_network_set_device(yb_network *n, int device) {
 int yb_network_set_precision(yb_network *n, int precision) {
     if (precision != YB_PREC_BF16_TC && precision != YB_PREC_FP32) { report("bad precision"); return -1; }
     n->net.precision = precision;
+    drop_engines(&n->net);
+    return 0;
+}
+int yb_network_set_xnor_rule(yb_network *n, int rule) {
+    if (rule != YB_XNOR_CPU && rule != YB_XNOR_GPU) { report("bad XNOR rule"); return -1; }
+    n->net.xnor_rule = rule;
     drop_engines(&n->net);
     return 0;
 }

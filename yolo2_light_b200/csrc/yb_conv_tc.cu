@@ -71,11 +71,13 @@ struct TcParams {
     int kind;                 // TcKind: TC_BF16 bf16 x bf16 -> f32;  TC_S8 s8 x s8 -> s32, exact requantising epilogue;
                               // TC_S8_GPU the same GEMM, the GPU rule's unscaled epilogue;
                               // TC_XNOR XNOR layer as +-1 s8 on the s8 wgmma (dot = 2*count - K exactly), reference float epilogue;
+                              // TC_XNOR_GPU the same GEMM, the GPU XNOR rule's bit-GEMM epilogue; TC_PM1Z_GPU zero-padded +-1
+                              // s8 GEMM, the GPU XNOR rule's epilogue of the layers below 32 channels;
                               // TC_TF32 f32 operands read as tf32 (K = 8 per MMA) -> f32: float heads of the exact nets
     int kk;                   // MMAs per K-block (BK bytes / 32)
     float alpha1;             // INT8: R_MULT / (input_mult * weights_mult); TC_S8_GPU: 1 / (input_mult * weights_mult)
-    const float *mean;        // kind 2 (XNOR as +-1 s8): per-filter mean |w|; out = (float)dot * mean + bias
-    int xK;                   // kind 2: true K (size*size*C) for the raw popcount dump: count = (dot + K) / 2
+    const float *mean;        // the XNOR kinds (2, 5, 6): per-filter mean |w|
+    int xK;                   // kinds 2 and 5: true K (size*size*C) for the raw popcount dump: count = (dot + K) / 2
     int *acc_out;             // INT8: optional raw s32 accumulators, NCHW (tests)
     float *yolo_out;          // fused [yolo] layer (reference yolov2_forward_network.c:453-472): NCHW f32 destination, or null
     int yolo_per;             // 4 + classes + 1
@@ -534,11 +536,15 @@ __device__ __forceinline__ void tc_mma_loop(T (&d)[BN / 2], const TcParams &p, u
 }
 
 // The reference's float epilogue of the integer kinds (bit-exact): TC_S8 int8_epilogue; TC_S8_GPU int8_gpu_epilogue; TC_XNOR
-// xnor_epilogue, where the s8 wgmma's acc is dot = 2*count - K exactly.  f: filter index (TC_XNOR reads its mean |w|).
+// xnor_epilogue and TC_XNOR_GPU xnor_gpu_epilogue, where the s8 wgmma's acc is dot = 2*count - K exactly; TC_PM1Z_GPU
+// pm1z_gpu_epilogue, where acc is the zero-padded +-1 sum.  f: filter index (the XNOR kinds read its mean |w|).
 __device__ __forceinline__ float int_epilogue(const TcParams &p, int kind, int acc, int f, float bias) {
     if (kind == TC_S8) return int8_epilogue(acc, p.alpha1, bias, p.act);
     if (kind == TC_S8_GPU) return int8_gpu_epilogue(acc, p.alpha1, bias, p.act);
-    return xnor_epilogue(acc, (f < p.n) ? __ldg(p.mean + f) : 0.f, bias, p.act);
+    const float mean = (f < p.n) ? __ldg(p.mean + f) : 0.f;
+    if (kind == TC_XNOR_GPU) return xnor_gpu_epilogue(acc, mean, bias, p.act);
+    if (kind == TC_PM1Z_GPU) return pm1z_gpu_epilogue(acc, mean, bias, p.act);
+    return xnor_epilogue(acc, mean, bias, p.act);
 }
 
 // One CTA per 128-pixel x BN-filter tile, persistent over the tiles (grid <= #SMs, one CTA per SM).
@@ -611,7 +617,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
             });
         };
         auto run_mainloop = [&]() {
-            // EPI 2: TC_S8_GPU and TC_XNOR run the same s8 wgmma as TC_S8
+            // EPI 2: TC_S8_GPU and the XNOR kinds run the same s8 wgmma as TC_S8
             if constexpr (EPI == 2) mainloop(std::integral_constant<TcKind, TC_S8>{});
             else if (p.kind == TC_BF16) mainloop(std::integral_constant<TcKind, TC_BF16>{});
             else mainloop(std::integral_constant<TcKind, TC_TF32>{});
@@ -798,12 +804,16 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                         for (int j = 0; j < 32; ++j) {
                             const int f = n0 + f0 + j;
                             // raw results: the INT8 accumulator; XNOR: the reference's popcount, (dot + K) / 2
-                            if (f < p.n) p.acc_out[(((size_t)img * p.n + f) * p.OH + oy) * p.OW + ox] = KIND == TC_XNOR ? ((int)v0[j] + p.xK) / 2 : (int)v0[j];
+                            if (f < p.n)
+                                p.acc_out[(((size_t)img * p.n + f) * p.OH + oy) * p.OW + ox] =
+                                    (KIND == TC_XNOR || KIND == TC_XNOR_GPU) ? ((int)v0[j] + p.xK) / 2 : (int)v0[j];
                         }
                     }
                 };
                 if (p.kind == TC_XNOR) int_slabs(std::integral_constant<TcKind, TC_XNOR>{});
                 else if (p.kind == TC_S8_GPU) int_slabs(std::integral_constant<TcKind, TC_S8_GPU>{});
+                else if (p.kind == TC_XNOR_GPU) int_slabs(std::integral_constant<TcKind, TC_XNOR_GPU>{});
+                else if (p.kind == TC_PM1Z_GPU) int_slabs(std::integral_constant<TcKind, TC_PM1Z_GPU>{});
                 else int_slabs(std::integral_constant<TcKind, TC_S8>{});
             } else {
                 for (int f0 = cbeg; f0 < cend; f0 += 64) {
@@ -1543,7 +1553,7 @@ int sm_count() {
     return sms;
 }
 
-bool is_integer(int kind) { return kind == TC_S8 || kind == TC_S8_GPU || kind == TC_XNOR; }
+bool is_integer(int kind) { return kind == TC_S8 || kind == TC_S8_GPU || kind == TC_XNOR || kind == TC_XNOR_GPU || kind == TC_PM1Z_GPU; }
 int elem_size(int kind) { return kind == TC_TF32 ? 4 : is_integer(kind) ? 1 : 2; }   // operand element size
 // operand channels per pixel: the integer kinds read the s8 input's zero-padded channels (their weights are padded alike)
 int operand_channels(const TcConv &c) { return is_integer(c.kind) ? c.in.ldc : c.l->c; }

@@ -33,7 +33,7 @@ struct TcConv {
     int ldn = 0;
     const float *bias = nullptr;
     float alpha1 = 0.f;            // TC_S8: R_MULT / (input_mult * weights_mult); TC_S8_GPU: 1 / (input_mult * weights_mult)
-    const float *mean = nullptr;   // TC_XNOR: per-filter mean |w|
+    const float *mean = nullptr;   // TC_XNOR, TC_XNOR_GPU, TC_PM1Z_GPU: per-filter mean |w|
     int *acc_out = nullptr;        // integer kinds: raw s32 accumulators / popcounts, NCHW (tests), or null
     float *yolo_out = nullptr;     // fused [yolo] layer: its NCHW f32 output, or null
     int yolo_classes = 0;

@@ -53,6 +53,8 @@ enum TcKind {
     TC_TF32 = 3,   // f32 operands read as tf32: the float detection heads of the exact (INT8 / XNOR) networks, and every float
                    // convolution of the GPU INT8 rule; f32 output
     TC_S8_GPU = 4, // INT8 of the GPU rule: s8 x s8 -> s32, the unscaled epilogue int8_gpu_epilogue; f32 output
+    TC_XNOR_GPU = 5,  // XNOR layer of the GPU XNOR rule, c % 32 == 0: TC_XNOR's GEMM, the bit GEMM's epilogue xnor_gpu_epilogue
+    TC_PM1Z_GPU = 6,  // XNOR layer of the GPU XNOR rule, c < 32: +-1 s8 (SIDE_PM1Z_S8) x +-1 s8 -> s32, pm1z_gpu_epilogue
 };
 
 // The converted ("side") input of an integer convolution, padded NHWC.  The four integer formats are what the kernels write;
@@ -64,12 +66,15 @@ enum SideFmt {
     SIDE_PM1_S8,     // +-1 bytes, +1 where x > 0: XNOR layers on the s8 wgmma
     SIDE_BITS,       // sign bits, bit = (x > 0), 32 channels per 32-bit word: XNOR layers on the popcount kernels
     SIDE_S8_SAT,     // s8 quant_i8_sat(x, the layer's input multiplier): INT8 convolutions of the GPU rule
+    SIDE_PM1Z_S8,    // +-1 bytes, +1 where x >= 0, zero border: XNOR layers below 32 channels under the GPU XNOR rule
 };
 
 // channels per 32-bit word of an integer side format
 __host__ __device__ constexpr int side_per_word(SideFmt f) { return f == SIDE_BITS ? 32 : 4; }
 // the formats the kernels write: everything but the plan-only SIDE_NONE and SIDE_PM1_F32
-__host__ __device__ constexpr bool side_int(SideFmt f) { return f == SIDE_S8 || f == SIDE_PM1_S8 || f == SIDE_BITS || f == SIDE_S8_SAT; }
+__host__ __device__ constexpr bool side_int(SideFmt f) {
+    return f == SIDE_S8 || f == SIDE_PM1_S8 || f == SIDE_BITS || f == SIDE_S8_SAT || f == SIDE_PM1Z_S8;
+}
 // the s8 formats of the INT8 layers: the byte is the quantised activation under the layer's input multiplier
 __host__ __device__ constexpr bool side_s8(SideFmt f) { return f == SIDE_S8 || f == SIDE_S8_SAT; }
 
@@ -98,13 +103,15 @@ __device__ __forceinline__ int quant_i8_sat(float x, float mult) {
 }
 
 // One f32 value in side format F: the s8 byte (mult: the layer's input multiplier), the +-1 byte or the sign bit, in the low
-// bits of the result.  The sign is x > 0 (binarize_cpu, float_to_bit): NaN, -inf and -FLT_MAX give -1 / 0 alike.
+// bits of the result.  The sign is x > 0 (binarize_cpu, float_to_bit): NaN, -inf and -FLT_MAX give -1 / 0 alike.  SIDE_PM1Z_S8
+// takes x >= 0 instead (binarize_kernel of the GPU build, gpu.cu:813-818): +0 and -0 give +1, NaN gives -1.
 template <SideFmt F>
 __device__ __forceinline__ uint32_t side_code(float x, float mult) {
     static_assert(side_int(F), "integer side formats only");
     if constexpr (F == SIDE_S8) return (uint32_t)quant_i8(x, mult) & 0xffu;
     else if constexpr (F == SIDE_S8_SAT) return (uint32_t)quant_i8_sat(x, mult) & 0xffu;
     else if constexpr (F == SIDE_PM1_S8) return x > 0.f ? 0x01u : 0xFFu;
+    else if constexpr (F == SIDE_PM1Z_S8) return x >= 0.f ? 0x01u : 0xFFu;
     else return x > 0.f ? 1u : 0u;
 }
 
@@ -159,6 +166,30 @@ __device__ __forceinline__ float int8_epilogue(int acc, float alpha1, float bias
 // Monotone non-decreasing in acc for alpha1 > 0, as the fused max-pool needs.
 __device__ __forceinline__ float int8_gpu_epilogue(int acc, float alpha1, float bias, int act) {
     return act_exact(__fadd_rn(__fmul_rn((float)acc, alpha1), bias), act);
+}
+
+// The activations of the GPU XNOR rule.  Leaky is the bit GEMM's fused `v >= 0 ? v : 0.1f*v` (gpu.cu:1983), a float product;
+// it equals the activation kernel's `(x > 0) ? x : .1f*x` on every input, -0 included.  The others are act_exact: relu is the
+// same expression as the reference's; logistic there is `1.f/(1.f+expf(-x))` in float, which may differ from act_exact's
+// double-precision logistic in the last bit.
+__device__ __forceinline__ float act_gpu(float x, int act) {
+    if (act == ACT_LEAKY) return x >= 0.f ? x : __fmul_rn(0.1f, x);
+    return act_exact(x, act);
+}
+
+// Epilogue of an XNOR layer with c % 32 == 0 under the GPU XNOR rule (gemm_nn_custom_bin_mean_transposed_tensor_kernel,
+// gpu.cu:1974-1990), dot = 2*count - K: `(float)dot * mean + bias`, which nvcc contracts to one FFMA -- one rounding -- then
+// the activation.  Monotone non-decreasing in dot for mean > 0, as the fused max-pool needs.
+__device__ __forceinline__ float xnor_gpu_epilogue(int dot, float mean, float bias, int act) {
+    return act_gpu(__fmaf_rn((float)dot, mean, bias), act);
+}
+
+// Epilogue of an XNOR layer with c < 32 under the GPU XNOR rule (yolov2_forward_network_gpu.cu:94-138): s = sum of
+// sign(w) * b(x) with b(x) = x >= 0 ? +1 : -1 and out-of-image taps 0, the convolution of the +-mean weights as the exact
+// integer s times mean, rounded once; then add_bias_gpu (a second rounding) and the activation.  cuDNN's own summation order
+// is not reproduced: this is the correctly rounded convolution.
+__device__ __forceinline__ float pm1z_gpu_epilogue(int s, float mean, float bias, int act) {
+    return act_gpu(__fadd_rn(__fmul_rn((float)s, mean), bias), act);
 }
 
 }  // namespace yb

@@ -55,8 +55,8 @@ struct ConvWeights {   // offsets into the weight arena
     int cpad = 0;     // padded channels of the s8 / bits / bf16 layouts
 };
 
-// The diagnostic YB_* switches of the library (DESIGN, appendix), read once when an engine is built; nothing else reads the
-// environment.
+// The diagnostic YB_* switches of the library (DESIGN, appendix), read once when an engine is built; nothing else in the engine
+// reads the environment (YB_XNOR_RULE, a network's initial XNOR rule, is read when the network is created).
 struct Switches {
     bool no_graph, no_nccl, no_tc, no_tf32, no_stem, no_stem_tc, no_stem_u8, no_stem_pool_fuse, no_stem_s2_fuse,
          no_conv_pool_fuse, no_pool_fuse, no_yolo_fuse;
@@ -187,7 +187,8 @@ template <typename T> struct same_type { using type = T; };   // keeps a paramet
 // plan only: each picks its kernel instantiation and launch shape once, and the op repeats that launch.
 
 enum FirstOp { FIRST_NHWC, FIRST_STEM_SIMT, FIRST_STEM_TC, FIRST_STEM_S2, FIRST_STEM_POOL };
-enum ConvPath { CP_NONE, CP_TC, CP_TF32, CP_SIMT, CP_XNOR_FALLBACK, CP_XNOR_TC, CP_XNOR_SMALLK, CP_XNOR_GENERAL, CP_I8_TC, CP_I8_SIMT };
+enum ConvPath { CP_NONE, CP_TC, CP_TF32, CP_SIMT, CP_XNOR_FALLBACK, CP_XNOR_TC, CP_XNOR_SMALLK, CP_XNOR_GENERAL, CP_I8_TC, CP_I8_SIMT,
+                CP_PM1Z_TC, CP_PM1Z_SIMT };
 
 struct LayerPlan {
     int variant = 0;            // convolutions: 0 fp32, 1 xnor, 2 int8
@@ -198,6 +199,7 @@ struct LayerPlan {
     SideFmt pool = SIDE_NONE;   // conv: runs the max-pool behind it and writes layer i+2's converted input (in its side format)
     bool pool_in_conv = false;  // max-pool: runs in the epilogue of the convolution in front of it
     bool pool_to_side = false;  // max-pool: writes the next convolution's converted input instead of its own output
+    bool sc_bin = false;        // shortcut: behind a GPU-rule XNOR layer, whose bit GEMM adds it without its activation
     bool prefilled = false;     // conv: its converted input is written by the op in front of it
     bool in_first_op = false;   // computed by the op that reads the caller's images
     int out_dt = DT_F32;
@@ -272,11 +274,28 @@ struct Builder {
     bool xnor_on_tc(const Layer &l) const {
         return sw.xnor_tc && l.xnor && l.c % 16 == 0 && l.c >= sw.xnor_tc_minc && l.size == 3 && l.stride == 1 && l.pad == 1 && l.n >= 8;
     }
-    // XNOR layers with stride != 1 or pad != 1 never reach the bit GEMM in the reference: forward_convolutional_layer_cpu
-    // binarises the input to +-1 floats (binarize_cpu, additionally.c:128-134), swaps in the +-mean weights (binarize_weights,
-    // :113-126) and runs the ordinary im2col + gemm_nn (yolov2_forward_network.c:40-50, :204) -- out-of-image taps count 0 there,
-    // not -1.  Same here: k_binarize_pm1 + the exact-order float convolution.
-    static bool xnor_fallback(const Layer &l) { return l.xnor && !(l.stride == 1 && l.pad == 1); }
+    // CPU XNOR rule: XNOR layers with stride != 1 or pad != 1 never reach the bit GEMM in the reference:
+    // forward_convolutional_layer_cpu binarises the input to +-1 floats (binarize_cpu, additionally.c:128-134), swaps in the +-mean
+    // weights (binarize_weights, :113-126) and runs the ordinary im2col + gemm_nn (yolov2_forward_network.c:40-50, :204) --
+    // out-of-image taps count 0 there, not -1.  Same here: k_binarize_pm1 + the exact-order float convolution.  The GPU XNOR rule
+    // runs every geometry of c % 32 == 0 on the bit GEMM.
+    bool xnor_fallback(const Layer &l) const { return l.xnor && opt.xnor_rule == YB_XNOR_CPU && !(l.stride == 1 && l.pad == 1); }
+    // GPU XNOR rule (forward_convolutional_layer_gpu_cudnn, yolov2_forward_network_gpu.cu:23-139): an XNOR layer below 32 channels
+    // is a zero-padded +-1 convolution (path B); one with c % 32 == 0 runs the bit GEMM (path A).
+    bool xnor_gpu(int i) const { return L[i].variant == 1 && opt.xnor_rule == YB_XNOR_GPU; }
+    bool pm1z(int i) const { return xnor_gpu(i) && layer(i).c < 32; }
+    // XNOR layer i on the s8 wgmma; under the GPU XNOR rule only where the tile takes its activation, the others stay on the
+    // CUDA cores
+    bool xnor_tc(int i) const {
+        const Layer &l = layer(i);
+        return xnor_on_tc(l) && (!xnor_gpu(i) || l.activation == YB_LEAKY || l.activation == YB_LINEAR);
+    }
+    // a [shortcut] the GPU build folds into XNOR layer i's bit GEMM (calculate_binary_weights, additionally.c:326-338)
+    bool bin_shortcut(int i) const {
+        if (opt.xnor_rule != YB_XNOR_GPU || !layer(i).xnor || i + 1 >= nl) return false;
+        const Layer &s = layer(i + 1);
+        return s.type == YB_SHORTCUT && s.w == s.out_w && s.h == s.out_h && s.c == s.out_c;
+    }
 
     // conv i -> 2x2/2 max-pool i+1 -> integer conv i+2, nothing else reading i or i+1: the pool and the next layer's input
     // conversion may run in conv i's epilogue.  Returns layer i+2's side format, or SIDE_NONE.
@@ -327,7 +346,9 @@ struct Builder {
         auto out = [&](int j) { return placed ? e.out_tv[j] : layout_view(j); };
         auto side = [&](int j) { return placed ? side_placed(j) : side_view(j, kLayoutBase); };
         TcConv c;
-        c.kind = p.variant == 2 ? (opt.rule == YB_QUANT_GPU ? TC_S8_GPU : TC_S8) : p.variant == 1 ? TC_XNOR : ADT == DT_BF16 ? TC_BF16 : TC_TF32;
+        c.kind = p.variant == 2 ? (opt.rule == YB_QUANT_GPU ? TC_S8_GPU : TC_S8)
+               : p.variant == 1 ? (pm1z(i) ? TC_PM1Z_GPU : xnor_gpu(i) ? TC_XNOR_GPU : TC_XNOR)
+               : ADT == DT_BF16 ? TC_BF16 : TC_TF32;
         c.l = &l;
         c.in = p.variant != 0 ? side(i) : !placed ? layout_in(i) : i == 0 ? e.in0 : e.out_tv[i - 1];
         c.out = out(tgt);
@@ -348,7 +369,8 @@ struct Builder {
         c.ldn = cw[i].ldn;
         c.bias = bias(i);
         if (c.kind == TC_S8 || c.kind == TC_S8_GPU) c.alpha1 = alpha1(l);
-        if (c.kind == TC_XNOR) c.mean = reinterpret_cast<const float *>(e.w_arena.get() + cw[i].mean);
+        if (c.kind == TC_XNOR || c.kind == TC_XNOR_GPU || c.kind == TC_PM1Z_GPU)
+            c.mean = reinterpret_cast<const float *>(e.w_arena.get() + cw[i].mean);
         c.acc_out = e.counts[i].get();
         if (p.yolo_fused) {
             c.yolo_out = e.finals[i + 1].d.get();
@@ -359,6 +381,9 @@ struct Builder {
 
     // ---- pass 1: the layer plan ------------------------------------------------------------------------------------------
     void plan_layers() {
+        // no reference binary runs the CPU build's INT8 forward with the GPU build's XNOR arithmetic
+        if (opt.rule == YB_QUANT_CPU && opt.xnor_rule == YB_XNOR_GPU)
+            fatal_throw("engine: the GPU XNOR rule runs with quantized = 0 or 2 (YB_QUANT_GPU), not with the CPU INT8 rule (quantized = 1)");
         bool any_xnor = false;
         for (int i = 0; i < nl; ++i) {
             const Layer &l = layer(i);
@@ -391,6 +416,9 @@ struct Builder {
                 L[i + 1].fused_sc = true;
             }
         }
+
+        for (int i = 0; i + 1 < nl; ++i)
+            if (is_conv(i) && bin_shortcut(i)) L[i + 1].sc_bin = true;
 
         // output dtypes and homes (own buffer, or a channel slice of a concat buffer)
         for (int i = 0; i < nl; ++i) {
@@ -431,8 +459,9 @@ struct Builder {
             if (!is_conv(i)) continue;
             const Layer &l = layer(i);
             LayerPlan &p = L[i];
-            if (p.variant == 1 && xnor_fallback(l)) { p.side = SIDE_PM1_F32; p.side_ld = l.c; }
-            else if (p.variant == 1 && xnor_on_tc(l)) { p.side = SIDE_PM1_S8; p.side_ld = (int)align_up(l.c, 32); }   // pad channels meet zero weights
+            if (pm1z(i)) { p.side = SIDE_PM1Z_S8; p.side_ld = (int)align_up(l.c, 32); }   // zero border, pad channels meet zero weights
+            else if (p.variant == 1 && xnor_fallback(l)) { p.side = SIDE_PM1_F32; p.side_ld = l.c; }
+            else if (p.variant == 1 && xnor_tc(i)) { p.side = SIDE_PM1_S8; p.side_ld = (int)align_up(l.c, 32); }   // pad channels meet zero weights
             else if (p.variant == 1) { p.side = SIDE_BITS; p.side_ld = (l.c + 31) / 32; }
             else if (p.variant == 2) {   // every INT8 layer fits the s8 wgmma tile
                 p.side = opt.rule == YB_QUANT_GPU ? SIDE_S8_SAT : SIDE_S8;
@@ -461,6 +490,7 @@ struct Builder {
             switch (l.type) {
             case YB_CONVOLUTIONAL: {
                 if (!L[p.fused_into >= 0 ? p.fused_into : i].has_out) fatal_throw("engine: conv output not placed");
+                if (opt.xnor_rule == YB_XNOR_GPU && l.xnor) reject_xnor_gpu(i);
                 const int in_c = i == 0 ? net.c : layer(i - 1).out_c, in_h = i == 0 ? net.h : layer(i - 1).out_h,
                           in_w = i == 0 ? net.w : layer(i - 1).out_w;
                 if (in_c != l.c || in_h != l.h || in_w != l.w) fatal_throw("engine: conv input shape mismatch");
@@ -497,6 +527,22 @@ struct Builder {
         }
     }
 
+    // the XNOR layers the GPU XNOR rule cannot state as a convolution
+    void reject_xnor_gpu(int i) const {
+        const Layer &l = layer(i);
+        const std::string at = "engine: GPU XNOR rule: XNOR layer " + std::to_string(i) + " (" + std::to_string(l.c) + " channels) ";
+        // the bit GEMM without the weight inversion (additionally.c:221-261): a sign-flipped, offset value read from
+        // alignment bits of an uninitialised workspace
+        if (l.c >= 32 && l.c % 32 != 0) fatal_throw(at + "has c >= 32 and c % 32 != 0, where the reference computes no convolution");
+        if (!(i + 1 < nl && L[i + 1].sc_bin)) return;
+        // the GPU build turns the shortcut into a blank layer and only the bit GEMM writes its output
+        if (L[i].variant == 2) fatal_throw(at + "runs in INT8, so nothing writes the output of the [shortcut] behind it");
+        if (l.c < 32) fatal_throw(at + "is a +-1 convolution below 32 channels, so nothing writes the output of the [shortcut] behind it");
+        // the sum takes the leaky-only value, which the engine keeps as the layer's output for leaky and linear layers only
+        if (l.activation != YB_LEAKY && l.activation != YB_LINEAR)
+            fatal_throw(at + "is followed by a [shortcut] and has an activation other than leaky or linear, which is not supported");
+    }
+
     int conv_path(int i) const {
         const Layer &l = layer(i);
         const LayerPlan &p = L[i];
@@ -522,15 +568,17 @@ struct Builder {
         if (idt != DT_F32 || odt != DT_F32)
             fatal_throw(p.variant == 1 ? "engine: xnor path needs f32 activations" : "engine: int8 path needs f32 activations");
         if (p.variant == 2) return (!sw.no_tc && tc_conv_supported(tc_query)) ? CP_I8_TC : CP_I8_SIMT;
+        if (pm1z(i)) return (xnor_tc(i) && tc_conv_supported(tc_query)) ? CP_PM1Z_TC : CP_PM1Z_SIMT;
         if (xnor_fallback(l)) return CP_XNOR_FALLBACK;
-        if (xnor_on_tc(l) && vec4_view(tin)) {
+        if (xnor_tc(i) && vec4_view(tin)) {
             if (!tc_conv_supported(tc_query)) fatal_throw("engine: xnor tensor-core layer not supported by the i8 tile");
             return CP_XNOR_TC;
         }
         // small K: one thread per pixel, all filters (weights broadcast from shared memory).  It stores 4 filters per float4,
         // so every pixel of its output must be 16-byte aligned: a channel slice of a route's buffer may not be.
         const int CW = p.side_ld;
-        if (CW <= 2 && l.size == 3 && (size_t)l.n * 9 * CW * 4 <= 40 * 1024 && vec4_view(tout)) return CP_XNOR_SMALLK;
+        if (CW <= 2 && l.size == 3 && l.stride == 1 && l.pad == 1 && (size_t)l.n * 9 * CW * 4 <= 40 * 1024 && vec4_view(tout))
+            return CP_XNOR_SMALLK;
         return CP_XNOR_GENERAL;
     }
 
@@ -588,7 +636,7 @@ struct Builder {
             // max-pool i+1 and layer i+2's input conversion in the epilogue
             const SideFmt pf = conv_pool_fmt(i);
             bool pool = false;
-            if (p.path == CP_XNOR_TC || p.path == CP_I8_TC) {
+            if (p.path == CP_XNOR_TC || p.path == CP_I8_TC || p.path == CP_PM1Z_TC) {
                 pool = pf != SIDE_NONE && tc_conv_supported(tc_conv(i, false, pf));
             } else if (p.path == CP_XNOR_SMALLK) {
                 pool = pf == SIDE_PM1_S8 || pf == SIDE_BITS;
@@ -771,12 +819,13 @@ struct Builder {
         const Layer &l0 = layer(0);
         const int act = l0.activation, H = l0.h, W = l0.w;
         if (first == FIRST_STEM_POOL) {
-            // by layer 2's side format (SIDE_S8, SIDE_PM1_S8, SIDE_BITS, SIDE_S8_SAT) and the stem's activation
-            decltype(&k_stem_pool<SIDE_S8, ACT_LEAKY>) const k[4][2] = {
+            // by layer 2's side format (SIDE_S8, SIDE_PM1_S8, SIDE_BITS, SIDE_S8_SAT, SIDE_PM1Z_S8) and the stem's activation
+            decltype(&k_stem_pool<SIDE_S8, ACT_LEAKY>) const k[5][2] = {
                 {k_stem_pool<SIDE_S8, ACT_LEAKY>, k_stem_pool<SIDE_S8, ACT_LINEAR>},
                 {k_stem_pool<SIDE_PM1_S8, ACT_LEAKY>, k_stem_pool<SIDE_PM1_S8, ACT_LINEAR>},
                 {k_stem_pool<SIDE_BITS, ACT_LEAKY>, k_stem_pool<SIDE_BITS, ACT_LINEAR>},
-                {k_stem_pool<SIDE_S8_SAT, ACT_LEAKY>, k_stem_pool<SIDE_S8_SAT, ACT_LINEAR>}};
+                {k_stem_pool<SIDE_S8_SAT, ACT_LEAKY>, k_stem_pool<SIDE_S8_SAT, ACT_LINEAR>},
+                {k_stem_pool<SIDE_PM1Z_S8, ACT_LEAKY>, k_stem_pool<SIDE_PM1Z_S8, ACT_LINEAR>}};
             const Layer &c2 = layer(2);
             push_input_kernel(OP_CONV_SIMT, 0, k[L[2].side - SIDE_S8][act == ACT_LEAKY ? 0 : 1],
                               (unsigned)(((long)B * c2.h * c2.w + 127) / 128), 128, side_placed(2), stem_weights<16>(l0), act, H, W,
@@ -807,9 +856,9 @@ struct Builder {
     // k_int_input: convolution j's converted input from tin, behind a size x size / stride max-pool (1 / 1 / 0: the conversion
     // alone)
     void push_int_input(int kind, int i, int j, const TV &tin, int size, int stride, int pad) {
-        const SideFmt f = L[j].side;   // SIDE_S8, SIDE_PM1_S8, SIDE_BITS or SIDE_S8_SAT
-        void (*const k[4])(TV, TV, int, int, int, float) = {k_int_input<SIDE_S8>, k_int_input<SIDE_PM1_S8>, k_int_input<SIDE_BITS>,
-                                                            k_int_input<SIDE_S8_SAT>};
+        const SideFmt f = L[j].side;   // SIDE_S8, SIDE_PM1_S8, SIDE_BITS, SIDE_S8_SAT or SIDE_PM1Z_S8
+        void (*const k[5])(TV, TV, int, int, int, float) = {k_int_input<SIDE_S8>, k_int_input<SIDE_PM1_S8>, k_int_input<SIDE_BITS>,
+                                                            k_int_input<SIDE_S8_SAT>, k_int_input<SIDE_PM1Z_S8>};
         const TV q = side_placed(j);
         push_kernel(kind, i, k[f - SIDE_S8], grid_for((long)B * q.H * q.W * int_input_groups(f, tin.C)), 256, 0, tin, q, size, stride, pad,
                     side_mult(j));
@@ -846,6 +895,10 @@ struct Builder {
             sp.CW = p.side_ld / 4;
             sp.w = e.w_arena.get() + cw[i].w_s8;
             sp.alpha1 = alpha1(l);
+        } else if (p.side == SIDE_PM1Z_S8) {
+            sp.CW = p.side_ld / 4;
+            sp.w = e.w_arena.get() + cw[i].w_s8;
+            sp.mean = reinterpret_cast<const float *>(e.w_arena.get() + cw[i].mean);
         }
         if (sp.CW) {
             sp.K = taps * sp.CW;
@@ -892,12 +945,17 @@ struct Builder {
             return;
         }
         int32_t *cnt_dbg = counts_buffer(i);
-        if (p.path == CP_XNOR_TC) {
+        const bool gpu = xnor_gpu(i);
+        if (p.path == CP_XNOR_TC || p.path == CP_PM1Z_TC) {
             push_tc_plan(OP_CONV_TC_I8, i);
             return;
         }
+        if (p.path == CP_PM1Z_SIMT) {
+            push_conv_simt(OP_CONV_XNOR, i, k_conv_simt<SimtPm1zGpu>, side_placed(i), tout);
+            return;
+        }
         if (p.path == CP_XNOR_GENERAL) {
-            push_conv_simt(OP_CONV_XNOR, i, k_conv_simt<SimtXnor>, side_placed(i), tout);
+            push_conv_simt(OP_CONV_XNOR, i, gpu ? k_conv_simt<SimtXnorGpu> : k_conv_simt<SimtXnor>, side_placed(i), tout);
             return;
         }
         const int CW = p.side_ld;
@@ -913,16 +971,20 @@ struct Builder {
         if (p.pool != SIDE_NONE) {
             // the 2x2 max-pool behind this layer and the next XNOR layer's sign extraction run in this kernel, which reads only
             // the shape of the output it does not write.  By sign words per tap and the next layer's side format (SIDE_PM1_S8,
-            // SIDE_BITS).
-            void (*const k[2][2])(XnorP, TV) = {{k_conv_xnor_smallk_pool<1, SIDE_PM1_S8>, k_conv_xnor_smallk_pool<1, SIDE_BITS>},
-                                                {k_conv_xnor_smallk_pool<2, SIDE_PM1_S8>, k_conv_xnor_smallk_pool<2, SIDE_BITS>}};
+            // SIDE_BITS) and the XNOR rule.
+            void (*const k[2][2][2])(XnorP, TV) = {
+                {{k_conv_xnor_smallk_pool<1, SIDE_PM1_S8>, k_conv_xnor_smallk_pool<1, SIDE_BITS>},
+                 {k_conv_xnor_smallk_pool<2, SIDE_PM1_S8>, k_conv_xnor_smallk_pool<2, SIDE_BITS>}},
+                {{k_conv_xnor_smallk_pool_gpu<1, SIDE_PM1_S8>, k_conv_xnor_smallk_pool_gpu<1, SIDE_BITS>},
+                 {k_conv_xnor_smallk_pool_gpu<2, SIDE_PM1_S8>, k_conv_xnor_smallk_pool_gpu<2, SIDE_BITS>}}};
             xp.out = make_tv(nullptr, B, l.out_h, l.out_w, l.n, L[i].ldc, P, DT_F32, 0);
             const Layer &c2 = layer(i + 2);
-            push_kernel(OP_CONV_XNOR, i, k[CW - 1][p.pool - SIDE_PM1_S8], (unsigned)(((long)B * c2.h * c2.w + 127) / 128), 128, smem, xp,
+            push_kernel(OP_CONV_XNOR, i, k[gpu][CW - 1][p.pool - SIDE_PM1_S8], (unsigned)(((long)B * c2.h * c2.w + 127) / 128), 128, smem, xp,
                         side_placed(i + 2));
             return;
         }
-        push_kernel(OP_CONV_XNOR, i, CW == 1 ? k_conv_xnor_smallk<1> : k_conv_xnor_smallk<2>, (unsigned)((M + 127) / 128), 128, smem, xp);
+        void (*const k[2][2])(XnorP) = {{k_conv_xnor_smallk<1>, k_conv_xnor_smallk<2>}, {k_conv_xnor_smallk_gpu<1>, k_conv_xnor_smallk_gpu<2>}};
+        push_kernel(OP_CONV_XNOR, i, k[gpu][CW - 1], (unsigned)((M + 127) / 128), 128, smem, xp);
     }
 
     void emit_conv_int8(int i) {
@@ -968,11 +1030,13 @@ struct Builder {
         }
         case YB_SHORTCUT: {
             if (p.fused_sc) break;
-            // shortcut_cpu(batch, w1=l.w, h1=l.h, c1=l.c (from), add, w2=l.out_w, ...): yolov2_forward_network.c:410
+            // shortcut_cpu(batch, w1=l.w, h1=l.h, c1=l.c (from), add, w2=l.out_w, ...): yolov2_forward_network.c:410.  Behind a
+            // GPU-rule XNOR layer (sc_bin): the bit GEMM's `shortcut_out = shortcut_in + v` (gpu.cu:1988-1990), without the
+            // shortcut's activation; the layer plan admits only leaky and linear layers there, whose output is v.
             const int stride = std::max(l.w / l.out_w, 1), sample = std::max(l.out_w / l.w, 1);
             const int minw = std::min(l.w, l.out_w), minh = std::min(l.h, l.out_h), minc = std::min(l.c, l.out_c);
             push_kernel(OP_SHORTCUT, i, BY_DT(k_shortcut, dt), g, 256, 0, tin, e.out_tv[l.index], tout, stride, sample, minw, minh,
-                        minc, l.activation);
+                        minc, p.sc_bin ? (int)ACT_LINEAR : l.activation);
             break;
         }
         case YB_ROUTE: {
@@ -1645,6 +1709,7 @@ int engine_op_kernels(Engine *e, int *layer, int *kind, const char **name, int m
 }
 long engine_info(Engine *e, const char *key) {
     if (!strcmp(key, "launches")) return (long)e->ops.size();
+    if (!strcmp(key, "xnor_rule")) return e->opt.xnor_rule;
     if (!strcmp(key, "tc_layers")) return e->n_tc;
     if (!strcmp(key, "act_bytes")) return (long)e->act_arena.count();
     return -1;

@@ -22,6 +22,7 @@ struct EngineOptions {
     int device = 0;
     int precision = YB_PREC_BF16_TC;
     int rule = YB_QUANT_NONE;  // INT8 layer rule: none, the CPU build's (yolov2_forward_network_q) or the GPU build's (l.quantized)
+    int xnor_rule = YB_XNOR_CPU;   // XNOR arithmetic: the CPU build's or the GPU build's (forward_convolutional_layer_gpu_cudnn)
     bool fuse = true;          // conv + shortcut fusion, route aliasing (YB_NO_FUSE=1 turns it off in every engine)
     bool upload = true;        // upload the weight arena (false on non-root ranks before the broadcast)
     int q_index_offset = 0;    // added to the layer index in the `i >= 1` INT8 rule of YB_QUANT_CPU (single-layer runs)

@@ -289,6 +289,10 @@ static __global__ void __launch_bounds__(RS_THREADS) k_resize_frames(const Image
 //   SimtInt8  words of 4 s8 values (reference yolov2_forward_network_quantized.c:527-631): acc32 = sum xq*wq (dp4a, exact),
 //       out = int8_epilogue(acc32).  INT8 layers the s8 wgmma tile refuses.
 //   SimtInt8Gpu  the same GEMM, out = int8_gpu_epilogue(acc32): the INT8 layers of the GPU rule the s8 wgmma tile refuses.
+//   SimtXnorGpu  SimtXnor's GEMM, out = xnor_gpu_epilogue(2*count - K, mean[f], bias[f]): the XNOR layers with c % 32 == 0 of
+//       the GPU XNOR rule, of any size, stride and pad, off the s8 wgmma and the small-K kernel.
+//   SimtPm1zGpu  SimtInt8's GEMM over +-1 bytes (SIDE_PM1Z_S8, +-1 weights), out = pm1z_gpu_epilogue(s, mean[f], bias[f]): the
+//       XNOR layers below 32 channels of the GPU XNOR rule that the s8 wgmma tile does not take.  Out-of-image taps read 0.
 // The integer inputs are written by k_int_input or by the fused kernels in front of the convolution.
 // ------------------------------------------------------------------------------------------------------
 struct SimtP {
@@ -415,6 +419,18 @@ struct SimtInt8 : SimtWords<int8_t, 0u> {
 struct SimtInt8Gpu : SimtInt8 {
     static __device__ __forceinline__ float finish(const SimtP &p, int acc, int f, const float *) {
         return int8_gpu_epilogue(acc, p.alpha1, p.bias[f], p.act);
+    }
+};
+
+struct SimtXnorGpu : SimtXnor {
+    static __device__ __forceinline__ float finish(const SimtP &p, int acc, int f, const float *) {
+        return xnor_gpu_epilogue(2 * raw(p, acc) - p.bits, p.mean[f], p.bias[f], p.act);
+    }
+};
+
+struct SimtPm1zGpu : SimtInt8 {
+    static __device__ __forceinline__ float finish(const SimtP &p, int acc, int f, const float *) {
+        return pm1z_gpu_epilogue(acc, p.mean[f], p.bias[f], p.act);
     }
 };
 
@@ -603,9 +619,10 @@ struct XnorP {                // the small-K XNOR convolutions, 3x3 / stride 1 /
 // per POOLED pixel computes the four popcount outputs of its window for every filter, takes the reference's max (max-pool
 // semantics: elements outside the image are skipped) and writes only the sign the next layer would have extracted, in its side
 // format F: SIDE_PM1_S8 (next layer runs as +-1 on the s8 wgmma) or SIDE_BITS (next layer on the popcount kernels).  The f32
-// activation and the pooled f32 tensor are never written.  Bit-identical to conv -> max-pool -> k_int_input.
-template <int CW, SideFmt F>
-__global__ void __launch_bounds__(128) k_conv_xnor_smallk_pool(XnorP p, TV q /* next layer's input */) {
+// activation and the pooled f32 tensor are never written.  Bit-identical to conv -> max-pool -> k_int_input.  GPU: the epilogue of
+// the GPU XNOR rule (xnor_gpu_epilogue, k_conv_xnor_smallk_pool_gpu), else the CPU build's (xnor_epilogue).
+template <int CW, SideFmt F, bool GPU>
+__device__ __forceinline__ void xnor_smallk_pool(const XnorP &p, const TV &q) {
     extern __shared__ uint32_t wsm[];            // [n][9*CW]
     constexpr int KW = 9 * CW;
     for (int i = threadIdx.x; i < p.n * KW; i += blockDim.x) wsm[i] = p.w[i];
@@ -636,7 +653,8 @@ __global__ void __launch_bounds__(128) k_conv_xnor_smallk_pool(XnorP p, TV q /* 
             for (int t = 0; t < 9; ++t)
 #pragma unroll
                 for (int c = 0; c < CW; ++c) cnt += __popc(~(a[((t / 3 + dy) * 4 + t % 3 + dx) * CW + c] ^ wf[t * CW + c]));
-            const float v = xnor_epilogue(2 * (cnt - p.padbits) - p.K, p.mean[f], p.bias[f], p.act);
+            const int dot = 2 * (cnt - p.padbits) - p.K;
+            const float v = GPU ? xnor_gpu_epilogue(dot, p.mean[f], p.bias[f], p.act) : xnor_epilogue(dot, p.mean[f], p.bias[f], p.act);
             mx = v > mx ? v : mx;
         }
         // one store per word (+-1 bytes: the filter count of an XNOR layer feeding the tensor-core path is a multiple of 16)
@@ -648,9 +666,10 @@ __global__ void __launch_bounds__(128) k_conv_xnor_smallk_pool(XnorP p, TV q /* 
 
 // XNOR convolution for small K (one or two words per tap): one thread per output pixel keeps its 9 x CW input
 // words in registers and walks all filters, whose sign words sit in shared memory (broadcast reads).  Whole groups of 4
-// filters are stored as one float4: the output must be a vec4_view (16-byte aligned pixels), which the layer plan checks.
-template <int CW>
-__global__ void __launch_bounds__(128) k_conv_xnor_smallk(XnorP p) {
+// filters are stored as one float4: the output must be a vec4_view (16-byte aligned pixels), which the layer plan checks.  GPU:
+// as in xnor_smallk_pool.
+template <int CW, bool GPU>
+__device__ __forceinline__ void xnor_smallk(const XnorP &p) {
     extern __shared__ uint32_t wsm[];            // [n][9*CW]
     constexpr int KW = 9 * CW;
     for (int i = threadIdx.x; i < p.n * KW; i += blockDim.x) wsm[i] = p.w[i];
@@ -682,12 +701,22 @@ __global__ void __launch_bounds__(128) k_conv_xnor_smallk(XnorP p) {
             }
             const int count = cnt - p.padbits;
             if (p.counts && f < p.n) p.counts[(((size_t)n * p.n + f) * H + y) * W + x] = count;
-            r[j] = xnor_epilogue(2 * count - p.K, (f < p.n) ? p.mean[f] : 0.f, (f < p.n) ? p.bias[f] : 0.f, p.act);
+            const float mean = (f < p.n) ? p.mean[f] : 0.f, bias = (f < p.n) ? p.bias[f] : 0.f;
+            r[j] = GPU ? xnor_gpu_epilogue(2 * count - p.K, mean, bias, p.act) : xnor_epilogue(2 * count - p.K, mean, bias, p.act);
         }
         if (f0 + 3 < p.n) *reinterpret_cast<float4 *>(o + f0) = make_float4(r[0], r[1], r[2], r[3]);
         else for (int j = 0; j < 4 && f0 + j < p.n; ++j) o[f0 + j] = r[j];
     }
 }
+
+template <int CW>
+__global__ void __launch_bounds__(128) k_conv_xnor_smallk(XnorP p) { xnor_smallk<CW, false>(p); }
+template <int CW>
+__global__ void __launch_bounds__(128) k_conv_xnor_smallk_gpu(XnorP p) { xnor_smallk<CW, true>(p); }
+template <int CW, SideFmt F>
+__global__ void __launch_bounds__(128) k_conv_xnor_smallk_pool(XnorP p, TV q /* next layer's input */) { xnor_smallk_pool<CW, F, false>(p, q); }
+template <int CW, SideFmt F>
+__global__ void __launch_bounds__(128) k_conv_xnor_smallk_pool_gpu(XnorP p, TV q) { xnor_smallk_pool<CW, F, true>(p, q); }
 
 // ------------------------------------------------------------------------------------------------------
 // small layers (one thread per output element, channels innermost -> coalesced)

@@ -46,6 +46,7 @@ struct Network {
     std::vector<Layer> layers;
     int device = 0;
     int precision = YB_PREC_BF16_TC;
+    int xnor_rule = YB_XNOR_CPU;   // see EngineOptions
     std::shared_ptr<Engine> engine[3];   // by INT8 rule: [YB_QUANT_NONE], [YB_QUANT_CPU], [YB_QUANT_GPU]
     int last_launches = 0;
     bool fuse = true;          // conv+shortcut fusion / route aliasing (diagnostic switch)
