@@ -1,11 +1,11 @@
 """The GPU build's INT8 mode (YB_QUANT_GPU = 2, network_predict_gpu_cudnn_quantized) on the H100: the INT8 layers are the
 parser's l.quantized, with the saturating input conversion and the unscaled epilogue; everything else as in the float forward
-with f32 activations.  Checked bit for bit against the oracle's run_network_gpu (tests/gpu_rule_oracle.py) at YB_PREC_FP32, and against the
+with f32 activations.  Checked bit for bit against the oracle's forward under the GPU rule (tests/rule_oracle.py) at YB_PREC_FP32, and against the
 oracle's INT8 convolution on the engine's own inputs at the default precision, where the float layers run on tf32.  GPU box only."""
 import numpy as np
 import pytest
 
-import gpu_rule_oracle as gro
+import rule_oracle as ro
 import ybtest_util as util
 from yolo2_light_b200 import cfgs
 
@@ -46,7 +46,7 @@ def test_yolov3_tiny_416_fp32_bit_exact(tiny416):
     assert _int8_layers(net) == [2, 4, 6, 8, 10, 12]
     net.predict(x, quantized=Q)
     layers = net.layers
-    outs = gro.run_network_gpu(layers, x)
+    outs = ro.forward(layers, x, Q)
     for i in _int8_layers(net):
         _, acc = util.oracle_layer(layers[i], i, outs[i - 1], Q)
         assert np.array_equal(net.fetch_counts(i, quantized=Q), acc), i
@@ -122,12 +122,12 @@ def test_edges_bit_exact(mode, edge_net, monkeypatch):
     assert _int8_layers(net) == [1, 2, 4, 5]
     net.predict(x, quantized=Q)
     layers = net.layers
-    outs = gro.run_network_gpu(layers, x)
+    outs = ro.forward(layers, x, Q)
     _assert_bit_exact(net, outs, need=(1, 5))
     # some inputs of the INT8 layers convert differently under the two rules: the saturating conversion ran
     differ = [i for i in _int8_layers(net)
               if not np.array_equal(port.quantize_input(outs[i - 1], layers[i]["input_quant_multipler"]),
-                                    gro.quantize_input_gpu(outs[i - 1], layers[i]["input_quant_multipler"]))]
+                                    ro.quantize_input_gpu(outs[i - 1], layers[i]["input_quant_multipler"]))]
     assert differ == _int8_layers(net), differ
     ops = [(li, k) for li, k, _ in net.profile(quantized=Q)]
     names = {li: nm for li, _, nm in net.op_kernels(quantized=Q)}
@@ -199,7 +199,7 @@ def test_true_dropin_gpu_rule_behind_reference_host_code(workdir):
     mine = util.load(cfg, wts, 1, quantized=1)
     assert [i for i, L in enumerate(rnet.layers) if L["type_name"] == "CONVOLUTIONAL" and L["quantized"]] == _int8_layers(mine)
     got = rnet.predict_b200_batch(x, 1)
-    outs = gro.run_network_gpu(mine.layers, x)
+    outs = ro.forward(mine.layers, x, Q)
     err = util.rel_l2(got, outs[-1].reshape(got.shape))
     assert err <= 1e-3, err
     # the CPU rule on the same layers is farther away than that: the GPU rule ran
@@ -219,7 +219,7 @@ def test_yolov3_608_batch2(tmp_path_factory):
     assert len(q) == 26 and q[0] == 1 and max(q) == 78
     exact.predict(x, quantized=Q)
     ref_out = exact.detection_outputs()
-    outs = gro.run_network_gpu(exact.layers, x)
+    outs = ro.forward(exact.layers, x, Q)
     for i, o in ref_out.items():
         assert util.bits_equal(o, outs[i].reshape(o.shape)), i
     fast = util.load(cfg, wts, 2, quantized=1)

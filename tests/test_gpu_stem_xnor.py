@@ -30,7 +30,7 @@ from yolo2_light_b200 import cfgs
 LINEAR, LEAKY, RELU, LOGISTIC = "linear", "leaky", "relu", "logistic"
 XNOR = {"xnor": 1, "bin_output": 1}
 ACT_CODE = {LEAKY: 7, LINEAR: 3}                                # the ACT_* template argument of k_stem_pool
-SMALLK_SMEM = 40 * 1024                                         # conv_path: n * 9 * CW * 4 bytes of sign words at most
+SMALLK_SMEM = 40 * 1024                                         # conv_kern: n * 9 * CW * 4 bytes of sign words at most
 
 
 # ---- kernel names -------------------------------------------------------------------------------------------------------
@@ -77,6 +77,7 @@ class Case:
     """A network on a 3-channel input, the engine's settings, and what it must run and compute:
     kernels  layer -> the one instantiation of a TRACKED kernel that runs it (layer -1: the input conversion); no other
              TRACKED kernel may run
+    inputs   layer -> the side format of the one k_int_input op that converts its input
     no_ops   layers with no op of their own (fused into the op in front)
     hidden   layers whose output no op writes: fetch_layer raises
     tc       layer -> its tensor-core plan's kernel
@@ -89,7 +90,7 @@ class Case:
         self.net = Net(3, h, w, batch, seed, calib=[16] * 8 if quantized else None)
         self.q = quantized
         self.fuse, self.keep_counts, self.env = 1, False, {}
-        self.kernels, self.no_ops, self.hidden, self.tc, self.chains, self.checked = {}, [], [], {}, [], []
+        self.kernels, self.inputs, self.no_ops, self.hidden, self.tc, self.chains, self.checked = {}, {}, [], [], {}, [], []
 
     h = property(lambda self: self.net.h)
     w = property(lambda self: self.net.w)
@@ -262,6 +263,20 @@ def c_slice_xnor(coff, h, w, batch):
     return c
 
 
+def c_slice_xnor_input(coff, h, w, batch):
+    """(g) XNOR layer 2 (C = 16, a shape the s8 tile takes) reads layer 1, the channel slice at coff of route 3's buffer: the
+    tile needs a 16-byte aligned input, so at coff = 6 the layer takes sign bits on k_conv_xnor_smallk"""
+    c = Case("slice", h, w, batch, "int", 2900 + coff + h * w)
+    c.conv(coff, 3, LEAKY)                        # 0: first slice of route 3
+    c.conv(16, 3, LEAKY)                          # 1: second slice, at channel coff
+    c.conv(16, 3, LEAKY, **XNOR)                  # 2
+    c.net.add("route", layers="0, 1")             # 3
+    c.kernels.update({-1: nchw("f32"), 0: SIMT_F32, 1: SIMT_F32, 2: smallk(1)})
+    c.inputs[2] = "SIDE_BITS"
+    c.chains = [(0, 0), (1, 1), (2, 2), (3, 3)]
+    return c
+
+
 def c_slice_stem(coff, dt, h, w, batch, stem_tc=True):
     """(g) the stem (16 filters) writes channels coff.. of route 2's buffer, behind layer 1's coff channels: unless the slice
     is 16-byte aligned, the stem runs as a plain convolution behind the input conversion.  bf16 on grid data, layer 1 a
@@ -331,6 +346,7 @@ CASES = {
     # (g) route slices
     "slice_xnor_at6_13x11": lambda: c_slice_xnor(6, 13, 11, 3),
     "slice_xnor_at4_11x13_b1": lambda: c_slice_xnor(4, 11, 13, 1),
+    "slice_xnor_input_at6_13x11": lambda: c_slice_xnor_input(6, 13, 11, 3),
     "slice_stem_at6_f32_13x11": lambda: c_slice_stem(6, "f32", 13, 11, 3),
     "slice_stem_at8_f32_11x15_b1": lambda: c_slice_stem(8, "f32", 11, 15, 1),
     "slice_stem_at6_bf16_13x11": lambda: c_slice_stem(6, "bf16", 13, 11, 3),
@@ -487,6 +503,9 @@ def test_stem_xnor(name, workdir, monkeypatch):
         if k is not None and any(b in k for b in TRACKED) and kernel_inst(k)[0] in TRACKED:
             ran.setdefault(j, []).append(kernel_inst(k))
     assert ran == {j: [k] for j, k in case.kernels.items()}, (name, ran)
+    for j, side in case.inputs.items():
+        conv = [kernel_inst(k) for jj, _, k in ops if jj == j and util.kernel_is(k, "k_int_input")]
+        assert conv == [inst("k_int_input", side)], (name, j, conv)
     for j in case.no_ops:
         assert not [op for op in ops if op[0] == j], (name, j, ops)
     for j, kern in case.tc.items():

@@ -555,7 +555,7 @@ INT_SHAPES = [   # kind, C, n, h, w, stride, batch: padded channels (C % 32 != 0
 @pytest.mark.parametrize("kind,C,n,h,w,stride,batch", INT_SHAPES)
 def test_integer_kinds_exact(kind, C, n, h, w, stride, batch, workdir):
     """s8_gpu: also with input multipliers of 2^20, where the GPU rule's conversion saturates at +-127"""
-    import gpu_rule_oracle as gro
+    import rule_oracle as ro
     q = RULE_OF[kind]
     for calib in (16, 2 ** 20) if q == 2 else (16,):
         secs = _int_secs(C, h, w, q, calib)
@@ -569,7 +569,7 @@ def test_integer_kinds_exact(kind, C, n, h, w, stride, batch, workdir):
         m.predict(cfgs.synthetic_images(batch, 3, h, w, seed=C), quantized=q)
         x = m.fetch_layer(0, quantized=q)
         if calib != 16:
-            xq = gro.quantize_input_gpu(x, m.layers[1]["input_quant_multipler"])
+            xq = ro.quantize_input_gpu(x, m.layers[1]["input_quant_multipler"])
             assert np.any(xq == 127) and np.any(xq == -127), (x.min(), x.max())
         exp, acc = util.oracle_layer(m.layers[1], 1, x, q)
         assert np.array_equal(m.fetch_counts(1, quantized=q), acc)

@@ -1,10 +1,10 @@
 """The GPU build's XNOR arithmetic (YB_XNOR_GPU) on the H100: path A (the bit GEMM's FMA epilogue and folded shortcut, every
 geometry at c % 32 == 0) and path B (zero-padded +-1 layers below 32 channels), checked bit for bit against the restatement
-in tests/gpu_xnor_oracle.py, per layer and on the final tensors.  GPU box only."""
+in tests/rule_oracle.py, per layer and on the final tensors.  GPU box only."""
 import numpy as np
 import pytest
 
-import gpu_xnor_oracle as gxo
+import rule_oracle as ro
 import ybtest_util as util
 from yolo2_light_b200 import cfgs
 
@@ -77,8 +77,9 @@ def test_edges_bit_exact(mode, edge_net, monkeypatch):
     assert net.get_info("xnor_rule") == yb.YB_XNOR_GPU
     net.predict(x)
     layers = net.layers
-    assert gxo.xnor_paths(layers) == {2: "B", 4: "B", 5: "A", 7: "A", 8: "A", 9: "A", 11: "A", 12: "A", 13: "A"}
-    outs = gxo.run_network_xnor_gpu(layers, x)
+    A, B = "xnor_gpu", "pm1z_gpu"
+    assert util.xnor_gpu_layers(layers) == {2: B, 4: B, 5: A, 7: A, 8: A, 9: A, 11: A, 12: A, 13: A}
+    outs = ro.forward(layers, x, 0, ro.XNOR_GPU)
     got = _check(net, outs, 0)
     assert {2, 4, 9, 10, 11, 12, 13} <= set(got)
     # the GPU build's arithmetic, not the CPU build's
@@ -100,16 +101,16 @@ def test_edges_default_precision_and_counts(edge_net):
     net = _load(cfg, wts, 2, fuse=0, keep_counts=True)
     net.predict(x)
     layers = net.layers
-    outs = gxo.run_network_xnor_gpu(layers, x)
+    outs = ro.forward(layers, x, 0, ro.XNOR_GPU)
     _check(net, outs, 0, upto=14)
     for i, o in net.detection_outputs().items():
         assert util.rel_l2(o, outs[i].reshape(o.shape)) <= 1e-3, i
-    for i, path in gxo.xnor_paths(layers).items():
-        fn = gxo.bin_dot if path == "A" else gxo.pm1z_sum
+    for i, arith in util.xnor_gpu_layers(layers).items():
+        fn = ro.bin_dot if arith == "xnor_gpu" else ro.pm1z_sum
         L = layers[i]
         raw = fn(outs[i - 1], L["weights"], L["n"], L["size"], L["stride"], L["pad"])
         cnt = net.fetch_counts(i)
-        assert np.array_equal(cnt, (raw + L["size"] ** 2 * L["c"]) // 2 if path == "A" else raw), i
+        assert np.array_equal(cnt, (raw + L["size"] ** 2 * L["c"]) // 2 if arith == "xnor_gpu" else raw), i
 
 
 @pytest.mark.parametrize("precision", ["fp32", "default"])
@@ -121,9 +122,9 @@ def test_gpu_int8_rule_with_xnor_layers(precision, edge_net):
     net = _load(cfg, wts, 2, quantized=1, precision=yb.YB_PREC_FP32 if precision == "fp32" else None, fuse=0)
     layers = net.layers
     assert [i for i, L in enumerate(layers) if L["type_name"] == "CONVOLUTIONAL" and L["quantized"]] == [2, 3, 4, 5, 7, 8]
-    assert gxo.xnor_paths(layers, int8_gpu=True) == {9: "A", 11: "A", 12: "A", 13: "A"}
+    assert util.xnor_gpu_layers(layers, quantized=2) == {9: "xnor_gpu", 11: "xnor_gpu", 12: "xnor_gpu", 13: "xnor_gpu"}
     net.predict(x, quantized=2)
-    outs = gxo.run_network_xnor_gpu(layers, x, int8_gpu=True)
+    outs = ro.forward(layers, x, 2, ro.XNOR_GPU)
     _check(net, outs, 2, upto=None if precision == "fp32" else 14)
     with pytest.raises(yb.YbError, match="quantized = 1"):
         net.predict(x, quantized=1)
@@ -138,7 +139,7 @@ def test_xnor64_both_precisions(workdir):
     x = util.images("xnor64", 3)
     exact = _load(cfg, wts, 3, precision=yb.YB_PREC_FP32)
     exact.predict(x)
-    outs = gxo.run_network_xnor_gpu(exact.layers, x)
+    outs = ro.forward(exact.layers, x, 0, ro.XNOR_GPU)
     _check(exact, outs, 0, upto=15)
     region = exact.detection_outputs()[15]
     assert np.allclose(region, outs[15].reshape(region.shape), rtol=2.0 ** -20, atol=0)
@@ -208,7 +209,7 @@ def test_true_dropin_behind_reference_host_code(workdir, monkeypatch):
     got = rnet.predict_b200_batch(x, 1)
     monkeypatch.delenv("YB_XNOR_RULE")
     mine = util.load(cfg, wts, 1)
-    outs = gxo.run_network_xnor_gpu(mine.layers, x)
+    outs = ro.forward(mine.layers, x, 0, ro.XNOR_GPU)
     err = util.rel_l2(got, outs[-1].reshape(got.shape))
     assert err <= 1e-3, err
     cpu = port.run_network(mine.layers, x)

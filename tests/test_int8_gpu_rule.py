@@ -8,7 +8,7 @@ import os
 import numpy as np
 import pytest
 
-import gpu_rule_oracle as gro
+import rule_oracle as ro
 import ybtest_util as util
 
 ASSETS = sorted(glob.glob(os.path.join(util.GOLDEN, "assets", "*.cfg")))
@@ -54,7 +54,7 @@ def test_gpu_input_conversion_edges():
     m = np.float32(8.0)
     v = np.array([126.9, -126.9, 127, -127, 32767.5, -32767.5, 40000, -40000, 2.0 ** 31, -(2.0 ** 31)], np.float64)
     x = np.concatenate([(v / float(m)).astype(np.float32), np.array([np.inf, -np.inf, np.nan, -0.0], np.float32)])
-    got = gro.quantize_input_gpu(x, m)
+    got = ro.quantize_input_gpu(x, m)
     exp = np.array([126, -126, 127, -127, 127, -127, 127, -127, 127, -127, 127, -127, 0, 0], np.int8)
     assert np.array_equal(got, exp), got
     cpu = port.quantize_input(x, m)
@@ -74,10 +74,10 @@ def test_gpu_conv_epilogue_formula():
     mi, mw = np.float32(11.0), np.float32(37.0)
     for stride in (1, 2):
         _, a_cpu = port.conv_int8(x, w, b, mi, mw, 4, 3, stride, 1, 3, want_acc=True)
-        _, a_gpu = gro.conv_int8_gpu(x, w, b, mi, mw, 4, 3, stride, 1, 3, want_acc=True)
+        _, a_gpu = ro.conv_int8_gpu(x, w, b, mi, mw, 4, 3, stride, 1, 3, want_acc=True)
         assert np.array_equal(a_cpu, a_gpu), stride
     for act in (3, 7, 0):
-        y, acc = gro.conv_int8_gpu(x, w, b, mi, mw, 4, 3, 1, 1, act, want_acc=True)
+        y, acc = ro.conv_int8_gpu(x, w, b, mi, mw, 4, 3, 1, 1, act, want_acc=True)
         alpha = np.float32(1) / (mi * mw)
         z = (acc.astype(np.float32) * alpha).astype(np.float32) + b[None, :, None, None]
         if act == 7:
@@ -110,10 +110,10 @@ def test_int8_accumulators_match_reference_gemm(c, h, w, n, size, stride):
     x = rng.normal(0, 0.15, (1, c, h, w)).astype(np.float32) * np.float32(16) / np.float32(m_in)
     x.ravel()[0], x.ravel()[-1] = 1e9 / m_in, -40000 / m_in   # where the two rules' conversions part
     pad = L["pad"]
-    _, acc = gro.conv_int8_gpu(x, wq.reshape(n, c, size, size), np.zeros(n, np.float32), m_in, L["weights_quant_multipler"],
+    _, acc = ro.conv_int8_gpu(x, wq.reshape(n, c, size, size), np.zeros(n, np.float32), m_in, L["weights_quant_multipler"],
                                 n, size, stride, pad, 3, want_acc=True)
     assert np.abs(acc).max() <= 32767
-    xq = gro.quantize_input_gpu(x, m_in)
+    xq = ro.quantize_input_gpu(x, m_in)
     oh, ow = (h + 2 * pad - size) // stride + 1, (w + 2 * pad - size) // stride + 1
     col = np.zeros(K * oh * ow, np.int8)
     out = np.zeros(n * oh * ow, np.int32)

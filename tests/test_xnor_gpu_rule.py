@@ -6,7 +6,7 @@ import os
 import numpy as np
 import pytest
 
-import gpu_xnor_oracle as gxo
+import rule_oracle as ro
 import ybtest_util as util
 from yolo2_light_b200 import cfgs
 
@@ -33,18 +33,19 @@ def _parsed(secs, tmp_path, name):
 
 
 def test_paths_of_tiny_yolo_obj_xnor():
-    """tiny-yolo-obj_xnor: the 16-channel XNOR layer behind the stem's max-pool is path B, the wider ones path A."""
+    """tiny-yolo-obj_xnor: the 16-channel XNOR layer behind the stem's max-pool is path B (pm1z_gpu), the wider ones path A
+    (xnor_gpu)."""
     if util.have_ref():
         from oracle import ref
         layers = ref.RefNet(XNOR_CFG, None, 1, 0, 0).layers
     else:
         import yolo2_light_b200 as yb
         layers = yb.parse_network_cfg(XNOR_CFG, 1, 0).layers
-    paths = gxo.xnor_paths(layers)
+    paths = util.xnor_gpu_layers(layers)
     xnor = [i for i, L in enumerate(layers) if L["type_name"] == "CONVOLUTIONAL" and L["xnor"]]
     assert sorted(paths) == xnor
-    assert {i: p for i, p in paths.items() if p == "B"} == {i: "B" for i in xnor if layers[i]["c"] < 32}
-    assert [paths[i] for i in xnor].count("B") == 1 and layers[xnor[0]]["c"] == 16
+    assert {i: p for i, p in paths.items() if p == "pm1z_gpu"} == {i: "pm1z_gpu" for i in xnor if layers[i]["c"] < 32}
+    assert [paths[i] for i in xnor].count("pm1z_gpu") == 1 and layers[xnor[0]]["c"] == 16
 
 
 @pytest.mark.parametrize("case", ["c48", "sc_pathB", "sc_logistic", "sc_ok", "s2_1x1"])
@@ -57,22 +58,22 @@ def test_paths_and_rejections_of_small_cfgs(case, tmp_path):
     elif case == "sc_logistic":
         secs, want = _secs(cfgs._conv(32, 3), _xconv(32, act="logistic"), sc), "non-leaky"
     elif case == "sc_ok":
-        secs, want = _secs(cfgs._conv(32, 3), _xconv(32), sc), {1: "A"}
+        secs, want = _secs(cfgs._conv(32, 3), _xconv(32), sc), {1: "xnor_gpu"}
     else:
-        secs, want = _secs(cfgs._conv(32, 3), _xconv(64, 3, 2), _xconv(64, 1), _xconv(8, 3)), {1: "A", 2: "A", 3: "A"}
+        secs, want = _secs(cfgs._conv(32, 3), _xconv(64, 3, 2), _xconv(64, 1), _xconv(8, 3)), {1: "xnor_gpu", 2: "xnor_gpu", 3: "xnor_gpu"}
     layers = _parsed(secs, tmp_path, case)
     if isinstance(want, dict):
-        assert gxo.xnor_paths(layers) == want
+        assert util.xnor_gpu_layers(layers) == want
     else:
-        with pytest.raises(gxo.Rejected, match=want):
-            gxo.xnor_paths(layers)
+        with pytest.raises(ro.Rejected, match=want):
+            util.xnor_gpu_layers(layers)
 
 
 def test_int8_layers_of_the_gpu_int8_rule_keep_no_xnor_path():
     layers = [dict(type_name="CONVOLUTIONAL", xnor=1, quantized=1, c=32, activation=7),
               dict(type_name="CONVOLUTIONAL", xnor=1, quantized=0, c=32, activation=7)]
-    assert gxo.xnor_paths(layers, int8_gpu=True) == {1: "A"}
-    assert gxo.xnor_paths(layers) == {0: "A", 1: "A"}
+    assert util.xnor_gpu_layers(layers, quantized=2) == {1: "xnor_gpu"}
+    assert util.xnor_gpu_layers(layers) == {0: "xnor_gpu", 1: "xnor_gpu"}
 
 
 def test_fmaf_is_correctly_rounded():
@@ -82,19 +83,19 @@ def test_fmaf_is_correctly_rounded():
     a = rng.integers(-4000, 4000, 3000).astype(F32)
     b = rng.uniform(0.001, 2, 3000).astype(F32)
     c = rng.normal(0, 50, 3000).astype(F32)
-    got = gxo.fmaf_f32(a, b, c)
-    exp = np.array([gxo.fmaf_exact(*t) for t in zip(a, b, c)], F32)
+    got = ro.fmaf_f32(a, b, c)
+    exp = np.array([ro.fmaf_exact(*t) for t in zip(a, b, c)], F32)
     assert util.bits_equal(got, exp)
     two = ((a * b).astype(F32) + c).astype(F32)
     assert not util.bits_equal(got, two)
     # dot * mean lands between two float32 values next to 1.0: the separately rounded product loses what fmaf keeps
     m = F32(1.0) + F32(2.0 ** -23)
     a2, b2, c2 = F32(3.0), m, F32(-3.0)
-    assert gxo.fmaf_f32(a2, b2, c2) == gxo.fmaf_exact(a2, b2, c2) == F32(3 * 2.0 ** -23)
+    assert ro.fmaf_f32(a2, b2, c2) == ro.fmaf_exact(a2, b2, c2) == F32(3 * 2.0 ** -23)
     assert F32(F32(a2 * b2) + c2) != F32(3 * 2.0 ** -23)
     # a tie of the double sum decided by the TwoSum error
     a3, b3, c3 = F32(1.0), F32(1.0 + 2.0 ** -23), F32(2.0 ** -24 + 2.0 ** -48)
-    assert gxo.fmaf_f32(a3, b3, c3) == gxo.fmaf_exact(a3, b3, c3)
+    assert ro.fmaf_f32(a3, b3, c3) == ro.fmaf_exact(a3, b3, c3)
 
 
 def test_epilogue_edges():
@@ -102,19 +103,19 @@ def test_epilogue_edges():
     while path A's bit is x > 0."""
     from oracle import port
     y = np.array([-0.0, 0.0, -1e-30, -3.3333333, 7.0], F32)
-    got = gxo.act_gpu(y, port.LEAKY)
+    got = ro.act_gpu(y, port.LEAKY)
     assert got[0] == 0 and np.signbit(got[0]) and not np.signbit(got[1])
     assert got[3] == F32(0.1) * F32(-3.3333333)
     v = np.arange(1, 20000, dtype=F32) * F32(-0.37)
-    assert not util.bits_equal(gxo.act_gpu(v, port.LEAKY), (0.1 * v.astype(np.float64)).astype(F32))
+    assert not util.bits_equal(ro.act_gpu(v, port.LEAKY), (0.1 * v.astype(np.float64)).astype(F32))
     x = np.array([[[[0.0, -0.0, 1.0, -1.0]]]], F32)
     w = np.ones(1, F32)
-    assert gxo.pm1z_sum(x, w, 1, 1, 1, 0).ravel().tolist() == [1, 1, 1, -1]
-    assert gxo.bin_dot(x, w, 1, 1, 1, 0).ravel().tolist() == [-1, -1, 1, -1]
+    assert ro.pm1z_sum(x, w, 1, 1, 1, 0).ravel().tolist() == [1, 1, 1, -1]
+    assert ro.bin_dot(x, w, 1, 1, 1, 0).ravel().tolist() == [-1, -1, 1, -1]
     # out-of-image taps: -1 on path A, 0 on path B
     ones = np.ones((1, 1, 2, 2), F32)
-    assert gxo.bin_dot(ones, np.ones(9, F32), 1, 3, 1, 1).ravel().tolist() == [-1] * 4
-    assert gxo.pm1z_sum(ones, np.ones(9, F32), 1, 3, 1, 1).ravel().tolist() == [4] * 4
+    assert ro.bin_dot(ones, np.ones(9, F32), 1, 3, 1, 1).ravel().tolist() == [-1] * 4
+    assert ro.pm1z_sum(ones, np.ones(9, F32), 1, 3, 1, 1).ravel().tolist() == [4] * 4
 
 
 @pytest.mark.parametrize("c", [32, 64])
@@ -128,7 +129,7 @@ def test_path_a_dot_is_the_cpu_oracles(c):
     x[0, 0, 0, :3] = 0.0
     L = dict(n=n, size=3, stride=1, pad=1, activation=port.LINEAR, weights=rng.normal(0, 1, n * c * 9).astype(F32),
              biases=rng.normal(0, 1, n).astype(F32), mean_arr=rng.uniform(0.01, 1, n).astype(F32))
-    y, dot = gxo.conv_xnor_a(x, L, want_raw=True)
+    y, dot = ro.conv_xnor_a(x, L, want_raw=True)
     cpu, counts = port.conv_xnor(x, L["weights"], L["biases"], L["mean_arr"], n, 3, port.LINEAR, want_counts=True)
     assert np.array_equal(dot, 2 * counts - c * 9)
     # one rounding of the product apart: within an ulp of its magnitude

@@ -178,11 +178,12 @@ def profile_kinds(net, quantized=False):
 
 
 # ---- the oracle ---------------------------------------------------------------------------------------------------------
-def oracle_layer(L, i, x, rule, frm=None):
+def oracle_layer(L, i, x, rule, frm=None, xnor_rule=0):
     """Layer i (layer dict L) of the oracle on its input x (frm: a shortcut's `from` output), under the integer rule of
-    `quantized` = rule: 1 the CPU rule (port.run_network), 2 the GPU rule (gpu_rule_oracle).  Returns (output, the raw XNOR
-    popcounts or INT8 accumulators, or None)."""
+    `quantized` = rule (0 none, 1 the CPU rule, 2 the GPU rule) and the XNOR rule (rule_oracle.conv_arith).  Returns (output,
+    the raw XNOR results or INT8 accumulators, or None)."""
     from oracle import port
+    import rule_oracle
     t = L["type_name"]
     if t == "MAXPOOL":
         return port.maxpool(x, L["size"], L["stride"], L["pad"]), None
@@ -193,23 +194,24 @@ def oracle_layer(L, i, x, rule, frm=None):
     if t == "SHORTCUT":
         return port.shortcut(x, frm, L["activation"]), None
     assert t == "CONVOLUTIONAL", t
-    if rule == 2 and L["quantized"]:
-        import gpu_rule_oracle as gro
-        return gro.conv_int8_gpu(x, L["weights_int8"], L["biases"], L["input_quant_multipler"], L["weights_quant_multipler"],
-                                 L["n"], L["size"], L["stride"], L["pad"], L["activation"], want_acc=True)
-    if rule == 1 and i >= 1 and L["activation"] != port.LINEAR:
-        return port.conv_int8(x, L["weights_int8"], L["biases"], L["input_quant_multipler"], L["weights_quant_multipler"],
-                              L["n"], L["size"], L["stride"], L["pad"], L["activation"], want_acc=True)
-    if L["xnor"]:
-        return port.conv_xnor(x, L["weights"], L["biases"], L["mean_arr"], L["n"], L["size"], L["activation"], want_counts=True)
-    return port.conv_fp32(x, L["weights"], L["biases"], L["n"], L["size"], L["stride"], L["pad"], L["activation"]), None
+    layers = [None] * i + [L]    # conv_arith looks at layer i and the one behind it, which a lone layer does not have
+    return rule_oracle.conv(L, rule_oracle.conv_arith(layers, i, rule, xnor_rule), x, want_raw=True)
 
 
-def oracle_outs(net, x, rule):
-    """every layer's output of the oracle (port.run_network, rule 0 or 1), image by image, concatenated over the batch"""
-    from oracle import port
-    per_image = [port.run_network(net.layers, x[b:b + 1], quantized=bool(rule)) for b in range(x.shape[0])]
+def oracle_outs(net, x, rule, xnor_rule=0):
+    """every layer's output of the oracle (rule_oracle.forward), image by image, concatenated over the batch"""
+    import rule_oracle
+    per_image = [rule_oracle.forward(net.layers, x[b:b + 1], rule, xnor_rule) for b in range(x.shape[0])]
     return [np.concatenate([pi[i] for pi in per_image], axis=0) for i in range(net.n)]
+
+
+def xnor_gpu_layers(layers, quantized=0):
+    """convolution -> its arithmetic under the GPU XNOR rule, for the XNOR layers that run as XNOR (not as INT8 under the
+    GPU INT8 rule, quantized = 2); raises rule_oracle.Rejected where the engine refuses the network"""
+    import rule_oracle
+    ar = {i: rule_oracle.conv_arith(layers, i, quantized, rule_oracle.XNOR_GPU)
+          for i, L in enumerate(layers) if L["type_name"] == "CONVOLUTIONAL"}
+    return {i: a for i, a in ar.items() if a in ("xnor_gpu", "pm1z_gpu")}
 
 
 # ---- kernel names -------------------------------------------------------------------------------------------------------
