@@ -222,7 +222,7 @@ __device__ __forceinline__ void wg_fence_operand(T (&d)[N]) {
 }
 
 // One M=64 x N x (32 bytes of K) wgmma per call; d: this thread's accumulator fragment (N/2 values).  scale_d == 0 overwrites.
-// TC_BF16: bf16 -> f32, TC_S8 (and TC_XNOR): s8 -> s32, TC_TF32: tf32 -> f32.
+// TC_BF16: bf16 -> f32, TC_S8 (every integer kind): s8 -> s32, TC_TF32: tf32 -> f32.
 template <TcKind KIND, int N> struct Wg;
 template <> struct Wg<TC_BF16, 32> {
     static __device__ __forceinline__ void mma(float (&d)[16], uint64_t a, uint64_t b, uint32_t scale_d) {
@@ -324,7 +324,6 @@ template <> struct Wg<TC_TF32, 128> {
             : "l"(a), "l"(b), "r"(scale_d) : "memory");
     }
 };
-template <int N> struct Wg<TC_XNOR, N> : Wg<TC_S8, N> {};
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
     __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
@@ -535,16 +534,11 @@ __device__ __forceinline__ void tc_mma_loop(T (&d)[BN / 2], const TcParams &p, u
     if (pend >= 0) release(pend);
 }
 
-// The reference's float epilogue of the integer kinds (bit-exact): TC_S8 int8_epilogue; TC_S8_GPU int8_gpu_epilogue; TC_XNOR
-// xnor_epilogue and TC_XNOR_GPU xnor_gpu_epilogue, where the s8 wgmma's acc is dot = 2*count - K exactly; TC_PM1Z_GPU
-// pm1z_gpu_epilogue, where acc is the zero-padded +-1 sum.  f: filter index (the XNOR kinds read its mean |w|).
-__device__ __forceinline__ float int_epilogue(const TcParams &p, int kind, int acc, int f, float bias) {
-    if (kind == TC_S8) return int8_epilogue(acc, p.alpha1, bias, p.act);
-    if (kind == TC_S8_GPU) return int8_gpu_epilogue(acc, p.alpha1, bias, p.act);
-    const float mean = (f < p.n) ? __ldg(p.mean + f) : 0.f;
-    if (kind == TC_XNOR_GPU) return xnor_gpu_epilogue(acc, mean, bias, p.act);
-    if (kind == TC_PM1Z_GPU) return pm1z_gpu_epilogue(acc, mean, bias, p.act);
-    return xnor_epilogue(acc, mean, bias, p.act);
+// The reference's float epilogue of integer arithmetic A (bit-exact) on the s8 wgmma's accumulator, which is A's signed result
+// (IntEpi).  f: filter index (the XNOR arithmetics read its mean |w|).
+template <Arith A>
+__device__ __forceinline__ float int_epilogue(const TcParams &p, int acc, int f, float bias) {
+    return IntEpi<A>::finish(acc, IntEpi<A>::MEAN ? ((f < p.n) ? __ldg(p.mean + f) : 0.f) : p.alpha1, bias, p.act);
 }
 
 // One CTA per 128-pixel x BN-filter tile, persistent over the tiles (grid <= #SMs, one CTA per SM).
@@ -608,7 +602,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                 constexpr TcKind KIND = decltype(kind_c)::value;
                 constexpr int BN = decltype(bn_c)::value;
                 constexpr int KK = decltype(kk_c)::value;   // wgmmas per K-block
-                using T = typename std::conditional<KIND == TC_S8 || KIND == TC_XNOR, uint32_t, float>::type;
+                using T = typename std::conditional<KIND == TC_S8, uint32_t, float>::type;
                 T d[BN / 2];
                 tc_mma_loop<KIND, BN, KK, ST>(d, p, base, wg, lane, ring, w_full);
                 named_bar_sync(TC_ACC_BAR, 32 * TC_EPI_WARPS);   // every warp is done with the previous tile's accumulators
@@ -726,7 +720,8 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
             // pixels wide).  The reduction is a reduce-scatter: lane^1 halves the 32 columns, lane^8 halves them again, every lane
             // ends up with the maxima of 8 columns of its window and finishes those -- a quarter of the float work per lane.
             // Elements outside the image count as "skipped" (INT_MIN) like the reference's out-of-range taps (additionally.c:1448-1482).
-            auto pool_store_raw = [&](const uint32_t (&v)[32], int f0) {
+            auto pool_store_raw = [&](auto arith_c, const uint32_t (&v)[32], int f0) {
+                constexpr Arith A = decltype(arith_c)::value;
                 const bool b0 = lane & 1, b3 = lane & 8;
                 int h16[16], h8[8];
 #pragma unroll
@@ -747,7 +742,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
                     const int f = n0 + cbase + j;
-                    const float t = int_epilogue(p, p.kind, h8[j], f, bs[cbase + j]);
+                    const float t = int_epilogue<A>(p, h8[j], f, bs[cbase + j]);
                     uint32_t b8 = (p.pool_fmt == SIDE_S8) ? side_code<SIDE_S8>(t, p.pool_mult)
                                 : (p.pool_fmt == SIDE_S8_SAT) ? side_code<SIDE_S8_SAT>(t, p.pool_mult) : side_code<SIDE_PM1_S8>(t, 0.f);
                     if (f >= p.n) b8 = 0;
@@ -787,34 +782,32 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
             };
 
             if constexpr (EPI == 2) {
-                // ---- integer kinds: the exact float epilogue per 32-column slab (or the fused max-pool), f32 stores
-                auto int_slabs = [&](auto kind_c) {
-                    constexpr TcKind KIND = decltype(kind_c)::value;
+                // ---- integer kinds: the exact float epilogue of the kind's arithmetic per 32-column slab (or the fused max-pool),
+                // f32 stores
+                auto int_slabs = [&](auto arith_c) {
+                    constexpr Arith A = decltype(arith_c)::value;
                     for (int f0 = cbeg; f0 < cend; f0 += 32) {
                         uint32_t v0[32];
                         acc_ld32(taddr + 4u * (uint32_t)f0, v0);
-                        if (p.pool_fmt != SIDE_NONE) { pool_store_raw(v0, f0); continue; }
+                        if (p.pool_fmt != SIDE_NONE) { pool_store_raw(arith_c, v0, f0); continue; }
                         float y[32];
 #pragma unroll
-                        for (int j = 0; j < 32; ++j) y[j] = int_epilogue(p, KIND, (int)v0[j], n0 + f0 + j, bs[f0 + j]);
+                        for (int j = 0; j < 32; ++j) y[j] = int_epilogue<A>(p, (int)v0[j], n0 + f0 + j, bs[f0 + j]);
                         if (p.tma_epi) tma_store_f32_slab(y, f0);
                         else store_f32_slab(y, f0);
                         if (!valid || !p.acc_out) continue;
 #pragma unroll
                         for (int j = 0; j < 32; ++j) {
                             const int f = n0 + f0 + j;
-                            // raw results: the INT8 accumulator; XNOR: the reference's popcount, (dot + K) / 2
-                            if (f < p.n)
-                                p.acc_out[(((size_t)img * p.n + f) * p.OH + oy) * p.OW + ox] =
-                                    (KIND == TC_XNOR || KIND == TC_XNOR_GPU) ? ((int)v0[j] + p.xK) / 2 : (int)v0[j];
+                            if (f < p.n) p.acc_out[(((size_t)img * p.n + f) * p.OH + oy) * p.OW + ox] = IntEpi<A>::raw((int)v0[j], p.xK);
                         }
                     }
                 };
-                if (p.kind == TC_XNOR) int_slabs(std::integral_constant<TcKind, TC_XNOR>{});
-                else if (p.kind == TC_S8_GPU) int_slabs(std::integral_constant<TcKind, TC_S8_GPU>{});
-                else if (p.kind == TC_XNOR_GPU) int_slabs(std::integral_constant<TcKind, TC_XNOR_GPU>{});
-                else if (p.kind == TC_PM1Z_GPU) int_slabs(std::integral_constant<TcKind, TC_PM1Z_GPU>{});
-                else int_slabs(std::integral_constant<TcKind, TC_S8>{});
+                if (p.kind == TC_XNOR) int_slabs(std::integral_constant<Arith, AR_XNOR>{});
+                else if (p.kind == TC_S8_GPU) int_slabs(std::integral_constant<Arith, AR_INT8_GPU>{});
+                else if (p.kind == TC_XNOR_GPU) int_slabs(std::integral_constant<Arith, AR_XNOR_GPU>{});
+                else if (p.kind == TC_PM1Z_GPU) int_slabs(std::integral_constant<Arith, AR_PM1Z_GPU>{});
+                else int_slabs(std::integral_constant<Arith, AR_INT8>{});
             } else {
                 for (int f0 = cbeg; f0 < cend; f0 += 64) {
                     if (cend - f0 >= 64) {

@@ -1,7 +1,8 @@
 // yb_device.cuh -- what the SIMT kernels (yb_kernels.cuh) and the tensor-core kernels (yb_conv_tc.cu) share: the tensor view,
 // the activations, the operand kinds and, defined once, the integer layers' arithmetic -- the conversion of an f32 activation
-// into an integer convolution's input and the reference's float epilogues of the XNOR and INT8 convolutions.  Every kernel
-// that converts or finishes an integer layer calls these, so all of them stay bit-identical to the reference together.
+// into an integer convolution's input and the reference's float epilogues of the XNOR and INT8 convolutions, chosen per
+// arithmetic by IntEpi.  Every kernel that converts or finishes an integer layer calls these, so all of them stay
+// bit-identical to the reference together.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -44,6 +45,18 @@ __device__ __forceinline__ float act_exact(float x, int a) {
     if (a == ACT_RELU) return x * (x > 0.f);
     return x;
 }
+
+// The arithmetic of a convolution, decided once per convolution by the engine's layer plan (Builder::conv_arith).  The five
+// integer ones are defined by IntEpi below.
+enum Arith {
+    AR_F32,            // float convolution
+    AR_XNOR_PM1_F32,   // CPU XNOR rule, stride != 1 or pad != 1: the reference's float-GEMM fallback over +-1 floats
+    AR_XNOR,           // CPU XNOR rule: popcounts, xnor_epilogue
+    AR_XNOR_GPU,       // GPU XNOR rule, c % 32 == 0 (path A): the bit GEMM's count, xnor_gpu_epilogue
+    AR_PM1Z_GPU,       // GPU XNOR rule, c < 32 (path B): zero-padded +-1 convolution, pm1z_gpu_epilogue
+    AR_INT8,           // CPU INT8 rule: s8 quant_i8 inputs, int8_epilogue
+    AR_INT8_GPU,       // GPU INT8 rule: s8 quant_i8_sat inputs, int8_gpu_epilogue
+};
 
 // Operand types of a tensor-core convolution
 enum TcKind {
@@ -191,5 +204,26 @@ __device__ __forceinline__ float xnor_gpu_epilogue(int dot, float mean, float bi
 __device__ __forceinline__ float pm1z_gpu_epilogue(int s, float mean, float bias, int act) {
     return act_gpu(__fadd_rn(__fmul_rn((float)s, mean), bias), act);
 }
+
+// whether arithmetic a's epilogue scales by the filter's mean |w| (the XNOR arithmetics) rather than the layer's ALPHA1 (INT8)
+__host__ __device__ constexpr bool arith_mean(Arith a) { return a == AR_XNOR || a == AR_XNOR_GPU || a == AR_PM1Z_GPU; }
+
+// Integer arithmetic A as every integer kernel finishes it, from its signed integer result r: the s32 accumulator (INT8), dot =
+// 2*count - K (XNOR) or the zero-padded +-1 sum (PM1Z).  The s8 wgmma computes r directly; the popcount kernels form it from
+// their count as 2*(count - padbits) - K.
+template <Arith A>
+struct IntEpi {
+    static_assert(A == AR_XNOR || A == AR_XNOR_GPU || A == AR_PM1Z_GPU || A == AR_INT8 || A == AR_INT8_GPU, "integer arithmetics only");
+    static constexpr bool MEAN = arith_mean(A);   // scale: the filter's mean |w|, else the layer's ALPHA1
+    static __device__ __forceinline__ float finish(int r, float scale, float bias, int act) {
+        if constexpr (A == AR_XNOR) return xnor_epilogue(r, scale, bias, act);
+        else if constexpr (A == AR_XNOR_GPU) return xnor_gpu_epilogue(r, scale, bias, act);
+        else if constexpr (A == AR_PM1Z_GPU) return pm1z_gpu_epilogue(r, scale, bias, act);
+        else if constexpr (A == AR_INT8) return int8_epilogue(r, scale, bias, act);
+        else return int8_gpu_epilogue(r, scale, bias, act);
+    }
+    // the raw result keep_counts stores, K = size*size*C: the reference's popcount (r + K) / 2 for the two XNOR arithmetics
+    static __device__ __forceinline__ int raw(int r, int K) { return A == AR_XNOR || A == AR_XNOR_GPU ? (r + K) / 2 : r; }
+};
 
 }  // namespace yb

@@ -284,15 +284,14 @@ static __global__ void __launch_bounds__(RS_THREADS) k_resize_frames(const Image
 //       yolov2_forward_network.c:204-261), out = act(sum_{c,ky,kx} w*in + bias) with zero padding; optional fused shortcut
 //       (reference :443-449), out = act2(act(..) + residual).  Validation precision (YB_PREC_FP32), the FP32 layers of XNOR /
 //       INT8 networks, the bf16 layers the tensor cores refuse, and the XNOR layers of the float-GEMM fallback.
-//   SimtXnor  words of 32 sign bits (reference yolov2_forward_network.c:116-203): count = sum popc(~(a ^ w)) - (pad bits),
-//       out = xnor_epilogue(2*count - K, mean[f], bias[f]).  XNOR layers off the s8 wgmma with more than 2 words per tap.
-//   SimtInt8  words of 4 s8 values (reference yolov2_forward_network_quantized.c:527-631): acc32 = sum xq*wq (dp4a, exact),
-//       out = int8_epilogue(acc32).  INT8 layers the s8 wgmma tile refuses.
-//   SimtInt8Gpu  the same GEMM, out = int8_gpu_epilogue(acc32): the INT8 layers of the GPU rule the s8 wgmma tile refuses.
-//   SimtXnorGpu  SimtXnor's GEMM, out = xnor_gpu_epilogue(2*count - K, mean[f], bias[f]): the XNOR layers with c % 32 == 0 of
-//       the GPU XNOR rule, of any size, stride and pad, off the s8 wgmma and the small-K kernel.
-//   SimtPm1zGpu  SimtInt8's GEMM over +-1 bytes (SIDE_PM1Z_S8, +-1 weights), out = pm1z_gpu_epilogue(s, mean[f], bias[f]): the
-//       XNOR layers below 32 channels of the GPU XNOR rule that the s8 wgmma tile does not take.  Out-of-image taps read 0.
+//   SimtPopc<A>  words of 32 sign bits (reference yolov2_forward_network.c:116-203): count = sum popc(~(a ^ w)) - (pad bits),
+//       out = IntEpi<A>::finish(2*count - K, mean[f], bias[f]).  SimtXnor (AR_XNOR): the XNOR layers off the s8 wgmma with more
+//       than 2 words per tap; SimtXnorGpu (AR_XNOR_GPU): the XNOR layers with c % 32 == 0 of the GPU XNOR rule, of any size,
+//       stride and pad, off the s8 wgmma and the small-K kernel.
+//   SimtDp4a<A>  words of 4 s8 values: acc32 = sum xq*wq (dp4a, exact), out = IntEpi<A>::finish(acc32, ..).  SimtInt8 (AR_INT8,
+//       reference yolov2_forward_network_quantized.c:527-631) and SimtInt8Gpu (AR_INT8_GPU): the INT8 layers the s8 wgmma tile
+//       refuses; SimtPm1zGpu (AR_PM1Z_GPU), over +-1 bytes (SIDE_PM1Z_S8, +-1 weights): the XNOR layers below 32 channels of the
+//       GPU XNOR rule that the s8 wgmma tile does not take.  Out-of-image taps read 0.
 // The integer inputs are written by k_int_input or by the fused kernels in front of the convolution.
 // ------------------------------------------------------------------------------------------------------
 struct SimtP {
@@ -400,39 +399,35 @@ struct SimtWords {
     }
 };
 
-struct SimtXnor : SimtWords<uint32_t, 0xffffffffu> {   // a ^ b all ones in the tail: xnor counts 0
+// the integer policies' epilogue: IntEpi<A> on the signed result r of filter f
+template <Arith A>
+__device__ __forceinline__ float simt_int_finish(const SimtP &p, int r, int f) {
+    return IntEpi<A>::finish(r, IntEpi<A>::MEAN ? p.mean[f] : p.alpha1, p.bias[f], p.act);
+}
+
+// xor + popc over sign words (AR_XNOR, AR_XNOR_GPU): r = 2*(count - padbits) - bits
+template <Arith A>
+struct SimtPopc : SimtWords<uint32_t, 0xffffffffu> {   // a ^ b all ones in the tail: xnor counts 0
     static __device__ __forceinline__ void mac(int &acc, uint32_t a, uint32_t b) { acc += __popc(~(a ^ b)); }
-    static __device__ __forceinline__ int raw(const SimtP &p, int acc) { return acc - p.padbits; }
-    static __device__ __forceinline__ float finish(const SimtP &p, int acc, int f, const float *) {
-        return xnor_epilogue(2 * raw(p, acc) - p.bits, p.mean[f], p.bias[f], p.act);
-    }
+    static __device__ __forceinline__ int dot(const SimtP &p, int acc) { return 2 * (acc - p.padbits) - p.bits; }
+    static __device__ __forceinline__ int raw(const SimtP &p, int acc) { return IntEpi<A>::raw(dot(p, acc), p.bits); }
+    static __device__ __forceinline__ float finish(const SimtP &p, int acc, int f, const float *) { return simt_int_finish<A>(p, dot(p, acc), f); }
 };
 
-struct SimtInt8 : SimtWords<int8_t, 0u> {
+// dp4a over s8 or +-1 bytes (AR_INT8, AR_INT8_GPU, AR_PM1Z_GPU): r = the s32 accumulator
+template <Arith A>
+struct SimtDp4a : SimtWords<int8_t, 0u> {
     static __device__ __forceinline__ void mac(int &acc, uint32_t a, uint32_t b) { acc = __dp4a((int)a, (int)b, acc); }
-    static __device__ __forceinline__ int raw(const SimtP &, int acc) { return acc; }
-    static __device__ __forceinline__ float finish(const SimtP &p, int acc, int f, const float *) {
-        return int8_epilogue(acc, p.alpha1, p.bias[f], p.act);
-    }
+    static __device__ __forceinline__ int raw(const SimtP &p, int acc) { return IntEpi<A>::raw(acc, p.bits); }
+    static __device__ __forceinline__ float finish(const SimtP &p, int acc, int f, const float *) { return simt_int_finish<A>(p, acc, f); }
 };
 
-struct SimtInt8Gpu : SimtInt8 {
-    static __device__ __forceinline__ float finish(const SimtP &p, int acc, int f, const float *) {
-        return int8_gpu_epilogue(acc, p.alpha1, p.bias[f], p.act);
-    }
-};
-
-struct SimtXnorGpu : SimtXnor {
-    static __device__ __forceinline__ float finish(const SimtP &p, int acc, int f, const float *) {
-        return xnor_gpu_epilogue(2 * raw(p, acc) - p.bits, p.mean[f], p.bias[f], p.act);
-    }
-};
-
-struct SimtPm1zGpu : SimtInt8 {
-    static __device__ __forceinline__ float finish(const SimtP &p, int acc, int f, const float *) {
-        return pm1z_gpu_epilogue(acc, p.mean[f], p.bias[f], p.act);
-    }
-};
+// the integer policies by the names their k_conv_simt instantiations carry (Network.op_kernels)
+struct SimtXnor : SimtPopc<AR_XNOR> {};
+struct SimtXnorGpu : SimtPopc<AR_XNOR_GPU> {};
+struct SimtPm1zGpu : SimtDp4a<AR_PM1Z_GPU> {};
+struct SimtInt8 : SimtDp4a<AR_INT8> {};
+struct SimtInt8Gpu : SimtDp4a<AR_INT8_GPU> {};
 
 template <typename V>
 __global__ void __launch_bounds__(256) k_conv_simt(SimtP p) {
@@ -619,9 +614,9 @@ struct XnorP {                // the small-K XNOR convolutions, 3x3 / stride 1 /
 // per POOLED pixel computes the four popcount outputs of its window for every filter, takes the reference's max (max-pool
 // semantics: elements outside the image are skipped) and writes only the sign the next layer would have extracted, in its side
 // format F: SIDE_PM1_S8 (next layer runs as +-1 on the s8 wgmma) or SIDE_BITS (next layer on the popcount kernels).  The f32
-// activation and the pooled f32 tensor are never written.  Bit-identical to conv -> max-pool -> k_int_input.  GPU: the epilogue of
-// the GPU XNOR rule (xnor_gpu_epilogue, k_conv_xnor_smallk_pool_gpu), else the CPU build's (xnor_epilogue).
-template <int CW, SideFmt F, bool GPU>
+// activation and the pooled f32 tensor are never written.  Bit-identical to conv -> max-pool -> k_int_input.  A: AR_XNOR or
+// AR_XNOR_GPU, whose IntEpi finishes each dot.
+template <int CW, SideFmt F, Arith A>
 __device__ __forceinline__ void xnor_smallk_pool(const XnorP &p, const TV &q) {
     extern __shared__ uint32_t wsm[];            // [n][9*CW]
     constexpr int KW = 9 * CW;
@@ -654,7 +649,7 @@ __device__ __forceinline__ void xnor_smallk_pool(const XnorP &p, const TV &q) {
 #pragma unroll
                 for (int c = 0; c < CW; ++c) cnt += __popc(~(a[((t / 3 + dy) * 4 + t % 3 + dx) * CW + c] ^ wf[t * CW + c]));
             const int dot = 2 * (cnt - p.padbits) - p.K;
-            const float v = GPU ? xnor_gpu_epilogue(dot, p.mean[f], p.bias[f], p.act) : xnor_epilogue(dot, p.mean[f], p.bias[f], p.act);
+            const float v = IntEpi<A>::finish(dot, p.mean[f], p.bias[f], p.act);
             mx = v > mx ? v : mx;
         }
         // one store per word (+-1 bytes: the filter count of an XNOR layer feeding the tensor-core path is a multiple of 16)
@@ -666,9 +661,9 @@ __device__ __forceinline__ void xnor_smallk_pool(const XnorP &p, const TV &q) {
 
 // XNOR convolution for small K (one or two words per tap): one thread per output pixel keeps its 9 x CW input
 // words in registers and walks all filters, whose sign words sit in shared memory (broadcast reads).  Whole groups of 4
-// filters are stored as one float4: the output must be a vec4_view (16-byte aligned pixels), which the layer plan checks.  GPU:
-// as in xnor_smallk_pool.
-template <int CW, bool GPU>
+// filters are stored as one float4: the output must be a vec4_view (16-byte aligned pixels), which the layer plan checks.  A: as
+// in xnor_smallk_pool.
+template <int CW, Arith A>
 __device__ __forceinline__ void xnor_smallk(const XnorP &p) {
     extern __shared__ uint32_t wsm[];            // [n][9*CW]
     constexpr int KW = 9 * CW;
@@ -699,24 +694,25 @@ __device__ __forceinline__ void xnor_smallk(const XnorP &p) {
 #pragma unroll
                 for (int k = 0; k < KW; ++k) cnt += __popc(~(a[k] ^ wf[k]));
             }
-            const int count = cnt - p.padbits;
-            if (p.counts && f < p.n) p.counts[(((size_t)n * p.n + f) * H + y) * W + x] = count;
+            const int dot = 2 * (cnt - p.padbits) - p.K;
+            if (p.counts && f < p.n) p.counts[(((size_t)n * p.n + f) * H + y) * W + x] = IntEpi<A>::raw(dot, p.K);
             const float mean = (f < p.n) ? p.mean[f] : 0.f, bias = (f < p.n) ? p.bias[f] : 0.f;
-            r[j] = GPU ? xnor_gpu_epilogue(2 * count - p.K, mean, bias, p.act) : xnor_epilogue(2 * count - p.K, mean, bias, p.act);
+            r[j] = IntEpi<A>::finish(dot, mean, bias, p.act);
         }
         if (f0 + 3 < p.n) *reinterpret_cast<float4 *>(o + f0) = make_float4(r[0], r[1], r[2], r[3]);
         else for (int j = 0; j < 4 && f0 + j < p.n; ++j) o[f0 + j] = r[j];
     }
 }
 
+// the kernels, by arithmetic: AR_XNOR k_conv_xnor_smallk[_pool], AR_XNOR_GPU k_conv_xnor_smallk[_pool]_gpu
 template <int CW>
-__global__ void __launch_bounds__(128) k_conv_xnor_smallk(XnorP p) { xnor_smallk<CW, false>(p); }
+__global__ void __launch_bounds__(128) k_conv_xnor_smallk(XnorP p) { xnor_smallk<CW, AR_XNOR>(p); }
 template <int CW>
-__global__ void __launch_bounds__(128) k_conv_xnor_smallk_gpu(XnorP p) { xnor_smallk<CW, true>(p); }
+__global__ void __launch_bounds__(128) k_conv_xnor_smallk_gpu(XnorP p) { xnor_smallk<CW, AR_XNOR_GPU>(p); }
 template <int CW, SideFmt F>
-__global__ void __launch_bounds__(128) k_conv_xnor_smallk_pool(XnorP p, TV q /* next layer's input */) { xnor_smallk_pool<CW, F, false>(p, q); }
+__global__ void __launch_bounds__(128) k_conv_xnor_smallk_pool(XnorP p, TV q /* next layer's input */) { xnor_smallk_pool<CW, F, AR_XNOR>(p, q); }
 template <int CW, SideFmt F>
-__global__ void __launch_bounds__(128) k_conv_xnor_smallk_pool_gpu(XnorP p, TV q) { xnor_smallk_pool<CW, F, true>(p, q); }
+__global__ void __launch_bounds__(128) k_conv_xnor_smallk_pool_gpu(XnorP p, TV q) { xnor_smallk_pool<CW, F, AR_XNOR_GPU>(p, q); }
 
 // ------------------------------------------------------------------------------------------------------
 // small layers (one thread per output element, channels innermost -> coalesced)
