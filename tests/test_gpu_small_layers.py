@@ -294,9 +294,9 @@ def test_small_layer(name, dt, workdir):
             assert not mine, (name, dt, i, mine)     # every source writes its own slice
             continue
         assert mine and all(kernel_is(k, kern[dt]) for k in mine), (name, dt, i, mine)
-        if kern[dt] != "k_upsample_vec16":   # the templated kernels: instantiated for the layer's activation dtype
-            assert all(("__nv_bfloat16" in k) == (dt == "bf16" and kern[dt] not in ("k_yolo", "k_region")) for k in mine), \
-                (name, dt, i, mine)
+        # the templated kernels: instantiated for the layer's activation dtype
+        assert all(("__nv_bfloat16" in k) == (dt == "bf16" and kern[dt] not in ("k_yolo", "k_region")) for k in mine), \
+            (name, dt, i, mine)
     if name.startswith("route"):
         for r, n in ROUTE_COPIES[case.fuse].items():
             assert sum(1 for (j, kind, _) in ops if j == r and kind == "route_copy") == n, (name, dt, r, ops)

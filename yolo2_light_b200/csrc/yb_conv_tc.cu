@@ -1807,16 +1807,15 @@ void encode_maps(TcPlan &plan, const TcConv &c, bool reg) {
 int tc_conv_supported(const TcConv &c) {
     const Layer &l = *c.l;
     const bool integer = is_integer(c.kind);
-    // a view TMA can address: 16-byte aligned base and pixel rows
-    auto aligned = [](const TV &t, int esz) { return (reinterpret_cast<uintptr_t>(t.base) & 15) == 0 && t.ldc * esz % 16 == 0; };
+    // every view it reads or writes must be one TMA can address: a vec16_view
     if (!geometry_ok(l) || l.n < 8 || (l.activation != YB_LEAKY && l.activation != YB_LINEAR)) return 0;
-    if (channel_row(operand_channels(c), elem_size(c.kind)) == 0 || c.in.P != 1 || !aligned(c.in, elem_size(c.kind))) return 0;
+    if (channel_row(operand_channels(c), elem_size(c.kind)) == 0 || c.in.P != 1 || !vec16_view(c.in, elem_size(c.kind))) return 0;
     // bf16 output: the bf16 kind only, whole 16-byte filter groups
     if (c.out_bf16 && (c.kind != TC_BF16 || l.n % 8 != 0)) return 0;
-    if (c.out.base ? (c.out.P != 1 || !aligned(c.out, c.out_bf16 ? 2 : 4)) : !(c.yolo_out || c.pool_fmt != SIDE_NONE)) return 0;
+    if (c.out.base ? (c.out.P != 1 || !vec16_view(c.out, c.out_bf16 ? 2 : 4)) : !(c.yolo_out || c.pool_fmt != SIDE_NONE)) return 0;
     // fused shortcut: k_conv_tc_reg at stride 1
     if (c.res.base && !(c.kind == TC_BF16 && c.out_bf16 && l.stride == 1 && c.res.H == l.out_h && c.res.W == l.out_w &&
-                        c.res.C == l.n && aligned(c.res, 2)))
+                        c.res.C == l.n && vec16_view(c.res, 2)))
         return 0;
     // fused [yolo]: the f32 epilogue of k_conv_tc
     if (c.yolo_out && (integer || c.out_bf16)) return 0;
@@ -1824,7 +1823,7 @@ int tc_conv_supported(const TcConv &c) {
     // straddle tiles when the padded height and the output size are even; the epilogue writes whole 32-filter groups of bytes
     if (c.pool_fmt != SIDE_NONE && !(integer && (side_s8(c.pool_fmt) || c.pool_fmt == SIDE_PM1_S8) && !c.acc_out && l.size == 3 && l.stride == 1 &&
                          l.h % 2 == 0 && l.out_h % 2 == 0 && l.out_w % 2 == 0 && l.n % 32 == 0 &&
-                         c.pool_next.H == l.out_h / 2 && c.pool_next.W == l.out_w / 2 && aligned(c.pool_next, 1)))
+                         c.pool_next.H == l.out_h / 2 && c.pool_next.W == l.out_w / 2 && vec16_view(c.pool_next, 1)))
         return 0;
     return 1;
 }
@@ -1864,8 +1863,7 @@ TcPlanPtr tc_make_plan(const TcConv &c) {
 struct StemPlan { StemTcP p; int grid; bool s2; };   // s2: k_stem_s2_tc (stem + layer 1)
 int tc_stem_supported(const Layer &l, const TV &out) {
     return l.c == 3 && l.size == 3 && l.stride == 1 && l.pad == 1 && (l.n == 16 || l.n == 32) &&
-           (l.activation == YB_LEAKY || l.activation == YB_LINEAR) && out.base && out.ldc % 8 == 0 &&
-           (reinterpret_cast<uintptr_t>(out.base) & 15) == 0;
+           (l.activation == YB_LEAKY || l.activation == YB_LINEAR) && out.base && vec16_view(out, 2);
 }
 // d_w: device buffer of 32*32 bf16 ([filter][k], k = (ky,kx,c), zero padded), d_bias: device f32[>= n]
 StemPlanPtr tc_stem_make_plan(const Layer &l, const TV &out, const void *d_w, const float *d_bias) {
@@ -1882,7 +1880,7 @@ StemPlanPtr tc_stem_make_plan(const Layer &l, const TV &out, const void *d_w, co
 int tc_stem_s2_supported(const Layer &l0, const Layer &l1, const TV &out1) {
     return l0.n == 32 && l1.c == 32 && l1.n == 64 && l1.size == 3 && l1.stride == 2 && l1.pad == 1 && l1.h == l0.h && l1.w == l0.w &&
            l0.h % 2 == 0 && l0.w % 2 == 0 && (l1.activation == YB_LEAKY || l1.activation == YB_LINEAR) && out1.base && out1.P == 1 &&
-           out1.H == l0.h / 2 && out1.W == l0.w / 2 && out1.ldc % 8 == 0 && (reinterpret_cast<uintptr_t>(out1.base) & 15) == 0;
+           out1.H == l0.h / 2 && out1.W == l0.w / 2 && vec16_view(out1, 2);
 }
 // d_w1: layer 1's bf16 [64][9 * 32] filter matrix (K ordered (ky, kx, c)), d_bias1: its f32 bias
 StemPlanPtr tc_stem_s2_make_plan(const Layer &l0, const Layer &l1, const TV &out1, const void *d_w, const float *d_bias,

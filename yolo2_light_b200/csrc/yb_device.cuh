@@ -23,9 +23,10 @@ __device__ __forceinline__ T *tv_px(const TV &t, int n, int y, int x) {
     return reinterpret_cast<T *>(t.base) + ((size_t)(n * t.Hp + y + t.P) * t.Wp + (x + t.P)) * (size_t)t.ldc;
 }
 
-// an f32 view whose every 4-channel group can be read with one 16-byte load
-__host__ __device__ __forceinline__ bool vec4_view(const TV &t) {
-    return t.ldc % 4 == 0 && (reinterpret_cast<uintptr_t>(t.base) & 15) == 0;
+// a view of esz-byte elements whose every pixel starts 16-byte aligned: a 16-byte aligned base and pixel stride.  Every
+// kernel that loads or stores 16 bytes of a pixel's channels at a time is placed only on such a view.
+__host__ __device__ __forceinline__ bool vec16_view(const TV &t, int esz) {
+    return (reinterpret_cast<uintptr_t>(t.base) & 15) == 0 && t.ldc * esz % 16 == 0;
 }
 
 __device__ __forceinline__ float to_f32(float v) { return v; }

@@ -582,7 +582,7 @@ struct Builder {
         if (int8) return (!sw.no_tc && tc_conv_supported(tc_query)) ? KERN_TC : KERN_SIMT;
         if (p.arith == AR_PM1Z_GPU) return (xnor_tc(i) && tc_conv_supported(tc_query)) ? KERN_TC : KERN_SIMT;
         if (p.arith == AR_XNOR_PM1_F32) return KERN_SIMT;
-        if (xnor_tc(i) && vec4_view(tin)) {
+        if (xnor_tc(i) && vec16_view(tin, 4)) {
             if (!tc_conv_supported(tc_query)) fatal_throw("engine: xnor tensor-core layer not supported by the i8 tile");
             return KERN_TC;
         }
@@ -590,7 +590,7 @@ struct Builder {
         // stores 4 filters per float4, so every pixel of its output must be 16-byte aligned: a channel slice of a route's
         // buffer may not be.
         const int CW = (l.c + 31) / 32;
-        if (CW <= 2 && l.size == 3 && l.stride == 1 && l.pad == 1 && (size_t)l.n * 9 * CW * 4 <= 40 * 1024 && vec4_view(tout))
+        if (CW <= 2 && l.size == 3 && l.stride == 1 && l.pad == 1 && (size_t)l.n * 9 * CW * 4 <= 40 * 1024 && vec16_view(tout, 4))
             return KERN_SMALLK;
         return KERN_SIMT;
     }
@@ -602,8 +602,7 @@ struct Builder {
     void plan_first_op() {
         const Layer &l0 = layer(0);
         const TV out0 = layout_view(0);
-        const bool out_vec = L[0].out_dt == DT_F32 ? vec4_view(out0)
-                                                   : out0.ldc % 8 == 0 && (reinterpret_cast<uintptr_t>(out0.base) & 15) == 0;
+        const bool out_vec = vec16_view(out0, (int)dt_size(L[0].out_dt));
         const bool stem_ok = l0.type == YB_CONVOLUTIONAL && L[0].arith == AR_F32 && L[0].kern == KERN_SIMT && l0.c == 3 &&
                              l0.size == 3 && l0.stride == 1 && l0.pad == 1 && (l0.n == 16 || l0.n == 32) && L[0].fused_into < 0 &&
                              L[0].has_out && !sw.no_stem && out_vec;
@@ -981,6 +980,11 @@ struct Builder {
         const int dt = in_dt(i);
         const TV tout = e.out_tv[i];
         const int g = grid_for((long)B * l.out_h * l.out_w * l.out_c);
+        // the 16-byte forms of max-pool and upsample (one thread per 16 bytes of channels): whole 16-byte channel rows of
+        // 16-byte aligned pixels
+        const int esz = (int)dt_size(dt);
+        const bool vec = l.out_c * esz % 16 == 0 && vec16_view(tin, esz) && vec16_view(tout, esz);
+        const int gv = grid_for((long)B * l.out_h * l.out_w * ((l.out_c * esz) / 16 + 1));
         switch (l.type) {
         case YB_MAXPOOL: {
             if (p.pool_in_conv) break;    // done in the epilogue of the integer convolution in front of it
@@ -988,21 +992,13 @@ struct Builder {
                 push_int_input(OP_MAXPOOL, i, i + 1, tin, l.size, l.stride, l.pad);
                 break;
             }
-            const int esz = (int)dt_size(dt);
-            const bool vec = (l.out_c * esz) % 16 == 0 && (tin.ldc * esz) % 16 == 0 && (tout.ldc * esz) % 16 == 0 &&
-                             (reinterpret_cast<uintptr_t>(tin.base) & 15) == 0 && (reinterpret_cast<uintptr_t>(tout.base) & 15) == 0;
-            const int gv = grid_for((long)B * l.out_h * l.out_w * ((l.out_c * esz) / 16 + 1));
             push_kernel(OP_MAXPOOL, i, vec ? BY_DT(k_maxpool_vec, dt) : BY_DT(k_maxpool, dt), vec ? gv : g, 256, 0, tin, tout, l.size,
                         l.stride, l.pad);
             break;
         }
         case YB_UPSAMPLE: {
-            const int esz = (int)dt_size(dt);
-            const bool vec = l.scale == 1.f && (l.out_c * esz) % 16 == 0 && (tin.ldc * esz) % 16 == 0 && (tout.ldc * esz) % 16 == 0 &&
-                             (reinterpret_cast<uintptr_t>(tin.base) & 15) == 0 && (reinterpret_cast<uintptr_t>(tout.base) & 15) == 0;
-            if (vec)
-                push_kernel(OP_UPSAMPLE, i, k_upsample_vec16, grid_for((long)B * l.out_h * l.out_w * ((l.out_c * esz) / 16 + 1)), 256, 0,
-                            tin, tout, l.stride, esz);
+            if (vec && l.scale == 1.f)
+                push_kernel(OP_UPSAMPLE, i, BY_DT(k_upsample_vec16, dt), gv, 256, 0, tin, tout, l.stride);
             else
                 push_kernel(OP_UPSAMPLE, i, BY_DT(k_upsample, dt), g, 256, 0, tin, tout, l.stride, l.scale);
             break;

@@ -556,7 +556,7 @@ __global__ void __launch_bounds__(128) k_conv_stem(const float *__restrict__ in,
     }
     TOut *o = tv_px<TOut>(out, n, y, x);
     if constexpr (sizeof(TOut) == 2) {
-        uint4 *op = reinterpret_cast<uint4 *>(o);     // 8 filters per store: the layer plan checks a 16-byte aligned base, ldc % 8 == 0
+        uint4 *op = reinterpret_cast<uint4 *>(o);     // 8 filters per store: the layer plan checks vec16_view(out, 2)
 #pragma unroll
         for (int g = 0; g < NF / 8; ++g) {
             float t[8];
@@ -573,7 +573,7 @@ __global__ void __launch_bounds__(128) k_conv_stem(const float *__restrict__ in,
             op[g] = v;
         }
     } else {
-        float4 *op = reinterpret_cast<float4 *>(o);   // NF*4 bytes per pixel, 16-byte aligned: the layer plan checks vec4_view(out)
+        float4 *op = reinterpret_cast<float4 *>(o);   // NF*4 bytes per pixel, 16-byte aligned: the layer plan checks vec16_view(out, 4)
 #pragma unroll
         for (int g = 0; g < NF / 4; ++g)
             op[g] = make_float4(act_exact(__fadd_rn(acc[g * 4 + 0], sw.b[g * 4 + 0]), act), act_exact(__fadd_rn(acc[g * 4 + 1], sw.b[g * 4 + 1]), act),
@@ -661,7 +661,7 @@ __device__ __forceinline__ void xnor_smallk_pool(const XnorP &p, const TV &q) {
 
 // XNOR convolution for small K (one or two words per tap): one thread per output pixel keeps its 9 x CW input
 // words in registers and walks all filters, whose sign words sit in shared memory (broadcast reads).  Whole groups of 4
-// filters are stored as one float4: the output must be a vec4_view (16-byte aligned pixels), which the layer plan checks.  A: as
+// filters are stored as one float4: the output must be a vec16_view (16-byte aligned pixels), which the layer plan checks.  A: as
 // in xnor_smallk_pool.
 template <int CW, Arith A>
 __device__ __forceinline__ void xnor_smallk(const XnorP &p) {
@@ -718,78 +718,88 @@ __global__ void __launch_bounds__(128) k_conv_xnor_smallk_pool_gpu(XnorP p, TV q
 // small layers (one thread per output element, channels innermost -> coalesced)
 // ------------------------------------------------------------------------------------------------------
 
-// forward_maxpool_layer_avx scalar build (reference additionally.c:1448-1482): window origin
-// (o*stride - pad/2), out-of-image taps ignored, init -FLT_MAX.
-template <typename T>
-__global__ void k_maxpool(TV in, TV out, int size, int stride, int pad) {
-    const long total = (long)out.N * out.H * out.W * out.C;
-    const int off = -pad / 2;
-    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-        const int c = (int)(i % out.C);
-        const long pxl = i / out.C;
-        const int x = (int)(pxl % out.W);
-        const int y = (int)((pxl / out.W) % out.H);
-        const int n = (int)(pxl / ((long)out.W * out.H));
-        float m = -3.402823466e+38f;
+// The max-pool window of forward_maxpool_layer_avx's scalar build (reference additionally.c:1448-1482), for output pixel
+// (n, y, x) and channels c0 .. c0+V-1: m[k] starts at -FLT_MAX and takes each in-image tap of the window (origin
+// o*stride - pad/2, out-of-image taps skipped) that is strictly greater.  Channels past in.C keep -FLT_MAX.  With vec (the
+// input is a vec16_view) a group wholly inside in.C is read with 16-byte loads, all issued together; otherwise value by value.
+// The window is walked by one loop per load form, so the 16-byte loop carries no per-tap branch and unrolls.
+template <typename T, int V>
+__device__ __forceinline__ void pool_window(const TV &in, int n, int y, int x, int c0, int size, int stride, int pad, bool vec,
+                                            float (&m)[V]) {
+#pragma unroll
+    for (int k = 0; k < V; ++k) m[k] = -3.402823466e+38f;
+    auto window = [&](auto fold) {   // fold(src) for each in-image tap, src: channel c0 of the tap's pixel
+        const int off = -pad / 2;
         for (int a = 0; a < size; ++a) {
             const int iy = off + y * stride + a;
             if (iy < 0 || iy >= in.H) continue;
             for (int b = 0; b < size; ++b) {
                 const int ix = off + x * stride + b;
                 if (ix < 0 || ix >= in.W) continue;
-                const float v = to_f32(tv_px<T>(in, n, iy, ix)[c]);
-                m = (v > m) ? v : m;
+                fold(tv_px<T>(in, n, iy, ix) + c0);
             }
         }
-        tv_px<T>(out, n, y, x)[c] = from_f32<T>(m);
+    };
+    constexpr int L = (V * sizeof(T) + 15) / 16;   // 16-byte loads per group, where the group is whole ones
+    if (V * sizeof(T) % 16 == 0 && vec && c0 + V <= in.C) {
+        window([&](const T *src) {
+            uint4 raw[L];
+#pragma unroll
+            for (int k = 0; k < L; ++k) raw[k] = __ldg(reinterpret_cast<const uint4 *>(src) + k);
+            const T *v = reinterpret_cast<const T *>(raw);
+#pragma unroll
+            for (int k = 0; k < V; ++k) { const float f = to_f32(v[k]); m[k] = f > m[k] ? f : m[k]; }
+        });
+    } else {
+        window([&](const T *src) {
+#pragma unroll
+            for (int k = 0; k < V; ++k)
+                if (c0 + k < in.C) { const float f = to_f32(src[k]); m[k] = f > m[k] ? f : m[k]; }
+        });
     }
 }
 
-// same, 16 bytes (4 f32 / 8 bf16 channels) per thread
-template <typename T>
-__global__ void k_maxpool_vec(TV in, TV out, int size, int stride, int pad) {
-    constexpr int V = 16 / sizeof(T);
-    const int chunks = out.C / V;
-    const long total = (long)out.N * out.H * out.W * chunks;
-    const int off = -pad / 2;
+// Max-pool: one thread per element, or with VEC one per 16 bytes of channels (4 f32 / 8 bf16), which the engine runs on
+// vec16_view input and output whose channel rows are whole 16-byte groups.
+template <typename T, bool VEC>
+__device__ __forceinline__ void maxpool(const TV &in, const TV &out, int size, int stride, int pad) {
+    constexpr int V = VEC ? 16 / sizeof(T) : 1;   // channels per thread
+    const int groups = out.C / V;
+    const long total = (long)out.N * out.H * out.W * groups;
     for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-        const int ch = (int)(i % chunks);
-        const long pxl = i / chunks;
+        const int g = (int)(i % groups);
+        const long pxl = i / groups;
         const int x = (int)(pxl % out.W);
         const int y = (int)((pxl / out.W) % out.H);
         const int n = (int)(pxl / ((long)out.W * out.H));
         float m[V];
+        pool_window<T>(in, n, y, x, g * V, size, stride, pad, VEC, m);
+        T *dst = tv_px<T>(out, n, y, x) + g * V;
+        if constexpr (VEC) {
+            uint4 o;
+            T *ov = reinterpret_cast<T *>(&o);
 #pragma unroll
-        for (int k = 0; k < V; ++k) m[k] = -3.402823466e+38f;
-        for (int a = 0; a < size; ++a) {
-            const int iy = off + y * stride + a;
-            if (iy < 0 || iy >= in.H) continue;
-            for (int b = 0; b < size; ++b) {
-                const int ix = off + x * stride + b;
-                if (ix < 0 || ix >= in.W) continue;
-                const uint4 raw = __ldg(reinterpret_cast<const uint4 *>(tv_px<T>(in, n, iy, ix)) + ch);
-                const T *v = reinterpret_cast<const T *>(&raw);
-#pragma unroll
-                for (int k = 0; k < V; ++k) { const float f = to_f32(v[k]); m[k] = (f > m[k]) ? f : m[k]; }
-            }
+            for (int k = 0; k < V; ++k) ov[k] = from_f32<T>(m[k]);
+            *reinterpret_cast<uint4 *>(dst) = o;
+        } else {
+            *dst = from_f32<T>(m[0]);
         }
-        uint4 o;
-        T *ov = reinterpret_cast<T *>(&o);
-#pragma unroll
-        for (int k = 0; k < V; ++k) ov[k] = from_f32<T>(m[k]);
-        reinterpret_cast<uint4 *>(tv_px<T>(out, n, y, x))[ch] = o;
     }
 }
+// the kernels, by form: k_maxpool (one thread per element), k_maxpool_vec (16 bytes per thread)
+template <typename T>
+__global__ void k_maxpool(TV in, TV out, int size, int stride, int pad) { maxpool<T, false>(in, out, size, stride, pad); }
+template <typename T>
+__global__ void k_maxpool_vec(TV in, TV out, int size, int stride, int pad) { maxpool<T, true>(in, out, size, stride, pad); }
 
 // The input conversion of an integer convolution: f32 activation -> side format F (yb_device.cuh), optionally behind a max-pool.
 // With a 1x1 window (size 1, stride 1, pad 0) it is the conversion alone (the reference's quantisation / binarize_cpu /
-// float_to_bit); with the max-pool's window it is forward_maxpool_layer_avx's scalar build (window origin o*stride - pad/2,
-// out-of-image taps ignored, -FLT_MAX start, strict >) followed by the conversion, so the f32 pooled tensor never goes to HBM.
-// Either way the bytes are those of the unfused layers: a NaN or -inf input leaves -FLT_MAX, which converts as they do.
-// One thread per int_input_channels(F) channels: 16 s8 channels (one 16-byte store; s8 pixel strides are multiples of 32) or
-// one word of 32 sign bits.  In the last group, channels past in.C keep -FLT_MAX (s8 0, +-1 byte -1, bit 0); the 16-channel
-// groups wholly past in.C are not written and keep the values the engine placed there (s8 0, +-1 byte -1), the same bytes.
-// The input is read with 16-byte loads when the view allows it (vec4_view), with scalar loads otherwise.
+// float_to_bit); with the max-pool's window it is that max-pool (pool_window) followed by the conversion, so the f32 pooled
+// tensor never goes to HBM.  Either way the bytes are those of the unfused layers: a NaN or -inf input leaves -FLT_MAX, which
+// converts as they do.  One thread per int_input_channels(F) channels: 16 s8 channels (one 16-byte store; s8 pixel strides are
+// multiples of 32) or one word of 32 sign bits.  In the last group, channels past in.C keep -FLT_MAX (s8 0, +-1 byte -1, bit
+// 0); the 16-channel groups wholly past in.C are not written and keep the values the engine placed there (s8 0, +-1 byte -1),
+// the same bytes.  The input is read with 16-byte loads when it is a vec16_view, with scalar loads otherwise.
 __host__ __device__ constexpr int int_input_channels(SideFmt f) { return f == SIDE_BITS ? 32 : 16; }
 // k_int_input's threads per pixel of an input of C channels
 __host__ __device__ constexpr int int_input_groups(SideFmt f, int C) { return (C + int_input_channels(f) - 1) / int_input_channels(f); }
@@ -800,8 +810,7 @@ __global__ void k_int_input(TV in /* f32 */, TV q, int size, int stride, int pad
     const int groups = int_input_groups(F, in.C);                // threads per pixel
     const int OH = q.H, OW = q.W;
     const long total = (long)q.N * OH * OW * groups;
-    const int off = -pad / 2;
-    const bool vec = vec4_view(in);
+    const bool vec = vec16_view(in, 4);
     for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
         const int g = (int)(i % groups);
         const long pxl = i / groups;
@@ -809,37 +818,12 @@ __global__ void k_int_input(TV in /* f32 */, TV q, int size, int stride, int pad
         const int y = (int)((pxl / OW) % OH);
         const int n = (int)(pxl / ((long)OW * OH));
         float m[V];
-#pragma unroll
-        for (int k = 0; k < V; ++k) m[k] = -3.402823466e+38f;
-        for (int a = 0; a < size; ++a) {
-            const int iy = off + y * stride + a;
-            if (iy < 0 || iy >= in.H) continue;
-            for (int b = 0; b < size; ++b) {
-                const int ix = off + x * stride + b;
-                if (ix < 0 || ix >= in.W) continue;
-                const float *src = tv_px<float>(in, n, iy, ix) + g * V;
-                if (vec && g * V + V <= in.C) {     // the whole group, all loads issued together
-                    float4 v[V / 4];
-#pragma unroll
-                    for (int k = 0; k < V / 4; ++k) v[k] = __ldg(reinterpret_cast<const float4 *>(src) + k);
-#pragma unroll
-                    for (int k = 0; k < V / 4; ++k) {
-                        m[4 * k] = v[k].x > m[4 * k] ? v[k].x : m[4 * k]; m[4 * k + 1] = v[k].y > m[4 * k + 1] ? v[k].y : m[4 * k + 1];
-                        m[4 * k + 2] = v[k].z > m[4 * k + 2] ? v[k].z : m[4 * k + 2]; m[4 * k + 3] = v[k].w > m[4 * k + 3] ? v[k].w : m[4 * k + 3];
-                    }
-                } else {
-#pragma unroll
-                    for (int k = 0; k < V; ++k)
-                        if (g * V + k < in.C) { const float f = __ldg(src + k); m[k] = f > m[k] ? f : m[k]; }
-                }
-            }
-        }
+        pool_window<float>(in, n, y, x, g * V, size, stride, pad, vec, m);
         if constexpr (F == SIDE_BITS) side_px<F>(q, n, y, x)[g] = side_word<F>(m, mult);
         else reinterpret_cast<uint4 *>(side_px<F>(q, n, y, x))[g] = side_word4<F>(m, mult);
     }
 }
 
-// upsample_cpu forward (reference yolov2_forward_network.c:380-394): out = scale * in[y/stride][x/stride]
 // Pairs of f32 lanes (filter 2j, 2j + 1) in one 64-bit value, each lane rounded on its own: exactly __fmul_rn / __fadd_rn
 // twice.  __fmul_rn / __fadd_rn are never contracted into an FMA, which keeps the reference's separately rounded gemm_nn order.
 __device__ __forceinline__ unsigned long long f2_pack(float lo, float hi) {
@@ -937,35 +921,31 @@ __global__ void __launch_bounds__(128) k_stem_pool(const float *__restrict__ in,
     }
 }
 
+// upsample_cpu forward (reference yolov2_forward_network.c:380-394): out = scale * in[y/stride][x/stride].  One thread per
+// element, or with VEC one per 16 bytes of channels, which the engine runs at scale 1 only -- a copy of the bits, exact for
+// any dtype -- on vec16_view input and output whose channel rows are whole 16-byte groups.
+template <typename T, bool VEC>
+__device__ __forceinline__ void upsample(const TV &in, const TV &out, int stride, float scale) {
+    constexpr int V = VEC ? 16 / sizeof(T) : 1;   // channels per thread
+    const int groups = out.C / V;
+    const long total = (long)out.N * out.H * out.W * groups;
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+        const int g = (int)(i % groups);
+        const long pxl = i / groups;
+        const int x = (int)(pxl % out.W);
+        const int y = (int)((pxl / out.W) % out.H);
+        const int n = (int)(pxl / ((long)out.W * out.H));
+        const T *src = tv_px<T>(in, n, y / stride, x / stride) + g * V;
+        T *dst = tv_px<T>(out, n, y, x) + g * V;
+        if constexpr (VEC) *reinterpret_cast<uint4 *>(dst) = __ldg(reinterpret_cast<const uint4 *>(src));
+        else *dst = from_f32<T>(__fmul_rn(scale, to_f32(*src)));
+    }
+}
+// the kernels, by form: k_upsample (one thread per element), k_upsample_vec16 (16 bytes per thread, scale 1)
 template <typename T>
-__global__ void k_upsample(TV in, TV out, int stride, float scale) {
-    const long total = (long)out.N * out.H * out.W * out.C;
-    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-        const int c = (int)(i % out.C);
-        const long pxl = i / out.C;
-        const int x = (int)(pxl % out.W);
-        const int y = (int)((pxl / out.W) % out.H);
-        const int n = (int)(pxl / ((long)out.W * out.H));
-        const float v = to_f32(tv_px<T>(in, n, y / stride, x / stride)[c]);
-        tv_px<T>(out, n, y, x)[c] = from_f32<T>(__fmul_rn(scale, v));
-    }
-}
-
-// same, 16 bytes per thread (scale == 1: a pure copy of bits, exact for any dtype)
-static __global__ void k_upsample_vec16(TV in, TV out, int stride, int esize) {
-    const int chunks = (out.C * esize) >> 4;
-    const long total = (long)out.N * out.H * out.W * chunks;
-    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-        const int ch = (int)(i % chunks);
-        const long pxl = i / chunks;
-        const int x = (int)(pxl % out.W);
-        const int y = (int)((pxl / out.W) % out.H);
-        const int n = (int)(pxl / ((long)out.W * out.H));
-        const char *src = in.base + (((size_t)(n * in.Hp + y / stride + in.P) * in.Wp + (x / stride + in.P)) * (size_t)in.ldc) * esize;
-        char *dst = out.base + (((size_t)(n * out.Hp + y + out.P) * out.Wp + (x + out.P)) * (size_t)out.ldc) * esize;
-        reinterpret_cast<uint4 *>(dst)[ch] = __ldg(reinterpret_cast<const uint4 *>(src) + ch);
-    }
-}
+__global__ void k_upsample(TV in, TV out, int stride, float scale) { upsample<T, false>(in, out, stride, scale); }
+template <typename T>
+__global__ void k_upsample_vec16(TV in, TV out, int stride) { upsample<T, true>(in, out, stride, 1.f); }
 
 // forward_shortcut_layer_cpu (reference yolov2_forward_network.c:443-449, shortcut_cpu :410-432):
 // out = act(in + from) with the general stride/sample subsampling of shortcut_cpu.
